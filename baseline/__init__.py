@@ -18,7 +18,7 @@ def build(force: bool = False) -> str:
     if not force and os.path.exists(SO_PATH) and os.path.getmtime(SO_PATH) >= os.path.getmtime(SRC):
         return SO_PATH
     nvcc = shutil.which("nvcc") or "/usr/local/cuda/bin/nvcc"
-    cmd = [nvcc, "-std=c++17", "-O3", "-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-shared",
+    cmd = [nvcc, "-std=c++17", "-O3", "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-shared",
            "-Xcompiler", "-fPIC", "-o", SO_PATH, SRC, "-lcublasLt", "-Xlinker", "-rpath", "-Xlinker", "/usr/local/cuda/lib64"]
     res = subprocess.run(cmd, capture_output=True, text=True)
     if res.returncode != 0:

@@ -154,7 +154,7 @@ int bl_pairwise_l2(void* stream, float* dist, const float* x, const float* y, fl
   bl_row_norm_kernel<<<static_cast<unsigned>((m + 7) / 8), 256, 0, s>>>(xn, x, m, static_cast<int>(k));
   bl_row_norm_kernel<<<static_cast<unsigned>((n + 7) / 8), 256, 0, s>>>(yn, y, n, static_cast<int>(k));
   if (bl_gemm_nt(s, dist, x, y, m, n, k, ws, ws_bytes)) return 1;
-  bl_l2_epilogue_kernel<<<148 * 16, 256, 0, s>>>(dist, xn, yn, m, n, do_sqrt);
+  bl_l2_epilogue_kernel<<<132 * 16, 256, 0, s>>>(dist, xn, yn, m, n, do_sqrt);
   const cudaError_t e = cudaGetLastError();
   return e == cudaSuccess ? 0 : fail(cudaGetErrorString(e), e);
 }
@@ -172,7 +172,7 @@ int bl_l2_nn(void* stream, float* best_val, int* best_idx, const float* x, const
     const int64_t nc = n - j0 < chunk_rows ? n - j0 : chunk_rows;
     bl_row_norm_kernel<<<static_cast<unsigned>((nc + 7) / 8), 256, 0, s>>>(yn, y + j0 * k, nc, static_cast<int>(k));
     if (bl_gemm_nt(s, tile, x, y + j0 * k, m, nc, k, ws, ws_bytes)) return 1;
-    bl_l2_epilogue_kernel<<<148 * 16, 256, 0, s>>>(tile, xn, yn, m, nc, 0);
+    bl_l2_epilogue_kernel<<<132 * 16, 256, 0, s>>>(tile, xn, yn, m, nc, 0);
     bl_row_argmin_kernel<<<static_cast<unsigned>(m), 256, 0, s>>>(tile, nc, best_val, best_idx, static_cast<int>(j0), j0 == 0);
   }
   const cudaError_t e = cudaGetLastError();

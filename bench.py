@@ -1,8 +1,8 @@
 #!/usr/bin/env python
-"""bench.py -- headline benchmark of the B200 pairwise-distance engine (contract: task statement).
+"""bench.py -- headline benchmark of the H100 pairwise-distance engine.
 
 N = 1 : one step = raft_b200.distance.pairwise_distance L2Expanded 100000 x 100000 x 128 fp32
-        (BASELINE.json configs[1]; operand prep + tcgen05 kernel), inputs resident in HBM.
+        (BASELINE.json configs[1]; operand prep + wgmma kernel), inputs resident in HBM.
         After the timed region the result of the last step is CHECKED (fp64 re-evaluation of sampled pairs on
         the device, oracle/device_check.py -> "parity"), the GPU baselines are timed on the same shapes in the
         same process ("gpu_baselines": cuBLASLt-SGEMM composition of the reference's surviving primitives,
@@ -14,7 +14,10 @@ N > 1 : one step = fusedL2NN 1,000,000 queries x 8,000,000 db rows x 96 (configs
         against the exact fp64 arg-min over its own shard (combined across ranks) -> "parity".
 --impl reference : the CPU restatement (oracle port: numpy expanded form on multithreaded BLAS,
         all host cores) on a bounded sample of the same workload.  The reference's own kernels for
-        this path are not in /root/reference (SURVEY.md section 0), so there is nothing else to run.
+        this path are not in the reference snapshot (SURVEY.md section 0), so there is nothing else to run.
+--dump-outputs DIR : after the timed steps, what the timed path returned in its last step goes to DIR/<name>.npy
+        (float32 / float64; a fixed, seeded sample of the 40 GB distance matrix), so that two builds can be
+        compared output for output on identical inputs.
 """
 from __future__ import annotations
 
@@ -39,21 +42,22 @@ def measured_peaks():
     try:
         return json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json"))), "measured"
     except Exception:
-        return {"hbm_gbs": 6650.0, "bf16_tflops": 1590.0, "bf16_tflops_sustained": 1400.0}, "fallback"
+        # NVIDIA's H100 SXM data sheet (700 W): 3.35 TB/s HBM3, 989 TFLOP/s dense FP16 / BF16 -- not reached figures
+        return {"hbm_gbs": 3350.0, "bf16_tflops": 989.0, "bf16_tflops_sustained": 989.0}, "H100 SXM data sheet"
 
 
-def ncu_traffic(name):
-    """dram bytes per launch of the dominant kernel from the committed ncu capture, if any."""
-    for f in ("r02_traffic.json", "r01_traffic.json"):
-        try:
-            return json.load(open(os.path.join(ROOT, "profiles", f)))[name]
-        except Exception:
-            continue
-    return None
+def dump_outputs(out_dir, arrays):
+    """--dump-outputs: one DIR/<name>.npy per array (float32 / float64 only)."""
+    import numpy as np
+    os.makedirs(out_dir, exist_ok=True)
+    for name, a in arrays.items():
+        a = np.ascontiguousarray(a)
+        assert a.dtype in (np.float32, np.float64), (name, a.dtype)
+        np.save(os.path.join(out_dir, name + ".npy"), a)
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons DURING the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks / throttle reasons DURING the timed region (read-only queries)."""
     Q = ("clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,"
          "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,"
          "clocks_event_reasons.sw_power_cap")
@@ -216,7 +220,7 @@ def time_steps(fn, steps, warmup, torch, sync_all=None):
 
 def gpu_baselines_pairwise(x, y, out, m, n, k, ours_ms, torch, steps=5, warm=2):
     """GPU baselines for configs[1] (L2Expanded m x n x k fp32), timed like the engine (CUDA events, output buffer
-    reused; every step streams 40+ GB through the 126 MB L2, so nothing is cached between steps)."""
+    reused; every step streams 40+ GB through the 50 MB L2, so nothing is cached between steps)."""
     import baseline
     res = {}
     dev = x.device
@@ -241,7 +245,8 @@ def gpu_baselines_pairwise(x, y, out, m, n, k, ours_ms, torch, steps=5, warm=2):
         del xn, yn, ws
     except Exception as e:  # noqa: BLE001
         res["cublaslt_sgemm_composition"] = {"unavailable": repr(e)[:200]}
-    # (ii) torch.cdist (cuBLAS SGEMM path, TF32 off = torch default) -- needs its own 40 GB result (+ temporaries)
+    # (ii) torch.cdist (cuBLAS SGEMM path, TF32 off = torch default) -- needs its own 40 GB result (+ temporaries),
+    #      more than an 80 GB card has left next to the engine's output: then reported as unavailable
     try:
         torch.backends.cuda.matmul.allow_tf32 = False
         fn = lambda: torch.cdist(x, y, p=2.0, compute_mode="use_mm_for_euclid_dist")
@@ -333,6 +338,14 @@ def run_pairwise_1gpu(args):
     out.fill_(float("nan"))
     with ClockSampler(0) as cs:
         ms, per = time_steps(fn_counted, args.steps, args.warmup, torch)
+    if args.dump_outputs:
+        # the last timed step's [m, n] result, sampled: 2M seeded (row, column) pairs (the full matrix is 40 GB)
+        g = torch.Generator(device=dev).manual_seed(7)
+        ri = torch.randint(0, m, (1 << 21,), device=dev, generator=g)
+        ci = torch.randint(0, n, (1 << 21,), device=dev, generator=g)
+        dump_outputs(args.dump_outputs, {"distance_sample": out[ri, ci].cpu().numpy(),
+                                         "sample_rows": ri.double().cpu().numpy(),
+                                         "sample_cols": ci.double().cpu().numpy()})
     kbuf = (ctypes.c_float * max(1, args.steps))()
     kcnt = ctypes.c_int(0)
     _lib.check(L.b2d_profile_end(kbuf, max(1, args.steps), ctypes.byref(kcnt)))
@@ -347,12 +360,11 @@ def run_pairwise_1gpu(args):
     alg_bytes = 4 * (m * k + n * k) + 4 * m * n
     roof = {"bound": "hbm", "achieved": alg_bytes / (k_ms * 1e-3) / 1e9, "peak": peaks["hbm_gbs"], "unit": "GB/s",
             "peak_source": f"{peak_src} (MEASURED_PEAKS.json hbm_gbs, copy read+write)",
-            "kernel": "expanded_tc_kernel (tcgen05, EPI_STORE): mean launch duration over the timed steps, CUDA events "
+            "kernel": "expanded_tc_kernel (wgmma, EPI_STORE): mean launch duration over the timed steps, CUDA events "
                       "on the launching stream (b2d_profile_begin/end)",
             "kernel_ms": k_ms, "launches_timed": len(kernel_ms),
             "whole_step": {"achieved": alg_bytes / (ms * 1e-3) / 1e9, "frac": alg_bytes / (ms * 1e-3) / 1e9 / peaks["hbm_gbs"],
-                           "note": "the same bytes over the whole step, i.e. incl. the two operand-prep launches"},
-            "traffic": ncu_traffic("pairwise_100k")}
+                           "note": "the same bytes over the whole step, i.e. incl. the two operand-prep launches"}}
     roof["frac"] = roof["achieved"] / roof["peak"]
     # ---- GPU baselines on the same shapes, same process, same timing method
     gpu_bl = gpu_baselines_pairwise(x, y, out, m, n, k, ms, torch)
@@ -380,7 +392,7 @@ def run_pairwise_1gpu(args):
         others[f"{name} 50000x50000x256 f32"] = {
             "ms": ms_o, "pairs_per_s": m3 * m3 / (ms_o * 1e-3),
             "hbm_gbs": (8.0 * m3 * k3 + 4.0 * m3 * m3) / (ms_o * 1e-3) / 1e9,
-            "fp32_lane_ops_per_s": 2.0 * m3 * m3 * k3 / (ms_o * 1e-3), "bound": "fp32 pipe (148 SMs x 128 lanes x clk)",
+            "fp32_lane_ops_per_s": 2.0 * m3 * m3 * k3 / (ms_o * 1e-3), "bound": "fp32 pipe (132 SMs x 128 lanes x clk)",
             "parity": chk(out3, x3, y3, mt)}
     del x3, y3
     # fused brute-force kNN (SURVEY.md 8(f2)): top-16 of every row of the 100000x100000x128 problem, matrix never written
@@ -454,8 +466,8 @@ def run_pairwise_1gpu(args):
             "vs_baseline": None, "dtype": "f32",
             "data": "synthetic make_blobs-like (5 centres U[-10,10]^k, sigma 1, seeds 1234/4321), generated on device",
             "config": {"workload": "pairwise_distance L2Expanded 100000x100000x128 fp32 -> fp32 [m,n]",
-                       "precision": "fp32-grade: 3-term fp16 hi/lo split, fp32 accumulate in TMEM",
-                       "l2": "every step streams 40 GB of output through the 126 MB L2 (no reuse across steps)"},
+                       "precision": "fp32-grade: 3-term fp16 hi/lo split, fp32 accumulate (wgmma)",
+                       "l2": "every step streams 40 GB of output through the 50 MB L2 (no reuse across steps)"},
             "roofline": roof, "parity": parity, "gpu_baselines": gpu_bl, "cpu_baseline": cb, "e2e": e2e,
             "gpu_launches": 3 * args.steps, "clocks": clocks, "fused_l2_nn": nn, "other_configs": others,
             "ms_per_step_all": [round(v, 4) for v in per]}
@@ -539,6 +551,9 @@ def run_fused_nn_multi(args):
     if world > 1:
         dist.all_reduce(t, op=dist.ReduceOp.MAX)
     ms = float(t.item())
+    if rank == 0 and args.dump_outputs:   # the last timed step's reduced result: (index, squared distance) per query
+        dump_outputs(args.dump_outputs, {"nn_index": last["iv"][0].double().cpu().numpy(),
+                                         "nn_distance": last["iv"][1].float().cpu().numpy()})
     # ---- parity on EVERY rank: the reduced result vs the exact fp64 arg-min (own shard, combined across ranks)
     g = torch.Generator(device=dev).manual_seed(3)
     rows = torch.randperm(m, device=dev, generator=g)[:8192]
@@ -587,9 +602,8 @@ def run_fused_nn_multi(args):
         tf = 2.0 * m * n * k / (ms * 1e-3) / 1e12
         roof = {"bound": "tensor", "achieved": tf, "peak": peaks["bf16_tflops_sustained"] * world, "unit": "TFLOP/s",
                 "peak_source": f"{peak_src} (MEASURED_PEAKS.json bf16_tflops_sustained x n_gpus)",
-                "kernel": "screen_tc_kernel (tcgen05, 1-product screen) + expanded_tc_kernel (EPI_MINLOC, exact on 1/32 of "
-                          "the db blocks and wherever screening is called off); algorithmic 2mnk FLOP / time",
-                "traffic": ncu_traffic("screen_tc_per_launch")}
+                "kernel": "screen_tc_kernel (wgmma, 1-product screen) + expanded_tc_kernel (EPI_MINLOC, exact on 1/32 of "
+                          "the db blocks and wherever screening is called off); algorithmic 2mnk FLOP / time"}
         roof["frac"] = roof["achieved"] / roof["peak"]
         cb, _, _ = cpu_baseline("fused_l2_nn", seconds_budget=8.0)
         from raft_b200.distance.fused_l2_nn import plan_exchanges
@@ -604,7 +618,7 @@ def run_fused_nn_multi(args):
                 "config": {"workload": "fusedL2NN 1000000 queries x 8000000 db x 96 fp32, db row-sharded",
                            "parallelism": f"db_shard{world}",
                            "exchange": f"{n_calls} x all_reduce(int64 MIN) of 1M packed (dist,idx) keys per step (bounds between sub-chunks of the shard, result at the end)",
-                           "l2": "db shard + queries exceed L2 for world<=8 (>=768 MB per rank)"},
+                           "l2": "db shard + queries exceed the 50 MB L2 for world<=8 (>=768 MB per rank)"},
                 "roofline": roof, "parity": parity, "cpu_baseline": cb,
                 "e2e": None, "gpu_launches": nn_launches(n // world, world) * args.steps, "clocks": cs.summary(),
                 "ms_per_step_all": [round(v, 3) for v in per]}
@@ -648,6 +662,8 @@ def main():
     ap.add_argument("--steps", type=int, default=10)
     ap.add_argument("--warmup", type=int, default=3)
     ap.add_argument("--impl", default="ours", choices=["ours", "reference"])
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write what the timed path computed in its last step to DIR/<name>.npy")
     args = ap.parse_args()
     args.warmup = max(args.warmup, 3) if args.impl == "ours" else args.warmup
     if args.impl == "reference":

@@ -1,5 +1,5 @@
 // raft::distance::pairwise_distance -- header-only shim with the signatures of the removed
-// raft/distance/distance.cuh, dispatching through the C ABI (include/raft_b200.h) into the sm_100a
+// raft/distance/distance.cuh, dispatching through the C ABI (include/raft_b200.h) into the sm_90a
 // kernels.  Call shapes kept (verbatim from the surviving callers):
 //   pairwise_distance(handle, x, y, dist, m, n, k, metric)             cpp/include/raft/stats/detail/silhouette_score.cuh:205-206
 //   pairwise_distance(handle, x, y, dist, m, n, k, metric, isRowMajor, metric_arg)

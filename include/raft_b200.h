@@ -1,7 +1,7 @@
-/* raft_b200 -- C ABI of the B200-native pairwise-distance / fusedL2NN engine.
+/* raft_b200 -- C ABI of the H100-native pairwise-distance / fusedL2NN engine.
  *
  * This is the drop-in boundary: every entry point below is what a RAFT-side binding for the
- * distance path would call.  Reference interfaces replaced (all relative to /root/reference;
+ * distance path would call.  Reference interfaces replaced (all relative to the reference snapshot;
  * the distance sources themselves were deleted upstream in raft 26.02, CHANGELOG.md:59, so the
  * citations are the surviving call sites / patterns -- see SURVEY.md section 8(a),(b)):
  *
@@ -27,7 +27,7 @@
  * *_workspace_bytes query -- the counterpart of the handle's workspace memory resource,
  * cpp/include/raft/core/resource/device_memory_resource.hpp:100-129), is thread-safe, and
  * returns a status code instead of throwing.  There is no CPU fallback: on a machine without
- * an sm_100 GPU every compute entry point returns B2D_ERR_CUDA.
+ * an sm_90 GPU every compute entry point returns B2D_ERR_CUDA.
  */
 #ifndef RAFT_B200_H_
 #define RAFT_B200_H_

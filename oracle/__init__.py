@@ -3,7 +3,7 @@
 Only tests/, __graft_entry__.smoke() and bench.py's cpu_baseline / --impl reference legs
 may import this package.  The product (raft_b200) never does.
 
-PARITY UNPINNED: the reference snapshot (/root/reference, raft 26.06) no longer contains
+PARITY UNPINNED: the reference snapshot (raft 26.06) no longer contains
 raft::distance (removed upstream in 26.02, CHANGELOG.md:59), so no reference test pins
 results at this boundary.  The oracle restates the metric definitions (identical to
 scipy.spatial.distance.cdist) in fp64 and is pinned against

@@ -1,4 +1,4 @@
-"""Build the sm_100a CUDA library in-tree (raft_b200/libraft_b200.so) with nvcc."""
+"""Build the sm_90a CUDA library in-tree (raft_b200/libraft_b200.so) with nvcc."""
 from __future__ import annotations
 
 import os
@@ -10,7 +10,7 @@ CSRC = os.path.join(_HERE, "csrc")
 SO_PATH = os.path.join(_HERE, "libraft_b200.so")
 
 NVCC_FLAGS = [
-    "-std=c++17", "-O3", "-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo",
+    "-std=c++17", "-O3", "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo",
     "--expt-relaxed-constexpr", "-shared", "-Xcompiler", "-fPIC",
 ]
 

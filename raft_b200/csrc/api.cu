@@ -14,7 +14,6 @@
 
 #include "../../include/raft_b200.h"
 #include "expanded_tc.cuh"
-#include "expanded_tc2.cuh"
 #include "screen_tc.cuh"
 #include "prep.cuh"
 #include "unexpanded_simt.cuh"
@@ -178,8 +177,8 @@ static TcWorkspace tc_layout(void* base, int64_t m, int64_t n, int64_t k, bool w
   // screened fusedL2NN scratch: thresholds, counters, candidate list (128 per row and 1M-row chunk of y;
   // ~54 measured on far-from-origin clusters; overflow falls back to the exact pass on the device,
   // never to a wrong answer)
-  // (+2^19: the coarse kernel's warps take list slots in blocks of 64 -- 148 x 16 warps x 2 launches leave up to
-  // ~300k slots unused, which must not look like an overflow when m is small)
+  // (+2^19: the coarse kernel's warps take list slots in blocks of 64 -- 132 x 8 warps x 2 launches leave up to
+  // ~135k slots unused, which must not look like an overflow when m is small)
   w.cand_cap = with_keys ? static_cast<unsigned>(std::min<int64_t>(128 * m + (1 << 19), 0x7fffffff)) : 0u;
   w.aux      = reinterpret_cast<float4*>(c + take(with_keys ? static_cast<size_t>(m) * 16 : 0));
   w.cand_cnt = reinterpret_cast<unsigned*>(c + take(with_keys ? 32 : 0));
@@ -235,89 +234,28 @@ static int launch_prep(cudaStream_t s, const TcWorkspace& w, const void* x, int6
   return B2D_OK;
 }
 
-// dist [m][n] fp32 (row pitch ldd) seen as [m][chunks of 128 columns][128]: box {132, 2, 8} = 8 rows x 2 chunks, the
-// 4 trailing floats of every chunk fall outside dimension 0 and are never written (padded smem rows, see
-// expanded_tc.cuh).  `first_col`/`cols`: the column range the map covers (the ragged last chunk has its own map).
-static int make_dist_map3(CUtensorMap* map, const float* base, int64_t m, int64_t first_col, int64_t cols, int64_t ldd)
-{
-  EncodeTiledFn enc = get_encode();
-  if (!enc) return fail(B2D_ERR_CUDA, "cuTensorMapEncodeTiled entry point unavailable (no CUDA driver?)");
-  const cuuint64_t inner = cols >= 128 ? 128 : static_cast<cuuint64_t>(cols);
-  cuuint64_t dims[3]    = {inner, static_cast<cuuint64_t>(cols >= 128 ? cols / 128 : 1), static_cast<cuuint64_t>(m)};
-  cuuint64_t strides[2] = {512, static_cast<cuuint64_t>(ldd) * 4};
-  cuuint32_t box[3]     = {132, 2, 8};
-  cuuint32_t estr[3]    = {1, 1, 1};
-  CUresult r = enc(map, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 3, const_cast<float*>(base + first_col), dims, strides, box, estr,
-                   CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_NONE,
-                   CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  if (r != CUDA_SUCCESS) return fail(B2D_ERR_CUDA, "cuTensorMapEncodeTiled(dist) failed: " + std::to_string((int)r));
-  return B2D_OK;
-}
-
-template <bool kRes, int kEpi, int kPost, bool kTma>
-static int launch_tc_inst(cudaStream_t s, const CUtensorMap& ma, const CUtensorMap& mb, const CUtensorMap& md,
-                          const CUtensorMap& mr, const TcParams& p, int grid)
+template <bool kRes, int kEpi, int kPost>
+static int launch_tc_inst(cudaStream_t s, const CUtensorMap& ma, const CUtensorMap& mb, const TcParams& p, int grid)
 {
   // the attribute is per device and per function: cheap, set on every launch
-  B2D_CUDA(cudaFuncSetAttribute(expanded_tc_kernel<kRes, kEpi, kPost, kTma>,
-                                cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(TC_SMEM_BYTES)));
-  expanded_tc_kernel<kRes, kEpi, kPost, kTma><<<grid, TC_THREADS, TC_SMEM_BYTES, s>>>(ma, mb, md, mr, p);
+  B2D_CUDA(cudaFuncSetAttribute(expanded_tc_kernel<kRes, kEpi, kPost>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                static_cast<int>(TC_SMEM_BYTES)));
+  expanded_tc_kernel<kRes, kEpi, kPost><<<grid, TC_THREADS, TC_SMEM_BYTES, s>>>(ma, mb, p);
   B2D_CUDA(cudaGetLastError());
   return B2D_OK;
 }
 
-template <bool kRes, bool kTma>
-static int launch_tc_store(cudaStream_t s, const CUtensorMap& ma, const CUtensorMap& mb, const CUtensorMap& md,
-                           const CUtensorMap& mr, const TcParams& p, int grid, int post)
+template <bool kRes>
+static int launch_tc_epi(cudaStream_t s, const CUtensorMap& ma, const CUtensorMap& mb, const TcParams& p, int grid, int epi,
+                         int post)
 {
-  if (post == POST_NONE) return launch_tc_inst<kRes, EPI_STORE, POST_NONE, kTma>(s, ma, mb, md, mr, p, grid);
-  if (post == POST_CLAMP) return launch_tc_inst<kRes, EPI_STORE, POST_CLAMP, kTma>(s, ma, mb, md, mr, p, grid);
-  if (post == POST_JACCARD) return launch_tc_inst<kRes, EPI_STORE, POST_JACCARD, false>(s, ma, mb, md, mr, p, grid);
-  if (post == POST_DICE) return launch_tc_inst<kRes, EPI_STORE, POST_DICE, false>(s, ma, mb, md, mr, p, grid);
-  return launch_tc_inst<kRes, EPI_STORE, POST_CLAMP_SQRT, kTma>(s, ma, mb, md, mr, p, grid);
-}
-
-static std::atomic<int> g_pair_kernel{0};  // b2d_set_option("pairwise_2cta", 1): the CTA-pair kernel (expanded_tc2.cuh) for k <= 128
-
-// K1, 2-CTA form (expanded_tc2.cuh): EPI_STORE, k <= 128, aligned output
-template <int kPost>
-static int launch_tc2_inst(cudaStream_t s, const CUtensorMap& ma, const CUtensorMap& mb, const CUtensorMap& md,
-                           const TcParams& p, int grid)
-{
-  B2D_CUDA(cudaFuncSetAttribute(expanded_tc2_kernel<kPost>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                static_cast<int>(T2_SMEM_BYTES)));
-  expanded_tc2_kernel<kPost><<<grid, T2_THREADS, T2_SMEM_BYTES, s>>>(ma, mb, md, p);
-  B2D_CUDA(cudaGetLastError());
-  return B2D_OK;
-}
-
-static int launch_tc2(cudaStream_t s, const TcWorkspace& w, TcParams p, int64_t k, int post, int sms)
-{
-  p.nkb     = static_cast<int>((k + 31) / 32);
-  p.tiles_m = static_cast<int>((p.m + TC_BM - 1) / TC_BM);
-  p.tiles_n = static_cast<int>((p.n + TC_BN - 1) / TC_BN);
-  const int clusters  = std::max(1, sms / 2);
-  const int pairs_m   = (p.tiles_m + 1) / 2;
-  const int64_t total = static_cast<int64_t>(pairs_m) * p.tiles_n;
-  int64_t chunk       = total / (static_cast<int64_t>(clusters) * 6);
-  chunk               = std::max<int64_t>(1, std::min<int64_t>(chunk, 16));
-  chunk               = std::min<int64_t>(chunk, pairs_m);
-  p.chunk    = static_cast<int>(chunk);        // PAIRS of x tiles per work item
-  p.chunks_m = (pairs_m + p.chunk - 1) / p.chunk;
-  p.n_items  = static_cast<int64_t>(p.tiles_n) * p.chunks_m;
-  p.xt = w.xt; p.yt = w.yt; p.coef = w.coef; p.has_lo = w.has_lo; p.xsc = w.xsc; p.ysc = w.ysc; p.nonuni = w.nonuni;
-  if (p.n_items == 0) return B2D_OK;
-  CUtensorMap ma, mb, md;
-  memset(&md, 0, sizeof(md));
-  int rc = make_operand_map(&ma, w.xop, p.m, p.nkb, TC_BM);
-  if (rc) return rc;
-  rc = make_operand_map(&mb, w.yop, p.n, p.nkb, 128);   // each CTA of a pair loads ITS 128 rows of the y block
-  if (rc) return rc;
-  if (p.n >= 128) { rc = make_dist_map3(&md, p.dist, p.m, 0, p.n / 128 * 128, p.ldd); if (rc) return rc; }
-  const int grid = 2 * static_cast<int>(std::min<int64_t>(p.n_items, clusters));
-  if (post == POST_NONE) return launch_tc2_inst<POST_NONE>(s, ma, mb, md, p, grid);
-  if (post == POST_CLAMP) return launch_tc2_inst<POST_CLAMP>(s, ma, mb, md, p, grid);
-  return launch_tc2_inst<POST_CLAMP_SQRT>(s, ma, mb, md, p, grid);
+  if (epi == EPI_MINLOC) return launch_tc_inst<kRes, EPI_MINLOC, POST_NONE>(s, ma, mb, p, grid);
+  if (epi == EPI_TOPK) return launch_tc_inst<kRes, EPI_TOPK, POST_NONE>(s, ma, mb, p, grid);
+  if (post == POST_NONE) return launch_tc_inst<kRes, EPI_STORE, POST_NONE>(s, ma, mb, p, grid);
+  if (post == POST_CLAMP) return launch_tc_inst<kRes, EPI_STORE, POST_CLAMP>(s, ma, mb, p, grid);
+  if (post == POST_JACCARD) return launch_tc_inst<kRes, EPI_STORE, POST_JACCARD>(s, ma, mb, p, grid);
+  if (post == POST_DICE) return launch_tc_inst<kRes, EPI_STORE, POST_DICE>(s, ma, mb, p, grid);
+  return launch_tc_inst<kRes, EPI_STORE, POST_CLAMP_SQRT>(s, ma, mb, p, grid);
 }
 
 static int launch_tc(cudaStream_t s, const TcWorkspace& w, TcParams p, int64_t k, int epi, int post, int kb0 = 0,
@@ -326,7 +264,7 @@ static int launch_tc(cudaStream_t s, const TcWorkspace& w, TcParams p, int64_t k
   int sms = 0, cc = 0;
   int rc  = device_sms(&sms, &cc);
   if (rc) return rc;
-  if (cc != 10) return fail(B2D_ERR_CUDA, "raft_b200 requires an sm_100 (B200) device; found cc major " + std::to_string(cc));
+  if (cc != 9) return fail(B2D_ERR_CUDA, "raft_b200 requires an sm_90 (H100) device; found cc major " + std::to_string(cc));
   const int nkb_total = static_cast<int>((k + 31) / 32);
   p.nkb     = nkb_chunk ? nkb_chunk : nkb_total;
   p.tiles_m = static_cast<int>((p.m + TC_BM - 1) / TC_BM);
@@ -348,51 +286,15 @@ static int launch_tc(cudaStream_t s, const TcWorkspace& w, TcParams p, int64_t k
   p.ysc      = w.ysc;
   p.nonuni   = w.nonuni;
   if (p.n_items == 0) return B2D_OK;
-  CUtensorMap ma, mb, md, mr;
-  memset(&md, 0, sizeof(md));
-  memset(&mr, 0, sizeof(mr));
+  const bool resident = p.nkb <= TC_MAX_RES_KB;
+  CUtensorMap ma, mb;
   rc = make_operand_map(&ma, w.xop, p.m, p.nkb, TC_BM, kb0, nkb_total);
   if (rc) return rc;
-  rc = make_operand_map(&mb, w.yop, p.n, p.nkb, TC_BN, kb0, nkb_total);
+  // resident: the whole 256-row y block in one box per k-block; streaming: one 128-row half per stage
+  rc = make_operand_map(&mb, w.yop, p.n, p.nkb, resident ? TC_BN : TC_HN, kb0, nkb_total);
   if (rc) return rc;
-  const int grid      = static_cast<int>(p.n_items < sms ? p.n_items : sms);
-  const bool resident = p.nkb <= TC_MAX_RES_KB;
-  if (epi == EPI_MINLOC) {
-    return resident ? launch_tc_inst<true, EPI_MINLOC, POST_NONE, false>(s, ma, mb, md, mr, p, grid)
-                    : launch_tc_inst<false, EPI_MINLOC, POST_NONE, false>(s, ma, mb, md, mr, p, grid);
-  }
-  if (epi == EPI_TOPK) {
-    return resident ? launch_tc_inst<true, EPI_TOPK, POST_NONE, false>(s, ma, mb, md, mr, p, grid)
-                    : launch_tc_inst<false, EPI_TOPK, POST_NONE, false>(s, ma, mb, md, mr, p, grid);
-  }
-  // bulk row stores (cp.async.bulk shared -> global) need 16-byte aligned addresses and sizes, i.e. a
-  // 16-byte aligned base and row pitch and n % 4 == 0; ragged or unaligned outputs take the direct
-  // register->global path
-  bool tma = (reinterpret_cast<uintptr_t>(p.dist) % 16 == 0) && (p.ldd % 4 == 0) && (p.n % 4 == 0) &&
-             p.acc_mode == 0 && post < POST_JACCARD;  // the K-chunked read-modify-write epilogue lives in the direct path
-  // k <= 128 with an aligned output: the CTA-pair kernel (full-width output rows, expanded_tc2.cuh)
-  if (tma && resident && p.sel_s <= 1 && p.run_flag == nullptr && sms >= 2 && g_pair_kernel.load(std::memory_order_relaxed))
-    return launch_tc2(s, w, p, k, post, sms);
-  if (tma) {
-    // dist [m][n] fp32 (row pitch ldd), box = 32 x 32, SWIZZLE_128B (inner box = 128 bytes); edge clipping works in
-    // 16-byte units, hence n % 4 == 0 above
-    EncodeTiledFn enc = get_encode();
-    if (!enc) return fail(B2D_ERR_CUDA, "cuTensorMapEncodeTiled entry point unavailable (no CUDA driver?)");
-    cuuint64_t dims[2]    = {static_cast<cuuint64_t>(p.n), static_cast<cuuint64_t>(p.m)};
-    cuuint64_t strides[1] = {static_cast<cuuint64_t>(p.ldd) * 4};
-    cuuint32_t box[2]     = {32, 32};
-    cuuint32_t estr[2]    = {1, 1};
-    CUresult r = enc(&md, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, p.dist, dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                     CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_NONE, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    if (r != CUDA_SUCCESS) return fail(B2D_ERR_CUDA, "cuTensorMapEncodeTiled(dist) failed: " + std::to_string((int)r));
-    mr = md;
-    // k <= 64: the full-width store path of the same kernel (3-D box {132, 2, 8} over the 128-column chunks)
-    if (p.n >= 128) { rc = make_dist_map3(&mr, p.dist, p.m, 0, p.n / 128 * 128, p.ldd); if (rc) return rc; }
-    return resident ? launch_tc_store<true, true>(s, ma, mb, md, mr, p, grid, post)
-                    : launch_tc_store<false, true>(s, ma, mb, md, mr, p, grid, post);
-  }
-  return resident ? launch_tc_store<true, false>(s, ma, mb, md, mr, p, grid, post)
-                  : launch_tc_store<false, false>(s, ma, mb, md, mr, p, grid, post);
+  const int grid = static_cast<int>(p.n_items < sms ? p.n_items : sms);
+  return resident ? launch_tc_epi<true>(s, ma, mb, p, grid, epi, post) : launch_tc_epi<false>(s, ma, mb, p, grid, epi, post);
 }
 
 // coarse screening pass of the screened fusedL2NN (screen_tc.cuh) over the y blocks with
@@ -403,7 +305,7 @@ static int launch_screen(cudaStream_t s, const TcWorkspace& w, int64_t m, int64_
   int sms = 0, cc = 0;
   int rc  = device_sms(&sms, &cc);
   if (rc) return rc;
-  if (cc != 10) return fail(B2D_ERR_CUDA, "raft_b200 requires an sm_100 (B200) device; found cc major " + std::to_string(cc));
+  if (cc != 9) return fail(B2D_ERR_CUDA, "raft_b200 requires an sm_90 (H100) device; found cc major " + std::to_string(cc));
   ScreenParams p;
   memset(&p, 0, sizeof(p));
   p.m = m; p.n = n;
@@ -649,10 +551,8 @@ int b2d_set_option(const char* name, double value)
     g_nn_tau.store(static_cast<float>(value));
   } else if (n == "nn_screen") {
     g_nn_screen.store(value != 0.0 ? 1 : 0);
-  } else if (n == "pairwise_2cta") {
-    g_pair_kernel.store(value != 0.0 ? 1 : 0);
   } else {
-    return fail(B2D_ERR_INVALID_ARG, "unknown option '" + n + "' (nn_tau, nn_screen, pairwise_2cta)");
+    return fail(B2D_ERR_INVALID_ARG, "unknown option '" + n + "' (nn_tau, nn_screen)");
   }
   return B2D_OK;
 }
@@ -668,15 +568,6 @@ int b2d_debug_nn_stats(void* stream, const void* workspace, int64_t m, int64_t n
   return B2D_OK;
 }
 const char* b2d_last_error(void) { return g_err.c_str(); }
-#ifdef SC_TRACE
-int b2d_debug_screen_trace(long long* out_host)
-{
-  B2D_CUDA(cudaDeviceSynchronize());
-  B2D_CUDA(cudaMemcpyFromSymbol(out_host, g_sc_trace, sizeof(long long) * 8 * 4096));
-  B2D_CUDA(cudaMemcpyFromSymbol(out_host + 8 * 4096, g_sc_wtrace, sizeof(long long) * 3 * 16 * 2048));
-  return B2D_OK;
-}
-#endif
 
 size_t b2d_pairwise_workspace_bytes(int metric, int dtype, int64_t m, int64_t n, int64_t k)
 {
@@ -706,7 +597,7 @@ int b2d_pairwise_distance(void* stream, int metric, int dtype, const void* x, in
     if (ldx < m || ldy < n || ldd < m) return fail(B2D_ERR_INVALID_ARG, "leading dimension smaller than the column length");
   }
   if (!is_expanded(metric) && !is_unexpanded(metric))
-    return fail(B2D_ERR_UNSUPPORTED, "metric " + std::to_string(metric) + " is not on the B200 distance path");
+    return fail(B2D_ERR_UNSUPPORTED, "metric " + std::to_string(metric) + " is not on the tensor-core / SIMT distance path");
   if (dtype != B2D_F32 && dtype != B2D_F16 && dtype != B2D_F64) return fail(B2D_ERR_UNSUPPORTED, "dtype");
   if (metric == B2D_LpUnexpanded && !(metric_arg > 0.f)) return fail(B2D_ERR_INVALID_ARG, "LpUnexpanded needs p > 0");
   if (dtype == B2D_F64) {   // double in / double out: the SIMT fp64 path, every metric
@@ -783,7 +674,7 @@ int b2d_pairwise_distance(void* stream, int metric, int dtype, const void* x, in
   int cc = 0, sms = 0;
   int rc = device_sms(&sms, &cc);
   if (rc) return rc;
-  if (cc != 10) return fail(B2D_ERR_CUDA, "raft_b200 requires an sm_100 (B200) device");
+  if (cc != 9) return fail(B2D_ERR_CUDA, "raft_b200 requires an sm_90 (H100) device");
   switch (metric) {
     case B2D_L1: return launch_ux_inst<UX_L1>(s, p, tiles);
     case B2D_L2Unexpanded: return launch_ux_inst<UX_L2>(s, p, tiles);
@@ -1277,7 +1168,7 @@ int b2d_silhouette_score(void* stream, float* score, float* per_sample, const fl
   if (n_labels > 12000) return fail(B2D_ERR_UNSUPPORTED, "n_labels > 12000");
   if (ldx < k) return fail(B2D_ERR_INVALID_ARG, "leading dimension smaller than k");
   const size_t need = b2d_silhouette_score_workspace_bytes(n, k, n_labels, metric, chunk_rows);
-  if (need == static_cast<size_t>(-1)) return fail(B2D_ERR_UNSUPPORTED, "metric " + std::to_string(metric) + " is not on the B200 distance path");
+  if (need == static_cast<size_t>(-1)) return fail(B2D_ERR_UNSUPPORTED, "metric " + std::to_string(metric) + " is not on the tensor-core / SIMT distance path");
   if (!workspace || workspace_bytes < need)
     return fail(B2D_ERR_WORKSPACE, "workspace too small: need " + std::to_string(need) + " bytes");
   if (reinterpret_cast<uintptr_t>(workspace) % 256) return fail(B2D_ERR_INVALID_ARG, "workspace must be 256-byte aligned");
@@ -1372,7 +1263,7 @@ int b2d_trustworthiness_score(void* stream, double* score, const float* x, int64
     return fail(B2D_ERR_INVALID_ARG, "n_neighbors must be smaller than n / 2");
   if (ldx < m || lde < d) return fail(B2D_ERR_INVALID_ARG, "leading dimension smaller than the row length");
   const size_t need = b2d_trustworthiness_score_workspace_bytes(n, m, d, n_neighbors, metric, batch_rows);
-  if (need == static_cast<size_t>(-1)) return fail(B2D_ERR_UNSUPPORTED, "metric " + std::to_string(metric) + " is not on the B200 distance path");
+  if (need == static_cast<size_t>(-1)) return fail(B2D_ERR_UNSUPPORTED, "metric " + std::to_string(metric) + " is not on the tensor-core / SIMT distance path");
   if (!workspace || workspace_bytes < need)
     return fail(B2D_ERR_WORKSPACE, "workspace too small: need " + std::to_string(need) + " bytes");
   if (reinterpret_cast<uintptr_t>(workspace) % 256) return fail(B2D_ERR_INVALID_ARG, "workspace must be 256-byte aligned");

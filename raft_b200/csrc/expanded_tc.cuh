@@ -1,4 +1,4 @@
-// K1 / K3: expanded-form metrics on tcgen05 tensor cores (sm_100a).
+// K1 / K3: expanded-form metrics on Hopper tensor cores (sm_90a, wgmma).
 //
 // Replaces the pair loop of raft::distance::pairwise_distance for L2Expanded / L2SqrtExpanded /
 // CosineExpanded / CorrelationExpanded / InnerProduct (+ Hellinger, RusselRao) and of
@@ -7,45 +7,36 @@
 // port of it).
 //
 // Numerics: fp32 inputs are pre-split (prep.cuh) into fp16 hi/lo with one power-of-two scale per
-// matrix; acc = hi*hi + hi*lo + lo*hi accumulates in fp32 in TMEM (products of fp16 pairs are
-// exact in fp32), i.e. ~22 significant bits per operand -- fp32-grade, same idea as the
-// reference's 3xTF32 but at the 2x higher kind::f16 rate and with 4 B/element staged instead of 8.
-// The tensor core aligns every product to the accumulator's exponent and truncates, so the error
-// grows with the number of MMAs that touch a LARGE accumulator: the 2^-11-sized cross terms must
-// not be mixed into the running hi*hi sum (measured: 1.0e-4 -> 4.5e-5 max relative error at k = 128).
+// matrix; acc = hi*hi + hi*lo + lo*hi accumulates in fp32 (products of fp16 pairs are exact in
+// fp32), i.e. ~22 significant bits per operand -- fp32-grade, same idea as the reference's 3xTF32
+// but at the 2x higher fp16 rate and with 4 B/element staged instead of 8.  The tensor core aligns
+// every product to the accumulator's exponent and truncates, so the error grows with the number of
+// MMAs that touch a LARGE accumulator: the 2^-11-sized cross terms are kept in an accumulator of
+// their own and added to the hi*hi sum in the epilogue with one round-to-nearest fp32 add.
 // Operands that are exact in fp16 (fp16 inputs, small integers) skip the cross terms altogether.
 //
-// Structure (one persistent CTA per SM, 320 threads):
-//   warp 0     TMA producer    cp.async.bulk.tensor 2-D, SWIZZLE_128B, mbarrier complete_tx
-//   warp 1     MMA issuer      warp-uniform loop, one elected lane issues tcgen05.mma.kind::f16
-//   warps 2-9  epilogue        warp w reads TMEM lane quarter (w & 3); warps 2-5 own the left 128
-//                              columns of every tile, warps 6-9 the right 128
-// Work item = (256-row block of y, run of 128-row tiles of x); tile = 128 x 256 outputs.
+// Structure (one persistent CTA per SM, 384 threads = 3 warpgroups):
+//   warpgroup 0     TMA producer: warp 0, one elected lane issues cp.async.bulk.tensor 2-D loads
+//                   (SWIZZLE_128B, mbarrier complete_tx); the other warps only hand their registers over
+//   warpgroups 1-2  consumers: warpgroup c owns rows [64c, 64c+64) of every x tile; it issues the
+//                   wgmma.m64n128k16 of its rows and runs the epilogue on the accumulator fragments
+// Work item = (256-row block of y, run of 128-row tiles of x); every x tile is worked through as two
+// 128 x 128 halves (one per 128-row half of the y block): main (hi*hi) + cross accumulators of a
+// 64 x 128 warpgroup tile are 128 fp32 registers per thread.
 //
 //  kResident (k <= 128): the y block (all of K, <= 128 KB) stays in shared memory for the whole run;
-//    x tiles stream through a ring of 16 KB stages (6, or 4 when the TMA-store staging block takes
-//    the other 32 KB).  Each tile is a TWO-PASS N=256 MMA sequence into ONE 256-column accumulator:
-//    first every cross term of every k-block (accumulator still tiny), then every hi*hi term --
-//    2 large-accumulator MMAs per k-block, N=256 instructions (96 B/clk of shared-memory operand
-//    reads instead of 128 B/clk for N=128), TMEM double-buffered across tiles (2 x 256 columns).
-//  !kResident (k > 128): both operands stream per k-block (4 stages of 48 KB); a tile is two 128-column
-//    halves, each with its own `main` and `cross` accumulator (4 x 128 = all 512 TMEM columns).
+//    x k-blocks stream through a ring of 16 KB stages.
+//  !kResident (k > 128): both operands stream per k-block (stages of 16 KB of x + 16 KB of the y half).
 //
-// Epilogues: d = acc * c + (t_x[i] + t_y[j]) on packed f32x2 pipes (FADD2/FFMA2; c is one scalar)
-//   EPI_STORE, kTma   (dist 16-byte aligned, n % 4 == 0) tcgen05.ld.32x32b (thread == row), clamp /
-//                     sqrt, 32x32 block staged in shared memory with the 128-byte XOR swizzle, one
-//                     TMA tensor store per warp per 32 columns -- whole 128-byte lines, hardware
-//                     edge clipping.  Measured: 5.9 TB/s is the ceiling of every store mechanism
-//                     for this tile footprint at full clock (scripts/probes/).
-//   EPI_STORE, !kTma  tcgen05.ld.16x256b.x8 gives each thread 2 adjacent columns of 2 rows per
-//                     8-column group (the m16n8 fragment): registers go straight to global memory,
-//                     a warp-wide 8-byte store writes 8 rows x one full 32-byte sector.  Also the
+// Epilogues (straight from the registers; d = acc * c + (t_x[i] + t_y[j]), c one scalar):
+//   EPI_STORE         each thread holds 2 adjacent columns of 2 rows per 8-column group: a warp-wide
+//                     8-byte streaming store writes 8 rows x one full 32-byte sector.  Also the
 //                     read-modify-write path of K-chunked accumulation (k > 320).
-//   EPI_MINLOC        16x256b fragments; per row an FMNMX3 tree over the thread's 16 values is
-//                     compared with the row's current global best (read from keys at tile start:
-//                     an upper bound, keys only decrease); only a candidate that can change the
-//                     result takes the slow path (smallest-column scan + packed 64-bit atomicMin).
-//   EPI_TOPK          fused brute-force kNN: the same tree and vote against the row's current k-th best;
+//   EPI_MINLOC        per row the minimum of the thread's 16 values of a 64-column chunk is compared with
+//                     the row's current global best (read from keys at tile start: an upper bound, keys
+//                     only decrease); only a candidate that can change the result takes the slow path
+//                     (smallest-column scan + packed 64-bit atomicMin).
+//   EPI_TOPK          fused brute-force kNN: the same minimum and vote against the row's current k-th best;
 //                     every pair at or below it is appended to the row's candidate list (see the kNN
 //                     helpers at the end of this file).
 #pragma once
@@ -58,14 +49,15 @@ namespace b2d {
 
 constexpr int TC_BM          = 128;
 constexpr int TC_BN          = 256;
+constexpr int TC_HN          = 128;          // columns of one wgmma (half of a y block)
 constexpr int TC_A_BYTES     = TC_BM * 128;  // one k-block of A: 128 rows x 128 B
-constexpr int TC_B_BYTES     = TC_BN * 128;  // one k-block of B: 256 rows x 128 B
+constexpr int TC_B_BYTES     = TC_BN * 128;  // one k-block of the resident y block: 256 rows x 128 B
+constexpr int TC_BH_BYTES    = TC_HN * 128;  // one k-block of a streamed y half: 128 rows x 128 B
 constexpr int TC_MAX_RES_KB  = 4;            // resident-B variant: k <= 128
-constexpr int TC_STAGES_RES  = 6;            // A-only stages (16 KB) next to the resident y block
-constexpr int TC_STAGES_STR  = 4;            // A+B stages (48 KB) when both operands stream
+constexpr int TC_STAGES_RES  = 5;            // A-only stages (16 KB) next to the resident y block
+constexpr int TC_STAGES_STR  = 6;            // A + B-half stages (32 KB) when both operands stream
 constexpr int TC_MAX_STAGES  = 6;
-constexpr int TC_EPI_WARPS   = 8;
-constexpr int TC_THREADS     = 64 + 32 * TC_EPI_WARPS;
+constexpr int TC_THREADS     = 384;
 
 enum TcEpilogue : int { EPI_STORE = 0, EPI_MINLOC = 1, EPI_TOPK = 2 };
 // max(v, 0) that keeps a NaN (fmaxf(NaN, 0) = 0 would turn a poisoned distance into a perfect match)
@@ -77,7 +69,7 @@ __device__ __forceinline__ float clamp0(float v)
 }
 
 enum TcPost : int { POST_NONE = 0, POST_CLAMP = 1, POST_CLAMP_SQRT = 2,
-                    POST_JACCARD = 3,  // d = 1 - a / (s - a), a = <x,y>, s = |x|^2 + |y|^2 (0/0 -> 0): direct-store path only
+                    POST_JACCARD = 3,  // d = 1 - a / (s - a), a = <x,y>, s = |x|^2 + |y|^2 (0/0 -> 0)
                     POST_DICE    = 4 };  // d = 1 - 2 a / s
 
 // ratio metrics on the tensor path: a = acc * c (the inner product), s = t_x + t_y (the squared norms)
@@ -125,9 +117,8 @@ struct TcParams {
                           //     anything that matters was lost; rows where it was are redone by knn_fix_kernel)
 };
 
-constexpr size_t TC_SMEM_OPERANDS = (size_t)TC_MAX_RES_KB * TC_B_BYTES + (size_t)TC_STAGES_RES * TC_A_BYTES;  // 224 KB
-static_assert((size_t)TC_STAGES_STR * (TC_A_BYTES + TC_B_BYTES) <= TC_SMEM_OPERANDS, "streaming carve fits");
-constexpr int TC_STG_ROW      = 1024 + 32;  // k <= 64 store path: staged tile row = 2 chunks x (128 + 4) floats
+constexpr size_t TC_SMEM_OPERANDS = (size_t)TC_MAX_RES_KB * TC_B_BYTES + (size_t)TC_STAGES_RES * TC_A_BYTES;  // 208 KB
+static_assert((size_t)TC_STAGES_STR * (TC_A_BYTES + TC_BH_BYTES) <= TC_SMEM_OPERANDS, "streaming carve fits");
 constexpr size_t TC_SMEM_BYTES = TC_SMEM_OPERANDS + TC_BN * 4 + 256;
 static_assert(TC_SMEM_BYTES <= 232448, "exceeds the 227 KB per-CTA limit");
 
@@ -153,58 +144,13 @@ __device__ __forceinline__ int ordered_bits(float v)
   return b < 0 ? (b ^ 0x7FFFFFFF) : b;
 }
 
-// packed f32x2 helpers (FADD2 / FMUL2 / FFMA2: two fp32 lanes per issue slot)
-__device__ __forceinline__ uint64_t pk(float lo, float hi)
-{
-  uint64_t r;
-  asm("mov.b64 %0, {%1, %2};" : "=l"(r) : "f"(lo), "f"(hi));
-  return r;
-}
-__device__ __forceinline__ uint64_t pk(uint32_t lo, uint32_t hi)
-{
-  uint64_t r;
-  asm("mov.b64 %0, {%1, %2};" : "=l"(r) : "r"(lo), "r"(hi));
-  return r;
-}
-__device__ __forceinline__ void unpk(uint64_t v, float& lo, float& hi)
-{
-  asm("mov.b64 {%0, %1}, %2;" : "=f"(lo), "=f"(hi) : "l"(v));
-}
-__device__ __forceinline__ uint64_t add2(uint64_t a, uint64_t b)
-{
-  uint64_t r;
-  asm("add.rn.f32x2 %0, %1, %2;" : "=l"(r) : "l"(a), "l"(b));
-  return r;
-}
-__device__ __forceinline__ uint64_t mul2(uint64_t a, uint64_t b)
-{
-  uint64_t r;
-  asm("mul.rn.f32x2 %0, %1, %2;" : "=l"(r) : "l"(a), "l"(b));
-  return r;
-}
-__device__ __forceinline__ uint64_t fma2(uint64_t a, uint64_t b, uint64_t c)
-{
-  uint64_t r;
-  asm("fma.rn.f32x2 %0, %1, %2, %3;" : "=l"(r) : "l"(a), "l"(b), "l"(c));
-  return r;
-}
-__device__ __forceinline__ float min3(float a, float b, float c)
-{
-  float r;
-  asm("min.f32 %0, %1, %2, %3;" : "=f"(r) : "f"(a), "f"(b), "f"(c));
-  return r;
-}
+__device__ __forceinline__ float min3(float a, float b, float c) { return fminf(fminf(a, b), c); }
+__device__ __forceinline__ float max3(float a, float b, float c) { return fmaxf(fmaxf(a, b), c); }
 
-__device__ __forceinline__ float max3(float a, float b, float c)
-{
-  float r;
-  asm("max.f32 %0, %1, %2, %3;" : "=f"(r) : "f"(a), "f"(b), "f"(c));
-  return r;
-}
-
-// EPI_TOPK slow path (one row of one fragment: 16 values, columns col0 + 8 i + e): every value at or below the row's
-// k-th best so far takes a slot of the row's list; a full list keeps the smallest dropped key (knn_merge_kernel decides
-// from it whether the row must be repaired).  Deliberately NOT inlined, see the call site.
+// EPI_TOPK slow path (one row of one 64-column chunk: 16 values, columns col0 + 8 i + e): every value at or below the
+// row's k-th best so far takes a slot of the row's list; a full list keeps the smallest dropped key (knn_merge_kernel
+// decides from it whether the row must be repaired).  Deliberately NOT inlined: one copy instead of one per call site
+// keeps the kNN instantiation inside the instruction cache.
 __device__ __noinline__ void knn_append16(unsigned* cnt, long long* cand, unsigned cap, long long* dropmin, int64_t row,
                                           long long col0, float xn, float thr, float a0, float a1, float a2, float a3,
                                           float a4, float a5, float a6, float a7, float a8, float a9, float a10, float a11,
@@ -225,58 +171,191 @@ __device__ __noinline__ void knn_append16(unsigned* cnt, long long* cand, unsign
   }
 }
 
-template <bool kResident, int kEpi, int kPost, bool kTma>
-__global__ void __launch_bounds__(TC_THREADS, 1)
-expanded_tc_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b,
-                   const __grid_constant__ CUtensorMap tmap_d, const __grid_constant__ CUtensorMap tmap_r, const TcParams p)
+// Epilogue of one 64 x 128 warpgroup tile.  v[4i + 2j + e] holds row row0 + 8j, column gc0 + 8i + e of the accumulator
+// (main + cross already summed); on return (EPI_STORE) the values have been written.
+template <int kEpi, int kPost>
+__device__ __forceinline__ void tc_epilogue(float (&v)[64], const TcParams& p, const float* col_tb, int cl0, int64_t gc0,
+                                            int64_t row0, const float (&ta)[2], const float (&cfr)[2], float (&thr)[2],
+                                            const float (&xnr)[2], bool ynu)
 {
-  // kTma (EPI_STORE only): results leave through a swizzled shared-memory staging block and one TMA
-  // tensor store per warp per 32 columns (whole 128-byte lines); the 32 KB of staging replace two
-  // of the six x stages.
-  constexpr int kStages = kResident ? (kTma ? TC_STAGES_RES - 2 : TC_STAGES_RES) : TC_STAGES_STR;
+  // d = acc * c_row (* column factor) + (t_x + t_y); the arg-min modes leave the row-constant t_x out (added on the
+  // slow path only)
+#pragma unroll
+  for (int i = 0; i < 16; ++i) {
+    const float2 tb = *reinterpret_cast<const float2*>(&col_tb[cl0 + 8 * i]);
+    float sb0 = 1.f, sb1 = 1.f;
+    if (ynu) {  // rows of y with their own exponent: per-column factors straight from global memory (rare)
+      const int64_t gc = gc0 + 8 * i;
+      sb0 = gc < p.n ? __ldg(&p.ysc[gc]) : 1.f;
+      sb1 = gc + 1 < p.n ? __ldg(&p.ysc[gc + 1]) : 1.f;
+    }
+#pragma unroll
+    for (int j = 0; j < 2; ++j) {
+      float a0 = v[4 * i + 2 * j], a1 = v[4 * i + 2 * j + 1];
+      if (ynu) { a0 *= sb0; a1 *= sb1; }
+      if (kEpi == EPI_STORE && kPost >= POST_JACCARD) {
+        v[4 * i + 2 * j]     = post_ratio<kPost>(a0 * cfr[j], ta[j] + tb.x);
+        v[4 * i + 2 * j + 1] = post_ratio<kPost>(a1 * cfr[j], ta[j] + tb.y);
+      } else if (kEpi == EPI_STORE) {
+        v[4 * i + 2 * j]     = fmaf(a0, cfr[j], ta[j] + tb.x);
+        v[4 * i + 2 * j + 1] = fmaf(a1, cfr[j], ta[j] + tb.y);
+      } else {
+        v[4 * i + 2 * j]     = fmaf(a0, cfr[j], tb.x);
+        v[4 * i + 2 * j + 1] = fmaf(a1, cfr[j], tb.y);
+      }
+    }
+  }
+  if (kEpi == EPI_STORE) {
+    const bool fast = row0 + 8 < p.m && gc0 + 127 < p.n && p.pair_ok;
+    if (p.acc_mode >= 2) {
+      // K-chunked accumulation (k > 320): add this chunk's contribution to what the earlier chunks left in dist -- a
+      // round-to-nearest fp32 add per chunk instead of ever longer truncating MMA chains on one accumulator
+#pragma unroll
+      for (int j = 0; j < 2; ++j) {
+        const int64_t gi = row0 + 8 * j;
+        const float* q   = p.dist + gi * p.ldd + gc0;
+#pragma unroll
+        for (int i = 0; i < 16; ++i) {
+          if (fast) {
+            const float2 o = __ldcs(reinterpret_cast<const float2*>(q + 8 * i));
+            v[4 * i + 2 * j] += o.x;
+            v[4 * i + 2 * j + 1] += o.y;
+          } else if (gi < p.m) {
+            if (gc0 + 8 * i < p.n) v[4 * i + 2 * j] += __ldcs(q + 8 * i);
+            if (gc0 + 8 * i + 1 < p.n) v[4 * i + 2 * j + 1] += __ldcs(q + 8 * i + 1);
+          }
+        }
+      }
+    }
+    if (kPost != POST_NONE && kPost < POST_JACCARD && (p.acc_mode == 0 || p.acc_mode == 3)) {
+#pragma unroll
+      for (int c = 0; c < 64; ++c) v[c] = clamp0(v[c]);
+      if (p.diag_zero) {
+#pragma unroll
+        for (int i = 0; i < 16; ++i)
+#pragma unroll
+          for (int j = 0; j < 2; ++j) {
+            if (row0 + 8 * j == gc0 + 8 * i) v[4 * i + 2 * j] = 0.f;
+            if (row0 + 8 * j == gc0 + 8 * i + 1) v[4 * i + 2 * j + 1] = 0.f;
+          }
+      }
+      if (kPost == POST_CLAMP_SQRT) {
+#pragma unroll
+        for (int c = 0; c < 64; ++c) asm("sqrt.approx.f32 %0, %1;" : "=f"(v[c]) : "f"(v[c]));
+      }
+    }
+#pragma unroll
+    for (int j = 0; j < 2; ++j) {
+      const int64_t gi = row0 + 8 * j;
+      float* q         = p.dist + gi * p.ldd + gc0;
+#pragma unroll
+      for (int i = 0; i < 16; ++i) {
+        if (fast) {
+          ptx::st_global_cs_v2(q + 8 * i, v[4 * i + 2 * j], v[4 * i + 2 * j + 1]);
+        } else if (gi < p.m) {
+          if (gc0 + 8 * i < p.n) ptx::st_global_cs(q + 8 * i, v[4 * i + 2 * j]);
+          if (gc0 + 8 * i + 1 < p.n) ptx::st_global_cs(q + 8 * i + 1, v[4 * i + 2 * j + 1]);
+        }
+      }
+    }
+    return;
+  }
+  // Arg-min modes, per 64-column chunk and row: the minimum of this thread's 16 values is compared with the row's
+  // current global best.  Only a candidate that can change the result (value <= best: '<=' so that an equal value with
+  // a smaller index still gets through) takes the slow path: locate the smallest column holding the minimum (ascending
+  // scan) and let the packed 64-bit atomicMin decide -- (value, index) order == raft::argmin_op
+  // (cpp/include/raft/core/operators.hpp:187-194).  After the first few y blocks this is rare.
+  const float inf = __int_as_float(0x7f800000);
+#pragma unroll
+  for (int cc = 0; cc < 2; ++cc) {
+#pragma unroll
+    for (int j = 0; j < 2; ++j) {
+      const int b = 32 * cc + 2 * j;   // v[b + 4i + e], i in [0, 8)
+      float m0 = min3(v[b], v[b + 1], v[b + 4]);
+      float m1 = min3(v[b + 5], v[b + 8], v[b + 9]);
+      float m2 = min3(v[b + 12], v[b + 13], v[b + 16]);
+      float m3 = min3(v[b + 17], v[b + 20], v[b + 21]);
+      m0       = min3(m0, v[b + 24], v[b + 25]);
+      m1       = min3(m1, v[b + 28], v[b + 29]);
+      const float mn = fminf(min3(m0, m1, m2), m3);
+      // (+inf marks columns beyond n: never a candidate).  Keys hold the full distance |x|^2 + v, so the row term is
+      // added for the comparison -- one FADD per row here instead of one per element
+      const bool cand = (mn + xnr[j]) <= thr[j] && mn < inf;
+      if (__any_sync(0xffffffffu, cand) && cand) {
+        const int64_t gcc = gc0 + 64 * cc;   // global column of v[b]
+        if (kEpi == EPI_MINLOC) {
+          int cbest = 0;
+#pragma unroll
+          for (int i = 7; i >= 0; --i) {
+            if (v[b + 4 * i + 1] == mn) cbest = 8 * i + 1;
+            if (v[b + 4 * i] == mn) cbest = 8 * i;
+          }
+          const float dv = mn + xnr[j];
+          long long gj   = gcc + cbest;
+          if (p.col_map != nullptr) {  // permuted columns: the smallest SOURCE index among the equal minima
+            int best = 0x7fffffff;
+#pragma unroll
+            for (int i = 0; i < 8; ++i)
+#pragma unroll
+              for (int e = 0; e < 2; ++e)
+                if (v[b + 4 * i + e] == mn) best = min(best, __ldg(&p.col_map[gcc + 8 * i + e]));
+            gj = best;
+          }
+          gj += p.idx_offset;
+          const long long key = (static_cast<long long>(ordered_bits(dv)) << 32) | (gj & 0xFFFFFFFFll);
+          atomicMin(&p.keys[row0 + 8 * j], key);
+          thr[j] = dv;
+        } else {
+          knn_append16(p.knn_cnt, p.knn_cand, p.knn_cap, p.knn_dropmin, row0 + 8 * j, gcc + p.idx_offset, xnr[j], thr[j],
+                       v[b], v[b + 1], v[b + 4], v[b + 5], v[b + 8], v[b + 9], v[b + 12], v[b + 13], v[b + 16], v[b + 17],
+                       v[b + 20], v[b + 21], v[b + 24], v[b + 25], v[b + 28], v[b + 29]);
+        }
+      }
+    }
+  }
+}
+
+template <bool kResident, int kEpi, int kPost>
+__global__ void __launch_bounds__(TC_THREADS, 1)
+expanded_tc_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b, const TcParams p)
+{
+  constexpr int kStages          = kResident ? TC_STAGES_RES : TC_STAGES_STR;
+  constexpr uint32_t kStageBytes = kResident ? TC_A_BYTES : TC_A_BYTES + TC_BH_BYTES;
   if (p.run_flag != nullptr && __ldg(p.run_flag) == 0u) return;  // conditional launch (no host round trip)
   extern __shared__ __align__(1024) uint8_t smem[];
   // SWIZZLE_128B atoms need 1024-byte alignment; the dynamic window starts 1024-aligned (no static
   // shared memory in this kernel).  Checked, not assumed: a misaligned base traps.
   if ((ptx::smem_u32(smem) & 1023u) != 0u) __trap();
-  uint8_t* b_base = smem;  // resident slabs, or per-stage B
-  uint8_t* a_base = smem + (kResident ? TC_MAX_RES_KB * TC_B_BYTES : TC_STAGES_STR * TC_B_BYTES);
-  uint8_t* stg    = smem + TC_SMEM_OPERANDS - 32768;  // kTma only: 8 x 4 KB of store staging (one 32x32 block per epilogue warp)
+  uint8_t* b_base = smem;  // resident: [nkb] k-blocks of the y block
+  uint8_t* a_base = smem + (kResident ? TC_MAX_RES_KB * TC_B_BYTES : 0);  // stages: x k-block (+ y half k-block)
   float* col_tb   = reinterpret_cast<float*>(smem + TC_SMEM_OPERANDS);  // [256] t_y of this y block
   uint64_t* bars  = reinterpret_cast<uint64_t*>(col_tb + TC_BN);
   uint64_t* afull = bars;                       // [TC_MAX_STAGES]
   uint64_t* aempty = bars + TC_MAX_STAGES;      // [TC_MAX_STAGES]
   uint64_t* bfull = bars + 2 * TC_MAX_STAGES;   // [TC_MAX_RES_KB]
-  uint64_t* bempty = bfull + TC_MAX_RES_KB;
-  uint64_t* tfull = bempty + TC_MAX_RES_KB;     // [2] resident: per accumulator stage; streaming: per half
-  uint64_t* tempty = tfull + 2;                 // [2]
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(tempty + 2);
+  uint64_t* bempty = bfull + TC_MAX_RES_KB;     // [TC_MAX_RES_KB]
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
 
   if (threadIdx.x == 0) {
-    for (int i = 0; i < TC_MAX_STAGES; ++i) { ptx::mbar_init(&afull[i], 1); ptx::mbar_init(&aempty[i], 1); }
-    for (int i = 0; i < TC_MAX_RES_KB; ++i) { ptx::mbar_init(&bfull[i], 1); ptx::mbar_init(&bempty[i], 1); }
-    for (int i = 0; i < 2; ++i) { ptx::mbar_init(&tfull[i], 1); ptx::mbar_init(&tempty[i], kResident ? 8 : 4); }
+    // empty barriers: one arrival per consumer warpgroup
+    for (int i = 0; i < TC_MAX_STAGES; ++i) { ptx::mbar_init(&afull[i], 1); ptx::mbar_init(&aempty[i], 2); }
+    for (int i = 0; i < TC_MAX_RES_KB; ++i) { ptx::mbar_init(&bfull[i], 1); ptx::mbar_init(&bempty[i], 2); }
     ptx::fence_mbar_init();
     ptx::prefetch_tmap(&tmap_a);
     ptx::prefetch_tmap(&tmap_b);
   }
-  if (warp == 1) ptx::tmem_alloc<512>(tmem_slot);
-  ptx::tc_fence_before();
   __syncthreads();
-  ptx::tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
 
   const int nkb = p.nkb;
 
-  if (warp == 0) {
+  if (warp < 4) {
     // ================================ TMA producer =================================
-    // The whole warp runs the loop with warp-uniform values and one elected lane issues: inside a
-    // divergent `if (lane == 0)` the compiler cannot keep descriptors / barrier addresses in
-    // uniform registers and wraps every UTMALDG / UTCHMMA in an ELECT + R2UR.BROADCAST waterfall
-    // loop (measured: the MMA issue loop itself became the bottleneck).
+    asm volatile("setmaxnreg.dec.sync.aligned.u32 40;");
+    if (warp != 0) return;
+    // The whole warp runs the loop with warp-uniform values and one elected lane issues (inside a divergent
+    // `if (lane == 0)` the compiler cannot keep descriptors / barrier addresses in uniform registers).
     const uint64_t pol = ptx::policy_evict_last();
     uint32_t a_it = 0, it_local = 0;
     for (int64_t item = blockIdx.x; item < p.n_items; item += gridDim.x, ++it_local) {
@@ -284,576 +363,138 @@ expanded_tc_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_cons
       const int ch    = static_cast<int>(item / p.tiles_sel);
       const int mt0   = ch * p.chunk;
       const int mt1   = min(mt0 + p.chunk, p.tiles_m);
+      const int nh    = static_cast<int64_t>(n_blk) * TC_BN + TC_HN < p.n ? 2 : 1;  // halves of the y block inside the matrix
       for (int mt = mt0; mt < mt1; ++mt) {
-        for (int kb = 0; kb < nkb; ++kb, ++a_it) {
-          if (kResident && mt == mt0) {
-            ptx::mbar_wait(&bempty[kb], (it_local & 1) ^ 1);
-            if (ptx::elect_one()) {
-              ptx::mbar_expect_tx(&bfull[kb], TC_B_BYTES);
-              ptx::tma_load_2d(b_base + kb * TC_B_BYTES, &tmap_b, &bfull[kb], kb * 64, n_blk * TC_BN, pol);
-            }
-          }
-          const uint32_t s = a_it % kStages, ph = (a_it / kStages) & 1;
-          ptx::mbar_wait(&aempty[s], ph ^ 1);
-          if (ptx::elect_one()) {
-            ptx::mbar_expect_tx(&afull[s], kResident ? TC_A_BYTES : TC_A_BYTES + TC_B_BYTES);
-            ptx::tma_load_2d(a_base + s * TC_A_BYTES, &tmap_a, &afull[s], kb * 64, mt * TC_BM, pol);
-            if (!kResident)
-              ptx::tma_load_2d(b_base + s * TC_B_BYTES, &tmap_b, &afull[s], kb * 64, n_blk * TC_BN, pol);
-          }
-          __syncwarp();
-        }
-      }
-    }
-  } else if (warp == 1) {
-    // ================================ MMA issuer ===================================
-    // descriptor start-address units are 16 B; inside the 128-B swizzled row of a k-block:
-    //   hi k[0,16) +0, hi k[16,32) +2, lo k[0,16) +4, lo k[16,32) +6
-    uint32_t a_it = 0, t_it = 0, it_local = 0;
-    const bool has_lo = __ldg(p.has_lo) != 0u;
-    for (int64_t item = blockIdx.x; item < p.n_items; item += gridDim.x, ++it_local) {
-      const int ch  = static_cast<int>(item / p.tiles_sel);
-      const int mt0 = ch * p.chunk;
-      const int mt1 = min(mt0 + p.chunk, p.tiles_m);
-      for (int mt = mt0; mt < mt1; ++mt, ++t_it) {
-        if (kResident) {
-          constexpr uint32_t idesc = ptx::umma_idesc_f16(TC_BM, TC_BN);
-          const uint32_t as = t_it & 1, aph = (t_it >> 1) & 1;
-          ptx::mbar_wait(&tempty[as], aph ^ 1);
-          ptx::tc_fence_after();
-          const uint32_t d = tmem_base + as * TC_BN;
-          // pass 1: every cross term of every k-block, while the accumulator is still tiny
-          for (int kb = 0; kb < nkb; ++kb) {
-            const uint32_t it = a_it + kb, s = it % kStages, ph = (it / kStages) & 1;
-            if (mt == mt0) ptx::mbar_wait(&bfull[kb], it_local & 1);
-            ptx::mbar_wait(&afull[s], ph);
-            ptx::tc_fence_after();
-            if (has_lo && ptx::elect_one()) {
-              const uint64_t da = ptx::umma_desc_sw128(ptx::smem_u32(a_base + s * TC_A_BYTES));
-              const uint64_t db = ptx::umma_desc_sw128(ptx::smem_u32(b_base + kb * TC_B_BYTES));
-              ptx::mma_f16_ss(d, da + 4, db + 0, idesc, kb > 0 ? 1u : 0u);  // lo0 * hi0
-              ptx::mma_f16_ss(d, da + 6, db + 2, idesc, 1u);               // lo1 * hi1
-              ptx::mma_f16_ss(d, da + 0, db + 4, idesc, 1u);               // hi0 * lo0
-              ptx::mma_f16_ss(d, da + 2, db + 6, idesc, 1u);               // hi1 * lo1
-            }
-            __syncwarp();
-          }
-          // pass 2: the hi*hi terms; each x stage is released as soon as its last MMA is queued
-          for (int kb = 0; kb < nkb; ++kb) {
-            const uint32_t it = a_it + kb, s = it % kStages;
-            if (ptx::elect_one()) {
-              const uint64_t da = ptx::umma_desc_sw128(ptx::smem_u32(a_base + s * TC_A_BYTES));
-              const uint64_t db = ptx::umma_desc_sw128(ptx::smem_u32(b_base + kb * TC_B_BYTES));
-              ptx::mma_f16_ss(d, da + 0, db + 0, idesc, (has_lo || kb > 0) ? 1u : 0u);  // hi0 * hi0
-              ptx::mma_f16_ss(d, da + 2, db + 2, idesc, 1u);                           // hi1 * hi1
-              ptx::mma_commit(&aempty[s]);
-              if (mt == mt1 - 1) ptx::mma_commit(&bempty[kb]);
-            }
-            __syncwarp();
-          }
-          if (ptx::elect_one()) ptx::mma_commit(&tfull[as]);
-          __syncwarp();
-          a_it += nkb;
-        } else {
-          constexpr uint32_t idesc = ptx::umma_idesc_f16(TC_BM, TC_BN / 2);
-          const uint32_t tph = t_it & 1;
-          ptx::mbar_wait(&tempty[0], tph ^ 1);
-          ptx::mbar_wait(&tempty[1], tph ^ 1);
-          ptx::tc_fence_after();
+        for (int h = 0; h < nh; ++h) {
           for (int kb = 0; kb < nkb; ++kb, ++a_it) {
+            if (kResident && mt == mt0 && h == 0) {
+              ptx::mbar_wait(&bempty[kb], (it_local & 1) ^ 1);
+              if (ptx::elect_one()) {
+                ptx::mbar_expect_tx(&bfull[kb], TC_B_BYTES);
+                ptx::tma_load_2d(b_base + kb * TC_B_BYTES, &tmap_b, &bfull[kb], kb * 64, n_blk * TC_BN, pol);
+              }
+            }
             const uint32_t s = a_it % kStages, ph = (a_it / kStages) & 1;
-            ptx::mbar_wait(&afull[s], ph);
-            ptx::tc_fence_after();
+            ptx::mbar_wait(&aempty[s], ph ^ 1);
             if (ptx::elect_one()) {
-              const uint32_t acc = kb > 0 ? 1u : 0u;
-              const uint64_t da  = ptx::umma_desc_sw128(ptx::smem_u32(a_base + s * TC_A_BYTES));
-#pragma unroll
-              for (int h = 0; h < 2; ++h) {
-                const uint64_t db = ptx::umma_desc_sw128(ptx::smem_u32(b_base + s * TC_B_BYTES + h * (TC_B_BYTES / 2)));
-                const uint32_t d  = tmem_base + h * 256;  // main at +0, cross at +128
-                if (has_lo) {
-                  ptx::mma_f16_ss(d + 128, da + 4, db + 0, idesc, acc);
-                  ptx::mma_f16_ss(d + 128, da + 6, db + 2, idesc, 1u);
-                  ptx::mma_f16_ss(d + 128, da + 0, db + 4, idesc, 1u);
-                  ptx::mma_f16_ss(d + 128, da + 2, db + 6, idesc, 1u);
-                }
-                ptx::mma_f16_ss(d, da + 0, db + 0, idesc, acc);
-                ptx::mma_f16_ss(d, da + 2, db + 2, idesc, 1u);
-              }
-              ptx::mma_commit(&aempty[s]);
+              ptx::mbar_expect_tx(&afull[s], kStageBytes);
+              ptx::tma_load_2d(a_base + s * kStageBytes, &tmap_a, &afull[s], kb * 64, mt * TC_BM, pol);
+              if (!kResident)
+                ptx::tma_load_2d(a_base + s * kStageBytes + TC_A_BYTES, &tmap_b, &afull[s], kb * 64,
+                                 n_blk * TC_BN + h * TC_HN, pol);
             }
             __syncwarp();
-          }
-          if (ptx::elect_one()) {
-            ptx::mma_commit(&tfull[0]);
-            ptx::mma_commit(&tfull[1]);
-          }
-          __syncwarp();
-        }
-      }
-    }
-  } else {
-    // ================================ epilogue warps ===============================
-    const int q    = warp & 3;          // TMEM lane quarter this warp may read: tile rows [32q, 32q+32)
-    const int g    = (warp - 2) >> 2;   // column half of the tile this warp drains: [128g, 128g+128)
-    const int et   = threadIdx.x - 64;  // 0..255 (fills the per-column terms)
-    const int quad = lane >> 2;         // fragment row inside a 16-row group (and +8)
-    const int tq   = lane & 3;          // fragment column pair inside an 8-column group
-    uint32_t t_it  = 0;
-    const float cf     = __ldg(p.coef);
-    const bool add_cross = !kResident && __ldg(p.has_lo) != 0u;  // streaming layout keeps cross terms apart
-    const uint64_t pol_st = ptx::policy_evict_first();
-    // rows with their own exponent (prep.cuh): per-row factor on x (free: one multiply per row and tile), per-column
-    // factor on y only when some row of y has one (rare; read straight from global memory then)
-    const bool xnu = __ldg(&p.nonuni[0]) != 0u, ynu = __ldg(&p.nonuni[1]) != 0u;
-    for (int64_t item = blockIdx.x; item < p.n_items; item += gridDim.x) {
-      const int n_blk = sel_to_blk(static_cast<int>(item % p.tiles_sel), p.sel_s, p.sel_lo, p.sel_hi);
-      const int ch    = static_cast<int>(item / p.tiles_sel);
-      const int mt0   = ch * p.chunk;
-      const int mt1   = min(mt0 + p.chunk, p.tiles_m);
-      // per-column epilogue terms of this y block (shared by every tile of the item)
-      ptx::bar_sync(1, 32 * TC_EPI_WARPS);
-      if (et < TC_BN) {
-        const int64_t gj = static_cast<int64_t>(n_blk) * TC_BN + et;
-        float tv = kEpi != EPI_STORE ? __int_as_float(0x7f800000) : 0.f;  // +inf: never the arg-min
-        if (gj < p.n) tv = __ldg(&p.yt[gj]);
-        if (kEpi == EPI_STORE && p.acc_mode >= 2) tv = 0.f;  // the t terms entered with the first K chunk
-        col_tb[et] = tv;
-      }
-      ptx::bar_sync(1, 32 * TC_EPI_WARPS);
-      const int64_t col0 = static_cast<int64_t>(n_blk) * TC_BN + g * 128;  // first global column of this warp
-      const bool cols_in = col0 + 127 < p.n;
-
-      for (int mt = mt0; mt < mt1; ++mt, ++t_it) {
-        // ---- k <= 64: full-width store path (the resident y block leaves 64 KB of shared memory free) ----
-        // warp (q, h = g) owns tile rows 32q + 16h + [0,16) over ALL 256 columns: a private buffer of 8 full-width rows
-        // in the smem image of a 3-D TMA box {132, 2, 8} (padded rows: conflict-free fragment stores), ONE tensor store
-        // per 8 rows x 1 KB -- the widest-row pattern of scripts/probes/store_width.cu (22 B/clk/SM vs 19.5 for 32x32 boxes)
-        if (kTma && kResident && nkb <= 2 && static_cast<int64_t>(n_blk + 1) * TC_BN <= p.n) {
-          const int w8     = (warp - 2) & 7;
-          uint8_t* wbuf    = w8 < 7 ? b_base + 2 * TC_B_BYTES + w8 * (8 * TC_STG_ROW) : stg;
-          const uint32_t tb_idx = t_it & 1, tph = (t_it >> 1) & 1;
-          const int64_t rbase   = static_cast<int64_t>(mt) * TC_BM + q * 32 + 16 * g;   // first of this warp's 16 rows
-          uint64_t ta2[2], cfr2[2];
-#pragma unroll
-          for (int rr = 0; rr < 2; ++rr) {
-            const int64_t gi = rbase + 8 * rr + quad;
-            float rv = 0.f, cr = cf;
-            if (gi < p.m) {
-              rv = __ldg(&p.xt[gi]);
-              if (xnu) cr *= __ldg(&p.xsc[gi]);
-            }
-            ta2[rr]  = pk(rv, rv);
-            cfr2[rr] = pk(cr, cr);
-          }
-          ptx::mbar_wait(&tfull[tb_idx], tph);
-          ptx::tc_fence_after();
-          const uint32_t t_base = tmem_base + (static_cast<uint32_t>(q * 32 + 16 * g) << 16) + (t_it & 1) * TC_BN;
-#pragma unroll 1
-          for (int rr = 0; rr < 2; ++rr) {
-            const int64_t gi = rbase + 8 * rr + quad;
-#pragma unroll 1
-            for (int cp = 0; cp < 2; ++cp) {
-              uint32_t r0[32], r1[32];
-              ptx::tmem_ld_16x256_x8(t_base + 128 * cp, r0);
-              ptx::tmem_ld_16x256_x8(t_base + 128 * cp + 64, r1);
-              ptx::tmem_ld_wait();
-              if (rr == 1 && cp == 1) {  // last read of the accumulator: hand it back
-                ptx::tc_fence_before();
-                __syncwarp();
-                if (lane == 0) ptx::mbar_arrive(&tempty[tb_idx]);
-              }
-              float v[32];
-              const int64_t gj = static_cast<int64_t>(n_blk) * TC_BN + 128 * cp + 2 * tq;
-#pragma unroll
-              for (int i = 0; i < 16; ++i) {
-                const uint32_t* R = i < 8 ? r0 : r1;
-                const int ii      = i & 7;
-                const float2 tb   = *reinterpret_cast<const float2*>(&col_tb[128 * cp + 8 * i + 2 * tq]);
-                uint64_t a        = rr == 0 ? pk(R[4 * ii], R[4 * ii + 1]) : pk(R[4 * ii + 2], R[4 * ii + 3]);
-                if (ynu) {
-                  const int64_t gc = gj + 8 * i;
-                  a = mul2(a, pk(__ldg(&p.ysc[gc]), __ldg(&p.ysc[gc + 1])));
-                }
-                unpk(fma2(a, cfr2[rr], add2(ta2[rr], pk(tb.x, tb.y))), v[2 * i], v[2 * i + 1]);
-              }
-              if (kPost != POST_NONE) {
-#pragma unroll
-                for (int c = 0; c < 32; ++c) v[c] = clamp0(v[c]);
-                if (p.diag_zero && gi >= gj && gi < gj + 128) {
-#pragma unroll
-                  for (int i = 0; i < 16; ++i) {
-                    if (gi == gj + 8 * i) v[2 * i] = 0.f;
-                    if (gi == gj + 8 * i + 1) v[2 * i + 1] = 0.f;
-                  }
-                }
-                if (kPost == POST_CLAMP_SQRT) {
-#pragma unroll
-                  for (int c = 0; c < 32; ++c) asm("sqrt.approx.f32 %0, %1;" : "=f"(v[c]) : "f"(v[c]));
-                }
-              }
-              if (cp == 0) {  // the previous store out of this buffer has left it
-                if (lane == 0) ptx::tma_store_wait_read();
-                __syncwarp();
-              }
-              uint8_t* rowp = wbuf + quad * TC_STG_ROW + cp * 528 + 8 * tq;
-#pragma unroll
-              for (int i = 0; i < 16; ++i) *reinterpret_cast<float2*>(rowp + 32 * i) = make_float2(v[2 * i], v[2 * i + 1]);
-            }
-            ptx::fence_proxy_async_smem();
-            __syncwarp();
-            if (lane == 0) {
-              ptx::tma_store_3d(&tmap_r, wbuf, 0, 2 * n_blk, static_cast<int32_t>(rbase + 8 * rr), pol_st);
-              ptx::tma_store_commit();
-            }
-          }
-          continue;
-        }
-        if (kTma) {
-          // ---------------- EPI_STORE through shared memory + TMA tensor store ----------------
-          uint32_t tb_idx, tph;
-          if (kResident) { tb_idx = t_it & 1; tph = (t_it >> 1) & 1; }
-          else { tb_idx = g; tph = t_it & 1; }
-          const int64_t gi = static_cast<int64_t>(mt) * TC_BM + q * 32 + lane;  // thread == output row
-          float tav        = 0.f;
-          float crow       = cf;
-          if (gi < p.m) {
-            tav = __ldg(&p.xt[gi]);
-            if (xnu) crow *= __ldg(&p.xsc[gi]);  // a row with its own exponent (prep.cuh): thread == row, so it is free
-          }
-          const uint64_t tav2 = pk(tav, tav);
-          const uint64_t cf2  = pk(crow, crow);
-          // k <= 96 leaves the 4th y slab unused: a second staging block per warp lets the TMA store
-          // of chunk c overlap the staging of chunk c+1
-          const bool dbuf     = kResident && nkb <= 3;
-          float* stg_a        = reinterpret_cast<float*>(stg) + ((warp - 2) & 7) * 1024;
-          float* stg_b        = dbuf ? reinterpret_cast<float*>(b_base + 3 * TC_B_BYTES) + ((warp - 2) & 7) * 1024 : stg_a;
-          ptx::mbar_wait(&tfull[tb_idx], tph);
-          ptx::tc_fence_after();
-          const uint32_t t_base = tmem_base + (static_cast<uint32_t>(q * 32) << 16) +
-                                  (kResident ? (t_it & 1) * TC_BN + g * 128 : g * 256);
-          uint32_t r[32], rc[32];
-          ptx::tmem_ld_32x32(t_base, r);
-          if (!kResident) ptx::tmem_ld_32x32(t_base + 128, rc);
-#pragma unroll 1
-          for (int chunk = 0; chunk < 4; ++chunk) {
-            const int cbase = g * 128 + chunk * 32;
-            ptx::tmem_ld_wait();
-            if (chunk == 3) {
-              ptx::tc_fence_before();
-              __syncwarp();
-              if (lane == 0) ptx::mbar_arrive(&tempty[tb_idx]);
-            }
-            float v[32];
-#pragma unroll
-            for (int c = 0; c < 32; c += 4) {
-              const float4 tb = *reinterpret_cast<const float4*>(&col_tb[cbase + c]);
-              uint64_t a0 = pk(r[c], r[c + 1]), a1 = pk(r[c + 2], r[c + 3]);
-              if (add_cross) {
-                a0 = add2(a0, pk(rc[c], rc[c + 1]));
-                a1 = add2(a1, pk(rc[c + 2], rc[c + 3]));
-              }
-              if (ynu) {  // rows of y with their own exponent: per-column factors straight from global memory (rare)
-                const int64_t gc = static_cast<int64_t>(n_blk) * TC_BN + cbase + c;
-                a0 = mul2(a0, pk(gc < p.n ? __ldg(&p.ysc[gc]) : 1.f, gc + 1 < p.n ? __ldg(&p.ysc[gc + 1]) : 1.f));
-                a1 = mul2(a1, pk(gc + 2 < p.n ? __ldg(&p.ysc[gc + 2]) : 1.f, gc + 3 < p.n ? __ldg(&p.ysc[gc + 3]) : 1.f));
-              }
-              unpk(fma2(a0, cf2, add2(tav2, pk(tb.x, tb.y))), v[c], v[c + 1]);
-              unpk(fma2(a1, cf2, add2(tav2, pk(tb.z, tb.w))), v[c + 2], v[c + 3]);
-            }
-            if (chunk < 3) {
-              ptx::tmem_ld_32x32(t_base + (chunk + 1) * 32, r);
-              if (!kResident) ptx::tmem_ld_32x32(t_base + (chunk + 1) * 32 + 128, rc);
-            }
-            const int64_t gj0 = static_cast<int64_t>(n_blk) * TC_BN + cbase;
-            if (kPost != POST_NONE) {
-#pragma unroll
-              for (int c = 0; c < 32; ++c) v[c] = clamp0(v[c]);
-              if (p.diag_zero && gi >= gj0 && gi < gj0 + 32) {
-#pragma unroll
-                for (int c = 0; c < 32; ++c)
-                  if (gi == gj0 + c) v[c] = 0.f;
-              }
-              if (kPost == POST_CLAMP_SQRT) {
-#pragma unroll
-                for (int c = 0; c < 32; ++c) asm("sqrt.approx.f32 %0, %1;" : "=f"(v[c]) : "f"(v[c]));
-              }
-            }
-            // 16-byte chunks XOR-swizzled by (row & 7): conflict-free, and exactly SWIZZLE_128B
-            float* my_stg = (chunk & 1) ? stg_b : stg_a;
-            if (lane == 0) {  // the previous store out of this buffer has left it
-              if (dbuf) ptx::tma_store_wait_read1();
-              else ptx::tma_store_wait_read();
-            }
-            __syncwarp();
-#pragma unroll
-            for (int c4 = 0; c4 < 8; ++c4)
-              *reinterpret_cast<float4*>(my_stg + lane * 32 + ((c4 ^ (lane & 7)) << 2)) =
-                make_float4(v[4 * c4], v[4 * c4 + 1], v[4 * c4 + 2], v[4 * c4 + 3]);
-            {
-              ptx::fence_proxy_async_smem();
-              __syncwarp();
-              if (lane == 0) {
-                ptx::tma_store_2d(&tmap_d, my_stg, static_cast<int32_t>(gj0), mt * TC_BM + q * 32, pol_st);
-                ptx::tma_store_commit();
-              }
-            }
-          }
-          continue;
-        }
-        // the 4 tile rows this thread owns: 32q + quad + 8j, j = 0..3  (j = 2*rh + (0|1))
-        const int64_t row0 = static_cast<int64_t>(mt) * TC_BM + q * 32 + quad;
-        uint64_t ta2[4], cfr2[4];
-        float thr[4];  // arg-min modes: the row's current best (an upper bound: keys only decrease)
-        float xnr[4];  // EPI_MINLOC: the row term |x_i|^2 (cosine family: 1)
-        {
-#pragma unroll
-          for (int j = 0; j < 4; ++j) {
-            float rv = 0.f, cr = cf;
-            thr[j]   = __int_as_float(0xff800000);  // -inf: rows outside the matrix never trigger
-            xnr[j]   = 0.f;
-            if (row0 + 8 * j < p.m) {
-              if (xnu) cr *= __ldg(&p.xsc[row0 + 8 * j]);
-              if (kEpi != EPI_STORE || p.acc_mode < 2) rv = __ldg(&p.xt[row0 + 8 * j]);
-              xnr[j] = rv;
-              if (kEpi == EPI_TOPK) thr[j] = __ldg(&p.knn_thr[row0 + 8 * j]);
-              if (kEpi == EPI_MINLOC) {
-                const long long ck = *reinterpret_cast<volatile long long*>(&p.keys[row0 + 8 * j]);
-                const int sb       = static_cast<int>(ck >> 32);
-                thr[j]             = __int_as_float(sb < 0 ? (sb ^ 0x7FFFFFFF) : sb);
-                if (ck == 0x7FFFFFFFFFFFFFFFll) thr[j] = __int_as_float(0x7f800000);
-              }
-            }
-            ta2[j]  = pk(rv, rv);
-            cfr2[j] = pk(cr, cr);
-          }
-        }
-        const bool rows_in = static_cast<int64_t>(mt) * TC_BM + q * 32 + 31 < p.m;
-
-        uint32_t tb_idx, tph;
-        if (kResident) { tb_idx = t_it & 1; tph = (t_it >> 1) & 1; }
-        else { tb_idx = g; tph = t_it & 1; }
-        ptx::mbar_wait(&tfull[tb_idx], tph);
-        ptx::tc_fence_after();
-        // TMEM address of (lane 32q, first column of this warp's 128)
-        const uint32_t t_base = tmem_base + (static_cast<uint32_t>(q * 32) << 16) +
-                                (kResident ? (t_it & 1) * TC_BN + g * 128 : g * 256);
-
-        // 4 fragments per tile: (cc, rh) = 64-column chunk x 16-row half
-        uint32_t r[32], rc[32];
-        ptx::tmem_ld_16x256_x8(t_base, r);
-        if (!kResident) ptx::tmem_ld_16x256_x8(t_base + 128, rc);
-#pragma unroll
-        for (int f = 0; f < 4; ++f) {
-          const int cc = f >> 1, rh = f & 1;
-          ptx::tmem_ld_wait();
-          if (f == 3) {
-            // everything this warp needs from the accumulator is in registers: hand it back
-            ptx::tc_fence_before();
-            __syncwarp();
-            if (lane == 0) ptx::mbar_arrive(&tempty[tb_idx]);
-          }
-          float v[32];  // v[4i..4i+1]: row rh*2, cols 8i+2tq+{0,1}; v[4i+2..4i+3]: row rh*2+1
-          const int cl0 = g * 128 + cc * 64 + 2 * tq;  // this thread's first column inside the tile
-#pragma unroll
-          for (int i = 0; i < 8; ++i) {
-            const float2 tb = *reinterpret_cast<const float2*>(&col_tb[cl0 + 8 * i]);
-            uint64_t a0 = pk(r[4 * i], r[4 * i + 1]), a1 = pk(r[4 * i + 2], r[4 * i + 3]);
-            if (add_cross) {
-              a0 = add2(a0, pk(rc[4 * i], rc[4 * i + 1]));
-              a1 = add2(a1, pk(rc[4 * i + 2], rc[4 * i + 3]));
-            }
-            const uint64_t tb2 = pk(tb.x, tb.y);
-            if (ynu) {
-              const int64_t gc   = static_cast<int64_t>(n_blk) * TC_BN + cl0 + 8 * i;
-              const uint64_t sb2 = pk(gc < p.n ? __ldg(&p.ysc[gc]) : 1.f, gc + 1 < p.n ? __ldg(&p.ysc[gc + 1]) : 1.f);
-              a0 = mul2(a0, sb2);
-              a1 = mul2(a1, sb2);
-            }
-            uint64_t t0, t1;
-            if (kEpi == EPI_STORE) {
-              t0 = add2(ta2[2 * rh], tb2);
-              t1 = add2(ta2[2 * rh + 1], tb2);
-            } else {  // the row-constant |x_i|^2 does not change the arg-min: added on the slow path only
-              t0 = tb2;
-              t1 = tb2;
-            }
-            if (kEpi == EPI_STORE && kPost >= POST_JACCARD) {
-              float a00, a01, a10, a11, s00, s01, s10, s11;
-              unpk(mul2(a0, cfr2[2 * rh]), a00, a01);
-              unpk(mul2(a1, cfr2[2 * rh + 1]), a10, a11);
-              unpk(t0, s00, s01);
-              unpk(t1, s10, s11);
-              v[4 * i]     = post_ratio<kPost>(a00, s00);
-              v[4 * i + 1] = post_ratio<kPost>(a01, s01);
-              v[4 * i + 2] = post_ratio<kPost>(a10, s10);
-              v[4 * i + 3] = post_ratio<kPost>(a11, s11);
-            } else {
-              uint64_t w0 = fma2(a0, cfr2[2 * rh], t0), w1 = fma2(a1, cfr2[2 * rh + 1], t1);
-              unpk(w0, v[4 * i], v[4 * i + 1]);
-              unpk(w1, v[4 * i + 2], v[4 * i + 3]);
-            }
-          }
-          if (f < 3) {  // r / rc are dead: fetch the next fragment while this one is stored / reduced
-            const int nf       = f + 1;
-            const uint32_t off = (static_cast<uint32_t>((nf & 1) * 16) << 16) + (nf >> 1) * 64;
-            ptx::tmem_ld_16x256_x8(t_base + off, r);
-            if (!kResident) ptx::tmem_ld_16x256_x8(t_base + off + 128, rc);
-          }
-          if (kEpi == EPI_STORE) {
-            const int64_t gi0 = row0 + 16 * rh;                 // global row of v[4i], v[4i+1]
-            const int64_t gj0 = col0 + cc * 64 + 2 * tq;        // global column of v[4i]
-            if (p.acc_mode >= 2) {
-              // K-chunked accumulation (k > 256): add this chunk's contribution to what the earlier
-              // chunks left in dist -- a round-to-nearest fp32 add per chunk instead of ever longer
-              // truncating MMA chains on one accumulator
-              if (rows_in && cols_in && p.pair_ok) {
-                const float* q0 = p.dist + gi0 * p.ldd + gj0;
-                const float* q1 = q0 + 8 * p.ldd;
-                float2 o0[8], o1[8];
-#pragma unroll
-                for (int i = 0; i < 8; ++i) {
-                  o0[i] = __ldcs(reinterpret_cast<const float2*>(q0 + 8 * i));
-                  o1[i] = __ldcs(reinterpret_cast<const float2*>(q1 + 8 * i));
-                }
-#pragma unroll
-                for (int i = 0; i < 8; ++i) {
-                  v[4 * i] += o0[i].x; v[4 * i + 1] += o0[i].y;
-                  v[4 * i + 2] += o1[i].x; v[4 * i + 3] += o1[i].y;
-                }
-              } else {
-#pragma unroll
-                for (int i = 0; i < 8; ++i) {
-                  const int64_t gj = gj0 + 8 * i;
-                  const float* q0  = p.dist + gi0 * p.ldd + gj;
-                  const float* q1  = q0 + 8 * p.ldd;
-                  if (gi0 < p.m) {
-                    if (gj < p.n) v[4 * i] += __ldcs(q0);
-                    if (gj + 1 < p.n) v[4 * i + 1] += __ldcs(q0 + 1);
-                  }
-                  if (gi0 + 8 < p.m) {
-                    if (gj < p.n) v[4 * i + 2] += __ldcs(q1);
-                    if (gj + 1 < p.n) v[4 * i + 3] += __ldcs(q1 + 1);
-                  }
-                }
-              }
-            }
-            if (kPost != POST_NONE && kPost < POST_JACCARD && (p.acc_mode == 0 || p.acc_mode == 3)) {
-#pragma unroll
-              for (int c = 0; c < 32; ++c) v[c] = clamp0(v[c]);
-              if (p.diag_zero) {
-#pragma unroll
-                for (int i = 0; i < 8; ++i) {
-                  if (gi0 == gj0 + 8 * i) v[4 * i] = 0.f;
-                  if (gi0 == gj0 + 8 * i + 1) v[4 * i + 1] = 0.f;
-                  if (gi0 + 8 == gj0 + 8 * i) v[4 * i + 2] = 0.f;
-                  if (gi0 + 8 == gj0 + 8 * i + 1) v[4 * i + 3] = 0.f;
-                }
-              }
-              if (kPost == POST_CLAMP_SQRT) {
-#pragma unroll
-                for (int c = 0; c < 32; ++c) asm("sqrt.approx.f32 %0, %1;" : "=f"(v[c]) : "f"(v[c]));
-              }
-            }
-            float* p0 = p.dist + gi0 * p.ldd + gj0;
-            float* p1 = p0 + 8 * p.ldd;
-            if (rows_in && cols_in && p.pair_ok) {
-#pragma unroll
-              for (int i = 0; i < 8; ++i) {
-                ptx::st_global_cs_v2(p0 + 8 * i, v[4 * i], v[4 * i + 1]);
-                ptx::st_global_cs_v2(p1 + 8 * i, v[4 * i + 2], v[4 * i + 3]);
-              }
-            } else {
-#pragma unroll
-              for (int i = 0; i < 8; ++i) {
-                const int64_t gj = gj0 + 8 * i;
-                if (gi0 < p.m) {
-                  if (gj < p.n) ptx::st_global_cs(p0 + 8 * i, v[4 * i]);
-                  if (gj + 1 < p.n) ptx::st_global_cs(p0 + 8 * i + 1, v[4 * i + 1]);
-                }
-                if (gi0 + 8 < p.m) {
-                  if (gj < p.n) ptx::st_global_cs(p1 + 8 * i, v[4 * i + 2]);
-                  if (gj + 1 < p.n) ptx::st_global_cs(p1 + 8 * i + 1, v[4 * i + 3]);
-                }
-              }
-            }
-          } else {
-            // per row: min of this thread's 16 values with 3-input FMNMX, compared with the row's
-            // current global best.  Only a candidate that can change the result (value <= best:
-            // '<=' so that an equal value with a smaller index still gets through) takes the slow
-            // path: locate the smallest column holding the minimum (ascending scan) and let the
-            // packed 64-bit atomicMin decide -- (value, index) order == raft::argmin_op
-            // (cpp/include/raft/core/operators.hpp:187-194).  After the first few y blocks this is rare,
-            // so the common path is FFMA2 + FMNMX3 + one warp vote per row.
-#pragma unroll
-            for (int rr = 0; rr < 2; ++rr) {
-              const int o = 2 * rr;
-              float m0    = min3(v[o], v[o + 1], v[4 + o]);
-              float m1    = min3(v[4 + o + 1], v[8 + o], v[8 + o + 1]);
-              float m2    = min3(v[12 + o], v[12 + o + 1], v[16 + o]);
-              float m3    = min3(v[16 + o + 1], v[20 + o], v[20 + o + 1]);
-              m0          = min3(m0, v[24 + o], v[24 + o + 1]);
-              m1          = min3(m1, v[28 + o], v[28 + o + 1]);
-              const float mn = fminf(min3(m0, m1, m2), m3);
-              const int j    = 2 * rh + rr;
-              // (+inf marks columns beyond n: never a candidate).  Keys hold the full distance
-              // |x|^2 + v, so the row term is added for the comparison -- one FADD per row here
-              // instead of one per element
-              const float inf = __int_as_float(0x7f800000);
-              const bool cand = (mn + xnr[j]) <= thr[j] && mn < inf;
-              if (__any_sync(0xffffffffu, cand)) {
-                if (cand) {
-                  if (kEpi == EPI_MINLOC) {
-                    int cbest = 0;
-#pragma unroll
-                    for (int i = 7; i >= 0; --i) {
-                      if (v[4 * i + o + 1] == mn) cbest = 8 * i + 1;
-                      if (v[4 * i + o] == mn) cbest = 8 * i;
-                    }
-                    const float dv      = mn + xnr[j];
-                    long long gj        = static_cast<long long>(n_blk) * TC_BN + cl0 + cbest;
-                    if (p.col_map != nullptr) {  // permuted columns: the smallest SOURCE index among the equal minima
-                      int best = 0x7fffffff;
-#pragma unroll
-                      for (int i = 0; i < 8; ++i)
-#pragma unroll
-                        for (int e = 0; e < 2; ++e)
-                          if (v[4 * i + o + e] == mn)
-                            best = min(best, __ldg(&p.col_map[static_cast<int64_t>(n_blk) * TC_BN + cl0 + 8 * i + e]));
-                      gj = best;
-                    }
-                    gj += p.idx_offset;
-                    const long long key = (static_cast<long long>(ordered_bits(dv)) << 32) | (gj & 0xFFFFFFFFll);
-                    atomicMin(&p.keys[row0 + 8 * j], key);
-                    thr[j] = dv;
-                  } else {
-                    // EPI_TOPK: everything at or below the row's k-th best so far goes to the row's list.  ONE copy of that
-                    // code: unrolled into the 8 (fragment, row) sites of the tile loop it made this instantiation ~50 KB
-                    // larger than the instruction cache holds -- ncu: 61 % of the stall samples "no instruction", issue slots
-                    // 6 % busy, the passes at a fifth of the arg-min kernel's rate.
-                    knn_append16(p.knn_cnt, p.knn_cand, p.knn_cap, p.knn_dropmin, row0 + 8 * j,
-                                 static_cast<long long>(n_blk) * TC_BN + cl0 + p.idx_offset, xnr[j], thr[j], v[o], v[o + 1],
-                                 v[4 + o], v[4 + o + 1], v[8 + o], v[8 + o + 1], v[12 + o], v[12 + o + 1], v[16 + o], v[16 + o + 1],
-                                 v[20 + o], v[20 + o + 1], v[24 + o], v[24 + o + 1], v[28 + o], v[28 + o + 1]);
-                  }
-                }
-              }
-            }
           }
         }
       }
     }
+    return;
   }
 
-  if (kTma && warp >= 2) {
-    if (lane == 0) ptx::tma_store_wait_all();
-    __syncwarp();
-  }
-  ptx::tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    ptx::tc_fence_after();
-    ptx::tmem_dealloc<512>(tmem_base);
+  // ================================ consumer warpgroups ================================
+  asm volatile("setmaxnreg.inc.sync.aligned.u32 232;");
+  const int wg     = (threadIdx.x >> 7) - 1;  // rows [64 wg, 64 wg + 64) of every x tile
+  const int ct     = threadIdx.x - 128;       // 0..255 (fills the per-column terms)
+  const bool lead  = (threadIdx.x & 127) == 0;  // arrives on the empty barriers for its warpgroup
+  const int quad   = lane >> 2;               // fragment row inside a 16-row group (and +8)
+  const int tq     = lane & 3;                // fragment column pair inside an 8-column group
+  const bool has_lo = __ldg(p.has_lo) != 0u;
+  const float cf    = __ldg(p.coef);
+  // rows with their own exponent (prep.cuh): per-row factor on x (one multiply per row and tile), per-column factor on y
+  // only when some row of y has one (rare; read straight from global memory then)
+  const bool xnu = __ldg(&p.nonuni[0]) != 0u, ynu = __ldg(&p.nonuni[1]) != 0u;
+  uint32_t a_it = 0, it_local = 0;
+  float acc[64], crs[64];
+  for (int64_t item = blockIdx.x; item < p.n_items; item += gridDim.x, ++it_local) {
+    const int n_blk = sel_to_blk(static_cast<int>(item % p.tiles_sel), p.sel_s, p.sel_lo, p.sel_hi);
+    const int ch    = static_cast<int>(item / p.tiles_sel);
+    const int mt0   = ch * p.chunk;
+    const int mt1   = min(mt0 + p.chunk, p.tiles_m);
+    const int nh    = static_cast<int64_t>(n_blk) * TC_BN + TC_HN < p.n ? 2 : 1;
+    // per-column epilogue terms of this y block (shared by every tile of the item)
+    ptx::bar_sync(1, 256);
+    {
+      const int64_t gj = static_cast<int64_t>(n_blk) * TC_BN + ct;
+      float tv = kEpi != EPI_STORE ? __int_as_float(0x7f800000) : 0.f;  // +inf: never the arg-min
+      if (gj < p.n) tv = __ldg(&p.yt[gj]);
+      if (kEpi == EPI_STORE && p.acc_mode >= 2) tv = 0.f;  // the t terms entered with the first K chunk
+      col_tb[ct] = tv;
+    }
+    ptx::bar_sync(1, 256);
+
+    for (int mt = mt0; mt < mt1; ++mt) {
+      // the two tile rows this thread owns: row0 and row0 + 8
+      const int64_t row0 = static_cast<int64_t>(mt) * TC_BM + 64 * wg + 16 * (warp & 3) + quad;
+      float ta[2], cfr[2], thr[2], xnr[2];
+#pragma unroll
+      for (int j = 0; j < 2; ++j) {
+        const int64_t gi = row0 + 8 * j;
+        float rv = 0.f, cr = cf;
+        thr[j] = __int_as_float(0xff800000);  // -inf: rows outside the matrix never trigger
+        if (gi < p.m) {
+          if (xnu) cr *= __ldg(&p.xsc[gi]);
+          if (kEpi != EPI_STORE || p.acc_mode < 2) rv = __ldg(&p.xt[gi]);
+          if (kEpi == EPI_TOPK) thr[j] = __ldg(&p.knn_thr[gi]);
+          if (kEpi == EPI_MINLOC) {  // the row's current best (an upper bound: keys only decrease)
+            const long long ck = *reinterpret_cast<volatile long long*>(&p.keys[gi]);
+            const int sb       = static_cast<int>(ck >> 32);
+            thr[j]             = __int_as_float(sb < 0 ? (sb ^ 0x7FFFFFFF) : sb);
+            if (ck == 0x7FFFFFFFFFFFFFFFll) thr[j] = __int_as_float(0x7f800000);
+          }
+        }
+        ta[j]  = rv;
+        xnr[j] = rv;
+        cfr[j] = cr;
+      }
+      for (int h = 0; h < nh; ++h) {
+        if (!has_lo) {
+#pragma unroll
+          for (int c = 0; c < 64; ++c) crs[c] = 0.f;
+        }
+        // descriptor start-address units are 16 B; inside the 128-B swizzled row of a k-block:
+        //   hi k[0,16) +0, hi k[16,32) +2, lo k[0,16) +4, lo k[16,32) +6
+        for (int kb = 0; kb < nkb; ++kb, ++a_it) {
+          const uint32_t s = a_it % kStages, ph = (a_it / kStages) & 1;
+          if (kResident && mt == mt0 && h == 0) ptx::mbar_wait(&bfull[kb], it_local & 1);
+          ptx::mbar_wait(&afull[s], ph);
+          const uint64_t da = ptx::gmma_desc_sw128(ptx::smem_u32(a_base + s * kStageBytes) + wg * 64 * 128);
+          const uint64_t db = ptx::gmma_desc_sw128(kResident ? ptx::smem_u32(b_base + kb * TC_B_BYTES) + h * TC_BH_BYTES
+                                                             : ptx::smem_u32(a_base + s * kStageBytes + TC_A_BYTES));
+          const uint32_t accum = kb > 0 ? 1u : 0u;
+          ptx::fence_regs(acc);
+          ptx::fence_regs(crs);
+          ptx::wgmma_fence();
+          if (has_lo) {
+            ptx::wgmma_m64n128k16_f16(crs, da + 4, db + 0, accum);  // lo0 * hi0
+            ptx::wgmma_m64n128k16_f16(crs, da + 6, db + 2, 1u);     // lo1 * hi1
+            ptx::wgmma_m64n128k16_f16(crs, da + 0, db + 4, 1u);     // hi0 * lo0
+            ptx::wgmma_m64n128k16_f16(crs, da + 2, db + 6, 1u);     // hi1 * lo1
+          }
+          ptx::wgmma_m64n128k16_f16(acc, da + 0, db + 0, accum);    // hi0 * hi0
+          ptx::wgmma_m64n128k16_f16(acc, da + 2, db + 2, 1u);       // hi1 * hi1
+          ptx::wgmma_commit();
+          ptx::fence_regs(acc);
+          ptx::fence_regs(crs);
+          if (kb > 0) {  // the previous k-block's MMAs have finished reading their stage: hand it back
+            ptx::wgmma_wait<1>();
+            if (lead) ptx::mbar_arrive(&aempty[(a_it - 1) % kStages]);
+          }
+        }
+        ptx::wgmma_wait<0>();
+        ptx::fence_regs(acc);
+        ptx::fence_regs(crs);
+        if (lead) {
+          ptx::mbar_arrive(&aempty[(a_it - 1) % kStages]);
+          if (kResident && mt == mt1 - 1 && h == nh - 1)
+            for (int kb = 0; kb < nkb; ++kb) ptx::mbar_arrive(&bempty[kb]);
+        }
+#pragma unroll
+        for (int c = 0; c < 64; ++c) acc[c] += crs[c];
+        const int cl0 = h * TC_HN + 2 * tq;  // this thread's first column inside the tile
+        tc_epilogue<kEpi, kPost>(acc, p, col_tb, cl0, static_cast<int64_t>(n_blk) * TC_BN + cl0, row0, ta, cfr, thr, xnr,
+                                 ynu);
+      }
+    }
   }
 }
 

@@ -1,5 +1,5 @@
 // fp64 pairwise distances (SURVEY.md 8(a2): "fp32 in/acc/out (also fp64 ...)", 8(f4)): one register-tiled SIMT kernel
-// for every metric of the enum, in double precision end to end.  B200 has no fp64 tensor-core path worth the name for
+// for every metric of the enum, in double precision end to end.  The fp64 tensor-core path (DMMA) is not worth it for
 // this shape (DESIGN.md), and the reference's own fp64 instantiation was a SIMT kernel too, so this is a plain
 // 64 x 64 tile, 256 threads x (4 x 4) outputs, 16-deep k-blocks through shared memory; any row / column stride,
 // zero-filled tails.  Expanded metrics are evaluated from <x,y> and per-row statistics (sum, sum of squares) computed by

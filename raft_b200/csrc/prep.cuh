@@ -10,7 +10,7 @@
 //                      kernel's TMA descriptor expects:
 //                          row r, k-block b (32 source columns):  [ hi[0..32) | lo[0..32) ] = 128 bytes
 //                      so that one 128-byte SWIZZLE_128B shared-memory row carries both halves of a
-//                      k-block and hi*hi, hi*lo, lo*hi are K=16 tcgen05.mma steps over the same tile.
+//                      k-block and hi*hi, hi*lo, lo*hi are K=16 wgmma steps over the same tile.
 // One scale per matrix (not per row): fp16 keeps 11 bits at any normal magnitude, so rows up to
 // 2^18 below the matrix maximum still split without loss, and a single scale makes the undo a
 // single scalar -- the epilogue is d = acc * c + (t_x[i] + t_y[j]) with

@@ -1,7 +1,6 @@
-// Thin inline-PTX wrappers for sm_100a: mbarrier, TMA (cp.async.bulk.tensor), tcgen05 (TMEM
-// alloc / mma / commit / ld), fences.  No CUTLASS dependency: bit layouts of the UMMA shared-
-// memory and instruction descriptors are restated here from the PTX ISA (the same layouts the
-// vendored CuTe headers document in cute/arch/mma_sm100_desc.hpp).
+// Thin inline-PTX wrappers for sm_90a: mbarrier, TMA (cp.async.bulk.tensor), wgmma (warpgroup MMA
+// with shared-memory operand descriptors), fences.  No CUTLASS dependency: the bit layout of the
+// wgmma shared-memory matrix descriptor is restated here from the PTX ISA.
 #pragma once
 #include <cstdint>
 #include <cuda_runtime.h>
@@ -71,8 +70,6 @@ __device__ __forceinline__ void fence_proxy_async_smem()
 {
   asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
 }
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
 
 __device__ __forceinline__ void bar_sync(uint32_t id, uint32_t nthreads)
 {
@@ -156,129 +153,71 @@ __device__ __forceinline__ uint64_t policy_evict_first()
   return p;
 }
 
-// ------------------------------------------------------------------ TMEM
-template <uint32_t kCols>
-__device__ __forceinline__ void tmem_alloc(uint32_t* smem_result)
+// ------------------------------------------------------------------ wgmma
+// A warpgroup (4 consecutive warps, 128 threads) issues one wgmma together; the accumulator lives in
+// the registers of its threads.  Fragment of an m64nN accumulator (the m16n8 layout per warp,
+// repeated along columns): warp w of the warpgroup, lane l, for i in [0, N/8):
+//   d[4i+0], d[4i+1] = row 16w + l/4,     columns 8i + 2(l%4) + {0,1}
+//   d[4i+2], d[4i+3] = row 16w + l/4 + 8, same columns
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+// keeps the compiler from moving accesses of the accumulator registers across wgmma issue / wait
+__device__ __forceinline__ void fence_regs(float (&d)[64])
 {
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(
-                 smem_u32(smem_result)),
-               "r"(kCols)
-               : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-template <uint32_t kCols>
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr)
-{
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(kCols)
-               : "memory");
+#pragma unroll
+  for (int i = 0; i < 64; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
 
-// D[tmem] (+)= A[smem desc] * B[smem desc], kind::f16 (fp16 operands, fp32 accumulate).
-__device__ __forceinline__ void mma_f16_ss(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b,
-                                           uint32_t idesc, uint32_t accumulate)
+// D[64 x 128] (+)= A[64 x 16] * B[128 x 16]^T, fp16 operands from shared memory (both K-major), fp32
+// accumulate in registers.  accumulate == 0: D = A * B.
+__device__ __forceinline__ void wgmma_m64n128k16_f16(float (&d)[64], uint64_t desc_a, uint64_t desc_b, uint32_t accumulate)
 {
   asm volatile(
     "{\n\t.reg .pred p;\n\t"
-    "setp.ne.b32 p, %4, 0;\n\t"
-    "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}\n"
-    :
-    : "r"(tmem_d), "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
+    "setp.ne.b32 p, %66, 0;\n\t"
+    "wgmma.mma_async.sync.aligned.m64n128k16.f32.f16.f16 "
+    "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, %64, %65, p, 1, 1, 0, 0;\n\t}\n"
+    : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+      "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+      "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+      "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]),
+      "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]),
+      "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
+      "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]),
+      "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+    : "l"(desc_a), "l"(desc_b), "r"(accumulate)
     : "memory");
 }
-// Arrive on an mbarrier once every previously issued tcgen05.mma of this thread has completed
-// (implies tcgen05.fence::before_thread_sync).
-__device__ __forceinline__ void mma_commit(uint64_t* bar)
-{
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(
-                 smem_u32(bar))
-               : "memory");
-}
-
-// TMEM -> registers: 32 lanes x 32 consecutive 32-bit columns; thread t of the warp gets lane
-// (base_lane + t), r[c] = column (base_col + c).
-__device__ __forceinline__ void tmem_ld_32x32(uint32_t taddr, uint32_t (&r)[32])
-{
-  asm volatile(
-    "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-    "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-    "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-    : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]),
-      "=r"(r[7]), "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]),
-      "=r"(r[14]), "=r"(r[15]), "=r"(r[16]), "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]),
-      "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]),
-      "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-    : "r"(taddr)
-    : "memory");
-}
-// Same shape, 16 columns.
-__device__ __forceinline__ void tmem_ld_32x16(uint32_t taddr, uint32_t (&r)[16])
-{
-  asm volatile(
-    "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-    "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-    : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]),
-      "=r"(r[7]), "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]),
-      "=r"(r[14]), "=r"(r[15])
-    : "r"(taddr)
-    : "memory");
-}
-// TMEM -> registers, 16 lanes x 256 bits, x8: 16 rows x 64 fp32 columns per warp.  Fragment (the
-// m16n8 accumulator layout, repeated along columns): thread t holds, for i in [0,8):
-//   r[4i+0], r[4i+1] = row (t/4),     columns 8i + 2(t%4) + {0,1}
-//   r[4i+2], r[4i+3] = row (t/4) + 8, same columns
-// so a warp-wide 8-byte store of (r[4i], r[4i+1]) writes 8 rows x one full 32-byte sector.
-__device__ __forceinline__ void tmem_ld_16x256_x8(uint32_t taddr, uint32_t (&r)[32])
-{
-  asm volatile(
-    "tcgen05.ld.sync.aligned.16x256b.x8.b32 "
-    "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-    "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-    : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]),
-      "=r"(r[7]), "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]),
-      "=r"(r[14]), "=r"(r[15]), "=r"(r[16]), "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]),
-      "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]),
-      "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-    : "r"(taddr)
-    : "memory");
-}
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
 
 // ------------------------------------------------------------------ descriptors
-// UMMA shared-memory matrix descriptor, K-major operand, SWIZZLE_128B, rows of 128 bytes:
+// wgmma shared-memory matrix descriptor, K-major operand, rows of 128 bytes, SWIZZLE_128B:
 //   bits [0,14)  start address >> 4
 //   bits [16,30) leading byte offset >> 4 (unused for swizzled K-major; 1)
 //   bits [32,46) stride byte offset >> 4 (distance between 8-row groups = 1024 B -> 64)
-//   bits [46,48) descriptor version = 1 (Blackwell)
-//   bits [61,64) layout type = 2 (SWIZZLE_128B)
-__device__ __forceinline__ uint64_t umma_desc_sw128(uint32_t smem_addr)
+//   bits [62,64) layout type = 1 (SWIZZLE_128B)
+// A k-step of 16 fp16 inside the swizzled row advances the start address by 32 bytes (+2).
+__device__ __forceinline__ uint64_t gmma_desc_sw128(uint32_t smem_addr)
 {
   uint64_t d = 0;
   d |= static_cast<uint64_t>((smem_addr & 0x3FFFF) >> 4);
   d |= static_cast<uint64_t>(1) << 16;
   d |= static_cast<uint64_t>(1024 >> 4) << 32;
-  d |= static_cast<uint64_t>(1) << 46;
-  d |= static_cast<uint64_t>(2) << 61;
+  d |= static_cast<uint64_t>(1) << 62;
   return d;
 }
 
-// Same, SWIZZLE_64B with rows of 64 bytes (8-row groups of 512 B; layout type 4): used where only
+// Same, SWIZZLE_64B with rows of 64 bytes (8-row groups of 512 B; layout type 2): used where only
 // half of a packed k-block is staged.
-__device__ __forceinline__ uint64_t umma_desc_sw64(uint32_t smem_addr)
+__device__ __forceinline__ uint64_t gmma_desc_sw64(uint32_t smem_addr)
 {
   uint64_t d = 0;
   d |= static_cast<uint64_t>((smem_addr & 0x3FFFF) >> 4);
   d |= static_cast<uint64_t>(1) << 16;
   d |= static_cast<uint64_t>(512 >> 4) << 32;
-  d |= static_cast<uint64_t>(1) << 46;
-  d |= static_cast<uint64_t>(4) << 61;
+  d |= static_cast<uint64_t>(2) << 62;
   return d;
-}
-
-// Instruction descriptor, kind::f16: D=f32 (bits[4,6)=1), A=B=f16 (formats 0), both K-major,
-// N>>3 at bits [17,23), M>>4 at bits [24,29).
-__host__ __device__ constexpr uint32_t umma_idesc_f16(uint32_t M, uint32_t N)
-{
-  return (1u << 4) | ((N >> 3) << 17) | ((M >> 4) << 24);
 }
 
 // ------------------------------------------------------------------ misc

@@ -1,4 +1,4 @@
-// K3b: coarse screening pass of the screened fusedL2NN (sm_100a, tcgen05).
+// K3b: coarse screening pass of the screened fusedL2NN (sm_90a, wgmma).
 //
 // fused_nn_keys (api.cu) first runs the exact arg-min kernel on every S-th 256-row block of y, which
 // leaves each x row with an upper bound U_i of its minimum.  This kernel visits the other blocks with
@@ -8,44 +8,26 @@
 //     margin_i = f (|x_i| YL + |xl_i| Y + 3 |xl_i| YL) + f 0.05 * 2^-10 |x_i| Y      (Y, YL: block maxima of |y_j|, |yl_j|)
 // where xl = x - (its hi part) is MEASURED per row by prep.cuh and f = 2 (L2) or 1 (cosine / correlation: rows are
 // unit vectors after prep, d = 1 + acc * c): Cauchy-Schwarz on the three dropped products; the last term and the
-// 2^-21 |y|^2 cover the fp32 rounding of the accumulation and of the epilogue.  Only pairs with L_ij <= U_i can hold the minimum: they go to a candidate list that
-// nn_exact_kernel re-measures straight from the fp32 inputs.  The margin is a per-row constant
-// inside a y block, so it moves into the row's threshold.  The element loop does not even form L_ij:
-// it bounds a whole 32-column group G by  c max_{j in G} acc_ij + min_{j in G} |y_j|^2 (1 - 2^-21)  (c < 0),
-// one FMNMX3 per two pairs, and only a group that reaches the threshold is read again column by column.
-// The database chunk is packed in the order of |y_j|^2 (api.cu), which makes the group bound as good as the
-// per-column one and the per-block margin (max_j' |y_j'|) local; `col_map` translates a packed position
-// back to the caller's row where an index leaves the kernel.
+// 2^-21 |y|^2 cover the fp32 rounding of the accumulation and of the epilogue.  Only pairs with L_ij <= U_i can hold
+// the minimum: they go to a candidate list that nn_exact_kernel re-measures straight from the fp32 inputs.  The margin
+// is a per-row constant inside a y block, so it moves into the row's threshold.  The element loop does not even form
+// L_ij: it bounds the thread's 8 values of a 32-column group G by  c max acc_ij + min_{j in G} |y_j|^2 (1 - 2^-21)
+// (c < 0), and only a group that reaches the threshold is looked at column by column.  The database chunk is packed
+// in the order of |y_j|^2 (api.cu), which makes the group bound as good as the per-column one and the per-block
+// margin (max_j' |y_j'|) local; `col_map` translates a packed position back to the caller's row where an index
+// leaves the kernel.
 //
 // Every coarse value is also an UPPER bound of a real pair's distance (value + margin), so a row's
-// bound tightens (atomic min on aux[i].x) whenever one of its candidates is found: 2.3 candidates per
-// row on 1M x 1M x 96 Gaussian data instead of the 7.3 that a fixed 1/8 sample leaves, which is
-// what lets the exact pass sample only every 32nd block.
+// bound tightens (atomic min on aux[i].x) whenever one of its candidates is found, which is what lets
+// the exact pass sample only every 32nd block.
 //
-// A 128 x 256 tile is ~770 tensor cycles here (6 MMAs at k = 96) instead of 2300, so everything
-// around the tensor core had to shrink with it.  Measured with clock64 timelines per role
-// (1M x 1M x 96, cycles per tile): the first version re-used the exact kernel's roles and took 2300
-// -- the single MMA warp spent 740 issuing (tcgen05.mma issue blocks while the pipe's queue is full),
-// 810 + 690 in barrier polls and bookkeeping while the pipe idled, and the epilogue exposed one TMEM
-// load latency per fragment.  This kernel: ~1350 (ncu: tensor pipe 56 % active); isolation runs:
-// operands + MMAs alone 1010, epilogue alone 1100, synchronisation skeleton alone 620 -- the two halves
-// still contend (TMEM ports, issue slots) instead of overlapping fully.
-//   operands   hi halves only: TMA boxes of 32 fp16 (64 B, SWIZZLE_64B) out of the packed
-//              [hi32|lo32] k-blocks; a stage is one whole x tile (nkb x 8 KB), 5-6 stages deep,
-//              one mbarrier round trip per TILE; the y block (nkb x 16 KB) is resident per item
-//   MMA        two issuer warps, one per TMEM accumulator stage (even / odd tiles): while one is
-//              blocked in issue the other has finished its polls, so the pipe stays fed.  All waits
-//              first, then one elected region queues every MMA of the tile and the commits
-//              (x stage free, accumulator full).  Both issuers poll EVERY barrier in order, also for
-//              tiles they do not own: a parity wait is only sound at most one phase behind
-//   epilogue   16 warps on every tile (32 rows x 64 columns each), thread == row
-//              (tcgen05.ld.32x32b, the fastest TMEM read shape: 403 vs 571 cycles per tile for
-//              16x256b, scripts/probes/tmem_probe.cu), software-pipelined over two 16-column register
-//              buffers so that the load of fragment f+1 overlaps the arithmetic of fragment f, no
-//              branches inside: per 32-column group one compare sets a bit of a hit mask.  A warp
-//              with a hit (1-2 % of the warp-tiles) reads those groups again, notes the candidate
-//              columns in a 64-bit mask, hands the accumulator back and only then takes the atomics
-//              (list append, bound update)
+//   operands   hi halves only: TMA boxes of 32 fp16 (64 B, SWIZZLE_64B) out of the packed [hi32|lo32] k-blocks;
+//              a stage is one whole x tile (nkb x 8 KB), one mbarrier round trip per TILE; the y block
+//              (nkb x 16 KB) is resident per item
+//   warpgroup 0      TMA producer (warp 0)
+//   warpgroups 1-2   consumers: warpgroup c owns rows [64c, 64c+64) of every x tile and all 256 columns (two
+//                    wgmma.m64n128k16 accumulators), releases the x stage as soon as its MMAs have finished and
+//                    screens from the registers; a warp with a hit takes the atomics (list append, bound update)
 #pragma once
 #include "expanded_tc.cuh"
 
@@ -55,26 +37,12 @@ constexpr int SC_A_KB_BYTES   = TC_BM * 64;  // one k-block of an x tile, hi hal
 constexpr int SC_B_KB_BYTES   = TC_BN * 64;  // one k-block of the y block:          256 rows x 64 B
 constexpr int SC_MAX_KB       = 4;           // k <= 128
 constexpr int SC_MAX_STAGES   = 8;
-constexpr int SC_EPI_WARPS    = 16;
-constexpr int SC_BLK          = 64;           // candidate-list slots an epilogue warp reserves at a time
-#ifndef SC_SETS
-#define SC_SETS 1
-#endif
-constexpr int SC_CW           = 64 * SC_SETS;  // columns of a tile one epilogue warp drains
-constexpr int SC_MMA2_WARP    = 2 + SC_EPI_WARPS;  // second MMA issuer (the first is warp 1)
-constexpr int SC_THREADS      = 96 + 32 * SC_EPI_WARPS;
-constexpr size_t SC_A_RING    = 160 * 1024;
-constexpr size_t SC_SMEM_OPERANDS = (size_t)SC_MAX_KB * SC_B_KB_BYTES + SC_A_RING;  // 224 KB
+constexpr int SC_BLK          = 64;          // candidate-list slots a warp reserves at a time
+constexpr int SC_THREADS      = 384;
+constexpr size_t SC_A_RING    = 128 * 1024;
+constexpr size_t SC_SMEM_OPERANDS = (size_t)SC_MAX_KB * SC_B_KB_BYTES + SC_A_RING;  // 192 KB
 constexpr size_t SC_SMEM_BYTES    = SC_SMEM_OPERANDS + TC_BN * 4 + 96 + 256;
 static_assert(SC_SMEM_BYTES <= 232448, "exceeds the 227 KB per-CTA limit");
-
-#ifdef SC_TRACE
-__device__ long long g_sc_trace[8][4096];
-__device__ long long g_sc_wtrace[3][16][2048];   // per epilogue warp: tfull seen, arrive, hit flag
-#define SC_STAMP(EV, TT) do { if (blockIdx.x == 0 && (TT) < 4096u) g_sc_trace[EV][TT] = clock64(); } while (0)
-#else
-#define SC_STAMP(EV, TT) do { } while (0)
-#endif
 
 struct ScreenParams {
   int64_t m, n;
@@ -99,22 +67,6 @@ struct ScreenParams {
   int unit_norm;          // cosine family: rows are unit vectors, d = 1 + acc * c (c without the factor 2)
 };
 
-// 16 columns of this thread's row folded into four running maxima of the RAW accumulator (no branches, no column
-// terms: the fragments of a tile overlap in the instruction stream).  c < 0, so for a 32-column group G
-//   min_{j in G} (acc_ij c + t_j)  >=  c max_{j in G} acc_ij + min_{j in G} t_j :
-// one FMNMX3 per two pairs here and one FFMA + compare per group, instead of an FFMA2 + FMNMX3 per two pairs and a
-// broadcast shared-memory read of t_j per pair (those reads were as many shared-memory wavefronts as the tensor
-// core's operand reads: ncu, DESIGN.md K3b).  The group bound is tight because the host packs the chunk in the
-// order of |y_j|^2, so the t_j of 32 neighbouring columns differ by next to nothing.
-#define B2D_SCREEN_FRAGMENT(R)                                                                          \
-  _Pragma("unroll") for (int c = 0; c < 16; c += 8)                                                     \
-  {                                                                                                     \
-    m0 = max3(m0, __uint_as_float(R[c]), __uint_as_float(R[c + 1]));                                    \
-    m1 = max3(m1, __uint_as_float(R[c + 2]), __uint_as_float(R[c + 3]));                                \
-    m2 = max3(m2, __uint_as_float(R[c + 4]), __uint_as_float(R[c + 5]));                                \
-    m3 = max3(m3, __uint_as_float(R[c + 6]), __uint_as_float(R[c + 7]));                                \
-  }
-
 __global__ void __launch_bounds__(SC_THREADS, 1)
 screen_tc_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b,
                  const ScreenParams p)
@@ -133,34 +85,29 @@ screen_tc_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_consta
   uint64_t* aempty = bars + SC_MAX_STAGES;      // [SC_MAX_STAGES]
   uint64_t* bfull  = bars + 2 * SC_MAX_STAGES;  // [1]
   uint64_t* bempty = bfull + 1;                 // [1]
-  uint64_t* tfull  = bempty + 1;                // [2]
-  uint64_t* tempty = tfull + 2;                 // [2]
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(tempty + 2);
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
 
   if (threadIdx.x == 0) {
-    for (int i = 0; i < SC_MAX_STAGES; ++i) { ptx::mbar_init(&afull[i], 1); ptx::mbar_init(&aempty[i], 1); }
+    // empty barriers: one arrival per consumer warpgroup
+    for (int i = 0; i < SC_MAX_STAGES; ++i) { ptx::mbar_init(&afull[i], 1); ptx::mbar_init(&aempty[i], 2); }
     ptx::mbar_init(bfull, 1);
-    ptx::mbar_init(bempty, 2);  // one arrival per MMA issuer
-    for (int i = 0; i < 2; ++i) { ptx::mbar_init(&tfull[i], 1); ptx::mbar_init(&tempty[i], SC_EPI_WARPS / SC_SETS); }
+    ptx::mbar_init(bempty, 2);
     ptx::fence_mbar_init();
     ptx::prefetch_tmap(&tmap_a);
     ptx::prefetch_tmap(&tmap_b);
   }
-  if (warp == 1) ptx::tmem_alloc<512>(tmem_slot);
-  ptx::tc_fence_before();
   __syncthreads();
-  ptx::tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
 
   const int nkb              = p.nkb;
   const uint32_t stage_bytes = static_cast<uint32_t>(nkb) * SC_A_KB_BYTES;
   const uint32_t n_stages    = static_cast<uint32_t>(p.n_stages);
 
-  if (warp == 0) {
+  if (warp < 4) {
     // ================================ TMA producer =================================
+    asm volatile("setmaxnreg.dec.sync.aligned.u32 40;");
+    if (warp != 0) return;
     const uint64_t pol = ptx::policy_evict_last();
     uint32_t t_it = 0, it_local = 0;
     for (int64_t item = blockIdx.x; item < p.n_items; item += gridDim.x, ++it_local) {
@@ -187,326 +134,227 @@ screen_tc_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_consta
         __syncwarp();
       }
     }
-  } else if (warp == 1 || warp == SC_MMA2_WARP) {
-    // ================================ MMA issuers ==================================
-    // Two issuer warps, one per accumulator stage (even / odd tiles).  tcgen05.mma issue blocks while
-    // the tensor pipe's queue is full, i.e. for most of a tile's execution; with a single issuer the
-    // pipe then idles during that warp's bookkeeping for the next tile (barrier polls, descriptors,
-    // commits: ~500 cycles against ~770 of tensor work).  The two warps' tiles are independent (other
-    // accumulator, other x stage), so the order in which the pipe receives them does not matter.
-    const uint32_t parity = warp == 1 ? 0u : 1u;
-    constexpr uint32_t idesc = ptx::umma_idesc_f16(TC_BM, TC_BN);
-    const uint32_t d = tmem_base + parity * TC_BN;
-    uint32_t t_it = 0, it_local = 0;
-    for (int64_t item = blockIdx.x; item < p.n_items; item += gridDim.x, ++it_local) {
-      const int ch  = static_cast<int>(item / p.tiles_sel);
-      const int mt0 = ch * p.chunk;
-      const int mt1 = min(mt0 + p.chunk, p.tiles_m);
-      // Both issuers wait for the y block and walk EVERY tile of the item, polling the x-stage barrier
-      // also for the tiles of the other issuer: an mbarrier parity wait is only sound for a waiter that is
-      // at most one phase behind, so no barrier may be skipped (a warp that skipped bfull of an item it
-      // owns no tile of -- items of a single tile, fewer than 129 query rows -- ran two phases ahead and
-      // issued MMAs on a y block that had not arrived).
-      ptx::mbar_wait(bfull, it_local & 1);
-      const int own0 = mt0 + static_cast<int>((parity ^ t_it) & 1u);   // our first tile of the item
-      if (own0 >= mt1) {  // none: our half of the y-block release (the bfull wait above closed the previous phase)
-        if (ptx::elect_one()) ptx::mbar_arrive(bempty);
-        __syncwarp();
-      }
-      for (int mt = mt0; mt < mt1; ++mt) {
-        const uint32_t tt = t_it + static_cast<uint32_t>(mt - mt0);
-        const uint32_t s = tt % n_stages, ph = (tt / n_stages) & 1;
-        if (((tt ^ parity) & 1u) != 0u) {  // the other issuer's tile: keep in step with its x stage only
-          ptx::mbar_wait(&afull[s], ph);
-          continue;
+    return;
+  }
+
+  // ================================ consumer warpgroups ================================
+  asm volatile("setmaxnreg.inc.sync.aligned.u32 232;");
+  const int wg    = (threadIdx.x >> 7) - 1;  // rows [64 wg, 64 wg + 64) of every x tile
+  const int et    = threadIdx.x - 128;       // 0..255
+  const bool lead = (threadIdx.x & 127) == 0;
+  const int quad  = lane >> 2, tq = lane & 3;
+  const float cf0 = __ldg(p.coef);
+  const bool xnu  = __ldg(&p.nonuni[0]) != 0u;
+  const float4 aux_none = make_float4(__int_as_float(0xff800000), 0.f, 0.f, 0.f);  // rows beyond m: threshold -inf, never taken
+  unsigned blk_base = 0;      // this warp's block of candidate-list slots ...
+  int blk_used      = SC_BLK; // ... and how many of them are taken (SC_BLK: none reserved yet)
+  bool list_full    = false;  // a reservation of this warp came back beyond the list's capacity (sticky, warp-uniform)
+  uint32_t t_it = 0, it_local = 0;
+  float acc[2][64];           // columns [0, 128) and [128, 256) of the y block
+  for (int64_t item = blockIdx.x; item < p.n_items; item += gridDim.x, ++it_local) {
+    const int n_blk = sel_to_blk(static_cast<int>(item % p.tiles_sel), p.sel_s, p.sel_lo, p.sel_hi);
+    const int ch    = static_cast<int>(item / p.tiles_sel);
+    const int mt0   = ch * p.chunk;
+    const int mt1   = min(mt0 + p.chunk, p.tiles_m);
+    // per-column terms of this y block (shared by every tile of the item)
+    ptx::bar_sync(1, 256);
+    {
+      const int64_t gj = static_cast<int64_t>(n_blk) * TC_BN + et;
+      float tv = __int_as_float(0x7f800000), nyv = 0.f, nlv = 0.f;  // +inf: never a candidate
+      if (gj < p.n) {
+        nlv = __ldg(&p.ylo[gj]);
+        if (p.unit_norm) {  // |y_j| = 1, column term 0
+          tv  = 0.f;
+          nyv = 1.f;
+        } else {
+          tv  = __ldg(&p.yt[gj]);
+          nyv = sqrtf(tv) * (1.f + 1.f / 4194304.f);
+          tv  = tv - tv * (1.f / 2097152.f);
         }
-        ptx::mbar_wait(&afull[s], ph);   // (the operands arrive long before the accumulator is free: off the critical path)
-        if (lane == 0) SC_STAMP(1, tt);
-        ptx::mbar_wait(&tempty[parity], ((tt >> 1) & 1) ^ 1);
-        if (lane == 0) SC_STAMP(0, tt);
-        ptx::tc_fence_after();
-        if (ptx::elect_one()) {
-          const uint64_t da = ptx::umma_desc_sw64(ptx::smem_u32(a_base + s * stage_bytes));
-          const uint64_t db = ptx::umma_desc_sw64(ptx::smem_u32(b_base));
+      }
 #pragma unroll
-          for (int kb = 0; kb < SC_MAX_KB; ++kb) {
-            if (kb < nkb) {
-              // descriptor address units are 16 B: k[0,16) of the 64-byte row at +0, k[16,32) at +2
-              const uint64_t dak = da + static_cast<uint64_t>(kb * (SC_A_KB_BYTES >> 4));
-              const uint64_t dbk = db + static_cast<uint64_t>(kb * (SC_B_KB_BYTES >> 4));
-              ptx::mma_f16_ss(d, dak, dbk, idesc, kb > 0 ? 1u : 0u);
-              ptx::mma_f16_ss(d, dak + 2, dbk + 2, idesc, 1u);
-            }
-          }
-          ptx::mma_commit(&aempty[s]);
-          if (mt + 2 >= mt1) ptx::mma_commit(bempty);  // our last tile of the item
-          ptx::mma_commit(&tfull[parity]);
-          SC_STAMP(2, tt);
-        }
-        __syncwarp();
+      for (int o = 16; o > 0; o >>= 1) {
+        nyv = fmaxf(nyv, __shfl_xor_sync(0xffffffffu, nyv, o));
+        nlv = fmaxf(nlv, __shfl_xor_sync(0xffffffffu, nlv, o));
       }
-      t_it += static_cast<uint32_t>(mt1 - mt0);
+      float gm = tv;
+#pragma unroll
+      for (int o = 16; o > 0; o >>= 1) gm = fminf(gm, __shfl_xor_sync(0xffffffffu, gm, o));
+      if (lane == 0) { col_ny[et >> 5] = nyv; col_nl[et >> 5] = nlv; col_gm[et >> 5] = gm; }
+      col_tb[et] = tv;
     }
-  } else {
-    // ================================ epilogue warps ===============================
-    const int w   = warp - 2;        // 0..15
-    const int set = SC_SETS == 2 ? (w >> 3) : 0;  // SC_SETS == 2: accumulator stage (tile parity) this warp drains
-    const int q   = warp & 3;        // TMEM lane quarter this warp may read: tile rows [32q, 32q+32)
-    const int g   = SC_SETS == 2 ? ((w & 7) >> 2) : (w >> 2);  // column slice of the tile: [SC_CW g, SC_CW (g+1))
-    const int et  = threadIdx.x - 64;
-    const float cf0 = __ldg(p.coef);
-    const bool xnu  = __ldg(&p.nonuni[0]) != 0u;
-    const float4 aux_none = make_float4(__int_as_float(0xff800000), 0.f, 0.f, 0.f);  // rows beyond m: threshold -inf, never taken
-    unsigned blk_base = 0;      // this warp's block of candidate-list slots ...
-    int blk_used      = SC_BLK; // ... and how many of them are taken (SC_BLK: none reserved yet)
-    bool list_full    = false;  // a reservation of this warp came back beyond the list's capacity (sticky, warp-uniform)
-    uint32_t t_it = 0;
-    for (int64_t item = blockIdx.x; item < p.n_items; item += gridDim.x) {
-      const int n_blk = sel_to_blk(static_cast<int>(item % p.tiles_sel), p.sel_s, p.sel_lo, p.sel_hi);
-      const int ch    = static_cast<int>(item / p.tiles_sel);
-      const int mt0   = ch * p.chunk;
-      const int mt1   = min(mt0 + p.chunk, p.tiles_m);
-      // this warp's first tile of the item, and its row data (global-load latency hides behind the
-      // column-term barrier below)
-      int mt_own = SC_SETS == 2 ? mt0 + ((set ^ static_cast<int>(t_it)) & 1) : mt0;
-      float4 aux_nxt = aux_none;
-      {
-        const int64_t r = static_cast<int64_t>(mt_own) * TC_BM + q * 32 + lane;
-        if (mt_own < mt1 && r < p.m) aux_nxt = __ldg(&p.aux[r]);
-      }
-      // per-column terms of this y block (shared by every tile of the item)
-      ptx::bar_sync(1, 32 * SC_EPI_WARPS);
-      if (et < TC_BN) {
-        const int64_t gj = static_cast<int64_t>(n_blk) * TC_BN + et;
-        float tv = __int_as_float(0x7f800000), nyv = 0.f, nlv = 0.f;  // +inf: never a candidate
-        if (gj < p.n) {
-          nlv = __ldg(&p.ylo[gj]);
-          if (p.unit_norm) {  // |y_j| = 1, column term 0
-            tv  = 0.f;
-            nyv = 1.f;
-          } else {
-            tv  = __ldg(&p.yt[gj]);
-            nyv = sqrtf(tv) * (1.f + 1.f / 4194304.f);
-            tv  = tv - tv * (1.f / 2097152.f);
-          }
-        }
+    ptx::bar_sync(1, 256);
+    // What the coarse product leaves out of <x, y>:  xh.yl + xl.yh + xl.yl  with x = xh + xl (hi part + the rest), so by
+    // Cauchy-Schwarz at most |x| |yl| + |xl| |y| + 3 |xl| |yl|; the residual norms are MEASURED per row by prep.cuh
+    // (about 0.2 * 2^-10 of the row norm for fp16 rounding, against the worst case 2^-11 per element).
+    // With Y = max |y_j|, YL = max |yl_j| over the block and f = 2 (L2: d = .. - 2 <x, y>) or 1 (cosine family):
+    //   margin_i = |x_i| P + |xl_i| Q,   P = f (YL + 0.05 * 2^-10 Y),   Q = f (Y + 3 YL)
+    // (the 0.05 * 2^-10 |x| |y| term covers the fp32 rounding of the accumulation and of the epilogue).
+    float y_max = 0.f, yl_max = 0.f;
 #pragma unroll
-        for (int o = 16; o > 0; o >>= 1) {
-          nyv = fmaxf(nyv, __shfl_xor_sync(0xffffffffu, nyv, o));
-          nlv = fmaxf(nlv, __shfl_xor_sync(0xffffffffu, nlv, o));
-        }
-        float gm = tv;
-#pragma unroll
-        for (int o = 16; o > 0; o >>= 1) gm = fminf(gm, __shfl_xor_sync(0xffffffffu, gm, o));
-        if (lane == 0) { col_ny[et >> 5] = nyv; col_nl[et >> 5] = nlv; col_gm[et >> 5] = gm; }
-        col_tb[et] = tv;
-      }
-      ptx::bar_sync(1, 32 * SC_EPI_WARPS);
-      // What the coarse product leaves out of <x, y>:  xh.yl + xl.yh + xl.yl  with x = xh + xl (hi part + the rest), so by
-      // Cauchy-Schwarz at most |x| |yl| + |xl| |y| + 3 |xl| |yl|; the residual norms are MEASURED per row by prep.cuh
-      // (about 0.2 * 2^-10 of the row norm for fp16 rounding, against the worst case 2^-11 per element that the first
-      // version of this bound assumed: the margin, and with it the number of candidates it lets through, drops to ~45 %).
-      // With Y = max |y_j|, YL = max |yl_j| over the block and f = 2 (L2: d = .. - 2 <x, y>) or 1 (cosine family):
-      //   margin_i = |x_i| P + |xl_i| Q,   P = f (YL + 0.05 * 2^-10 Y),   Q = f (Y + 3 YL)
-      // (the 0.05 * 2^-10 |x| |y| term covers the fp32 rounding of the accumulation and of the epilogue, as before).
-      float y_max = 0.f, yl_max = 0.f;
-#pragma unroll
-      for (int i = 0; i < TC_BN / 32; ++i) { y_max = fmaxf(y_max, col_ny[i]); yl_max = fmaxf(yl_max, col_nl[i]); }
-      const float ff     = p.unit_norm ? 1.f : 2.f;
-      const float marg_p = ff * fmaf(y_max, 0.05f / 1024.f, yl_max) * (1.f + 1.f / 1048576.f);
-      const float marg_q = ff * fmaf(3.f, yl_max, y_max) * (1.f + 1.f / 1048576.f);
-      const float yn_max = y_max * y_max;  // max |y_j|^2 of the block
+    for (int i = 0; i < TC_BN / 32; ++i) { y_max = fmaxf(y_max, col_ny[i]); yl_max = fmaxf(yl_max, col_nl[i]); }
+    const float ff     = p.unit_norm ? 1.f : 2.f;
+    const float marg_p = ff * fmaf(y_max, 0.05f / 1024.f, yl_max) * (1.f + 1.f / 1048576.f);
+    const float marg_q = ff * fmaf(3.f, yl_max, y_max) * (1.f + 1.f / 1048576.f);
+    const float yn_max = y_max * y_max;  // max |y_j|^2 of the block
 
-      const uint32_t t_item0 = t_it;
-      for (; mt_own < mt1; mt_own += SC_SETS) {
-        const uint32_t tt   = t_item0 + static_cast<uint32_t>(mt_own - mt0);  // global tile counter of this tile
-        const int64_t row   = static_cast<int64_t>(mt_own) * TC_BM + q * 32 + lane;
-        const float4 aux_c  = aux_nxt;
-        aux_nxt             = aux_none;
-        if (mt_own + SC_SETS < mt1 && row + SC_SETS * TC_BM < p.m) aux_nxt = __ldg(&p.aux[row + SC_SETS * TC_BM]);
-        // thread == row: a row with its own exponent just has its own coefficient
-        const float cf     = (xnu && row < p.m) ? cf0 * __ldg(&p.xsc[row]) : cf0;
+    ptx::mbar_wait(bfull, it_local & 1);
+    for (int mt = mt0; mt < mt1; ++mt, ++t_it) {
+      // the two rows this thread owns: row[0] and row[0] + 8
+      int64_t row[2];
+      float4 aux_c[2];
+      float cf[2], margin[2], thr[2];
+#pragma unroll
+      for (int j = 0; j < 2; ++j) {
+        row[j]   = static_cast<int64_t>(mt) * TC_BM + 64 * wg + 16 * (warp & 3) + quad + 8 * j;
+        aux_c[j] = row[j] < p.m ? __ldg(&p.aux[row[j]]) : aux_none;
+        cf[j]    = (xnu && row[j] < p.m) ? cf0 * __ldg(&p.xsc[row[j]]) : cf0;  // a row with its own exponent
         // U_i - |x_i|^2 + margin_i, nudged up so that it stays an upper bound
-        const float margin = fmaf(aux_c.y, marg_p, aux_c.z * marg_q);
-        float thr = aux_c.x + margin;
-        thr       = thr + fabsf(thr) * (1.f / 4194304.f);
+        margin[j] = fmaf(aux_c[j].y, marg_p, aux_c[j].z * marg_q);
+        thr[j]    = aux_c[j].x + margin[j];
+        thr[j]    = thr[j] + fabsf(thr[j]) * (1.f / 4194304.f);
+      }
 
-        const uint32_t as = tt & 1, aph = (tt >> 1) & 1;
-        ptx::mbar_wait(&tfull[as], aph);
-        ptx::tc_fence_after();
-#ifdef SC_TRACE
-        if (lane == 0 && blockIdx.x == 0 && tt < 2048u) g_sc_wtrace[0][w][tt] = clock64();
-#endif
-        if (lane == 0 && w == 0) SC_STAMP(3, tt);
-        if (lane == 0 && w == 9) SC_STAMP(7, tt);
-#ifdef SC_NO_EPILOGUE   // diagnostic build (DESIGN.md K3b item 3): the MMA / TMA side alone
-        ptx::tc_fence_before();
-        __syncwarp();
-        if (lane == 0) ptx::mbar_arrive(&tempty[as]);
-        continue;
-#endif
-        const uint32_t t_base = tmem_base + (static_cast<uint32_t>(q * 32) << 16) + as * TC_BN + g * SC_CW;
-        const int cb          = g * SC_CW;
-        uint32_t ra[16], rb[16];
-        unsigned hitmask = 0;  // bit gp: some column of the gp-th 32-column group reaches the threshold
-        float m0, m1, m2, m3;
-#define B2D_GROUP_BEGIN m0 = m1 = m2 = m3 = __int_as_float(0xff800000);
-#define B2D_GROUP_END(GP) hitmask |= (fmaf(fmaxf(max3(m0, m1, m2), m3), cf, col_gm[(cb >> 5) + (GP)]) <= thr) ? (1u << (GP)) : 0u;
-        ptx::tmem_ld_32x16(t_base, ra);
+      const uint32_t s = t_it % n_stages, ph = (t_it / n_stages) & 1;
+      ptx::mbar_wait(&afull[s], ph);
+      ptx::fence_regs(acc[0]);
+      ptx::fence_regs(acc[1]);
+      ptx::wgmma_fence();
 #pragma unroll
-        for (int gp = 0; gp < SC_CW / 32; ++gp) {  // two register buffers: the next load is in flight during the math
-          ptx::tmem_ld_wait();
-          ptx::tmem_ld_32x16(t_base + 32 * gp + 16, rb);
-          B2D_GROUP_BEGIN
-          B2D_SCREEN_FRAGMENT(ra)
-          ptx::tmem_ld_wait();
-          if (gp + 1 < SC_CW / 32) ptx::tmem_ld_32x16(t_base + 32 * gp + 32, ra);
-          B2D_SCREEN_FRAGMENT(rb)
-          B2D_GROUP_END(gp)
+      for (int kb = 0; kb < SC_MAX_KB; ++kb) {
+        if (kb < nkb) {
+          // descriptor address units are 16 B: k[0,16) of the 64-byte row at +0, k[16,32) at +2
+          const uint64_t da = ptx::gmma_desc_sw64(ptx::smem_u32(a_base + s * stage_bytes + kb * SC_A_KB_BYTES) + wg * 64 * 64);
+          const uint64_t db = ptx::gmma_desc_sw64(ptx::smem_u32(b_base + kb * SC_B_KB_BYTES));
+          const uint64_t db1 = db + ((TC_HN * 64) >> 4);   // rows [128, 256) of the y block
+          ptx::wgmma_m64n128k16_f16(acc[0], da, db, kb > 0 ? 1u : 0u);
+          ptx::wgmma_m64n128k16_f16(acc[1], da, db1, kb > 0 ? 1u : 0u);
+          ptx::wgmma_m64n128k16_f16(acc[0], da + 2, db + 2, 1u);
+          ptx::wgmma_m64n128k16_f16(acc[1], da + 2, db1 + 2, 1u);
         }
-#undef B2D_GROUP_BEGIN
-#undef B2D_GROUP_END
-        if (lane == 0 && w == 0) SC_STAMP(4, tt);
-        unsigned long long cmask[SC_SETS] = {};  // columns of this row (bit = column - cb) that go to the exact pass
-        float vmin = __int_as_float(0x7f800000);
-        const bool any_hit = __any_sync(0xffffffffu, hitmask != 0u);
-        if (any_hit) {
-          // 8-9 % of the warp-tiles on the benchmark's data in the first chunk, a fraction of a per cent later: some
-          // column of some row of this warp can still hold the minimum.  The accumulator is still ours: a group
-          // that hit is read again (both halves in flight together) and looked at column by column.  (Doing this on
-          // the spot per fragment, from the registers of the main pass, costs a vote and a branch per fragment on
-          // EVERY warp-tile: measured slower as soon as hits are rare, i.e. for every chunk but the first.)
-#pragma unroll 1
-          for (int gp = 0; gp < SC_CW / 32; ++gp) {
-            const bool mine = (hitmask >> gp) & 1u;
-            if (!__any_sync(0xffffffffu, mine)) continue;
-            ptx::tmem_ld_32x16(t_base + 32 * gp, ra);
-            ptx::tmem_ld_32x16(t_base + 32 * gp + 16, rb);
-            ptx::tmem_ld_wait();
-            if (mine) {
-              // (the instruction count is what this path costs -- one warp's share of the issue slots: 32 x (FFMA,
-              // compare, predicated OR) plus a min3 tree; the smallest value of the group is a candidate whenever any is)
-              const float* tb = &col_tb[cb + 32 * gp];
-              const float thr_f = fminf(thr, 3.0e38f);   // +inf columns (beyond n) never pass, even against an infinite bound
-              float lv[32];
+      }
+      ptx::wgmma_commit();
+      ptx::wgmma_wait<0>();
+      ptx::fence_regs(acc[0]);
+      ptx::fence_regs(acc[1]);
+      if (lead) {   // the x stage (and, after the item's last tile, the y block) is free again
+        ptx::mbar_arrive(&aempty[s]);
+        if (mt == mt1 - 1) ptx::mbar_arrive(bempty);
+      }
+
+      // per row and 32-column group gp: this thread holds 8 of the group's values, acc[gp >> 2][4i + 2j + e] with
+      // i in [4 (gp & 3), 4 (gp & 3) + 4).  c < 0, so  c max acc + min_{j in G} t_j  bounds all 8 from below, and a
+      // group holds a value at or below the threshold only if the bound of some thread's 8 values reaches it.
+      unsigned hitmask[2] = {0u, 0u};
 #pragma unroll
-              for (int c = 0; c < 16; ++c) {
-                lv[c]      = fmaf(__uint_as_float(ra[c]), cf, tb[c]);
-                lv[16 + c] = fmaf(__uint_as_float(rb[c]), cf, tb[16 + c]);
+      for (int gp = 0; gp < 8; ++gp) {
+#pragma unroll
+        for (int j = 0; j < 2; ++j) {
+          const float* a = &acc[gp >> 2][16 * (gp & 3) + 2 * j];
+          const float mx = fmaxf(max3(max3(a[0], a[1], a[4]), max3(a[5], a[8], a[9]), a[12]), a[13]);
+          hitmask[j] |= (fmaf(mx, cf[j], col_gm[gp]) <= thr[j]) ? (1u << gp) : 0u;
+        }
+      }
+      unsigned long long cmask[2] = {0ull, 0ull};  // bit 2i + e: column 8i + 2tq + e of the block goes to the exact pass
+      float vmin[2] = {__int_as_float(0x7f800000), __int_as_float(0x7f800000)};
+      if (__any_sync(0xffffffffu, (hitmask[0] | hitmask[1]) != 0u)) {
+        // rare after the first y blocks: some column of some row of this warp can still hold the minimum
+#pragma unroll
+        for (int j = 0; j < 2; ++j) {
+          const float thr_f = fminf(thr[j], 3.0e38f);   // +inf columns (beyond n) never pass, even against an infinite bound
+#pragma unroll
+          for (int gp = 0; gp < 8; ++gp) {
+            if ((hitmask[j] >> gp) & 1u) {
+#pragma unroll
+              for (int ii = 0; ii < 4; ++ii) {
+                const int i = 4 * gp + ii;   // 8-column group of the block, 0..31
+#pragma unroll
+                for (int e = 0; e < 2; ++e) {
+                  const float lv = fmaf(acc[i >> 4][4 * (i & 15) + 2 * j + e], cf[j], col_tb[8 * i + 2 * tq + e]);
+                  if (lv <= thr_f) {
+                    cmask[j] |= 1ull << (2 * i + e);
+                    vmin[j] = fminf(vmin[j], lv);
+                  }
+                }
               }
-              unsigned bits = 0;
-#pragma unroll
-              for (int c = 0; c < 32; ++c) bits |= (lv[c] <= thr_f) ? (1u << c) : 0u;
-              float g0 = min3(lv[0], lv[1], lv[2]), g1 = min3(lv[3], lv[4], lv[5]), g2 = min3(lv[6], lv[7], lv[8]),
-                    g3 = min3(lv[9], lv[10], lv[11]);
-#pragma unroll
-              for (int c = 12; c < 32; c += 8) {
-                g0 = min3(g0, lv[c], lv[c + 1]);
-                g1 = min3(g1, lv[c + 2], lv[c + 3]);
-                if (c + 4 < 32) g2 = min3(g2, lv[c + 4], lv[c + 5]);
-                if (c + 6 < 32) g3 = min3(g3, lv[c + 6], lv[c + 7]);
-              }
-              if (bits != 0u) vmin = fminf(vmin, fminf(min3(g0, g1, g2), g3));
-              cmask[gp >> 1] |= static_cast<unsigned long long>(bits) << (32 * (gp & 1));
             }
           }
         }
-        // hand the accumulator back to the MMA warp
-        ptx::tc_fence_before();
-        __syncwarp();
-#ifdef SC_TRACE
-        { const bool hit = __any_sync(0xffffffffu, any_hit);
-          if (lane == 0 && blockIdx.x == 0 && tt < 2048u) { g_sc_wtrace[1][w][tt] = clock64(); g_sc_wtrace[2][w][tt] = hit ? 1 : 0; } }
-#endif
-        if (lane == 0 && w == 0) SC_STAMP(5, tt);
-        if (lane == 0 && w == 15) SC_STAMP(6, tt);
-        if (lane == 0) ptx::mbar_arrive(&tempty[as]);
-        // Nothing below may make this warp late for its next tile (the accumulator stage is free again only when
-        // all 16 warps have drained it): the timeline showed warps arriving 1000-3000 cycles late after an
-        // atomicCAS round trip on the bound plus one same-address atomicAdd per candidate.  So: the bound is lowered
-        // with a fire-and-forget reduction (no return value), and list slots come out of a private block of SC_BLK
-        // entries per warp, reserved with ONE atomicAdd when the previous block is used up (unused entries of a
-        // block are marked invalid, nn_exact_kernel skips them); the entry holds the packed POSITION, which
-        // nn_exact_kernel translates (a dependent col_map load here would stall the store).
-        int ncand = 0;
+      }
+      // The bound is lowered with a fire-and-forget reduction (no return value), and list slots come out of a private
+      // block of SC_BLK entries per warp, reserved with ONE atomicAdd when the previous block is used up (unused entries
+      // of a block are marked invalid, nn_exact_kernel skips them); the entry holds the packed POSITION, which
+      // nn_exact_kernel translates.
+      const int ncand = __popcll(cmask[0]) + __popcll(cmask[1]);
+      if (__any_sync(0xffffffffu, ncand != 0)) {
 #pragma unroll
-        for (int wd = 0; wd < SC_SETS; ++wd) ncand += __popcll(cmask[wd]);
-        if (__any_sync(0xffffffffu, ncand != 0)) {
-          if (ncand != 0) {
+        for (int j = 0; j < 2; ++j) {
+          if (cmask[j] != 0ull) {
             // every coarse value is also an UPPER bound of a real pair's distance (value + margin): later
             // tiles of this row, here and on the other SMs, screen against the tighter bound
-            float nb = vmin + margin;
-            nb += (fabsf(nb) + 2.f * (aux_c.y * aux_c.y + yn_max)) * (1.f / 2097152.f);
-            if (nb < aux_c.x) {   // float min as integer reductions: non-negative -> signed min, negative -> unsigned max
-              if (nb >= 0.f) atomicMin(reinterpret_cast<int*>(&p.aux[row].x), __float_as_int(nb));
-              else atomicMax(reinterpret_cast<unsigned*>(&p.aux[row].x), __float_as_uint(nb));
+            float nb = vmin[j] + margin[j];
+            nb += (fabsf(nb) + 2.f * (aux_c[j].y * aux_c[j].y + yn_max)) * (1.f / 2097152.f);
+            if (nb < aux_c[j].x) {   // float min as integer reductions: non-negative -> signed min, negative -> unsigned max
+              if (nb >= 0.f) atomicMin(reinterpret_cast<int*>(&p.aux[row[j]].x), __float_as_int(nb));
+              else atomicMax(reinterpret_cast<unsigned*>(&p.aux[row[j]].x), __float_as_uint(nb));
             }
           }
-          if (list_full) {
-            // (warp-uniform) a reservation of this warp already came back beyond the end of the list: the overflow flag
-            // is up, the exact pass will redo these blocks, and the slot counter must not keep growing -- data on which
-            // everything is a candidate would otherwise wrap it around and overwrite the incumbents' entries
-            if (lane == 0) *p.overflow = 1u;
+        }
+        if (list_full) {
+          // (warp-uniform) a reservation of this warp already came back beyond the end of the list: the overflow flag
+          // is up, the exact pass will redo these blocks, and the slot counter must not keep growing -- data on which
+          // everything is a candidate would otherwise wrap it around and overwrite the incumbents' entries
+          if (lane == 0) *p.overflow = 1u;
+        } else {
+          int incl = ncand;
+#pragma unroll
+          for (int o = 1; o < 32; o <<= 1) {
+            const int v = __shfl_up_sync(0xffffffffu, incl, o);
+            if (lane >= o) incl += v;
+          }
+          const int total = __shfl_sync(0xffffffffu, incl, 31);
+          if (lane == 0) atomicAdd(p.cand_cnt + 6, static_cast<unsigned>(total));   // real candidates (slots include unused ones)
+          unsigned slot;
+          if (total > SC_BLK) {  // (more candidates in one warp-tile than a block holds: a reservation of its own)
+            unsigned base = 0;
+            if (lane == 0) base = atomicAdd(p.cand_cnt, static_cast<unsigned>(total));
+            base = __shfl_sync(0xffffffffu, base, 0);
+            if (base >= p.cand_cap) list_full = true;
+            slot = base + static_cast<unsigned>(incl - ncand);
           } else {
-            int incl = ncand;
-#pragma unroll
-            for (int o = 1; o < 32; o <<= 1) {
-              const int v = __shfl_up_sync(0xffffffffu, incl, o);
-              if (lane >= o) incl += v;
-            }
-            const int total = __shfl_sync(0xffffffffu, incl, 31);
-            if (lane == 0) atomicAdd(p.cand_cnt + 6, static_cast<unsigned>(total));   // real candidates (slots include unused ones)
-            unsigned slot;
-            if (total > SC_BLK) {  // (more candidates in one warp-tile than a block holds: a reservation of its own)
+            if (blk_used + total > SC_BLK) {
+#pragma unroll 1
+              for (int i = blk_used + lane; i < SC_BLK; i += 32)
+                if (blk_base + i < p.cand_cap) p.cand[blk_base + i] = make_int2(-1, -1);
               unsigned base = 0;
-              if (lane == 0) base = atomicAdd(p.cand_cnt, static_cast<unsigned>(total));
-              base = __shfl_sync(0xffffffffu, base, 0);
-              if (base >= p.cand_cap) list_full = true;
-              slot = base + static_cast<unsigned>(incl - ncand);
-            } else {
-              if (blk_used + total > SC_BLK) {
-#pragma unroll 1
-                for (int i = blk_used + lane; i < SC_BLK; i += 32)
-                  if (blk_base + i < p.cand_cap) p.cand[blk_base + i] = make_int2(-1, -1);
-                unsigned base = 0;
-                if (lane == 0) base = atomicAdd(p.cand_cnt, static_cast<unsigned>(SC_BLK));
-                blk_base = __shfl_sync(0xffffffffu, base, 0);
-                blk_used = 0;
-                if (blk_base >= p.cand_cap) list_full = true;
-              }
-              slot = blk_base + static_cast<unsigned>(blk_used + incl - ncand);
-              blk_used += total;
+              if (lane == 0) base = atomicAdd(p.cand_cnt, static_cast<unsigned>(SC_BLK));
+              blk_base = __shfl_sync(0xffffffffu, base, 0);
+              blk_used = 0;
+              if (blk_base >= p.cand_cap) list_full = true;
             }
+            slot = blk_base + static_cast<unsigned>(blk_used + incl - ncand);
+            blk_used += total;
+          }
 #pragma unroll
-            for (int wd = 0; wd < SC_SETS; ++wd) {
-              unsigned long long cm = cmask[wd];
+          for (int j = 0; j < 2; ++j) {
+            unsigned long long cm = cmask[j];
 #pragma unroll 1
-              while (cm != 0ull) {
-                const int c = __ffsll(static_cast<long long>(cm)) - 1 + 64 * wd;
-                cm &= cm - 1ull;
-                if (slot < p.cand_cap) p.cand[slot] = make_int2(static_cast<int>(row), n_blk * TC_BN + cb + c);
-                else *p.overflow = 1u;
-                ++slot;
-              }
+            while (cm != 0ull) {
+              const int b = __ffsll(static_cast<long long>(cm)) - 1;
+              cm &= cm - 1ull;
+              const int col = 8 * (b >> 1) + 2 * tq + (b & 1);
+              if (slot < p.cand_cap) p.cand[slot] = make_int2(static_cast<int>(row[j]), n_blk * TC_BN + col);
+              else *p.overflow = 1u;
+              ++slot;
             }
           }
         }
       }
-      t_it += static_cast<uint32_t>(mt1 - mt0);
     }
+  }
 #pragma unroll 1
-    for (int i = blk_used + lane; i < SC_BLK; i += 32)   // the unused rest of this warp's last block
-      if (blk_base + i < p.cand_cap) p.cand[blk_base + i] = make_int2(-1, -1);
-  }
-
-  ptx::tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    ptx::tc_fence_after();
-    ptx::tmem_dealloc<512>(tmem_base);
-  }
+  for (int i = blk_used + lane; i < SC_BLK; i += 32)   // the unused rest of this warp's last block
+    if (blk_base + i < p.cand_cap) p.cand[blk_base + i] = make_int2(-1, -1);
 }
-
-#undef B2D_SCREEN_FRAGMENT
 
 }  // namespace b2d

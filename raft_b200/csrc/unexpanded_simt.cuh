@@ -225,24 +225,23 @@ __device__ __forceinline__ void ux_unpk(uint64_t v, float& lo, float& hi)
 {
   asm("mov.b64 {%0, %1}, %2;" : "=f"(lo), "=f"(hi) : "l"(v));
 }
+// (Hopper has no packed f32x2 pipe: two scalar operations on the halves of the pair)
 __device__ __forceinline__ uint64_t ux_add2(uint64_t a, uint64_t b)
 {
-  uint64_t r;
-  asm("add.rn.f32x2 %0, %1, %2;" : "=l"(r) : "l"(a), "l"(b));
-  return r;
+  float a0, a1, b0, b1;
+  ux_unpk(a, a0, a1);
+  ux_unpk(b, b0, b1);
+  return ux_pk(a0 + b0, a1 + b1);
 }
 __device__ __forceinline__ uint64_t ux_fma2(uint64_t a, uint64_t b, uint64_t c)
 {
-  uint64_t r;
-  asm("fma.rn.f32x2 %0, %1, %2, %3;" : "=l"(r) : "l"(a), "l"(b), "l"(c));
-  return r;
+  float a0, a1, b0, b1, c0, c1;
+  ux_unpk(a, a0, a1);
+  ux_unpk(b, b0, b1);
+  ux_unpk(c, c0, c1);
+  return ux_pk(fmaf(a0, b0, c0), fmaf(a1, b1, c1));
 }
-__device__ __forceinline__ float ux_max3(float a, float b, float c)
-{
-  float r;
-  asm("max.f32 %0, %1, %2, %3;" : "=f"(r) : "f"(a), "f"(b), "f"(c));
-  return r;
-}
+__device__ __forceinline__ float ux_max3(float a, float b, float c) { return fmaxf(fmaxf(a, b), c); }
 
 // TMA-fed variant (rows 16-byte aligned, k % 4 == 0, row-major): the same 128x128x32 tiles arrive
 // by cp.async.bulk.tensor with SWIZZLE_128B -- the XOR pattern the manual loader writes -- through
@@ -283,7 +282,7 @@ unexpanded_tma_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_c
   if (tid == 0)
     for (int kb = 0; kb < UX_TMA_STAGES - 1 && kb < nkb; ++kb) issue(kb);
 
-  // L2 / L2Sqrt: packed f32x2 math (FADD2 + FFMA2: one issue slot per pair-element instead of two);
+  // L2 / L2Sqrt: (even-k, odd-k) pair math;
   // every output keeps an (even-k, odd-k) pair of partial sums that is folded at the end.
   constexpr bool kPackedL2 = (kMetric == UX_L2 || kMetric == UX_L2SQRT);
   constexpr int kD = kMetric == UX_BRAYCURTIS ? 8 : 1;

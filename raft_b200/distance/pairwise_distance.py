@@ -2,7 +2,7 @@
 (removed from the reference snapshot, CHANGELOG.md:59; API per SURVEY.md 8(b); wrapper
 conventions per python/pylibraft/pylibraft/random/rmat_rectangular_generator.pyx:24-69).
 
-Dispatches through the C ABI (include/raft_b200.h: b2d_pairwise_distance) into the sm_100a
+Dispatches through the C ABI (include/raft_b200.h: b2d_pairwise_distance) into the sm_90a
 kernels.  No CPU fallback."""
 from __future__ import annotations
 

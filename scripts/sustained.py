@@ -5,9 +5,6 @@ from raft_b200.distance import pairwise_distance
 from raft_b200.common import DeviceResources
 m = n = 100000; k = int(sys.argv[1]) if len(sys.argv) > 1 else 128; steps = int(sys.argv[2]) if len(sys.argv) > 2 else 60
 h = DeviceResources()
-if len(sys.argv) > 3:   # third argument: 0 forces the 1-CTA store kernel
-    from raft_b200 import _lib
-    _lib.check(_lib.lib().b2d_set_option(b"pairwise_2cta", float(sys.argv[3])))
 g = torch.Generator(device="cuda").manual_seed(0)
 x = torch.randn(m, k, device="cuda", generator=g) * 3; y = torch.randn(n, k, device="cuda", generator=g) * 3
 out = torch.empty(m, n, device="cuda")

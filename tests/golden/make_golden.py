@@ -1,6 +1,6 @@
 """Generates tests/golden/*.npz (run once, here, where scipy is installed; outputs are committed).
 
-Why scipy: the reference's own implementation of this path is absent from /root/reference
+Why scipy: the reference's own implementation of this path is absent from the reference snapshot
 (raft::distance and pylibraft.distance were removed upstream in 26.02, CHANGELOG.md:59), so the
 reference itself cannot be imported to generate vectors.  The historical pylibraft tests compared
 against scipy.spatial.distance.cdist (SURVEY.md section 4, [RECALLED]) and BASELINE.json configs[0]
@@ -35,7 +35,8 @@ def main():
         out[f"{name}_x"], out[f"{name}_y"] = x, y
         x64, y64 = x.astype(np.float64), y.astype(np.float64)
         for metric, sp in SCIPY.items():
-            out[f"{name}_{metric}"] = cdist(x64, y64, sp)
+            if metric not in ("L2Unexpanded", "L2SqrtUnexpanded"):   # same values as the expanded forms: the golden
+                out[f"{name}_{metric}"] = cdist(x64, y64, sp)       # fixture (tests/conftest.py) aliases them
         out[f"{name}_LpUnexpanded_p3"] = cdist(x64, y64, "minkowski", p=3.0)
         out[f"{name}_InnerProduct"] = x64 @ y64.T
         d = cdist(x64, y64, "sqeuclidean")

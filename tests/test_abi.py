@@ -28,16 +28,16 @@ def test_library_builds_and_exports_every_declared_symbol():
     assert sorted(_lib.SYMBOLS) == syms
 
 
-def test_library_is_sm100a_only_and_has_tcgen05_tma():
+def test_library_is_sm90a_only_and_has_wgmma_tma():
     import shutil
     import subprocess
     cuobjdump = shutil.which("cuobjdump") or "/usr/local/cuda/bin/cuobjdump"
     if not os.path.exists(cuobjdump):
         pytest.skip("cuobjdump not available")
     out = subprocess.run([cuobjdump, "-lelf", _build.SO_PATH], capture_output=True, text=True).stdout
-    assert "sm_100a" in out
+    assert "sm_90a" in out and "sm_100" not in out
     sass = subprocess.run([cuobjdump, "-sass", _build.SO_PATH], capture_output=True, text=True).stdout
-    for mnemonic in ("UTCHMMA", "UTMALDG", "LDTM", "UTMASTG"):
+    for mnemonic in ("HGMMA", "UTMALDG", "SYNCS"):
         assert mnemonic in sass, mnemonic
 
 

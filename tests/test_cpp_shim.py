@@ -61,7 +61,7 @@ def test_block_selection_helpers_partition_the_blocks():
     pass, the trial screen and the main screen visit every y block exactly once, in ascending order."""
     nvcc = shutil.which("nvcc") or "/usr/local/cuda/bin/nvcc"
     exe = os.path.join(ROOT, "tests", "cpp", "host_logic_test")
-    cmd = [nvcc, "-std=c++17", "-O1", "--expt-relaxed-constexpr", "-gencode", "arch=compute_100a,code=sm_100a", "-o", exe,
+    cmd = [nvcc, "-std=c++17", "-O1", "--expt-relaxed-constexpr", "-gencode", "arch=compute_90a,code=sm_90a", "-o", exe,
            os.path.join(ROOT, "tests", "cpp", "host_logic_test.cu")]
     res = subprocess.run(cmd, capture_output=True, text=True)
     assert res.returncode == 0, res.stdout + res.stderr

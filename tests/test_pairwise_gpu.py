@@ -324,33 +324,6 @@ def test_outlier_rows_do_not_degrade_ordinary_rows(metric, where):
         check(got, ref)
 
 
-@pytest.fixture
-def cta_pair_kernel():
-    """Routes k <= 128 aligned-output problems through the CTA-pair kernel (expanded_tc2.cuh: cluster of 2,
-    tcgen05 cta_group::2, full-width output rows); the default is the 1-CTA kernel (same speed, DESIGN.md)."""
-    from raft_b200 import _lib
-    _lib.check(_lib.lib().b2d_set_option(b"pairwise_2cta", 1.0))
-    yield
-    _lib.check(_lib.lib().b2d_set_option(b"pairwise_2cta", 0.0))
-
-
-@pytest.mark.parametrize("metric", [DT.L2Expanded, DT.L2SqrtExpanded, DT.CosineExpanded, DT.CorrelationExpanded])
-@pytest.mark.parametrize("shape", [(1024, 1024, 32), (700, 1300, 128), (129, 260, 96), (3000, 2048, 64), (100, 8, 5)])
-def test_cta_pair_kernel_vs_oracle(cta_pair_kernel, metric, shape):
-    # odd numbers of x tiles (the second CTA of the last pair runs past m), y blocks cut by the right edge, tiny shapes
-    x, y = blobs(*shape)
-    check(run(x, y, metric), oracle.pairwise_distance(x, y, metric))
-
-
-def test_cta_pair_kernel_self_distance_and_outliers(cta_pair_kernel):
-    x, _ = blobs(900, 4, 100)
-    x[5] *= 1.0e9                                       # a row with its own exponent (per-row / per-column scales)
-    xd = torch.from_numpy(x).cuda()
-    got = pairwise_distance(xd, xd, metric=DT.L2Expanded).copy_to_host()   # the SAME device array: x == y aliasing
-    assert (np.diag(got) == 0).all()
-    check(got, oracle.pairwise_distance(x, x, DT.L2Expanded))
-
-
 F64_METRICS = [DT.L2Expanded, DT.L2SqrtExpanded, DT.CosineExpanded, DT.CorrelationExpanded, DT.InnerProduct, DT.L1,
                DT.L2Unexpanded, DT.L2SqrtUnexpanded, DT.Linf, DT.Canberra, DT.LpUnexpanded]
 
