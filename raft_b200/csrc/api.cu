@@ -234,28 +234,46 @@ static int launch_prep(cudaStream_t s, const TcWorkspace& w, const void* x, int6
   return B2D_OK;
 }
 
-template <bool kRes, int kEpi, int kPost>
-static int launch_tc_inst(cudaStream_t s, const CUtensorMap& ma, const CUtensorMap& mb, const TcParams& p, int grid)
+// the pairwise output dist[rows][cols] (row pitch ldd) as the target of the EPI_STORE TMA stores: boxes of 32 columns x
+// 64 rows, SWIZZLE_128B (expanded_tc.cuh tc_stage_store); needs a 16-byte aligned base and pitch
+static int make_dist_map(CUtensorMap* map, float* dist, int64_t rows, int64_t cols, int64_t ldd)
 {
+  EncodeTiledFn enc = get_encode();
+  if (!enc) return fail(B2D_ERR_CUDA, "cuTensorMapEncodeTiled entry point unavailable (no CUDA driver?)");
+  cuuint64_t dims[2]    = {static_cast<cuuint64_t>(cols), static_cast<cuuint64_t>(rows)};
+  cuuint64_t strides[1] = {static_cast<cuuint64_t>(ldd) * 4};
+  cuuint32_t box[2]     = {TC_D_BOX_COLS, TC_D_BOX_ROWS};
+  cuuint32_t estr[2]    = {1, 1};
+  CUresult r = enc(map, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, dist, dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
+                   CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_NONE, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  if (r != CUDA_SUCCESS) return fail(B2D_ERR_CUDA, "cuTensorMapEncodeTiled(dist) failed: " + std::to_string((int)r));
+  return B2D_OK;
+}
+
+template <bool kRes, int kEpi, int kPost>
+static int launch_tc_inst(cudaStream_t s, const CUtensorMap& ma, const CUtensorMap& mb, const CUtensorMap& md,
+                          const TcParams& p, int grid)
+{
+  constexpr size_t smem = TcCarve<kRes, kEpi>::bytes;
   // the attribute is per device and per function: cheap, set on every launch
   B2D_CUDA(cudaFuncSetAttribute(expanded_tc_kernel<kRes, kEpi, kPost>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                static_cast<int>(TC_SMEM_BYTES)));
-  expanded_tc_kernel<kRes, kEpi, kPost><<<grid, TC_THREADS, TC_SMEM_BYTES, s>>>(ma, mb, p);
+                                static_cast<int>(smem)));
+  expanded_tc_kernel<kRes, kEpi, kPost><<<grid, TC_THREADS, smem, s>>>(ma, mb, md, p);
   B2D_CUDA(cudaGetLastError());
   return B2D_OK;
 }
 
 template <bool kRes>
-static int launch_tc_epi(cudaStream_t s, const CUtensorMap& ma, const CUtensorMap& mb, const TcParams& p, int grid, int epi,
-                         int post)
+static int launch_tc_epi(cudaStream_t s, const CUtensorMap& ma, const CUtensorMap& mb, const CUtensorMap& md,
+                         const TcParams& p, int grid, int epi, int post)
 {
-  if (epi == EPI_MINLOC) return launch_tc_inst<kRes, EPI_MINLOC, POST_NONE>(s, ma, mb, p, grid);
-  if (epi == EPI_TOPK) return launch_tc_inst<kRes, EPI_TOPK, POST_NONE>(s, ma, mb, p, grid);
-  if (post == POST_NONE) return launch_tc_inst<kRes, EPI_STORE, POST_NONE>(s, ma, mb, p, grid);
-  if (post == POST_CLAMP) return launch_tc_inst<kRes, EPI_STORE, POST_CLAMP>(s, ma, mb, p, grid);
-  if (post == POST_JACCARD) return launch_tc_inst<kRes, EPI_STORE, POST_JACCARD>(s, ma, mb, p, grid);
-  if (post == POST_DICE) return launch_tc_inst<kRes, EPI_STORE, POST_DICE>(s, ma, mb, p, grid);
-  return launch_tc_inst<kRes, EPI_STORE, POST_CLAMP_SQRT>(s, ma, mb, p, grid);
+  if (epi == EPI_MINLOC) return launch_tc_inst<kRes, EPI_MINLOC, POST_NONE>(s, ma, mb, md, p, grid);
+  if (epi == EPI_TOPK) return launch_tc_inst<kRes, EPI_TOPK, POST_NONE>(s, ma, mb, md, p, grid);
+  if (post == POST_NONE) return launch_tc_inst<kRes, EPI_STORE, POST_NONE>(s, ma, mb, md, p, grid);
+  if (post == POST_CLAMP) return launch_tc_inst<kRes, EPI_STORE, POST_CLAMP>(s, ma, mb, md, p, grid);
+  if (post == POST_JACCARD) return launch_tc_inst<kRes, EPI_STORE, POST_JACCARD>(s, ma, mb, md, p, grid);
+  if (post == POST_DICE) return launch_tc_inst<kRes, EPI_STORE, POST_DICE>(s, ma, mb, md, p, grid);
+  return launch_tc_inst<kRes, EPI_STORE, POST_CLAMP_SQRT>(s, ma, mb, md, p, grid);
 }
 
 static int launch_tc(cudaStream_t s, const TcWorkspace& w, TcParams p, int64_t k, int epi, int post, int kb0 = 0,
@@ -293,8 +311,15 @@ static int launch_tc(cudaStream_t s, const TcWorkspace& w, TcParams p, int64_t k
   // resident: the whole 256-row y block in one box per k-block; streaming: one 128-row half per stage
   rc = make_operand_map(&mb, w.yop, p.n, p.nkb, resident ? TC_BN : TC_HN, kb0, nkb_total);
   if (rc) return rc;
+  CUtensorMap md;   // only read by the kernel when EPI_STORE goes through TMA
+  memset(&md, 0, sizeof(md));
+  if (epi == EPI_STORE && p.tma_store) {
+    rc = make_dist_map(&md, p.dist, p.m, p.n, p.ldd);
+    if (rc) return rc;
+  }
   const int grid = static_cast<int>(p.n_items < sms ? p.n_items : sms);
-  return resident ? launch_tc_epi<true>(s, ma, mb, p, grid, epi, post) : launch_tc_epi<false>(s, ma, mb, p, grid, epi, post);
+  return resident ? launch_tc_epi<true>(s, ma, mb, md, p, grid, epi, post)
+                  : launch_tc_epi<false>(s, ma, mb, md, p, grid, epi, post);
 }
 
 // coarse screening pass of the screened fusedL2NN (screen_tc.cuh) over the y blocks with
@@ -643,13 +668,21 @@ int b2d_pairwise_distance(void* stream, int metric, int dtype, const void* x, in
     memset(&p, 0, sizeof(p));
     p.m = ma; p.n = na; p.dist = dist; p.ldd = ldd;
     p.diag_zero = (post != POST_NONE && x == y && m == n && ldx == ldy && mode == PREP_L2) ? 1 : 0;
-    p.pair_ok   = (reinterpret_cast<uintptr_t>(dist) % 8 == 0 && ldd % 2 == 0) ? 1 : 0;
+    // the result leaves through shared-memory staging and TMA stores wherever TMA can address dist: 16-byte aligned
+    // base and pitch, row and column coordinates within int32 (the store takes 32-bit coordinates), and rows that end
+    // on a 16-byte boundary.  The last condition is from observation: on an H100, with n = 150 and ldd = 160, the
+    // box stores also wrote columns 150 and 151, i.e. the partial 16 bytes at the end of each row, into the caller's
+    // padding (tests/test_pairwise_gpu.py::test_padded_leading_dimensions_and_out_param).  Otherwise, and for the
+    // read-modify-write K chunks below, the epilogue stores from registers.
+    p.tma_store = (reinterpret_cast<uintptr_t>(dist) % 16 == 0 && ldd % 4 == 0 && na % 4 == 0 && ma <= 0x7fffffffll &&
+                   na <= 0x7fffffffll) ? 1 : 0;
     // k > 320: accumulate K in chunks of 256 columns, each added to dist with a round-to-nearest fp32
     // add -- bounds the truncation bias of long MMA chains (DESIGN.md, numerics)
     const int nkb_total = static_cast<int>((k + 31) / 32);
     constexpr int kChunk = 8;
     ProfileScope prof(s);  // the main kernel(s) only: the operand preparation above is outside
     if (nkb_total > 10 && post < POST_JACCARD) {  // (the ratio metrics need the whole inner product at once)
+      p.tma_store = 0;
       for (int kb0 = 0; kb0 < nkb_total; kb0 += kChunk) {
         const int nk = nkb_total - kb0 < kChunk ? nkb_total - kb0 : kChunk;
         p.acc_mode   = kb0 == 0 ? 1 : (kb0 + nk >= nkb_total ? 3 : 2);

@@ -29,9 +29,12 @@
 //  !kResident (k > 128): both operands stream per k-block (stages of 16 KB of x + 16 KB of the y half).
 //
 // Epilogues (straight from the registers; d = acc * c + (t_x[i] + t_y[j]), c one scalar):
-//   EPI_STORE         each thread holds 2 adjacent columns of 2 rows per 8-column group: a warp-wide
-//                     8-byte streaming store writes 8 rows x one full 32-byte sector.  Also the
-//                     read-modify-write path of K-chunked accumulation (k > 320).
+//   EPI_STORE         the finished 64 x 128 fragment goes to the warpgroup's own staging boxes in shared
+//                     memory (SWIZZLE_128B, a ring of 64-row x 32-column boxes) and leaves by TMA stores that
+//                     drain while the warpgroup runs the next half's MMAs (tc_stage_store).  Where TMA cannot
+//                     address dist (unaligned base or pitch) and in the read-modify-write path of K-chunked
+//                     accumulation (k > 320), each thread stores its 2 adjacent columns of 2 rows per
+//                     8-column group straight from the registers (8-byte streaming stores).
 //   EPI_MINLOC        per row the minimum of the thread's 16 values of a 64-column chunk is compared with
 //                     the row's current global best (read from keys at tile start: an upper bound, keys
 //                     only decrease); only a candidate that can change the result takes the slow path
@@ -56,8 +59,17 @@ constexpr int TC_BH_BYTES    = TC_HN * 128;  // one k-block of a streamed y half
 constexpr int TC_MAX_RES_KB  = 4;            // resident-B variant: k <= 128
 constexpr int TC_STAGES_RES  = 5;            // A-only stages (16 KB) next to the resident y block
 constexpr int TC_STAGES_STR  = 6;            // A + B-half stages (32 KB) when both operands stream
+constexpr int TC_STAGES_RES_ST = 4;          // the same with the output staging of EPI_STORE beside them
+constexpr int TC_STAGES_STR_ST = 6;
 constexpr int TC_MAX_STAGES  = 6;
 constexpr int TC_THREADS     = 384;
+// EPI_STORE output staging: TMA boxes of 64 rows x 32 fp32 columns (128-byte rows, SWIZZLE_128B), a ring of
+// TC_STG_BOXES per consumer warpgroup (DESIGN.md section 2 K1: the carve against the x stages, measured).  The ring
+// logic of tc_stage_store is written for exactly two boxes.
+constexpr int TC_D_BOX_COLS  = 32;
+constexpr int TC_D_BOX_ROWS  = 64;
+constexpr int TC_D_BOX_BYTES = TC_D_BOX_COLS * TC_D_BOX_ROWS * 4;
+constexpr int TC_STG_BOXES   = 2;
 
 enum TcEpilogue : int { EPI_STORE = 0, EPI_MINLOC = 1, EPI_TOPK = 2 };
 // max(v, 0) that keeps a NaN (fmaxf(NaN, 0) = 0 would turn a poisoned distance into a perfect match)
@@ -101,7 +113,7 @@ struct TcParams {
   float* dist;
   int64_t ldd;
   int diag_zero;          // x and y alias: force d(i,i) = 0 (reference: CHANGELOG.md:1057,1213)
-  int pair_ok;            // dist 8-byte aligned and ldd even -> st.v2
+  int tma_store;          // dist goes out through the staging boxes and the dist tensor map (api.cu: aligned, single pass)
   int acc_mode;           // K-chunked accumulation: 0 single pass, 1 first chunk (raw store), 2 middle (+=), 3 last (+=, post)
   // EPI_MINLOC
   long long* keys;        // [m] packed (ordered bits of the distance << 32 | index)
@@ -119,8 +131,24 @@ struct TcParams {
 
 constexpr size_t TC_SMEM_OPERANDS = (size_t)TC_MAX_RES_KB * TC_B_BYTES + (size_t)TC_STAGES_RES * TC_A_BYTES;  // 208 KB
 static_assert((size_t)TC_STAGES_STR * (TC_A_BYTES + TC_BH_BYTES) <= TC_SMEM_OPERANDS, "streaming carve fits");
-constexpr size_t TC_SMEM_BYTES = TC_SMEM_OPERANDS + TC_BN * 4 + 256;
-static_assert(TC_SMEM_BYTES <= 232448, "exceeds the 227 KB per-CTA limit");
+
+// Shared-memory carve of one instantiation: [resident y block][x (+ y half) stages][output staging][t_y][barriers].
+// The arg-min / top-k epilogues store nothing and keep 208 KB of operands; EPI_STORE trades one x stage for 32 KB of
+// output staging (the streaming variant fits it beside all of its stages).
+template <bool kResident, int kEpi>
+struct TcCarve {
+  static constexpr int stages = kEpi == EPI_STORE ? (kResident ? TC_STAGES_RES_ST : TC_STAGES_STR_ST)
+                                                  : (kResident ? TC_STAGES_RES : TC_STAGES_STR);
+  static constexpr uint32_t stage_bytes = kResident ? TC_A_BYTES : TC_A_BYTES + TC_BH_BYTES;
+  static constexpr size_t a_off   = kResident ? (size_t)TC_MAX_RES_KB * TC_B_BYTES : 0;
+  static constexpr size_t stg_off = a_off + (size_t)stages * stage_bytes;
+  static constexpr size_t tb_off  = kEpi == EPI_STORE ? stg_off + 2 * (size_t)TC_STG_BOXES * TC_D_BOX_BYTES : TC_SMEM_OPERANDS;
+  static constexpr size_t bytes   = tb_off + TC_BN * 4 + 256;
+  static_assert(stages <= TC_MAX_STAGES, "barrier arrays hold TC_MAX_STAGES stages");
+  static_assert(stg_off % 1024 == 0, "SWIZZLE_128B staging boxes need 1024-byte alignment");
+  static_assert(kEpi == EPI_STORE || stg_off <= TC_SMEM_OPERANDS, "operands fit");
+  static_assert(bytes <= 232448, "exceeds the 227 KB per-CTA limit");
+};
 
 // index of the s-th selected y block (see TcParams::sel_s)
 __host__ __device__ __forceinline__ int sel_to_blk(int s, int S, int lo, int hi)
@@ -172,7 +200,8 @@ __device__ __noinline__ void knn_append16(unsigned* cnt, long long* cand, unsign
 }
 
 // Epilogue of one 64 x 128 warpgroup tile.  v[4i + 2j + e] holds row row0 + 8j, column gc0 + 8i + e of the accumulator
-// (main + cross already summed); on return (EPI_STORE) the values have been written.
+// (main + cross already summed); on return (EPI_STORE) v holds the finished distances, and they have been written
+// unless p.tma_store (then tc_stage_store writes them).
 template <int kEpi, int kPost>
 __device__ __forceinline__ void tc_epilogue(float (&v)[64], const TcParams& p, const float* col_tb, int cl0, int64_t gc0,
                                             int64_t row0, const float (&ta)[2], const float (&cfr)[2], float (&thr)[2],
@@ -206,7 +235,8 @@ __device__ __forceinline__ void tc_epilogue(float (&v)[64], const TcParams& p, c
     }
   }
   if (kEpi == EPI_STORE) {
-    const bool fast = row0 + 8 < p.m && gc0 + 127 < p.n && p.pair_ok;
+    // (the manual stores: 8-byte vectors when dist and its pitch allow them)
+    const bool fast = row0 + 8 < p.m && gc0 + 127 < p.n && ((reinterpret_cast<uintptr_t>(p.dist) | p.ldd * 4) & 7u) == 0;
     if (p.acc_mode >= 2) {
       // K-chunked accumulation (k > 320): add this chunk's contribution to what the earlier chunks left in dist -- a
       // round-to-nearest fp32 add per chunk instead of ever longer truncating MMA chains on one accumulator
@@ -244,6 +274,7 @@ __device__ __forceinline__ void tc_epilogue(float (&v)[64], const TcParams& p, c
         for (int c = 0; c < 64; ++c) asm("sqrt.approx.f32 %0, %1;" : "=f"(v[c]) : "f"(v[c]));
       }
     }
+    if (p.tma_store) return;
 #pragma unroll
     for (int j = 0; j < 2; ++j) {
       const int64_t gi = row0 + 8 * j;
@@ -315,20 +346,64 @@ __device__ __forceinline__ void tc_epilogue(float (&v)[64], const TcParams& p, c
   }
 }
 
+// EPI_STORE through TMA: the warpgroup's finished 64 x 128 tile v (fragment layout as in tc_epilogue) is written into
+// its ring of staging boxes and stored with one cp.async.bulk.tensor per 64 x 32 box (L2 evict-first: the result is not
+// read again here).  Only this warpgroup writes its boxes and only its lead thread (`issuer`) issues and waits for their
+// stores, so a box is rewritten only after that thread has seen the box's previous store finish reading it and the
+// warpgroup has passed its named barrier.  Boxes outside the matrix are skipped; TMA clips the ragged ones.  After the
+// CTA's last tile (`last`) the issuer waits for all its stores, so the CTA's shared memory outlives them.
+//   box element (r, c) sits at byte r * 128 + ((c / 4) ^ (r % 8)) * 16 + (c % 4) * 4 (SWIZZLE_128B): the warp's 8-byte
+//   writes (8 rows x 2 adjacent 16-byte chunks) cover every bank exactly twice -- no conflicts.
+__device__ __forceinline__ void tc_stage_store(const float (&v)[64], const CUtensorMap* tmap_d, uint32_t stg, bool issuer,
+                                               bool last, int wg, int64_t row_w, int64_t col_w, const TcParams& p)
+{
+  static_assert(TC_STG_BOXES == 2, "one box per barrier pair, slot = box parity, wait_group.read 1");
+  const int lane       = threadIdx.x & 31;
+  const int quad = lane >> 2, tq = lane & 3;
+  // this thread's rows 16 w + quad (+8) of the box and the swizzled 16-byte chunk of its column pair
+  const uint32_t t_off = (16 * ((threadIdx.x >> 5) & 3) + quad) * 128 + 8 * (tq & 1);
+  const uint32_t t_xor = static_cast<uint32_t>((tq >> 1) ^ quad) * 16;
+#pragma unroll
+  for (int b = 0; b < 4; ++b) {   // the tile's 4 boxes of 32 columns; a tile is 4 boxes, so box b uses slot b % 2
+    const uint32_t box = stg + (b & 1) * TC_D_BOX_BYTES;
+    // the store issued two boxes ago read this slot: it must be done (the latest store may still be reading)
+    if (issuer) ptx::tma_store_wait_read<1>();
+    ptx::bar_sync(2 + wg, 128);
+#pragma unroll
+    for (int ii = 0; ii < 4; ++ii) {
+      const int i = 4 * b + ii;   // 8-column group of the tile
+#pragma unroll
+      for (int j = 0; j < 2; ++j)
+        ptx::st_shared_v2(box + t_off + 8 * j * 128 + ((32 * ii) ^ t_xor), v[4 * i + 2 * j], v[4 * i + 2 * j + 1]);
+    }
+    ptx::fence_proxy_async_smem();   // the generic-proxy writes become visible to the TMA unit
+    ptx::bar_sync(2 + wg, 128);
+    if (issuer) {
+      const int64_t gc = col_w + TC_D_BOX_COLS * b;
+      if (gc < p.n && row_w < p.m)
+        ptx::tma_store_2d(tmap_d, box, static_cast<int32_t>(gc), static_cast<int32_t>(row_w), ptx::policy_evict_first());
+      ptx::tma_store_commit();   // one group per box (possibly empty): the wait above counts boxes
+    }
+  }
+  if (issuer && last) ptx::tma_store_wait_all();   // the CTA's last tile: its shared memory outlives every store
+}
+
 template <bool kResident, int kEpi, int kPost>
 __global__ void __launch_bounds__(TC_THREADS, 1)
-expanded_tc_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b, const TcParams p)
+expanded_tc_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b,
+                   const __grid_constant__ CUtensorMap tmap_d, const TcParams p)
 {
-  constexpr int kStages          = kResident ? TC_STAGES_RES : TC_STAGES_STR;
-  constexpr uint32_t kStageBytes = kResident ? TC_A_BYTES : TC_A_BYTES + TC_BH_BYTES;
+  using Carve                    = TcCarve<kResident, kEpi>;
+  constexpr int kStages          = Carve::stages;
+  constexpr uint32_t kStageBytes = Carve::stage_bytes;
   if (p.run_flag != nullptr && __ldg(p.run_flag) == 0u) return;  // conditional launch (no host round trip)
   extern __shared__ __align__(1024) uint8_t smem[];
   // SWIZZLE_128B atoms need 1024-byte alignment; the dynamic window starts 1024-aligned (no static
   // shared memory in this kernel).  Checked, not assumed: a misaligned base traps.
   if ((ptx::smem_u32(smem) & 1023u) != 0u) __trap();
   uint8_t* b_base = smem;  // resident: [nkb] k-blocks of the y block
-  uint8_t* a_base = smem + (kResident ? TC_MAX_RES_KB * TC_B_BYTES : 0);  // stages: x k-block (+ y half k-block)
-  float* col_tb   = reinterpret_cast<float*>(smem + TC_SMEM_OPERANDS);  // [256] t_y of this y block
+  uint8_t* a_base = smem + Carve::a_off;  // stages: x k-block (+ y half k-block)
+  float* col_tb   = reinterpret_cast<float*>(smem + Carve::tb_off);  // [256] t_y of this y block
   uint64_t* bars  = reinterpret_cast<uint64_t*>(col_tb + TC_BN);
   uint64_t* afull = bars;                       // [TC_MAX_STAGES]
   uint64_t* aempty = bars + TC_MAX_STAGES;      // [TC_MAX_STAGES]
@@ -345,6 +420,7 @@ expanded_tc_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_cons
     ptx::fence_mbar_init();
     ptx::prefetch_tmap(&tmap_a);
     ptx::prefetch_tmap(&tmap_b);
+    if (kEpi == EPI_STORE && p.tma_store) ptx::prefetch_tmap(&tmap_d);
   }
   __syncthreads();
 
@@ -493,6 +569,10 @@ expanded_tc_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_cons
         const int cl0 = h * TC_HN + 2 * tq;  // this thread's first column inside the tile
         tc_epilogue<kEpi, kPost>(acc, p, col_tb, cl0, static_cast<int64_t>(n_blk) * TC_BN + cl0, row0, ta, cfr, thr, xnr,
                                  ynu);
+        if (kEpi == EPI_STORE && p.tma_store)   // (this warpgroup's staging boxes: computed here, not kept live)
+          tc_stage_store(acc, &tmap_d, ptx::smem_u32(smem + Carve::stg_off) + wg * TC_STG_BOXES * TC_D_BOX_BYTES, lead,
+                         item + gridDim.x >= p.n_items && mt == mt1 - 1 && h == nh - 1, wg,
+                         static_cast<int64_t>(mt) * TC_BM + 64 * wg, static_cast<int64_t>(n_blk) * TC_BN + h * TC_HN, p);
       }
     }
   }

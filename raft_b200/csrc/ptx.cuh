@@ -99,39 +99,20 @@ __device__ __forceinline__ void tma_load_2d(void* smem_dst, const void* tmap, ui
     : "memory");
 }
 // 2-D tiled store shared -> global (bulk async-group completion); OOB parts of the box are clipped.
-__device__ __forceinline__ void tma_store_2d(const void* tmap, const void* smem_src, int32_t c0, int32_t c1,
-                                             uint64_t policy)
+// smem_src is a shared-window address (smem_u32).
+__device__ __forceinline__ void tma_store_2d(const void* tmap, uint32_t smem_src, int32_t c0, int32_t c1, uint64_t policy)
 {
   asm volatile(
     "cp.async.bulk.tensor.2d.global.shared::cta.bulk_group.L2::cache_hint [%0, {%2, %3}], [%1], %4;"
     :
-    : "l"(reinterpret_cast<uint64_t>(tmap)), "r"(smem_u32(smem_src)), "r"(c0), "r"(c1), "l"(policy)
-    : "memory");
-}
-// 1-D bulk copy shared -> global (UBLKCP), bulk async-group completion, L2 cache-policy hint.
-// Both addresses 16-byte aligned, bytes a multiple of 16.
-__device__ __forceinline__ void bulk_store(void* gmem_dst, const void* smem_src, uint32_t bytes, uint64_t policy)
-{
-  asm volatile("cp.async.bulk.global.shared::cta.bulk_group.L2::cache_hint [%0], [%1], %2, %3;"
-               :
-               : "l"(gmem_dst), "r"(smem_u32(smem_src)), "r"(bytes), "l"(policy)
-               : "memory");
-}
-// 3-D tiled store shared -> global; box elements outside the tensor are not written (also for negative coordinates)
-__device__ __forceinline__ void tma_store_3d(const void* tmap, const void* smem_src, int32_t c0, int32_t c1, int32_t c2,
-                                             uint64_t policy)
-{
-  asm volatile(
-    "cp.async.bulk.tensor.3d.global.shared::cta.bulk_group.L2::cache_hint [%0, {%2, %3, %4}], [%1], %5;"
-    :
-    : "l"(reinterpret_cast<uint64_t>(tmap)), "r"(smem_u32(smem_src)), "r"(c0), "r"(c1), "r"(c2), "l"(policy)
+    : "l"(reinterpret_cast<uint64_t>(tmap)), "r"(smem_src), "r"(c0), "r"(c1), "l"(policy)
     : "memory");
 }
 __device__ __forceinline__ void tma_store_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
-// all committed bulk stores of this thread have finished READING shared memory
-__device__ __forceinline__ void tma_store_wait_read() { asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory"); }
-// all but the most recent committed bulk store have finished reading shared memory
-__device__ __forceinline__ void tma_store_wait_read1() { asm volatile("cp.async.bulk.wait_group.read 1;" ::: "memory"); }
+// all but the N most recent committed bulk-store groups of this thread have finished READING shared memory
+template <int N>
+__device__ __forceinline__ void tma_store_wait_read() { asm volatile("cp.async.bulk.wait_group.read %0;" ::"n"(N) : "memory"); }
+// every committed bulk-store group of this thread has completed (writes included)
 __device__ __forceinline__ void tma_store_wait_all() { asm volatile("cp.async.bulk.wait_group 0;" ::: "memory"); }
 
 __device__ __forceinline__ uint64_t policy_evict_last()
@@ -221,11 +202,9 @@ __device__ __forceinline__ uint64_t gmma_desc_sw64(uint32_t smem_addr)
 }
 
 // ------------------------------------------------------------------ misc
-__device__ __forceinline__ void st_global_cs_v4(float* p, float4 v)
+__device__ __forceinline__ void st_shared_v2(uint32_t addr, float a, float b)
 {
-  asm volatile("st.global.cs.v4.f32 [%0], {%1, %2, %3, %4};" ::"l"(p), "f"(v.x), "f"(v.y), "f"(v.z),
-               "f"(v.w)
-               : "memory");
+  asm volatile("st.shared.v2.f32 [%0], {%1, %2};" ::"r"(addr), "f"(a), "f"(b) : "memory");
 }
 __device__ __forceinline__ void st_global_cs_v2(float* p, float a, float b)
 {
