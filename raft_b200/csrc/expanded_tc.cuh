@@ -25,7 +25,8 @@
 // 64 x 128 warpgroup tile are 128 fp32 registers per thread.
 //
 //  kResident (k <= 128): the y block (all of K, <= 128 KB) stays in shared memory for the whole run;
-//    x k-blocks stream through a ring of 16 KB stages.
+//    x k-blocks stream through a ring of 16 KB stages, loaded once per tile: both halves read them, the
+//    last half releases them (the ring holds a whole tile, so it wraps across tiles when nkb < stages).
 //  !kResident (k > 128): both operands stream per k-block (stages of 16 KB of x + 16 KB of the y half).
 //
 // Epilogues (straight from the registers; d = acc * c + (t_x[i] + t_y[j]), c one scalar):
@@ -145,6 +146,7 @@ struct TcCarve {
   static constexpr size_t tb_off  = kEpi == EPI_STORE ? stg_off + 2 * (size_t)TC_STG_BOXES * TC_D_BOX_BYTES : TC_SMEM_OPERANDS;
   static constexpr size_t bytes   = tb_off + TC_BN * 4 + 256;
   static_assert(stages <= TC_MAX_STAGES, "barrier arrays hold TC_MAX_STAGES stages");
+  static_assert(!kResident || stages >= TC_MAX_RES_KB, "resident: the ring holds every x k-block of a tile (both halves read them)");
   static_assert(stg_off % 1024 == 0, "SWIZZLE_128B staging boxes need 1024-byte alignment");
   static_assert(kEpi == EPI_STORE || stg_off <= TC_SMEM_OPERANDS, "operands fit");
   static_assert(bytes <= 232448, "exceeds the 227 KB per-CTA limit");
@@ -440,8 +442,10 @@ expanded_tc_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_cons
       const int mt0   = ch * p.chunk;
       const int mt1   = min(mt0 + p.chunk, p.tiles_m);
       const int nh    = static_cast<int64_t>(n_blk) * TC_BN + TC_HN < p.n ? 2 : 1;  // halves of the y block inside the matrix
+      // resident: one load of an x k-block serves both halves of the tile; streaming: every stage carries its y half
+      const int nh_load = kResident ? 1 : nh;
       for (int mt = mt0; mt < mt1; ++mt) {
-        for (int h = 0; h < nh; ++h) {
+        for (int h = 0; h < nh_load; ++h) {
           for (int kb = 0; kb < nkb; ++kb, ++a_it) {
             if (kResident && mt == mt0 && h == 0) {
               ptx::mbar_wait(&bempty[kb], (it_local & 1) ^ 1);
@@ -527,10 +531,15 @@ expanded_tc_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_cons
 #pragma unroll
           for (int c = 0; c < 64; ++c) crs[c] = 0.f;
         }
+        // Resident: both halves read the tile's nkb x stages (a_it counts (tile, kb)), and only the last half hands
+        // them back.  In an earlier half the stage's phase cannot advance, so waiting on it again returns at once.
+        const bool release = !kResident || h == nh - 1;
+        const uint32_t it0 = a_it;
         // descriptor start-address units are 16 B; inside the 128-B swizzled row of a k-block:
         //   hi k[0,16) +0, hi k[16,32) +2, lo k[0,16) +4, lo k[16,32) +6
-        for (int kb = 0; kb < nkb; ++kb, ++a_it) {
-          const uint32_t s = a_it % kStages, ph = (a_it / kStages) & 1;
+        for (int kb = 0; kb < nkb; ++kb) {
+          const uint32_t it = it0 + kb;
+          const uint32_t s = it % kStages, ph = (it / kStages) & 1;
           if (kResident && mt == mt0 && h == 0) ptx::mbar_wait(&bfull[kb], it_local & 1);
           ptx::mbar_wait(&afull[s], ph);
           const uint64_t da = ptx::gmma_desc_sw128(ptx::smem_u32(a_base + s * kStageBytes) + wg * 64 * 128);
@@ -551,18 +560,21 @@ expanded_tc_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_cons
           ptx::wgmma_commit();
           ptx::fence_regs(acc);
           ptx::fence_regs(crs);
-          if (kb > 0) {  // the previous k-block's MMAs have finished reading their stage: hand it back
+          if (release && kb > 0) {  // the previous k-block's MMAs have finished reading their stage: hand it back
             ptx::wgmma_wait<1>();
-            if (lead) ptx::mbar_arrive(&aempty[(a_it - 1) % kStages]);
+            if (lead) ptx::mbar_arrive(&aempty[(it - 1) % kStages]);
           }
         }
         ptx::wgmma_wait<0>();
         ptx::fence_regs(acc);
         ptx::fence_regs(crs);
-        if (lead) {
-          ptx::mbar_arrive(&aempty[(a_it - 1) % kStages]);
-          if (kResident && mt == mt1 - 1 && h == nh - 1)
-            for (int kb = 0; kb < nkb; ++kb) ptx::mbar_arrive(&bempty[kb]);
+        if (release) {
+          a_it = it0 + nkb;
+          if (lead) {
+            ptx::mbar_arrive(&aempty[(a_it - 1) % kStages]);
+            if (kResident && mt == mt1 - 1 && h == nh - 1)   // the item's last MMAs on the y block are done
+              for (int kb = 0; kb < nkb; ++kb) ptx::mbar_arrive(&bempty[kb]);
+          }
         }
 #pragma unroll
         for (int c = 0; c < 64; ++c) acc[c] += crs[c];
