@@ -69,6 +69,19 @@ auto make_device_strided_matrix_view(T* p, IdxT rows, IdxT cols, IdxT ld)
     p, typename layout_stride::template mapping<matrix_extent<IdxT>>{matrix_extent<IdxT>{rows, cols}, strides}};
 }
 
+// device_vector_view<T, IdxT, Layout>: a 1-d cuda::std::mdspan (device_mdspan.hpp, make_device_vector_view)
+using layout_c_contiguous = row_major;
+template <typename IndexType>
+using vector_extent = cuda::std::extents<IndexType, dynamic_extent>;
+template <typename T, typename IdxT = std::uint32_t, typename Layout = row_major>
+using device_vector_view = cuda::std::mdspan<T, vector_extent<IdxT>, Layout>;
+
+template <typename T, typename IdxT = std::uint32_t>
+auto constexpr make_device_vector_view(T* p, IdxT n)
+{
+  return device_vector_view<T, IdxT>{p, vector_extent<IdxT>{n}};
+}
+
 template <typename K, typename V>
 struct KeyValuePair {
   K key;

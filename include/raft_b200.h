@@ -126,6 +126,21 @@ int b2d_fused_distance_nn(void* stream, b2d_kvp_if* out, int metric, const float
                           const float* y, int64_t ldy, const float* xn, const float* yn, int64_t m,
                           int64_t n, int64_t k, int init_out, void* workspace, size_t workspace_bytes);
 
+/* raft::distance::masked_l2_nn: b2d_fused_l2_nn restricted by a row x group adjacency mask.  Group g holds the rows
+ * [group_idxs[g-1], group_idxs[g]) of y (group_idxs[-1] = 0: group_idxs is the inclusive scan of the group sizes);
+ * rows at or after group_idxs[num_groups-1] are in no group.  adj [m][num_groups] bytes, row pitch ld_adj >= num_groups,
+ * nonzero = adjacent (a C++ bool array qualifies).  out[i] = {argmin_j, min_j} ||x_i - y_j||^2 (do_sqrt: Euclidean)
+ * over the rows j whose group is adjacent to row i, ties to the smaller j; a row without any such j gets
+ * {0x7fffffff, FLT_MAX} (init_out == 0: the caller's value stays).  Always the exact arg-min kernel, which skips the
+ * MMAs of tiles the mask rules out.  group_idxs must be non-decreasing and inside [0, n]; this is checked on the device
+ * without a synchronisation: when it fails, every row of out becomes {0x7fffffff, NaN}.  xn / yn: optional squared row
+ * norms.  m, n, num_groups < 2^31. */
+size_t b2d_masked_l2_nn_workspace_bytes(int64_t m, int64_t n, int64_t k, int64_t num_groups);
+int b2d_masked_l2_nn(void* stream, b2d_kvp_if* out, const float* x, int64_t ldx, const float* y, int64_t ldy,
+                     const float* xn, const float* yn, const uint8_t* adj, int64_t ld_adj, const int32_t* group_idxs,
+                     int64_t num_groups, int64_t m, int64_t n, int64_t k, int do_sqrt, int init_out, void* workspace,
+                     size_t workspace_bytes);
+
 /* Multi-GPU building blocks.  keys[i] = (order-preserving bits of ||x_i - y_j||^2 << 32)
  * | (j + idx_offset), reduced with signed 64-bit MIN: over this GPU's y shard here, then across
  * GPUs by the caller's all-reduce(INT64, MIN).  init_keys != 0 resets keys to +max first;

@@ -15,7 +15,7 @@ SYMBOLS = [
     "b2d_fused_l2_nn_finalize", "b2d_row_norm", "b2d_knn_l2_workspace_bytes", "b2d_knn_l2", "b2d_knn",
     "b2d_silhouette_score_workspace_bytes", "b2d_silhouette_score",
     "b2d_trustworthiness_score_workspace_bytes", "b2d_trustworthiness_score", "b2d_profile_begin", "b2d_profile_end",
-    "b2d_row_argmin", "b2d_fused_l2_nn_multi",
+    "b2d_row_argmin", "b2d_fused_l2_nn_multi", "b2d_masked_l2_nn_workspace_bytes", "b2d_masked_l2_nn",
 ]
 
 B2D_OK, B2D_ERR_INVALID_ARG, B2D_ERR_CUDA, B2D_ERR_UNSUPPORTED, B2D_ERR_WORKSPACE = range(5)
@@ -61,6 +61,10 @@ def lib() -> ctypes.CDLL:
     L.b2d_fused_l2_nn.argtypes = [vp, vp, vp, i64, vp, i64, vp, vp, i64, i64, i64, ci, ci, vp, sz]
     L.b2d_fused_distance_nn.restype = ci
     L.b2d_fused_distance_nn.argtypes = [vp, vp, ci, vp, i64, vp, i64, vp, vp, i64, i64, i64, ci, vp, sz]
+    L.b2d_masked_l2_nn_workspace_bytes.restype = sz
+    L.b2d_masked_l2_nn_workspace_bytes.argtypes = [i64, i64, i64, i64]
+    L.b2d_masked_l2_nn.restype = ci
+    L.b2d_masked_l2_nn.argtypes = [vp, vp, vp, i64, vp, i64, vp, vp, vp, i64, vp, i64, i64, i64, i64, ci, ci, vp, sz]
     L.b2d_fused_l2_nn_keys.restype = ci
     L.b2d_fused_l2_nn_keys.argtypes = [vp, vp, vp, i64, vp, i64, vp, vp, i64, i64, i64, i64, ci, vp, sz]
     L.b2d_fused_l2_nn_finalize.restype = ci

@@ -14,6 +14,7 @@
 
 #include "../../include/raft_b200.h"
 #include "expanded_tc.cuh"
+#include "masked_nn.cuh"
 #include "screen_tc.cuh"
 #include "prep.cuh"
 #include "unexpanded_simt.cuh"
@@ -268,6 +269,7 @@ static int launch_tc_epi(cudaStream_t s, const CUtensorMap& ma, const CUtensorMa
                          const TcParams& p, int grid, int epi, int post)
 {
   if (epi == EPI_MINLOC) return launch_tc_inst<kRes, EPI_MINLOC, POST_NONE>(s, ma, mb, md, p, grid);
+  if (epi == EPI_MINLOC_MASKED) return launch_tc_inst<kRes, EPI_MINLOC_MASKED, POST_NONE>(s, ma, mb, md, p, grid);
   if (epi == EPI_TOPK) return launch_tc_inst<kRes, EPI_TOPK, POST_NONE>(s, ma, mb, md, p, grid);
   if (post == POST_NONE) return launch_tc_inst<kRes, EPI_STORE, POST_NONE>(s, ma, mb, md, p, grid);
   if (post == POST_CLAMP) return launch_tc_inst<kRes, EPI_STORE, POST_CLAMP>(s, ma, mb, md, p, grid);
@@ -1007,6 +1009,98 @@ int b2d_fused_distance_nn(void* stream, b2d_kvp_if* out, int metric, const float
   if (rc) return rc;
   minloc_finalize_kernel<<<static_cast<unsigned>((m + 255) / 256), 256, 0, s>>>(
     reinterpret_cast<KvpIF*>(out), w.keys, m, 0, init_out ? 0 : 1);
+  B2D_CUDA(cudaGetLastError());
+  return B2D_OK;
+}
+
+// ------------------------------------------------------------------------------------------
+// Masked fusedL2NN (masked_nn.cuh): the operands of the tensor-core path (without the screened search's scratch), then
+// the keys and the mask's device tables
+namespace {
+struct MaskedLayout {
+  TcWorkspace w;      // w.keys: [m]
+  unsigned* bad;      // [1] group_idxs is invalid
+  int* grp;           // [n] group of every row of y
+  unsigned* bits;     // [ceil(m/32)][G] adjacency bits
+  uint8_t* cls;       // [tiles_n][tiles_m] tile classes
+  size_t bytes;
+};
+}  // namespace
+
+static MaskedLayout masked_layout(void* base, int64_t m, int64_t n, int64_t k, int64_t G)
+{
+  MaskedLayout L;
+  L.w        = tc_layout(base, m, n, k, false);
+  size_t off = L.w.bytes;
+  auto take  = [&](size_t b) {
+    size_t o = off;
+    off += align_up(b, 1024);
+    return o;
+  };
+  char* c   = static_cast<char*>(base);
+  L.w.keys  = reinterpret_cast<long long*>(c + take(static_cast<size_t>(m) * 8));
+  L.bad     = reinterpret_cast<unsigned*>(c + take(32));
+  L.grp     = reinterpret_cast<int*>(c + take(static_cast<size_t>(n) * 4));
+  L.bits    = reinterpret_cast<unsigned*>(c + take(static_cast<size_t>((m + 31) / 32) * G * 4));
+  L.cls     = reinterpret_cast<uint8_t*>(c + take(static_cast<size_t>((m + TC_BM - 1) / TC_BM) * ((n + TC_BN - 1) / TC_BN)));
+  L.bytes   = off;
+  return L;
+}
+
+size_t b2d_masked_l2_nn_workspace_bytes(int64_t m, int64_t n, int64_t k, int64_t num_groups)
+{
+  if (m < 0 || n < 0 || k < 0 || num_groups < 0) return static_cast<size_t>(-1);
+  return masked_layout(nullptr, m, n, k, num_groups).bytes;
+}
+
+int b2d_masked_l2_nn(void* stream, b2d_kvp_if* out, const float* x, int64_t ldx, const float* y, int64_t ldy,
+                     const float* xn, const float* yn, const uint8_t* adj, int64_t ld_adj, const int32_t* group_idxs,
+                     int64_t num_groups, int64_t m, int64_t n, int64_t k, int do_sqrt, int init_out, void* workspace,
+                     size_t workspace_bytes)
+{
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  const int64_t G = num_groups;
+  if (m < 0 || n < 0 || k < 0 || G < 0) return fail(B2D_ERR_INVALID_ARG, "negative extent");
+  if (m == 0) return B2D_OK;
+  if (k == 0) return fail(B2D_ERR_INVALID_ARG, "k must be positive");
+  if (!out || !x || (n > 0 && !y)) return fail(B2D_ERR_INVALID_ARG, "null out / x / y");
+  if (G > 0 && (!adj || !group_idxs)) return fail(B2D_ERR_INVALID_ARG, "null adj / group_idxs");
+  if (ld_adj < G) return fail(B2D_ERR_INVALID_ARG, "ld_adj smaller than num_groups");
+  if (ldx < k || ldy < k) return fail(B2D_ERR_INVALID_ARG, "leading dimension smaller than k");
+  if (m > 0x7fffffffll || n > 0x7fffffffll || G > 0x7fffffffll) return fail(B2D_ERR_INVALID_ARG, "index range exceeds 32 bits");
+  const size_t need = masked_layout(nullptr, m, n, k, G).bytes;
+  if (!workspace || workspace_bytes < need)
+    return fail(B2D_ERR_WORKSPACE, "workspace too small: need " + std::to_string(need) + " bytes");
+  if (reinterpret_cast<uintptr_t>(workspace) % 256) return fail(B2D_ERR_INVALID_ARG, "workspace must be 256-byte aligned");
+  MaskedLayout L = masked_layout(workspace, m, n, k, G);
+  const unsigned mblocks = static_cast<unsigned>((m + 255) / 256);
+  minloc_init_kernel<<<mblocks, 256, 0, s>>>(L.w.keys, m);
+  B2D_CUDA(cudaGetLastError());
+  masked_validate_kernel<<<1, 1024, 0, s>>>(L.bad, group_idxs, G, n);
+  B2D_CUDA(cudaGetLastError());
+  if (n > 0 && G > 0) {
+    int rc = launch_prep<float>(s, L.w, x, ldx, 1, m, y, ldy, 1, n, k, xn, yn, PREP_L2, 0);
+    if (rc) return rc;
+    masked_group_map_kernel<<<static_cast<unsigned>((n + 255) / 256), 256, 0, s>>>(L.grp, group_idxs, G, n);
+    B2D_CUDA(cudaGetLastError());
+    masked_adj_bits_kernel<<<static_cast<unsigned>((m + 31) / 32), 256, 0, s>>>(L.bits, adj, ld_adj, m, G);
+    B2D_CUDA(cudaGetLastError());
+    const int tiles_m = static_cast<int>((m + TC_BM - 1) / TC_BM), tiles_n = static_cast<int>((n + TC_BN - 1) / TC_BN);
+    const int64_t ntiles = static_cast<int64_t>(tiles_m) * tiles_n;
+    masked_classify_kernel<<<static_cast<unsigned>((ntiles + 255) / 256), 256, 0, s>>>(L.cls, L.bits, group_idxs, G, m, n,
+                                                                                       tiles_m, tiles_n, L.bad);
+    B2D_CUDA(cudaGetLastError());
+    TcParams p;
+    memset(&p, 0, sizeof(p));
+    p.m = m; p.n = n; p.keys = L.w.keys;
+    p.mask_cls = L.cls; p.mask_grp = L.grp; p.mask_bits = L.bits; p.mask_groups = G;
+    ProfileScope prof(s);
+    rc = launch_tc(s, L.w, p, k, EPI_MINLOC_MASKED, POST_NONE);
+    if (rc) return rc;
+  }
+  minloc_finalize_kernel<<<mblocks, 256, 0, s>>>(reinterpret_cast<KvpIF*>(out), L.w.keys, m, do_sqrt, init_out ? 0 : 1);
+  B2D_CUDA(cudaGetLastError());
+  masked_poison_kernel<<<mblocks, 256, 0, s>>>(reinterpret_cast<KvpIF*>(out), L.bad, m);
   B2D_CUDA(cudaGetLastError());
   return B2D_OK;
 }

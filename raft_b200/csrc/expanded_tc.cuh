@@ -40,6 +40,8 @@
 //                     the row's current global best (read from keys at tile start: an upper bound, keys
 //                     only decrease); only a candidate that can change the result takes the slow path
 //                     (smallest-column scan + packed 64-bit atomicMin).
+//   EPI_MINLOC_MASKED EPI_MINLOC under a row x group adjacency mask (masked_nn.cuh): tiles the mask rules out are not
+//                     loaded or multiplied, partly adjacent ones set the non-adjacent values to +inf first.
 //   EPI_TOPK          fused brute-force kNN: the same minimum and vote against the row's current k-th best;
 //                     every pair at or below it is appended to the row's candidate list (see the kNN
 //                     helpers at the end of this file).
@@ -72,7 +74,15 @@ constexpr int TC_D_BOX_ROWS  = 64;
 constexpr int TC_D_BOX_BYTES = TC_D_BOX_COLS * TC_D_BOX_ROWS * 4;
 constexpr int TC_STG_BOXES   = 2;
 
-enum TcEpilogue : int { EPI_STORE = 0, EPI_MINLOC = 1, EPI_TOPK = 2 };
+enum TcEpilogue : int { EPI_STORE = 0, EPI_MINLOC = 1, EPI_TOPK = 2, EPI_MINLOC_MASKED = 3 };
+
+// EPI_MINLOC_MASKED (masked_nn.cuh): class of one (64-row slab of x, 128-column half of a y block) tile.  Byte
+// TcParams::mask_cls[n_blk][mt] holds the four classes of an (x tile, y block) pair, 2 bits each at bit 2 (2 h + s)
+// for slab s (= consumer warpgroup) and half h.  A byte of 0 is a tile with nothing to do.
+enum MaskClass : int { MASK_NONE = 0, MASK_ALL = 1, MASK_PARTIAL = 2 };
+__host__ __device__ __forceinline__ int mask_class_of(unsigned cls_byte, int h, int s) { return (cls_byte >> (2 * (2 * h + s))) & 3; }
+// some slab of half h is live: the streaming variant loads the half's stages
+__host__ __device__ __forceinline__ bool mask_half_live(unsigned cls_byte, int h) { return ((cls_byte >> (4 * h)) & 15u) != 0u; }
 // max(v, 0) that keeps a NaN (fmaxf(NaN, 0) = 0 would turn a poisoned distance into a perfect match)
 __device__ __forceinline__ float clamp0(float v)
 {
@@ -128,6 +138,11 @@ struct TcParams {
   unsigned knn_cap;
   long long* knn_dropmin; // [m] smallest key that did not fit into the row's list this pass (knn_merge_kernel decides whether
                           //     anything that matters was lost; rows where it was are redone by knn_fix_kernel)
+  // EPI_MINLOC_MASKED (masked_nn.cuh): only pairs whose row of x is adjacent to the group of the row of y are candidates
+  const uint8_t* mask_cls;    // [tiles_n][tiles_m] tile classes (MaskClass, see mask_class_of)
+  const int* mask_grp;        // [n] group of every row of y (-1: in no group)
+  const unsigned* mask_bits;  // [ceil(m/32)][mask_groups] bit i % 32 of word (i / 32, g): row i of x is adjacent to group g
+  int64_t mask_groups;
 };
 
 constexpr size_t TC_SMEM_OPERANDS = (size_t)TC_MAX_RES_KB * TC_B_BYTES + (size_t)TC_STAGES_RES * TC_A_BYTES;  // 208 KB
@@ -144,7 +159,8 @@ struct TcCarve {
   static constexpr size_t a_off   = kResident ? (size_t)TC_MAX_RES_KB * TC_B_BYTES : 0;
   static constexpr size_t stg_off = a_off + (size_t)stages * stage_bytes;
   static constexpr size_t tb_off  = kEpi == EPI_STORE ? stg_off + 2 * (size_t)TC_STG_BOXES * TC_D_BOX_BYTES : TC_SMEM_OPERANDS;
-  static constexpr size_t bytes   = tb_off + TC_BN * 4 + 256;
+  static constexpr size_t grp_off = tb_off + TC_BN * 4 + 256;   // EPI_MINLOC_MASKED: [256] group of every column
+  static constexpr size_t bytes   = grp_off + (kEpi == EPI_MINLOC_MASKED ? TC_BN * 4 : 0);
   static_assert(stages <= TC_MAX_STAGES, "barrier arrays hold TC_MAX_STAGES stages");
   static_assert(!kResident || stages >= TC_MAX_RES_KB, "resident: the ring holds every x k-block of a tile (both halves read them)");
   static_assert(stg_off % 1024 == 0, "SWIZZLE_128B staging boxes need 1024-byte alignment");
@@ -201,13 +217,38 @@ __device__ __noinline__ void knn_append16(unsigned* cnt, long long* cand, unsign
   }
 }
 
+// EPI_MINLOC_MASKED, PARTIAL tiles: bit 4i + 2j + e of the result is set when row row0 + 8j of x is adjacent to the group
+// of column cl0 + 8i + e of the y block (col_grp: the block's column groups in shared memory).  Not inlined, for the
+// same reason as knn_append16.
+__device__ __noinline__ unsigned long long masked_keep64(const int* col_grp, int cl0, const unsigned* bits, int64_t groups,
+                                                         int64_t row0, int64_t m)
+{
+  unsigned long long keep = 0ull;
+#pragma unroll
+  for (int j = 0; j < 2; ++j) {
+    const int64_t r = row0 + 8 * j;
+    if (r >= m) continue;
+    const unsigned* word = bits + (r >> 5) * groups;
+    const int sh         = static_cast<int>(r & 31);
+#pragma unroll
+    for (int i = 0; i < 16; ++i)
+#pragma unroll
+      for (int e = 0; e < 2; ++e) {
+        const int g = col_grp[cl0 + 8 * i + e];
+        if (g >= 0 && ((__ldg(&word[g]) >> sh) & 1u)) keep |= 1ull << (4 * i + 2 * j + e);
+      }
+  }
+  return keep;
+}
+
 // Epilogue of one 64 x 128 warpgroup tile.  v[4i + 2j + e] holds row row0 + 8j, column gc0 + 8i + e of the accumulator
 // (main + cross already summed); on return (EPI_STORE) v holds the finished distances, and they have been written
-// unless p.tma_store (then tc_stage_store writes them).
+// unless p.tma_store (then tc_stage_store writes them).  EPI_MINLOC_MASKED: the values whose bit in `keep` is clear
+// become +inf (never a candidate) before the minimum.
 template <int kEpi, int kPost>
 __device__ __forceinline__ void tc_epilogue(float (&v)[64], const TcParams& p, const float* col_tb, int cl0, int64_t gc0,
                                             int64_t row0, const float (&ta)[2], const float (&cfr)[2], float (&thr)[2],
-                                            const float (&xnr)[2], bool ynu)
+                                            const float (&xnr)[2], bool ynu, unsigned long long keep = ~0ull)
 {
   // d = acc * c_row (* column factor) + (t_x + t_y); the arg-min modes leave the row-constant t_x out (added on the
   // slow path only)
@@ -299,6 +340,11 @@ __device__ __forceinline__ void tc_epilogue(float (&v)[64], const TcParams& p, c
   // scan) and let the packed 64-bit atomicMin decide -- (value, index) order == raft::argmin_op
   // (cpp/include/raft/core/operators.hpp:187-194).  After the first few y blocks this is rare.
   const float inf = __int_as_float(0x7f800000);
+  if (kEpi == EPI_MINLOC_MASKED && keep != ~0ull) {
+#pragma unroll
+    for (int c = 0; c < 64; ++c)
+      if (!((keep >> c) & 1ull)) v[c] = inf;
+  }
 #pragma unroll
   for (int cc = 0; cc < 2; ++cc) {
 #pragma unroll
@@ -316,7 +362,7 @@ __device__ __forceinline__ void tc_epilogue(float (&v)[64], const TcParams& p, c
       const bool cand = (mn + xnr[j]) <= thr[j] && mn < inf;
       if (__any_sync(0xffffffffu, cand) && cand) {
         const int64_t gcc = gc0 + 64 * cc;   // global column of v[b]
-        if (kEpi == EPI_MINLOC) {
+        if (kEpi != EPI_TOPK) {
           int cbest = 0;
 #pragma unroll
           for (int i = 7; i >= 0; --i) {
@@ -398,6 +444,8 @@ expanded_tc_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_cons
   using Carve                    = TcCarve<kResident, kEpi>;
   constexpr int kStages          = Carve::stages;
   constexpr uint32_t kStageBytes = Carve::stage_bytes;
+  constexpr bool kMasked         = kEpi == EPI_MINLOC_MASKED;
+  constexpr bool kMinloc         = kEpi == EPI_MINLOC || kMasked;
   if (p.run_flag != nullptr && __ldg(p.run_flag) == 0u) return;  // conditional launch (no host round trip)
   extern __shared__ __align__(1024) uint8_t smem[];
   // SWIZZLE_128B atoms need 1024-byte alignment; the dynamic window starts 1024-aligned (no static
@@ -406,6 +454,7 @@ expanded_tc_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_cons
   uint8_t* b_base = smem;  // resident: [nkb] k-blocks of the y block
   uint8_t* a_base = smem + Carve::a_off;  // stages: x k-block (+ y half k-block)
   float* col_tb   = reinterpret_cast<float*>(smem + Carve::tb_off);  // [256] t_y of this y block
+  int* col_grp    = reinterpret_cast<int*>(smem + Carve::grp_off);  // masked: [256] group of every column of the y block
   uint64_t* bars  = reinterpret_cast<uint64_t*>(col_tb + TC_BN);
   uint64_t* afull = bars;                       // [TC_MAX_STAGES]
   uint64_t* aempty = bars + TC_MAX_STAGES;      // [TC_MAX_STAGES]
@@ -436,34 +485,79 @@ expanded_tc_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_cons
     // `if (lane == 0)` the compiler cannot keep descriptors / barrier addresses in uniform registers).
     const uint64_t pol = ptx::policy_evict_last();
     uint32_t a_it = 0, it_local = 0;
-    for (int64_t item = blockIdx.x; item < p.n_items; item += gridDim.x, ++it_local) {
-      const int n_blk = sel_to_blk(static_cast<int>(item % p.tiles_sel), p.sel_s, p.sel_lo, p.sel_hi);
-      const int ch    = static_cast<int>(item / p.tiles_sel);
-      const int mt0   = ch * p.chunk;
-      const int mt1   = min(mt0 + p.chunk, p.tiles_m);
-      const int nh    = static_cast<int64_t>(n_blk) * TC_BN + TC_HN < p.n ? 2 : 1;  // halves of the y block inside the matrix
-      // resident: one load of an x k-block serves both halves of the tile; streaming: every stage carries its y half
-      const int nh_load = kResident ? 1 : nh;
-      for (int mt = mt0; mt < mt1; ++mt) {
-        for (int h = 0; h < nh_load; ++h) {
-          for (int kb = 0; kb < nkb; ++kb, ++a_it) {
-            if (kResident && mt == mt0 && h == 0) {
-              ptx::mbar_wait(&bempty[kb], (it_local & 1) ^ 1);
-              if (ptx::elect_one()) {
-                ptx::mbar_expect_tx(&bfull[kb], TC_B_BYTES);
-                ptx::tma_load_2d(b_base + kb * TC_B_BYTES, &tmap_b, &bfull[kb], kb * 64, n_blk * TC_BN, pol);
+    if constexpr (kEpi == EPI_MINLOC_MASKED) {
+      // Masked: the same loads, minus those of dead tiles (DESIGN.md section 2 K3m, skip invariants).  A tile whose class
+      // byte is 0 loads nothing; in the streaming variant a half no slab needs loads nothing; an item without a live
+      // tile loads no y block and does not count in it_local (the bfull / bempty parity).  Apart from these skips the
+      // loop is the unmasked one below (kept apart so that the other instantiations compile as before): a change to
+      // either loop belongs in both.
+      for (int64_t item = blockIdx.x; item < p.n_items; item += gridDim.x) {
+        const int n_blk = sel_to_blk(static_cast<int>(item % p.tiles_sel), p.sel_s, p.sel_lo, p.sel_hi);
+        const int ch    = static_cast<int>(item / p.tiles_sel);
+        const int mt0   = ch * p.chunk;
+        const int mt1   = min(mt0 + p.chunk, p.tiles_m);
+        const int nh    = static_cast<int64_t>(n_blk) * TC_BN + TC_HN < p.n ? 2 : 1;
+        const uint8_t* cls = p.mask_cls + static_cast<int64_t>(n_blk) * p.tiles_m;
+        bool b_loaded = false;
+        for (int mt = mt0; mt < mt1; ++mt) {
+          const unsigned tcls = __ldg(&cls[mt]);
+          if (tcls == 0u) continue;
+          for (int h = 0; h < (kResident ? 1 : nh); ++h) {
+            if (!kResident && !mask_half_live(tcls, h)) continue;
+            for (int kb = 0; kb < nkb; ++kb, ++a_it) {
+              if (kResident && !b_loaded) {
+                ptx::mbar_wait(&bempty[kb], (it_local & 1) ^ 1);
+                if (ptx::elect_one()) {
+                  ptx::mbar_expect_tx(&bfull[kb], TC_B_BYTES);
+                  ptx::tma_load_2d(b_base + kb * TC_B_BYTES, &tmap_b, &bfull[kb], kb * 64, n_blk * TC_BN, pol);
+                }
               }
+              const uint32_t s = a_it % kStages, ph = (a_it / kStages) & 1;
+              ptx::mbar_wait(&aempty[s], ph ^ 1);
+              if (ptx::elect_one()) {
+                ptx::mbar_expect_tx(&afull[s], kStageBytes);
+                ptx::tma_load_2d(a_base + s * kStageBytes, &tmap_a, &afull[s], kb * 64, mt * TC_BM, pol);
+                if (!kResident)
+                  ptx::tma_load_2d(a_base + s * kStageBytes + TC_A_BYTES, &tmap_b, &afull[s], kb * 64,
+                                   n_blk * TC_BN + h * TC_HN, pol);
+              }
+              __syncwarp();
             }
-            const uint32_t s = a_it % kStages, ph = (a_it / kStages) & 1;
-            ptx::mbar_wait(&aempty[s], ph ^ 1);
-            if (ptx::elect_one()) {
-              ptx::mbar_expect_tx(&afull[s], kStageBytes);
-              ptx::tma_load_2d(a_base + s * kStageBytes, &tmap_a, &afull[s], kb * 64, mt * TC_BM, pol);
-              if (!kResident)
-                ptx::tma_load_2d(a_base + s * kStageBytes + TC_A_BYTES, &tmap_b, &afull[s], kb * 64,
-                                 n_blk * TC_BN + h * TC_HN, pol);
+            b_loaded = true;
+          }
+        }
+        if (b_loaded) ++it_local;
+      }
+    } else {   // (mirrored, with the skips, by the masked loop above)
+      for (int64_t item = blockIdx.x; item < p.n_items; item += gridDim.x, ++it_local) {
+        const int n_blk = sel_to_blk(static_cast<int>(item % p.tiles_sel), p.sel_s, p.sel_lo, p.sel_hi);
+        const int ch    = static_cast<int>(item / p.tiles_sel);
+        const int mt0   = ch * p.chunk;
+        const int mt1   = min(mt0 + p.chunk, p.tiles_m);
+        const int nh    = static_cast<int64_t>(n_blk) * TC_BN + TC_HN < p.n ? 2 : 1;  // halves of the y block inside the matrix
+        // resident: one load of an x k-block serves both halves of the tile; streaming: every stage carries its y half
+        const int nh_load = kResident ? 1 : nh;
+        for (int mt = mt0; mt < mt1; ++mt) {
+          for (int h = 0; h < nh_load; ++h) {
+            for (int kb = 0; kb < nkb; ++kb, ++a_it) {
+              if (kResident && mt == mt0 && h == 0) {
+                ptx::mbar_wait(&bempty[kb], (it_local & 1) ^ 1);
+                if (ptx::elect_one()) {
+                  ptx::mbar_expect_tx(&bfull[kb], TC_B_BYTES);
+                  ptx::tma_load_2d(b_base + kb * TC_B_BYTES, &tmap_b, &bfull[kb], kb * 64, n_blk * TC_BN, pol);
+                }
+              }
+              const uint32_t s = a_it % kStages, ph = (a_it / kStages) & 1;
+              ptx::mbar_wait(&aempty[s], ph ^ 1);
+              if (ptx::elect_one()) {
+                ptx::mbar_expect_tx(&afull[s], kStageBytes);
+                ptx::tma_load_2d(a_base + s * kStageBytes, &tmap_a, &afull[s], kb * 64, mt * TC_BM, pol);
+                if (!kResident)
+                  ptx::tma_load_2d(a_base + s * kStageBytes + TC_A_BYTES, &tmap_b, &afull[s], kb * 64,
+                                   n_blk * TC_BN + h * TC_HN, pol);
+              }
+              __syncwarp();
             }
-            __syncwarp();
           }
         }
       }
@@ -491,6 +585,18 @@ expanded_tc_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_cons
     const int mt0   = ch * p.chunk;
     const int mt1   = min(mt0 + p.chunk, p.tiles_m);
     const int nh    = static_cast<int64_t>(n_blk) * TC_BN + TC_HN < p.n ? 2 : 1;
+    // masked: the item's last loaded tile (its y block is handed back after it); no loaded tile: the producer skipped
+    // the item, and it does not count in it_local
+    int mt_last = mt1 - 1;
+    const uint8_t* cls = nullptr;
+    if constexpr (kMasked) {
+      cls     = p.mask_cls + static_cast<int64_t>(n_blk) * p.tiles_m;
+      mt_last = -1;
+      for (int mt = mt0; mt < mt1; ++mt)
+        if (__ldg(&cls[mt]) != 0u) mt_last = mt;
+      if (mt_last < 0) { --it_local; continue; }
+    }
+    bool b_first = true;   // masked: this warpgroup has not waited for the item's y block yet
     // per-column epilogue terms of this y block (shared by every tile of the item)
     ptx::bar_sync(1, 256);
     {
@@ -499,10 +605,16 @@ expanded_tc_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_cons
       if (gj < p.n) tv = __ldg(&p.yt[gj]);
       if (kEpi == EPI_STORE && p.acc_mode >= 2) tv = 0.f;  // the t terms entered with the first K chunk
       col_tb[ct] = tv;
+      if (kMasked) col_grp[ct] = gj < p.n ? __ldg(&p.mask_grp[gj]) : -1;
     }
     ptx::bar_sync(1, 256);
 
     for (int mt = mt0; mt < mt1; ++mt) {
+      unsigned tcls = 0u;
+      if constexpr (kMasked) {
+        tcls = __ldg(&cls[mt]);
+        if (tcls == 0u) continue;   // not loaded
+      }
       // the two tile rows this thread owns: row0 and row0 + 8
       const int64_t row0 = static_cast<int64_t>(mt) * TC_BM + 64 * wg + 16 * (warp & 3) + quad;
       float ta[2], cfr[2], thr[2], xnr[2];
@@ -515,7 +627,7 @@ expanded_tc_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_cons
           if (xnu) cr *= __ldg(&p.xsc[gi]);
           if (kEpi != EPI_STORE || p.acc_mode < 2) rv = __ldg(&p.xt[gi]);
           if (kEpi == EPI_TOPK) thr[j] = __ldg(&p.knn_thr[gi]);
-          if (kEpi == EPI_MINLOC) {  // the row's current best (an upper bound: keys only decrease)
+          if (kMinloc) {  // the row's current best (an upper bound: keys only decrease)
             const long long ck = *reinterpret_cast<volatile long long*>(&p.keys[gi]);
             const int sb       = static_cast<int>(ck >> 32);
             thr[j]             = __int_as_float(sb < 0 ? (sb ^ 0x7FFFFFFF) : sb);
@@ -527,6 +639,35 @@ expanded_tc_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_cons
         cfr[j] = cr;
       }
       for (int h = 0; h < nh; ++h) {
+        int hcls = MASK_ALL;
+        if constexpr (kMasked) {
+          hcls = mask_class_of(tcls, h, wg);
+          if (hcls == MASK_NONE) {
+            // nothing of this warpgroup's slab is adjacent: no MMAs, no epilogue.  Stages the producer loaded (the
+            // tile's, resident; the half's when the other slab needs it, streaming) are still waited for and handed
+            // back by this warpgroup, and so is the y block after the item's last loaded tile.  Stage by stage, every
+            // thread waits, as in a live half, and the warpgroup meets at its named barrier before the lead hands the
+            // stage back.  Both matter: a warp that skipped the waits could run ahead to a later live tile and find a
+            // stage's barrier a whole phase behind (try_wait.parity would pass at once, on an old tile), and a warp
+            // still waiting when the lead handed the stage back could find it refilled, its barrier two phases on, and
+            // wait forever.  One stage at a time: a streamed half has more k-blocks (k > 192) than the ring has stages,
+            // so holding them all before handing any back would starve the producer.  (Barrier 2 + wg is free here:
+            // only EPI_STORE uses it.)
+            if (!kResident && !mask_half_live(tcls, h)) continue;   // not loaded
+            if (!kResident || h == nh - 1) {
+              for (int kb = 0; kb < nkb; ++kb) {
+                const uint32_t it = a_it + kb;
+                ptx::mbar_wait(&afull[it % kStages], (it / kStages) & 1);
+                ptx::bar_sync(2 + wg, 128);
+                if (lead) ptx::mbar_arrive(&aempty[it % kStages]);
+              }
+              if (kResident && lead && mt == mt_last)
+                for (int kb = 0; kb < nkb; ++kb) ptx::mbar_arrive(&bempty[kb]);
+              a_it += nkb;
+            }
+            continue;
+          }
+        }
         if (!has_lo) {
 #pragma unroll
           for (int c = 0; c < 64; ++c) crs[c] = 0.f;
@@ -540,7 +681,8 @@ expanded_tc_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_cons
         for (int kb = 0; kb < nkb; ++kb) {
           const uint32_t it = it0 + kb;
           const uint32_t s = it % kStages, ph = (it / kStages) & 1;
-          if (kResident && mt == mt0 && h == 0) ptx::mbar_wait(&bfull[kb], it_local & 1);
+          // (the first MMAs of the item on the resident y block wait for it)
+          if (kResident && (kMasked ? b_first : (mt == mt0 && h == 0))) ptx::mbar_wait(&bfull[kb], it_local & 1);
           ptx::mbar_wait(&afull[s], ph);
           const uint64_t da = ptx::gmma_desc_sw128(ptx::smem_u32(a_base + s * kStageBytes) + wg * 64 * 128);
           const uint64_t db = ptx::gmma_desc_sw128(kResident ? ptx::smem_u32(b_base + kb * TC_B_BYTES) + h * TC_BH_BYTES
@@ -568,19 +710,22 @@ expanded_tc_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_cons
         ptx::wgmma_wait<0>();
         ptx::fence_regs(acc);
         ptx::fence_regs(crs);
+        if (kMasked) b_first = false;
         if (release) {
           a_it = it0 + nkb;
           if (lead) {
             ptx::mbar_arrive(&aempty[(a_it - 1) % kStages]);
-            if (kResident && mt == mt1 - 1 && h == nh - 1)   // the item's last MMAs on the y block are done
+            if (kResident && mt == (kMasked ? mt_last : mt1 - 1) && h == nh - 1)   // the item's last MMAs on the y block are done
               for (int kb = 0; kb < nkb; ++kb) ptx::mbar_arrive(&bempty[kb]);
           }
         }
 #pragma unroll
         for (int c = 0; c < 64; ++c) acc[c] += crs[c];
         const int cl0 = h * TC_HN + 2 * tq;  // this thread's first column inside the tile
+        unsigned long long keep = ~0ull;
+        if (kMasked && hcls == MASK_PARTIAL) keep = masked_keep64(col_grp, cl0, p.mask_bits, p.mask_groups, row0, p.m);
         tc_epilogue<kEpi, kPost>(acc, p, col_tb, cl0, static_cast<int64_t>(n_blk) * TC_BN + cl0, row0, ta, cfr, thr, xnr,
-                                 ynu);
+                                 ynu, keep);
         if (kEpi == EPI_STORE && p.tma_store)   // (this warpgroup's staging boxes: computed here, not kept live)
           tc_stage_store(acc, &tmap_d, ptx::smem_u32(smem + Carve::stg_off) + wg * TC_STG_BOXES * TC_D_BOX_BYTES, lead,
                          item + gridDim.x >= p.n_items && mt == mt1 - 1 && h == nh - 1, wg,
