@@ -85,12 +85,14 @@ static int make_operand_map(CUtensorMap* map, const void* base, int64_t rows, in
   return B2D_OK;
 }
 
-static int device_sms(int* sms, int* cc_major)
+// SM count of the current device; every kernel of the library is built for sm_90a only, so any other device is an error
+static int device_sms(int* sms)
 {
-  int dev = 0;
+  int dev = 0, cc = 0;
   B2D_CUDA(cudaGetDevice(&dev));
   B2D_CUDA(cudaDeviceGetAttribute(sms, cudaDevAttrMultiProcessorCount, dev));
-  B2D_CUDA(cudaDeviceGetAttribute(cc_major, cudaDevAttrComputeCapabilityMajor, dev));
+  B2D_CUDA(cudaDeviceGetAttribute(&cc, cudaDevAttrComputeCapabilityMajor, dev));
+  if (cc != 9) return fail(B2D_ERR_CUDA, "raft_b200 requires an sm_90 (H100) device; found cc major " + std::to_string(cc));
   return B2D_OK;
 }
 
@@ -278,26 +280,38 @@ static int launch_tc_epi(cudaStream_t s, const CUtensorMap& ma, const CUtensorMa
   return launch_tc_inst<kRes, EPI_STORE, POST_CLAMP_SQRT>(s, ma, mb, md, p, grid);
 }
 
+// Schedule of a persistent tensor-core launch (TcParams or ScreenParams, tc_item): fills tiles_m, tiles_sel, chunk,
+// chunks_m and n_items of p from m, n and the y block selection, and sets *grid to one CTA per SM (fewer if there are
+// fewer items).  The x tiles are cut into runs so that each SM gets about items_per_sm items; a run holds at most
+// max_chunk tiles.
+template <class P>
+static int plan_tc_items(P& p, int items_per_sm, int max_chunk, int* grid)
+{
+  int sms = 0;
+  const int rc = device_sms(&sms);
+  if (rc) return rc;
+  p.tiles_m         = static_cast<int>((p.m + TC_BM - 1) / TC_BM);
+  const int tiles_n = static_cast<int>((p.n + TC_BN - 1) / TC_BN);
+  p.tiles_sel       = sel_count(tiles_n, p.sel_s, p.sel_lo, p.sel_hi);
+  int64_t chunk     = static_cast<int64_t>(p.tiles_m) * p.tiles_sel / (static_cast<int64_t>(sms) * items_per_sm);
+  chunk             = std::max<int64_t>(1, std::min<int64_t>(chunk, max_chunk));
+  chunk             = std::min<int64_t>(chunk, p.tiles_m);
+  p.chunk           = static_cast<int>(chunk);
+  p.chunks_m        = (p.tiles_m + p.chunk - 1) / p.chunk;
+  p.n_items         = static_cast<int64_t>(p.tiles_sel) * p.chunks_m;
+  *grid             = static_cast<int>(p.n_items < sms ? p.n_items : sms);
+  return B2D_OK;
+}
+
 static int launch_tc(cudaStream_t s, const TcWorkspace& w, TcParams p, int64_t k, int epi, int post, int kb0 = 0,
                      int nkb_chunk = 0)
 {
-  int sms = 0, cc = 0;
-  int rc  = device_sms(&sms, &cc);
-  if (rc) return rc;
-  if (cc != 9) return fail(B2D_ERR_CUDA, "raft_b200 requires an sm_90 (H100) device; found cc major " + std::to_string(cc));
   const int nkb_total = static_cast<int>((k + 31) / 32);
   p.nkb     = nkb_chunk ? nkb_chunk : nkb_total;
-  p.tiles_m = static_cast<int>((p.m + TC_BM - 1) / TC_BM);
   p.tiles_n = static_cast<int>((p.n + TC_BN - 1) / TC_BN);
-  p.tiles_sel = sel_count(p.tiles_n, p.sel_s, p.sel_lo, p.sel_hi);
-  int64_t total = static_cast<int64_t>(p.tiles_m) * p.tiles_sel;
-  int64_t chunk = total / (static_cast<int64_t>(sms) * 6);
-  if (chunk < 1) chunk = 1;
-  if (chunk > 32) chunk = 32;
-  if (chunk > p.tiles_m) chunk = p.tiles_m;
-  p.chunk    = static_cast<int>(chunk);
-  p.chunks_m = (p.tiles_m + p.chunk - 1) / p.chunk;
-  p.n_items  = static_cast<int64_t>(p.tiles_sel) * p.chunks_m;
+  int grid  = 0;
+  int rc    = plan_tc_items(p, 6, 32, &grid);
+  if (rc) return rc;
   p.xt       = w.xt;
   p.yt       = w.yt;
   p.coef     = w.coef;
@@ -319,7 +333,6 @@ static int launch_tc(cudaStream_t s, const TcWorkspace& w, TcParams p, int64_t k
     rc = make_dist_map(&md, p.dist, p.m, p.n, p.ldd);
     if (rc) return rc;
   }
-  const int grid = static_cast<int>(p.n_items < sms ? p.n_items : sms);
   return resident ? launch_tc_epi<true>(s, ma, mb, md, p, grid, epi, post)
                   : launch_tc_epi<false>(s, ma, mb, md, p, grid, epi, post);
 }
@@ -329,28 +342,17 @@ static int launch_tc(cudaStream_t s, const TcWorkspace& w, TcParams p, int64_t k
 static int launch_screen(cudaStream_t s, const TcWorkspace& w, int64_t m, int64_t n, int64_t k, int sel_s, int sel_lo,
                          int sel_hi, unsigned* overflow, const unsigned* run_flag, int unit_norm, const int* col_map)
 {
-  int sms = 0, cc = 0;
-  int rc  = device_sms(&sms, &cc);
-  if (rc) return rc;
-  if (cc != 9) return fail(B2D_ERR_CUDA, "raft_b200 requires an sm_90 (H100) device; found cc major " + std::to_string(cc));
   ScreenParams p;
   memset(&p, 0, sizeof(p));
   p.m = m; p.n = n;
   p.nkb     = static_cast<int>((k + 31) / 32);
   if (p.nkb > SC_MAX_KB) return fail(B2D_ERR_UNSUPPORTED, "internal: screening needs k <= 128");
   p.n_stages = static_cast<int>(std::min<size_t>(SC_MAX_STAGES, SC_A_RING / (static_cast<size_t>(p.nkb) * SC_A_KB_BYTES)));
-  p.tiles_m = static_cast<int>((m + TC_BM - 1) / TC_BM);
-  const int tiles_n = static_cast<int>((n + TC_BN - 1) / TC_BN);
   p.sel_s = sel_s; p.sel_lo = sel_lo; p.sel_hi = sel_hi;
-  p.tiles_sel = sel_count(tiles_n, sel_s, sel_lo, sel_hi);
   // long runs of x tiles per y block: the y block load is not overlapped with the previous item
-  int64_t total = static_cast<int64_t>(p.tiles_m) * p.tiles_sel;
-  int64_t chunk = total / (static_cast<int64_t>(sms) * 4);
-  chunk = std::max<int64_t>(1, std::min<int64_t>(chunk, 128));
-  chunk = std::min<int64_t>(chunk, p.tiles_m);
-  p.chunk    = static_cast<int>(chunk);
-  p.chunks_m = (p.tiles_m + p.chunk - 1) / p.chunk;
-  p.n_items  = static_cast<int64_t>(p.tiles_sel) * p.chunks_m;
+  int grid = 0;
+  int rc   = plan_tc_items(p, 4, 128, &grid);
+  if (rc) return rc;
   p.xsc = w.xsc; p.nonuni = w.nonuni;
   p.yt = w.yt; p.ylo = w.ylo; p.coef = w.coef; p.aux = w.aux; p.cand = w.cand; p.cand_cnt = w.cand_cnt; p.cand_cap = w.cand_cap;
   p.overflow = overflow; p.run_flag = run_flag; p.unit_norm = unit_norm; p.col_map = col_map;
@@ -360,7 +362,6 @@ static int launch_screen(cudaStream_t s, const TcWorkspace& w, int64_t m, int64_
   if (rc) return rc;
   rc = make_operand_map(&mb, w.yop, n, p.nkb, TC_BN, 0, 0, true);
   if (rc) return rc;
-  const int grid = static_cast<int>(p.n_items < sms ? p.n_items : sms);
   B2D_CUDA(cudaFuncSetAttribute(screen_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                 static_cast<int>(SC_SMEM_BYTES)));
   screen_tc_kernel<<<grid, SC_THREADS, SC_SMEM_BYTES, s>>>(ma, mb, p);
@@ -706,10 +707,9 @@ int b2d_pairwise_distance(void* stream, int metric, int dtype, const void* x, in
   p.p = metric_arg; p.inv_p = metric == B2D_HammingUnexpanded ? 1.f / static_cast<float>(k) : 1.f / metric_arg;
   p.tiles_n = static_cast<int>((na + UX_BN - 1) / UX_BN);
   const int64_t tiles = ((ma + UX_BM - 1) / UX_BM) * p.tiles_n;
-  int cc = 0, sms = 0;
-  int rc = device_sms(&sms, &cc);
+  int sms = 0;
+  int rc  = device_sms(&sms);
   if (rc) return rc;
-  if (cc != 9) return fail(B2D_ERR_CUDA, "raft_b200 requires an sm_90 (H100) device");
   switch (metric) {
     case B2D_L1: return launch_ux_inst<UX_L1>(s, p, tiles);
     case B2D_L2Unexpanded: return launch_ux_inst<UX_L2>(s, p, tiles);
@@ -805,8 +805,8 @@ static int fused_nn_keys_chunk(cudaStream_t s, int64_t* keys, const float* x, in
   if (rc) return rc;
   nn_decide_kernel<<<1, 1, 0, s>>>(flags, static_cast<unsigned>(m), tau, 2, w.nonuni);
   B2D_CUDA(cudaGetLastError());
-  int sms = 0, cc = 0;
-  rc = device_sms(&sms, &cc);
+  int sms = 0;
+  rc = device_sms(&sms);
   if (rc) return rc;
   nn_exact_kernel<<<sms * 8, 256, 0, s>>>(reinterpret_cast<long long*>(keys), w.cand, w.cand_cnt, w.cand_cap, x, ldx, y,
                                           ldy, static_cast<int>(k), idx_offset, unit_norm, center, static_cast<unsigned>(m), col_map);
@@ -1157,8 +1157,8 @@ static int knn_pass(KnnCtx& c, int64_t off, int64_t width)
                                                                             dc, c.p.m, c.kk);
   B2D_CUDA(cudaGetLastError());
   if (width > KNN_CAP) {  // (a pass of at most KNN_CAP columns cannot overflow)
-    int sms = 0, cc = 0;
-    rc = device_sms(&sms, &cc);
+    int sms = 0;
+    rc = device_sms(&sms);
     if (rc) return rc;
     knn_fix_kernel<<<sms * 2, 256, 0, c.s>>>(c.topk, c.thr, c.dirty, dc, c.x, c.ldx, c.y, c.ldy, static_cast<int>(c.k), c.kk, off,
                                              width, c.family, c.center);

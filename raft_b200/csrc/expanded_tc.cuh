@@ -49,6 +49,7 @@
 #include <cuda.h>
 #include <cuda_runtime.h>
 #include <cstdint>
+#include "nn_key.cuh"
 #include "ptx.cuh"
 
 namespace b2d {
@@ -183,11 +184,85 @@ __host__ __device__ __forceinline__ int sel_count(int tiles_n, int S, int lo, in
   return (tiles_n / S) * (hi - lo) + max(0, min(rem, hi) - lo);
 }
 
-// float -> int whose signed order equals the float order
-__device__ __forceinline__ int ordered_bits(float v)
+// Work item `item` of a persistent tensor-core launch (TcParams or ScreenParams): y block n_blk, x tiles [mt0, mt1), and
+// the nh halves of the y block that lie inside the matrix.
+struct TcItem {
+  int n_blk, mt0, mt1, nh;
+};
+template <class P>
+__host__ __device__ __forceinline__ TcItem tc_item(const P& p, int64_t item)
 {
-  int b = __float_as_int(v);
-  return b < 0 ? (b ^ 0x7FFFFFFF) : b;
+  TcItem t;
+  t.n_blk = sel_to_blk(static_cast<int>(item % p.tiles_sel), p.sel_s, p.sel_lo, p.sel_hi);
+  t.mt0   = static_cast<int>(item / p.tiles_sel) * p.chunk;
+  t.mt1   = min(t.mt0 + p.chunk, p.tiles_m);
+  t.nh    = static_cast<int64_t>(t.n_blk) * TC_BN + TC_HN < p.n ? 2 : 1;
+  return t;
+}
+
+// EPI_MINLOC_MASKED skip decisions (DESIGN.md section 2 K3m), shared by the producer, the consumers and the host replay of
+// the schedule (tests/cpp/masked_schedule_test.cu).  Class bytes are read through mask_cls_at.
+__host__ __device__ __forceinline__ unsigned mask_cls_at(const uint8_t* cls, int mt)
+{
+#ifdef __CUDA_ARCH__
+  return __ldg(&cls[mt]);
+#else
+  return cls[mt];
+#endif
+}
+// the item's last loaded tile (its y block is handed back after it); -1: no tile is loaded, the item is skipped
+__host__ __device__ __forceinline__ int mask_mt_last(const uint8_t* cls, int mt0, int mt1)
+{
+  int mt_last = -1;
+  for (int mt = mt0; mt < mt1; ++mt)
+    if (mask_cls_at(cls, mt) != 0u) mt_last = mt;
+  return mt_last;
+}
+// half h of a tile with class byte tcls != 0 has stages in the ring: resident, the tile's stages serve both halves;
+// streaming, a half no slab needs is not loaded
+__host__ __device__ __forceinline__ bool mask_half_loaded(bool resident, unsigned tcls, int h)
+{
+  return resident || mask_half_live(tcls, h);
+}
+// half h of nh hands its stages back (resident: the tile's last half, after both have read them)
+__host__ __device__ __forceinline__ bool tc_half_releases(bool resident, int h, int nh) { return !resident || h == nh - 1; }
+
+// The producer's load order, one definition for every instantiation and for the host replay of the masked schedule:
+// load_b(kb, it_local, t) for each k-block of a resident y block, load_a(a_it, t, mt, h, kb) for each stage (t: the
+// work item, tc_item).
+// kMasked skips the loads of dead tiles: a tile whose class byte is 0 loads nothing; in the streaming variant a half no
+// slab needs loads nothing; an item without a live tile loads no y block and does not count in it_local (the bfull /
+// bempty parity).
+#pragma nv_exec_check_disable
+template <bool kResident, bool kMasked, class P, class LoadB, class LoadA>
+__host__ __device__ __forceinline__ void tc_producer_walk(const P& p, int nkb, int64_t first_item, int64_t stride,
+                                                          LoadB&& load_b, LoadA&& load_a)
+{
+  uint32_t a_it = 0, it_local = 0;
+  for (int64_t item = first_item; item < p.n_items; item += stride) {
+    const TcItem t     = tc_item(p, item);
+    const uint8_t* cls = kMasked ? p.mask_cls + static_cast<int64_t>(t.n_blk) * p.tiles_m : nullptr;
+    bool b_loaded      = false;
+    for (int mt = t.mt0; mt < t.mt1; ++mt) {
+      unsigned tcls = 0u;
+      if constexpr (kMasked) {
+        tcls = mask_cls_at(cls, mt);
+        if (tcls == 0u) continue;
+      }
+      // resident: one load of an x k-block serves both halves of the tile; streaming: every stage carries its y half
+      for (int h = 0; h < (kResident ? 1 : t.nh); ++h) {
+        if constexpr (kMasked)
+          if (!mask_half_loaded(kResident, tcls, h)) continue;
+        for (int kb = 0; kb < nkb; ++kb, ++a_it) {
+          // the item's first loaded tile brings its y block (unmasked, every tile is loaded)
+          if (kResident && (kMasked ? !b_loaded : mt == t.mt0)) load_b(kb, it_local, t);
+          load_a(a_it, t, mt, h, kb);
+        }
+        b_loaded = true;
+      }
+    }
+    if (!kMasked || b_loaded) ++it_local;
+  }
 }
 
 __device__ __forceinline__ float min3(float a, float b, float c) { return fminf(fminf(a, b), c); }
@@ -208,8 +283,7 @@ __device__ __noinline__ void knn_append16(unsigned* cnt, long long* cand, unsign
     const float lv = a[t];
     const float dv = lv + xn;
     if (dv <= thr && lv < __int_as_float(0x7f800000)) {
-      const long long gj  = col0 + 8 * (t >> 1) + (t & 1);
-      const long long key = (static_cast<long long>(ordered_bits(dv)) << 32) | (gj & 0xFFFFFFFFll);
+      const long long key = key_pack(dv, col0 + 8 * (t >> 1) + (t & 1));
       const unsigned slot = atomicAdd(&cnt[row], 1u);
       if (slot < cap) cand[row * cap + slot] = key;
       else atomicMin(&dropmin[row], key);   // list full (ordered / adversarial data): remember the best key that was dropped
@@ -380,9 +454,7 @@ __device__ __forceinline__ void tc_epilogue(float (&v)[64], const TcParams& p, c
                 if (v[b + 4 * i + e] == mn) best = min(best, __ldg(&p.col_map[gcc + 8 * i + e]));
             gj = best;
           }
-          gj += p.idx_offset;
-          const long long key = (static_cast<long long>(ordered_bits(dv)) << 32) | (gj & 0xFFFFFFFFll);
-          atomicMin(&p.keys[row0 + 8 * j], key);
+          atomicMin(&p.keys[row0 + 8 * j], key_pack(dv, gj + p.idx_offset));
           thr[j] = dv;
         } else {
           knn_append16(p.knn_cnt, p.knn_cand, p.knn_cap, p.knn_dropmin, row0 + 8 * j, gcc + p.idx_offset, xnr[j], thr[j],
@@ -484,84 +556,27 @@ expanded_tc_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_cons
     // The whole warp runs the loop with warp-uniform values and one elected lane issues (inside a divergent
     // `if (lane == 0)` the compiler cannot keep descriptors / barrier addresses in uniform registers).
     const uint64_t pol = ptx::policy_evict_last();
-    uint32_t a_it = 0, it_local = 0;
-    if constexpr (kEpi == EPI_MINLOC_MASKED) {
-      // Masked: the same loads, minus those of dead tiles (DESIGN.md section 2 K3m, skip invariants).  A tile whose class
-      // byte is 0 loads nothing; in the streaming variant a half no slab needs loads nothing; an item without a live
-      // tile loads no y block and does not count in it_local (the bfull / bempty parity).  Apart from these skips the
-      // loop is the unmasked one below (kept apart so that the other instantiations compile as before): a change to
-      // either loop belongs in both.
-      for (int64_t item = blockIdx.x; item < p.n_items; item += gridDim.x) {
-        const int n_blk = sel_to_blk(static_cast<int>(item % p.tiles_sel), p.sel_s, p.sel_lo, p.sel_hi);
-        const int ch    = static_cast<int>(item / p.tiles_sel);
-        const int mt0   = ch * p.chunk;
-        const int mt1   = min(mt0 + p.chunk, p.tiles_m);
-        const int nh    = static_cast<int64_t>(n_blk) * TC_BN + TC_HN < p.n ? 2 : 1;
-        const uint8_t* cls = p.mask_cls + static_cast<int64_t>(n_blk) * p.tiles_m;
-        bool b_loaded = false;
-        for (int mt = mt0; mt < mt1; ++mt) {
-          const unsigned tcls = __ldg(&cls[mt]);
-          if (tcls == 0u) continue;
-          for (int h = 0; h < (kResident ? 1 : nh); ++h) {
-            if (!kResident && !mask_half_live(tcls, h)) continue;
-            for (int kb = 0; kb < nkb; ++kb, ++a_it) {
-              if (kResident && !b_loaded) {
-                ptx::mbar_wait(&bempty[kb], (it_local & 1) ^ 1);
-                if (ptx::elect_one()) {
-                  ptx::mbar_expect_tx(&bfull[kb], TC_B_BYTES);
-                  ptx::tma_load_2d(b_base + kb * TC_B_BYTES, &tmap_b, &bfull[kb], kb * 64, n_blk * TC_BN, pol);
-                }
-              }
-              const uint32_t s = a_it % kStages, ph = (a_it / kStages) & 1;
-              ptx::mbar_wait(&aempty[s], ph ^ 1);
-              if (ptx::elect_one()) {
-                ptx::mbar_expect_tx(&afull[s], kStageBytes);
-                ptx::tma_load_2d(a_base + s * kStageBytes, &tmap_a, &afull[s], kb * 64, mt * TC_BM, pol);
-                if (!kResident)
-                  ptx::tma_load_2d(a_base + s * kStageBytes + TC_A_BYTES, &tmap_b, &afull[s], kb * 64,
-                                   n_blk * TC_BN + h * TC_HN, pol);
-              }
-              __syncwarp();
-            }
-            b_loaded = true;
+    tc_producer_walk<kResident, kMasked>(
+        p, nkb, blockIdx.x, gridDim.x,
+        [&](int kb, uint32_t it_local, const TcItem& t) {
+          ptx::mbar_wait(&bempty[kb], (it_local & 1) ^ 1);
+          if (ptx::elect_one()) {
+            ptx::mbar_expect_tx(&bfull[kb], TC_B_BYTES);
+            ptx::tma_load_2d(b_base + kb * TC_B_BYTES, &tmap_b, &bfull[kb], kb * 64, t.n_blk * TC_BN, pol);
           }
-        }
-        if (b_loaded) ++it_local;
-      }
-    } else {   // (mirrored, with the skips, by the masked loop above)
-      for (int64_t item = blockIdx.x; item < p.n_items; item += gridDim.x, ++it_local) {
-        const int n_blk = sel_to_blk(static_cast<int>(item % p.tiles_sel), p.sel_s, p.sel_lo, p.sel_hi);
-        const int ch    = static_cast<int>(item / p.tiles_sel);
-        const int mt0   = ch * p.chunk;
-        const int mt1   = min(mt0 + p.chunk, p.tiles_m);
-        const int nh    = static_cast<int64_t>(n_blk) * TC_BN + TC_HN < p.n ? 2 : 1;  // halves of the y block inside the matrix
-        // resident: one load of an x k-block serves both halves of the tile; streaming: every stage carries its y half
-        const int nh_load = kResident ? 1 : nh;
-        for (int mt = mt0; mt < mt1; ++mt) {
-          for (int h = 0; h < nh_load; ++h) {
-            for (int kb = 0; kb < nkb; ++kb, ++a_it) {
-              if (kResident && mt == mt0 && h == 0) {
-                ptx::mbar_wait(&bempty[kb], (it_local & 1) ^ 1);
-                if (ptx::elect_one()) {
-                  ptx::mbar_expect_tx(&bfull[kb], TC_B_BYTES);
-                  ptx::tma_load_2d(b_base + kb * TC_B_BYTES, &tmap_b, &bfull[kb], kb * 64, n_blk * TC_BN, pol);
-                }
-              }
-              const uint32_t s = a_it % kStages, ph = (a_it / kStages) & 1;
-              ptx::mbar_wait(&aempty[s], ph ^ 1);
-              if (ptx::elect_one()) {
-                ptx::mbar_expect_tx(&afull[s], kStageBytes);
-                ptx::tma_load_2d(a_base + s * kStageBytes, &tmap_a, &afull[s], kb * 64, mt * TC_BM, pol);
-                if (!kResident)
-                  ptx::tma_load_2d(a_base + s * kStageBytes + TC_A_BYTES, &tmap_b, &afull[s], kb * 64,
-                                   n_blk * TC_BN + h * TC_HN, pol);
-              }
-              __syncwarp();
-            }
+        },
+        [&](uint32_t a_it, const TcItem& t, int mt, int h, int kb) {
+          const uint32_t s = a_it % kStages, ph = (a_it / kStages) & 1;
+          ptx::mbar_wait(&aempty[s], ph ^ 1);
+          if (ptx::elect_one()) {
+            ptx::mbar_expect_tx(&afull[s], kStageBytes);
+            ptx::tma_load_2d(a_base + s * kStageBytes, &tmap_a, &afull[s], kb * 64, mt * TC_BM, pol);
+            if (!kResident)
+              ptx::tma_load_2d(a_base + s * kStageBytes + TC_A_BYTES, &tmap_b, &afull[s], kb * 64,
+                               t.n_blk * TC_BN + h * TC_HN, pol);
           }
-        }
-      }
-    }
+          __syncwarp();
+        });
     return;
   }
 
@@ -580,20 +595,15 @@ expanded_tc_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_cons
   uint32_t a_it = 0, it_local = 0;
   float acc[64], crs[64];
   for (int64_t item = blockIdx.x; item < p.n_items; item += gridDim.x, ++it_local) {
-    const int n_blk = sel_to_blk(static_cast<int>(item % p.tiles_sel), p.sel_s, p.sel_lo, p.sel_hi);
-    const int ch    = static_cast<int>(item / p.tiles_sel);
-    const int mt0   = ch * p.chunk;
-    const int mt1   = min(mt0 + p.chunk, p.tiles_m);
-    const int nh    = static_cast<int64_t>(n_blk) * TC_BN + TC_HN < p.n ? 2 : 1;
+    const TcItem t  = tc_item(p, item);
+    const int n_blk = t.n_blk, mt0 = t.mt0, mt1 = t.mt1, nh = t.nh;
     // masked: the item's last loaded tile (its y block is handed back after it); no loaded tile: the producer skipped
     // the item, and it does not count in it_local
     int mt_last = mt1 - 1;
     const uint8_t* cls = nullptr;
     if constexpr (kMasked) {
       cls     = p.mask_cls + static_cast<int64_t>(n_blk) * p.tiles_m;
-      mt_last = -1;
-      for (int mt = mt0; mt < mt1; ++mt)
-        if (__ldg(&cls[mt]) != 0u) mt_last = mt;
+      mt_last = mask_mt_last(cls, mt0, mt1);
       if (mt_last < 0) { --it_local; continue; }
     }
     bool b_first = true;   // masked: this warpgroup has not waited for the item's y block yet
@@ -612,7 +622,7 @@ expanded_tc_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_cons
     for (int mt = mt0; mt < mt1; ++mt) {
       unsigned tcls = 0u;
       if constexpr (kMasked) {
-        tcls = __ldg(&cls[mt]);
+        tcls = mask_cls_at(cls, mt);
         if (tcls == 0u) continue;   // not loaded
       }
       // the two tile rows this thread owns: row0 and row0 + 8
@@ -627,12 +637,8 @@ expanded_tc_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_cons
           if (xnu) cr *= __ldg(&p.xsc[gi]);
           if (kEpi != EPI_STORE || p.acc_mode < 2) rv = __ldg(&p.xt[gi]);
           if (kEpi == EPI_TOPK) thr[j] = __ldg(&p.knn_thr[gi]);
-          if (kMinloc) {  // the row's current best (an upper bound: keys only decrease)
-            const long long ck = *reinterpret_cast<volatile long long*>(&p.keys[gi]);
-            const int sb       = static_cast<int>(ck >> 32);
-            thr[j]             = __int_as_float(sb < 0 ? (sb ^ 0x7FFFFFFF) : sb);
-            if (ck == 0x7FFFFFFFFFFFFFFFll) thr[j] = __int_as_float(0x7f800000);
-          }
+          if (kMinloc)  // the row's current best (an upper bound: keys only decrease)
+            thr[j] = key_bound(*reinterpret_cast<volatile long long*>(&p.keys[gi]));
         }
         ta[j]  = rv;
         xnr[j] = rv;
@@ -653,8 +659,8 @@ expanded_tc_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_cons
             // wait forever.  One stage at a time: a streamed half has more k-blocks (k > 192) than the ring has stages,
             // so holding them all before handing any back would starve the producer.  (Barrier 2 + wg is free here:
             // only EPI_STORE uses it.)
-            if (!kResident && !mask_half_live(tcls, h)) continue;   // not loaded
-            if (!kResident || h == nh - 1) {
+            if (!mask_half_loaded(kResident, tcls, h)) continue;
+            if (tc_half_releases(kResident, h, nh)) {
               for (int kb = 0; kb < nkb; ++kb) {
                 const uint32_t it = a_it + kb;
                 ptx::mbar_wait(&afull[it % kStages], (it / kStages) & 1);
@@ -674,6 +680,7 @@ expanded_tc_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_cons
         }
         // Resident: both halves read the tile's nkb x stages (a_it counts (tile, kb)), and only the last half hands
         // them back.  In an earlier half the stage's phase cannot advance, so waiting on it again returns at once.
+        // (the rule of tc_half_releases, written out: through the call the resident instantiations schedule differently)
         const bool release = !kResident || h == nh - 1;
         const uint32_t it0 = a_it;
         // descriptor start-address units are 16 B; inside the 128-B swizzled row of a k-block:
@@ -741,7 +748,7 @@ expanded_tc_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_cons
 __global__ void minloc_init_kernel(long long* keys, int64_t m)
 {
   int64_t i = static_cast<int64_t>(blockIdx.x) * blockDim.x + threadIdx.x;
-  if (i < m) keys[i] = 0x7FFFFFFFFFFFFFFFll;
+  if (i < m) keys[i] = KEY_EMPTY;
 }
 
 struct KvpIF {
@@ -756,15 +763,13 @@ __global__ void minloc_finalize_kernel(KvpIF* out, const long long* keys, int64_
   int64_t i = static_cast<int64_t>(blockIdx.x) * blockDim.x + threadIdx.x;
   if (i >= m) return;
   const long long key = keys[i];
-  int s               = static_cast<int>(key >> 32);
-  int bits            = s < 0 ? (s ^ 0x7FFFFFFF) : s;
-  float v             = __int_as_float(bits);
+  const float v       = key_dist(key);
   float d             = v < 0.f ? 0.f : v;  // clamp at 0; NaN (zero-norm rows under cosine / NaN inputs) stays NaN
   if (do_sqrt) d = sqrtf(d);
   KvpIF o;
-  o.key   = static_cast<int>(key & 0xFFFFFFFFll);
+  o.key   = static_cast<int>(key_index(key));
   o.value = d;
-  if (key == 0x7FFFFFFFFFFFFFFFll) {  // no candidate (n == 0)
+  if (key == KEY_EMPTY) {  // no candidate (n == 0)
     o.key   = 0x7fffffff;
     o.value = __int_as_float(0x7f7fffff);
   }
@@ -816,15 +821,14 @@ __global__ void nn_seed_kernel(long long* keys, float4* aux, const float* xt, co
   }
   if (i >= m) return;
   const long long key = keys[i];
-  float t             = __int_as_float(0x7f800000);
+  float t             = __int_as_float(0x7f800000);   // no incumbent: no bound
   int2 c              = make_int2(-1, -1);
-  if (key != 0x7FFFFFFFFFFFFFFFll) {
-    const int sb = static_cast<int>(key >> 32);
-    t            = __int_as_float(sb < 0 ? (sb ^ 0x7FFFFFFF) : sb);
-    const long long j = (key & 0xFFFFFFFFll) - idx_offset;
+  if (key != KEY_EMPTY) {
+    t                 = key_dist(key);
+    const long long j = key_index(key) - idx_offset;
     if (j >= 0 && j < n) {  // incumbent of THIS shard: re-measured with the exact arithmetic below
       c       = make_int2(static_cast<int>(i), static_cast<int>(j));
-      keys[i] = 0x7FFFFFFFFFFFFFFFll;
+      keys[i] = KEY_EMPTY;
     }                        // else: a key merged in from another shard stays as it is
   }
   // screening compares v = d - |x|^2 with (bound - |x|^2), rounded up so that it stays an upper bound
@@ -911,11 +915,7 @@ __global__ void __launch_bounds__(256) nn_exact_kernel(long long* keys, const in
       }
       res = 1.f - dot / sqrtf(nx * ny);
     }
-    if (lane == 0) {
-      const long long gj  = static_cast<long long>(ij.y) + idx_offset;
-      const long long key = (static_cast<long long>(ordered_bits(res)) << 32) | (gj & 0xFFFFFFFFll);
-      atomicMin(&keys[ij.x], key);
-    }
+    if (lane == 0) atomicMin(&keys[ij.x], key_pack(res, static_cast<long long>(ij.y) + idx_offset));
   }
 }
 
@@ -934,8 +934,8 @@ __global__ void knn_init_kernel(long long* topk, float* thr, unsigned* cnt, long
 {
   const int64_t i = static_cast<int64_t>(blockIdx.x) * blockDim.x + threadIdx.x;
   if (i < 64) dirty_cnt[i] = 0u;   // one counter per pass
-  if (i < m) { thr[i] = __int_as_float(0x7f800000); cnt[i] = 0u; dropmin[i] = 0x7FFFFFFFFFFFFFFFll; }
-  if (i < m * kk) topk[i] = 0x7FFFFFFFFFFFFFFFll;
+  if (i < m) { thr[i] = __int_as_float(0x7f800000); cnt[i] = 0u; dropmin[i] = KEY_EMPTY; }
+  if (i < m * kk) topk[i] = KEY_EMPTY;
 }
 
 // one warp per row: sort (top-k so far) + (this pass's list) by (distance, index), keep the first kk.  A row whose list
@@ -957,7 +957,7 @@ __global__ void __launch_bounds__(256) knn_merge_kernel(long long* topk, const l
   int ssz = 32;
   while (ssz < kk + static_cast<int>(nc)) ssz <<= 1;
   for (int t = lane; t < ssz; t += 32) {
-    long long key = 0x7FFFFFFFFFFFFFFFll;
+    long long key = KEY_EMPTY;
     if (t < kk) key = topk[row * kk + t];
     else if (t - kk < static_cast<int>(nc)) key = cand[row * KNN_CAP + (t - kk)];
     b[t] = key;
@@ -977,13 +977,10 @@ __global__ void __launch_bounds__(256) knn_merge_kernel(long long* topk, const l
   if (lane == 0) {
     cnt[row]            = 0u;
     const long long kth = b[kk - 1];
-    if (kth != 0x7FFFFFFFFFFFFFFFll) {
-      const int sb = static_cast<int>(kth >> 32);
-      thr[row]     = __int_as_float(sb < 0 ? (sb ^ 0x7FFFFFFF) : sb);
-    }
+    if (kth != KEY_EMPTY) thr[row] = key_dist(kth);
     if (craw > static_cast<unsigned>(KNN_CAP)) {
       if (dropmin[row] <= kth) dirty[atomicAdd(dirty_cnt, 1u)] = static_cast<int>(row);
-      dropmin[row] = 0x7FFFFFFFFFFFFFFFll;
+      dropmin[row] = KEY_EMPTY;
     }
   }
 }
@@ -1020,11 +1017,11 @@ __global__ void __launch_bounds__(256) knn_fix_kernel(long long* topk, float* th
     for (int t = tid; t < k; t += 256) xs[t] = x[row * ldx + t] - xstat[0];
     // the row's top-k without what this pass had put in
     for (int t = tid; t < 512; t += 256) {
-      long long key = 0x7FFFFFFFFFFFFFFFll;
+      long long key = KEY_EMPTY;
       if (t < kk) {
         key = topk[row * kk + t];
-        const long long j = key & 0xFFFFFFFFll;
-        if (key != 0x7FFFFFFFFFFFFFFFll && j >= off && j < off + width) key = 0x7FFFFFFFFFFFFFFFll;
+        const long long j = key_index(key);
+        if (key != KEY_EMPTY && j >= off && j < off + width) key = KEY_EMPTY;
       }
       keys[t] = key;
     }
@@ -1052,7 +1049,7 @@ __global__ void __launch_bounds__(256) knn_fix_kernel(long long* topk, float* th
           for (int t = 0; t < k; ++t) { const float b = __ldg(yr + t) - my; dot = fmaf(xs[t], b, dot); ny = fmaf(b, b, ny); }
           val = 1.f - dot / sqrtf(xstat[1] * ny);
         }
-        const long long key = (static_cast<long long>(ordered_bits(val)) << 32) | ((off + j) & 0xFFFFFFFFll);
+        const long long key = key_pack(val, off + j);
         if (key < kth && val == val) keys[kk + atomicAdd(&ncand, 1u)] = key;   // (kk + 256 <= 320 < 512)
       }
       __syncthreads();
@@ -1066,7 +1063,7 @@ __global__ void __launch_bounds__(256) knn_fix_kernel(long long* topk, float* th
             if ((a > c) == up) { keys[i] = c; keys[jj] = a; }
             __syncthreads();
           }
-        for (int t = kk + tid; t < 512; t += 256) keys[t] = 0x7FFFFFFFFFFFFFFFll;
+        for (int t = kk + tid; t < 512; t += 256) keys[t] = KEY_EMPTY;
         if (tid == 0) ncand = 0u;
         __syncthreads();
       }
@@ -1082,11 +1079,7 @@ __global__ void __launch_bounds__(256) knn_fix_kernel(long long* topk, float* th
         __syncthreads();
       }
     for (int t = tid; t < kk; t += 256) topk[row * kk + t] = keys[t];
-    if (tid == 0) {
-      const long long kth = keys[kk - 1];
-      const int sb        = static_cast<int>(kth >> 32);
-      thr[row] = kth == 0x7FFFFFFFFFFFFFFFll ? __int_as_float(0x7f800000) : __int_as_float(sb < 0 ? (sb ^ 0x7FFFFFFF) : sb);
-    }
+    if (tid == 0) thr[row] = key_bound(keys[kk - 1]);
   }
 }
 
@@ -1096,12 +1089,11 @@ __global__ void knn_finalize_kernel(int64_t* out_idx, float* out_dist, const lon
   const int64_t i = static_cast<int64_t>(blockIdx.x) * blockDim.x + threadIdx.x;
   if (i >= total) return;
   const long long key = topk[i];
-  const int s         = static_cast<int>(key >> 32);
-  float d             = __int_as_float(s < 0 ? (s ^ 0x7FFFFFFF) : s);
+  float d             = key_dist(key);
   d                   = d < 0.f ? 0.f : d;  // NaN propagates
   if (do_sqrt) d = sqrtf(d);
-  out_idx[i]  = key == 0x7FFFFFFFFFFFFFFFll ? -1 : static_cast<int64_t>(key & 0xFFFFFFFFll);
-  out_dist[i] = key == 0x7FFFFFFFFFFFFFFFll ? __int_as_float(0x7f800000) : d;
+  out_idx[i]  = key == KEY_EMPTY ? -1 : static_cast<int64_t>(key_index(key));
+  out_dist[i] = key == KEY_EMPTY ? __int_as_float(0x7f800000) : d;
 }
 
 }  // namespace b2d

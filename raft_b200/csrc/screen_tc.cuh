@@ -111,10 +111,7 @@ screen_tc_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_consta
     const uint64_t pol = ptx::policy_evict_last();
     uint32_t t_it = 0, it_local = 0;
     for (int64_t item = blockIdx.x; item < p.n_items; item += gridDim.x, ++it_local) {
-      const int n_blk = sel_to_blk(static_cast<int>(item % p.tiles_sel), p.sel_s, p.sel_lo, p.sel_hi);
-      const int ch    = static_cast<int>(item / p.tiles_sel);
-      const int mt0   = ch * p.chunk;
-      const int mt1   = min(mt0 + p.chunk, p.tiles_m);
+      const auto [n_blk, mt0, mt1, nh] = tc_item(p, item);
       ptx::mbar_wait(bempty, (it_local & 1) ^ 1);
       if (ptx::elect_one()) {
         ptx::mbar_expect_tx(bfull, static_cast<uint32_t>(nkb) * SC_B_KB_BYTES);
@@ -152,10 +149,7 @@ screen_tc_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_consta
   uint32_t t_it = 0, it_local = 0;
   float acc[2][64];           // columns [0, 128) and [128, 256) of the y block
   for (int64_t item = blockIdx.x; item < p.n_items; item += gridDim.x, ++it_local) {
-    const int n_blk = sel_to_blk(static_cast<int>(item % p.tiles_sel), p.sel_s, p.sel_lo, p.sel_hi);
-    const int ch    = static_cast<int>(item / p.tiles_sel);
-    const int mt0   = ch * p.chunk;
-    const int mt1   = min(mt0 + p.chunk, p.tiles_m);
+    const auto [n_blk, mt0, mt1, nh] = tc_item(p, item);
     // per-column terms of this y block (shared by every tile of the item)
     ptx::bar_sync(1, 256);
     {

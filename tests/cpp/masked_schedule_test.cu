@@ -4,7 +4,9 @@
 //                     every (64-row slab, 128-column half) tile from masked_tile_class, one row of digits per slab
 //                     (compared with a numpy restatement by tests/test_masked_nn.py)
 //   replay            replays the producer and the two consumer warpgroups of expanded_tc_kernel<kResident,
-//                     EPI_MINLOC_MASKED> over random class bytes, resident and streaming, and checks the invariants of
+//                     EPI_MINLOC_MASKED> over random class bytes, resident and streaming (the kernel's own
+//                     tc_producer_walk and skip helpers; only the consumers' waits and hand-backs are restated), and
+//                     checks the invariants of
 //                     DESIGN.md section 2 K3m: the same stage sequence on both sides, every loaded stage released by
 //                     both warpgroups exactly once, the y block of every loaded item waited for and handed back by
 //                     both, and nothing for a skipped item.  (Counts and order per warpgroup: that every warp of a
@@ -44,12 +46,12 @@ static int classify()
 
 // one (tile, k-block) stage load of the producer, and what the consumers did with it
 struct Stage {
-  int item, mt, h, kb;
+  int n_blk, mt0, mt, h, kb;
   int waits[2] = {0, 0}, releases[2] = {0, 0};
 };
 
-static int replay_case(bool resident, int nkb, int tiles_m, int nblocks, int n_last_half, int chunk, int grid, std::mt19937& rng,
-                       double p_dead)
+template <bool kResident>
+static int replay_case(int nkb, int tiles_m, int nblocks, int n_last_half, int chunk, int grid, std::mt19937& rng, double p_dead)
 {
   int bad = 0;
   // class bytes: a tile is dead with probability p_dead, otherwise random classes per (slab, half); a y block's second
@@ -65,38 +67,31 @@ static int replay_case(bool resident, int nkb, int tiles_m, int nblocks, int n_l
           for (int s = 0; s < 2; ++s) b |= static_cast<unsigned>(rng() % 3) << (2 * (2 * h + s));
       cls[static_cast<size_t>(nb) * tiles_m + mt] = static_cast<uint8_t>(b);
     }
-  const int chunks_m = (tiles_m + chunk - 1) / chunk;
-  const long long n_items = static_cast<long long>(nblocks) * chunks_m;
+  // the schedule fields as launch_tc fills them (every y block selected); the last y block has one half unless n_last_half
+  TcParams p{};
+  p.n = static_cast<int64_t>(nblocks) * TC_BN - (n_last_half ? 0 : TC_HN);
+  p.tiles_m = tiles_m; p.tiles_sel = nblocks; p.chunk = chunk; p.chunks_m = (tiles_m + chunk - 1) / chunk;
+  p.n_items  = static_cast<int64_t>(nblocks) * p.chunks_m;
+  p.mask_cls = cls.data();
+  // liveness of the ring: the producer refills position P - stages as position P, so a warpgroup must have handed
+  // P - stages back before it waits for P
+  constexpr int stages = TcCarve<kResident, EPI_MINLOC_MASKED>::stages;
   for (int cta = 0; cta < grid; ++cta) {
-    // ---- producer (the masked loop of expanded_tc_kernel) ----
+    // ---- producer: the kernel's own load order, recorded ----
     std::vector<Stage> loads;
     std::vector<int> b_loads;   // it_local of every y block load
-    uint32_t it_local = 0;
-    for (long long item = cta; item < n_items; item += grid) {
-      const int n_blk = static_cast<int>(item % nblocks), ch = static_cast<int>(item / nblocks);
-      const int mt0 = ch * chunk, mt1 = std::min(mt0 + chunk, tiles_m);
-      const int nh  = (n_blk < nblocks - 1 || n_last_half) ? 2 : 1;
-      bool b_loaded = false;
-      for (int mt = mt0; mt < mt1; ++mt) {
-        const unsigned tcls = cls[static_cast<size_t>(n_blk) * tiles_m + mt];
-        if (tcls == 0u) continue;
-        for (int h = 0; h < (resident ? 1 : nh); ++h) {
-          if (!resident && !mask_half_live(tcls, h)) continue;
-          for (int kb = 0; kb < nkb; ++kb) {
-            if (resident && !b_loaded && kb == 0) b_loads.push_back(static_cast<int>(it_local));
-            loads.push_back(Stage{static_cast<int>(item), mt, h, kb});
-          }
-          b_loaded = true;
-        }
-      }
-      if (b_loaded) ++it_local;
-    }
-    // ---- consumer warpgroups (the masked paths of the consumer loop) ----
+    int items_loaded = 0;
+    tc_producer_walk<kResident, true>(
+        p, nkb, cta, grid,
+        [&](int kb, uint32_t it_local, const TcItem&) { if (kb == 0) b_loads.push_back(static_cast<int>(it_local)); },
+        [&](uint32_t a_it, const TcItem& t, int mt, int h, int kb) {
+          if (a_it != loads.size()) ++bad;   // a_it counts the loaded stages
+          if (loads.empty() || loads.back().n_blk != t.n_blk || loads.back().mt0 != t.mt0) ++items_loaded;
+          loads.push_back(Stage{t.n_blk, t.mt0, mt, h, kb});
+        });
+    // ---- consumer warpgroups: the masked paths of the consumer loop, with the kernel's own skip decisions ----
     std::vector<int> a_end(2);
     std::map<int, int> bwait_item[2], brel_item[2];   // it_local -> count
-    // liveness of the ring: the producer refills position P - stages as position P, so a warpgroup must have handed
-    // P - stages back before it waits for P
-    const int stages = resident ? TC_STAGES_RES : TC_STAGES_STR;
     for (int wg = 0; wg < 2; ++wg) {
       std::vector<char> released(loads.size() + 1, 0);
       auto wait_at = [&](uint32_t it) {
@@ -104,29 +99,25 @@ static int replay_case(bool resident, int nkb, int tiles_m, int nblocks, int n_l
       };
       auto release_at = [&](uint32_t it) { if (it < released.size()) released[it] = 1; };
       uint32_t a_it = 0, itl = 0;
-      for (long long item = cta; item < n_items; item += grid, ++itl) {
-        const int n_blk = static_cast<int>(item % nblocks), ch = static_cast<int>(item / nblocks);
-        const int mt0 = ch * chunk, mt1 = std::min(mt0 + chunk, tiles_m);
-        const int nh  = (n_blk < nblocks - 1 || n_last_half) ? 2 : 1;
-        const uint8_t* c = cls.data() + static_cast<size_t>(n_blk) * tiles_m;
-        int mt_last = -1;
-        for (int mt = mt0; mt < mt1; ++mt) if (c[mt] != 0u) mt_last = mt;
+      for (int64_t item = cta; item < p.n_items; item += grid, ++itl) {
+        const TcItem t     = tc_item(p, item);
+        const uint8_t* c   = p.mask_cls + static_cast<int64_t>(t.n_blk) * p.tiles_m;
+        const int mt_last  = mask_mt_last(c, t.mt0, t.mt1);
         if (mt_last < 0) { --itl; continue; }
         bool b_first = true;
-        for (int mt = mt0; mt < mt1; ++mt) {
-          const unsigned tcls = c[mt];
+        for (int mt = t.mt0; mt < t.mt1; ++mt) {
+          const unsigned tcls = mask_cls_at(c, mt);
           if (tcls == 0u) continue;
-          for (int h = 0; h < nh; ++h) {
-            const int hcls = mask_class_of(tcls, h, wg);
-            const bool release = !resident || h == nh - 1;
+          for (int h = 0; h < t.nh; ++h) {
+            const bool release = tc_half_releases(kResident, h, t.nh);
             auto stage_at = [&](uint32_t it) -> Stage* {
               if (it >= loads.size()) { ++bad; return nullptr; }
               Stage* st = &loads[it];
-              if (st->item != item || st->mt != mt || (!resident && st->h != h)) ++bad;   // the same stage sequence
+              if (st->n_blk != t.n_blk || st->mt != mt || (!kResident && st->h != h)) ++bad;   // the same stage sequence
               return st;
             };
-            if (hcls == MASK_NONE) {
-              if (!resident && !mask_half_live(tcls, h)) continue;
+            if (mask_class_of(tcls, h, wg) == MASK_NONE) {
+              if (!mask_half_loaded(kResident, tcls, h)) continue;
               if (release) {
                 for (int kb = 0; kb < nkb; ++kb) {   // wait, meet, hand back: one stage at a time
                   wait_at(a_it + kb);
@@ -134,12 +125,12 @@ static int replay_case(bool resident, int nkb, int tiles_m, int nblocks, int n_l
                   if (Stage* st = stage_at(a_it + kb)) { st->waits[wg]++; st->releases[wg]++; if (st->kb != kb) ++bad; }
                 }
                 a_it += nkb;
-                if (resident && mt == mt_last) brel_item[wg][static_cast<int>(itl)]++;
+                if (kResident && mt == mt_last) brel_item[wg][static_cast<int>(itl)]++;
               }
               continue;
             }
             for (int kb = 0; kb < nkb; ++kb) {   // live: wait for kb, then hand back kb - 1 (the last after the loop)
-              if (resident && b_first && kb == 0) bwait_item[wg][static_cast<int>(itl)]++;
+              if (kResident && b_first && kb == 0) bwait_item[wg][static_cast<int>(itl)]++;
               wait_at(a_it + kb);
               if (release && kb > 0) release_at(a_it + kb - 1);
               if (Stage* st = stage_at(a_it + kb)) { st->waits[wg]++; if (release) st->releases[wg]++; if (st->kb != kb) ++bad; }
@@ -148,13 +139,13 @@ static int replay_case(bool resident, int nkb, int tiles_m, int nblocks, int n_l
             b_first = false;
             if (release) {
               a_it += nkb;
-              if (resident && mt == mt_last && h == nh - 1) brel_item[wg][static_cast<int>(itl)]++;
+              if (kResident && mt == mt_last && h == t.nh - 1) brel_item[wg][static_cast<int>(itl)]++;
             }
           }
         }
       }
       a_end[wg] = static_cast<int>(a_it);
-      if (itl != it_local) ++bad;   // both sides count the same loaded items
+      if (static_cast<int>(itl) != items_loaded) ++bad;   // both sides count the same loaded items
     }
     // ---- invariants ----
     for (int wg = 0; wg < 2; ++wg)
@@ -162,13 +153,16 @@ static int replay_case(bool resident, int nkb, int tiles_m, int nblocks, int n_l
     for (const Stage& st : loads)
       for (int wg = 0; wg < 2; ++wg)
         if (st.releases[wg] != 1 || st.waits[wg] < 1) ++bad;   // waited for, and released once by each warpgroup
-    if (resident)
+    if (kResident)
       for (int it : b_loads)
         for (int wg = 0; wg < 2; ++wg) {
           if (brel_item[wg][it] != 1) ++bad;                    // the y block handed back once per loaded item
           if (bwait_item[wg][it] > 1) ++bad;                    // and waited for at most once (not at all: no MMAs)
         }
-    if (resident && static_cast<int>(b_loads.size()) != static_cast<int>(it_local)) ++bad;
+    if (kResident)   // it_local counts only loaded items: the i-th y block load has parity count i
+      for (size_t i = 0; i < b_loads.size(); ++i)
+        if (b_loads[i] != static_cast<int>(i)) ++bad;
+    if (kResident && static_cast<int>(b_loads.size()) != items_loaded) ++bad;
   }
   return bad;
 }
@@ -183,7 +177,9 @@ static int replay()
         for (int rep = 0; rep < 6; ++rep) {
           const int tiles_m = 1 + static_cast<int>(rng() % 40), nblocks = 1 + static_cast<int>(rng() % 9);
           const int chunk = 1 + static_cast<int>(rng() % 8), grid = 1 + static_cast<int>(rng() % 5);
-          const int b = replay_case(resident, nkb, tiles_m, nblocks, static_cast<int>(rng() % 2), chunk, grid, rng, p_dead);
+          const int nlh = static_cast<int>(rng() % 2);
+          const int b   = resident ? replay_case<true>(nkb, tiles_m, nblocks, nlh, chunk, grid, rng, p_dead)
+                                   : replay_case<false>(nkb, tiles_m, nblocks, nlh, chunk, grid, rng, p_dead);
           if (b) std::printf("case resident=%d nkb=%d tiles_m=%d blocks=%d: %d violations\n", resident, nkb, tiles_m, nblocks, b);
           bad += b;
           ++cases;

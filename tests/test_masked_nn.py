@@ -97,8 +97,8 @@ def test_valid_arguments_without_gpu_report_cuda_error():
     assert _call(L, G=0, adj=0, gidx=0, ld_adj=0) == _lib.B2D_ERR_CUDA
 
 
-def _schedule_exe():
-    exe = os.path.join(ROOT, "tests", "cpp", "masked_schedule_test")
+def _schedule_exe(build_dir):
+    exe = os.path.join(build_dir, "masked_schedule_test")
     cmd = [NVCC, "-std=c++17", "-O1", "--expt-relaxed-constexpr", "-gencode", "arch=compute_90a,code=sm_90a", "-o", exe,
            os.path.join(ROOT, "tests", "cpp", "masked_schedule_test.cu")]
     res = subprocess.run(cmd, capture_output=True, text=True)
@@ -107,8 +107,9 @@ def _schedule_exe():
 
 
 @pytest.fixture(scope="module")
-def schedule_exe():
-    return _schedule_exe()
+def schedule_exe(tmp_path_factory):
+    # built outside the source tree, which need not be writable
+    return _schedule_exe(str(tmp_path_factory.mktemp("cpp")))
 
 
 def _classify(exe, adj, gidx, m, n):
@@ -150,9 +151,9 @@ def test_skip_schedule_replay(schedule_exe):
     assert res.returncode == 0 and "PASS" in res.stdout, res.stdout + res.stderr
 
 
-def test_masked_shim_compiles_and_links():
+def test_masked_shim_compiles_and_links(tmp_path):
     _build.build()
-    exe = os.path.join(ROOT, "tests", "cpp", "masked_nn_test")
+    exe = str(tmp_path / "masked_nn_test")
     cmd = [NVCC, "-std=c++17", "-O1", "-I", os.path.join(ROOT, "include"), "-o", exe,
            os.path.join(ROOT, "tests", "cpp", "masked_nn_test.cu"), "-L", os.path.dirname(_build.SO_PATH),
            "-lraft_b200", "-Xlinker", "-rpath", "-Xlinker", os.path.dirname(_build.SO_PATH)]

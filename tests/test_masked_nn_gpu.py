@@ -242,7 +242,7 @@ def test_none_runs_for_one_slab_followed_by_live_tiles(k):
     run_and_check(x, y, adj, gidx)
 
 
-def test_cpp_shim_on_gpu():
+def test_cpp_shim_on_gpu(tmp_path):
     """raft::distance::masked_l2_nn with MinAndDistanceReduceOp (KVP out), MinReduceOp (float out, sqrt) and
     initOutBuffer = false, against a host brute force (tests/cpp/masked_nn_test.cu)."""
     import os
@@ -250,7 +250,7 @@ def test_cpp_shim_on_gpu():
     import subprocess
     from raft_b200 import _build
     root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-    exe = os.path.join(root, "tests", "cpp", "masked_nn_test")
+    exe = str(tmp_path / "masked_nn_test")   # built outside the source tree, which need not be writable
     nvcc = shutil.which("nvcc") or "/usr/local/cuda/bin/nvcc"
     _build.build()
     res = subprocess.run([nvcc, "-std=c++17", "-O1", "-I", os.path.join(root, "include"), "-o", exe,
