@@ -200,14 +200,22 @@ def fused_l2_nn(x, y, sqrt: bool = False, block: int = 4096):
 
 def knn(x, y, n_neighbors: int, metric, block: int = 4096):
     """k nearest rows of y under any metric of pairwise_distance, ascending by (distance, index) -- the
-    composition pairwise_distance + select_k(select_min, sorted) (see knn_l2)."""
+    composition pairwise_distance + select_k(select_min, sorted) (see knn_l2).  Blocked over the columns of y: memory
+    O(m * (n_neighbors + block)).  NaN distances sort after every number (then by index), as in one sort of the row."""
     x64 = np.ascontiguousarray(x, dtype=np.float64)
     y64 = np.ascontiguousarray(y, dtype=np.float64)
     m, n = x64.shape[0], y64.shape[0]
     kk = int(n_neighbors)
-    d = np.concatenate([pairwise_distance(x64, y64[j0:j0 + block], metric) for j0 in range(0, n, block)], axis=1)
-    order = np.lexsort((np.broadcast_to(np.arange(n), d.shape), d), axis=1)[:, :kk]
-    return order.astype(np.int64), np.take_along_axis(d, order, axis=1)
+    best_v = np.empty((m, 0))
+    best_i = np.empty((m, 0), dtype=np.int64)
+    for j0 in range(0, n, block):
+        d = pairwise_distance(x64, y64[j0:j0 + block], metric)
+        v = np.concatenate([best_v, d], axis=1)
+        i = np.concatenate([best_i, np.broadcast_to(np.arange(j0, j0 + d.shape[1], dtype=np.int64), d.shape)], axis=1)
+        order = np.lexsort((i, v), axis=1)[:, :kk]       # primary key: distance, then index
+        best_v = np.take_along_axis(v, order, axis=1)
+        best_i = np.take_along_axis(i, order, axis=1)
+    return best_i, best_v
 
 
 def knn_l2(x, y, n_neighbors: int, sqrt: bool = False, block: int = 4096):

@@ -1115,7 +1115,8 @@ size_t b2d_knn_l2_workspace_bytes(int64_t m, int64_t n, int64_t k, int64_t n_nei
 {
   if (m < 0 || n < 0 || k < 0 || n_neighbors < 1 || n_neighbors > KNN_MAX_K) return static_cast<size_t>(-1);
   return knn_topk_offset(m, n, k) + align_up(static_cast<size_t>(m) * n_neighbors * 8, 1024) +
-         align_up(static_cast<size_t>(m) * 8, 1024) + align_up(static_cast<size_t>(m) * 4, 1024) + 1024;  // + dropmin, dirty list, counters
+         align_up(static_cast<size_t>(m) * 8, 1024) + 3 * align_up(static_cast<size_t>(m) * 4, 1024) +
+         1024;  // + dropmin, dirty list, repaired flags, repaired-row list, counters
 }
 
 namespace {
@@ -1131,6 +1132,10 @@ struct KnnCtx {
   long long* dropmin;   // [m] best key that did not fit into a row's list this pass
   int* dirty;           // [m] rows to redo for the current pass
   unsigned* dirty_cnt;  // [64] one counter per pass
+  unsigned* repaired;   // [m] 1 once a row has been repaired in some pass
+  int* rep_list;        // [m] the repaired rows ...
+  unsigned* rep_cnt;    // ... and their count
+  bool any_fix;         // a knn_fix_kernel was launched
   int pass;
   const float* x; int64_t ldx;
   const float* y; int64_t ldy;
@@ -1154,7 +1159,7 @@ static int knn_pass(KnnCtx& c, int64_t off, int64_t width)
   if (rc) return rc;
   unsigned* dc = c.dirty_cnt + (c.pass & 63);
   knn_merge_kernel<<<static_cast<unsigned>((c.p.m + 7) / 8), 256, 0, c.s>>>(c.topk, c.p.knn_cand, c.cnt, c.thr, c.dropmin, c.dirty,
-                                                                            dc, c.p.m, c.kk);
+                                                                            dc, c.repaired, c.rep_list, c.rep_cnt, c.p.m, c.kk);
   B2D_CUDA(cudaGetLastError());
   if (width > KNN_CAP) {  // (a pass of at most KNN_CAP columns cannot overflow)
     int sms = 0;
@@ -1163,6 +1168,7 @@ static int knn_pass(KnnCtx& c, int64_t off, int64_t width)
     knn_fix_kernel<<<sms * 2, 256, 0, c.s>>>(c.topk, c.thr, c.dirty, dc, c.x, c.ldx, c.y, c.ldy, static_cast<int>(c.k), c.kk, off,
                                              width, c.family, c.center);
     B2D_CUDA(cudaGetLastError());
+    c.any_fix = true;
   }
   ++c.pass;
   return B2D_OK;
@@ -1216,14 +1222,19 @@ int b2d_knn(void* stream, int64_t* out_idx, float* out_dist, int metric, const f
     q += align_up(static_cast<size_t>(m) * 8, 1024);
     c.dirty     = reinterpret_cast<int*>(q);
     q += align_up(static_cast<size_t>(m) * 4, 1024);
+    c.repaired  = reinterpret_cast<unsigned*>(q);
+    q += align_up(static_cast<size_t>(m) * 4, 1024);
+    c.rep_list  = reinterpret_cast<int*>(q);
+    q += align_up(static_cast<size_t>(m) * 4, 1024);
     c.dirty_cnt = reinterpret_cast<unsigned*>(q);
+    c.rep_cnt   = c.dirty_cnt + 64;
   }
-  c.pass = 0; c.x = x; c.ldx = ldx; c.y = y; c.ldy = ldy;
+  c.pass = 0; c.any_fix = false; c.x = x; c.ldx = ldx; c.y = y; c.ldy = ldy;
   c.family = mode == PREP_COSINE ? 1 : 0; c.center = center;
   int rc = launch_prep<float>(s, c.w, x, ldx, 1, m, y, ldy, 1, n, k, nullptr, nullptr, mode, center);
   if (rc) return rc;
   const int64_t total = m * n_neighbors;
-  knn_init_kernel<<<static_cast<unsigned>((std::max<int64_t>(std::max<int64_t>(total, m), 64) + 255) / 256), 256, 0, s>>>(c.topk, c.thr, c.cnt, c.dropmin, c.dirty_cnt, m, c.kk);
+  knn_init_kernel<<<static_cast<unsigned>((std::max<int64_t>(std::max<int64_t>(total, m), 65) + 255) / 256), 256, 0, s>>>(c.topk, c.thr, c.cnt, c.dropmin, c.dirty_cnt, c.repaired, m, c.kk);
   B2D_CUDA(cudaGetLastError());
   memset(&c.p, 0, sizeof(c.p));
   c.p.m = m;
@@ -1237,6 +1248,14 @@ int b2d_knn(void* stream, int64_t* out_idx, float* out_dist, int metric, const f
     rc = knn_pass(c, off, width);
     if (rc) return rc;
     off += width;
+  }
+  if (c.any_fix) {  // every row repaired in some pass: measured again over all n columns, so one arithmetic ranks it
+    int sms = 0;
+    rc = device_sms(&sms);
+    if (rc) return rc;
+    knn_fix_kernel<<<sms * 2, 256, 0, s>>>(c.topk, c.thr, c.rep_list, c.rep_cnt, x, ldx, y, ldy, static_cast<int>(k), c.kk, 0, n,
+                                           c.family, c.center);
+    B2D_CUDA(cudaGetLastError());
   }
   knn_finalize_kernel<<<static_cast<unsigned>((total + 255) / 256), 256, 0, s>>>(out_idx, out_dist, c.topk, total, do_sqrt);
   B2D_CUDA(cudaGetLastError());

@@ -929,20 +929,23 @@ constexpr int KNN_MAX_K = 64;
 constexpr int KNN_CAP   = 128;   // list entries per row and pass
 constexpr int KNN_SORT  = 256;   // KNN_MAX_K + KNN_CAP padded to a power of two
 
-__global__ void knn_init_kernel(long long* topk, float* thr, unsigned* cnt, long long* dropmin, unsigned* dirty_cnt, int64_t m,
-                                int kk)
+__global__ void knn_init_kernel(long long* topk, float* thr, unsigned* cnt, long long* dropmin, unsigned* dirty_cnt,
+                                unsigned* repaired, int64_t m, int kk)
 {
   const int64_t i = static_cast<int64_t>(blockIdx.x) * blockDim.x + threadIdx.x;
-  if (i < 64) dirty_cnt[i] = 0u;   // one counter per pass
-  if (i < m) { thr[i] = __int_as_float(0x7f800000); cnt[i] = 0u; dropmin[i] = KEY_EMPTY; }
+  if (i < 65) dirty_cnt[i] = 0u;   // one counter per pass, then the counter of the repaired-row list
+  if (i < m) { thr[i] = __int_as_float(0x7f800000); cnt[i] = 0u; dropmin[i] = KEY_EMPTY; repaired[i] = 0u; }
   if (i < m * kk) topk[i] = KEY_EMPTY;
 }
 
 // one warp per row: sort (top-k so far) + (this pass's list) by (distance, index), keep the first kk.  A row whose list
 // was full lost entries; that only matters if the best dropped key could still enter the new top-k -- such rows go
-// to the pass's dirty list and knn_fix_kernel redoes them over the pass's columns (no host round trip anywhere).
+// to the pass's dirty list and knn_fix_kernel redoes them over the pass's columns (no host round trip anywhere).  A row
+// dirty for the first time also goes to the repaired-row list (rep_list / rep_cnt, flag repaired[row]), which is measured
+// again over all columns after the last pass.
 __global__ void __launch_bounds__(256) knn_merge_kernel(long long* topk, const long long* cand, unsigned* cnt, float* thr,
-                                                        long long* dropmin, int* dirty, unsigned* dirty_cnt, int64_t m, int kk)
+                                                        long long* dropmin, int* dirty, unsigned* dirty_cnt, unsigned* repaired,
+                                                        int* rep_list, unsigned* rep_cnt, int64_t m, int kk)
 {
   __shared__ long long buf[8][KNN_SORT];
   const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
@@ -979,7 +982,13 @@ __global__ void __launch_bounds__(256) knn_merge_kernel(long long* topk, const l
     const long long kth = b[kk - 1];
     if (kth != KEY_EMPTY) thr[row] = key_dist(kth);
     if (craw > static_cast<unsigned>(KNN_CAP)) {
-      if (dropmin[row] <= kth) dirty[atomicAdd(dirty_cnt, 1u)] = static_cast<int>(row);
+      if (dropmin[row] <= kth) {
+        dirty[atomicAdd(dirty_cnt, 1u)] = static_cast<int>(row);
+        if (!repaired[row]) {   // (one warp owns the row, and the merges of the passes run one after another)
+          repaired[row]                    = 1u;
+          rep_list[atomicAdd(rep_cnt, 1u)] = static_cast<int>(row);
+        }
+      }
       dropmin[row] = KEY_EMPTY;
     }
   }
@@ -990,6 +999,9 @@ __global__ void __launch_bounds__(256) knn_merge_kernel(long long* topk, const l
 // inputs -- family 0: sum (x - y)^2, family 1: 1 - <x', y'> / (|x'||y'|) with x' centred for correlation -- one column per
 // thread, and folds them into the row's top-k (entries this pass had already contributed are taken out first, so no
 // column can appear twice).  Exact for any input order; costs O(width * k) per dirty row, nothing when the list is empty.
+// After the last pass the same kernel measures every repaired row again over all columns (off = 0, width = n): the
+// entries of a repaired row would otherwise come from two arithmetics (tensor and direct), and exact duplicates could
+// then be ranked out of index order.
 __global__ void __launch_bounds__(256) knn_fix_kernel(long long* topk, float* thr, const int* dirty, const unsigned* dirty_cnt,
                                                       const float* x, int64_t ldx, const float* y, int64_t ldy, int k, int kk,
                                                       int64_t off, int64_t width, int family, int center)
@@ -1032,6 +1044,7 @@ __global__ void __launch_bounds__(256) knn_fix_kernel(long long* topk, float* th
       long long kth = 0;
       for (int t = 0; t < kk; ++t) kth = max(kth, keys[t]);
       const int64_t j = j0 + tid;
+      bool appended   = false;
       if (j < width) {
         const float* yr = y + (off + j) * ldy;
         float val;
@@ -1050,10 +1063,14 @@ __global__ void __launch_bounds__(256) knn_fix_kernel(long long* topk, float* th
           val = 1.f - dot / sqrtf(xstat[1] * ny);
         }
         const long long key = key_pack(val, off + j);
-        if (key < kth && val == val) keys[kk + atomicAdd(&ncand, 1u)] = key;   // (kk + 256 <= 320 < 512)
+        if (key < kth && val == val) {   // (kk + 256 <= 320 < 512)
+          keys[kk + atomicAdd(&ncand, 1u)] = key;
+          appended = true;
+        }
       }
-      __syncthreads();
-      if (ncand != 0u) {   // block-wide bitonic sort of the 512 slots, smallest first
+      // the branch must be block-uniform: a thread that read ncand after a barrier could see the next iteration's
+      // atomicAdd of a faster warp, so the decision comes from the barrier itself
+      if (__syncthreads_or(appended)) {   // block-wide bitonic sort of the 512 slots, smallest first
         for (int size = 2; size <= 512; size <<= 1)
           for (int stride = size >> 1; stride > 0; stride >>= 1) {
             const int t = tid;

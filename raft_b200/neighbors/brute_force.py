@@ -22,7 +22,9 @@ def knn(dataset, queries, k=None, indices=None, distances=None, metric="sqeuclid
 
     dataset [n, d] and queries [m, d]: any C-contiguous float32 ``__cuda_array_interface__`` objects.
     ``indices`` / ``distances``: optional preallocated outputs (k is then read from their shape).
-    metric: "sqeuclidean" (squared), "euclidean" / "l2", "cosine" or "correlation" (pylibraft's names)."""
+    metric: "sqeuclidean" (squared), "euclidean" / "l2", "cosine" or "correlation" (pylibraft's names).
+    Rows of ``dataset`` whose distance is NaN (a NaN element, a zero-norm row under cosine) are never returned; a
+    slot without a candidate (a NaN or zero-norm query) gets index -1 and distance +inf, ``global_id_offset`` or not."""
     if metric not in _METRICS:
         raise ValueError("metric %s is not supported by the fused kNN (L2 metrics, cosine, correlation)" % metric)
     d_cai, q_cai = cai_wrapper(dataset), cai_wrapper(queries)
@@ -52,9 +54,9 @@ def knn(dataset, queries, k=None, indices=None, distances=None, metric="sqeuclid
     ws = handle.workspace(need)
     _lib.check(L.b2d_knn(handle.stream_ptr, idx.data_ptr(), dist.data_ptr(), int(resolve_metric(metric)), q_cai.data, dim,
                          d_cai.data, dim, m, n, dim, k, ws.data_ptr(), ws.numel()))
-    if global_id_offset:
+    if global_id_offset:   # a slot without a candidate keeps index -1
         with torch.cuda.stream(handle.torch_stream):
-            idx += int(global_id_offset)
+            idx.copy_(torch.where(idx >= 0, idx + int(global_id_offset), idx))
     for out, res in ((indices, idx), (distances, dist)):
         if out is not None:
             o = cai_wrapper(out)

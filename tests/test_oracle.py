@@ -131,6 +131,26 @@ def test_knn_oracle_against_brute_force_sort():
     gi1, gv1 = oracle.knn_l2(x, y, 1)
     ni, nv = oracle.fused_l2_nn(x, y)
     assert (gi1[:, 0] == ni).all() and np.allclose(gv1[:, 0], nv)
+    # oracle.knn (any metric, blocked per 'block' columns) == one sort of the whole row, ties and NaN rows included
+    y[33] = np.nan                                         # NaN distances: after every number
+    y[150] = 0.0                                           # zero norm: NaN under the cosine family
+    x[5] = np.nan                                          # a row of NaN distances: index order
+    for mt in (oracle.DistanceType.L2Expanded, oracle.DistanceType.L2SqrtExpanded, oracle.DistanceType.CosineExpanded,
+               oracle.DistanceType.CorrelationExpanded):
+        d = oracle.pairwise_distance(x, y, mt)
+        order = np.lexsort((np.broadcast_to(np.arange(211), d.shape), d), axis=1)
+        for kk, block in ((13, 64), (13, 4096), (1, 50), (211, 100)):
+            gi, gv = oracle.knn(x, y, kk, mt, block=block)
+            assert gi.dtype == np.int64 and gi.shape == (37, kk)
+            assert (gi == order[:, :kk]).all(), (mt, kk, block)
+            want = np.take_along_axis(d, order[:, :kk], axis=1)
+            if block >= 211:   # the same pairwise_distance call as the whole row: bit-identical
+                assert np.array_equal(gv, want, equal_nan=True)
+            assert np.allclose(gv, want, rtol=1e-12, atol=1e-12, equal_nan=True)
+        assert (np.delete(order, 5, axis=0)[:, :209] != 33).all() and (order[5] == np.arange(211)).all()
+    gi, gv = oracle.knn(x, y, 13, oracle.DistanceType.L2Expanded, block=64)
+    ri, rv = oracle.knn_l2(x, y, 13, block=64)
+    assert (gi[x[:, 0] == x[:, 0]] == ri[x[:, 0] == x[:, 0]]).all()
 
 
 def test_silhouette_oracle_pinned_to_sklearn():
