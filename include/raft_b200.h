@@ -20,6 +20,9 @@
  *                              cpp/include/raft/comms/detail/std_comms.hpp:365-374)
  *   b2d_row_norm               raft::linalg::rowNorm / norm<ALONG_ROWS>
  *                              cpp/include/raft/linalg/norm.cuh:50-58,118-147
+ *   b2d_select_k               raft::matrix::select_k(handle, in_val, in_idx, out_val, out_idx, select_min,
+ *                              sorted, algo), cpp/include/raft/matrix/select_k.cuh:72-106: exact per-row
+ *                              top-k, the selection step after pairwise_distance in a brute-force kNN
  *
  * Conventions (same as the reference's, cpp/docs developer_guide.md:396-433): every call only
  * enqueues work on `stream` (a cudaStream_t passed as void*), never synchronises, never
@@ -232,6 +235,18 @@ int b2d_row_norm(void* stream, float* out, const float* x, int64_t ldx, int64_t 
  * value below +inf (all NaN / +inf) -> 0.  The separate-pass form of the arg-min that fusedL2NN fuses (SURVEY.md a9);
  * one read of the matrix. */
 int b2d_row_argmin(void* stream, int32_t* out, const float* in, int64_t ld, int64_t rows, int64_t n);
+
+/* raft::matrix::select_k (cpp/include/raft/matrix/select_k.cuh:72-106): for every row r of in_val:[rows,len] (row pitch
+ * ld), out_val[r, 0..k) / out_idx[r, 0..k) = the k smallest (select_min != 0) or largest values and their columns, or
+ * in_idx[r, column] when in_idx (int64, same pitch) is given.  Order: the float order with -0.0 == +0.0 and every NaN
+ * above +inf (so NaNs come first in a max selection, last in a min selection); among equal values the smaller column
+ * wins.  Every row is written sorted, best first, equal values in ascending column order.  The values are the input
+ * bits unchanged (-0.0 stays -0.0, a NaN keeps its payload).  1 <= k <= len (else B2D_ERR_INVALID_ARG); rows, len <
+ * 2^31 (else B2D_ERR_UNSUPPORTED); rows == 0 does nothing.  Exact radix selection on the (value, column) order
+ * (DESIGN.md K9).  The workspace query returns SIZE_MAX for invalid extents. */
+size_t b2d_select_k_workspace_bytes(int64_t rows, int64_t len, int64_t k);
+int b2d_select_k(void* stream, const float* in_val, int64_t ld, const int64_t* in_idx, int64_t rows, int64_t len, int64_t k,
+                 int select_min, float* out_val, int64_t* out_idx, void* workspace, size_t workspace_bytes);
 
 #ifdef __cplusplus
 }

@@ -11,6 +11,7 @@
 #include <string>
 #include <vector>
 #include <cub/device/device_radix_sort.cuh>
+#include <cub/device/device_segmented_radix_sort.cuh>
 
 #include "../../include/raft_b200.h"
 #include "expanded_tc.cuh"
@@ -20,6 +21,7 @@
 #include "unexpanded_simt.cuh"
 #include "stats.cuh"
 #include "fp64_simt.cuh"
+#include "select_k.cuh"
 
 namespace b2d {
 
@@ -534,6 +536,84 @@ static int pairwise_f64(cudaStream_t s, int metric, const double* x, int64_t xrs
     default: return fail(B2D_ERR_UNSUPPORTED, "metric");
   }
 }
+
+// ------------------------------------------------------------------------------------------
+// select_k (select_k.cuh): the layout is a function of the shape alone
+namespace {
+enum { SK_SORT_ROW = 0, SK_RADIX_ROW = 1, SK_SPLIT = 2 };
+constexpr int64_t kSkSplitRows = 264;        // fewer rows than two CTAs per SM of an H100 SXM (132 SMs): split each row
+constexpr int64_t kSkMinChunk  = 32768;      // columns per CTA of a split row, at least
+constexpr size_t kSkCubTmp     = 1u << 20;   // cub::DeviceSegmentedRadixSort scratch (checked at run time)
+constexpr int64_t kSkCubItems  = 1ll << 30;  // words per segmented sort call
+
+struct SkPlan {
+  int layout    = SK_SORT_ROW;
+  int64_t chunk = 0, chunks = 1;   // SK_SPLIT: columns per CTA, CTAs per row
+  bool list     = false;           // the k words of every row go through the workspace
+  bool cub      = false;           // ... and are sorted there by cub (k > kSkSortMax)
+  int sort_n    = 0;               // power-of-two size of the shared-memory sort
+  int cap       = 0;               // SK_RADIX_ROW: live words the row kernel's buffer holds
+  int64_t batch = 0;               // rows per segmented sort call
+};
+
+static SkPlan sk_plan(int64_t rows, int64_t len, int64_t k)
+{
+  SkPlan p;
+  if (len <= kSkRowSort) {
+    p.sort_n = sk_pow2(len);
+    return p;
+  }
+  const int64_t chunks = std::min((len + kSkMinChunk - 1) / kSkMinChunk, (kSkSplitRows + rows - 1) / rows);
+  p.layout = chunks > 1 ? SK_SPLIT : SK_RADIX_ROW;
+  p.cub    = k > kSkSortMax;
+  p.list   = p.layout == SK_SPLIT || p.cub;
+  p.sort_n = p.cub ? 0 : sk_pow2(k);
+  if (p.layout == SK_SPLIT) {
+    p.chunk  = ((len + chunks - 1) / chunks + 3) / 4 * 4;
+    p.chunks = (len + p.chunk - 1) / p.chunk;
+  } else {
+    p.cap = static_cast<int>((kSkRowSmem - kSkBuckets * 4 - (p.list ? 0 : p.sort_n * 8)) / 8);
+  }
+  if (p.cub) p.batch = std::min(rows, std::max<int64_t>(1, kSkCubItems / k));
+  return p;
+}
+
+struct SkLayout {
+  SkState* st    = nullptr;
+  uint32_t* hist = nullptr;
+  uint64_t* list = nullptr;
+  uint64_t* alt  = nullptr;
+  int* off       = nullptr;
+  void* tmp      = nullptr;
+  size_t bytes   = 0;
+};
+
+static SkLayout sk_layout(void* base, const SkPlan& p, int64_t rows, int64_t k)
+{
+  SkLayout w;
+  auto take = [&](size_t b) {
+    char* at = base ? static_cast<char*>(base) + w.bytes : nullptr;
+    w.bytes  = align_up(w.bytes + b, 256);
+    return at;
+  };
+  if (p.layout == SK_SPLIT) {
+    w.st   = reinterpret_cast<SkState*>(take(static_cast<size_t>(rows) * sizeof(SkState)));
+    w.hist = reinterpret_cast<uint32_t*>(take(static_cast<size_t>(rows) * kSkBuckets * 4));
+  }
+  if (p.list) w.list = reinterpret_cast<uint64_t*>(take(static_cast<size_t>(rows) * k * 8));
+  if (p.cub) {
+    w.alt = reinterpret_cast<uint64_t*>(take(static_cast<size_t>(p.batch) * k * 8));
+    w.off = reinterpret_cast<int*>(take(static_cast<size_t>(p.batch + 1) * 4));
+    w.tmp = take(kSkCubTmp);
+  }
+  return w;
+}
+
+static bool sk_extents_ok(int64_t rows, int64_t len, int64_t k)
+{
+  return rows >= 0 && rows <= 0x7fffffffll && k >= 1 && k <= len && len <= 0x7fffffffll;
+}
+}  // namespace
 
 extern "C" {
 
@@ -1464,6 +1544,77 @@ int b2d_row_norm(void* stream, float* out, const float* x, int64_t ldx, int64_t 
   row_norm_kernel<<<static_cast<unsigned>((rows + 7) / 8), 256, 0, s>>>(out, x, ldx, rows, static_cast<int>(k),
                                                                         norm_type, do_sqrt);
   B2D_CUDA(cudaGetLastError());
+  return B2D_OK;
+}
+
+size_t b2d_select_k_workspace_bytes(int64_t rows, int64_t len, int64_t k)
+{
+  if (!sk_extents_ok(rows, len, k)) return SIZE_MAX;
+  if (rows == 0) return 0;
+  return sk_layout(nullptr, sk_plan(rows, len, k), rows, k).bytes;
+}
+
+int b2d_select_k(void* stream, const float* in_val, int64_t ld, const int64_t* in_idx, int64_t rows, int64_t len, int64_t k,
+                 int select_min, float* out_val, int64_t* out_idx, void* workspace, size_t workspace_bytes)
+{
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  if (rows < 0 || len < 0) return fail(B2D_ERR_INVALID_ARG, "bad extents");
+  if (k < 1 || k > len) return fail(B2D_ERR_INVALID_ARG, "k must be in [1, len]");
+  if (len > 0x7fffffffll || rows > 0x7fffffffll) return fail(B2D_ERR_UNSUPPORTED, "rows and len must be below 2^31");
+  if (ld < len) return fail(B2D_ERR_INVALID_ARG, "ld < len");
+  if (rows == 0) return B2D_OK;
+  if (!in_val || !out_val || !out_idx) return fail(B2D_ERR_INVALID_ARG, "null in_val / out_val / out_idx");
+  const bool mn    = select_min != 0;
+  const SkPlan p   = sk_plan(rows, len, k);
+  const size_t need = sk_layout(nullptr, p, rows, k).bytes;
+  if (need && (!workspace || workspace_bytes < need))
+    return fail(B2D_ERR_WORKSPACE, "workspace too small: need " + std::to_string(need) + " bytes");
+  if (reinterpret_cast<uintptr_t>(workspace) % 256) return fail(B2D_ERR_INVALID_ARG, "workspace must be 256-byte aligned");
+  const SkLayout w = sk_layout(workspace, p, rows, k);
+  const unsigned R = static_cast<unsigned>(rows);
+  if (p.layout == SK_SORT_ROW) {
+    const int threads = std::max(32, std::min(512, p.sort_n / 2));
+    select_k_sort_row_kernel<<<R, threads, p.sort_n * 8, s>>>(in_val, ld, len, k, mn, in_idx, out_val, out_idx, p.sort_n);
+    B2D_CUDA(cudaGetLastError());
+    return B2D_OK;
+  }
+  if (p.layout == SK_RADIX_ROW) {
+    B2D_CUDA(cudaFuncSetAttribute(select_k_radix_row_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kSkRowSmem));
+    select_k_radix_row_kernel<<<R, kSkThreads, kSkRowSmem, s>>>(in_val, ld, len, k, mn, in_idx, out_val, out_idx,
+                                                                 p.list ? 0 : p.sort_n, p.cap, w.list);
+  } else {
+    B2D_CUDA(cudaMemsetAsync(w.st, 0, static_cast<size_t>(rows) * sizeof(SkState), s));
+    B2D_CUDA(cudaMemsetAsync(w.hist, 0, static_cast<size_t>(rows) * kSkBuckets * 4, s));
+    const dim3 grid(static_cast<unsigned>(p.chunks), R);
+    for (int pass = 0; pass <= kSkPasses; ++pass) {
+      select_k_split_read_kernel<<<grid, kSkThreads, 0, s>>>(in_val, ld, len, p.chunk, k, mn, w.st, w.hist, w.list, pass);
+      if (pass < kSkPasses) select_k_split_scan_kernel<<<R, kSkThreads, 0, s>>>(w.st, w.hist, k, pass);
+    }
+  }
+  B2D_CUDA(cudaGetLastError());
+  if (!p.list) return B2D_OK;
+  if (!p.cub) {
+    select_k_sort_list_kernel<<<R, kSkThreads, p.sort_n * 8, s>>>(w.list, in_val, ld, k, in_idx, out_val, out_idx, p.sort_n);
+    B2D_CUDA(cudaGetLastError());
+    return B2D_OK;
+  }
+  select_k_offsets_kernel<<<static_cast<unsigned>((p.batch + 256) / 256), 256, 0, s>>>(w.off, p.batch, k);
+  B2D_CUDA(cudaGetLastError());
+  for (int64_t r0 = 0; r0 < rows; r0 += p.batch) {
+    const int64_t nb = std::min(p.batch, rows - r0);
+    cub::DoubleBuffer<unsigned long long> db(reinterpret_cast<unsigned long long*>(w.list + r0 * k),
+                                             reinterpret_cast<unsigned long long*>(w.alt));
+    size_t tmp_need = 0;
+    B2D_CUDA(cub::DeviceSegmentedRadixSort::SortKeys(nullptr, tmp_need, db, static_cast<int>(nb * k), static_cast<int>(nb),
+                                                     w.off, w.off + 1, 0, 64, s));
+    if (tmp_need > kSkCubTmp)
+      return fail(B2D_ERR_WORKSPACE, "internal: segmented sort scratch " + std::to_string(tmp_need) + " bytes");
+    B2D_CUDA(cub::DeviceSegmentedRadixSort::SortKeys(w.tmp, tmp_need, db, static_cast<int>(nb * k), static_cast<int>(nb),
+                                                     w.off, w.off + 1, 0, 64, s));
+    select_k_gather_kernel<<<static_cast<unsigned>((nb * k + 255) / 256), 256, 0, s>>>(
+      reinterpret_cast<const uint64_t*>(db.Current()), in_val, ld, k, in_idx, out_val, out_idx, r0, nb);
+    B2D_CUDA(cudaGetLastError());
+  }
   return B2D_OK;
 }
 

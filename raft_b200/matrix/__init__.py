@@ -1,4 +1,5 @@
-"""raft::matrix::argmin -- the separate-pass row arg-min (cpp/include/raft/matrix/argmin.cuh:25-37), SURVEY.md 8(a9)."""
+"""raft::matrix::argmin -- the separate-pass row arg-min (cpp/include/raft/matrix/argmin.cuh:25-37), SURVEY.md 8(a9) --
+and raft::matrix::select_k, the exact per-row top-k (select_k.py)."""
 from __future__ import annotations
 
 import numpy as np
@@ -6,6 +7,7 @@ import torch
 
 from .. import _lib
 from ..common import auto_sync_handle, cai_wrapper
+from .select_k import select_k  # noqa: F401
 
 
 @auto_sync_handle
