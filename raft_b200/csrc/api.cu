@@ -324,7 +324,8 @@ static int launch_tc(cudaStream_t s, const TcWorkspace& w, TcParams p, int64_t k
   if (p.n_items == 0) return B2D_OK;
   const bool resident = p.nkb <= TC_MAX_RES_KB;
   CUtensorMap ma, mb;
-  rc = make_operand_map(&ma, w.xop, p.m, p.nkb, TC_BM, kb0, nkb_total);
+  // resident: each consumer warpgroup's ring takes the 64-row slab of an x tile it multiplies; streaming: whole tiles
+  rc = make_operand_map(&ma, w.xop, p.m, p.nkb, resident ? TC_BM / 2 : TC_BM, kb0, nkb_total);
   if (rc) return rc;
   // resident: the whole 256-row y block in one box per k-block; streaming: one 128-row half per stage
   rc = make_operand_map(&mb, w.yop, p.n, p.nkb, resident ? TC_BN : TC_HN, kb0, nkb_total);

@@ -16,7 +16,7 @@
 // Operands that are exact in fp16 (fp16 inputs, small integers) skip the cross terms altogether.
 //
 // Structure (one persistent CTA per SM, 384 threads = 3 warpgroups):
-//   warpgroup 0     TMA producer: warp 0, one elected lane issues cp.async.bulk.tensor 2-D loads
+//   warpgroup 0     TMA producer: one elected lane per feeding warp issues cp.async.bulk.tensor 2-D loads
 //                   (SWIZZLE_128B, mbarrier complete_tx); the other warps only hand their registers over
 //   warpgroups 1-2  consumers: warpgroup c owns rows [64c, 64c+64) of every x tile; it issues the
 //                   wgmma.m64n128k16 of its rows and runs the epilogue on the accumulator fragments
@@ -25,8 +25,10 @@
 // 64 x 128 warpgroup tile are 128 fp32 registers per thread.
 //
 //  kResident (k <= 128): the y block (all of K, <= 128 KB) stays in shared memory for the whole run;
-//    x k-blocks stream through a ring of 16 KB stages, loaded once per tile: both halves read them, the
-//    last half releases them (the ring holds a whole tile, so it wraps across tiles when nkb < stages).
+//    each consumer warpgroup has an x ring of its own (64-row k-blocks of its slab, fed by producer warp c), loaded once
+//    per tile: both halves read them, the last half releases them (a ring holds a whole tile, so it wraps across tiles
+//    when nkb < stages).  The two warpgroups take turns issuing their MMAs (named barriers 4 and 5), so one
+//    warpgroup's epilogue runs while the other's MMAs do.
 //  !kResident (k > 128): both operands stream per k-block (stages of 16 KB of x + 16 KB of the y half).
 //
 // Epilogues (straight from the registers; d = acc * c + (t_x[i] + t_y[j]), c one scalar):
@@ -152,10 +154,16 @@ static_assert((size_t)TC_STAGES_STR * (TC_A_BYTES + TC_BH_BYTES) <= TC_SMEM_OPER
 // Shared-memory carve of one instantiation: [resident y block][x (+ y half) stages][output staging][t_y][barriers].
 // The arg-min / top-k epilogues store nothing and keep 208 KB of operands; EPI_STORE trades one x stage for 32 KB of
 // output staging (the streaming variant fits it beside all of its stages).
+// x rings: streaming, one ring of `stages` stages that both consumer warpgroups read.  Resident, one ring of `stages`
+// 64-row k-blocks (8 KB) per consumer warpgroup, laid out in the same bytes: slot s of ring w is the 8 KB at w * 8 KB of
+// the 16 KB stage s, and every ring has full / empty mbarriers of its own.
+// mbarriers (after t_y): afull[rings * TC_MAX_STAGES], aempty[rings * TC_MAX_STAGES] (slot s of ring w at rings * s + w),
+// bfull[TC_MAX_RES_KB], bempty[TC_MAX_RES_KB].
 template <bool kResident, int kEpi>
 struct TcCarve {
   static constexpr int stages = kEpi == EPI_STORE ? (kResident ? TC_STAGES_RES_ST : TC_STAGES_STR_ST)
                                                   : (kResident ? TC_STAGES_RES : TC_STAGES_STR);
+  static constexpr int rings  = kResident ? 2 : 1;
   static constexpr uint32_t stage_bytes = kResident ? TC_A_BYTES : TC_A_BYTES + TC_BH_BYTES;
   static constexpr size_t a_off   = kResident ? (size_t)TC_MAX_RES_KB * TC_B_BYTES : 0;
   static constexpr size_t stg_off = a_off + (size_t)stages * stage_bytes;
@@ -163,6 +171,8 @@ struct TcCarve {
   static constexpr size_t grp_off = tb_off + TC_BN * 4 + 256;   // EPI_MINLOC_MASKED: [256] group of every column
   static constexpr size_t bytes   = grp_off + (kEpi == EPI_MINLOC_MASKED ? TC_BN * 4 : 0);
   static_assert(stages <= TC_MAX_STAGES, "barrier arrays hold TC_MAX_STAGES stages");
+  static_assert((2 * rings * TC_MAX_STAGES + 2 * TC_MAX_RES_KB) * 8 <= grp_off - tb_off - TC_BN * 4,
+                "the mbarriers of every ring fit in the 256 bytes after t_y");
   static_assert(!kResident || stages >= TC_MAX_RES_KB, "resident: the ring holds every x k-block of a tile (both halves read them)");
   static_assert(stg_off % 1024 == 0, "SWIZZLE_128B staging boxes need 1024-byte alignment");
   static_assert(kEpi == EPI_STORE || stg_off <= TC_SMEM_OPERANDS, "operands fit");
@@ -528,17 +538,18 @@ expanded_tc_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_cons
   float* col_tb   = reinterpret_cast<float*>(smem + Carve::tb_off);  // [256] t_y of this y block
   int* col_grp    = reinterpret_cast<int*>(smem + Carve::grp_off);  // masked: [256] group of every column of the y block
   uint64_t* bars  = reinterpret_cast<uint64_t*>(col_tb + TC_BN);
-  uint64_t* afull = bars;                       // [TC_MAX_STAGES]
-  uint64_t* aempty = bars + TC_MAX_STAGES;      // [TC_MAX_STAGES]
-  uint64_t* bfull = bars + 2 * TC_MAX_STAGES;   // [TC_MAX_RES_KB]
-  uint64_t* bempty = bfull + TC_MAX_RES_KB;     // [TC_MAX_RES_KB]
+  constexpr int kRings = Carve::rings;
+  uint64_t* afull  = bars;                               // [kRings * TC_MAX_STAGES]: slot s of ring w at kRings * s + w
+  uint64_t* aempty = bars + kRings * TC_MAX_STAGES;      // [kRings * TC_MAX_STAGES]
+  uint64_t* bfull  = bars + 2 * kRings * TC_MAX_STAGES;  // [TC_MAX_RES_KB]
+  uint64_t* bempty = bfull + TC_MAX_RES_KB;              // [TC_MAX_RES_KB]
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
 
   if (threadIdx.x == 0) {
-    // empty barriers: one arrival per consumer warpgroup
-    for (int i = 0; i < TC_MAX_STAGES; ++i) { ptx::mbar_init(&afull[i], 1); ptx::mbar_init(&aempty[i], 2); }
+    // empty barriers: one arrival per consumer warpgroup that reads the ring (resident: its own ring; streaming: both)
+    for (int i = 0; i < kRings * TC_MAX_STAGES; ++i) { ptx::mbar_init(&afull[i], 1); ptx::mbar_init(&aempty[i], kResident ? 1 : 2); }
     for (int i = 0; i < TC_MAX_RES_KB; ++i) { ptx::mbar_init(&bfull[i], 1); ptx::mbar_init(&bempty[i], 2); }
     ptx::fence_mbar_init();
     ptx::prefetch_tmap(&tmap_a);
@@ -552,13 +563,17 @@ expanded_tc_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_cons
   if (warp < 4) {
     // ================================ TMA producer =================================
     asm volatile("setmaxnreg.dec.sync.aligned.u32 40;");
-    if (warp != 0) return;
+    // resident: warp w feeds ring w with the 64-row slab w of every x tile (both walk the same load order), and warp 0
+    // alone loads the y block; streaming: warp 0 feeds the one ring
+    if (warp >= kRings) return;
     // The whole warp runs the loop with warp-uniform values and one elected lane issues (inside a divergent
     // `if (lane == 0)` the compiler cannot keep descriptors / barrier addresses in uniform registers).
     const uint64_t pol = ptx::policy_evict_last();
+    const int ring     = kResident ? warp : 0;
     tc_producer_walk<kResident, kMasked>(
         p, nkb, blockIdx.x, gridDim.x,
         [&](int kb, uint32_t it_local, const TcItem& t) {
+          if (warp != 0) return;
           ptx::mbar_wait(&bempty[kb], (it_local & 1) ^ 1);
           if (ptx::elect_one()) {
             ptx::mbar_expect_tx(&bfull[kb], TC_B_BYTES);
@@ -567,10 +582,12 @@ expanded_tc_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_cons
         },
         [&](uint32_t a_it, const TcItem& t, int mt, int h, int kb) {
           const uint32_t s = a_it % kStages, ph = (a_it / kStages) & 1;
-          ptx::mbar_wait(&aempty[s], ph ^ 1);
+          ptx::mbar_wait(&aempty[kRings * s + ring], ph ^ 1);
           if (ptx::elect_one()) {
-            ptx::mbar_expect_tx(&afull[s], kStageBytes);
-            ptx::tma_load_2d(a_base + s * kStageBytes, &tmap_a, &afull[s], kb * 64, mt * TC_BM, pol);
+            // resident: the ring's 64-row slab of the tile (the x tensor map has 64-row boxes then)
+            ptx::mbar_expect_tx(&afull[kRings * s + ring], kResident ? TC_A_BYTES / 2 : kStageBytes);
+            ptx::tma_load_2d(a_base + s * kStageBytes + ring * (TC_A_BYTES / 2), &tmap_a, &afull[kRings * s + ring], kb * 64,
+                             mt * TC_BM + 64 * ring, pol);
             if (!kResident)
               ptx::tma_load_2d(a_base + s * kStageBytes + TC_A_BYTES, &tmap_b, &afull[s], kb * 64,
                                t.n_blk * TC_BN + h * TC_HN, pol);
@@ -592,6 +609,17 @@ expanded_tc_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_cons
   // rows with their own exponent (prep.cuh): per-row factor on x (one multiply per row and tile), per-column factor on y
   // only when some row of y has one (rare; read straight from global memory then)
   const bool xnu = __ldg(&p.nonuni[0]) != 0u, ynu = __ldg(&p.nonuni[1]) != 0u;
+  // the x ring this warpgroup reads: resident, its own (its rows of every stage); streaming, the one both read
+  const int ring = kResident ? wg : 0;
+  // Resident: ordered MMA turns.  Both warpgroups walk the same (item, tile, half) units; warpgroup w takes its turn at
+  // named barrier 4 + w before a unit's first wgmma and passes it (bar.arrive on the other's barrier) after the unit's
+  // last commit, so one warpgroup's epilogue runs under the other's MMAs.  Warpgroup 0 takes the first turn; a unit
+  // without MMAs (a masked NONE half) still takes and passes it, so the counts always match.  After its last item,
+  // warpgroup 0 takes the turn warpgroup 1 passed last, so every arrival is matched (every CTA has an item: grid <=
+  // n_items).  (Constant barrier ids: no register holds them.)
+  auto take_turn = [&] { if (wg == 0) ptx::bar_sync(4, 256); else ptx::bar_sync(5, 256); };
+  auto pass_turn = [&] { if (wg == 0) ptx::bar_arrive(5, 256); else ptx::bar_arrive(4, 256); };
+  if (kResident && wg == 1) ptx::bar_arrive(4, 256);
   uint32_t a_it = 0, it_local = 0;
   float acc[64], crs[64];
   for (int64_t item = blockIdx.x; item < p.n_items; item += gridDim.x, ++it_local) {
@@ -604,7 +632,11 @@ expanded_tc_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_cons
     if constexpr (kMasked) {
       cls     = p.mask_cls + static_cast<int64_t>(n_blk) * p.tiles_m;
       mt_last = mask_mt_last(cls, mt0, mt1);
-      if (mt_last < 0) { --it_local; continue; }
+      if (mt_last < 0) {
+        if (kResident && wg == 0 && item + gridDim.x >= p.n_items) take_turn();   // warpgroup 1's last pass
+        --it_local;
+        continue;
+      }
     }
     bool b_first = true;   // masked: this warpgroup has not waited for the item's y block yet
     // per-column epilogue terms of this y block (shared by every tile of the item)
@@ -658,14 +690,18 @@ expanded_tc_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_cons
             // still waiting when the lead handed the stage back could find it refilled, its barrier two phases on, and
             // wait forever.  One stage at a time: a streamed half has more k-blocks (k > 192) than the ring has stages,
             // so holding them all before handing any back would starve the producer.  (Barrier 2 + wg is free here:
-            // only EPI_STORE uses it.)
+            // only EPI_STORE uses it.)  Resident, the half still takes and passes its MMA turn.
+            if (kResident) {
+              take_turn();
+              pass_turn();
+            }
             if (!mask_half_loaded(kResident, tcls, h)) continue;
             if (tc_half_releases(kResident, h, nh)) {
               for (int kb = 0; kb < nkb; ++kb) {
                 const uint32_t it = a_it + kb;
-                ptx::mbar_wait(&afull[it % kStages], (it / kStages) & 1);
+                ptx::mbar_wait(&afull[kRings * (it % kStages) + ring], (it / kStages) & 1);
                 ptx::bar_sync(2 + wg, 128);
-                if (lead) ptx::mbar_arrive(&aempty[it % kStages]);
+                if (lead) ptx::mbar_arrive(&aempty[kRings * (it % kStages) + ring]);
               }
               if (kResident && lead && mt == mt_last)
                 for (int kb = 0; kb < nkb; ++kb) ptx::mbar_arrive(&bempty[kb]);
@@ -683,14 +719,16 @@ expanded_tc_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_cons
         // (the rule of tc_half_releases, written out: through the call the resident instantiations schedule differently)
         const bool release = !kResident || h == nh - 1;
         const uint32_t it0 = a_it;
+        if (kResident) take_turn();   // this unit's MMA turn
         // descriptor start-address units are 16 B; inside the 128-B swizzled row of a k-block:
         //   hi k[0,16) +0, hi k[16,32) +2, lo k[0,16) +4, lo k[16,32) +6
         for (int kb = 0; kb < nkb; ++kb) {
           const uint32_t it = it0 + kb;
           const uint32_t s = it % kStages, ph = (it / kStages) & 1;
-          // (the first MMAs of the item on the resident y block wait for it)
+          // (the first MMAs of the item on the resident y block wait for it; the other warpgroup has passed the turn,
+          // so its hand-back of the previous y block does not wait on this one)
           if (kResident && (kMasked ? b_first : (mt == mt0 && h == 0))) ptx::mbar_wait(&bfull[kb], it_local & 1);
-          ptx::mbar_wait(&afull[s], ph);
+          ptx::mbar_wait(&afull[kRings * s + ring], ph);
           const uint64_t da = ptx::gmma_desc_sw128(ptx::smem_u32(a_base + s * kStageBytes) + wg * 64 * 128);
           const uint64_t db = ptx::gmma_desc_sw128(kResident ? ptx::smem_u32(b_base + kb * TC_B_BYTES) + h * TC_BH_BYTES
                                                              : ptx::smem_u32(a_base + s * kStageBytes + TC_A_BYTES));
@@ -709,10 +747,24 @@ expanded_tc_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_cons
           ptx::wgmma_commit();
           ptx::fence_regs(acc);
           ptx::fence_regs(crs);
-          if (release && kb > 0) {  // the previous k-block's MMAs have finished reading their stage: hand it back
+          if (!kResident && release && kb > 0) {  // the previous k-block's MMAs have finished reading their stage: hand it back
             ptx::wgmma_wait<1>();
-            if (lead) ptx::mbar_arrive(&aempty[(it - 1) % kStages]);
+            if (lead) ptx::mbar_arrive(&aempty[kRings * ((it - 1) % kStages) + ring]);
           }
+        }
+        if (kResident) {
+          // Every MMA of the unit is issued without waiting on any of them: the other warpgroup's turn.  Then the
+          // stages go back as the MMAs that read them finish (k-block kb's group is done once at most nkb - 1 - kb
+          // groups are pending; the last one after the wait for all).
+          pass_turn();
+          if (release)
+            for (int kb = 0; kb + 1 < nkb; ++kb) {
+              const int pending = nkb - 1 - kb;
+              if (pending >= 3) ptx::wgmma_wait<3>();
+              else if (pending == 2) ptx::wgmma_wait<2>();
+              else ptx::wgmma_wait<1>();
+              if (lead) ptx::mbar_arrive(&aempty[kRings * ((it0 + kb) % kStages) + ring]);
+            }
         }
         ptx::wgmma_wait<0>();
         ptx::fence_regs(acc);
@@ -721,7 +773,7 @@ expanded_tc_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_cons
         if (release) {
           a_it = it0 + nkb;
           if (lead) {
-            ptx::mbar_arrive(&aempty[(a_it - 1) % kStages]);
+            ptx::mbar_arrive(&aempty[kRings * ((a_it - 1) % kStages) + ring]);
             if (kResident && mt == (kMasked ? mt_last : mt1 - 1) && h == nh - 1)   // the item's last MMAs on the y block are done
               for (int kb = 0; kb < nkb; ++kb) ptx::mbar_arrive(&bempty[kb]);
           }
@@ -739,6 +791,7 @@ expanded_tc_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_cons
                          static_cast<int64_t>(mt) * TC_BM + 64 * wg, static_cast<int64_t>(n_blk) * TC_BN + h * TC_HN, p);
       }
     }
+    if (kResident && wg == 0 && item + gridDim.x >= p.n_items) take_turn();   // warpgroup 1's last pass
   }
 }
 
