@@ -7,8 +7,11 @@
 //       behind the kernels the call enqueued, exactly like the reference's own temporaries;
 //   stand-alone: cudaMallocAsync / cudaFreeAsync on the same stream (the default pool keeps the memory, so the
 //       steady state costs no driver call).
+// Entry points without a handle (epsUnexpL2SqNeighborhood) take the stand-alone way on their stream in either build.
 // Either way nothing synchronises and the scratch lives until the work enqueued so far has run.
 #pragma once
+#include <optional>
+
 #include "b200_compat.hpp"
 #ifdef RAFT_B200_USE_REAL_RAFT
 #include <raft/core/resource/device_memory_resource.hpp>
@@ -22,12 +25,18 @@ class scoped_workspace {
  public:
 #ifdef RAFT_B200_USE_REAL_RAFT
   scoped_workspace(raft::resources const& handle, std::size_t bytes)
-    : buf_(bytes + 256, raft::resource::get_cuda_stream(handle), raft::resource::get_workspace_resource_ref(handle))
+  {
+    buf_.emplace(bytes + 256, raft::resource::get_cuda_stream(handle), raft::resource::get_workspace_resource_ref(handle));
+  }
+#else
+  scoped_workspace(raft::resources const& handle, std::size_t bytes)
+    : scoped_workspace(raft::resource::get_cuda_stream(handle), bytes)
   {
   }
-  void* data() { return align(buf_.data()); }
-#else
-  scoped_workspace(raft::resources const& handle, std::size_t bytes) : stream_(raft::resource::get_cuda_stream(handle))
+#endif
+  // entry points that take a stream and no handle (the reference's pointer forms): cudaMallocAsync / cudaFreeAsync on
+  // that stream, in either build
+  scoped_workspace(cudaStream_t stream, std::size_t bytes) : stream_(stream)
   {
     if (bytes && cudaMallocAsync(&p_, bytes + 256, stream_) != cudaSuccess)
       throw raft::cuda_error("raft_b200: workspace allocation failed");
@@ -36,8 +45,13 @@ class scoped_workspace {
   {
     if (p_) cudaFreeAsync(p_, stream_);
   }
-  void* data() { return align(p_); }
+  void* data()
+  {
+#ifdef RAFT_B200_USE_REAL_RAFT
+    if (buf_) return align(buf_->data());
 #endif
+    return align(p_);
+  }
   scoped_workspace(const scoped_workspace&)            = delete;
   scoped_workspace& operator=(const scoped_workspace&) = delete;
 
@@ -46,11 +60,10 @@ class scoped_workspace {
   {
     return reinterpret_cast<void*>((reinterpret_cast<std::uintptr_t>(p) + 255) & ~static_cast<std::uintptr_t>(255));
   }
+  cudaStream_t stream_ = nullptr;
+  void* p_             = nullptr;
 #ifdef RAFT_B200_USE_REAL_RAFT
-  rmm::device_uvector<char> buf_;
-#else
-  cudaStream_t stream_;
-  void* p_ = nullptr;
+  std::optional<rmm::device_uvector<char>> buf_;
 #endif
 };
 

@@ -248,6 +248,28 @@ size_t b2d_select_k_workspace_bytes(int64_t rows, int64_t len, int64_t k);
 int b2d_select_k(void* stream, const float* in_val, int64_t ld, const int64_t* in_idx, int64_t rows, int64_t len, int64_t k,
                  int select_min, float* out_val, int64_t* out_idx, void* workspace, size_t workspace_bytes);
 
+/* raft::neighbors::epsilon_neighborhood::eps_neighbors_l2sq / epsUnexpL2SqNeighborhood ([RECALLED]; removed upstream with
+ * neighbors/, CHANGELOG.md:59): the epsilon neighbourhood of the rows of x:[m,k] among the rows of y:[n,k] (fp32,
+ * row-major, pitches ldx / ldy), the vertex-degree step of DBSCAN.  eps is the SQUARED radius.
+ *   adj[i * ld_adj + j] = (d(i, j) <= eps) as a 0 / 1 byte (a C++ bool array qualifies), ld_adj >= n, where d(i, j) is
+ *     exactly the value b2d_pairwise_distance(L2Expanded) returns for the pair: the call equals that matrix compared with
+ *     eps, bit for bit, without writing it.  A NaN distance is never adjacent; a NaN or negative eps makes nothing adjacent.
+ *   Self pairs: when y is x or a window of its rows (same buffer, ldx == ldy, y == x + off * ldx for an integer off), the
+ *     pairs i == j + off have d = 0, adjacent for every eps >= 0 (the tensor form alone does not give exactly 0 there).  A
+ *     copy of x in other memory gets no such rule.
+ *   vd[j] += #{i : adj[i, j]} for j < n and vd[n] += the total: PER-COLUMN degrees, length n + 1, as the reference's kernel
+ *     summed them ([RECALLED] updateVertexDegree; its doc comment said m + 1, and cuML swapped the operands to get row
+ *     degrees).  vd is int32 (wrapping modulo 2^32 like the reference's int) or, vd_int64 != 0, int64.  init_vd != 0 zeroes
+ *     vd first; init_vd == 0 adds to its contents (the reference atomicAdd-ed without clearing, [RECALLED]).
+ *   adj == NULL: count only; vd == NULL: adjacency only; both NULL is B2D_ERR_INVALID_ARG.
+ * k <= 320 (the whole distance at once; else B2D_ERR_UNSUPPORTED), m, n < 2^31.  m == 0 or n == 0 only zeroes vd when
+ * init_vd is set.  Workspace: the size of b2d_pairwise_workspace_bytes(L2Expanded, F32, m, n, k); SIZE_MAX for negative
+ * extents. */
+size_t b2d_eps_neighbors_l2sq_workspace_bytes(int64_t m, int64_t n, int64_t k);
+int b2d_eps_neighbors_l2sq(void* stream, uint8_t* adj, int64_t ld_adj, void* vd, int vd_int64, int init_vd,
+                           const float* x, int64_t ldx, const float* y, int64_t ldy, int64_t m, int64_t n, int64_t k,
+                           float eps, void* workspace, size_t workspace_bytes);
+
 #ifdef __cplusplus
 }
 #endif

@@ -255,6 +255,22 @@ static int make_dist_map(CUtensorMap* map, float* dist, int64_t rows, int64_t co
   return B2D_OK;
 }
 
+// the adjacency output adj[rows][cols] (uint8, row pitch ld) of EPI_EPS as the target of its TMA stores: boxes of 128 columns
+// x 64 rows, SWIZZLE_128B (expanded_tc.cuh tc_eps_tile); needs a 16-byte aligned base and pitch
+static int make_adj_map(CUtensorMap* map, uint8_t* adj, int64_t rows, int64_t cols, int64_t ld)
+{
+  EncodeTiledFn enc = get_encode();
+  if (!enc) return fail(B2D_ERR_CUDA, "cuTensorMapEncodeTiled entry point unavailable (no CUDA driver?)");
+  cuuint64_t dims[2]    = {static_cast<cuuint64_t>(cols), static_cast<cuuint64_t>(rows)};
+  cuuint64_t strides[1] = {static_cast<cuuint64_t>(ld)};
+  cuuint32_t box[2]     = {TC_HN, TC_D_BOX_ROWS};
+  cuuint32_t estr[2]    = {1, 1};
+  CUresult r = enc(map, CU_TENSOR_MAP_DATA_TYPE_UINT8, 2, adj, dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
+                   CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_NONE, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  if (r != CUDA_SUCCESS) return fail(B2D_ERR_CUDA, "cuTensorMapEncodeTiled(adj) failed: " + std::to_string((int)r));
+  return B2D_OK;
+}
+
 template <bool kRes, int kEpi, int kPost>
 static int launch_tc_inst(cudaStream_t s, const CUtensorMap& ma, const CUtensorMap& mb, const CUtensorMap& md,
                           const TcParams& p, int grid)
@@ -275,6 +291,7 @@ static int launch_tc_epi(cudaStream_t s, const CUtensorMap& ma, const CUtensorMa
   if (epi == EPI_MINLOC) return launch_tc_inst<kRes, EPI_MINLOC, POST_NONE>(s, ma, mb, md, p, grid);
   if (epi == EPI_MINLOC_MASKED) return launch_tc_inst<kRes, EPI_MINLOC_MASKED, POST_NONE>(s, ma, mb, md, p, grid);
   if (epi == EPI_TOPK) return launch_tc_inst<kRes, EPI_TOPK, POST_NONE>(s, ma, mb, md, p, grid);
+  if (epi == EPI_EPS) return launch_tc_inst<kRes, EPI_EPS, POST_CLAMP>(s, ma, mb, md, p, grid);
   if (post == POST_NONE) return launch_tc_inst<kRes, EPI_STORE, POST_NONE>(s, ma, mb, md, p, grid);
   if (post == POST_CLAMP) return launch_tc_inst<kRes, EPI_STORE, POST_CLAMP>(s, ma, mb, md, p, grid);
   if (post == POST_JACCARD) return launch_tc_inst<kRes, EPI_STORE, POST_JACCARD>(s, ma, mb, md, p, grid);
@@ -334,6 +351,10 @@ static int launch_tc(cudaStream_t s, const TcWorkspace& w, TcParams p, int64_t k
   memset(&md, 0, sizeof(md));
   if (epi == EPI_STORE && p.tma_store) {
     rc = make_dist_map(&md, p.dist, p.m, p.n, p.ldd);
+    if (rc) return rc;
+  }
+  if (epi == EPI_EPS && p.tma_store) {
+    rc = make_adj_map(&md, p.adj, p.m, p.n, p.ld_adj);
     if (rc) return rc;
   }
   return resident ? launch_tc_epi<true>(s, ma, mb, md, p, grid, epi, post)
@@ -1617,6 +1638,58 @@ int b2d_select_k(void* stream, const float* in_val, int64_t ld, const int64_t* i
     B2D_CUDA(cudaGetLastError());
   }
   return B2D_OK;
+}
+
+// ------------------------------------------------------------------------------------------
+// Epsilon neighbourhood (raft::neighbors::epsilon_neighborhood): the L2Expanded distance of pairwise_distance compared with
+// eps in the epilogue of the tensor kernel (expanded_tc.cuh, EPI_EPS), so the m x n matrix is never written.
+
+size_t b2d_eps_neighbors_l2sq_workspace_bytes(int64_t m, int64_t n, int64_t k)
+{
+  if (m < 0 || n < 0 || k < 0) return static_cast<size_t>(-1);
+  return tc_layout(nullptr, m, n, k, false).bytes;
+}
+
+int b2d_eps_neighbors_l2sq(void* stream, uint8_t* adj, int64_t ld_adj, void* vd, int vd_int64, int init_vd,
+                           const float* x, int64_t ldx, const float* y, int64_t ldy, int64_t m, int64_t n, int64_t k,
+                           float eps, void* workspace, size_t workspace_bytes)
+{
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  if (m < 0 || n < 0 || k < 0) return fail(B2D_ERR_INVALID_ARG, "negative extent");
+  if (!adj && !vd) return fail(B2D_ERR_INVALID_ARG, "adj and vd are both null: nothing to compute");
+  if (m > 0x7fffffffll || n > 0x7fffffffll) return fail(B2D_ERR_INVALID_ARG, "m and n must be below 2^31");
+  const bool work = m > 0 && n > 0;
+  if (work) {
+    if (k == 0) return fail(B2D_ERR_INVALID_ARG, "k must be positive");
+    if (k > 320) return fail(B2D_ERR_UNSUPPORTED, "eps_neighbors_l2sq supports k <= 320 (the whole distance at once)");
+    if (!x || !y) return fail(B2D_ERR_INVALID_ARG, "null x / y");
+    if (adj && ld_adj < n) return fail(B2D_ERR_INVALID_ARG, "ld_adj smaller than n");
+    if (ldx < k || ldy < k) return fail(B2D_ERR_INVALID_ARG, "leading dimension smaller than k");
+    const size_t need = tc_layout(nullptr, m, n, k, false).bytes;
+    if (!workspace || workspace_bytes < need)
+      return fail(B2D_ERR_WORKSPACE, "workspace too small: need " + std::to_string(need) + " bytes");
+    if (reinterpret_cast<uintptr_t>(workspace) % 256) return fail(B2D_ERR_INVALID_ARG, "workspace must be 256-byte aligned");
+  }
+  if (vd && init_vd) B2D_CUDA(cudaMemsetAsync(vd, 0, static_cast<size_t>(n + 1) * (vd_int64 ? 8 : 4), s));
+  if (!work) return B2D_OK;
+  TcWorkspace w = tc_layout(workspace, m, n, k, false);
+  int rc = launch_prep<float>(s, w, x, ldx, 1, m, y, ldy, 1, n, k, nullptr, nullptr, PREP_L2, 0);
+  if (rc) return rc;
+  TcParams p;
+  memset(&p, 0, sizeof(p));
+  p.m = m; p.n = n;
+  p.adj = adj; p.ld_adj = ld_adj; p.vd = vd; p.vd64 = vd_int64 ? 1 : 0; p.eps = eps;
+  // y is a window of x's rows (same memory, same pitch): row j of y is row j + off of x
+  p.diag_off = TC_NO_DIAG;
+  const intptr_t dy = reinterpret_cast<intptr_t>(y) - reinterpret_cast<intptr_t>(x);
+  if (ldx == ldy && dy % (ldx * static_cast<intptr_t>(sizeof(float))) == 0)
+    p.diag_off = dy / (ldx * static_cast<intptr_t>(sizeof(float)));
+  // adj leaves through the staging boxes where TMA can address it: 16-byte aligned base and pitch, and rows that end on a
+  // 16-byte boundary (the byte analogue of pairwise_distance's n % 4 rule for fp32 above); coordinates fit int32 (m, n <
+  // 2^31 above).  Otherwise the epilogue stores from registers.
+  p.tma_store = (adj && reinterpret_cast<uintptr_t>(adj) % 16 == 0 && ld_adj % 16 == 0 && n % 16 == 0) ? 1 : 0;
+  ProfileScope prof(s);
+  return launch_tc(s, w, p, k, EPI_EPS, POST_CLAMP);
 }
 
 }  // extern "C"

@@ -47,6 +47,9 @@
 //   EPI_TOPK          fused brute-force kNN: the same minimum and vote against the row's current k-th best;
 //                     every pair at or below it is appended to the row's candidate list (see the kNN
 //                     helpers at the end of this file).
+//   EPI_EPS           epsilon neighbourhood: the EPI_STORE / POST_CLAMP distance, compared with eps; the 0/1 bytes go to
+//                     the EPI_STORE staging ring (one 64 x 128-byte box per tile), leave from there by TMA or a copy, and
+//                     are counted per column into shared memory (tc_eps_tile).
 #pragma once
 #include <cuda.h>
 #include <cuda_runtime.h>
@@ -77,7 +80,8 @@ constexpr int TC_D_BOX_ROWS  = 64;
 constexpr int TC_D_BOX_BYTES = TC_D_BOX_COLS * TC_D_BOX_ROWS * 4;
 constexpr int TC_STG_BOXES   = 2;
 
-enum TcEpilogue : int { EPI_STORE = 0, EPI_MINLOC = 1, EPI_TOPK = 2, EPI_MINLOC_MASKED = 3 };
+enum TcEpilogue : int { EPI_STORE = 0, EPI_MINLOC = 1, EPI_TOPK = 2, EPI_MINLOC_MASKED = 3, EPI_EPS = 4 };
+constexpr int64_t TC_NO_DIAG = INT64_MIN;   // TcParams::diag_off: y is not a row window of x
 
 // EPI_MINLOC_MASKED (masked_nn.cuh): class of one (64-row slab of x, 128-column half of a y block) tile.  Byte
 // TcParams::mask_cls[n_blk][mt] holds the four classes of an (x tile, y block) pair, 2 bits each at bit 2 (2 h + s)
@@ -146,6 +150,14 @@ struct TcParams {
   const int* mask_grp;        // [n] group of every row of y (-1: in no group)
   const unsigned* mask_bits;  // [ceil(m/32)][mask_groups] bit i % 32 of word (i / 32, g): row i of x is adjacent to group g
   int64_t mask_groups;
+  // EPI_EPS (epsilon neighbourhood): adj[i][j] = (d(i, j) <= eps) with d the EPI_STORE / POST_CLAMP distance; vd[j] += the
+  // number of adjacent rows of column j, vd[n] += the total.  tma_store: adj leaves through the staging boxes
+  uint8_t* adj;           // [m][ld_adj] 0 / 1 bytes (null: count only)
+  int64_t ld_adj;
+  void* vd;               // [n + 1] uint32 counts, or uint64 when vd64 (null: adjacency only)
+  int vd64;
+  float eps;              // the squared radius
+  int64_t diag_off;       // row j of y is row j + diag_off of x (same memory): d = 0 there; TC_NO_DIAG: no such rows
 };
 
 constexpr size_t TC_SMEM_OPERANDS = (size_t)TC_MAX_RES_KB * TC_B_BYTES + (size_t)TC_STAGES_RES * TC_A_BYTES;  // 208 KB
@@ -159,23 +171,26 @@ static_assert((size_t)TC_STAGES_STR * (TC_A_BYTES + TC_BH_BYTES) <= TC_SMEM_OPER
 // the 16 KB stage s, and every ring has full / empty mbarriers of its own.
 // mbarriers (after t_y): afull[rings * TC_MAX_STAGES], aempty[rings * TC_MAX_STAGES] (slot s of ring w at rings * s + w),
 // bfull[TC_MAX_RES_KB], bempty[TC_MAX_RES_KB].
+// EPI_EPS has the carve of EPI_STORE (its adjacency boxes are the same 8 KB) plus the [256] column counts in the slot of the
+// masked kernel's groups.
 template <bool kResident, int kEpi>
 struct TcCarve {
-  static constexpr int stages = kEpi == EPI_STORE ? (kResident ? TC_STAGES_RES_ST : TC_STAGES_STR_ST)
-                                                  : (kResident ? TC_STAGES_RES : TC_STAGES_STR);
+  static constexpr bool staged = kEpi == EPI_STORE || kEpi == EPI_EPS;
+  static constexpr int stages = staged ? (kResident ? TC_STAGES_RES_ST : TC_STAGES_STR_ST)
+                                       : (kResident ? TC_STAGES_RES : TC_STAGES_STR);
   static constexpr int rings  = kResident ? 2 : 1;
   static constexpr uint32_t stage_bytes = kResident ? TC_A_BYTES : TC_A_BYTES + TC_BH_BYTES;
   static constexpr size_t a_off   = kResident ? (size_t)TC_MAX_RES_KB * TC_B_BYTES : 0;
   static constexpr size_t stg_off = a_off + (size_t)stages * stage_bytes;
-  static constexpr size_t tb_off  = kEpi == EPI_STORE ? stg_off + 2 * (size_t)TC_STG_BOXES * TC_D_BOX_BYTES : TC_SMEM_OPERANDS;
-  static constexpr size_t grp_off = tb_off + TC_BN * 4 + 256;   // EPI_MINLOC_MASKED: [256] group of every column
-  static constexpr size_t bytes   = grp_off + (kEpi == EPI_MINLOC_MASKED ? TC_BN * 4 : 0);
+  static constexpr size_t tb_off  = staged ? stg_off + 2 * (size_t)TC_STG_BOXES * TC_D_BOX_BYTES : TC_SMEM_OPERANDS;
+  static constexpr size_t grp_off = tb_off + TC_BN * 4 + 256;   // EPI_MINLOC_MASKED: [256] group, EPI_EPS: count of every column
+  static constexpr size_t bytes   = grp_off + (kEpi == EPI_MINLOC_MASKED || kEpi == EPI_EPS ? TC_BN * 4 : 0);
   static_assert(stages <= TC_MAX_STAGES, "barrier arrays hold TC_MAX_STAGES stages");
   static_assert((2 * rings * TC_MAX_STAGES + 2 * TC_MAX_RES_KB) * 8 <= grp_off - tb_off - TC_BN * 4,
                 "the mbarriers of every ring fit in the 256 bytes after t_y");
   static_assert(!kResident || stages >= TC_MAX_RES_KB, "resident: the ring holds every x k-block of a tile (both halves read them)");
   static_assert(stg_off % 1024 == 0, "SWIZZLE_128B staging boxes need 1024-byte alignment");
-  static_assert(kEpi == EPI_STORE || stg_off <= TC_SMEM_OPERANDS, "operands fit");
+  static_assert(staged || stg_off <= TC_SMEM_OPERANDS, "operands fit");
   static_assert(bytes <= 232448, "exceeds the 227 KB per-CTA limit");
 };
 
@@ -352,7 +367,7 @@ __device__ __forceinline__ void tc_epilogue(float (&v)[64], const TcParams& p, c
       if (kEpi == EPI_STORE && kPost >= POST_JACCARD) {
         v[4 * i + 2 * j]     = post_ratio<kPost>(a0 * cfr[j], ta[j] + tb.x);
         v[4 * i + 2 * j + 1] = post_ratio<kPost>(a1 * cfr[j], ta[j] + tb.y);
-      } else if (kEpi == EPI_STORE) {
+      } else if (kEpi == EPI_STORE || kEpi == EPI_EPS) {
         v[4 * i + 2 * j]     = fmaf(a0, cfr[j], ta[j] + tb.x);
         v[4 * i + 2 * j + 1] = fmaf(a1, cfr[j], ta[j] + tb.y);
       } else {
@@ -360,6 +375,23 @@ __device__ __forceinline__ void tc_epilogue(float (&v)[64], const TcParams& p, c
         v[4 * i + 2 * j + 1] = fmaf(a1, cfr[j], tb.y);
       }
     }
+  }
+  if constexpr (kEpi == EPI_EPS) {
+    // the POST_CLAMP distance of EPI_STORE; where row i of x is row j of y (i == j + diag_off) it is 0, as pairwise_distance
+    // makes it when x is y.  (Columns beyond n hold NaN from t_y and stay unmatched; the row window check keeps them out.)
+#pragma unroll
+    for (int c = 0; c < 64; ++c) v[c] = clamp0(v[c]);
+    if (p.diag_off != TC_NO_DIAG) {
+      const int64_t dd = row0 - p.diag_off - gc0;   // row0 + 8 j == gc0 + 8 i + e + diag_off  <=>  dd == 8 (i - j) + e
+#pragma unroll
+      for (int i = 0; i < 16; ++i)
+#pragma unroll
+        for (int j = 0; j < 2; ++j)
+#pragma unroll
+          for (int e = 0; e < 2; ++e)
+            if (dd == 8 * (i - j) + e && gc0 + 8 * i + e < p.n) v[4 * i + 2 * j + e] = 0.f;
+    }
+    return;
   }
   if (kEpi == EPI_STORE) {
     // (the manual stores: 8-byte vectors when dist and its pitch allow them)
@@ -518,6 +550,120 @@ __device__ __forceinline__ void tc_stage_store(const float (&v)[64], const CUten
   if (issuer && last) ptx::tma_store_wait_all();   // the CTA's last tile: its shared memory outlives every store
 }
 
+// EPI_EPS after tc_epilogue: the warpgroup's finished 64 x 128 tile v becomes 0 / 1 bytes in one 64-row x 128-byte box of
+// its EPI_STORE staging ring (slot = parity of the warpgroup's tile count box_it), byte (r, c) at
+// r * 128 + ((c / 16) ^ (r % 8)) * 16 + c % 16 (SWIZZLE_128B).  Rows beyond m never match (d is >= 0 or NaN), columns
+// beyond n hold NaN.  Each thread writes its flags as 2-byte shared stores (conflict-free: the 8 rows of a warp's store
+// hit 8 different 16-byte chunks).  Everything after reads the box, in every output mode:
+//   adjacency: TMA (p.tma_store) as in tc_stage_store, or else each warp copies 16 rows out, one row per step with 4 bytes
+//     per lane (2- or 1-byte stores where the base or pitch is not 4- or 2-byte aligned, and at the end of a row);
+//     count-only stores nothing.
+//   counts: thread t sums 4 rows of the 16-byte chunk t % 8 (bytes <= 4), the warp's 4 threads of a chunk add theirs by
+//     a reduce-scatter (3 shuffles; bytes <= 16), and each adds 4 column counts to the item's col_cnt in shared memory.
+// (The fragment's own registers are not an option for either: acc and crs keep 128 registers live through the epilogue.)
+__device__ __forceinline__ void tc_eps_tile(const float (&v)[64], const TcParams& p, uint32_t* col_cnt, int hcol, int64_t row0,
+                                            const CUtensorMap* tmap_d, uint32_t stg, bool issuer, bool last, int wg,
+                                            int64_t row_w, int64_t col_w, uint32_t& box_it)
+{
+  const int lane = threadIdx.x & 31;
+  const int quad = lane >> 2, tq = lane & 3;
+  const uint32_t box = stg + (box_it & 1u) * TC_D_BOX_BYTES;
+  ++box_it;
+  // TMA: the store issued two tiles ago read this slot, it must be done (the latest store may still be reading)
+  if (issuer && p.tma_store) ptx::tma_store_wait_read<1>();
+  ptx::bar_sync(2 + wg, 128);
+  const uint32_t t_off = box + (16 * ((threadIdx.x >> 5) & 3) + quad) * 128 + 2 * tq;
+#pragma unroll
+  for (int w = 0; w < 8; ++w) {   // the thread's columns 8 i + {0, 1}, i = 2 w, 2 w + 1 -> bytes 2 (i & 1) + {0, 1}
+#pragma unroll
+    for (int j = 0; j < 2; ++j) {
+      uint32_t word = 0u;
+#pragma unroll
+      for (int b = 0; b < 4; ++b)
+        if (v[4 * (2 * w + (b >> 1)) + 2 * j + (b & 1)] <= p.eps) word |= 1u << (8 * b);
+      if (row0 + 8 * j >= p.m) word = 0u;
+      const uint32_t o = t_off + 8 * j * 128 + ((16 * w) ^ (16 * quad));
+      ptx::st_shared_u16(o, word);
+      ptx::st_shared_u16(o + 8, word >> 16);
+    }
+  }
+  if (p.tma_store) ptx::fence_proxy_async_smem();   // the generic-proxy writes become visible to the TMA unit
+  ptx::bar_sync(2 + wg, 128);
+  if (p.tma_store) {
+    if (issuer) {
+      if (col_w < p.n && row_w < p.m)
+        ptx::tma_store_2d(tmap_d, box, static_cast<int32_t>(col_w), static_cast<int32_t>(row_w), ptx::policy_evict_first());
+      ptx::tma_store_commit();
+      if (last) ptx::tma_store_wait_all();   // the CTA's last tile: its shared memory outlives every store
+    }
+  } else if (p.adj != nullptr) {
+    // warp w copies rows [16 w, 16 w + 16) of the box, one row per step: lane l the 4 bytes at column 4 l, so every store
+    // instruction writes 128 contiguous bytes of one row
+    const int c       = 4 * lane;
+    const int64_t nc  = p.n - col_w - c;   // columns of this lane's 4 inside the matrix
+    const int al      = static_cast<int>((reinterpret_cast<uintptr_t>(p.adj) | static_cast<uintptr_t>(p.ld_adj)) & 3u);
+    const int w16     = 16 * ((threadIdx.x >> 5) & 3);
+#pragma unroll 4
+    for (int rr = 0; rr < 16; ++rr) {
+      const int r = w16 + rr;
+      if (row_w + r >= p.m || nc <= 0) continue;
+      uint32_t wd;
+      asm volatile("ld.shared.u32 %0, [%1];" : "=r"(wd) : "r"(box + r * 128 + (((lane >> 2) ^ (r & 7)) * 16) + 4 * (lane & 3)));
+      uint8_t* q = p.adj + (row_w + r) * p.ld_adj + col_w + c;
+      if (al == 0 && nc >= 4) {
+        __stcs(reinterpret_cast<unsigned*>(q), wd);
+      } else if ((al & 1) == 0) {
+        if (nc >= 2) __stcs(reinterpret_cast<unsigned short*>(q), static_cast<unsigned short>(wd & 0xffffu));
+        else __stcs(q, static_cast<unsigned char>(wd & 0xffu));
+        if (nc >= 4) __stcs(reinterpret_cast<unsigned short*>(q + 2), static_cast<unsigned short>(wd >> 16));
+        else if (nc == 3) __stcs(q + 2, static_cast<unsigned char>((wd >> 16) & 0xffu));
+      } else {
+#pragma unroll
+        for (int b = 0; b < 4; ++b)
+          if (b < nc) __stcs(q + b, static_cast<unsigned char>((wd >> (8 * b)) & 0xffu));
+      }
+    }
+  }
+  if (p.vd == nullptr) return;
+  const int cc = threadIdx.x & 7, rg = (threadIdx.x & 127) >> 3;   // chunk cc of rows [4 rg, 4 rg + 4)
+  uint4 s = make_uint4(0u, 0u, 0u, 0u);
+#pragma unroll
+  for (int u = 0; u < 4; ++u) {
+    const int r   = 4 * rg + u;
+    const uint4 d = ptx::ld_shared_v4(box + r * 128 + ((cc ^ (r & 7)) * 16));
+    s.x += d.x; s.y += d.y; s.z += d.z; s.w += d.w;
+  }
+  // lanes cc, cc + 8, cc + 16, cc + 24 of the warp hold the same chunk: lane bit 4 keeps words {z, w} or {x, y}, bit 3 one
+  // of those, so lane (lane >> 3) ends with word lane >> 3 of the chunk: columns 16 cc + 4 (lane >> 3) + {0..3}
+  const bool b4 = (lane & 16) != 0, b3 = (lane & 8) != 0;
+  const uint32_t k0 = (b4 ? s.z : s.x) + __shfl_xor_sync(0xffffffffu, b4 ? s.x : s.z, 16);
+  const uint32_t k1 = (b4 ? s.w : s.y) + __shfl_xor_sync(0xffffffffu, b4 ? s.y : s.w, 16);
+  const uint32_t c4 = (b3 ? k1 : k0) + __shfl_xor_sync(0xffffffffu, b3 ? k0 : k1, 8);
+  if (c4 != 0u) {
+#pragma unroll
+    for (int b = 0; b < 4; ++b) {
+      const uint32_t c = (c4 >> (8 * b)) & 0xffu;
+      if (c != 0u) atomicAdd(&col_cnt[hcol + 16 * cc + 4 * (lane >> 3) + b], c);
+    }
+  }
+}
+
+// EPI_EPS: the counts of y block n_blk go to vd, one atomic per column (ct: the consumer thread's column) and one per warp
+// for the total vd[n]
+__device__ __forceinline__ void tc_eps_flush(const TcParams& p, const uint32_t* col_cnt, int n_blk, int ct)
+{
+  const uint32_t c   = col_cnt[ct];
+  const int64_t gj   = static_cast<int64_t>(n_blk) * TC_BN + ct;
+  const uint32_t tot = __reduce_add_sync(0xffffffffu, c);
+  if (p.vd64) {
+    if (c != 0u) atomicAdd(static_cast<unsigned long long*>(p.vd) + gj, static_cast<unsigned long long>(c));
+    if ((threadIdx.x & 31) == 0 && tot != 0u) atomicAdd(static_cast<unsigned long long*>(p.vd) + p.n, static_cast<unsigned long long>(tot));
+  } else {
+    if (c != 0u) atomicAdd(static_cast<unsigned*>(p.vd) + gj, c);
+    if ((threadIdx.x & 31) == 0 && tot != 0u) atomicAdd(static_cast<unsigned*>(p.vd) + p.n, tot);
+  }
+}
+
 template <bool kResident, int kEpi, int kPost>
 __global__ void __launch_bounds__(TC_THREADS, 1)
 expanded_tc_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b,
@@ -554,7 +700,7 @@ expanded_tc_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_cons
     ptx::fence_mbar_init();
     ptx::prefetch_tmap(&tmap_a);
     ptx::prefetch_tmap(&tmap_b);
-    if (kEpi == EPI_STORE && p.tma_store) ptx::prefetch_tmap(&tmap_d);
+    if ((kEpi == EPI_STORE || kEpi == EPI_EPS) && p.tma_store) ptx::prefetch_tmap(&tmap_d);
   }
   __syncthreads();
 
@@ -622,6 +768,10 @@ expanded_tc_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_cons
   if (kResident && wg == 1) ptx::bar_arrive(4, 256);
   uint32_t a_it = 0, it_local = 0;
   float acc[64], crs[64];
+  // EPI_EPS: the item's column counts (flushed at the next item's t_y fill and after the last item) and the warpgroup's
+  // adjacency box count (tc_eps_tile)
+  uint32_t* col_cnt = reinterpret_cast<uint32_t*>(smem + Carve::grp_off);
+  uint32_t eps_box = 0u;
   for (int64_t item = blockIdx.x; item < p.n_items; item += gridDim.x, ++it_local) {
     const TcItem t  = tc_item(p, item);
     const int n_blk = t.n_blk, mt0 = t.mt0, mt1 = t.mt1, nh = t.nh;
@@ -641,9 +791,16 @@ expanded_tc_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_cons
     bool b_first = true;   // masked: this warpgroup has not waited for the item's y block yet
     // per-column epilogue terms of this y block (shared by every tile of the item)
     ptx::bar_sync(1, 256);
+    if constexpr (kEpi == EPI_EPS) {
+      if (p.vd != nullptr) {
+        if (item != blockIdx.x) tc_eps_flush(p, col_cnt, tc_item(p, item - gridDim.x).n_blk, ct);   // the previous item's
+        col_cnt[ct] = 0u;
+      }
+    }
     {
       const int64_t gj = static_cast<int64_t>(n_blk) * TC_BN + ct;
-      float tv = kEpi != EPI_STORE ? __int_as_float(0x7f800000) : 0.f;  // +inf: never the arg-min
+      // +inf: never the arg-min; NaN: never within eps
+      float tv = kEpi == EPI_EPS ? __int_as_float(0x7fffffff) : kEpi != EPI_STORE ? __int_as_float(0x7f800000) : 0.f;
       if (gj < p.n) tv = __ldg(&p.yt[gj]);
       if (kEpi == EPI_STORE && p.acc_mode >= 2) tv = 0.f;  // the t terms entered with the first K chunk
       col_tb[ct] = tv;
@@ -789,9 +946,21 @@ expanded_tc_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_cons
           tc_stage_store(acc, &tmap_d, ptx::smem_u32(smem + Carve::stg_off) + wg * TC_STG_BOXES * TC_D_BOX_BYTES, lead,
                          item + gridDim.x >= p.n_items && mt == mt1 - 1 && h == nh - 1, wg,
                          static_cast<int64_t>(mt) * TC_BM + 64 * wg, static_cast<int64_t>(n_blk) * TC_BN + h * TC_HN, p);
+        if constexpr (kEpi == EPI_EPS)
+          tc_eps_tile(acc, p, col_cnt, h * TC_HN, row0, &tmap_d,
+                      ptx::smem_u32(smem + Carve::stg_off) + wg * TC_STG_BOXES * TC_D_BOX_BYTES, lead,
+                      item + gridDim.x >= p.n_items && mt == mt1 - 1 && h == nh - 1, wg,
+                      static_cast<int64_t>(mt) * TC_BM + 64 * wg, static_cast<int64_t>(n_blk) * TC_BN + h * TC_HN, eps_box);
       }
     }
     if (kResident && wg == 0 && item + gridDim.x >= p.n_items) take_turn();   // warpgroup 1's last pass
+  }
+  if constexpr (kEpi == EPI_EPS) {
+    if (p.vd != nullptr) {   // the last item's counts
+      ptx::bar_sync(1, 256);
+      const int64_t last_item = blockIdx.x + (p.n_items - 1 - blockIdx.x) / gridDim.x * gridDim.x;   // (grid <= n_items)
+      tc_eps_flush(p, col_cnt, tc_item(p, last_item).n_blk, ct);
+    }
   }
 }
 

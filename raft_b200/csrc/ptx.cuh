@@ -206,6 +206,16 @@ __device__ __forceinline__ void st_shared_v2(uint32_t addr, float a, float b)
 {
   asm volatile("st.shared.v2.f32 [%0], {%1, %2};" ::"r"(addr), "f"(a), "f"(b) : "memory");
 }
+__device__ __forceinline__ uint4 ld_shared_v4(uint32_t addr)
+{
+  uint4 v;
+  asm volatile("ld.shared.v4.u32 {%0, %1, %2, %3}, [%4];" : "=r"(v.x), "=r"(v.y), "=r"(v.z), "=r"(v.w) : "r"(addr) : "memory");
+  return v;
+}
+__device__ __forceinline__ void st_shared_u16(uint32_t addr, uint32_t v)
+{
+  asm volatile("st.shared.u16 [%0], %1;" ::"r"(addr), "h"(static_cast<unsigned short>(v)) : "memory");
+}
 __device__ __forceinline__ void st_global_cs_v2(float* p, float a, float b)
 {
   asm volatile("st.global.cs.v2.f32 [%0], {%1, %2};" ::"l"(p), "f"(a), "f"(b) : "memory");

@@ -1,2 +1,4 @@
 """Mirror of the (removed) ``pylibraft.neighbors`` entry points that sit directly behind the distance path."""
 from . import brute_force  # noqa: F401
+from . import epsilon_neighborhood  # noqa: F401
+from .epsilon_neighborhood import eps_neighbors_l2sq  # noqa: F401
