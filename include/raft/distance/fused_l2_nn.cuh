@@ -32,12 +32,9 @@ void fusedL2NNMinReduce(OutT* min, const DataT* x, const DataT* y, const DataT* 
   static_assert(std::is_same<DataT, float>::value && sizeof(OutT) == sizeof(b2d_kvp_if),
                 "raft_b200: fusedL2NN is provided for <float, KeyValuePair<int,float>, int>");
   const size_t need = b2d_fused_l2_nn_workspace_bytes(m, n, k);
-  void* ws          = nullptr;
-  if (cudaMallocAsync(&ws, need, stream) != cudaSuccess) throw raft::cuda_error("fusedL2NN: scratch allocation failed");
-  const int st = b2d_fused_l2_nn(stream, reinterpret_cast<b2d_kvp_if*>(min), x, k, y, k, xn, yn, m, n, k, sqrt ? 1 : 0,
-                                 initOutBuffer ? 1 : 0, ws, need);
-  cudaFreeAsync(ws, stream);
-  detail::b2d_check(st);
+  raft::b200::scoped_workspace ws(stream, need);
+  detail::b2d_check(b2d_fused_l2_nn(stream, reinterpret_cast<b2d_kvp_if*>(min), x, k, y, k, xn, yn, m, n, k, sqrt ? 1 : 0,
+                                    initOutBuffer ? 1 : 0, ws.data(), need));
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -106,16 +103,13 @@ void fusedL2NN(OutT* min, const DataT* x, const DataT* y, const DataT* xn, const
   static_assert(std::is_same<DataT, float>::value && sizeof(IdxT) == 4, "raft_b200: fusedL2NN is provided for DataT = float, 32-bit IdxT");
   const size_t need = b2d_fused_l2_nn_workspace_bytes(m, n, k);
   const size_t kvpb = (static_cast<size_t>(m) * sizeof(b2d_kvp_if) + 255) / 256 * 256;
-  char* scratch     = nullptr;
-  if (cudaMallocAsync(reinterpret_cast<void**>(&scratch), need + kvpb + 256, stream) != cudaSuccess)
-    throw raft::cuda_error("fusedL2NN: scratch allocation failed");
-  char* base      = reinterpret_cast<char*>((reinterpret_cast<uintptr_t>(scratch) + 255) & ~static_cast<uintptr_t>(255));
-  b2d_kvp_if* nn  = reinterpret_cast<b2d_kvp_if*>(base);
-  const int st    = b2d_fused_l2_nn(stream, nn, x, k, y, k, xn, yn, m, n, k, sqrt ? 1 : 0, 1, base + kvpb, need);
+  raft::b200::scoped_workspace ws(stream, kvpb + need);   // the per-row arg-min in front of the engine's scratch
+  char* base     = static_cast<char*>(ws.data());
+  b2d_kvp_if* nn = reinterpret_cast<b2d_kvp_if*>(base);
+  const int st   = b2d_fused_l2_nn(stream, nn, x, k, y, k, xn, yn, m, n, k, sqrt ? 1 : 0, 1, base + kvpb, need);
   if (st == B2D_OK && m > 0)
     detail::b2d_apply_reduce_kernel<OutT, IdxT, DataT, ReduceOpT><<<static_cast<unsigned>((m + 255) / 256), 256, 0, stream>>>(
       min, nn, m, redOp, initOutBuffer, 3.402823466e+38f);
-  cudaFreeAsync(scratch, stream);
   detail::b2d_check(st);
 }
 #endif  // __CUDACC__

@@ -41,6 +41,31 @@ static int fail(int code, const std::string& msg)
 
 static size_t align_up(size_t v, size_t a) { return (v + a - 1) / a * a; }
 
+// Cuts a caller's workspace into consecutive regions, each rounded up to `align` bytes.  With a null base it only
+// counts the bytes (the *_workspace_bytes queries): every region is then null, and no pointer is formed from null.
+struct Carve {
+  char* base;
+  size_t align;
+  size_t bytes = 0;
+  Carve(void* b, size_t a) : base(static_cast<char*>(b)), align(a) {}
+  template <typename T>
+  T* take(size_t count)
+  {
+    T* at = base ? reinterpret_cast<T*>(base + bytes) : nullptr;
+    bytes += align_up(count * sizeof(T), align);
+    return at;
+  }
+};
+
+// the caller's workspace holds `need` bytes (none needed: anything goes) and starts on an `align`-byte boundary
+static int check_workspace(const void* ws, size_t bytes, size_t need, size_t align = 256)
+{
+  if (need > 0 && (!ws || bytes < need))
+    return fail(B2D_ERR_WORKSPACE, "workspace too small: need " + std::to_string(need) + " bytes");
+  if (reinterpret_cast<uintptr_t>(ws) % align) return fail(B2D_ERR_INVALID_ARG, "workspace must be 256-byte aligned");
+  return B2D_OK;
+}
+
 // process-wide tuning / test hooks (b2d_set_option): nothing on the hot path reads the environment
 static std::atomic<float> g_nn_tau{6.0f};   // screened fusedL2NN: candidates per row above which the trial calls screening off
 static std::atomic<int> g_nn_screen{1};     // 0: always the exact arg-min kernel
@@ -67,6 +92,25 @@ static EncodeTiledFn get_encode()
   return fn;
 }
 
+// a row-major matrix [rows][cols] of `dtype` with a row pitch of pitch_bytes, in boxes of box_cols x box_rows;
+// `tag` names the map in the error message
+static int encode_2d(CUtensorMap* map, CUtensorMapDataType dtype, const void* base, int64_t cols, int64_t rows,
+                     int64_t pitch_bytes, unsigned box_cols, unsigned box_rows, CUtensorMapSwizzle swizzle,
+                     CUtensorMapL2promotion promotion, const char* tag)
+{
+  EncodeTiledFn enc = get_encode();
+  if (!enc) return fail(B2D_ERR_CUDA, "cuTensorMapEncodeTiled entry point unavailable (no CUDA driver?)");
+  cuuint64_t dims[2]    = {static_cast<cuuint64_t>(cols), static_cast<cuuint64_t>(rows)};
+  cuuint64_t strides[1] = {static_cast<cuuint64_t>(pitch_bytes)};
+  cuuint32_t box[2]     = {box_cols, box_rows};
+  cuuint32_t estr[2]    = {1, 1};
+  CUresult r = enc(map, dtype, 2, const_cast<void*>(base), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, swizzle,
+                   promotion, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  if (r != CUDA_SUCCESS)
+    return fail(B2D_ERR_CUDA, std::string("cuTensorMapEncodeTiled") + tag + " failed: " + std::to_string((int)r));
+  return B2D_OK;
+}
+
 // packed operand [rows][nkb*64] fp16, box = 64 x box_rows, SWIZZLE_128B
 // (hi_only: boxes of the 32 hi halves of a k-block, 64 B rows, SWIZZLE_64B -- the coarse screening pass)
 static int make_operand_map(CUtensorMap* map, const void* base, int64_t rows, int nkb, int box_rows,
@@ -74,17 +118,9 @@ static int make_operand_map(CUtensorMap* map, const void* base, int64_t rows, in
 {
   if (nkb_total == 0) nkb_total = nkb;
   base = static_cast<const char*>(base) + static_cast<size_t>(kb0) * 128;  // K chunk [kb0, kb0 + nkb) of every row
-  EncodeTiledFn enc = get_encode();
-  if (!enc) return fail(B2D_ERR_CUDA, "cuTensorMapEncodeTiled entry point unavailable (no CUDA driver?)");
-  cuuint64_t dims[2]    = {static_cast<cuuint64_t>(nkb) * 64, static_cast<cuuint64_t>(rows)};
-  cuuint64_t strides[1] = {static_cast<cuuint64_t>(nkb_total) * 128};
-  cuuint32_t box[2]     = {hi_only ? 32u : 64u, static_cast<cuuint32_t>(box_rows)};
-  cuuint32_t estr[2]    = {1, 1};
-  CUresult r = enc(map, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, const_cast<void*>(base), dims, strides, box,
-                   estr, CU_TENSOR_MAP_INTERLEAVE_NONE, hi_only ? CU_TENSOR_MAP_SWIZZLE_64B : CU_TENSOR_MAP_SWIZZLE_128B,
-                   CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  if (r != CUDA_SUCCESS) return fail(B2D_ERR_CUDA, "cuTensorMapEncodeTiled failed: " + std::to_string((int)r));
-  return B2D_OK;
+  return encode_2d(map, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, base, static_cast<int64_t>(nkb) * 64, rows,
+                   static_cast<int64_t>(nkb_total) * 128, hi_only ? 32u : 64u, static_cast<unsigned>(box_rows),
+                   hi_only ? CU_TENSOR_MAP_SWIZZLE_64B : CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, "");
 }
 
 // SM count of the current device; every kernel of the library is built for sm_90a only, so any other device is an error
@@ -154,54 +190,56 @@ struct TcWorkspace {
   unsigned* sort_key[2];  // [min(n, 2^20)] each
   int* sort_val[2];       // [min(n, 2^20)] each: position -> source row
   void* sort_tmp;
-  size_t bytes;
+  size_t bytes;      // end of these regions in the workspace
 };
 constexpr int64_t kNnChunkRows  = 1 << 20;   // database rows per screened chunk
 constexpr size_t kSortTmpBytes  = 4u << 20;  // cub::DeviceRadixSort scratch for <= 2^20 pairs (checked at run time)
 
-static TcWorkspace tc_layout(void* base, int64_t m, int64_t n, int64_t k, bool with_keys)
+// the tensor-core path's regions at the front of `c` (1024-byte alignment); with_keys: the screened arg-min's too
+static TcWorkspace tc_layout(Carve& c, int64_t m, int64_t n, int64_t k, bool with_keys)
 {
   const int nkb = static_cast<int>((k + 31) / 32);
-  size_t off    = 0;
-  auto take     = [&](size_t b) {
-    size_t o = off;
-    off += align_up(b, 1024);
-    return o;
-  };
-  char* c = static_cast<char*>(base);
-  TcWorkspace w;
-  // scalars, xt and keys come first so that their offsets depend on m only
-  // (b2d_fused_l2_nn_finalize finds |x_i|^2 again without knowing n or k)
-  w.gmax = reinterpret_cast<unsigned*>(c + take(32));
-  w.coef = reinterpret_cast<float*>(w.gmax + 2);
-  w.has_lo = w.gmax + 3;
-  w.nonuni = w.gmax + 4;
-  w.xt   = reinterpret_cast<float*>(c + take(static_cast<size_t>(m) * 4));
-  w.xsc  = reinterpret_cast<float*>(c + take(static_cast<size_t>(m) * 4));
-  w.keys = reinterpret_cast<long long*>(c + take(with_keys ? static_cast<size_t>(m) * 8 : 0));
+  TcWorkspace w{};
+  w.gmax = c.take<unsigned>(8);   // gmax[2], coef, has_lo, nonuni[2]
+  if (w.gmax) {
+    w.coef   = reinterpret_cast<float*>(w.gmax + 2);
+    w.has_lo = w.gmax + 3;
+    w.nonuni = w.gmax + 4;
+  }
+  w.xt   = c.take<float>(m);
+  w.xsc  = c.take<float>(m);
+  w.keys = c.take<long long>(with_keys ? m : 0);
   // screened fusedL2NN scratch: thresholds, counters, candidate list (128 per row and 1M-row chunk of y;
   // ~54 measured on far-from-origin clusters; overflow falls back to the exact pass on the device,
   // never to a wrong answer)
   // (+2^19: the coarse kernel's warps take list slots in blocks of 64 -- 132 x 8 warps x 2 launches leave up to
   // ~135k slots unused, which must not look like an overflow when m is small)
   w.cand_cap = with_keys ? static_cast<unsigned>(std::min<int64_t>(128 * m + (1 << 19), 0x7fffffff)) : 0u;
-  w.aux      = reinterpret_cast<float4*>(c + take(with_keys ? static_cast<size_t>(m) * 16 : 0));
-  w.cand_cnt = reinterpret_cast<unsigned*>(c + take(with_keys ? 32 : 0));
-  w.cand     = reinterpret_cast<int2*>(c + take(static_cast<size_t>(w.cand_cap) * 8));
-  w.yt   = reinterpret_cast<float*>(c + take(static_cast<size_t>(n) * 4));
-  w.ysc  = reinterpret_cast<float*>(c + take(static_cast<size_t>(n) * 4));
-  w.xop  = reinterpret_cast<__half*>(c + take(static_cast<size_t>(m) * nkb * 128));
-  w.yop  = reinterpret_cast<__half*>(c + take(static_cast<size_t>(n) * nkb * 128));
+  w.aux      = c.take<float4>(with_keys ? m : 0);
+  w.cand_cnt = c.take<unsigned>(with_keys ? 8 : 0);
+  w.cand     = c.take<int2>(w.cand_cap);
+  w.yt   = c.take<float>(n);
+  w.ysc  = c.take<float>(n);
+  w.xop  = c.take<__half>(static_cast<size_t>(m) * nkb * 64);
+  w.yop  = c.take<__half>(static_cast<size_t>(n) * nkb * 64);
   const size_t ns = with_keys ? static_cast<size_t>(std::min<int64_t>(n, kNnChunkRows)) : 0;
   for (int i = 0; i < 2; ++i) {
-    w.sort_key[i] = reinterpret_cast<unsigned*>(c + take(ns * 4));
-    w.sort_val[i] = reinterpret_cast<int*>(c + take(ns * 4));
+    w.sort_key[i] = c.take<unsigned>(ns);
+    w.sort_val[i] = c.take<int>(ns);
   }
-  w.sort_tmp = c + take(with_keys ? kSortTmpBytes : 0);
-  w.xlo = with_keys ? reinterpret_cast<float*>(c + take(static_cast<size_t>(m) * 4)) : nullptr;
-  w.ylo = with_keys ? reinterpret_cast<float*>(c + take(static_cast<size_t>(n) * 4)) : nullptr;
-  w.bytes = off;
+  w.sort_tmp = c.take<char>(with_keys ? kSortTmpBytes : 0);
+  if (with_keys) {
+    w.xlo = c.take<float>(m);
+    w.ylo = c.take<float>(n);
+  }
+  w.bytes = c.bytes;
   return w;
+}
+
+static TcWorkspace tc_layout(void* base, int64_t m, int64_t n, int64_t k, bool with_keys)
+{
+  Carve c(base, 1024);
+  return tc_layout(c, m, n, k, with_keys);
 }
 
 static bool is_expanded(int metric)
@@ -236,38 +274,6 @@ static int launch_prep(cudaStream_t s, const TcWorkspace& w, const void* x, int6
   B2D_CUDA(cudaGetLastError());
   prep_split_kernel<T><<<static_cast<unsigned>(blocks), 256, 0, s>>>(p);
   B2D_CUDA(cudaGetLastError());
-  return B2D_OK;
-}
-
-// the pairwise output dist[rows][cols] (row pitch ldd) as the target of the EPI_STORE TMA stores: boxes of 32 columns x
-// 64 rows, SWIZZLE_128B (expanded_tc.cuh tc_stage_store); needs a 16-byte aligned base and pitch
-static int make_dist_map(CUtensorMap* map, float* dist, int64_t rows, int64_t cols, int64_t ldd)
-{
-  EncodeTiledFn enc = get_encode();
-  if (!enc) return fail(B2D_ERR_CUDA, "cuTensorMapEncodeTiled entry point unavailable (no CUDA driver?)");
-  cuuint64_t dims[2]    = {static_cast<cuuint64_t>(cols), static_cast<cuuint64_t>(rows)};
-  cuuint64_t strides[1] = {static_cast<cuuint64_t>(ldd) * 4};
-  cuuint32_t box[2]     = {TC_D_BOX_COLS, TC_D_BOX_ROWS};
-  cuuint32_t estr[2]    = {1, 1};
-  CUresult r = enc(map, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, dist, dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                   CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_NONE, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  if (r != CUDA_SUCCESS) return fail(B2D_ERR_CUDA, "cuTensorMapEncodeTiled(dist) failed: " + std::to_string((int)r));
-  return B2D_OK;
-}
-
-// the adjacency output adj[rows][cols] (uint8, row pitch ld) of EPI_EPS as the target of its TMA stores: boxes of 128 columns
-// x 64 rows, SWIZZLE_128B (expanded_tc.cuh tc_eps_tile); needs a 16-byte aligned base and pitch
-static int make_adj_map(CUtensorMap* map, uint8_t* adj, int64_t rows, int64_t cols, int64_t ld)
-{
-  EncodeTiledFn enc = get_encode();
-  if (!enc) return fail(B2D_ERR_CUDA, "cuTensorMapEncodeTiled entry point unavailable (no CUDA driver?)");
-  cuuint64_t dims[2]    = {static_cast<cuuint64_t>(cols), static_cast<cuuint64_t>(rows)};
-  cuuint64_t strides[1] = {static_cast<cuuint64_t>(ld)};
-  cuuint32_t box[2]     = {TC_HN, TC_D_BOX_ROWS};
-  cuuint32_t estr[2]    = {1, 1};
-  CUresult r = enc(map, CU_TENSOR_MAP_DATA_TYPE_UINT8, 2, adj, dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                   CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_NONE, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  if (r != CUDA_SUCCESS) return fail(B2D_ERR_CUDA, "cuTensorMapEncodeTiled(adj) failed: " + std::to_string((int)r));
   return B2D_OK;
 }
 
@@ -347,14 +353,18 @@ static int launch_tc(cudaStream_t s, const TcWorkspace& w, TcParams p, int64_t k
   // resident: the whole 256-row y block in one box per k-block; streaming: one 128-row half per stage
   rc = make_operand_map(&mb, w.yop, p.n, p.nkb, resident ? TC_BN : TC_HN, kb0, nkb_total);
   if (rc) return rc;
-  CUtensorMap md;   // only read by the kernel when EPI_STORE goes through TMA
+  CUtensorMap md;   // only read by the kernel when EPI_STORE or EPI_EPS goes through TMA
   memset(&md, 0, sizeof(md));
+  // both need a 16-byte aligned base and pitch.  EPI_STORE: dist [m][n] fp32 in boxes of 32 columns x 64 rows
+  // (expanded_tc.cuh tc_stage_store); EPI_EPS: adj [m][n] bytes in boxes of 128 columns x 64 rows (tc_eps_tile)
   if (epi == EPI_STORE && p.tma_store) {
-    rc = make_dist_map(&md, p.dist, p.m, p.n, p.ldd);
+    rc = encode_2d(&md, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, p.dist, p.n, p.m, p.ldd * 4, TC_D_BOX_COLS, TC_D_BOX_ROWS,
+                   CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_NONE, "(dist)");
     if (rc) return rc;
   }
   if (epi == EPI_EPS && p.tma_store) {
-    rc = make_adj_map(&md, p.adj, p.m, p.n, p.ld_adj);
+    rc = encode_2d(&md, CU_TENSOR_MAP_DATA_TYPE_UINT8, p.adj, p.n, p.m, p.ld_adj, TC_HN, TC_D_BOX_ROWS,
+                   CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_NONE, "(adj)");
     if (rc) return rc;
   }
   return resident ? launch_tc_epi<true>(s, ma, mb, md, p, grid, epi, post)
@@ -393,30 +403,16 @@ static int launch_screen(cudaStream_t s, const TcWorkspace& w, int64_t m, int64_
   return B2D_OK;
 }
 
-// fp32 row-major matrix [rows][k] with row pitch ld: box = 32 floats x 128 rows, SWIZZLE_128B
-static int make_f32_map(CUtensorMap* map, const float* base, int64_t rows, int64_t k, int64_t ld)
-{
-  EncodeTiledFn enc = get_encode();
-  if (!enc) return fail(B2D_ERR_CUDA, "cuTensorMapEncodeTiled entry point unavailable (no CUDA driver?)");
-  cuuint64_t dims[2]    = {static_cast<cuuint64_t>(k), static_cast<cuuint64_t>(rows)};
-  cuuint64_t strides[1] = {static_cast<cuuint64_t>(ld) * 4};
-  cuuint32_t box[2]     = {UX_KB, UX_BM};
-  cuuint32_t estr[2]    = {1, 1};
-  CUresult r = enc(map, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, const_cast<float*>(base), dims, strides, box, estr,
-                   CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                   CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  if (r != CUDA_SUCCESS) return fail(B2D_ERR_CUDA, "cuTensorMapEncodeTiled(f32 operand) failed: " + std::to_string((int)r));
-  return B2D_OK;
-}
-
 template <int kMetric>
 static int launch_ux_inst(cudaStream_t s, const UxParams& p, int64_t tiles)
 {
-  if (p.vec_x && p.vec_y) {  // TMA-legal operands: hardware-staged tiles
+  if (p.vec_x && p.vec_y) {  // TMA-legal operands: hardware-staged tiles of 32 floats x 128 rows, SWIZZLE_128B
     CUtensorMap mx, my;
-    int rc = make_f32_map(&mx, p.x, p.m, p.k, p.xrs);
+    int rc = encode_2d(&mx, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, p.x, p.k, p.m, p.xrs * 4, UX_KB, UX_BM,
+                       CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, "(f32 operand)");
     if (rc) return rc;
-    rc = make_f32_map(&my, p.y, p.n, p.k, p.yrs);
+    rc = encode_2d(&my, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, p.y, p.k, p.n, p.yrs * 4, UX_KB, UX_BM,
+                   CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, "(f32 operand)");
     if (rc) return rc;
     B2D_CUDA(cudaFuncSetAttribute(unexpanded_tma_kernel<kMetric>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                   UX_TMA_SMEM_BYTES));
@@ -533,8 +529,8 @@ static int pairwise_f64(cudaStream_t s, int metric, const double* x, int64_t xrs
                         int64_t ycs, double* dist, int64_t ldd, int64_t m, int64_t n, int64_t k, int swapped, double metric_arg,
                         void* workspace, size_t workspace_bytes)
 {
-  const size_t need = align_up(static_cast<size_t>(m + n) * 16, 1024);
-  if (!workspace || workspace_bytes < need) return fail(B2D_ERR_WORKSPACE, "workspace too small: need " + std::to_string(need) + " bytes");
+  const int rc = check_workspace(workspace, workspace_bytes, align_up(static_cast<size_t>(m + n) * 16, 1024), 1);
+  if (rc) return rc;
   double* xs = static_cast<double*>(workspace);
   double* ys = xs + 2 * m;
   f64_row_stats_kernel<<<static_cast<unsigned>((m + 7) / 8), 256, 0, s>>>(xs, x, xrs, xcs, m, static_cast<int>(k));
@@ -612,22 +608,19 @@ struct SkLayout {
 
 static SkLayout sk_layout(void* base, const SkPlan& p, int64_t rows, int64_t k)
 {
+  Carve c(base, 256);
   SkLayout w;
-  auto take = [&](size_t b) {
-    char* at = base ? static_cast<char*>(base) + w.bytes : nullptr;
-    w.bytes  = align_up(w.bytes + b, 256);
-    return at;
-  };
   if (p.layout == SK_SPLIT) {
-    w.st   = reinterpret_cast<SkState*>(take(static_cast<size_t>(rows) * sizeof(SkState)));
-    w.hist = reinterpret_cast<uint32_t*>(take(static_cast<size_t>(rows) * kSkBuckets * 4));
+    w.st   = c.take<SkState>(rows);
+    w.hist = c.take<uint32_t>(static_cast<size_t>(rows) * kSkBuckets);
   }
-  if (p.list) w.list = reinterpret_cast<uint64_t*>(take(static_cast<size_t>(rows) * k * 8));
+  if (p.list) w.list = c.take<uint64_t>(static_cast<size_t>(rows) * k);
   if (p.cub) {
-    w.alt = reinterpret_cast<uint64_t*>(take(static_cast<size_t>(p.batch) * k * 8));
-    w.off = reinterpret_cast<int*>(take(static_cast<size_t>(p.batch + 1) * 4));
-    w.tmp = take(kSkCubTmp);
+    w.alt = c.take<uint64_t>(static_cast<size_t>(p.batch) * k);
+    w.off = c.take<int>(p.batch + 1);
+    w.tmp = c.take<char>(kSkCubTmp);
   }
+  w.bytes = c.bytes;
   return w;
 }
 
@@ -747,10 +740,8 @@ int b2d_pairwise_distance(void* stream, int metric, int dtype, const void* x, in
   else { xa = y; ya = x; ma = n; na = m; xrs = 1; xcs = ldy; yrs = 1; ycs = ldx; }
 
   if (is_expanded(metric)) {
-    const size_t need = tc_layout(nullptr, ma, na, k, false).bytes;
-    if (!workspace || workspace_bytes < need)
-      return fail(B2D_ERR_WORKSPACE, "workspace too small: need " + std::to_string(need) + " bytes");
-    if (reinterpret_cast<uintptr_t>(workspace) % 256) return fail(B2D_ERR_INVALID_ARG, "workspace must be 256-byte aligned");
+    int rc = check_workspace(workspace, workspace_bytes, tc_layout(nullptr, ma, na, k, false).bytes);
+    if (rc) return rc;
     TcWorkspace w = tc_layout(workspace, ma, na, k, false);
     int mode = PREP_L2, center = 0, post = POST_NONE, xform = 0;
     float coef_mul = 1.f, tx_const = 0.f;
@@ -763,11 +754,11 @@ int b2d_pairwise_distance(void* stream, int metric, int dtype, const void* x, in
     else if (metric == B2D_JaccardExpanded) { mode = PREP_INNER_NORM; post = POST_JACCARD; }
     else if (metric == B2D_DiceExpanded) { mode = PREP_INNER_NORM; post = POST_DICE; }
     else { mode = PREP_INNER; }
-    int rc = dtype == B2D_F32
-               ? launch_prep<float>(s, w, xa, xrs, xcs, ma, ya, yrs, ycs, na, k, nullptr, nullptr, mode, center, xform,
-                                    coef_mul, tx_const)
-               : launch_prep<__half>(s, w, xa, xrs, xcs, ma, ya, yrs, ycs, na, k, nullptr, nullptr, mode, center, xform,
-                                     coef_mul, tx_const);
+    rc = dtype == B2D_F32
+           ? launch_prep<float>(s, w, xa, xrs, xcs, ma, ya, yrs, ycs, na, k, nullptr, nullptr, mode, center, xform,
+                                coef_mul, tx_const)
+           : launch_prep<__half>(s, w, xa, xrs, xcs, ma, ya, yrs, ycs, na, k, nullptr, nullptr, mode, center, xform,
+                                 coef_mul, tx_const);
     if (rc) return rc;
     TcParams p;
     memset(&p, 0, sizeof(p));
@@ -930,10 +921,8 @@ static int fused_nn_keys(void* stream, int64_t* keys, const float* x, int64_t ld
   if (!keys || !x || (n > 0 && !y)) return fail(B2D_ERR_INVALID_ARG, "null keys / x / y");
   if (ldx < k || ldy < k) return fail(B2D_ERR_INVALID_ARG, "leading dimension smaller than k");
   if (n + idx_offset > 0xFFFFFFFFll || idx_offset < 0) return fail(B2D_ERR_INVALID_ARG, "index range exceeds 32 bits");
-  const size_t need = tc_layout(nullptr, m, n, k, true).bytes;
-  if (!workspace || workspace_bytes < need)
-    return fail(B2D_ERR_WORKSPACE, "workspace too small: need " + std::to_string(need) + " bytes");
-  if (reinterpret_cast<uintptr_t>(workspace) % 256) return fail(B2D_ERR_INVALID_ARG, "workspace must be 256-byte aligned");
+  const int rc = check_workspace(workspace, workspace_bytes, tc_layout(nullptr, m, n, k, true).bytes);
+  if (rc) return rc;
   const bool screen_off = g_nn_screen.load(std::memory_order_relaxed) == 0;
   if (init_keys) {
     minloc_init_kernel<<<static_cast<unsigned>((m + 255) / 256), 256, 0, s>>>(reinterpret_cast<long long*>(keys), m);
@@ -980,25 +969,34 @@ int b2d_fused_l2_nn_finalize(void* stream, b2d_kvp_if* out, const int64_t* keys,
   return B2D_OK;
 }
 
-int b2d_fused_l2_nn(void* stream, b2d_kvp_if* out, const float* x, int64_t ldx, const float* y, int64_t ldy,
-                    const float* xn, const float* yn, int64_t m, int64_t n, int64_t k, int do_sqrt, int init_out,
-                    void* workspace, size_t workspace_bytes)
+// fusedL2NN and fusedDistanceNN: the keys of every row in the workspace, then unpacked into out.  (The cosine family,
+// mode PREP_COSINE: rows are normalised in prep, keys hold -cos, the row term t_x = 1 turns it into 1 - cos.)
+static int fused_nn(void* stream, b2d_kvp_if* out, const float* x, int64_t ldx, const float* y, int64_t ldy,
+                    const float* xn, const float* yn, int64_t m, int64_t n, int64_t k, int mode, int center, int do_sqrt,
+                    int init_out, void* workspace, size_t workspace_bytes)
 {
   cudaStream_t s = static_cast<cudaStream_t>(stream);
   if (m < 0 || n < 0 || k < 0) return fail(B2D_ERR_INVALID_ARG, "negative extent");
   if (m == 0) return B2D_OK;
   if (!out) return fail(B2D_ERR_INVALID_ARG, "null out");
-  const size_t need = tc_layout(nullptr, m, n, k, true).bytes;
-  if (!workspace || workspace_bytes < need)
-    return fail(B2D_ERR_WORKSPACE, "workspace too small: need " + std::to_string(need) + " bytes");
+  // (the alignment is checked by fused_nn_keys, after the rest of its arguments)
+  int rc = check_workspace(workspace, workspace_bytes, tc_layout(nullptr, m, n, k, true).bytes, 1);
+  if (rc) return rc;
   TcWorkspace w = tc_layout(workspace, m, n, k, true);
-  int rc = b2d_fused_l2_nn_keys(stream, reinterpret_cast<int64_t*>(w.keys), x, ldx, y, ldy, xn, yn, m, n, k, 0, 1,
-                                workspace, workspace_bytes);
+  rc = fused_nn_keys(stream, reinterpret_cast<int64_t*>(w.keys), x, ldx, y, ldy, xn, yn, m, n, k, 0, 1, workspace,
+                     workspace_bytes, mode, center);
   if (rc) return rc;
   minloc_finalize_kernel<<<static_cast<unsigned>((m + 255) / 256), 256, 0, s>>>(
     reinterpret_cast<KvpIF*>(out), w.keys, m, do_sqrt, init_out ? 0 : 1);
   B2D_CUDA(cudaGetLastError());
   return B2D_OK;
+}
+
+int b2d_fused_l2_nn(void* stream, b2d_kvp_if* out, const float* x, int64_t ldx, const float* y, int64_t ldy,
+                    const float* xn, const float* yn, int64_t m, int64_t n, int64_t k, int do_sqrt, int init_out,
+                    void* workspace, size_t workspace_bytes)
+{
+  return fused_nn(stream, out, x, ldx, y, ldy, xn, yn, m, n, k, PREP_L2, 0, do_sqrt, init_out, workspace, workspace_bytes);
 }
 
 // ------------------------------------------------------------------------------------------
@@ -1092,27 +1090,13 @@ int b2d_fused_distance_nn(void* stream, b2d_kvp_if* out, int metric, const float
                           int64_t ldy, const float* xn, const float* yn, int64_t m, int64_t n, int64_t k, int init_out,
                           void* workspace, size_t workspace_bytes)
 {
-  cudaStream_t s = static_cast<cudaStream_t>(stream);
   if (metric == B2D_L2Expanded || metric == B2D_L2SqrtExpanded)
     return b2d_fused_l2_nn(stream, out, x, ldx, y, ldy, xn, yn, m, n, k, metric == B2D_L2SqrtExpanded ? 1 : 0, init_out,
                            workspace, workspace_bytes);
   if (metric != B2D_CosineExpanded && metric != B2D_CorrelationExpanded)
     return fail(B2D_ERR_UNSUPPORTED, "fusedDistanceNN supports L2Expanded, L2SqrtExpanded, CosineExpanded, CorrelationExpanded");
-  if (m < 0 || n < 0 || k < 0) return fail(B2D_ERR_INVALID_ARG, "negative extent");
-  if (m == 0) return B2D_OK;
-  if (!out) return fail(B2D_ERR_INVALID_ARG, "null out");
-  const size_t need = tc_layout(nullptr, m, n, k, true).bytes;
-  if (!workspace || workspace_bytes < need)
-    return fail(B2D_ERR_WORKSPACE, "workspace too small: need " + std::to_string(need) + " bytes");
-  TcWorkspace w = tc_layout(workspace, m, n, k, true);
-  // cosine family: rows are normalised in prep, keys hold -cos, the row term t_x = 1 turns it into 1 - cos
-  int rc = fused_nn_keys(stream, reinterpret_cast<int64_t*>(w.keys), x, ldx, y, ldy, nullptr, nullptr, m, n, k, 0, 1,
-                         workspace, workspace_bytes, PREP_COSINE, metric == B2D_CorrelationExpanded ? 1 : 0);
-  if (rc) return rc;
-  minloc_finalize_kernel<<<static_cast<unsigned>((m + 255) / 256), 256, 0, s>>>(
-    reinterpret_cast<KvpIF*>(out), w.keys, m, 0, init_out ? 0 : 1);
-  B2D_CUDA(cudaGetLastError());
-  return B2D_OK;
+  return fused_nn(stream, out, x, ldx, y, ldy, nullptr, nullptr, m, n, k, PREP_COSINE,
+                  metric == B2D_CorrelationExpanded ? 1 : 0, 0, init_out, workspace, workspace_bytes);
 }
 
 // ------------------------------------------------------------------------------------------
@@ -1131,21 +1115,15 @@ struct MaskedLayout {
 
 static MaskedLayout masked_layout(void* base, int64_t m, int64_t n, int64_t k, int64_t G)
 {
+  Carve c(base, 1024);
   MaskedLayout L;
-  L.w        = tc_layout(base, m, n, k, false);
-  size_t off = L.w.bytes;
-  auto take  = [&](size_t b) {
-    size_t o = off;
-    off += align_up(b, 1024);
-    return o;
-  };
-  char* c   = static_cast<char*>(base);
-  L.w.keys  = reinterpret_cast<long long*>(c + take(static_cast<size_t>(m) * 8));
-  L.bad     = reinterpret_cast<unsigned*>(c + take(32));
-  L.grp     = reinterpret_cast<int*>(c + take(static_cast<size_t>(n) * 4));
-  L.bits    = reinterpret_cast<unsigned*>(c + take(static_cast<size_t>((m + 31) / 32) * G * 4));
-  L.cls     = reinterpret_cast<uint8_t*>(c + take(static_cast<size_t>((m + TC_BM - 1) / TC_BM) * ((n + TC_BN - 1) / TC_BN)));
-  L.bytes   = off;
+  L.w      = tc_layout(c, m, n, k, false);
+  L.w.keys = c.take<long long>(m);
+  L.bad    = c.take<unsigned>(8);
+  L.grp    = c.take<int>(n);
+  L.bits   = c.take<unsigned>(static_cast<size_t>((m + 31) / 32) * G);
+  L.cls    = c.take<uint8_t>(static_cast<size_t>((m + TC_BM - 1) / TC_BM) * ((n + TC_BN - 1) / TC_BN));
+  L.bytes  = c.bytes;
   return L;
 }
 
@@ -1170,10 +1148,8 @@ int b2d_masked_l2_nn(void* stream, b2d_kvp_if* out, const float* x, int64_t ldx,
   if (ld_adj < G) return fail(B2D_ERR_INVALID_ARG, "ld_adj smaller than num_groups");
   if (ldx < k || ldy < k) return fail(B2D_ERR_INVALID_ARG, "leading dimension smaller than k");
   if (m > 0x7fffffffll || n > 0x7fffffffll || G > 0x7fffffffll) return fail(B2D_ERR_INVALID_ARG, "index range exceeds 32 bits");
-  const size_t need = masked_layout(nullptr, m, n, k, G).bytes;
-  if (!workspace || workspace_bytes < need)
-    return fail(B2D_ERR_WORKSPACE, "workspace too small: need " + std::to_string(need) + " bytes");
-  if (reinterpret_cast<uintptr_t>(workspace) % 256) return fail(B2D_ERR_INVALID_ARG, "workspace must be 256-byte aligned");
+  int rc = check_workspace(workspace, workspace_bytes, masked_layout(nullptr, m, n, k, G).bytes);
+  if (rc) return rc;
   MaskedLayout L = masked_layout(workspace, m, n, k, G);
   const unsigned mblocks = static_cast<unsigned>((m + 255) / 256);
   minloc_init_kernel<<<mblocks, 256, 0, s>>>(L.w.keys, m);
@@ -1181,7 +1157,7 @@ int b2d_masked_l2_nn(void* stream, b2d_kvp_if* out, const float* x, int64_t ldx,
   masked_validate_kernel<<<1, 1024, 0, s>>>(L.bad, group_idxs, G, n);
   B2D_CUDA(cudaGetLastError());
   if (n > 0 && G > 0) {
-    int rc = launch_prep<float>(s, L.w, x, ldx, 1, m, y, ldy, 1, n, k, xn, yn, PREP_L2, 0);
+    rc = launch_prep<float>(s, L.w, x, ldx, 1, m, y, ldy, 1, n, k, xn, yn, PREP_L2, 0);
     if (rc) return rc;
     masked_group_map_kernel<<<static_cast<unsigned>((n + 255) / 256), 256, 0, s>>>(L.grp, group_idxs, G, n);
     B2D_CUDA(cudaGetLastError());
@@ -1211,32 +1187,56 @@ int b2d_masked_l2_nn(void* stream, b2d_kvp_if* out, const float* x, int64_t ldx,
 // Fused brute-force kNN (SURVEY.md 8(f2)): raft::neighbors::brute_force::knn / fused_l2_knn for the
 // L2 metrics without ever writing the m x n matrix (expanded_tc.cuh, EPI_TOPK).
 
-static size_t knn_topk_offset(int64_t m, int64_t n, int64_t k) { return align_up(tc_layout(nullptr, m, n, k, true).bytes, 1024); }
+// The tensor-core workspace with keys, then the kNN's own regions.  Two regions of the tensor workspace are borrowed:
+// thr and cnt live in aux ([m] floats, then [m] counters: 8 of its 16 bytes per row), and the per-row candidate lists
+// (KNN_CAP entries of 8 bytes per row) in cand, which b2d_knn guards with m * KNN_CAP <= cand_cap.
+namespace {
+struct KnnLayout {
+  TcWorkspace w;
+  long long* topk;      // [m][n_neighbors]
+  float* thr;           // [m]
+  unsigned* cnt;        // [m]
+  long long* dropmin;   // [m] best key that did not fit into a row's list this pass
+  int* dirty;           // [m] rows to redo for the current pass
+  unsigned* repaired;   // [m] 1 once a row has been repaired in some pass
+  int* rep_list;        // [m] the repaired rows ...
+  unsigned* dirty_cnt;  // [64] one counter per pass
+  unsigned* rep_cnt;    // [1] ... and their count, right behind dirty_cnt
+  size_t bytes;
+};
+}  // namespace
+
+static KnnLayout knn_layout(void* base, int64_t m, int64_t n, int64_t k, int64_t n_neighbors)
+{
+  Carve c(base, 1024);
+  KnnLayout L;
+  L.w         = tc_layout(c, m, n, k, true);
+  L.thr       = reinterpret_cast<float*>(L.w.aux);
+  L.cnt       = L.w.aux ? reinterpret_cast<unsigned*>(L.w.aux) + m : nullptr;
+  L.topk      = c.take<long long>(static_cast<size_t>(m) * n_neighbors);
+  L.dropmin   = c.take<long long>(m);
+  L.dirty     = c.take<int>(m);
+  L.repaired  = c.take<unsigned>(m);
+  L.rep_list  = c.take<int>(m);
+  L.dirty_cnt = c.take<unsigned>(65);
+  L.rep_cnt   = L.dirty_cnt ? L.dirty_cnt + 64 : nullptr;
+  L.bytes     = c.bytes;
+  return L;
+}
 
 size_t b2d_knn_l2_workspace_bytes(int64_t m, int64_t n, int64_t k, int64_t n_neighbors)
 {
   if (m < 0 || n < 0 || k < 0 || n_neighbors < 1 || n_neighbors > KNN_MAX_K) return static_cast<size_t>(-1);
-  return knn_topk_offset(m, n, k) + align_up(static_cast<size_t>(m) * n_neighbors * 8, 1024) +
-         align_up(static_cast<size_t>(m) * 8, 1024) + 3 * align_up(static_cast<size_t>(m) * 4, 1024) +
-         1024;  // + dropmin, dirty list, repaired flags, repaired-row list, counters
+  return knn_layout(nullptr, m, n, k, n_neighbors).bytes;
 }
 
 namespace {
 struct KnnCtx {
   cudaStream_t s;
-  TcWorkspace w;
+  KnnLayout L;
   TcParams p;       // m, knn_* set; n / idx_offset per pass
   int64_t k;
   int nkb;
-  long long* topk;
-  float* thr;
-  unsigned* cnt;
-  long long* dropmin;   // [m] best key that did not fit into a row's list this pass
-  int* dirty;           // [m] rows to redo for the current pass
-  unsigned* dirty_cnt;  // [64] one counter per pass
-  unsigned* repaired;   // [m] 1 once a row has been repaired in some pass
-  int* rep_list;        // [m] the repaired rows ...
-  unsigned* rep_cnt;    // ... and their count
   bool any_fix;         // a knn_fix_kernel was launched
   int pass;
   const float* x; int64_t ldx;
@@ -1250,24 +1250,25 @@ struct KnnCtx {
 // that matters (knn_merge_kernel / knn_fix_kernel) -- all on the device: the call only enqueues work
 static int knn_pass(KnnCtx& c, int64_t off, int64_t width)
 {
-  TcWorkspace w2 = c.w;
-  w2.yop         = c.w.yop + static_cast<size_t>(off) * c.nkb * 64;
-  w2.yt          = c.w.yt + off;
-  w2.ysc         = c.w.ysc + off;
+  const KnnLayout& L = c.L;
+  TcWorkspace w2 = L.w;
+  w2.yop         = L.w.yop + static_cast<size_t>(off) * c.nkb * 64;
+  w2.yt          = L.w.yt + off;
+  w2.ysc         = L.w.ysc + off;
   TcParams p     = c.p;
   p.n            = width;
   p.idx_offset   = off;
   int rc         = launch_tc(c.s, w2, p, c.k, EPI_TOPK, POST_NONE);
   if (rc) return rc;
-  unsigned* dc = c.dirty_cnt + (c.pass & 63);
-  knn_merge_kernel<<<static_cast<unsigned>((c.p.m + 7) / 8), 256, 0, c.s>>>(c.topk, c.p.knn_cand, c.cnt, c.thr, c.dropmin, c.dirty,
-                                                                            dc, c.repaired, c.rep_list, c.rep_cnt, c.p.m, c.kk);
+  unsigned* dc = L.dirty_cnt + (c.pass & 63);
+  knn_merge_kernel<<<static_cast<unsigned>((c.p.m + 7) / 8), 256, 0, c.s>>>(L.topk, c.p.knn_cand, L.cnt, L.thr, L.dropmin, L.dirty,
+                                                                            dc, L.repaired, L.rep_list, L.rep_cnt, c.p.m, c.kk);
   B2D_CUDA(cudaGetLastError());
   if (width > KNN_CAP) {  // (a pass of at most KNN_CAP columns cannot overflow)
     int sms = 0;
     rc = device_sms(&sms);
     if (rc) return rc;
-    knn_fix_kernel<<<sms * 2, 256, 0, c.s>>>(c.topk, c.thr, c.dirty, dc, c.x, c.ldx, c.y, c.ldy, static_cast<int>(c.k), c.kk, off,
+    knn_fix_kernel<<<sms * 2, 256, 0, c.s>>>(L.topk, L.thr, L.dirty, dc, c.x, c.ldx, c.y, c.ldy, static_cast<int>(c.k), c.kk, off,
                                              width, c.family, c.center);
     B2D_CUDA(cudaGetLastError());
     c.any_fix = true;
@@ -1303,45 +1304,29 @@ int b2d_knn(void* stream, int64_t* out_idx, float* out_dist, int metric, const f
   if (!out_idx || !out_dist || !x || !y) return fail(B2D_ERR_INVALID_ARG, "null out / x / y");
   if (ldx < k || ldy < k) return fail(B2D_ERR_INVALID_ARG, "leading dimension smaller than k");
   if (n > 0xFFFFFFFFll) return fail(B2D_ERR_INVALID_ARG, "index range exceeds 32 bits");
-  if (m * static_cast<int64_t>(KNN_CAP) > tc_layout(nullptr, m, n, k, true).cand_cap)
+  const KnnLayout need = knn_layout(nullptr, m, n, k, n_neighbors);
+  if (m * static_cast<int64_t>(KNN_CAP) > need.w.cand_cap)
     return fail(B2D_ERR_UNSUPPORTED, "kNN: too many query rows for one call (m * 128 must stay below 2^31): split the queries");
-  const size_t need = b2d_knn_l2_workspace_bytes(m, n, k, n_neighbors);
-  if (!workspace || workspace_bytes < need)
-    return fail(B2D_ERR_WORKSPACE, "workspace too small: need " + std::to_string(need) + " bytes");
-  if (reinterpret_cast<uintptr_t>(workspace) % 256) return fail(B2D_ERR_INVALID_ARG, "workspace must be 256-byte aligned");
+  int rc = check_workspace(workspace, workspace_bytes, need.bytes);
+  if (rc) return rc;
   KnnCtx c;
   c.s   = s;
-  c.w   = tc_layout(workspace, m, n, k, true);
+  c.L   = knn_layout(workspace, m, n, k, n_neighbors);
   c.k   = k;
   c.nkb = static_cast<int>((k + 31) / 32);
   c.kk  = static_cast<int>(n_neighbors);
-  c.topk     = reinterpret_cast<long long*>(static_cast<char*>(workspace) + knn_topk_offset(m, n, k));
-  c.thr      = reinterpret_cast<float*>(c.w.aux);          // [m] floats ...
-  c.cnt      = reinterpret_cast<unsigned*>(c.w.aux) + m;   // ... and [m] counters share the aux block (8 B per row)
-  {
-    char* q     = reinterpret_cast<char*>(c.topk) + align_up(static_cast<size_t>(m) * n_neighbors * 8, 1024);
-    c.dropmin   = reinterpret_cast<long long*>(q);
-    q += align_up(static_cast<size_t>(m) * 8, 1024);
-    c.dirty     = reinterpret_cast<int*>(q);
-    q += align_up(static_cast<size_t>(m) * 4, 1024);
-    c.repaired  = reinterpret_cast<unsigned*>(q);
-    q += align_up(static_cast<size_t>(m) * 4, 1024);
-    c.rep_list  = reinterpret_cast<int*>(q);
-    q += align_up(static_cast<size_t>(m) * 4, 1024);
-    c.dirty_cnt = reinterpret_cast<unsigned*>(q);
-    c.rep_cnt   = c.dirty_cnt + 64;
-  }
   c.pass = 0; c.any_fix = false; c.x = x; c.ldx = ldx; c.y = y; c.ldy = ldy;
   c.family = mode == PREP_COSINE ? 1 : 0; c.center = center;
-  int rc = launch_prep<float>(s, c.w, x, ldx, 1, m, y, ldy, 1, n, k, nullptr, nullptr, mode, center);
+  const KnnLayout& L = c.L;
+  rc = launch_prep<float>(s, L.w, x, ldx, 1, m, y, ldy, 1, n, k, nullptr, nullptr, mode, center);
   if (rc) return rc;
   const int64_t total = m * n_neighbors;
-  knn_init_kernel<<<static_cast<unsigned>((std::max<int64_t>(std::max<int64_t>(total, m), 65) + 255) / 256), 256, 0, s>>>(c.topk, c.thr, c.cnt, c.dropmin, c.dirty_cnt, c.repaired, m, c.kk);
+  knn_init_kernel<<<static_cast<unsigned>((std::max<int64_t>(std::max<int64_t>(total, m), 65) + 255) / 256), 256, 0, s>>>(L.topk, L.thr, L.cnt, L.dropmin, L.dirty_cnt, L.repaired, m, c.kk);
   B2D_CUDA(cudaGetLastError());
   memset(&c.p, 0, sizeof(c.p));
   c.p.m = m;
-  c.p.knn_thr = c.thr; c.p.knn_cnt = c.cnt; c.p.knn_cand = reinterpret_cast<long long*>(c.w.cand);
-  c.p.knn_cap = KNN_CAP; c.p.knn_dropmin = c.dropmin;
+  c.p.knn_thr = L.thr; c.p.knn_cnt = L.cnt; c.p.knn_cand = reinterpret_cast<long long*>(L.w.cand);
+  c.p.knn_cap = KNN_CAP; c.p.knn_dropmin = L.dropmin;
   // pass widths KNN_CAP, KNN_CAP, 2 KNN_CAP, 4 KNN_CAP, ...: with the k-th best of the s columns seen so far as
   // threshold, a pass over the next s columns appends ~n_neighbors entries per row on unordered data
   int64_t off = 0;
@@ -1355,11 +1340,11 @@ int b2d_knn(void* stream, int64_t* out_idx, float* out_dist, int metric, const f
     int sms = 0;
     rc = device_sms(&sms);
     if (rc) return rc;
-    knn_fix_kernel<<<sms * 2, 256, 0, s>>>(c.topk, c.thr, c.rep_list, c.rep_cnt, x, ldx, y, ldy, static_cast<int>(k), c.kk, 0, n,
+    knn_fix_kernel<<<sms * 2, 256, 0, s>>>(L.topk, L.thr, L.rep_list, L.rep_cnt, x, ldx, y, ldy, static_cast<int>(k), c.kk, 0, n,
                                            c.family, c.center);
     B2D_CUDA(cudaGetLastError());
   }
-  knn_finalize_kernel<<<static_cast<unsigned>((total + 255) / 256), 256, 0, s>>>(out_idx, out_dist, c.topk, total, do_sqrt);
+  knn_finalize_kernel<<<static_cast<unsigned>((total + 255) / 256), 256, 0, s>>>(out_idx, out_dist, L.topk, total, do_sqrt);
   B2D_CUDA(cudaGetLastError());
   return B2D_OK;
 }
@@ -1368,31 +1353,47 @@ int b2d_knn(void* stream, int64_t* out_idx, float* out_dist, int metric, const f
 // raft::stats::silhouette_score on the distance engine (SURVEY.md 8(f3); stats.cuh)
 
 namespace {
-struct SilLayout {
-  size_t counts, offsets, cursor, bad, total, where, ys, slab, pw, bytes;
+// silhouette and trustworthiness work through the n x n distances in [chunk x n] fp32 slabs, row pitch ld: chunk is the
+// caller's row count or about 1 GiB, a multiple of 128 and at most max(n, 1)
+struct Slab {
   int64_t chunk, ld;
-  size_t pw_bytes;
 };
-SilLayout sil_layout(int64_t n, int64_t k, int n_labels, int metric, int64_t chunk_rows)
+Slab slab_shape(int64_t n, int64_t chunk_rows)
 {
-  SilLayout L;
-  L.ld = (n + 3) / 4 * 4;
-  int64_t c = chunk_rows > 0 ? chunk_rows : (int64_t(1) << 30) / (4 * std::max<int64_t>(L.ld, 1));
+  Slab sl;
+  sl.ld     = (n + 3) / 4 * 4;
+  int64_t c = chunk_rows > 0 ? chunk_rows : (int64_t(1) << 30) / (4 * std::max<int64_t>(sl.ld, 1));
   c         = std::max<int64_t>(128, c / 128 * 128);
-  L.chunk   = std::min<int64_t>(c, std::max<int64_t>(n, 1));
-  size_t off = 0;
-  auto take  = [&](size_t b) { size_t o = off; off += align_up(b, 1024); return o; };
-  L.counts  = take(static_cast<size_t>(n_labels) * 4);
-  L.offsets = take(static_cast<size_t>(n_labels + 1) * 4);
-  L.cursor  = take(static_cast<size_t>(n_labels) * 4);
-  L.bad     = take(4);
-  L.total   = take(8);
-  L.where   = take(static_cast<size_t>(n) * 4);
-  L.ys      = take(static_cast<size_t>(n) * k * 4);
-  L.slab    = take(static_cast<size_t>(L.chunk) * L.ld * 4);
-  L.pw_bytes = b2d_pairwise_workspace_bytes(metric, B2D_F32, L.chunk, n, k);
-  L.pw      = take(L.pw_bytes == static_cast<size_t>(-1) ? 0 : L.pw_bytes);
-  L.bytes   = off;
+  sl.chunk  = std::min<int64_t>(c, std::max<int64_t>(n, 1));
+  return sl;
+}
+
+struct SilLayout {
+  Slab sl;
+  int *counts, *offsets, *cursor;  // zeroed together with bad and total: everything in front of where
+  unsigned* bad;
+  double* total;
+  int* where;
+  float *ys, *slab;
+  void* pw;                        // b2d_pairwise_distance's workspace
+  size_t pw_bytes, bytes;
+};
+SilLayout sil_layout(void* base, int64_t n, int64_t k, int n_labels, int metric, int64_t chunk_rows)
+{
+  Carve c(base, 1024);
+  SilLayout L;
+  L.sl       = slab_shape(n, chunk_rows);
+  L.counts   = c.take<int>(n_labels);
+  L.offsets  = c.take<int>(n_labels + 1);
+  L.cursor   = c.take<int>(n_labels);
+  L.bad      = c.take<unsigned>(1);
+  L.total    = c.take<double>(1);
+  L.where    = c.take<int>(n);
+  L.ys       = c.take<float>(static_cast<size_t>(n) * k);
+  L.slab     = c.take<float>(static_cast<size_t>(L.sl.chunk) * L.sl.ld);
+  L.pw_bytes = b2d_pairwise_workspace_bytes(metric, B2D_F32, L.sl.chunk, n, k);
+  L.pw       = c.take<char>(L.pw_bytes == static_cast<size_t>(-1) ? 0 : L.pw_bytes);
+  L.bytes    = c.bytes;
   return L;
 }
 }  // namespace
@@ -1401,7 +1402,7 @@ size_t b2d_silhouette_score_workspace_bytes(int64_t n, int64_t k, int n_labels, 
 {
   if (n < 0 || k < 0 || n_labels < 1 || chunk_rows < 0) return static_cast<size_t>(-1);
   if (b2d_pairwise_workspace_bytes(metric, B2D_F32, 1, 1, k) == static_cast<size_t>(-1)) return static_cast<size_t>(-1);
-  return sil_layout(n, k, n_labels, metric, chunk_rows).bytes;
+  return sil_layout(nullptr, n, k, n_labels, metric, chunk_rows).bytes;
 }
 
 int b2d_silhouette_score(void* stream, float* score, float* per_sample, const float* x, int64_t ldx, const int* labels,
@@ -1417,37 +1418,27 @@ int b2d_silhouette_score(void* stream, float* score, float* per_sample, const fl
   if (ldx < k) return fail(B2D_ERR_INVALID_ARG, "leading dimension smaller than k");
   const size_t need = b2d_silhouette_score_workspace_bytes(n, k, n_labels, metric, chunk_rows);
   if (need == static_cast<size_t>(-1)) return fail(B2D_ERR_UNSUPPORTED, "metric " + std::to_string(metric) + " is not on the tensor-core / SIMT distance path");
-  if (!workspace || workspace_bytes < need)
-    return fail(B2D_ERR_WORKSPACE, "workspace too small: need " + std::to_string(need) + " bytes");
-  if (reinterpret_cast<uintptr_t>(workspace) % 256) return fail(B2D_ERR_INVALID_ARG, "workspace must be 256-byte aligned");
-  const SilLayout L = sil_layout(n, k, n_labels, metric, chunk_rows);
-  char* base    = static_cast<char*>(workspace);
-  int* counts   = reinterpret_cast<int*>(base + L.counts);
-  int* offsets  = reinterpret_cast<int*>(base + L.offsets);
-  int* cursor   = reinterpret_cast<int*>(base + L.cursor);
-  unsigned* bad = reinterpret_cast<unsigned*>(base + L.bad);
-  double* total = reinterpret_cast<double*>(base + L.total);
-  int* where    = reinterpret_cast<int*>(base + L.where);
-  float* ys     = reinterpret_cast<float*>(base + L.ys);
-  float* slab   = reinterpret_cast<float*>(base + L.slab);
-  B2D_CUDA(cudaMemsetAsync(base, 0, L.where, s));  // counts, offsets, cursor, bad, total
+  int rc = check_workspace(workspace, workspace_bytes, need);
+  if (rc) return rc;
+  const SilLayout L = sil_layout(workspace, n, k, n_labels, metric, chunk_rows);
+  B2D_CUDA(cudaMemsetAsync(workspace, 0, reinterpret_cast<char*>(L.where) - static_cast<char*>(workspace), s));
   const unsigned nb = static_cast<unsigned>((n + 255) / 256);
-  sil_count_kernel<<<nb, 256, 0, s>>>(labels, counts, n, n_labels, bad);
-  sil_scan_kernel<<<1, 32, 0, s>>>(counts, offsets, cursor, n_labels);
-  sil_gather_kernel<<<static_cast<unsigned>((n + 7) / 8), 256, 0, s>>>(x, ldx, labels, cursor, ys, where, n, static_cast<int>(k), n_labels);
+  sil_count_kernel<<<nb, 256, 0, s>>>(labels, L.counts, n, n_labels, L.bad);
+  sil_scan_kernel<<<1, 32, 0, s>>>(L.counts, L.offsets, L.cursor, n_labels);
+  sil_gather_kernel<<<static_cast<unsigned>((n + 7) / 8), 256, 0, s>>>(x, ldx, labels, L.cursor, L.ys, L.where, n, static_cast<int>(k), n_labels);
   B2D_CUDA(cudaGetLastError());
   // labels outside [0, n_labels) are detected on the device (no host round trip: the call stays asynchronous);
   // they poison the result: *score and the per-sample values of the offending rows become NaN
-  for (int64_t r0 = 0; r0 < n; r0 += L.chunk) {
-    const int64_t rows = std::min<int64_t>(L.chunk, n - r0);
-    int rc = b2d_pairwise_distance(stream, metric, B2D_F32, x + r0 * ldx, ldx, ys, k, slab, L.ld, rows, n, k, 1, metric_arg,
-                                   base + L.pw, L.pw_bytes);
+  for (int64_t r0 = 0; r0 < n; r0 += L.sl.chunk) {
+    const int64_t rows = std::min<int64_t>(L.sl.chunk, n - r0);
+    rc = b2d_pairwise_distance(stream, metric, B2D_F32, x + r0 * ldx, ldx, L.ys, k, L.slab, L.sl.ld, rows, n, k, 1,
+                               metric_arg, L.pw, L.pw_bytes);
     if (rc) return rc;
     sil_row_kernel<<<static_cast<unsigned>(rows), 256, static_cast<size_t>(n_labels) * 4, s>>>(
-      slab, L.ld, r0, rows, labels, counts, offsets, where, n_labels, per_sample, total);
+      L.slab, L.sl.ld, r0, rows, labels, L.counts, L.offsets, L.where, n_labels, per_sample, L.total);
     B2D_CUDA(cudaGetLastError());
   }
-  sil_finish_kernel<<<1, 32, 0, s>>>(total, score, n, bad);
+  sil_finish_kernel<<<1, 32, 0, s>>>(L.total, score, n, L.bad);
   B2D_CUDA(cudaGetLastError());
   return B2D_OK;
 }
@@ -1455,29 +1446,28 @@ int b2d_silhouette_score(void* stream, float* score, float* per_sample, const fl
 // raft::stats::trustworthiness_score on the kNN + distance engine (stats.cuh)
 namespace {
 struct TrustLayout {
-  size_t penalty, emb_idx, emb_dist, slab, scratch, bytes;
-  int64_t chunk, ld;
-  size_t knn_bytes, pw_bytes;
+  Slab sl;
+  unsigned long long* penalty;
+  int64_t* emb_idx;
+  float *emb_dist, *slab;
+  void* scratch;    // the kNN's workspace, then b2d_pairwise_distance's
+  size_t knn_bytes, pw_bytes, bytes;
 };
-TrustLayout trust_layout(int64_t n, int64_t m, int64_t d, int n_neighbors, int metric, int64_t batch_rows)
+TrustLayout trust_layout(void* base, int64_t n, int64_t m, int64_t d, int n_neighbors, int metric, int64_t batch_rows)
 {
+  Carve c(base, 1024);
   TrustLayout L;
-  L.ld = (n + 3) / 4 * 4;
-  int64_t c = batch_rows > 0 ? batch_rows : (int64_t(1) << 30) / (4 * std::max<int64_t>(L.ld, 1));
-  c         = std::max<int64_t>(128, c / 128 * 128);
-  L.chunk   = std::min<int64_t>(c, std::max<int64_t>(n, 1));
-  size_t off = 0;
-  auto take  = [&](size_t b) { size_t o = off; off += align_up(b, 1024); return o; };
-  L.penalty  = take(8);
-  L.emb_idx  = take(static_cast<size_t>(n) * (n_neighbors + 1) * 8);
-  L.emb_dist = take(static_cast<size_t>(n) * (n_neighbors + 1) * 4);
-  L.slab     = take(static_cast<size_t>(L.chunk) * L.ld * 4);
+  L.sl        = slab_shape(n, batch_rows);
+  L.penalty   = c.take<unsigned long long>(1);
+  L.emb_idx   = c.take<int64_t>(static_cast<size_t>(n) * (n_neighbors + 1));
+  L.emb_dist  = c.take<float>(static_cast<size_t>(n) * (n_neighbors + 1));
+  L.slab      = c.take<float>(static_cast<size_t>(L.sl.chunk) * L.sl.ld);
   L.knn_bytes = b2d_knn_l2_workspace_bytes(n, n, d, n_neighbors + 1);
-  L.pw_bytes  = b2d_pairwise_workspace_bytes(metric, B2D_F32, L.chunk, n, m);
+  L.pw_bytes  = b2d_pairwise_workspace_bytes(metric, B2D_F32, L.sl.chunk, n, m);
   const size_t a = L.knn_bytes == static_cast<size_t>(-1) ? 0 : L.knn_bytes;
   const size_t b = L.pw_bytes == static_cast<size_t>(-1) ? 0 : L.pw_bytes;
-  L.scratch  = take(std::max(a, b));
-  L.bytes    = off;
+  L.scratch   = c.take<char>(std::max(a, b));
+  L.bytes     = c.bytes;
   return L;
 }
 }  // namespace
@@ -1487,7 +1477,7 @@ size_t b2d_trustworthiness_score_workspace_bytes(int64_t n, int64_t m, int64_t d
 {
   if (n < 0 || m < 0 || d < 0 || n_neighbors < 1 || n_neighbors + 1 > KNN_MAX_K || batch_rows < 0) return static_cast<size_t>(-1);
   if (b2d_pairwise_workspace_bytes(metric, B2D_F32, 1, 1, m) == static_cast<size_t>(-1)) return static_cast<size_t>(-1);
-  return trust_layout(n, m, d, n_neighbors, metric, batch_rows).bytes;
+  return trust_layout(nullptr, n, m, d, n_neighbors, metric, batch_rows).bytes;
 }
 
 int b2d_trustworthiness_score(void* stream, double* score, const float* x, int64_t ldx, const float* x_embedded,
@@ -1512,30 +1502,24 @@ int b2d_trustworthiness_score(void* stream, double* score, const float* x, int64
   if (ldx < m || lde < d) return fail(B2D_ERR_INVALID_ARG, "leading dimension smaller than the row length");
   const size_t need = b2d_trustworthiness_score_workspace_bytes(n, m, d, n_neighbors, metric, batch_rows);
   if (need == static_cast<size_t>(-1)) return fail(B2D_ERR_UNSUPPORTED, "metric " + std::to_string(metric) + " is not on the tensor-core / SIMT distance path");
-  if (!workspace || workspace_bytes < need)
-    return fail(B2D_ERR_WORKSPACE, "workspace too small: need " + std::to_string(need) + " bytes");
-  if (reinterpret_cast<uintptr_t>(workspace) % 256) return fail(B2D_ERR_INVALID_ARG, "workspace must be 256-byte aligned");
-  const TrustLayout L = trust_layout(n, m, d, n_neighbors, metric, batch_rows);
-  char* base = static_cast<char*>(workspace);
-  unsigned long long* penalty = reinterpret_cast<unsigned long long*>(base + L.penalty);
-  int64_t* emb_idx = reinterpret_cast<int64_t*>(base + L.emb_idx);
-  float* emb_dist  = reinterpret_cast<float*>(base + L.emb_dist);
-  float* slab      = reinterpret_cast<float*>(base + L.slab);
-  const int kk1    = n_neighbors + 1;
-  B2D_CUDA(cudaMemsetAsync(penalty, 0, 8, s));
-  // neighbours in the embedded space (the sample itself included, as in the reference)
-  int rc = b2d_knn(stream, emb_idx, emb_dist, knn_metric, x_embedded, lde, x_embedded, lde, n, n, d, kk1, base + L.scratch,
-                   L.knn_bytes);
+  int rc = check_workspace(workspace, workspace_bytes, need);
   if (rc) return rc;
-  for (int64_t r0 = 0; r0 < n; r0 += L.chunk) {
-    const int64_t rows = std::min<int64_t>(L.chunk, n - r0);
-    rc = b2d_pairwise_distance(stream, metric, B2D_F32, x + r0 * ldx, ldx, x, ldx, slab, L.ld, rows, n, m, 1, 2.0f,
-                               base + L.scratch, L.pw_bytes);
+  const TrustLayout L = trust_layout(workspace, n, m, d, n_neighbors, metric, batch_rows);
+  const int kk1       = n_neighbors + 1;
+  B2D_CUDA(cudaMemsetAsync(L.penalty, 0, 8, s));
+  // neighbours in the embedded space (the sample itself included, as in the reference)
+  rc = b2d_knn(stream, L.emb_idx, L.emb_dist, knn_metric, x_embedded, lde, x_embedded, lde, n, n, d, kk1, L.scratch,
+               L.knn_bytes);
+  if (rc) return rc;
+  for (int64_t r0 = 0; r0 < n; r0 += L.sl.chunk) {
+    const int64_t rows = std::min<int64_t>(L.sl.chunk, n - r0);
+    rc = b2d_pairwise_distance(stream, metric, B2D_F32, x + r0 * ldx, ldx, x, ldx, L.slab, L.sl.ld, rows, n, m, 1, 2.0f,
+                               L.scratch, L.pw_bytes);
     if (rc) return rc;
-    trust_rank_kernel<<<static_cast<unsigned>(rows), 256, 0, s>>>(slab, L.ld, r0, n, emb_idx, kk1, n_neighbors, penalty);
+    trust_rank_kernel<<<static_cast<unsigned>(rows), 256, 0, s>>>(L.slab, L.sl.ld, r0, n, L.emb_idx, kk1, n_neighbors, L.penalty);
     B2D_CUDA(cudaGetLastError());
   }
-  trust_finish_kernel<<<1, 1, 0, s>>>(penalty, score, n, n_neighbors);
+  trust_finish_kernel<<<1, 1, 0, s>>>(L.penalty, score, n, n_neighbors);
   B2D_CUDA(cudaGetLastError());
   return B2D_OK;
 }
@@ -1588,10 +1572,8 @@ int b2d_select_k(void* stream, const float* in_val, int64_t ld, const int64_t* i
   if (!in_val || !out_val || !out_idx) return fail(B2D_ERR_INVALID_ARG, "null in_val / out_val / out_idx");
   const bool mn    = select_min != 0;
   const SkPlan p   = sk_plan(rows, len, k);
-  const size_t need = sk_layout(nullptr, p, rows, k).bytes;
-  if (need && (!workspace || workspace_bytes < need))
-    return fail(B2D_ERR_WORKSPACE, "workspace too small: need " + std::to_string(need) + " bytes");
-  if (reinterpret_cast<uintptr_t>(workspace) % 256) return fail(B2D_ERR_INVALID_ARG, "workspace must be 256-byte aligned");
+  const int rc      = check_workspace(workspace, workspace_bytes, sk_layout(nullptr, p, rows, k).bytes);
+  if (rc) return rc;
   const SkLayout w = sk_layout(workspace, p, rows, k);
   const unsigned R = static_cast<unsigned>(rows);
   if (p.layout == SK_SORT_ROW) {
@@ -1665,10 +1647,8 @@ int b2d_eps_neighbors_l2sq(void* stream, uint8_t* adj, int64_t ld_adj, void* vd,
     if (!x || !y) return fail(B2D_ERR_INVALID_ARG, "null x / y");
     if (adj && ld_adj < n) return fail(B2D_ERR_INVALID_ARG, "ld_adj smaller than n");
     if (ldx < k || ldy < k) return fail(B2D_ERR_INVALID_ARG, "leading dimension smaller than k");
-    const size_t need = tc_layout(nullptr, m, n, k, false).bytes;
-    if (!workspace || workspace_bytes < need)
-      return fail(B2D_ERR_WORKSPACE, "workspace too small: need " + std::to_string(need) + " bytes");
-    if (reinterpret_cast<uintptr_t>(workspace) % 256) return fail(B2D_ERR_INVALID_ARG, "workspace must be 256-byte aligned");
+    const int rc = check_workspace(workspace, workspace_bytes, tc_layout(nullptr, m, n, k, false).bytes);
+    if (rc) return rc;
   }
   if (vd && init_vd) B2D_CUDA(cudaMemsetAsync(vd, 0, static_cast<size_t>(n + 1) * (vd_int64 ? 8 : 4), s));
   if (!work) return B2D_OK;

@@ -1,0 +1,138 @@
+"""Generates tests/golden/workspace_contract.json (run here, without a GPU; the output is committed).
+
+The fixture pins the workspace contract of the C ABI:
+  bytes   every *_workspace_bytes query over a grid that reaches every branch of the workspace layouts;
+  errors  (status, b2d_last_error()) of every entry point that takes a workspace, given a null workspace, one byte too
+          few at an aligned address, or the full size at an odd address -- with every other argument valid.
+Pointers are fake addresses: the calls must fail in validation, before anything reaches the device.  A case that
+returns B2D_OK or B2D_ERR_CUDA got past validation, so it is refused rather than recorded.  The library is the one
+raft_b200._lib loads (RAFT_B200_LIB selects another build of the same ABI).
+"""
+import json
+import os
+import sys
+
+HERE = os.path.dirname(os.path.abspath(__file__))
+sys.path.insert(0, os.path.dirname(os.path.dirname(HERE)))
+
+from raft_b200 import _lib  # noqa: E402
+
+OUT = os.path.join(HERE, "workspace_contract.json")
+
+METRICS = list(range(-1, 21))                   # every DistanceType value, 13 (Haversine) and two out of range
+DTYPES = [0, 1, 2, 3]                           # F32, F16, F64 and one unknown
+KS = [1, 31, 32, 33, 128, 129, 320, 321]
+NEG = [(-1, 29, 32), (37, -1, 32), (37, 29, -1)]
+NN_N = [1000, (1 << 20) - 1, 1 << 20, (1 << 20) + 1]   # around the 2^20-row chunk of the screened search
+BIG_M = 1 << 24                                 # 128 m + 2^19 > 2^31 - 1: the candidate list is clamped
+
+
+def byte_queries():
+    q = {}
+    edges = [(0, 29, 32), (37, 0, 32), (37, 29, 0)] + NEG
+    shapes = [(37, 29, k) for k in KS] + edges + [(BIG_M, 1000, 96)]
+    # every metric and dtype at one shape and the edges; every k for an expanded and an unexpanded metric
+    q["b2d_pairwise_workspace_bytes"] = [(mt, dt) + s for mt in METRICS for dt in DTYPES for s in [(37, 29, 33)] + edges] + \
+                                        [(mt, dt) + s for mt in (0, 3) for dt in DTYPES for s in shapes]
+    nn = [(m, n, k) for m in (1, 100) for n in NN_N for k in KS] + \
+         [(0, 29, 32), (37, 0, 32), (37, 29, 0), (BIG_M, 1000, 96), (BIG_M, 1 << 20, 128)] + NEG
+    q["b2d_fused_l2_nn_workspace_bytes"] = nn
+    q["b2d_eps_neighbors_l2sq_workspace_bytes"] = [s for s in shapes] + [(1000, 1 << 20, 128)]
+    # G = 0, G <= m / 32 and G > m / 32
+    q["b2d_masked_l2_nn_workspace_bytes"] = [(m, n, k, g) for m, n in ((1, 1), (1000, 3000), (4096, 777))
+                                             for k in (1, 32, 129, 320) for g in (0, 1, 20, 200)] + \
+                                            [(-1, 5, 8, 1), (5, -1, 8, 1), (5, 5, -1, 1), (5, 5, 8, -1), (0, 5, 8, 3)]
+    q["b2d_knn_l2_workspace_bytes"] = [(m, n, k, kk) for m in (1, 1000, BIG_M) for n in (64, 5000)
+                                       for k in (1, 32, 129, 320) for kk in (1, 64)] + \
+                                      [(100, 100, 32, 0), (100, 100, 32, 65), (-1, 5, 8, 1), (5, -1, 8, 1), (5, 5, -1, 1),
+                                       (0, 5, 8, 3)]
+    # default (0) and explicit chunk rows; L2Expanded, L1 (no pairwise scratch), Haversine (not supported)
+    q["b2d_silhouette_score_workspace_bytes"] = [(n, k, nl, mt, c) for n in (0, 1000, 300000) for k in (3, 129)
+                                                 for nl in (1, 50) for mt in (0, 3, 13)
+                                                 for c in (0, 1, 1000, 1 << 20)] + \
+                                                [(-1, 3, 2, 0, 0), (10, -1, 2, 0, 0), (10, 3, 0, 0, 0), (10, 3, 2, 0, -1)]
+    q["b2d_trustworthiness_score_workspace_bytes"] = [(n, m, d, kk, mt, b) for n in (0, 100, 300000) for m in (8, 129)
+                                                      for d in (2, 64) for kk in (1, 63) for mt in (0, 2, 13, 3)
+                                                      for b in (0, 1000)] + \
+                                                     [(100, 8, 2, 0, 0, 0), (100, 8, 2, 64, 0, 0), (-1, 8, 2, 5, 0, 0),
+                                                      (100, -1, 2, 5, 0, 0), (100, 8, -1, 5, 0, 0), (100, 8, 2, 5, 0, -1)]
+    # sort-row, radix-row (list in shared memory, list + cub), split (shared-memory sort, cub), cub in several batches
+    q["b2d_select_k_workspace_bytes"] = [
+        (100000, 1024, 32), (4, 2048, 2048), (16384, 100000, 1024), (264, 40000, 10), (300, 100000, 5000),
+        (1, 1 << 28, 1024), (2, 200000, 5), (263, 40000, 10), (1, 1 << 20, 5000), (2000, 1 << 20, 1 << 20),
+        (0, 5, 3), (0, 5, 0), (1, 5, 0), (1, 5, 6), (-1, 5, 1), (1, 1 << 31, 1), (1 << 31, 10, 1)]
+    return q
+
+
+D = 0x10000000                # fake data pointer
+WS = 0x20000000               # fake workspace, 256-byte aligned
+ODD = WS + 1                  # fake workspace at an odd address
+
+
+def error_cases(L):
+    """(name, function, arguments before the workspace pair, bytes needed, has an alignment check)"""
+    pw = L.b2d_pairwise_workspace_bytes
+    nn = L.b2d_fused_l2_nn_workspace_bytes
+    m, n, k = 300, 500, 96
+    return [
+        ("pairwise L2Expanded f32", "b2d_pairwise_distance", [None, 0, 0, D, k, D, k, D, n, m, n, k, 1, 2.0], pw(0, 0, m, n, k), True),
+        ("pairwise Cosine f16 col-major", "b2d_pairwise_distance", [None, 2, 1, D, m, D, n, D, m, m, n, k, 0, 2.0],
+         pw(2, 1, n, m, k), True),
+        ("pairwise L1 f64", "b2d_pairwise_distance", [None, 3, 2, D, k, D, k, D, n, m, n, k, 1, 2.0], pw(3, 2, m, n, k), False),
+        ("fused_l2_nn", "b2d_fused_l2_nn", [None, D, D, k, D, k, None, None, m, n, k, 1, 1], nn(m, n, k), True),
+        ("fused_distance_nn L2SqrtExpanded", "b2d_fused_distance_nn", [None, D, 1, D, k, D, k, None, None, m, n, k, 1],
+         nn(m, n, k), True),
+        ("fused_distance_nn CosineExpanded", "b2d_fused_distance_nn", [None, D, 2, D, k, D, k, None, None, m, n, k, 1],
+         nn(m, n, k), True),
+        ("fused_distance_nn CorrelationExpanded", "b2d_fused_distance_nn", [None, D, 10, D, k, D, k, None, None, m, n, k, 0],
+         nn(m, n, k), True),
+        ("fused_l2_nn_keys", "b2d_fused_l2_nn_keys", [None, D, D, k, D, k, None, None, m, n, k, 7, 1], nn(m, n, k), True),
+        ("fused_l2_nn_finalize", "b2d_fused_l2_nn_finalize", [None, D, D, m, 0], 1024 + 4 * m, False),
+        ("masked_l2_nn", "b2d_masked_l2_nn", [None, D, D, k, D, k, None, None, D, 16, D, 9, m, n, k, 0, 1],
+         L.b2d_masked_l2_nn_workspace_bytes(m, n, k, 9), True),
+        ("masked_l2_nn G=0", "b2d_masked_l2_nn", [None, D, D, k, D, k, None, None, None, 0, None, 0, m, n, k, 0, 1],
+         L.b2d_masked_l2_nn_workspace_bytes(m, n, k, 0), True),
+        ("knn CosineExpanded", "b2d_knn", [None, D, D, 2, D, k, D, k, m, n, k, 10], L.b2d_knn_l2_workspace_bytes(m, n, k, 10),
+         True),
+        ("knn_l2 sqrt", "b2d_knn_l2", [None, D, D, D, k, D, k, m, n, k, 64, 1], L.b2d_knn_l2_workspace_bytes(m, n, k, 64),
+         True),
+        ("silhouette L2Expanded", "b2d_silhouette_score", [None, D, D, D, k, D, n, k, 7, 0, 2.0, 0],
+         L.b2d_silhouette_score_workspace_bytes(n, k, 7, 0, 0), True),
+        ("silhouette L1 chunked", "b2d_silhouette_score", [None, D, None, D, k, D, n, k, 7, 3, 2.0, 128],
+         L.b2d_silhouette_score_workspace_bytes(n, k, 7, 3, 128), True),
+        ("trustworthiness L2SqrtUnexpanded", "b2d_trustworthiness_score", [None, D, D, k, D, 2, n, k, 2, 5, 5, 0],
+         L.b2d_trustworthiness_score_workspace_bytes(n, k, 2, 5, 5, 0), True),
+        ("select_k split", "b2d_select_k", [None, D, 200000, None, 2, 200000, 5, 1, D, D],
+         L.b2d_select_k_workspace_bytes(2, 200000, 5), True),
+        ("select_k radix-row cub", "b2d_select_k", [None, D, 100000, D, 300, 100000, 5000, 0, D, D],
+         L.b2d_select_k_workspace_bytes(300, 100000, 5000), True),
+        ("eps", "b2d_eps_neighbors_l2sq", [None, D, n, D, 0, 1, D, k, D, k, m, n, k, 4.0], L.b2d_eps_neighbors_l2sq_workspace_bytes(m, n, k),
+         True),
+    ]
+
+
+def main():
+    L = _lib.lib()
+    out = {"bytes": {}, "errors": []}
+    for fn, cases in byte_queries().items():
+        out["bytes"][fn] = [list(a) + [getattr(L, fn)(*a)] for a in cases]
+    for name, fn, args, need, aligned in error_cases(L):
+        assert 0 < need < 2 ** 63, (name, need)
+        variants = [("null", None, need), ("short", WS, need - 1)] + ([("odd", ODD, need)] if aligned else [])
+        for case, ws, nbytes in variants:
+            a = args + [ws, nbytes]
+            rc = getattr(L, fn)(*a)
+            if rc in (_lib.B2D_OK, _lib.B2D_ERR_CUDA):
+                raise SystemExit(f"{name} / {case}: status {rc} -- the call got past validation; not recorded")
+            out["errors"].append({"name": name, "case": case, "fn": fn, "args": a, "rc": rc,
+                                  "msg": L.b2d_last_error().decode()})
+    with open(OUT, "w") as f:   # one case per line, so that a change to the contract reads as a short diff
+        f.write('{"bytes": {\n')
+        f.write(",\n".join(json.dumps(fn) + ": [\n" + ",\n".join(json.dumps(r) for r in rows) + "]"
+                           for fn, rows in out["bytes"].items()))
+        f.write('},\n"errors": [\n' + ",\n".join(json.dumps(e) for e in out["errors"]) + "]}\n")
+    print("wrote", OUT, sum(map(len, out["bytes"].values())), "size queries,", len(out["errors"]), "error cases")
+
+
+if __name__ == "__main__":
+    main()
