@@ -27,5 +27,18 @@ enum DistanceType : unsigned short {
   DiceExpanded        = 19,
   Precomputed         = 100
 };
+
+namespace kernels {
+// raft::distance::kernels::KernelType / KernelParams ([RECALLED] raft/distance/distance_types.hpp, <= 25.12): the kernel
+// of a Gram matrix (raft/distance/kernels.cuh) and its parameters, gamma the gain and coef0 the offset
+enum KernelType { LINEAR, POLYNOMIAL, RBF, TANH };
+
+struct KernelParams {
+  KernelType kernel;
+  int degree;
+  double gamma;
+  double coef0;
+};
+}  // namespace kernels
 }  // namespace distance
 }  // namespace raft

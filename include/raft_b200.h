@@ -219,7 +219,7 @@ int b2d_trustworthiness_score(void* stream, double* score, const float* x, int64
                               size_t workspace_bytes);
 
 /* Measurement aid (bench.py's roofline): between b2d_profile_begin(capacity) and b2d_profile_end every
- * b2d_pairwise_distance call on the tensor path records a CUDA-event pair on ITS stream around its main
+ * b2d_pairwise_distance (and b2d_gram_matrix) call on the tensor path records a CUDA-event pair on ITS stream around its main
  * kernel launch(es) (operand preparation excluded).  Nothing synchronises until b2d_profile_end, which
  * waits for the recorded events and returns the durations in call order (milliseconds). */
 int b2d_profile_begin(int capacity);
@@ -269,6 +269,28 @@ size_t b2d_eps_neighbors_l2sq_workspace_bytes(int64_t m, int64_t n, int64_t k);
 int b2d_eps_neighbors_l2sq(void* stream, uint8_t* adj, int64_t ld_adj, void* vd, int vd_int64, int init_vd,
                            const float* x, int64_t ldx, const float* y, int64_t ldy, int64_t m, int64_t n, int64_t k,
                            float eps, void* workspace, size_t workspace_bytes);
+
+/* raft::distance::kernels::KernelType ([RECALLED] raft/distance/distance_types.hpp, <= 25.12) */
+enum { B2D_KERNEL_LINEAR = 0, B2D_KERNEL_POLYNOMIAL = 1, B2D_KERNEL_RBF = 2, B2D_KERNEL_TANH = 3 };
+
+/* raft::distance::kernels Gram matrices (GramMatrixBase / PolynomialKernel / RBFKernel / TanhKernel, [RECALLED] removed
+ * with the distance package, CHANGELOG.md:59), the kernel evaluations of cuML's SVM.  For x:[m,k], y:[n,k]:
+ *   LINEAR      out[i,j] = <x_i, y_j>, bit-identical to b2d_pairwise_distance(InnerProduct)
+ *   POLYNOMIAL  (gamma <x_i, y_j> + coef0)^degree, integer degree >= 0 by repeated squaring (degree 0: 1 everywhere)
+ *   RBF         exp(-gamma ||x_i - y_j||^2), the squared distance of b2d_pairwise_distance(L2Expanded); when x and y are
+ *               the same matrix (same pointer, m == n, ldx == ldy) the diagonal is exactly 1
+ *   TANH        tanh(gamma <x_i, y_j> + coef0)
+ * The transform runs in the epilogue of the distance kernel, so the matrix is written once.  Layout, leading dimensions,
+ * dtypes and the workspace are those of b2d_pairwise_distance (row_major == 0: Fortran order, out [m,n] with ldo >= m);
+ * out is float for fp32 / fp16 inputs and double for fp64.  gamma and coef0 are used as float for fp32 / fp16 inputs and
+ * as double for fp64, and must be finite in that precision; degree is read for POLYNOMIAL only.  An unknown kernel, a
+ * non-finite gamma / coef0, a negative POLYNOMIAL degree, k == 0 are B2D_ERR_INVALID_ARG; m == 0 or n == 0 does nothing.
+ * No precomputed norms: the operand preparation computes them.  The workspace query returns SIZE_MAX for an unknown
+ * kernel or dtype and for negative extents. */
+size_t b2d_gram_matrix_workspace_bytes(int kernel, int dtype, int64_t m, int64_t n, int64_t k);
+int b2d_gram_matrix(void* stream, int kernel, int degree, double gamma, double coef0, int dtype, const void* x, int64_t ldx,
+                    const void* y, int64_t ldy, void* out /* float*, or double* for B2D_F64 */, int64_t ldo, int64_t m,
+                    int64_t n, int64_t k, int row_major, void* workspace, size_t workspace_bytes);
 
 #ifdef __cplusplus
 }

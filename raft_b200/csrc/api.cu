@@ -2,6 +2,7 @@
 #include <cuda.h>
 #include <cuda_runtime.h>
 #include <dlfcn.h>
+#include <cmath>
 #include <cstdio>
 #include <cstring>
 #include <cstdlib>
@@ -302,6 +303,9 @@ static int launch_tc_epi(cudaStream_t s, const CUtensorMap& ma, const CUtensorMa
   if (post == POST_CLAMP) return launch_tc_inst<kRes, EPI_STORE, POST_CLAMP>(s, ma, mb, md, p, grid);
   if (post == POST_JACCARD) return launch_tc_inst<kRes, EPI_STORE, POST_JACCARD>(s, ma, mb, md, p, grid);
   if (post == POST_DICE) return launch_tc_inst<kRes, EPI_STORE, POST_DICE>(s, ma, mb, md, p, grid);
+  if (post == POST_RBF) return launch_tc_inst<kRes, EPI_STORE, POST_RBF>(s, ma, mb, md, p, grid);
+  if (post == POST_POLY) return launch_tc_inst<kRes, EPI_STORE, POST_POLY>(s, ma, mb, md, p, grid);
+  if (post == POST_TANH) return launch_tc_inst<kRes, EPI_STORE, POST_TANH>(s, ma, mb, md, p, grid);
   return launch_tc_inst<kRes, EPI_STORE, POST_CLAMP_SQRT>(s, ma, mb, md, p, grid);
 }
 
@@ -527,7 +531,7 @@ static int launch_f64_inst(cudaStream_t s, const F64Params& p, int64_t tiles)
 
 static int pairwise_f64(cudaStream_t s, int metric, const double* x, int64_t xrs, int64_t xcs, const double* y, int64_t yrs,
                         int64_t ycs, double* dist, int64_t ldd, int64_t m, int64_t n, int64_t k, int swapped, double metric_arg,
-                        void* workspace, size_t workspace_bytes)
+                        void* workspace, size_t workspace_bytes, double gamma = 0.0, double coef0 = 0.0, int degree = 0)
 {
   const int rc = check_workspace(workspace, workspace_bytes, align_up(static_cast<size_t>(m + n) * 16, 1024), 1);
   if (rc) return rc;
@@ -540,6 +544,7 @@ static int pairwise_f64(cudaStream_t s, int metric, const double* x, int64_t xrs
   p.x = x; p.y = y; p.dist = dist; p.xrs = xrs; p.xcs = xcs; p.yrs = yrs; p.ycs = ycs; p.ldd = ldd; p.m = m; p.n = n;
   p.k = static_cast<int>(k); p.metric = metric; p.swapped = swapped; p.p = metric_arg; p.inv_p = 1.0 / metric_arg;
   p.xs = xs; p.ys = ys;
+  p.gamma = gamma; p.coef0 = coef0; p.degree = degree;
   p.tiles_n = static_cast<int>((n + F64_T - 1) / F64_T);
   const int64_t tiles = ((m + F64_T - 1) / F64_T) * p.tiles_n;
   switch (metric) {
@@ -550,6 +555,7 @@ static int pairwise_f64(cudaStream_t s, int metric, const double* x, int64_t xrs
     B2D_F64_CASE(B2D_JaccardExpanded) B2D_F64_CASE(B2D_HellingerExpanded) B2D_F64_CASE(B2D_BrayCurtis)
     B2D_F64_CASE(B2D_JensenShannon) B2D_F64_CASE(B2D_HammingUnexpanded) B2D_F64_CASE(B2D_KLDivergence)
     B2D_F64_CASE(B2D_RusselRaoExpanded) B2D_F64_CASE(B2D_DiceExpanded)
+    B2D_F64_CASE(F64_GRAM_POLY) B2D_F64_CASE(F64_GRAM_RBF) B2D_F64_CASE(F64_GRAM_TANH)
 #undef B2D_F64_CASE
     default: return fail(B2D_ERR_UNSUPPORTED, "metric");
   }
@@ -692,6 +698,63 @@ int b2d_debug_nn_stats(void* stream, const void* workspace, int64_t m, int64_t n
 }
 const char* b2d_last_error(void) { return g_err.c_str(); }
 
+// What one dense m x n result on the tensor path (EPI_STORE) is made of: the operand preparation (prep.cuh) and the
+// epilogue's post-processing, with the kernel parameters of the Gram matrices (gram_post).
+struct TcStore {
+  int mode = PREP_L2, center = 0, post = POST_NONE, xform = 0;
+  float coef_mul = 1.f, tx_const = 0.f;
+  float gamma = 0.f, coef0 = 0.f;
+  int degree = 0;
+};
+
+// The tensor path of b2d_pairwise_distance and b2d_gram_matrix: x [ma, k] and y [na, k] with element strides (xrs, xcs) and
+// (yrs, ycs) (a column-major call arrives with the operands exchanged), dist [ma][ldd].  alias: x and y are the same matrix
+// (then the L2 family has d(i, i) = 0 exactly).
+static int tc_store(cudaStream_t s, const TcStore& c, int dtype, const void* xa, int64_t xrs, int64_t xcs, int64_t ma,
+                    const void* ya, int64_t yrs, int64_t ycs, int64_t na, int64_t k, float* dist, int64_t ldd, bool alias,
+                    void* workspace, size_t workspace_bytes)
+{
+  int rc = check_workspace(workspace, workspace_bytes, tc_layout(nullptr, ma, na, k, false).bytes);
+  if (rc) return rc;
+  TcWorkspace w = tc_layout(workspace, ma, na, k, false);
+  rc = dtype == B2D_F32
+         ? launch_prep<float>(s, w, xa, xrs, xcs, ma, ya, yrs, ycs, na, k, nullptr, nullptr, c.mode, c.center, c.xform,
+                              c.coef_mul, c.tx_const)
+         : launch_prep<__half>(s, w, xa, xrs, xcs, ma, ya, yrs, ycs, na, k, nullptr, nullptr, c.mode, c.center, c.xform,
+                               c.coef_mul, c.tx_const);
+  if (rc) return rc;
+  TcParams p;
+  memset(&p, 0, sizeof(p));
+  p.m = ma; p.n = na; p.dist = dist; p.ldd = ldd;
+  p.diag_zero = (c.post != POST_NONE && alias && c.mode == PREP_L2) ? 1 : 0;
+  p.gamma = c.gamma; p.coef0 = c.coef0; p.degree = c.degree;
+  // the result leaves through shared-memory staging and TMA stores wherever TMA can address dist: 16-byte aligned
+  // base and pitch, row and column coordinates within int32 (the store takes 32-bit coordinates), and rows that end
+  // on a 16-byte boundary.  The last condition is from observation: on an H100, with n = 150 and ldd = 160, the
+  // box stores also wrote columns 150 and 151, i.e. the partial 16 bytes at the end of each row, into the caller's
+  // padding (tests/test_pairwise_gpu.py::test_padded_leading_dimensions_and_out_param).  Otherwise, and for the
+  // read-modify-write K chunks below, the epilogue stores from registers.
+  p.tma_store = (reinterpret_cast<uintptr_t>(dist) % 16 == 0 && ldd % 4 == 0 && na % 4 == 0 && ma <= 0x7fffffffll &&
+                 na <= 0x7fffffffll) ? 1 : 0;
+  // k > 320: accumulate K in chunks of 256 columns, each added to dist with a round-to-nearest fp32
+  // add -- bounds the truncation bias of long MMA chains (DESIGN.md, numerics).  The post-processing (clamp, sqrt, the
+  // Gram transforms) runs on the last chunk only.
+  const int nkb_total = static_cast<int>((k + 31) / 32);
+  constexpr int kChunk = 8;
+  ProfileScope prof(s);  // the main kernel(s) only: the operand preparation above is outside
+  if (nkb_total > 10 && !tc_post_ratio(c.post)) {  // (the ratio metrics need the whole inner product at once)
+    p.tma_store = 0;
+    for (int kb0 = 0; kb0 < nkb_total; kb0 += kChunk) {
+      const int nk = nkb_total - kb0 < kChunk ? nkb_total - kb0 : kChunk;
+      p.acc_mode   = kb0 == 0 ? 1 : (kb0 + nk >= nkb_total ? 3 : 2);
+      rc           = launch_tc(s, w, p, k, EPI_STORE, c.post, kb0, nk);
+      if (rc) return rc;
+    }
+    return B2D_OK;
+  }
+  return launch_tc(s, w, p, k, EPI_STORE, c.post);
+}
+
 size_t b2d_pairwise_workspace_bytes(int metric, int dtype, int64_t m, int64_t n, int64_t k)
 {
   if (dtype != B2D_F32 && dtype != B2D_F16 && dtype != B2D_F64) return static_cast<size_t>(-1);
@@ -740,54 +803,18 @@ int b2d_pairwise_distance(void* stream, int metric, int dtype, const void* x, in
   else { xa = y; ya = x; ma = n; na = m; xrs = 1; xcs = ldy; yrs = 1; ycs = ldx; }
 
   if (is_expanded(metric)) {
-    int rc = check_workspace(workspace, workspace_bytes, tc_layout(nullptr, ma, na, k, false).bytes);
-    if (rc) return rc;
-    TcWorkspace w = tc_layout(workspace, ma, na, k, false);
-    int mode = PREP_L2, center = 0, post = POST_NONE, xform = 0;
-    float coef_mul = 1.f, tx_const = 0.f;
-    if (metric == B2D_L2Expanded) { post = POST_CLAMP; }
-    else if (metric == B2D_L2SqrtExpanded) { post = POST_CLAMP_SQRT; }
-    else if (metric == B2D_CosineExpanded) { mode = PREP_COSINE; }
-    else if (metric == B2D_CorrelationExpanded) { mode = PREP_COSINE; center = 1; }
-    else if (metric == B2D_HellingerExpanded) { mode = PREP_INNER; post = POST_CLAMP_SQRT; xform = 1; coef_mul = -1.f; tx_const = 1.f; }
-    else if (metric == B2D_RusselRaoExpanded) { mode = PREP_INNER; coef_mul = -1.f / static_cast<float>(k); tx_const = 1.f; }
-    else if (metric == B2D_JaccardExpanded) { mode = PREP_INNER_NORM; post = POST_JACCARD; }
-    else if (metric == B2D_DiceExpanded) { mode = PREP_INNER_NORM; post = POST_DICE; }
-    else { mode = PREP_INNER; }
-    rc = dtype == B2D_F32
-           ? launch_prep<float>(s, w, xa, xrs, xcs, ma, ya, yrs, ycs, na, k, nullptr, nullptr, mode, center, xform,
-                                coef_mul, tx_const)
-           : launch_prep<__half>(s, w, xa, xrs, xcs, ma, ya, yrs, ycs, na, k, nullptr, nullptr, mode, center, xform,
-                                 coef_mul, tx_const);
-    if (rc) return rc;
-    TcParams p;
-    memset(&p, 0, sizeof(p));
-    p.m = ma; p.n = na; p.dist = dist; p.ldd = ldd;
-    p.diag_zero = (post != POST_NONE && x == y && m == n && ldx == ldy && mode == PREP_L2) ? 1 : 0;
-    // the result leaves through shared-memory staging and TMA stores wherever TMA can address dist: 16-byte aligned
-    // base and pitch, row and column coordinates within int32 (the store takes 32-bit coordinates), and rows that end
-    // on a 16-byte boundary.  The last condition is from observation: on an H100, with n = 150 and ldd = 160, the
-    // box stores also wrote columns 150 and 151, i.e. the partial 16 bytes at the end of each row, into the caller's
-    // padding (tests/test_pairwise_gpu.py::test_padded_leading_dimensions_and_out_param).  Otherwise, and for the
-    // read-modify-write K chunks below, the epilogue stores from registers.
-    p.tma_store = (reinterpret_cast<uintptr_t>(dist) % 16 == 0 && ldd % 4 == 0 && na % 4 == 0 && ma <= 0x7fffffffll &&
-                   na <= 0x7fffffffll) ? 1 : 0;
-    // k > 320: accumulate K in chunks of 256 columns, each added to dist with a round-to-nearest fp32
-    // add -- bounds the truncation bias of long MMA chains (DESIGN.md, numerics)
-    const int nkb_total = static_cast<int>((k + 31) / 32);
-    constexpr int kChunk = 8;
-    ProfileScope prof(s);  // the main kernel(s) only: the operand preparation above is outside
-    if (nkb_total > 10 && post < POST_JACCARD) {  // (the ratio metrics need the whole inner product at once)
-      p.tma_store = 0;
-      for (int kb0 = 0; kb0 < nkb_total; kb0 += kChunk) {
-        const int nk = nkb_total - kb0 < kChunk ? nkb_total - kb0 : kChunk;
-        p.acc_mode   = kb0 == 0 ? 1 : (kb0 + nk >= nkb_total ? 3 : 2);
-        rc           = launch_tc(s, w, p, k, EPI_STORE, post, kb0, nk);
-        if (rc) return rc;
-      }
-      return B2D_OK;
-    }
-    return launch_tc(s, w, p, k, EPI_STORE, post);
+    TcStore c;
+    if (metric == B2D_L2Expanded) { c.post = POST_CLAMP; }
+    else if (metric == B2D_L2SqrtExpanded) { c.post = POST_CLAMP_SQRT; }
+    else if (metric == B2D_CosineExpanded) { c.mode = PREP_COSINE; }
+    else if (metric == B2D_CorrelationExpanded) { c.mode = PREP_COSINE; c.center = 1; }
+    else if (metric == B2D_HellingerExpanded) { c.mode = PREP_INNER; c.post = POST_CLAMP_SQRT; c.xform = 1; c.coef_mul = -1.f; c.tx_const = 1.f; }
+    else if (metric == B2D_RusselRaoExpanded) { c.mode = PREP_INNER; c.coef_mul = -1.f / static_cast<float>(k); c.tx_const = 1.f; }
+    else if (metric == B2D_JaccardExpanded) { c.mode = PREP_INNER_NORM; c.post = POST_JACCARD; }
+    else if (metric == B2D_DiceExpanded) { c.mode = PREP_INNER_NORM; c.post = POST_DICE; }
+    else { c.mode = PREP_INNER; }
+    return tc_store(s, c, dtype, xa, xrs, xcs, ma, ya, yrs, ycs, na, k, dist, ldd, x == y && m == n && ldx == ldy,
+                    workspace, workspace_bytes);
   }
 
   if (dtype != B2D_F32) return fail(B2D_ERR_UNSUPPORTED, "unexpanded metrics take fp32 inputs");
@@ -1670,6 +1697,67 @@ int b2d_eps_neighbors_l2sq(void* stream, uint8_t* adj, int64_t ld_adj, void* vd,
   p.tma_store = (adj && reinterpret_cast<uintptr_t>(adj) % 16 == 0 && ld_adj % 16 == 0 && n % 16 == 0) ? 1 : 0;
   ProfileScope prof(s);
   return launch_tc(s, w, p, k, EPI_EPS, POST_CLAMP);
+}
+
+// ------------------------------------------------------------------------------------------
+// Kernel Gram matrices (raft::distance::kernels): pairwise_distance's InnerProduct (LINEAR, POLYNOMIAL, TANH) or
+// L2Expanded (RBF) value, transformed in the epilogue of the same kernel (expanded_tc.cuh gram_post; fp64: f64_gram).
+
+// the pairwise metric whose value a kernel transforms
+static int gram_base_metric(int kernel) { return kernel == B2D_KERNEL_RBF ? B2D_L2Expanded : B2D_InnerProduct; }
+static bool gram_kernel_known(int kernel) { return kernel >= B2D_KERNEL_LINEAR && kernel <= B2D_KERNEL_TANH; }
+
+size_t b2d_gram_matrix_workspace_bytes(int kernel, int dtype, int64_t m, int64_t n, int64_t k)
+{
+  if (!gram_kernel_known(kernel)) return static_cast<size_t>(-1);
+  return b2d_pairwise_workspace_bytes(gram_base_metric(kernel), dtype, m, n, k);
+}
+
+int b2d_gram_matrix(void* stream, int kernel, int degree, double gamma, double coef0, int dtype, const void* x, int64_t ldx,
+                    const void* y, int64_t ldy, void* out, int64_t ldo, int64_t m, int64_t n, int64_t k, int row_major,
+                    void* workspace, size_t workspace_bytes)
+{
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  if (!gram_kernel_known(kernel)) return fail(B2D_ERR_INVALID_ARG, "unknown kernel " + std::to_string(kernel));
+  if (dtype != B2D_F32 && dtype != B2D_F16 && dtype != B2D_F64) return fail(B2D_ERR_UNSUPPORTED, "dtype");
+  // gamma and coef0 in the precision they are used in: double for fp64 inputs, float otherwise
+  const bool finite = dtype == B2D_F64 ? std::isfinite(gamma) && std::isfinite(coef0)
+                                       : std::isfinite(static_cast<float>(gamma)) && std::isfinite(static_cast<float>(coef0));
+  if (!finite) return fail(B2D_ERR_INVALID_ARG, "gamma and coef0 must be finite");
+  if (kernel == B2D_KERNEL_POLYNOMIAL && degree < 0) return fail(B2D_ERR_INVALID_ARG, "degree must be >= 0");
+  if (m < 0 || n < 0 || k < 0) return fail(B2D_ERR_INVALID_ARG, "negative extent");
+  if (m == 0 || n == 0) return B2D_OK;
+  if (k == 0) return fail(B2D_ERR_INVALID_ARG, "k must be positive");
+  if (!x || !y || !out) return fail(B2D_ERR_INVALID_ARG, "null x / y / out");
+  if (m > 0x7fffffffll * 128 || n > 0x7fffffffll || k > (1 << 24)) return fail(B2D_ERR_INVALID_ARG, "extent too large");
+  if (row_major) {
+    if (ldx < k || ldy < k || ldo < n) return fail(B2D_ERR_INVALID_ARG, "leading dimension smaller than the row length");
+  } else {
+    if (ldx < m || ldy < n || ldo < m) return fail(B2D_ERR_INVALID_ARG, "leading dimension smaller than the column length");
+  }
+  if (kernel != B2D_KERNEL_POLYNOMIAL) degree = 0;
+  if (dtype == B2D_F64) {
+    const int metric = kernel == B2D_KERNEL_LINEAR ? B2D_InnerProduct
+                     : kernel == B2D_KERNEL_POLYNOMIAL ? F64_GRAM_POLY
+                     : kernel == B2D_KERNEL_RBF ? F64_GRAM_RBF : F64_GRAM_TANH;
+    if (row_major)
+      return pairwise_f64(s, metric, static_cast<const double*>(x), ldx, 1, static_cast<const double*>(y), ldy, 1,
+                          static_cast<double*>(out), ldo, m, n, k, 0, 2.0, workspace, workspace_bytes, gamma, coef0, degree);
+    return pairwise_f64(s, metric, static_cast<const double*>(y), 1, ldy, static_cast<const double*>(x), 1, ldx,
+                        static_cast<double*>(out), ldo, n, m, k, 1, 2.0, workspace, workspace_bytes, gamma, coef0, degree);
+  }
+  // Fortran order: the row-major [n, m] matrix of K(y_j, x_i), the same values (every kernel is symmetric)
+  TcStore c;
+  c.mode   = kernel == B2D_KERNEL_RBF ? PREP_L2 : PREP_INNER;
+  c.post   = kernel == B2D_KERNEL_LINEAR ? POST_NONE
+           : kernel == B2D_KERNEL_POLYNOMIAL ? POST_POLY
+           : kernel == B2D_KERNEL_RBF ? POST_RBF : POST_TANH;
+  c.gamma  = static_cast<float>(gamma);
+  c.coef0  = static_cast<float>(coef0);
+  c.degree = degree;
+  const bool alias = x == y && m == n && ldx == ldy;
+  if (row_major) return tc_store(s, c, dtype, x, ldx, 1, m, y, ldy, 1, n, k, static_cast<float*>(out), ldo, alias, workspace, workspace_bytes);
+  return tc_store(s, c, dtype, y, 1, ldy, n, x, 1, ldx, m, k, static_cast<float*>(out), ldo, alias, workspace, workspace_bytes);
 }
 
 }  // extern "C"

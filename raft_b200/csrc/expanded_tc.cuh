@@ -37,8 +37,10 @@
 //                     drain while the warpgroup runs the next half's MMAs (tc_stage_store).  Where TMA cannot
 //                     address dist (unaligned base or pitch) and in the read-modify-write path of K-chunked
 //                     accumulation (k > 320), each thread stores its 2 adjacent columns of 2 rows per
-//                     8-column group straight from the registers (8-byte streaming stores).
-//   EPI_MINLOC        per row the minimum of the thread's 16 values of a 64-column chunk is compared with
+//                     8-column group straight from the registers (8-byte streaming stores).  The kernel Gram
+//                     matrices (POST_RBF / POST_POLY / POST_TANH) transform the final value in registers first
+//                     (gram_post), so the transformed matrix is the only one written.
+//   EPI_MINLOC       per row the minimum of the thread's 16 values of a 64-column chunk is compared with
 //                     the row's current global best (read from keys at tile start: an upper bound, keys
 //                     only decrease); only a candidate that can change the result takes the slow path
 //                     (smallest-column scan + packed 64-bit atomicMin).
@@ -100,7 +102,37 @@ __device__ __forceinline__ float clamp0(float v)
 
 enum TcPost : int { POST_NONE = 0, POST_CLAMP = 1, POST_CLAMP_SQRT = 2,
                     POST_JACCARD = 3,  // d = 1 - a / (s - a), a = <x,y>, s = |x|^2 + |y|^2 (0/0 -> 0)
-                    POST_DICE    = 4 };  // d = 1 - 2 a / s
+                    POST_DICE    = 4,  // d = 1 - 2 a / s
+                    // kernel Gram matrices (gram_post; TcParams::gamma / coef0 / degree):
+                    POST_RBF     = 5,  // exp(-gamma d), d the POST_CLAMP distance
+                    POST_POLY    = 6,  // (gamma <x,y> + coef0)^degree
+                    POST_TANH    = 7 };  // tanh(gamma <x,y> + coef0)
+
+// the ratio metrics: computed from the inner product and the squared norms at once (never K-chunked)
+__host__ __device__ constexpr bool tc_post_ratio(int post) { return post == POST_JACCARD || post == POST_DICE; }
+// the squared L2 distance, clamped at 0 (with d(i, i) = 0 when x and y alias) before anything else is done with it
+__host__ __device__ constexpr bool tc_post_clamps(int post)
+{
+  return post == POST_CLAMP || post == POST_CLAMP_SQRT || post == POST_RBF;
+}
+__host__ __device__ constexpr bool tc_post_gram(int post) { return post == POST_RBF || post == POST_POLY || post == POST_TANH; }
+
+// Gram-matrix transform of one finished value u (RBF: the clamped squared distance; POLY / TANH: the inner product), in
+// full-precision fp32: one rounding for gamma u (+ coef0), then expf / tanhf, or the power by binary exponentiation
+// (degree 0 gives 1 for every u, NaN included)
+template <int kPost>
+__device__ __forceinline__ float gram_post(float u, float gamma, float coef0, int degree)
+{
+  if constexpr (kPost == POST_RBF) return expf(-(gamma * u));
+  const float t = fmaf(gamma, u, coef0);
+  if constexpr (kPost == POST_TANH) return tanhf(t);
+  float r = 1.f, b = t;
+  for (unsigned e = static_cast<unsigned>(degree); e != 0u; e >>= 1) {
+    if (e & 1u) r *= b;
+    if (e > 1u) b *= b;
+  }
+  return r;
+}
 
 // ratio metrics on the tensor path: a = acc * c (the inner product), s = t_x + t_y (the squared norms)
 template <int kPost>
@@ -158,6 +190,10 @@ struct TcParams {
   int vd64;
   float eps;              // the squared radius
   int64_t diag_off;       // row j of y is row j + diag_off of x (same memory): d = 0 there; TC_NO_DIAG: no such rows
+  // EPI_STORE with POST_RBF / POST_POLY / POST_TANH (gram_post): the kernel parameters, applied to the final value only
+  float gamma;
+  float coef0;
+  int degree;
 };
 
 constexpr size_t TC_SMEM_OPERANDS = (size_t)TC_MAX_RES_KB * TC_B_BYTES + (size_t)TC_STAGES_RES * TC_A_BYTES;  // 208 KB
@@ -364,7 +400,7 @@ __device__ __forceinline__ void tc_epilogue(float (&v)[64], const TcParams& p, c
     for (int j = 0; j < 2; ++j) {
       float a0 = v[4 * i + 2 * j], a1 = v[4 * i + 2 * j + 1];
       if (ynu) { a0 *= sb0; a1 *= sb1; }
-      if (kEpi == EPI_STORE && kPost >= POST_JACCARD) {
+      if (kEpi == EPI_STORE && tc_post_ratio(kPost)) {
         v[4 * i + 2 * j]     = post_ratio<kPost>(a0 * cfr[j], ta[j] + tb.x);
         v[4 * i + 2 * j + 1] = post_ratio<kPost>(a1 * cfr[j], ta[j] + tb.y);
       } else if (kEpi == EPI_STORE || kEpi == EPI_EPS) {
@@ -416,7 +452,7 @@ __device__ __forceinline__ void tc_epilogue(float (&v)[64], const TcParams& p, c
         }
       }
     }
-    if (kPost != POST_NONE && kPost < POST_JACCARD && (p.acc_mode == 0 || p.acc_mode == 3)) {
+    if (tc_post_clamps(kPost) && (p.acc_mode == 0 || p.acc_mode == 3)) {
 #pragma unroll
       for (int c = 0; c < 64; ++c) v[c] = clamp0(v[c]);
       if (p.diag_zero) {
@@ -431,6 +467,12 @@ __device__ __forceinline__ void tc_epilogue(float (&v)[64], const TcParams& p, c
       if (kPost == POST_CLAMP_SQRT) {
 #pragma unroll
         for (int c = 0; c < 64; ++c) asm("sqrt.approx.f32 %0, %1;" : "=f"(v[c]) : "f"(v[c]));
+      }
+    }
+    if constexpr (tc_post_gram(kPost)) {
+      if (p.acc_mode == 0 || p.acc_mode == 3) {   // (K-chunked: the earlier chunks store the partial sum untransformed)
+#pragma unroll
+        for (int c = 0; c < 64; ++c) v[c] = gram_post<kPost>(v[c], p.gamma, p.coef0, p.degree);
       }
     }
     if (p.tma_store) return;

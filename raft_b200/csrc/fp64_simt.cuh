@@ -25,7 +25,13 @@ struct F64Params {
   const double* xs; // [m][2] (sum, sum of squares) of the rows of x (after the sqrt transform for Hellinger)
   const double* ys; // [n][2]
   int tiles_n;
+  double gamma, coef0;  // kernel Gram matrices (F64_GRAM_*)
+  int degree;
 };
+
+// Internal metric ids of the kernel Gram matrices (b2d_gram_matrix; no public DistanceType): the value of f64_acc /
+// f64_fin for the base metric, then f64_gram.  The linear kernel is B2D_InnerProduct itself.
+enum { F64_GRAM_POLY = 1001, F64_GRAM_RBF = 1002, F64_GRAM_TANH = 1003 };
 
 __global__ void f64_row_stats_kernel(double* out, const double* x, int64_t rs, int64_t cs, int64_t rows, int k)
 {
@@ -50,7 +56,7 @@ __global__ void f64_row_stats_kernel(double* out, const double* x, int64_t rs, i
 __device__ __forceinline__ void f64_acc(int metric, int swapped, double p, double a, double b, double& acc, double& aux)
 {
   switch (metric) {
-    case B2D_L2Expanded: case B2D_L2SqrtExpanded: case B2D_L2Unexpanded: case B2D_L2SqrtUnexpanded: {
+    case B2D_L2Expanded: case B2D_L2SqrtExpanded: case B2D_L2Unexpanded: case B2D_L2SqrtUnexpanded: case F64_GRAM_RBF: {
       const double d = a - b; acc = fma(d, d, acc); break; }
     case B2D_L1: acc += fabs(a - b); break;
     case B2D_Linf: acc = fmax(acc, fabs(a - b)); break;
@@ -91,7 +97,27 @@ __device__ __forceinline__ double f64_fin(int metric, double acc, double aux, do
       return 1.0 - num / den; }
     case B2D_JaccardExpanded: { const double den = xs1 + ys1 - acc; return den > 0.0 ? fmax(1.0 - acc / den, 0.0) : 0.0; }
     case B2D_DiceExpanded: { const double den = xs1 + ys1; return den > 0.0 ? fmax(1.0 - 2.0 * acc / den, 0.0) : 0.0; }
-    default: return acc;  // L1, Linf, Canberra, L2 (squared), InnerProduct
+    default: return acc;  // L1, Linf, Canberra, L2 (squared), InnerProduct, the Gram matrices' base values
+  }
+}
+
+// the kernel Gram matrices' transform of the base value u (RBF: the squared distance, difference form; POLY / TANH: the
+// inner product); every other metric passes through
+__device__ __forceinline__ double f64_gram(int metric, double u, const F64Params& p)
+{
+  switch (metric) {
+    case F64_GRAM_RBF: return exp(-(p.gamma * u));
+    case F64_GRAM_TANH: return tanh(fma(p.gamma, u, p.coef0));
+    case F64_GRAM_POLY: {   // binary exponentiation, as on the tensor path (degree 0: 1)
+      const double t = fma(p.gamma, u, p.coef0);
+      double r = 1.0, b = t;
+      for (unsigned e = static_cast<unsigned>(p.degree); e != 0u; e >>= 1) {
+        if (e & 1u) r *= b;
+        if (e > 1u) b *= b;
+      }
+      return r;
+    }
+    default: return u;
   }
 }
 
@@ -139,7 +165,7 @@ __global__ void __launch_bounds__(256) f64_pairwise_kernel(const F64Params p)
       if (gj >= p.n) continue;
       const double xs0 = p.xs ? p.xs[2 * gi] : 0.0, xs1 = p.xs ? p.xs[2 * gi + 1] : 0.0;
       const double ys0 = p.ys ? p.ys[2 * gj] : 0.0, ys1 = p.ys ? p.ys[2 * gj + 1] : 0.0;
-      p.dist[gi * p.ldd + gj] = f64_fin(kMetric, acc[i][j], aux[i][j], p.inv_p, p.k, xs0, xs1, ys0, ys1);
+      p.dist[gi * p.ldd + gj] = f64_gram(kMetric, f64_fin(kMetric, acc[i][j], aux[i][j], p.inv_p, p.k, xs0, xs1, ys0, ys1), p);
     }
   }
 }

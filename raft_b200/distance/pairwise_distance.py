@@ -46,6 +46,25 @@ def pairwise_distance(X, Y, out=None, metric="euclidean", p=2.0, handle=None):
     place and returned); ``metric`` a string from ``DISTANCE_TYPES`` or a ``DistanceType``;
     ``p`` the Minkowski exponent; ``handle`` a ``DeviceResources`` (None: one is created and
     synchronised before returning)."""
+    x_cai, y_cai, d_cai, dists, row_major, ldx, ldy, ldd = _operands(X, Y, out)
+    mt = resolve_metric(metric)
+    m, k = x_cai.shape
+    n = y_cai.shape[0]
+
+    L = _lib.lib()
+    dt = _DT[x_cai.dtype]
+    need = L.b2d_pairwise_workspace_bytes(int(mt), dt, m, n, k)
+    if need == 2 ** 64 - 1:
+        raise ValueError("metric %s is not supported for dtype %s" % (metric, x_cai.dtype))
+    ws = handle.workspace(need)
+    pairwise_distance_raw(handle.stream_ptr, mt, x_cai.data, ldx, y_cai.data, ldy, d_cai.data, ldd,
+                          m, n, k, row_major, p, ws.data_ptr(), ws.numel(), dtype=dt)
+    return dists
+
+
+def _operands(X, Y, out):
+    """The checked operands of an [m,n] result of X [m,k] and Y [n,k] (pairwise_distance, gram_matrix):
+    (x, y, out wrappers, the out array, row_major, ldx, ldy, ldo).  ``out`` None: a new array in the inputs' order."""
     x_cai, y_cai = cai_wrapper(X), cai_wrapper(Y)
     x_cai.validate_shape_dtype(expected_dims=2)
     y_cai.validate_shape_dtype(expected_dims=2)
@@ -57,7 +76,6 @@ def pairwise_distance(X, Y, out=None, metric="euclidean", p=2.0, handle=None):
         raise TypeError("Inputs must have the same dtypes")
     if x_cai.dtype not in _DT:
         raise TypeError("dtype %s not supported" % x_cai.dtype)
-    mt = resolve_metric(metric)
 
     x_rm, ldx = _layout(x_cai)
     y_rm, ldy = _layout(y_cai)
@@ -89,16 +107,7 @@ def pairwise_distance(X, Y, out=None, metric="euclidean", p=2.0, handle=None):
     if m > 1 and n > 1 and d_rm != row_major:
         raise ValueError("out must have the same memory order as the inputs")
     ldd = max(ldd, n if row_major else m)
-
-    L = _lib.lib()
-    dt = _DT[x_cai.dtype]
-    need = L.b2d_pairwise_workspace_bytes(int(mt), dt, m, n, k)
-    if need == 2 ** 64 - 1:
-        raise ValueError("metric %s is not supported for dtype %s" % (metric, x_cai.dtype))
-    ws = handle.workspace(need)
-    pairwise_distance_raw(handle.stream_ptr, mt, x_cai.data, ldx, y_cai.data, ldy, d_cai.data, ldd,
-                          m, n, k, row_major, p, ws.data_ptr(), ws.numel(), dtype=dt)
-    return dists
+    return x_cai, y_cai, d_cai, dists, row_major, ldx, ldy, ldd
 
 
 # alias kept by the reference for backwards compatibility
