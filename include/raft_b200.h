@@ -292,6 +292,45 @@ int b2d_gram_matrix(void* stream, int kernel, int degree, double gamma, double c
                     const void* y, int64_t ldy, void* out /* float*, or double* for B2D_F64 */, int64_t ldo, int64_t m,
                     int64_t n, int64_t k, int row_major, void* workspace, size_t workspace_bytes);
 
+/* raft::cluster::kmeans InitMethod ([RECALLED] raft/cluster/kmeans_types.hpp, <= 25.12) */
+enum { B2D_KMEANS_INIT_PLUS_PLUS = 0, B2D_KMEANS_INIT_RANDOM = 1, B2D_KMEANS_INIT_ARRAY = 2 };
+
+/* raft::cluster::kmeans ([RECALLED] removed with distance/, CHANGELOG.md:59): Lloyd's k-means under L2Expanded for fp32
+ * x:[m,k] (row-major, pitch ldx), centroids:[n_clusters,k] contiguous.
+ *   Assignment: label_i = argmin_j ||x_i - c_j||^2 by the exact arg-min of b2d_fused_l2_nn (the distance bits of its
+ *     unscreened kernel; ties to the smaller j).  A row with a NaN distance gets no label (-1) and makes the inertia NaN.
+ *   Update: c_j = sum_{label_i = j} w_i x_i / sum_{label_i = j} w_i, accumulated in fp64 in a fixed order and rounded once
+ *     to fp32; a cluster of zero weight keeps its previous centroid bit for bit; labels outside [0, n_clusters) are
+ *     skipped.  Results are bit-identical from run to run (no floating-point atomics).
+ *   fit: iteration t assigns with C_t and computes C_{t+1}; it stops when sum ||C_{t+1} - C_t||^2 < tol (fp64) or, with
+ *     inertia_check, after the first iteration when inertia_t / inertia_{t-1} > 1 - tol; at most max_iter iterations,
+ *     *n_iter = the iterations that ran.  *inertia = sum_i w_i ||x_i - c_{label_i}||^2 for the returned centroids, in fp64 in the difference
+ *     form (0 for a row equal to its centroid; inertia_check uses the arg-min's fp32 distances).  init:
+ *     ARRAY uses centroids as given (n_init ignored); RANDOM takes n_clusters distinct rows; PLUS_PLUS is greedy
+ *     k-means++ with 2 + floor(ln n_clusters) trials per round.  n_init > 1 runs seeds seed + r and keeps the first run of
+ *     strictly lowest inertia.  The loop runs on the device: max_iter iterations are enqueued and the ones after
+ *     convergence return at once.
+ *   Weights (optional, NULL = 1): fit and predict (normalize_weight != 0) scale them to sum to m; update_centroids uses
+ *     them as given.  A negative weight or a zero sum makes the inertia NaN.
+ *   predict: labels (int32, optional) and *inertia (optional) for the given centroids.  update_centroids: new_centroids
+ *     from given labels, weight_per_cluster[j] = the fp64 weight sum rounded to fp32 (optional).  init_plus_plus: the
+ *     k-means++ seeding alone, weights as given.
+ * 1 <= n_clusters <= m < 2^31 and 1 <= k <= 2^24 (the accuracy caveat of b2d_fused_l2_nn above k = 320 applies), else
+ * B2D_ERR_INVALID_ARG; m == 0 does nothing.  inertia and n_iter are device pointers.  No call synchronises or allocates,
+ * so every call can be captured in a CUDA graph.  The workspace query returns SIZE_MAX for negative extents. */
+size_t b2d_kmeans_workspace_bytes(int64_t m, int64_t k, int64_t n_clusters);
+int b2d_kmeans_fit(void* stream, int n_clusters, int max_iter, double tol, int init, int n_init, uint64_t seed,
+                   int inertia_check, const float* x, int64_t ldx, const float* sample_weight, int64_t m, int64_t k,
+                   float* centroids, double* inertia, int32_t* n_iter, void* workspace, size_t workspace_bytes);
+int b2d_kmeans_predict(void* stream, const float* x, int64_t ldx, const float* sample_weight, int64_t m, int64_t k,
+                       const float* centroids, int n_clusters, int32_t* labels, double* inertia, int normalize_weight,
+                       void* workspace, size_t workspace_bytes);
+int b2d_kmeans_update_centroids(void* stream, const float* x, int64_t ldx, const float* sample_weight, const int32_t* labels,
+                                int64_t m, int64_t k, const float* old_centroids, int n_clusters, float* new_centroids,
+                                float* weight_per_cluster, void* workspace, size_t workspace_bytes);
+int b2d_kmeans_init_plus_plus(void* stream, const float* x, int64_t ldx, const float* sample_weight, int64_t m, int64_t k,
+                              int n_clusters, uint64_t seed, float* centroids, void* workspace, size_t workspace_bytes);
+
 #ifdef __cplusplus
 }
 #endif

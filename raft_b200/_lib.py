@@ -17,12 +17,14 @@ SYMBOLS = [
     "b2d_trustworthiness_score_workspace_bytes", "b2d_trustworthiness_score", "b2d_profile_begin", "b2d_profile_end",
     "b2d_row_argmin", "b2d_fused_l2_nn_multi", "b2d_masked_l2_nn_workspace_bytes", "b2d_masked_l2_nn",
     "b2d_select_k_workspace_bytes", "b2d_select_k", "b2d_eps_neighbors_l2sq_workspace_bytes", "b2d_eps_neighbors_l2sq",
-    "b2d_gram_matrix_workspace_bytes", "b2d_gram_matrix",
+    "b2d_gram_matrix_workspace_bytes", "b2d_gram_matrix", "b2d_kmeans_workspace_bytes", "b2d_kmeans_fit",
+    "b2d_kmeans_predict", "b2d_kmeans_update_centroids", "b2d_kmeans_init_plus_plus",
 ]
 
 B2D_OK, B2D_ERR_INVALID_ARG, B2D_ERR_CUDA, B2D_ERR_UNSUPPORTED, B2D_ERR_WORKSPACE = range(5)
 B2D_F32, B2D_F16, B2D_F64 = 0, 1, 2
 B2D_KERNEL_LINEAR, B2D_KERNEL_POLYNOMIAL, B2D_KERNEL_RBF, B2D_KERNEL_TANH = range(4)
+B2D_KMEANS_INIT_PLUS_PLUS, B2D_KMEANS_INIT_RANDOM, B2D_KMEANS_INIT_ARRAY = range(3)
 
 
 class RaftB200Error(RuntimeError):
@@ -105,6 +107,17 @@ def lib() -> ctypes.CDLL:
     L.b2d_gram_matrix.restype = ci
     L.b2d_gram_matrix.argtypes = [vp, ci, ci, ctypes.c_double, ctypes.c_double, ci, vp, i64, vp, i64, vp, i64, i64, i64, i64,
                                   ci, vp, sz]
+    u64, cd = ctypes.c_uint64, ctypes.c_double
+    L.b2d_kmeans_workspace_bytes.restype = sz
+    L.b2d_kmeans_workspace_bytes.argtypes = [i64, i64, i64]
+    L.b2d_kmeans_fit.restype = ci
+    L.b2d_kmeans_fit.argtypes = [vp, ci, ci, cd, ci, ci, u64, ci, vp, i64, vp, i64, i64, vp, vp, vp, vp, sz]
+    L.b2d_kmeans_predict.restype = ci
+    L.b2d_kmeans_predict.argtypes = [vp, vp, i64, vp, i64, i64, vp, ci, vp, vp, ci, vp, sz]
+    L.b2d_kmeans_update_centroids.restype = ci
+    L.b2d_kmeans_update_centroids.argtypes = [vp, vp, i64, vp, vp, i64, i64, vp, ci, vp, vp, vp, sz]
+    L.b2d_kmeans_init_plus_plus.restype = ci
+    L.b2d_kmeans_init_plus_plus.argtypes = [vp, vp, i64, vp, i64, i64, ci, u64, vp, vp, sz]
     L.b2d_row_norm.restype = ci
     L.b2d_row_norm.argtypes = [vp, vp, vp, i64, i64, i64, ci, ci]
     _lib = L

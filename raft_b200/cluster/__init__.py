@@ -1,0 +1,3 @@
+from .kmeans import (  # noqa: F401
+    FitOutput, KMeansParams, cluster_cost, compute_new_centroids, fit, init_plus_plus, predict,
+)

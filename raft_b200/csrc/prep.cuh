@@ -57,6 +57,11 @@ struct PrepParams {
   float* coef;       // [1] the epilogue scalar c
   unsigned* has_lo;  // [1] set to 1 when any lo half is non-zero (zeroed before the kernels run)
   unsigned* nonuni;  // [2] set to 1 when some row of x / y took its own exponent (zeroed before the kernels run)
+  // Re-preparing y alone (the centroids of every k-means iteration): first_side = 1 skips the rows of x, whose packed
+  // rows, terms and exponent gmax[0] stay as an earlier launch left them; gmax[1] and nonuni[1] must be zeroed first.
+  // coef is written by the first prepared row either way.
+  int first_side;
+  const unsigned* run_flag;  // non-null: the launch is a no-op unless *run_flag != 0
 };
 
 template <typename T>
@@ -114,8 +119,9 @@ __device__ __forceinline__ void row_stats(const T* row, int64_t cs, int k, int c
 template <typename T>
 __global__ void __launch_bounds__(256) prep_max_kernel(PrepParams p)
 {
+  if (p.run_flag != nullptr && __ldg(p.run_flag) == 0u) return;
   const int lane  = threadIdx.x & 31;
-  int64_t r       = static_cast<int64_t>(blockIdx.x) * 8 + (threadIdx.x >> 5);
+  int64_t r       = static_cast<int64_t>(blockIdx.x) * 8 + (threadIdx.x >> 5) + (p.first_side ? p.side[0].rows : 0);
   const int which = r >= p.side[0].rows ? 1 : 0;
   if (which) r -= p.side[0].rows;
   const PrepSide& sd = p.side[which];
@@ -135,8 +141,9 @@ __global__ void __launch_bounds__(256) prep_max_kernel(PrepParams p)
 template <typename T>
 __global__ void __launch_bounds__(256) prep_split_kernel(PrepParams p)
 {
+  if (p.run_flag != nullptr && __ldg(p.run_flag) == 0u) return;
   const int lane  = threadIdx.x & 31;
-  int64_t r       = static_cast<int64_t>(blockIdx.x) * 8 + (threadIdx.x >> 5);
+  int64_t r       = static_cast<int64_t>(blockIdx.x) * 8 + (threadIdx.x >> 5) + (p.first_side ? p.side[0].rows : 0);
   const int which = r >= p.side[0].rows ? 1 : 0;
   if (which) r -= p.side[0].rows;
   const PrepSide& sd = p.side[which];
@@ -146,7 +153,7 @@ __global__ void __launch_bounds__(256) prep_split_kernel(PrepParams p)
 
   const int ex = scale_exponent(__uint_as_float(p.gmax[0]));
   const int ey = scale_exponent(__uint_as_float(p.gmax[1]));
-  if (which == 0 && r == 0 && lane == 0) {
+  if (which == p.first_side && r == 0 && lane == 0) {
     const float c = p.mode == PREP_L2 ? -2.f : (p.mode == PREP_COSINE ? -1.f : 1.f);  // (PREP_INNER / PREP_INNER_NORM: +1)
     *p.coef       = c * p.coef_mul * ldexpf(1.f, -ex) * ldexpf(1.f, -ey);
   }
