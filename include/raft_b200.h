@@ -331,6 +331,43 @@ int b2d_kmeans_update_centroids(void* stream, const float* x, int64_t ldx, const
 int b2d_kmeans_init_plus_plus(void* stream, const float* x, int64_t ldx, const float* sample_weight, int64_t m, int64_t k,
                               int n_clusters, uint64_t seed, float* centroids, void* workspace, size_t workspace_bytes);
 
+/* Minimum spanning forest of an edge list (the MST step of raft::cluster::single_linkage, [RECALLED]
+ * raft::sparse::solver::mst): Borůvka on the device.  Edge e = (src[e], dst[e], w[e]) (int32 vertices, fp32 weights) is
+ * ordered by (w[e], e): this order is strict, so the forest is unique.  Self-loops, duplicate and reversed edges are
+ * allowed; an edge with an endpoint outside [0, n_vertices) is ignored; a NaN weight orders by its bits (a positive NaN
+ * after +inf).  Outputs (device pointers): *out_count (int32) forest edges in (w, e) order in out_src / out_dst / out_w
+ * (capacity n_vertices - 1; each edge as given), and out_colour[v] = the smallest vertex of v's tree.  n_vertices < 2^30
+ * and n_edges < 2^32 - 1, else B2D_ERR_UNSUPPORTED.  Only enqueues work: the rounds run on the device and the ones after
+ * the last merge return at once.  The workspace query returns SIZE_MAX for negative extents. */
+size_t b2d_mst_workspace_bytes(int64_t n_vertices, int64_t n_edges);
+int b2d_mst(void* stream, const int32_t* src, const int32_t* dst, const float* w, int64_t n_vertices, int64_t n_edges,
+            int32_t* out_src, int32_t* out_dst, float* out_w, int32_t* out_colour, int32_t* out_count, void* workspace,
+            size_t workspace_bytes);
+
+/* raft::cluster::single_linkage with LinkageDistance::KNN_GRAPH ([RECALLED], <= 25.12) for fp32 x:[m,d] (row-major, pitch
+ * ldx), metric B2D_L2Expanded or B2D_L2SqrtExpanded (else B2D_ERR_UNSUPPORTED):
+ *   1. the kNN graph of x with n_nb = min(m, max(2, floor(log2 m) + c)) neighbours (the fused kNN), edge i n_nb + s =
+ *      (i, idx[i, s], squared distance); a row's edge to itself is never used;
+ *   2. edges ordered by (squared weight, position): the tree and the merge order do not depend on the metric;
+ *   3. its minimum spanning forest by Borůvka (b2d_mst);
+ *   4. connect_components while the forest has more than one tree: every tree's row i of smallest (d_i, i), d_i the
+ *      squared distance to i's nearest row of another tree (the masked 1-NN), gives the edge (i, that row), appended
+ *      after the edges so far; Borůvka again;
+ *   5. the m - 1 edges in key order, merged on the host: merge t creates cluster m + t; children[t] = the two merged ids,
+ *      smaller first; deltas[t] = its weight (its square root for L2SqrtExpanded); sizes[t] = the new cluster's size
+ *      (scipy.cluster.hierarchy.linkage's conventions).  labels[i] = the cluster of row i after the first
+ *      m - n_clusters merges, numbered 0 .. n_clusters - 1 in order of each cluster's smallest row.
+ * children [m-1][2], deltas [m-1], sizes [m-1], labels [m] (int32 / fp32) are device pointers; *n_components_out (host)
+ * = the number of trees of the kNN graph's forest (before step 4).  1 <= n_clusters <= m, m >= 1, d >= 1 and a finite x
+ * (else B2D_ERR_INVALID_ARG, the last one found on the device); d <= 320, n_nb <= 64, m < 2^30 and m (n_nb + 1) < 2^32 - 1
+ * (else B2D_ERR_UNSUPPORTED).  The call synchronises its stream: once after step 3, once per connect round and twice
+ * for the dendrogram.  The workspace depends on (m, d, n_nb) only; the query returns SIZE_MAX for negative extents and
+ * for an unsupported n_nb or m. */
+size_t b2d_single_linkage_workspace_bytes(int64_t m, int64_t d, int c);
+int b2d_single_linkage(void* stream, int metric, const float* x, int64_t ldx, int64_t m, int64_t d, int c, int n_clusters,
+                       int32_t* children, float* deltas, int32_t* sizes, int32_t* labels, int32_t* n_components_out,
+                       void* workspace, size_t workspace_bytes);
+
 #ifdef __cplusplus
 }
 #endif

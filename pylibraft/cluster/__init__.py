@@ -1,1 +1,1 @@
-from . import kmeans  # noqa: F401
+from . import kmeans, single_linkage  # noqa: F401
