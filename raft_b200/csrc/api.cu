@@ -245,6 +245,16 @@ static TcWorkspace tc_layout(void* base, int64_t m, int64_t n, int64_t k, bool w
   return tc_layout(c, m, n, k, with_keys);
 }
 
+// w with side 0 (x) or side 1 (y) starting at prepared row r0: the operand, t and scale rows the tensor kernels read
+static TcWorkspace tc_rows(TcWorkspace w, int side, int64_t r0, int64_t k)
+{
+  const int64_t nkb = (k + 31) / 32;
+  (side ? w.yop : w.xop) += static_cast<size_t>(r0) * nkb * 64;
+  (side ? w.yt : w.xt) += r0;
+  (side ? w.ysc : w.xsc) += r0;
+  return w;
+}
+
 static bool is_expanded(int metric)
 {
   return metric == B2D_L2Expanded || metric == B2D_L2SqrtExpanded || metric == B2D_CosineExpanded ||
@@ -1277,7 +1287,6 @@ struct KnnCtx {
   KnnLayout L;
   TcParams p;       // m, knn_* set; n / idx_offset per pass
   int64_t k;
-  int nkb;
   bool any_fix;         // a knn_fix_kernel was launched
   int pass;
   const float* x; int64_t ldx;
@@ -1292,10 +1301,7 @@ struct KnnCtx {
 static int knn_pass(KnnCtx& c, int64_t off, int64_t width)
 {
   const KnnLayout& L = c.L;
-  TcWorkspace w2 = L.w;
-  w2.yop         = L.w.yop + static_cast<size_t>(off) * c.nkb * 64;
-  w2.yt          = L.w.yt + off;
-  w2.ysc         = L.w.ysc + off;
+  TcWorkspace w2 = tc_rows(L.w, 1, off, c.k);
   TcParams p     = c.p;
   p.n            = width;
   p.idx_offset   = off;
@@ -1354,7 +1360,6 @@ int b2d_knn(void* stream, int64_t* out_idx, float* out_dist, int metric, const f
   c.s   = s;
   c.L   = knn_layout(workspace, m, n, k, n_neighbors);
   c.k   = k;
-  c.nkb = static_cast<int>((k + 31) / 32);
   c.kk  = static_cast<int>(n_neighbors);
   c.pass = 0; c.any_fix = false; c.x = x; c.ldx = ldx; c.y = y; c.ldy = ldy;
   c.family = mode == PREP_COSINE ? 1 : 0; c.center = center;
@@ -1781,31 +1786,11 @@ int b2d_gram_matrix(void* stream, int kernel, int degree, double gamma, double c
 namespace {
 constexpr int64_t kKmHistCap = 1ll << 24;   // histogram words (n_clusters x row blocks) the layout allows
 
-struct KmLayout {
-  TcWorkspace tc;   // x (side 0) and the centroids (side 1) of the arg-min, keys[m]
-  KmCtrl* ctrl;
-  int* labels;      // [m]
-  float* w;         // [m] the normalised weights
-  float* rowf;      // [m] k-means++ D^2 / Random: the uniforms
-  unsigned* hist;   // [nc * nblk] label counts per (cluster, row block), scanned in place into the sort cursors
-  unsigned* tiles;  // [ntiles]
-  int* perm;        // [m] row ids sorted by label
-  int* slab;        // [m] their labels
-  double *sums, *wsums, *part, *wpart, *shift, *ipart, *bs;
-  float* best;      // [nc * k] n_init: the best centroids so far
-  float* sk_val;    // Random: select_k outputs and workspace
-  int64_t* sk_idx;
-  void* sk_ws;
-  size_t sk_bytes;
-  int64_t rb, nblk, nhist, ntiles, nchunks, nb;
-  size_t bytes;
-};
-
 // The stable counting sort of m rows by a label in [0, nc) (km_assign_kernel's histogram, km_scan_*, km_scatter_kernel):
 // row blocks of 2048 rows, or more when nc x blocks would exceed kKmHistCap words.  A function of (m, nc) only, so the
-// summation order of k-means never depends on the device.  nhist <= min(nc * ceil(m / 2048), max(nc, kKmHistCap)).
+// summation order of k-means never depends on the device.
 struct KmSortPlan {
-  int64_t rb, nblk, nhist, ntiles;
+  int64_t rb, nblk, nhist;
 };
 
 static KmSortPlan km_sort_plan(int64_t m, int64_t nc)
@@ -1819,9 +1804,87 @@ static KmSortPlan km_sort_plan(int64_t m, int64_t nc)
   }
   P.nblk   = (mm + P.rb - 1) / P.rb;
   P.nhist  = ncc * P.nblk;
-  P.ntiles = (P.nhist + kKmScanTile - 1) / kKmScanTile;
   return P;
 }
+
+// the sort's regions in the workspace
+struct KmSort {
+  unsigned* hist;   // label counts per (label, row block), scanned in place into the sort cursors
+  unsigned* tiles;  // scan tile sums
+  int* perm;        // [m] row ids sorted by label
+  int* slab;        // [m] their labels
+  KmCtrl* ctrl;     // receives the scan total
+};
+
+// Sized for the plan of exactly nc labels, or with any_count for the plan of any label count up to nc:
+// km_sort_plan(m, c).nhist <= min(c * ceil(m / 2048), max(c, kKmHistCap)), which grows with c.  The histogram holds at
+// least nc words, so its tiles also serve a scan of nc words (km_scan).
+static KmSort km_sort_regions(Carve& c, int64_t m, int64_t nc, bool any_count)
+{
+  const int64_t mm = std::max<int64_t>(m, 1), ncc = std::max<int64_t>(nc, 1);
+  const int64_t words = any_count ? std::min(ncc * ((mm + kKmSub - 1) / kKmSub), std::max(ncc, kKmHistCap))
+                                  : km_sort_plan(m, nc).nhist;
+  KmSort S;
+  S.hist  = c.take<unsigned>(words);
+  S.tiles = c.take<unsigned>((words + kKmScanTile - 1) / kKmScanTile);
+  S.perm  = c.take<int>(m);
+  S.slab  = c.take<int>(m);
+  S.ctrl  = c.take<KmCtrl>(1);
+  return S;
+}
+
+static unsigned km_grid(int64_t n, int per = 256) { return static_cast<unsigned>(std::max<int64_t>(1, std::min<int64_t>((n + per - 1) / per, 1 << 16))); }
+
+// exclusive scan of the words a[0, n) in place, the total into ctrl->total
+static int km_scan(cudaStream_t s, const unsigned* run, unsigned* a, int64_t n, unsigned* tiles, KmCtrl* ctrl)
+{
+  const unsigned ntiles = static_cast<unsigned>((n + kKmScanTile - 1) / kKmScanTile);
+  km_scan_tiles_kernel<<<ntiles, kKmThreads, 0, s>>>(run, a, n, tiles);
+  km_scan_kernel<<<ntiles, kKmThreads, 0, s>>>(run, a, n, tiles, ctrl);
+  B2D_CUDA(cudaGetLastError());
+  return B2D_OK;
+}
+
+// the histogram of given labels (km_assign fuses it into the arg-min)
+static int km_sort_count(cudaStream_t s, const KmSort& S, const KmSortPlan& P, const int* labels, int64_t m, int64_t nc)
+{
+  km_begin_kernel<<<km_grid(P.nhist), 256, 0, s>>>(nullptr, nullptr, 0, nullptr, nullptr, S.hist, P.nhist);
+  km_assign_kernel<<<static_cast<unsigned>(P.nblk), kKmThreads, 0, s>>>(nullptr, nullptr, const_cast<int*>(labels), nullptr, m,
+                                                                        static_cast<int>(nc), P.rb, P.nblk, S.hist, nullptr);
+  B2D_CUDA(cudaGetLastError());
+  return B2D_OK;
+}
+
+// the histogram scanned into the sort cursors, then the rows scattered into perm / slab
+static int km_sort_scatter(cudaStream_t s, const unsigned* run, const KmSort& S, const KmSortPlan& P, const int* labels,
+                           int64_t m, int64_t nc)
+{
+  int rc = km_scan(s, run, S.hist, P.nhist, S.tiles, S.ctrl);
+  if (rc) return rc;
+  const int end_bit = 32 - __builtin_clz(static_cast<unsigned>(nc));
+  km_scatter_kernel<<<static_cast<unsigned>(P.nblk), kKmThreads, 0, s>>>(run, labels, m, static_cast<int>(nc), end_bit, P.rb,
+                                                                         P.nblk, S.hist, S.perm, S.slab);
+  B2D_CUDA(cudaGetLastError());
+  return B2D_OK;
+}
+
+struct KmLayout {
+  TcWorkspace tc;   // x (side 0) and the centroids (side 1) of the arg-min, keys[m]
+  KmSortPlan P;
+  KmSort sort;
+  KmCtrl* ctrl;     // the fit's control words: sort.ctrl
+  int* labels;      // [m]
+  float* w;         // [m] the normalised weights
+  float* rowf;      // [m] k-means++ D^2 / Random: the uniforms
+  double *sums, *wsums, *part, *wpart, *shift, *ipart, *bs;
+  float* best;      // [nc * k] n_init: the best centroids so far
+  float* sk_val;    // Random: select_k outputs and workspace
+  int64_t* sk_idx;
+  void* sk_ws;
+  size_t sk_bytes;
+  int64_t nchunks, nb;
+  size_t bytes;
+};
 
 static KmLayout km_layout(void* base, int64_t m, int64_t k, int64_t nc)
 {
@@ -1830,27 +1893,20 @@ static KmLayout km_layout(void* base, int64_t m, int64_t k, int64_t nc)
   L.tc      = tc_layout(c, m, nc, k, false);
   L.tc.keys = c.take<long long>(m);
   const int64_t mm = std::max<int64_t>(m, 1);
-  const KmSortPlan P = km_sort_plan(m, nc);
-  L.rb      = P.rb;
-  L.nblk    = P.nblk;
-  L.nhist   = P.nhist;
-  L.ntiles  = P.ntiles;
+  L.P       = km_sort_plan(m, nc);
   L.nchunks = (mm + kKmChunk - 1) / kKmChunk;
   L.nb      = (mm + kKmPpBlock - 1) / kKmPpBlock;
-  L.ctrl   = c.take<KmCtrl>(1);
   L.labels = c.take<int>(m);
   L.w      = c.take<float>(m);
   L.rowf   = c.take<float>(m);
-  L.hist   = c.take<unsigned>(L.nhist);
-  L.tiles  = c.take<unsigned>(L.ntiles);
-  L.perm   = c.take<int>(m);
-  L.slab   = c.take<int>(m);
+  L.sort   = km_sort_regions(c, m, nc, false);
+  L.ctrl   = L.sort.ctrl;
   L.sums   = c.take<double>(static_cast<size_t>(nc) * k);
   L.wsums  = c.take<double>(nc);
   L.part   = c.take<double>(static_cast<size_t>(L.nchunks) * 2 * k);
   L.wpart  = c.take<double>(L.nchunks * 2);
   L.shift  = c.take<double>(nc);
-  L.ipart  = c.take<double>(L.nblk);
+  L.ipart  = c.take<double>(L.P.nblk);
   L.bs     = c.take<double>(static_cast<size_t>(L.nb) * kKmPpMaxTrials);
   L.best   = c.take<float>(static_cast<size_t>(nc) * k);
   L.sk_val = c.take<float>(nc);
@@ -1872,16 +1928,14 @@ static int km_args(const float* x, int64_t ldx, int64_t m, int64_t k, int64_t nc
   return B2D_OK;
 }
 
-static unsigned km_grid(int64_t n, int per = 256) { return static_cast<unsigned>(std::max<int64_t>(1, std::min<int64_t>((n + per - 1) / per, 1 << 16))); }
-
 // arg-min of every row against the prepared centroids: labels, inertia partials, label histogram (when hist)
 static int km_assign(cudaStream_t s, const KmLayout& L, int64_t m, int64_t k, int64_t nc, const float* c, const float* w,
                      int* labels, const unsigned* run, bool prep_y, bool hist)
 {
-  const int64_t nh = hist ? L.nhist : 0;
+  const int64_t nh = hist ? L.P.nhist : 0;
   // (the centroid side's exponent and scale flag are zeroed only where it is prepared again below)
   km_begin_kernel<<<km_grid(std::max(m, nh)), 256, 0, s>>>(run, L.tc.keys, m, prep_y ? L.tc.gmax : nullptr, L.tc.nonuni,
-                                                           hist ? L.hist : nullptr, nh);
+                                                           hist ? L.sort.hist : nullptr, nh);
   B2D_CUDA(cudaGetLastError());
   if (prep_y) {
     int rc = launch_prep<float>(s, L.tc, nullptr, 0, 1, m, c, k, 1, nc, k, nullptr, nullptr, PREP_L2, 0, 0, 1.f, 0.f,
@@ -1893,30 +1947,25 @@ static int km_assign(cudaStream_t s, const KmLayout& L, int64_t m, int64_t k, in
   p.m = m; p.n = nc; p.keys = L.tc.keys; p.run_flag = run;
   int rc = launch_tc(s, L.tc, p, k, EPI_MINLOC, POST_NONE);
   if (rc) return rc;
-  km_assign_kernel<<<static_cast<unsigned>(L.nblk), kKmThreads, 0, s>>>(run, L.tc.keys, labels, w, m, static_cast<int>(nc),
-                                                                        L.rb, L.nblk, hist ? L.hist : nullptr, L.ipart);
+  km_assign_kernel<<<static_cast<unsigned>(L.P.nblk), kKmThreads, 0, s>>>(run, L.tc.keys, labels, w, m, static_cast<int>(nc),
+                                                                          L.P.rb, L.P.nblk, hist ? L.sort.hist : nullptr,
+                                                                          L.ipart);
   B2D_CUDA(cudaGetLastError());
   return B2D_OK;
 }
 
-// new centroids from the histogram km_assign (or a labels-only km_assign_kernel) left: scan, stable scatter, fp64 sums
+// new centroids from the histogram km_assign (or km_sort_count) left: scan, stable scatter, fp64 sums
 static int km_update(cudaStream_t s, const KmLayout& L, const float* x, int64_t ldx, int64_t m, int64_t k, int64_t nc,
                      const float* w, const int* labels, const float* old_c, float* out_c, float* wpc, const unsigned* run)
 {
-  km_scan_tiles_kernel<<<static_cast<unsigned>(L.ntiles), kKmThreads, 0, s>>>(run, L.hist, L.nhist, L.tiles);
-  B2D_CUDA(cudaGetLastError());
-  km_scan_kernel<<<static_cast<unsigned>(L.ntiles), kKmThreads, 0, s>>>(run, L.hist, L.nhist, L.tiles, L.ctrl);
-  B2D_CUDA(cudaGetLastError());
-  const int end_bit = 32 - __builtin_clz(static_cast<unsigned>(nc));
-  km_scatter_kernel<<<static_cast<unsigned>(L.nblk), kKmThreads, 0, s>>>(run, labels, m, static_cast<int>(nc), end_bit, L.rb,
-                                                                         L.nblk, L.hist, L.perm, L.slab);
-  B2D_CUDA(cudaGetLastError());
+  int rc = km_sort_scatter(s, run, L.sort, L.P, labels, m, nc);
+  if (rc) return rc;
   const dim3 g(static_cast<unsigned>(L.nchunks), static_cast<unsigned>(std::min<int64_t>((k + kKmCols - 1) / kKmCols, 65535)));
-  km_sum_kernel<<<g, kKmCols, 0, s>>>(run, x, ldx, static_cast<int>(k), w, L.perm, L.slab, L.hist, L.nblk, L.ctrl, L.sums,
-                                      L.wsums, L.part, L.wpart);
+  km_sum_kernel<<<g, kKmCols, 0, s>>>(run, x, ldx, static_cast<int>(k), w, L.sort.perm, L.sort.slab, L.sort.hist, L.P.nblk,
+                                      L.ctrl, L.sums, L.wsums, L.part, L.wpart);
   B2D_CUDA(cudaGetLastError());
-  km_finalize_kernel<<<static_cast<unsigned>(nc), kKmCols, 0, s>>>(run, static_cast<int>(k), L.hist, L.nblk, L.sums, L.wsums,
-                                                                   L.part, L.wpart, old_c, out_c, L.shift, wpc);
+  km_finalize_kernel<<<static_cast<unsigned>(nc), kKmCols, 0, s>>>(run, static_cast<int>(k), L.sort.hist, L.P.nblk, L.sums,
+                                                                   L.wsums, L.part, L.wpart, old_c, out_c, L.shift, wpc);
   B2D_CUDA(cudaGetLastError());
   return B2D_OK;
 }
@@ -2011,16 +2060,16 @@ int b2d_kmeans_fit(void* stream, int n_clusters, int max_iter, double tol, int i
       if (rc) return rc;
       rc = km_update(s, L, x, ldx, m, k, nc, w, L.labels, centroids, centroids, nullptr, run);
       if (rc) return rc;
-      km_converge_kernel<<<1, kKmThreads, 0, s>>>(run, L.ctrl, L.shift, static_cast<int>(nc), L.ipart, L.nblk, tol,
+      km_converge_kernel<<<1, kKmThreads, 0, s>>>(run, L.ctrl, L.shift, static_cast<int>(nc), L.ipart, L.P.nblk, tol,
                                                   inertia_check);
       B2D_CUDA(cudaGetLastError());
     }
     // the inertia of the returned centroids
     rc = km_assign(s, L, m, k, nc, centroids, w, L.labels, nullptr, true, false);
     if (rc) return rc;
-    km_cost_kernel<<<static_cast<unsigned>(L.nblk), kKmThreads, 0, s>>>(x, ldx, static_cast<int>(k), centroids, L.labels, w,
-                                                                        m, L.rb, L.ipart);
-    km_finish_kernel<<<1, kKmThreads, 0, s>>>(L.ctrl, L.ipart, L.nblk, runs == 1 ? inertia : nullptr,
+    km_cost_kernel<<<static_cast<unsigned>(L.P.nblk), kKmThreads, 0, s>>>(x, ldx, static_cast<int>(k), centroids, L.labels,
+                                                                          w, m, L.P.rb, L.ipart);
+    km_finish_kernel<<<1, kKmThreads, 0, s>>>(L.ctrl, L.ipart, L.P.nblk, runs == 1 ? inertia : nullptr,
                                               runs == 1 ? n_iter : nullptr);
     B2D_CUDA(cudaGetLastError());
     if (runs > 1) {
@@ -2058,9 +2107,9 @@ int b2d_kmeans_predict(void* stream, const float* x, int64_t ldx, const float* s
   int* lab = labels ? labels : L.labels;
   rc = km_assign(s, L, m, k, nc, centroids, w, lab, nullptr, false, false);
   if (rc) return rc;
-  km_cost_kernel<<<static_cast<unsigned>(L.nblk), kKmThreads, 0, s>>>(x, ldx, static_cast<int>(k), centroids, lab, w, m,
-                                                                      L.rb, L.ipart);
-  km_finish_kernel<<<1, kKmThreads, 0, s>>>(L.ctrl, L.ipart, L.nblk, inertia, nullptr);
+  km_cost_kernel<<<static_cast<unsigned>(L.P.nblk), kKmThreads, 0, s>>>(x, ldx, static_cast<int>(k), centroids, lab, w, m,
+                                                                        L.P.rb, L.ipart);
+  km_finish_kernel<<<1, kKmThreads, 0, s>>>(L.ctrl, L.ipart, L.P.nblk, inertia, nullptr);
   B2D_CUDA(cudaGetLastError());
   return B2D_OK;
 }
@@ -2078,10 +2127,8 @@ int b2d_kmeans_update_centroids(void* stream, const float* x, int64_t ldx, const
   rc = check_workspace(workspace, workspace_bytes, km_layout(nullptr, m, k, nc).bytes);
   if (rc) return rc;
   const KmLayout L = km_layout(workspace, m, k, nc);
-  km_begin_kernel<<<km_grid(L.nhist), 256, 0, s>>>(nullptr, nullptr, 0, nullptr, nullptr, L.hist, L.nhist);
-  km_assign_kernel<<<static_cast<unsigned>(L.nblk), kKmThreads, 0, s>>>(nullptr, nullptr, const_cast<int*>(labels), nullptr, m,
-                                                                        static_cast<int>(nc), L.rb, L.nblk, L.hist, nullptr);
-  B2D_CUDA(cudaGetLastError());
+  rc = km_sort_count(s, L.sort, L.P, labels, m, nc);
+  if (rc) return rc;
   return km_update(s, L, x, ldx, m, k, nc, sample_weight, labels, old_centroids, new_centroids, weight_per_cluster, nullptr);
 }
 
@@ -2225,10 +2272,9 @@ struct SlLayout {
   float* xs;                // [m, d] the colour-sorted rows
   long long *keys, *cbest;  // [m] masked arg-min of every sorted row, [c] best row of every component
   unsigned* bad;            // [8] masked_classify's flag: 0 (the component ends are valid by construction)
-  int *grp, *lab, *ends, *perm, *slab;   // [m]
+  int *grp, *lab, *ends;    // [m]
   unsigned* ids;            // [m] root flags, scanned into dense component ids
-  unsigned *hist, *tiles;   // counting sort (km_sort_plan for up to m components)
-  KmCtrl* kctrl;            // (km_scan_kernel's total)
+  KmSort sort;              // the rows sorted by component, for up to m components
   unsigned* bits;           // [5 m] adjacency bits of one chunk
   uint8_t* cls;             // tile classes of one chunk
   uint8_t* adj;             // [128 m] adjacency of one chunk
@@ -2264,14 +2310,9 @@ static SlLayout sl_layout(void* base, int64_t m, int64_t d, int64_t n_nb)
   L.grp   = b.take<int>(m);
   L.lab   = b.take<int>(m);
   L.ends  = b.take<int>(m);
-  L.perm  = b.take<int>(m);
-  L.slab  = b.take<int>(m);
   L.ids   = b.take<unsigned>(m);
+  L.sort  = km_sort_regions(b, m, m, true);
   const int64_t mm = std::max<int64_t>(m, 1);
-  const int64_t hist_cap = std::min<int64_t>(mm * ((mm + kKmSub - 1) / kKmSub), std::max<int64_t>(mm, kKmHistCap));
-  L.hist  = b.take<unsigned>(hist_cap);
-  L.tiles = b.take<unsigned>((std::max(hist_cap, mm) + kKmScanTile - 1) / kKmScanTile);
-  L.kctrl = b.take<KmCtrl>(1);
   L.bits  = b.take<unsigned>(static_cast<size_t>(5) * mm);
   L.cls   = b.take<uint8_t>(static_cast<size_t>(sl_max_chunk(m) / TC_BM) * ((mm + TC_BN - 1) / TC_BN));
   L.adj   = b.take<uint8_t>(static_cast<size_t>(128) * mm);
@@ -2286,47 +2327,39 @@ static int sl_connect(cudaStream_t s, const SlLayout& L, const float* x, int64_t
                       int64_t e0)
 {
   const MstLayout& T = L.mst;
-  const unsigned row_tiles = static_cast<unsigned>((m + kKmScanTile - 1) / kKmScanTile);
+  const KmSort& S = L.sort;
   sl_root_flags_kernel<<<sl_grid(m), 256, 0, s>>>(T.colour, L.ids, m);
-  km_scan_tiles_kernel<<<row_tiles, kKmThreads, 0, s>>>(nullptr, L.ids, m, L.tiles);
-  km_scan_kernel<<<row_tiles, kKmThreads, 0, s>>>(nullptr, L.ids, m, L.tiles, L.kctrl);
+  int rc = km_scan(s, nullptr, L.ids, m, S.tiles, S.ctrl);
+  if (rc) return rc;
   sl_dense_label_kernel<<<sl_grid(m), 256, 0, s>>>(T.colour, L.ids, L.lab, m);
   B2D_CUDA(cudaGetLastError());
   const KmSortPlan P = km_sort_plan(m, c);
-  km_begin_kernel<<<km_grid(P.nhist), 256, 0, s>>>(nullptr, nullptr, 0, nullptr, nullptr, L.hist, P.nhist);
-  km_assign_kernel<<<static_cast<unsigned>(P.nblk), kKmThreads, 0, s>>>(nullptr, nullptr, L.lab, nullptr, m, static_cast<int>(c),
-                                                                        P.rb, P.nblk, L.hist, nullptr);
-  km_scan_tiles_kernel<<<static_cast<unsigned>(P.ntiles), kKmThreads, 0, s>>>(nullptr, L.hist, P.nhist, L.tiles);
-  km_scan_kernel<<<static_cast<unsigned>(P.ntiles), kKmThreads, 0, s>>>(nullptr, L.hist, P.nhist, L.tiles, L.kctrl);
-  const int end_bit = 32 - __builtin_clz(static_cast<unsigned>(c));
-  km_scatter_kernel<<<static_cast<unsigned>(P.nblk), kKmThreads, 0, s>>>(nullptr, L.lab, m, static_cast<int>(c), end_bit, P.rb,
-                                                                         P.nblk, L.hist, L.perm, L.slab);
-  sl_ends_kernel<<<sl_grid(c), 256, 0, s>>>(L.hist, P.nblk, c, L.ends);
-  km_gather_rows_kernel<int><<<static_cast<unsigned>(m), 128, 0, s>>>(x, ldx, static_cast<int>(d), L.perm,
+  rc = km_sort_count(s, S, P, L.lab, m, c);
+  if (rc) return rc;
+  rc = km_sort_scatter(s, nullptr, S, P, L.lab, m, c);
+  if (rc) return rc;
+  sl_ends_kernel<<<sl_grid(c), 256, 0, s>>>(S.hist, P.nblk, c, L.ends);
+  km_gather_rows_kernel<int><<<static_cast<unsigned>(m), 128, 0, s>>>(x, ldx, static_cast<int>(d), S.perm,
                                                                       static_cast<int>(m), L.xs);
   B2D_CUDA(cudaGetLastError());
   // y (and x) prepared once per round; every chunk takes a window of the x side
-  int rc = launch_prep<float>(s, L.tc, L.xs, d, 1, m, L.xs, d, 1, m, d, nullptr, nullptr, PREP_L2, 0);
+  rc = launch_prep<float>(s, L.tc, L.xs, d, 1, m, L.xs, d, 1, m, d, nullptr, nullptr, PREP_L2, 0);
   if (rc) return rc;
   masked_group_map_kernel<<<sl_grid(m), 256, 0, s>>>(L.grp, L.ends, c, m);
   B2D_CUDA(cudaMemsetAsync(L.bad, 0, 32, s));
   minloc_init_kernel<<<sl_grid(m), 256, 0, s>>>(L.keys, m);
   minloc_init_kernel<<<sl_grid(c), 256, 0, s>>>(L.cbest, c);
   B2D_CUDA(cudaGetLastError());
-  const int64_t mc = sl_chunk_rows(m, c), nkb = (d + 31) / 32;
+  const int64_t mc = sl_chunk_rows(m, c);
   for (int64_t r0 = 0; r0 < m; r0 += mc) {
     const int64_t rows = std::min(mc, m - r0);
-    sl_adj_kernel<<<km_grid(rows * c), 256, 0, s>>>(L.slab, r0, rows, c, L.adj);
+    sl_adj_kernel<<<km_grid(rows * c), 256, 0, s>>>(S.slab, r0, rows, c, L.adj);
     B2D_CUDA(cudaGetLastError());
-    TcWorkspace w = L.tc;
-    w.xop += static_cast<size_t>(r0) * nkb * 64;
-    w.xt += r0;
-    w.xsc += r0;
-    rc = masked_keys(s, w, L.keys + r0, L.grp, L.bits, L.cls, L.bad, L.adj, c, L.ends, c, rows, m, d);
+    rc = masked_keys(s, tc_rows(L.tc, 0, r0, d), L.keys + r0, L.grp, L.bits, L.cls, L.bad, L.adj, c, L.ends, c, rows, m, d);
     if (rc) return rc;
   }
-  sl_comp_best_kernel<<<sl_grid(m), 256, 0, s>>>(L.keys, L.slab, m, L.cbest);
-  sl_connect_kernel<<<sl_grid(c), 256, 0, s>>>(L.cbest, L.keys, L.perm, L.slab, c, e0, L.src, L.dst, L.w, T.ctrl);
+  sl_comp_best_kernel<<<sl_grid(m), 256, 0, s>>>(L.keys, S.slab, m, L.cbest);
+  sl_connect_kernel<<<sl_grid(c), 256, 0, s>>>(L.cbest, L.keys, S.perm, S.slab, c, e0, L.src, L.dst, L.w, T.ctrl);
   B2D_CUDA(cudaGetLastError());
   return B2D_OK;
 }

@@ -1,9 +1,16 @@
-"""Generates tests/golden/workspace_contract.json (run here, without a GPU; the output is committed).
+"""Generates the workspace-contract fixtures under tests/golden (run here, without a GPU; the outputs are committed).
 
-The fixture pins the workspace contract of the C ABI:
-  bytes   every *_workspace_bytes query over a grid that reaches every branch of the workspace layouts;
-  errors  (status, b2d_last_error()) of every entry point that takes a workspace, given a null workspace, one byte too
-          few at an aligned address, or the full size at an odd address -- with every other argument valid.
+Each fixture pins the workspace contract of a group of C ABI entry points:
+  bytes   every *_workspace_bytes query of the group over a grid that reaches every branch of its workspace layouts;
+  errors  (status, b2d_last_error()) of every entry point of the group that takes a workspace, given a null workspace,
+          one byte too few at an aligned address, or the full size at an odd address -- with every other argument valid.
+The fixtures:
+  workspace_contract.json                 distances, nearest neighbours, select_k and the stats;
+  kmeans_workspace_contract.json          k-means, over row counts past the histogram cap and 1 to 10^5 clusters;
+  gram_workspace_contract.json            gram_matrix for every kernel id (and two invalid ones) and dtype;
+  single_linkage_workspace_contract.json  single_linkage over row counts from 1 to 10^6 (around the 2048-row sort blocks
+                                          and the 2^20-row tile-class cap) and c from -5 to 60 (n_nb from 2 to past 64),
+                                          and the edge-list MST.
 Pointers are fake addresses: the calls must fail in validation, before anything reaches the device.  A case that
 returns B2D_OK or B2D_ERR_CUDA got past validation, so it is refused rather than recorded.  The library is the one
 raft_b200._lib loads (RAFT_B200_LIB selects another build of the same ABI).
@@ -16,8 +23,6 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, os.path.dirname(os.path.dirname(HERE)))
 
 from raft_b200 import _lib  # noqa: E402
-
-OUT = os.path.join(HERE, "workspace_contract.json")
 
 METRICS = list(range(-1, 21))                   # every DistanceType value, 13 (Haversine) and two out of range
 DTYPES = [0, 1, 2, 3]                           # F32, F16, F64 and one unknown
@@ -111,12 +116,89 @@ def error_cases(L):
     ]
 
 
-def main():
-    L = _lib.lib()
+KM_MS = [1, 37, 2048, 2049, 100000, 1000000]
+KM_NCS = [1, 17, 1000, 100000]
+KM_NEG = [(-1, 32, 4), (37, -1, 4), (37, 32, -1)]
+
+
+def kmeans_byte_queries():
+    shapes = [(m, k, nc) for m in KM_MS for k in KS for nc in KM_NCS] + [(0, 32, 0), (37, 0, 4)] + KM_NEG
+    return {"b2d_kmeans_workspace_bytes": shapes}
+
+
+def kmeans_error_cases(L):
+    wb = L.b2d_kmeans_workspace_bytes
+    m, k, nc = 5000, 96, 40
+    return [
+        ("fit array", "b2d_kmeans_fit", [None, nc, 20, 1e-4, 2, 1, 0, 0, D, k, None, m, k, D, D, D], wb(m, k, nc), True),
+        ("fit k-means++ weighted n_init=3", "b2d_kmeans_fit", [None, nc, 20, 1e-4, 0, 3, 7, 1, D, k, D, m, k, D, D, D],
+         wb(m, k, nc), True),
+        ("predict", "b2d_kmeans_predict", [None, D, k, None, m, k, D, nc, D, D, 1], wb(m, k, nc), True),
+        ("update_centroids", "b2d_kmeans_update_centroids", [None, D, k, D, D, m, k, D, nc, D, None], wb(m, k, nc), True),
+        ("init_plus_plus", "b2d_kmeans_init_plus_plus", [None, D, k, None, m, k, nc, 3, D], wb(m, k, nc), True),
+    ]
+
+
+GRAM_KERNEL_IDS = list(range(-1, 5))   # LINEAR, POLYNOMIAL, RBF, TANH and one invalid id on either side
+
+
+def gram_byte_queries():
+    edges = [(0, 29, 32), (37, 0, 32), (37, 29, 0)] + NEG
+    shapes = [(37, 29, k) for k in KS] + edges + [(BIG_M, 1000, 96), (1000, 1 << 20, 128)]
+    return {"b2d_gram_matrix_workspace_bytes": [(kr, dt) + s for kr in GRAM_KERNEL_IDS for dt in DTYPES for s in shapes]}
+
+
+def gram_error_cases(L):
+    gw = L.b2d_gram_matrix_workspace_bytes
+    m, n, k = 300, 500, 96
+    return [
+        ("gram rbf f32", "b2d_gram_matrix", [None, 2, 0, 0.5, 0.0, 0, D, k, D, k, D, n, m, n, k, 1], gw(2, 0, m, n, k), True),
+        ("gram polynomial f16 col-major", "b2d_gram_matrix", [None, 1, 3, 0.1, 1.0, 1, D, m, D, n, D, m, m, n, k, 0],
+         gw(1, 1, n, m, k), True),
+        ("gram tanh f32 k=400", "b2d_gram_matrix", [None, 3, 0, 0.1, -1.0, 0, D, 400, D, 400, D, n, m, n, 400, 1],
+         gw(3, 0, m, n, 400), True),
+        ("gram linear f64", "b2d_gram_matrix", [None, 0, 0, 1.0, 0.0, 2, D, k, D, k, D, n, m, n, k, 1], gw(0, 2, m, n, k), False),
+        ("gram rbf f64 col-major", "b2d_gram_matrix", [None, 2, 0, 0.5, 0.0, 2, D, m, D, n, D, m, m, n, k, 0],
+         gw(2, 2, n, m, k), False),
+    ]
+
+
+SL_MS = [1, 2, 37, 2048, 2049, 100000, (1 << 20) + 1, 1000000]
+SL_CS = [-5, 1, 15, 45, 60]
+MST_NS = [0, 1, 1000, 1000000]
+MST_ES = [0, 5000, 10 ** 7]
+
+
+def single_linkage_byte_queries():
+    sl = [(m, d, c) for m in SL_MS for d in KS for c in SL_CS] + [(0, 32, 15), (-1, 32, 15), (37, -1, 15)]
+    mst = [(n, e) for n in MST_NS for e in MST_ES] + [(-1, 10), (10, -1)]
+    return {"b2d_single_linkage_workspace_bytes": sl, "b2d_mst_workspace_bytes": mst}
+
+
+def single_linkage_error_cases(L):
+    m, d, n, e = 5000, 96, 3000, 20000
+    return [
+        ("single_linkage euclidean", "b2d_single_linkage", [None, 1, D, d, m, d, 15, 7, D, D, D, D, D],
+         L.b2d_single_linkage_workspace_bytes(m, d, 15), True),
+        ("single_linkage sqeuclidean c=40", "b2d_single_linkage", [None, 0, D, d + 3, m, d, 40, 1, D, D, D, D, D],
+         L.b2d_single_linkage_workspace_bytes(m, d, 40), True),
+        ("mst", "b2d_mst", [None, D, D, D, n, e, D, D, D, D, D], L.b2d_mst_workspace_bytes(n, e), True),
+    ]
+
+
+FIXTURES = {   # file -> (size queries, error cases)
+    "workspace_contract.json": (byte_queries, error_cases),
+    "kmeans_workspace_contract.json": (kmeans_byte_queries, kmeans_error_cases),
+    "gram_workspace_contract.json": (gram_byte_queries, gram_error_cases),
+    "single_linkage_workspace_contract.json": (single_linkage_byte_queries, single_linkage_error_cases),
+}
+
+
+def record(L, queries, cases):
     out = {"bytes": {}, "errors": []}
-    for fn, cases in byte_queries().items():
-        out["bytes"][fn] = [list(a) + [getattr(L, fn)(*a)] for a in cases]
-    for name, fn, args, need, aligned in error_cases(L):
+    for fn, args in queries().items():
+        out["bytes"][fn] = [list(a) + [getattr(L, fn)(*a)] for a in args]
+    for name, fn, args, need, aligned in cases(L):
         assert 0 < need < 2 ** 63, (name, need)
         variants = [("null", None, need), ("short", WS, need - 1)] + ([("odd", ODD, need)] if aligned else [])
         for case, ws, nbytes in variants:
@@ -126,12 +208,20 @@ def main():
                 raise SystemExit(f"{name} / {case}: status {rc} -- the call got past validation; not recorded")
             out["errors"].append({"name": name, "case": case, "fn": fn, "args": a, "rc": rc,
                                   "msg": L.b2d_last_error().decode()})
-    with open(OUT, "w") as f:   # one case per line, so that a change to the contract reads as a short diff
-        f.write('{"bytes": {\n')
-        f.write(",\n".join(json.dumps(fn) + ": [\n" + ",\n".join(json.dumps(r) for r in rows) + "]"
-                           for fn, rows in out["bytes"].items()))
-        f.write('},\n"errors": [\n' + ",\n".join(json.dumps(e) for e in out["errors"]) + "]}\n")
-    print("wrote", OUT, sum(map(len, out["bytes"].values())), "size queries,", len(out["errors"]), "error cases")
+    return out
+
+
+def main():
+    L = _lib.lib()
+    for name, (queries, cases) in FIXTURES.items():
+        out = record(L, queries, cases)
+        path = os.path.join(HERE, name)
+        with open(path, "w") as f:   # one case per line, so that a change to the contract reads as a short diff
+            f.write('{"bytes": {\n')
+            f.write(",\n".join(json.dumps(fn) + ": [\n" + ",\n".join(json.dumps(r) for r in rows) + "]"
+                               for fn, rows in out["bytes"].items()))
+            f.write('},\n"errors": [\n' + ",\n".join(json.dumps(e) for e in out["errors"]) + "]}\n")
+        print("wrote", path, sum(map(len, out["bytes"].values())), "size queries,", len(out["errors"]), "error cases")
 
 
 if __name__ == "__main__":

@@ -2,18 +2,16 @@
 argument check of the C ABI, B2D_ERR_CUDA without a device, and the C++ shim's compile (its run on the GPU is marked
 gpu)."""
 import os
-import shutil
 import subprocess
 
 import numpy as np
 import pytest
 import torch
 
+import cpp_build
 import gram_ref
-from raft_b200 import _build, _lib
+from raft_b200 import _lib
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-NVCC = shutil.which("nvcc") or "/usr/local/cuda/bin/nvcc"
 
 SIZE_MAX = 2 ** 64 - 1
 P = 1 << 12   # a non-null pointer that is never dereferenced (every call below fails before any work)
@@ -126,15 +124,8 @@ def build_dir(tmp_path_factory):
 
 
 def compile_shim(build_dir, mock_raft):
-    _build.build()
     exe = os.path.join(build_dir, "gram_shim_mockraft" if mock_raft else "gram_shim")
-    extra = ["-DRAFT_B200_USE_REAL_RAFT", "-I", os.path.join(ROOT, "tests", "cpp", "mock_raft")] if mock_raft else []
-    cmd = [NVCC, "-std=c++17", "-O1", "-I", os.path.join(ROOT, "include")] + extra + [
-           "-o", exe, os.path.join(ROOT, "tests", "cpp", "gram_shim_test.cu"), "-L", os.path.dirname(_build.SO_PATH),
-           "-lraft_b200", "-Xlinker", "-rpath", "-Xlinker", os.path.dirname(_build.SO_PATH)]
-    res = subprocess.run(cmd, capture_output=True, text=True)
-    assert res.returncode == 0, res.stdout + res.stderr
-    return exe
+    return cpp_build.build("gram_shim_test.cu", exe, mock_raft)
 
 
 @pytest.mark.parametrize("mock_raft", [False, True])

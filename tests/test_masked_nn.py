@@ -2,7 +2,6 @@
 the tile classification and the kernel's skip schedule (host replay), and the C++ shim's compile."""
 import ctypes
 import os
-import shutil
 import subprocess
 
 import numpy as np
@@ -10,11 +9,9 @@ import pytest
 import torch
 from scipy.spatial.distance import cdist
 
+import cpp_build
 from masked_nn_ref import FLT_MAX, NO_CANDIDATE, column_groups, masked_l2_nn as ref_masked_l2_nn, tile_classes
-from raft_b200 import _build, _lib
-
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-NVCC = shutil.which("nvcc") or "/usr/local/cuda/bin/nvcc"
+from raft_b200 import _lib
 
 
 def brute(x, y, adj, gidx):
@@ -97,19 +94,10 @@ def test_valid_arguments_without_gpu_report_cuda_error():
     assert _call(L, G=0, adj=0, gidx=0, ld_adj=0) == _lib.B2D_ERR_CUDA
 
 
-def _schedule_exe(build_dir):
-    exe = os.path.join(build_dir, "masked_schedule_test")
-    cmd = [NVCC, "-std=c++17", "-O1", "--expt-relaxed-constexpr", "-gencode", "arch=compute_90a,code=sm_90a", "-o", exe,
-           os.path.join(ROOT, "tests", "cpp", "masked_schedule_test.cu")]
-    res = subprocess.run(cmd, capture_output=True, text=True)
-    assert res.returncode == 0, res.stdout + res.stderr
-    return exe
-
-
 @pytest.fixture(scope="module")
 def schedule_exe(tmp_path_factory):
-    # built outside the source tree, which need not be writable
-    return _schedule_exe(str(tmp_path_factory.mktemp("cpp")))
+    return cpp_build.build("masked_schedule_test.cu", str(tmp_path_factory.mktemp("cpp") / "masked_schedule_test"),
+                           standalone=True)
 
 
 def _classify(exe, adj, gidx, m, n):
@@ -152,10 +140,4 @@ def test_skip_schedule_replay(schedule_exe):
 
 
 def test_masked_shim_compiles_and_links(tmp_path):
-    _build.build()
-    exe = str(tmp_path / "masked_nn_test")
-    cmd = [NVCC, "-std=c++17", "-O1", "-I", os.path.join(ROOT, "include"), "-o", exe,
-           os.path.join(ROOT, "tests", "cpp", "masked_nn_test.cu"), "-L", os.path.dirname(_build.SO_PATH),
-           "-lraft_b200", "-Xlinker", "-rpath", "-Xlinker", os.path.dirname(_build.SO_PATH)]
-    res = subprocess.run(cmd, capture_output=True, text=True)
-    assert res.returncode == 0, res.stdout + res.stderr
+    assert os.path.exists(cpp_build.build("masked_nn_test.cu", str(tmp_path / "masked_nn_test")))

@@ -245,18 +245,8 @@ def test_none_runs_for_one_slab_followed_by_live_tiles(k):
 def test_cpp_shim_on_gpu(tmp_path):
     """raft::distance::masked_l2_nn with MinAndDistanceReduceOp (KVP out), MinReduceOp (float out, sqrt) and
     initOutBuffer = false, against a host brute force (tests/cpp/masked_nn_test.cu)."""
-    import os
-    import shutil
     import subprocess
-    from raft_b200 import _build
-    root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-    exe = str(tmp_path / "masked_nn_test")   # built outside the source tree, which need not be writable
-    nvcc = shutil.which("nvcc") or "/usr/local/cuda/bin/nvcc"
-    _build.build()
-    res = subprocess.run([nvcc, "-std=c++17", "-O1", "-I", os.path.join(root, "include"), "-o", exe,
-                          os.path.join(root, "tests", "cpp", "masked_nn_test.cu"), "-L", os.path.dirname(_build.SO_PATH),
-                          "-lraft_b200", "-Xlinker", "-rpath", "-Xlinker", os.path.dirname(_build.SO_PATH)],
-                         capture_output=True, text=True)
-    assert res.returncode == 0, res.stdout + res.stderr
+    import cpp_build
+    exe = cpp_build.build("masked_nn_test.cu", str(tmp_path / "masked_nn_test"))
     res = subprocess.run([exe], capture_output=True, text=True, timeout=120)
     assert res.returncode == 0 and "PASS" in res.stdout, res.stdout + res.stderr

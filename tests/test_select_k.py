@@ -1,18 +1,16 @@
 """select_k without a GPU: the ABI's workspace query and argument checks, the key transform compiled for the host
 against the numpy oracle, the oracle itself, and the C++ shim's compile (its run is marked gpu)."""
 import os
-import shutil
 import subprocess
 
 import numpy as np
 import pytest
 
+import cpp_build
 from oracle.select_k import select_k as ref_select_k
 from oracle.select_k import select_key
-from raft_b200 import _build, _lib
+from raft_b200 import _lib
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-NVCC = shutil.which("nvcc") or "/usr/local/cuda/bin/nvcc"
 SIZE_MAX = 2 ** 64 - 1
 
 
@@ -54,11 +52,7 @@ SPECIAL = [0x00000000, 0x80000000, 0x00000001, 0x80000001, 0x007FFFFF, 0x807FFFF
 
 
 def test_key_transform_matches_oracle(build_dir):
-    exe = os.path.join(build_dir, "select_k_key_test")
-    cmd = [NVCC, "-std=c++17", "-O1", "--expt-relaxed-constexpr", "-gencode", "arch=compute_90a,code=sm_90a", "-o", exe,
-           os.path.join(ROOT, "tests", "cpp", "select_k_key_test.cu")]
-    res = subprocess.run(cmd, capture_output=True, text=True)
-    assert res.returncode == 0, res.stdout + res.stderr
+    exe = cpp_build.build("select_k_key_test.cu", os.path.join(build_dir, "select_k_key_test"), standalone=True)
     bits = np.concatenate([np.array(SPECIAL, dtype=np.uint32),
                            np.random.default_rng(5).integers(0, 2 ** 32, 20000, dtype=np.uint64).astype(np.uint32)])
     res = subprocess.run([exe], input="\n".join("%08x" % b for b in bits), capture_output=True, text=True, timeout=60)
@@ -87,15 +81,8 @@ def test_oracle_order():
 
 
 def compile_shim(build_dir, mock_raft):
-    _build.build()
     exe = os.path.join(build_dir, "select_k_shim_mockraft" if mock_raft else "select_k_shim")
-    extra = ["-DRAFT_B200_USE_REAL_RAFT", "-I", os.path.join(ROOT, "tests", "cpp", "mock_raft")] if mock_raft else []
-    cmd = [NVCC, "-std=c++17", "-O1", "-I", os.path.join(ROOT, "include")] + extra + [
-           "-o", exe, os.path.join(ROOT, "tests", "cpp", "select_k_shim_test.cu"), "-L", os.path.dirname(_build.SO_PATH),
-           "-lraft_b200", "-Xlinker", "-rpath", "-Xlinker", os.path.dirname(_build.SO_PATH)]
-    res = subprocess.run(cmd, capture_output=True, text=True)
-    assert res.returncode == 0, res.stdout + res.stderr
-    return exe
+    return cpp_build.build("select_k_shim_test.cu", exe, mock_raft)
 
 
 @pytest.mark.parametrize("mock_raft", [False, True])

@@ -2,16 +2,13 @@
 mock raft headers on the CPU tier; on the GPU its dendrogram, labels and merge distances equal the Python call's bit for
 bit."""
 import os
-import shutil
 import subprocess
 
 import numpy as np
 import pytest
 
-from raft_b200 import _build
+import cpp_build
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-NVCC = shutil.which("nvcc") or "/usr/local/cuda/bin/nvcc"
 
 
 @pytest.fixture(scope="module")
@@ -20,15 +17,8 @@ def build_dir(tmp_path_factory):
 
 
 def compile_shim(build_dir, mock_raft):
-    _build.build()
     exe = os.path.join(build_dir, "sl_shim_mockraft" if mock_raft else "sl_shim")
-    extra = ["-DRAFT_B200_USE_REAL_RAFT", "-I", os.path.join(ROOT, "tests", "cpp", "mock_raft")] if mock_raft else []
-    cmd = [NVCC, "-std=c++17", "-O1", "-I", os.path.join(ROOT, "include")] + extra + [
-           "-o", exe, os.path.join(ROOT, "tests", "cpp", "single_linkage_shim_test.cu"), "-L",
-           os.path.dirname(_build.SO_PATH), "-lraft_b200", "-Xlinker", "-rpath", "-Xlinker", os.path.dirname(_build.SO_PATH)]
-    res = subprocess.run(cmd, capture_output=True, text=True)
-    assert res.returncode == 0, res.stdout + res.stderr
-    return exe
+    return cpp_build.build("single_linkage_shim_test.cu", exe, mock_raft)
 
 
 @pytest.mark.parametrize("mock_raft", [False, True])
