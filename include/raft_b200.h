@@ -368,6 +368,32 @@ int b2d_single_linkage(void* stream, int metric, const float* x, int64_t ldx, in
                        int32_t* children, float* deltas, int32_t* sizes, int32_t* labels, int32_t* n_components_out,
                        void* workspace, size_t workspace_bytes);
 
+/* DBSCAN (cuML's DBSCAN(eps, min_samples, metric, max_mbytes_per_batch), sklearn.cluster.DBSCAN's labels_ and
+ * core_sample_indices_) for fp32 x:[m,d] (row-major, pitch ldx), on the epsilon neighbourhood of b2d_eps_neighbors_l2sq.
+ * A is the m x m matrix one call b2d_eps_neighbors_l2sq(x, x, e) returns, bit for bit, for metric
+ *   B2D_L2SqrtExpanded  squared L2 distance <= e = fp32(eps^2), eps^2 formed in fp64
+ *   B2D_L2Expanded      squared L2 distance <= e = fp32(eps)
+ *   B2D_CosineExpanded  the distance of b2d_pairwise_distance(CosineExpanded) <= e = fp32(eps)
+ * with d(i, i) = 0 (every row is its own neighbour for eps >= 0); a NaN distance, a NaN or negative eps match nothing.
+ * deg(j) = #{i : A[i, j]}; j is core iff deg(j) >= min_samples.  Core i and j are linked iff A[i, j] or A[j, i]; clusters
+ * are the connected components of the core rows, numbered 0, 1, ... in order of their smallest row.  A non-core row b
+ * takes the smallest cluster number of the core rows c with A[b, c], or -1 (noise).  When A is symmetric this is
+ * sklearn.cluster.DBSCAN's result exactly.  Outputs (device pointers): labels [m]; core_sample_indices [m] (optional)
+ * the core rows ascending, then -1 up to m; *n_clusters (optional, int32).
+ * A is formed in batches of b = min(m, max(256, floor(max_bytes_per_batch / m / 256) * 256)) columns (0 means 2^30
+ * bytes) of the once-prepared x, in three passes (degrees; links; border), or once when b = m.  The results do not
+ * depend on the batch size, the device or the scheduling: the only atomics are an integer CAS and atomicMin.
+ * Precondition: x finite (a non-finite x is safe, its labels are unspecified).  metric outside the three above and
+ * d > 320 are B2D_ERR_UNSUPPORTED; m >= 2^31, d < 1, min_samples < 1, ldx < d, a negative max_bytes_per_batch and a null
+ * x / labels are B2D_ERR_INVALID_ARG; m == 0 does nothing.  Only enqueues work (no synchronisation, no allocation), so
+ * the call can be captured in a CUDA graph.  The workspace depends on (m, d, max_bytes_per_batch) only; the query returns
+ * SIZE_MAX for negative arguments. */
+size_t b2d_dbscan_workspace_bytes(int64_t m, int64_t d, int64_t max_bytes_per_batch);
+int b2d_dbscan_fit(void* stream, int metric, const float* x, int64_t ldx, int64_t m, int64_t d, double eps,
+                   int64_t min_samples, int64_t max_bytes_per_batch, int32_t* labels /* [m] */,
+                   int32_t* core_sample_indices /* [m] or NULL */, int32_t* n_clusters /* device, or NULL */,
+                   void* workspace, size_t workspace_bytes);
+
 #ifdef __cplusplus
 }
 #endif
