@@ -199,7 +199,8 @@ int b2d_knn_l2(void* stream, int64_t* out_idx, float* out_dist, const float* x, 
  * b2d_pairwise_distance (the reference's default is L2Unexpanded).  The n x n matrix is produced and
  * consumed in [chunk_rows x n] slabs (0 = about 1 GiB per slab), like the reference's batched variant
  * (detail/batched/silhouette_score.cuh:213-243).  Never synchronises: labels are validated on the device, a label
- * outside [0, n_labels) makes *score (and the per-sample value of that row) NaN. */
+ * outside [0, n_labels) makes *score (and the per-sample value of that row) NaN, and so do labels that leave fewer
+ * than two non-empty clusters (*score only). */
 size_t b2d_silhouette_score_workspace_bytes(int64_t n, int64_t k, int n_labels, int metric, int64_t chunk_rows);
 int b2d_silhouette_score(void* stream, float* score, float* per_sample, const float* x, int64_t ldx,
                          const int* labels, int64_t n, int64_t k, int n_labels, int metric, float metric_arg,
@@ -209,8 +210,9 @@ int b2d_silhouette_score(void* stream, float* score, float* per_sample, const fl
  * other dangling caller (SURVEY.md 8(f3)): x [n, m] original space, x_embedded [n, d]; neighbours in the
  * embedded space from the fused kNN and ranks in the original space both under `metric` (the reference's
  * distance_type template parameter; L2 / L2Sqrt (Expanded or Unexpanded), CosineExpanded, CorrelationExpanded),
- * ranks counted over [batch_rows x n] slabs (0 = about 1 GiB).  *score is a DEVICE double; the call never
- * synchronises.  n_neighbors <= 63. */
+ * ranks counted over [batch_rows x n] slabs (0 = about 1 GiB).  Every sample has exactly n_neighbors embedded
+ * neighbours: itself excluded, ties by index.  *score is a DEVICE double; the call never synchronises.
+ * n_neighbors <= 63. */
 size_t b2d_trustworthiness_score_workspace_bytes(int64_t n, int64_t m, int64_t d, int n_neighbors, int metric,
                                                  int64_t batch_rows);
 int b2d_trustworthiness_score(void* stream, double* score, const float* x, int64_t ldx,

@@ -270,31 +270,28 @@ def silhouette_score(x, labels, n_labels=None, metric=None, metric_arg=2.0, retu
 
 def trustworthiness_score(x, x_embedded, n_neighbors: int = 5, metric=None):
     """Restates raft::stats::trustworthiness_score (cpp/include/raft/stats/detail/
-    trustworthiness_score.cuh:113-211): neighbours j of i in the embedded space (n_neighbors + 1 with i
-    itself, in the caller's metric), r(i, j) = position of j in the order of the samples by original-space distance
-    from i (i first; ties by index), penalty max(0, r - n_neighbors).  Same value as
-    sklearn.manifold.trustworthiness."""
+    trustworthiness_score.cuh:113-211): the n_neighbors nearest samples j of i in the embedded space (in the caller's
+    metric; i itself excluded, ties by index), r(i, j) = position of j in the order of the samples by original-space
+    distance from i (i first; ties by index), penalty max(0, r - n_neighbors).  Every sample contributes exactly
+    n_neighbors neighbours, also when n_neighbors or more other samples coincide with it in the embedding.  Same value
+    as sklearn.manifold.trustworthiness wherever the embedded neighbour set has no ties at its boundary."""
     metric = DistanceType.L2SqrtUnexpanded if metric is None else metric
     x = np.asarray(x, dtype=np.float64)
     e = np.asarray(x_embedded, dtype=np.float64)
     n, k = x.shape[0], int(n_neighbors)
+    idx = np.broadcast_to(np.arange(n), (n, n))
     d = pairwise_distance(x, x, metric, 2.0)
     np.fill_diagonal(d, -np.inf)                                   # the sample itself comes first
-    order = np.lexsort((np.broadcast_to(np.arange(n), d.shape), d), axis=1)
+    order = np.lexsort((idx, d), axis=1)
     rank = np.empty_like(order)
-    np.put_along_axis(rank, order, np.broadcast_to(np.arange(n), d.shape), axis=1)
-    if metric in (DistanceType.L2SqrtUnexpanded, DistanceType.L2Unexpanded, DistanceType.L2Expanded,
-                  DistanceType.L2SqrtExpanded):
-        nbr, _ = knn_l2(e, e, k + 1)
-    else:   # run_knn<distance_type> (trustworthiness_score.cuh:79-104): the SAME metric in the embedded space
-        de = pairwise_distance(e, e, metric, 2.0)
-        np.fill_diagonal(de, -np.inf)
-        nbr = np.lexsort((np.broadcast_to(np.arange(n), de.shape), de), axis=1)[:, :k + 1]
-    t = 0.0
-    for i in range(n):
-        for j in nbr[i]:
-            if j != i:
-                t += max(0, int(rank[i, j]) - k)
+    np.put_along_axis(rank, order, idx, axis=1)
+    # run_knn<distance_type> (trustworthiness_score.cuh:79-104): the SAME metric in the embedded space; every L2 form
+    # orders like the squared distance, which no square root can merge
+    l2 = (DistanceType.L2SqrtUnexpanded, DistanceType.L2Unexpanded, DistanceType.L2Expanded, DistanceType.L2SqrtExpanded)
+    de = pairwise_distance(e, e, DistanceType.L2Expanded if metric in l2 else metric, 2.0)
+    np.fill_diagonal(de, np.inf)                                   # never its own neighbour
+    nbr = np.lexsort((idx, de), axis=1)[:, :k]
+    t = float(np.maximum(np.take_along_axis(rank, nbr, axis=1) - k, 0).sum())
     return 1.0 - (2.0 / ((n * k) * ((2.0 * n) - (3.0 * k) - 1.0))) * t
 
 

@@ -1485,7 +1485,7 @@ int b2d_silhouette_score(void* stream, float* score, float* per_sample, const fl
       L.slab, L.sl.ld, r0, rows, labels, L.counts, L.offsets, L.where, n_labels, per_sample, L.total);
     B2D_CUDA(cudaGetLastError());
   }
-  sil_finish_kernel<<<1, 32, 0, s>>>(L.total, score, n, L.bad);
+  sil_finish_kernel<<<1, 32, 0, s>>>(L.total, score, n, L.bad, L.counts, n_labels);
   B2D_CUDA(cudaGetLastError());
   return B2D_OK;
 }

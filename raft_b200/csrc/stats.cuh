@@ -93,17 +93,23 @@ __global__ void __launch_bounds__(256) sil_row_kernel(const float* slab, int64_t
 }
 
 // labels outside [0, n_labels) were flagged by sil_count_kernel: the score is NaN then (device-side validation,
-// the call never synchronises)
-__global__ void sil_finish_kernel(const double* total, float* score, int64_t n, const unsigned* bad)
+// the call never synchronises).  So it is when fewer than two clusters are non-empty: every b is FLT_MAX there and
+// s ~ 1 would score a clustering that is not one.
+__global__ void sil_finish_kernel(const double* total, float* score, int64_t n, const unsigned* bad, const int* counts,
+                                  int n_labels)
 {
-  if (threadIdx.x == 0 && blockIdx.x == 0)
-    *score = *bad ? __int_as_float(0x7fc00000) : static_cast<float>(*total / static_cast<double>(n));
+  if (threadIdx.x == 0 && blockIdx.x == 0) {
+    int present = 0;
+    for (int l = 0; l < n_labels; ++l) present += counts[l] > 0;
+    *score = *bad || present < 2 ? __int_as_float(0x7fc00000) : static_cast<float>(*total / static_cast<double>(n));
+  }
 }
 
 // ---------------------------------------------------------------------------------------------
 // Trustworthiness (raft::stats::trustworthiness_score, cpp/include/raft/stats/detail/
-// trustworthiness_score.cuh:113-211): for every sample i and each of its n_neighbors + 1 nearest
-// neighbours j in the EMBEDDED space, r(i, j) = position of j when the samples are ordered by their
+// trustworthiness_score.cuh:113-211): for every sample i and each of its n_neighbors nearest
+// neighbours j != i in the EMBEDDED space (from a kNN list of n_neighbors + 1 that normally holds i itself),
+// r(i, j) = position of j when the samples are ordered by their
 // ORIGINAL-space distance from i (i itself first), penalty max(0, r - n_neighbors);
 // score = 1 - 2 / (n k (2n - 3k - 1)) * sum of the penalties.  The reference sorts every row of the
 // original-space distance matrix (sort_cols_per_row + a lookup table); only k + 1 ranks per row are
@@ -134,6 +140,12 @@ __global__ void __launch_bounds__(256) trust_rank_kernel(const float* slab, int6
   }
   __syncthreads();
   if (threadIdx.x == 0) {
+    // exactly n_neighbors neighbours per sample: the list is ascending by (distance, index) (knn_finalize_kernel), so a
+    // sample missing from its own list (n_neighbors + 1 coincident rows of smaller index, or a rounded d(i, i) > 0
+    // above a neighbour's distance) drops the last entry, the farthest
+    bool self = false;
+    for (int q = 0; q < kk1; ++q) self |= emb_idx[row * kk1 + q] == row;
+    if (!self) { thr[kk1 - 1] = __int_as_float(0xff800000); nbr[kk1 - 1] = -1; }
     float tm = __int_as_float(0xff800000);
     for (int q = 0; q < kk1; ++q) tm = fmaxf(tm, thr[q]);
     tmax_s = tm;

@@ -50,6 +50,8 @@ def silhouette_score(X, labels, n_labels=None, metric="sqeuclidean_unexpanded", 
         lt = torch.as_tensor(labels, device=handle.device)
         if int(lt.min().item()) < 0 or int(lt.max().item()) >= int(n_labels):
             raise _lib.LogicError("labels must lie in [0, n_labels)")
+        if int(torch.unique(lt).numel()) < 2:
+            raise _lib.LogicError("silhouette score is not defined for fewer than 2 non-empty clusters")
     return (val, per) if return_samples else val
 
 

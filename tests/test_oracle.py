@@ -180,3 +180,60 @@ def test_trustworthiness_oracle_pinned_to_sklearn():
         for k in (3, 7):
             assert abs(oracle.trustworthiness_score(x, emb, k) - skm.trustworthiness(x, emb, n_neighbors=k)) < 1e-12
     assert oracle.trustworthiness_score(x, x, 5) == 1.0
+    # embeddings of coincident groups of exactly k + 1 points: a sample's k neighbours are its k group mates whichever
+    # tied mate a kNN lists first, so sklearn's neighbour sets are the oracle's
+    for k in (1, 4, 9):
+        groups = np.repeat(rng.standard_normal((180 // (k + 1), 2)), k + 1, axis=0)
+        emb = groups[rng.permutation(len(groups))]
+        xs = x[: len(emb)]
+        got = oracle.trustworthiness_score(xs, emb, k)
+        assert abs(got - skm.trustworthiness(xs, emb, n_neighbors=k)) < 1e-12, k
+        assert got < 0.9                                    # the embedding is not trustworthy: the check has teeth
+
+
+def _trustworthiness_by_definition(x, e, k):
+    """Trustworthiness by its definition with plain Python sorts: the k samples nearest to i in the embedding (i
+    excluded, ties to the smaller index), each ranked among all samples ordered by (original-space distance, index)
+    with i itself first."""
+    n = len(x)
+    dx = ((x[:, None, :] - x[None, :, :]) ** 2).sum(-1)
+    de = ((e[:, None, :] - e[None, :, :]) ** 2).sum(-1)
+    t = 0
+    for i in range(n):
+        nbrs = [j for _, j in sorted((de[i, j], j) for j in range(n) if j != i)[:k]]
+        order = [i] + [j for _, j in sorted((dx[i, j], j) for j in range(n) if j != i)]
+        pos = {j: r for r, j in enumerate(order)}
+        t += sum(max(0, pos[j] - k) for j in nbrs)
+    return 1.0 - 2.0 / (n * k * (2.0 * n - 3.0 * k - 1.0)) * t
+
+
+@pytest.mark.parametrize("group", [2, 3, 5, 8])
+def test_trustworthiness_oracle_counts_exactly_k_neighbours(group):
+    """Coincident groups in the embedding, larger than k + 1 for most k here, and duplicate rows in the original space:
+    a sample with k + 1 or more coincident mates of smaller index is not in its own (k + 1)-nearest list, and counting
+    the whole list would give it k + 1 neighbours.  Integer coordinates: every distance is exact, so the ties are
+    real ties and the tie rule decides."""
+    rng = np.random.default_rng(20 + group)
+    n = 120
+    e = np.repeat(rng.integers(-6, 7, (n // group, 2)), group, axis=0)[rng.permutation(n)].astype(np.float64)
+    x = rng.integers(-4, 5, (n, 5)).astype(np.float64)
+    x[10:14] = x[3]                                          # duplicate rows in the original space too
+    for k in (1, group - 1, group, group + 1):
+        if k < 1:
+            continue
+        want = _trustworthiness_by_definition(x, e, k)
+        assert 0.0 <= want <= 1.0                            # k neighbours per row: the normalisation holds
+        for metric in (DT.L2SqrtUnexpanded, DT.L2Unexpanded, DT.L2Expanded, DT.L2SqrtExpanded):
+            assert abs(oracle.trustworthiness_score(x, e, k, metric=metric) - want) < 1e-12, (k, metric)
+
+
+def test_silhouette_oracle_is_nan_for_one_non_empty_cluster():
+    """sklearn raises 'Number of labels is 1'; the restatement returns NaN (the C ABI's answer), whatever n_labels is
+    declared."""
+    rng = np.random.default_rng(9)
+    x = rng.standard_normal((50, 4))
+    with np.errstate(invalid="ignore"):
+        for labels, nl in ((np.zeros(50, int), 3), (np.full(50, 2), None), (np.full(50, 1), 2)):
+            assert np.isnan(oracle.silhouette_score(x, labels, nl))
+        x[:] = x[0]                                           # one cluster of identical points
+        assert np.isnan(oracle.silhouette_score(x, np.zeros(50, int), 2))
