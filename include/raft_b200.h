@@ -112,6 +112,23 @@ int b2d_pairwise_distance(void* stream, int metric, int dtype, const void* x, in
                           int64_t n, int64_t k, int row_major, float metric_arg, void* workspace,
                           size_t workspace_bytes);
 
+/* Diagnostic, host arithmetic only (no device, nothing is dereferenced): the kernels b2d_pairwise_distance would run for
+ * these arguments, which it also validates in the same way.  x, y and dist matter through their alignment.  out:
+ *   [0] path (B2D_PLAN_*)
+ *   [1] tensor path: 1 if the tiles leave through TMA stores, 0 from registers
+ *   [2] tensor path, register stores: 1 if tiles wholly inside dist go out as 8-byte vectors, 0 all scalar
+ *   [3], [4] fp32 unexpanded kernels: 16-byte loads of the kernel's first / second operand (in Fortran order the
+ *            first operand is y)
+ *   [5] number of launches L of the main kernel (the tensor path accumulates K in chunks when k > 320)
+ *   [6 + 4 i ...] launch i < L, as far as out_len allows: first k-block (32 columns each), k-blocks, accumulation
+ *            mode (0 single pass, 1 first chunk: store, 2 middle: add, 3 last: add and finish), 1 if the resident
+ *            kernel (<= 4 k-blocks) runs it, 0 the streaming one
+ * out_len >= 6. */
+enum { B2D_PLAN_NONE = 0, B2D_PLAN_TENSOR = 1, B2D_PLAN_F32_SIMT = 2, B2D_PLAN_F32_TMA = 3, B2D_PLAN_F64_SIMT = 4 };
+int b2d_debug_pairwise_plan(int metric, int dtype, const void* x, int64_t ldx, const void* y, int64_t ldy,
+                            const void* dist, int64_t ldd, int64_t m, int64_t n, int64_t k, int row_major, int* out,
+                            int out_len);
+
 size_t b2d_fused_l2_nn_workspace_bytes(int64_t m, int64_t n, int64_t k);
 
 /* out[i] = {argmin_j, min_j} ||x_i - y_j||^2 (sqrt != 0: of the Euclidean distance); ties go to

@@ -20,6 +20,7 @@ SYMBOLS = [
     "b2d_gram_matrix_workspace_bytes", "b2d_gram_matrix", "b2d_kmeans_workspace_bytes", "b2d_kmeans_fit",
     "b2d_kmeans_predict", "b2d_kmeans_update_centroids", "b2d_kmeans_init_plus_plus", "b2d_mst_workspace_bytes", "b2d_mst",
     "b2d_single_linkage_workspace_bytes", "b2d_single_linkage", "b2d_dbscan_workspace_bytes", "b2d_dbscan_fit",
+    "b2d_debug_pairwise_plan",
 ]
 
 B2D_OK, B2D_ERR_INVALID_ARG, B2D_ERR_CUDA, B2D_ERR_UNSUPPORTED, B2D_ERR_WORKSPACE = range(5)
@@ -61,6 +62,8 @@ def lib() -> ctypes.CDLL:
     L.b2d_pairwise_workspace_bytes.argtypes = [ci, ci, i64, i64, i64]
     L.b2d_pairwise_distance.restype = ci
     L.b2d_pairwise_distance.argtypes = [vp, ci, ci, vp, i64, vp, i64, vp, i64, i64, i64, i64, ci, cf, vp, sz]
+    L.b2d_debug_pairwise_plan.restype = ci
+    L.b2d_debug_pairwise_plan.argtypes = [ci, ci, vp, i64, vp, i64, vp, i64, i64, i64, i64, ci, vp, ci]
     L.b2d_fused_l2_nn_workspace_bytes.restype = sz
     L.b2d_fused_l2_nn_workspace_bytes.argtypes = [i64, i64, i64]
     L.b2d_fused_l2_nn.restype = ci

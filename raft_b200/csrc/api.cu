@@ -16,6 +16,7 @@
 
 #include "../../include/raft_b200.h"
 #include "expanded_tc.cuh"
+#include "dispatch_plan.cuh"
 #include "masked_nn.cuh"
 #include "screen_tc.cuh"
 #include "prep.cuh"
@@ -364,7 +365,7 @@ static int launch_tc(cudaStream_t s, const TcWorkspace& w, TcParams p, int64_t k
   p.ysc      = w.ysc;
   p.nonuni   = w.nonuni;
   if (p.n_items == 0) return B2D_OK;
-  const bool resident = p.nkb <= TC_MAX_RES_KB;
+  const bool resident = tc_resident(p.nkb);
   CUtensorMap ma, mb;
   // resident: each consumer warpgroup's ring takes the 64-row slab of an x tile it multiplies; streaming: whole tiles
   rc = make_operand_map(&ma, w.xop, p.m, p.nkb, resident ? TC_BM / 2 : TC_BM, kb0, nkb_total);
@@ -423,9 +424,9 @@ static int launch_screen(cudaStream_t s, const TcWorkspace& w, int64_t m, int64_
 }
 
 template <int kMetric>
-static int launch_ux_inst(cudaStream_t s, const UxParams& p, int64_t tiles)
+static int launch_ux_inst(cudaStream_t s, const UxParams& p, int64_t tiles, bool tma)
 {
-  if (p.vec_x && p.vec_y) {  // TMA-legal operands: hardware-staged tiles of 32 floats x 128 rows, SWIZZLE_128B
+  if (tma) {  // TMA-legal operands: hardware-staged tiles of 32 floats x 128 rows, SWIZZLE_128B
     CUtensorMap mx, my;
     int rc = encode_2d(&mx, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, p.x, p.k, p.m, p.xrs * 4, UX_KB, UX_BM,
                        CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, "(f32 operand)");
@@ -743,31 +744,17 @@ static int tc_store(cudaStream_t s, const TcStore& c, int dtype, const void* xa,
   p.m = ma; p.n = na; p.dist = dist; p.ldd = ldd;
   p.diag_zero = (c.post != POST_NONE && alias && c.mode == PREP_L2) ? 1 : 0;
   p.gamma = c.gamma; p.coef0 = c.coef0; p.degree = c.degree;
-  // the result leaves through shared-memory staging and TMA stores wherever TMA can address dist: 16-byte aligned
-  // base and pitch, row and column coordinates within int32 (the store takes 32-bit coordinates), and rows that end
-  // on a 16-byte boundary.  The last condition is from observation: on an H100, with n = 150 and ldd = 160, the
-  // box stores also wrote columns 150 and 151, i.e. the partial 16 bytes at the end of each row, into the caller's
-  // padding (tests/test_pairwise_gpu.py::test_padded_leading_dimensions_and_out_param).  Otherwise, and for the
-  // read-modify-write K chunks below, the epilogue stores from registers.
-  p.tma_store = (reinterpret_cast<uintptr_t>(dist) % 16 == 0 && ldd % 4 == 0 && na % 4 == 0 && ma <= 0x7fffffffll &&
-                 na <= 0x7fffffffll) ? 1 : 0;
-  // k > 320: accumulate K in chunks of 256 columns, each added to dist with a round-to-nearest fp32
-  // add -- bounds the truncation bias of long MMA chains (DESIGN.md, numerics).  The post-processing (clamp, sqrt, the
-  // Gram transforms) runs on the last chunk only.
-  const int nkb_total = static_cast<int>((k + 31) / 32);
-  constexpr int kChunk = 8;
+  // (dispatch_plan.cuh: TMA or register stores; k > 320: K chunks accumulated in dist, post-processed on the last)
+  const TcStorePlan pl = tc_store_plan(c.post, ma, na, k, reinterpret_cast<uintptr_t>(dist), ldd);
+  p.tma_store = pl.tma_store;
   ProfileScope prof(s);  // the main kernel(s) only: the operand preparation above is outside
-  if (nkb_total > 10 && !tc_post_ratio(c.post)) {  // (the ratio metrics need the whole inner product at once)
-    p.tma_store = 0;
-    for (int kb0 = 0; kb0 < nkb_total; kb0 += kChunk) {
-      const int nk = nkb_total - kb0 < kChunk ? nkb_total - kb0 : kChunk;
-      p.acc_mode   = kb0 == 0 ? 1 : (kb0 + nk >= nkb_total ? 3 : 2);
-      rc           = launch_tc(s, w, p, k, EPI_STORE, c.post, kb0, nk);
-      if (rc) return rc;
-    }
-    return B2D_OK;
+  for (int i = 0; i < pl.launches; ++i) {
+    const TcStoreLaunch l = tc_store_launch(pl, i);
+    p.acc_mode = l.acc_mode;
+    rc = launch_tc(s, w, p, k, EPI_STORE, c.post, l.kb0, l.nkb);
+    if (rc) return rc;
   }
-  return launch_tc(s, w, p, k, EPI_STORE, c.post);
+  return B2D_OK;
 }
 
 size_t b2d_pairwise_workspace_bytes(int metric, int dtype, int64_t m, int64_t n, int64_t k)
@@ -781,14 +768,13 @@ size_t b2d_pairwise_workspace_bytes(int metric, int dtype, int64_t m, int64_t n,
   return tc_layout(nullptr, m, n, k, false).bytes;
 }
 
-int b2d_pairwise_distance(void* stream, int metric, int dtype, const void* x, int64_t ldx, const void* y,
-                          int64_t ldy, void* dist_v, int64_t ldd, int64_t m, int64_t n, int64_t k,
-                          int row_major, float metric_arg, void* workspace, size_t workspace_bytes)
+// The argument checks of b2d_pairwise_distance.  *empty: nothing to compute (m or n is 0).
+static int pairwise_check(int metric, int dtype, const void* x, int64_t ldx, const void* y, int64_t ldy, const void* dist,
+                          int64_t ldd, int64_t m, int64_t n, int64_t k, int row_major, float metric_arg, bool* empty)
 {
-  float* dist = static_cast<float*>(dist_v);
-  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  *empty = false;
   if (m < 0 || n < 0 || k < 0) return fail(B2D_ERR_INVALID_ARG, "negative extent");
-  if (m == 0 || n == 0) return B2D_OK;
+  if (m == 0 || n == 0) { *empty = true; return B2D_OK; }
   if (k == 0) return fail(B2D_ERR_INVALID_ARG, "k must be positive");
   if (!x || !y || !dist) return fail(B2D_ERR_INVALID_ARG, "null x / y / dist");
   if (m > 0x7fffffffll * 128 || n > 0x7fffffffll || k > (1 << 24)) return fail(B2D_ERR_INVALID_ARG, "extent too large");
@@ -801,6 +787,75 @@ int b2d_pairwise_distance(void* stream, int metric, int dtype, const void* x, in
     return fail(B2D_ERR_UNSUPPORTED, "metric " + std::to_string(metric) + " is not on the tensor-core / SIMT distance path");
   if (dtype != B2D_F32 && dtype != B2D_F16 && dtype != B2D_F64) return fail(B2D_ERR_UNSUPPORTED, "dtype");
   if (metric == B2D_LpUnexpanded && !(metric_arg > 0.f)) return fail(B2D_ERR_INVALID_ARG, "LpUnexpanded needs p > 0");
+  if (dtype == B2D_F16 && !is_expanded(metric)) return fail(B2D_ERR_UNSUPPORTED, "unexpanded metrics take fp32 inputs");
+  return B2D_OK;
+}
+
+// The operands as the fp32 / fp16 kernels take them: dist is always written as a row-major [ma][ldd] matrix.
+// Fortran order: D^T (row-major [n,m]) = metric(y_j, x_i).  Every metric here is symmetric except
+// KLDivergence, which switches to the kernel with the operand roles exchanged (UX_KL_REV).
+struct PairwiseOperands {
+  const void *xa, *ya;
+  int64_t ma, na, xrs, xcs, yrs, ycs;
+};
+static PairwiseOperands pairwise_operands(const void* x, int64_t ldx, const void* y, int64_t ldy, int64_t m, int64_t n,
+                                          int row_major)
+{
+  if (row_major) return PairwiseOperands{x, y, m, n, ldx, 1, ldy, 1};
+  return PairwiseOperands{y, x, n, m, 1, ldy, 1, ldx};
+}
+
+// preparation and epilogue of the expanded metrics on the tensor path
+static TcStore pairwise_tc_store(int metric, int64_t k)
+{
+  TcStore c;
+  if (metric == B2D_L2Expanded) { c.post = POST_CLAMP; }
+  else if (metric == B2D_L2SqrtExpanded) { c.post = POST_CLAMP_SQRT; }
+  else if (metric == B2D_CosineExpanded) { c.mode = PREP_COSINE; }
+  else if (metric == B2D_CorrelationExpanded) { c.mode = PREP_COSINE; c.center = 1; }
+  else if (metric == B2D_HellingerExpanded) { c.mode = PREP_INNER; c.post = POST_CLAMP_SQRT; c.xform = 1; c.coef_mul = -1.f; c.tx_const = 1.f; }
+  else if (metric == B2D_RusselRaoExpanded) { c.mode = PREP_INNER; c.coef_mul = -1.f / static_cast<float>(k); c.tx_const = 1.f; }
+  else if (metric == B2D_JaccardExpanded) { c.mode = PREP_INNER_NORM; c.post = POST_JACCARD; }
+  else if (metric == B2D_DiceExpanded) { c.mode = PREP_INNER_NORM; c.post = POST_DICE; }
+  else { c.mode = PREP_INNER; }
+  return c;
+}
+
+int b2d_debug_pairwise_plan(int metric, int dtype, const void* x, int64_t ldx, const void* y, int64_t ldy, const void* dist,
+                            int64_t ldd, int64_t m, int64_t n, int64_t k, int row_major, int* out, int out_len)
+{
+  if (!out || out_len < 6) return fail(B2D_ERR_INVALID_ARG, "out must hold at least 6 words");
+  bool empty = false;
+  const int rc = pairwise_check(metric, dtype, x, ldx, y, ldy, dist, ldd, m, n, k, row_major, 2.0f, &empty);
+  if (rc) return rc;
+  for (int i = 0; i < out_len; ++i) out[i] = 0;
+  if (empty) { out[0] = B2D_PLAN_NONE; return B2D_OK; }
+  if (dtype == B2D_F64) { out[0] = B2D_PLAN_F64_SIMT; return B2D_OK; }
+  const PairwiseOperands o = pairwise_operands(x, ldx, y, ldy, m, n, row_major);
+  if (is_expanded(metric)) {
+    const TcStorePlan pl = tc_store_plan(pairwise_tc_store(metric, k).post, o.ma, o.na, k, reinterpret_cast<uintptr_t>(dist), ldd);
+    out[0] = B2D_PLAN_TENSOR; out[1] = pl.tma_store; out[2] = pl.vec2; out[5] = pl.launches;
+    for (int i = 0; i < pl.launches && 6 + 4 * i + 3 < out_len; ++i) {
+      const TcStoreLaunch l = tc_store_launch(pl, i);
+      out[6 + 4 * i] = l.kb0; out[7 + 4 * i] = l.nkb; out[8 + 4 * i] = l.acc_mode; out[9 + 4 * i] = l.resident;
+    }
+    return B2D_OK;
+  }
+  const UxPlan ux = ux_plan(o.xrs, o.xcs, reinterpret_cast<uintptr_t>(o.xa), o.yrs, o.ycs, reinterpret_cast<uintptr_t>(o.ya), k);
+  out[0] = ux.tma ? B2D_PLAN_F32_TMA : B2D_PLAN_F32_SIMT; out[3] = ux.vec_x; out[4] = ux.vec_y;
+  out[5] = 1;
+  return B2D_OK;
+}
+
+int b2d_pairwise_distance(void* stream, int metric, int dtype, const void* x, int64_t ldx, const void* y,
+                          int64_t ldy, void* dist_v, int64_t ldd, int64_t m, int64_t n, int64_t k,
+                          int row_major, float metric_arg, void* workspace, size_t workspace_bytes)
+{
+  float* dist = static_cast<float*>(dist_v);
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  bool empty = false;
+  int rc = pairwise_check(metric, dtype, x, ldx, y, ldy, dist_v, ldd, m, n, k, row_major, metric_arg, &empty);
+  if (rc || empty) return rc;
   if (dtype == B2D_F64) {   // double in / double out: the SIMT fp64 path, every metric
     if (row_major)
       return pairwise_f64(s, metric, static_cast<const double*>(x), ldx, 1, static_cast<const double*>(y), ldy, 1,
@@ -808,55 +863,35 @@ int b2d_pairwise_distance(void* stream, int metric, int dtype, const void* x, in
     return pairwise_f64(s, metric, static_cast<const double*>(y), 1, ldy, static_cast<const double*>(x), 1, ldx,
                         static_cast<double*>(dist_v), ldd, n, m, k, 1, metric_arg, workspace, workspace_bytes);
   }
+  const PairwiseOperands o = pairwise_operands(x, ldx, y, ldy, m, n, row_major);
+  if (is_expanded(metric))
+    return tc_store(s, pairwise_tc_store(metric, k), dtype, o.xa, o.xrs, o.xcs, o.ma, o.ya, o.yrs, o.ycs, o.na, k, dist, ldd,
+                    x == y && m == n && ldx == ldy, workspace, workspace_bytes);
 
-  // Fortran order: D^T (row-major [n,m]) = metric(y_j, x_i).  Every metric here is symmetric except
-  // KLDivergence, which switches to the kernel with the operand roles exchanged (UX_KL_REV).
-  const void *xa = x, *ya = y;
-  int64_t ma = m, na = n;
-  int64_t xrs, xcs, yrs, ycs;
-  if (row_major) { xrs = ldx; xcs = 1; yrs = ldy; ycs = 1; }
-  else { xa = y; ya = x; ma = n; na = m; xrs = 1; xcs = ldy; yrs = 1; ycs = ldx; }
-
-  if (is_expanded(metric)) {
-    TcStore c;
-    if (metric == B2D_L2Expanded) { c.post = POST_CLAMP; }
-    else if (metric == B2D_L2SqrtExpanded) { c.post = POST_CLAMP_SQRT; }
-    else if (metric == B2D_CosineExpanded) { c.mode = PREP_COSINE; }
-    else if (metric == B2D_CorrelationExpanded) { c.mode = PREP_COSINE; c.center = 1; }
-    else if (metric == B2D_HellingerExpanded) { c.mode = PREP_INNER; c.post = POST_CLAMP_SQRT; c.xform = 1; c.coef_mul = -1.f; c.tx_const = 1.f; }
-    else if (metric == B2D_RusselRaoExpanded) { c.mode = PREP_INNER; c.coef_mul = -1.f / static_cast<float>(k); c.tx_const = 1.f; }
-    else if (metric == B2D_JaccardExpanded) { c.mode = PREP_INNER_NORM; c.post = POST_JACCARD; }
-    else if (metric == B2D_DiceExpanded) { c.mode = PREP_INNER_NORM; c.post = POST_DICE; }
-    else { c.mode = PREP_INNER; }
-    return tc_store(s, c, dtype, xa, xrs, xcs, ma, ya, yrs, ycs, na, k, dist, ldd, x == y && m == n && ldx == ldy,
-                    workspace, workspace_bytes);
-  }
-
-  if (dtype != B2D_F32) return fail(B2D_ERR_UNSUPPORTED, "unexpanded metrics take fp32 inputs");
   UxParams p;
   memset(&p, 0, sizeof(p));
-  p.x = static_cast<const float*>(xa); p.y = static_cast<const float*>(ya); p.dist = dist;
-  p.xrs = xrs; p.xcs = xcs; p.yrs = yrs; p.ycs = ycs; p.ldd = ldd; p.m = ma; p.n = na; p.k = static_cast<int>(k);
-  p.vec_x = (xcs == 1 && xrs % 4 == 0 && k % 4 == 0 && reinterpret_cast<uintptr_t>(xa) % 16 == 0) ? 1 : 0;
-  p.vec_y = (ycs == 1 && yrs % 4 == 0 && k % 4 == 0 && reinterpret_cast<uintptr_t>(ya) % 16 == 0) ? 1 : 0;
+  p.x = static_cast<const float*>(o.xa); p.y = static_cast<const float*>(o.ya); p.dist = dist;
+  p.xrs = o.xrs; p.xcs = o.xcs; p.yrs = o.yrs; p.ycs = o.ycs; p.ldd = ldd; p.m = o.ma; p.n = o.na; p.k = static_cast<int>(k);
+  const UxPlan ux = ux_plan(o.xrs, o.xcs, reinterpret_cast<uintptr_t>(o.xa), o.yrs, o.ycs, reinterpret_cast<uintptr_t>(o.ya), k);
+  p.vec_x = ux.vec_x; p.vec_y = ux.vec_y;
   p.p = metric_arg; p.inv_p = metric == B2D_HammingUnexpanded ? 1.f / static_cast<float>(k) : 1.f / metric_arg;
-  p.tiles_n = static_cast<int>((na + UX_BN - 1) / UX_BN);
-  const int64_t tiles = ((ma + UX_BM - 1) / UX_BM) * p.tiles_n;
+  p.tiles_n = static_cast<int>((o.na + UX_BN - 1) / UX_BN);
+  const int64_t tiles = ((o.ma + UX_BM - 1) / UX_BM) * p.tiles_n;
   int sms = 0;
-  int rc  = device_sms(&sms);
+  rc      = device_sms(&sms);
   if (rc) return rc;
   switch (metric) {
-    case B2D_L1: return launch_ux_inst<UX_L1>(s, p, tiles);
-    case B2D_L2Unexpanded: return launch_ux_inst<UX_L2>(s, p, tiles);
-    case B2D_L2SqrtUnexpanded: return launch_ux_inst<UX_L2SQRT>(s, p, tiles);
-    case B2D_Linf: return launch_ux_inst<UX_LINF>(s, p, tiles);
-    case B2D_Canberra: return launch_ux_inst<UX_CANBERRA>(s, p, tiles);
-    case B2D_HammingUnexpanded: return launch_ux_inst<UX_HAMMING>(s, p, tiles);
+    case B2D_L1: return launch_ux_inst<UX_L1>(s, p, tiles, ux.tma);
+    case B2D_L2Unexpanded: return launch_ux_inst<UX_L2>(s, p, tiles, ux.tma);
+    case B2D_L2SqrtUnexpanded: return launch_ux_inst<UX_L2SQRT>(s, p, tiles, ux.tma);
+    case B2D_Linf: return launch_ux_inst<UX_LINF>(s, p, tiles, ux.tma);
+    case B2D_Canberra: return launch_ux_inst<UX_CANBERRA>(s, p, tiles, ux.tma);
+    case B2D_HammingUnexpanded: return launch_ux_inst<UX_HAMMING>(s, p, tiles, ux.tma);
     case B2D_KLDivergence:
-      return row_major ? launch_ux_inst<UX_KL>(s, p, tiles) : launch_ux_inst<UX_KL_REV>(s, p, tiles);
-    case B2D_JensenShannon: return launch_ux_inst<UX_JS>(s, p, tiles);
-    case B2D_BrayCurtis: return launch_ux_inst<UX_BRAYCURTIS>(s, p, tiles);
-    default: return launch_ux_inst<UX_LP>(s, p, tiles);
+      return row_major ? launch_ux_inst<UX_KL>(s, p, tiles, ux.tma) : launch_ux_inst<UX_KL_REV>(s, p, tiles, ux.tma);
+    case B2D_JensenShannon: return launch_ux_inst<UX_JS>(s, p, tiles, ux.tma);
+    case B2D_BrayCurtis: return launch_ux_inst<UX_BRAYCURTIS>(s, p, tiles, ux.tma);
+    default: return launch_ux_inst<UX_LP>(s, p, tiles, ux.tma);
   }
 }
 

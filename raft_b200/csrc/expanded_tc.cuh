@@ -116,6 +116,8 @@ __host__ __device__ constexpr bool tc_post_clamps(int post)
   return post == POST_CLAMP || post == POST_CLAMP_SQRT || post == POST_RBF;
 }
 __host__ __device__ constexpr bool tc_post_gram(int post) { return post == POST_RBF || post == POST_POLY || post == POST_TANH; }
+// EPI_STORE from registers: dist [.][ldd] takes 8-byte vector accesses at every even column of every row
+__host__ __device__ __forceinline__ bool tc_dist_vec2(uintptr_t dist, int64_t ldd) { return ((dist | static_cast<uintptr_t>(ldd * 4)) & 7u) == 0; }
 
 // Gram-matrix transform of one finished value u (RBF: the clamped squared distance; POLY / TANH: the inner product), in
 // full-precision fp32: one rounding for gamma u (+ coef0), then expf / tanhf, or the power by binary exponentiation
@@ -431,7 +433,7 @@ __device__ __forceinline__ void tc_epilogue(float (&v)[64], const TcParams& p, c
   }
   if (kEpi == EPI_STORE) {
     // (the manual stores: 8-byte vectors when dist and its pitch allow them)
-    const bool fast = row0 + 8 < p.m && gc0 + 127 < p.n && ((reinterpret_cast<uintptr_t>(p.dist) | p.ldd * 4) & 7u) == 0;
+    const bool fast = row0 + 8 < p.m && gc0 + 127 < p.n && tc_dist_vec2(reinterpret_cast<uintptr_t>(p.dist), p.ldd);
     if (p.acc_mode >= 2) {
       // K-chunked accumulation (k > 320): add this chunk's contribution to what the earlier chunks left in dist -- a
       // round-to-nearest fp32 add per chunk instead of ever longer truncating MMA chains on one accumulator

@@ -106,6 +106,8 @@ def _operands(X, Y, out):
     d_rm, ldd = _layout(d_cai)
     if m > 1 and n > 1 and d_rm != row_major:
         raise ValueError("out must have the same memory order as the inputs")
+    if not row_major:  # a single row reports C order with a pitch of n; in Fortran order its pitch is the column stride
+        ldd = d_cai.strides[1] // d_cai.dtype.itemsize if n > 1 else max(m, 1)
     ldd = max(ldd, n if row_major else m)
     return x_cai, y_cai, d_cai, dists, row_major, ldx, ldy, ldd
 

@@ -66,6 +66,23 @@ def test_cai_wrapper_and_layout():
         cai_wrapper(a)
 
 
+def test_single_row_fortran_output_pitch():
+    """x [1, k] against a Fortran-order y [n, k]: the result [1, n] is written in Fortran order, whose pitch is the
+    column stride of `out` -- a single contiguous row also reads as C order with a pitch of n, which would put element
+    (0, j) at j * n."""
+    from raft_b200.distance.pairwise_distance import _operands
+    x = np.zeros((1, 16), np.float32)
+    y = np.asfortranarray(np.zeros((130, 16), np.float32))
+    *_, row_major, ldx, ldy, ldd = _operands(FakeCai(x), FakeCai(y), FakeCai(np.zeros((1, 130), np.float32)))
+    assert (row_major, ldx, ldy, ldd) == (False, 1, 130, 1)
+    padded = np.zeros((130, 4), np.float32)[:, :1].T              # [1, 130] with a column stride of 4 elements
+    *_, row_major, ldx, ldy, ldd = _operands(FakeCai(x), FakeCai(y), FakeCai(padded))
+    assert (row_major, ldd) == (False, 4)
+    *_, row_major, ldx, ldy, ldd = _operands(FakeCai(np.zeros((3, 16), np.float32)), FakeCai(np.zeros((130, 16), np.float32)),
+                                             FakeCai(np.zeros((3, 136), np.float32)[:, :130]))
+    assert (row_major, ldx, ldy, ldd) == (True, 16, 16, 136)
+
+
 def test_shard_bounds_cover_database_exactly():
     for n, w in ((8_000_000, 8), (1001, 4), (7, 8), (5, 1)):
         cuts = [shard_bounds(n, w, r) for r in range(w)]
@@ -160,3 +177,70 @@ def test_exchange_plan_is_rank_invariant_and_covers_every_shard():
                 done += rows
             assert done == n_local
     assert plan_exchanges(1_000_000, 8)[0] == SHARD_HEAD_ROWS and len(plan_exchanges(1_000_000, 8)) >= 2
+
+
+def pairwise_plan(metric, dtype, m, n, k, x=0x1000, y=0x2000, dist=0x3000, ldx=None, ldy=None, ldd=None, row_major=True):
+    """b2d_debug_pairwise_plan as a dict; launches are (k-blocks, acc_mode, 'res' | 'str')."""
+    import ctypes
+    from raft_b200 import _lib
+    ldx = ldx or (k if row_major else m)
+    ldy = ldy or (k if row_major else n)
+    ldd = ldd or (n if row_major else m)
+    out = (ctypes.c_int * 70)()
+    rc = _lib.lib().b2d_debug_pairwise_plan(int(metric), dtype, x, ldx, y, ldy, dist, ldd, m, n, k, int(row_major), out, 70)
+    if rc:
+        return rc
+    path = ["none", "tensor", "simt", "simt-tma", "f64"][out[0]]
+    store = "tma" if out[1] else "vec2" if out[2] else "scalar"
+    launches = [(out[7 + 4 * i], out[8 + 4 * i], "res" if out[9 + 4 * i] else "str") for i in range(min(out[5], 16))]
+    assert [out[6 + 4 * i] for i in range(len(launches))] == [sum(l[0] for l in launches[:i]) for i in range(len(launches))]
+    return {"path": path, "store": store if path == "tensor" else None, "vec": (out[3], out[4]), "launches": launches}
+
+
+def test_pairwise_plan_boundaries():
+    """The dispatch decisions of b2d_pairwise_distance, without a device: resident | streaming at k = 128 | 129, one
+    pass | K chunks at 320 | 321, the remainder chunk's kernel at 384 | 385 and 512 | 513, TMA | register stores by
+    n % 4, ldd % 4 and the base address, 16-byte operand loads of the unexpanded kernels."""
+    from raft_b200 import _lib
+    DT = oracle.DistanceType
+    F32, F16, F64 = _lib.B2D_F32, _lib.B2D_F16, _lib.B2D_F64
+    for dt in (F32, F16):
+        plan = lambda k, **kw: pairwise_plan(DT.L2Expanded, dt, 300, 256, k, **kw)
+        assert plan(128) == {"path": "tensor", "store": "tma", "vec": (0, 0), "launches": [(4, 0, "res")]}
+        assert plan(129)["launches"] == [(5, 0, "str")]
+        assert plan(320)["launches"] == [(10, 0, "str")] and plan(320)["store"] == "tma"
+        assert plan(321)["launches"] == [(8, 1, "str"), (3, 3, "res")] and plan(321)["store"] == "vec2"
+        assert plan(384)["launches"] == [(8, 1, "str"), (4, 3, "res")]
+        assert plan(385)["launches"] == [(8, 1, "str"), (5, 3, "str")]
+        assert plan(512)["launches"] == [(8, 1, "str"), (8, 3, "str")]
+        assert plan(513)["launches"] == [(8, 1, "str"), (8, 2, "str"), (1, 3, "res")]
+        # the output's alignment decides how the tiles are stored
+        assert plan(64, dist=0x3004)["store"] == "scalar" and plan(64, dist=0x3008)["store"] == "vec2"
+        assert plan(64, ldd=257)["store"] == "scalar" and plan(64, ldd=258)["store"] == "vec2"
+        assert plan(64, ldd=260)["store"] == "tma"
+        assert plan(400, ldd=257)["store"] == "scalar" and plan(400, dist=0x3004)["store"] == "scalar"
+        assert pairwise_plan(DT.L2Expanded, dt, 300, 254, 64, ldd=256)["store"] == "vec2"
+        assert pairwise_plan(DT.L2Expanded, dt, 300, 252, 64)["store"] == "tma"
+        # Fortran order: dist is written as [n][m], so m takes the part of n
+        assert pairwise_plan(DT.L2Expanded, dt, 254, 300, 64, row_major=False)["store"] == "vec2"
+        assert pairwise_plan(DT.L2Expanded, dt, 256, 301, 64, row_major=False)["store"] == "tma"
+        # the ratio metrics run one pass at every k
+        for metric in (DT.JaccardExpanded, DT.DiceExpanded):
+            assert pairwise_plan(metric, dt, 300, 256, 1024)["launches"] == [(32, 0, "str")]
+        assert len(pairwise_plan(DT.InnerProduct, dt, 300, 256, 1024)["launches"]) == 4
+    # unexpanded kernels: fp32 only, each operand vectorised on its own
+    ux = lambda k, **kw: pairwise_plan(DT.L1, F32, 200, 100, k, **kw)
+    assert ux(32) == {"path": "simt-tma", "store": None, "vec": (1, 1), "launches": [(0, 0, "str")]}
+    assert ux(32, x=0x1004)["vec"] == (0, 1) and ux(32, y=0x2004)["vec"] == (1, 0) and ux(32, y=0x2004)["path"] == "simt"
+    assert ux(32, ldx=33)["vec"] == (0, 1) and ux(32, ldy=34)["vec"] == (1, 0) and ux(32, ldx=36, ldy=40)["vec"] == (1, 1)
+    assert ux(31)["vec"] == (0, 0) and ux(4)["vec"] == (1, 1) and ux(5)["vec"] == (0, 0)
+    assert ux(32, row_major=False)["vec"] == (0, 0)
+    assert pairwise_plan(DT.L1, F64, 200, 100, 32)["path"] == "f64"
+    assert pairwise_plan(DT.L2Expanded, F64, 200, 100, 32)["path"] == "f64"
+    assert pairwise_plan(DT.L1, F32, 0, 100, 32)["path"] == "none"
+    # refusals are those of b2d_pairwise_distance
+    for metric in oracle.UNEXPANDED:
+        assert pairwise_plan(metric, F16, 200, 100, 32) == _lib.B2D_ERR_UNSUPPORTED
+        assert _lib.lib().b2d_pairwise_workspace_bytes(int(metric), F16, 200, 100, 32) == 2 ** 64 - 1
+    assert pairwise_plan(13, F32, 200, 100, 32) == _lib.B2D_ERR_UNSUPPORTED
+    assert pairwise_plan(DT.L1, F32, 200, 100, 32, ldx=31) == _lib.B2D_ERR_INVALID_ARG
