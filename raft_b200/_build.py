@@ -37,8 +37,8 @@ def is_stale() -> bool:
 def build(force: bool = False, verbose: bool = False) -> str:
     if not force and not is_stale():
         return SO_PATH
-    cmd = [_nvcc()] + NVCC_FLAGS + (["-Xptxas", "-v"] if verbose else []) + \
-          ["-o", SO_PATH, os.path.join(CSRC, "api.cu"), "-ldl"]
+    units = [s for s in sources() if s.endswith(".cu")]
+    cmd = [_nvcc()] + NVCC_FLAGS + (["-Xptxas", "-v"] if verbose else []) + ["-o", SO_PATH] + units + ["-ldl"]
     res = subprocess.run(cmd, capture_output=True, text=True)
     if res.returncode != 0:
         raise RuntimeError("nvcc failed:\n" + res.stdout + res.stderr)

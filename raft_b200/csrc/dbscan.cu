@@ -1,0 +1,151 @@
+// DBSCAN (dbscan.cuh) on the epsilon neighbourhood of the tensor path.
+#include <cuda_runtime.h>
+#include <algorithm>
+#include <cmath>
+#include <cstring>
+
+#include "host.cuh"
+#include "dbscan.cuh"
+
+using namespace b2d;
+
+// ------------------------------------------------------------------------------------------
+// DBSCAN (dbscan.cuh): the epsilon neighbourhood of x against itself in column batches of the prepared rows, a device
+// union-find over the core points and the border rule.  Only enqueues work.
+namespace {
+constexpr int64_t kDbDefaultBatchBytes = 1ll << 30;
+
+// columns per batch: min(m, max(256, floor(max_bytes / m / 256) * 256)); max_bytes 0 means 2^30
+static int64_t db_batch(int64_t m, int64_t max_bytes)
+{
+  const int64_t mm = std::max<int64_t>(m, 1);
+  const int64_t mb = max_bytes > 0 ? max_bytes : kDbDefaultBatchBytes;
+  return std::min(mm, std::max<int64_t>(256, mb / mm / 256 * 256));
+}
+
+struct DbLayout {
+  TcWorkspace tc;    // x prepared once, as both operands
+  int64_t b, nb;     // columns per batch, batches
+  int64_t ld;        // adjacency row pitch: b rounded up to 16
+  unsigned* deg;     // [m + nb] per-column degrees, each batch's total behind its columns
+  int* parent;       // [m] union-find forest over the core rows (-1: not core)
+  int* border;       // [m] smallest root reaching a non-core row (INT_MAX: none)
+  unsigned* root;    // [m] root flags, scanned into cluster numbers
+  unsigned* core;    // [m] core flags, scanned into core_sample_indices positions
+  unsigned* tiles;   // scan tile sums
+  KmCtrl* ctrl;      // [2] scan totals: clusters, core rows
+  uint8_t* adj;      // [m][ld] adjacency of one batch
+  size_t bytes;
+};
+
+static DbLayout db_layout(void* base, int64_t m, int64_t d, int64_t max_bytes)
+{
+  Carve c(base, 1024);
+  DbLayout L{};
+  L.tc     = tc_layout(c, m, m, d, false);
+  L.b      = db_batch(m, max_bytes);
+  L.nb     = (m + L.b - 1) / L.b;
+  L.ld     = (L.b + 15) / 16 * 16;
+  L.deg    = c.take<unsigned>(m + L.nb);
+  L.parent = c.take<int>(m);
+  L.border = c.take<int>(m);
+  L.root   = c.take<unsigned>(m);
+  L.core   = c.take<unsigned>(m);
+  L.tiles  = c.take<unsigned>((m + kKmScanTile - 1) / kKmScanTile);
+  L.ctrl   = c.take<KmCtrl>(2);
+  L.adj    = c.take<uint8_t>(static_cast<size_t>(m) * L.ld);
+  L.bytes  = c.bytes;
+  return L;
+}
+
+// One EPI_EPS launch over the columns [s, s + w) of the prepared x (batch t): the adjacency into L.adj (adj) and / or
+// the degrees of those columns into deg[s + t, s + t + w] (deg).  diag_off = s keeps the self pairs.
+static int db_eps(cudaStream_t s, const DbLayout& L, int64_t m, int64_t d, float e, int64_t t, bool adj, bool deg)
+{
+  const int64_t c0 = t * L.b, w = std::min(L.b, m - c0);
+  TcParams p;
+  memset(&p, 0, sizeof(p));
+  p.m = m; p.n = w;
+  p.adj = adj ? L.adj : nullptr; p.ld_adj = L.ld;
+  p.vd = deg ? L.deg + c0 + t : nullptr; p.vd64 = 0; p.eps = e;
+  p.diag_off = c0;
+  p.tma_store = (adj && w % 16 == 0) ? 1 : 0;   // (L.adj is 1024-byte aligned and L.ld a multiple of 16)
+  return launch_tc(s, tc_rows(L.tc, 1, c0, d), p, d, EPI_EPS, POST_CLAMP);
+}
+
+static unsigned db_warp_grid(int64_t m) { return static_cast<unsigned>(std::min<int64_t>((m + 7) / 8, 1 << 16)); }
+}  // namespace
+
+size_t b2d_dbscan_workspace_bytes(int64_t m, int64_t d, int64_t max_bytes_per_batch)
+{
+  if (m < 0 || d < 0 || max_bytes_per_batch < 0) return static_cast<size_t>(-1);
+  return db_layout(nullptr, m, d, max_bytes_per_batch).bytes;
+}
+
+int b2d_dbscan_fit(void* stream, int metric, const float* x, int64_t ldx, int64_t m, int64_t d, double eps,
+                   int64_t min_samples, int64_t max_bytes_per_batch, int32_t* labels, int32_t* core_sample_indices,
+                   int32_t* n_clusters, void* workspace, size_t workspace_bytes)
+{
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  if (metric != B2D_L2SqrtExpanded && metric != B2D_L2Expanded && metric != B2D_CosineExpanded)
+    return fail(B2D_ERR_UNSUPPORTED, "dbscan supports the L2SqrtExpanded, L2Expanded and CosineExpanded metrics");
+  if (m < 0 || d < 0 || max_bytes_per_batch < 0) return fail(B2D_ERR_INVALID_ARG, "negative extent or batch size");
+  if (m == 0) return B2D_OK;
+  if (m > 0x7fffffffll) return fail(B2D_ERR_INVALID_ARG, "dbscan: m must be below 2^31");
+  if (d < 1) return fail(B2D_ERR_INVALID_ARG, "d must be positive");
+  if (d > 320) return fail(B2D_ERR_UNSUPPORTED, "dbscan supports d <= 320 (the whole distance at once)");
+  if (min_samples < 1) return fail(B2D_ERR_INVALID_ARG, "min_samples must be >= 1");
+  if (!x || !labels) return fail(B2D_ERR_INVALID_ARG, "null x / labels");
+  if (ldx < d) return fail(B2D_ERR_INVALID_ARG, "leading dimension smaller than d");
+  int rc = check_workspace(workspace, workspace_bytes, db_layout(nullptr, m, d, max_bytes_per_batch).bytes);
+  if (rc) return rc;
+  const DbLayout L = db_layout(workspace, m, d, max_bytes_per_batch);
+  // the threshold on the distance the kernel compares: eps^2 (rounded once from fp64) for L2SqrtExpanded; a NaN or
+  // negative eps matches nothing (every distance is >= 0 or NaN)
+  const float e = !(eps >= 0.0) ? -INFINITY : static_cast<float>(metric == B2D_L2SqrtExpanded ? eps * eps : eps);
+  const unsigned ms = static_cast<unsigned>(std::min<int64_t>(min_samples, m + 1));
+  // 0. x prepared once, as both operands; every batch takes a window of the y side
+  rc = launch_prep<float>(s, L.tc, x, ldx, 1, m, x, ldx, 1, m, d, nullptr, nullptr,
+                          metric == B2D_CosineExpanded ? PREP_COSINE : PREP_L2, 0);
+  if (rc) return rc;
+  // 1. degrees, then the core flags (one batch: the adjacency in the same launch)
+  B2D_CUDA(cudaMemsetAsync(L.deg, 0, static_cast<size_t>(m + L.nb) * sizeof(unsigned), s));
+  const bool one = L.nb == 1;
+  for (int64_t t = 0; t < L.nb; ++t) {
+    rc = db_eps(s, L, m, d, e, t, one, true);
+    if (rc) return rc;
+  }
+  db_core_kernel<<<sl_grid(m), 256, 0, s>>>(L.deg, m, L.b, ms, L.parent, L.border, L.core);
+  B2D_CUDA(cudaGetLastError());
+  // 2. links between core points
+  for (int64_t t = 0; t < L.nb; ++t) {
+    const int64_t c0 = t * L.b, w = std::min(L.b, m - c0);
+    if (!one) {
+      rc = db_eps(s, L, m, d, e, t, true, false);
+      if (rc) return rc;
+    }
+    db_link_kernel<<<db_warp_grid(m), kDbThreads, 0, s>>>(L.adj, L.ld, m, c0, w, L.core, L.parent);
+    B2D_CUDA(cudaGetLastError());
+  }
+  db_compress_kernel<<<sl_grid(m), 256, 0, s>>>(L.parent, m, L.root);
+  B2D_CUDA(cudaGetLastError());
+  // 3. border points
+  for (int64_t t = 0; t < L.nb; ++t) {
+    const int64_t c0 = t * L.b, w = std::min(L.b, m - c0);
+    if (!one) {
+      rc = db_eps(s, L, m, d, e, t, true, false);
+      if (rc) return rc;
+    }
+    db_border_kernel<<<db_warp_grid(m), kDbThreads, 0, s>>>(L.adj, L.ld, m, c0, w, L.parent, L.border);
+    B2D_CUDA(cudaGetLastError());
+  }
+  // 4. cluster numbers = ranks of the roots; core_sample_indices positions = ranks of the core rows
+  rc = km_scan(s, nullptr, L.root, m, L.tiles, L.ctrl);
+  if (rc) return rc;
+  rc = km_scan(s, nullptr, L.core, m, L.tiles, L.ctrl + 1);
+  if (rc) return rc;
+  db_label_kernel<<<sl_grid(m), 256, 0, s>>>(L.parent, L.border, L.root, L.core, m, &L.ctrl[0].total, &L.ctrl[1].total,
+                                             labels, core_sample_indices, n_clusters);
+  B2D_CUDA(cudaGetLastError());
+  return B2D_OK;
+}

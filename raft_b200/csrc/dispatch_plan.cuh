@@ -1,9 +1,9 @@
 // Which kernels a dense pairwise call runs, as host arithmetic on the shape, the pitches and the pointer alignments.
-// The launch code (api.cu: tc_store, launch_tc, b2d_pairwise_distance) follows these functions and
+// The launch code (tc_store and b2d_pairwise_distance in pairwise.cu, launch_tc in tensor_launch.cu) follows these functions and
 // b2d_debug_pairwise_plan reports them, so a test can name the path a shape takes without a device.
 #pragma once
 #include <cstdint>
-#include "expanded_tc.cuh"
+#include "tc_params.cuh"
 
 namespace b2d {
 

@@ -48,7 +48,7 @@
 //                     loaded or multiplied, partly adjacent ones set the non-adjacent values to +inf first.
 //   EPI_TOPK          fused brute-force kNN: the same minimum and vote against the row's current k-th best;
 //                     every pair at or below it is appended to the row's candidate list (see the kNN
-//                     helpers at the end of this file).
+//                     kernels in knn.cuh).
 //   EPI_EPS           epsilon neighbourhood: the EPI_STORE / POST_CLAMP distance, compared with eps; the 0/1 bytes go to
 //                     the EPI_STORE staging ring (one 64 x 128-byte box per tile), leave from there by TMA or a copy, and
 //                     are counted per column into shared memory (tc_eps_tile).
@@ -58,40 +58,10 @@
 #include <cstdint>
 #include "nn_key.cuh"
 #include "ptx.cuh"
+#include "tc_params.cuh"
 
 namespace b2d {
 
-constexpr int TC_BM          = 128;
-constexpr int TC_BN          = 256;
-constexpr int TC_HN          = 128;          // columns of one wgmma (half of a y block)
-constexpr int TC_A_BYTES     = TC_BM * 128;  // one k-block of A: 128 rows x 128 B
-constexpr int TC_B_BYTES     = TC_BN * 128;  // one k-block of the resident y block: 256 rows x 128 B
-constexpr int TC_BH_BYTES    = TC_HN * 128;  // one k-block of a streamed y half: 128 rows x 128 B
-constexpr int TC_MAX_RES_KB  = 4;            // resident-B variant: k <= 128
-constexpr int TC_STAGES_RES  = 5;            // A-only stages (16 KB) next to the resident y block
-constexpr int TC_STAGES_STR  = 6;            // A + B-half stages (32 KB) when both operands stream
-constexpr int TC_STAGES_RES_ST = 4;          // the same with the output staging of EPI_STORE beside them
-constexpr int TC_STAGES_STR_ST = 6;
-constexpr int TC_MAX_STAGES  = 6;
-constexpr int TC_THREADS     = 384;
-// EPI_STORE output staging: TMA boxes of 64 rows x 32 fp32 columns (128-byte rows, SWIZZLE_128B), a ring of
-// TC_STG_BOXES per consumer warpgroup (DESIGN.md section 2 K1: the carve against the x stages, measured).  The ring
-// logic of tc_stage_store is written for exactly two boxes.
-constexpr int TC_D_BOX_COLS  = 32;
-constexpr int TC_D_BOX_ROWS  = 64;
-constexpr int TC_D_BOX_BYTES = TC_D_BOX_COLS * TC_D_BOX_ROWS * 4;
-constexpr int TC_STG_BOXES   = 2;
-
-enum TcEpilogue : int { EPI_STORE = 0, EPI_MINLOC = 1, EPI_TOPK = 2, EPI_MINLOC_MASKED = 3, EPI_EPS = 4 };
-constexpr int64_t TC_NO_DIAG = INT64_MIN;   // TcParams::diag_off: y is not a row window of x
-
-// EPI_MINLOC_MASKED (masked_nn.cuh): class of one (64-row slab of x, 128-column half of a y block) tile.  Byte
-// TcParams::mask_cls[n_blk][mt] holds the four classes of an (x tile, y block) pair, 2 bits each at bit 2 (2 h + s)
-// for slab s (= consumer warpgroup) and half h.  A byte of 0 is a tile with nothing to do.
-enum MaskClass : int { MASK_NONE = 0, MASK_ALL = 1, MASK_PARTIAL = 2 };
-__host__ __device__ __forceinline__ int mask_class_of(unsigned cls_byte, int h, int s) { return (cls_byte >> (2 * (2 * h + s))) & 3; }
-// some slab of half h is live: the streaming variant loads the half's stages
-__host__ __device__ __forceinline__ bool mask_half_live(unsigned cls_byte, int h) { return ((cls_byte >> (4 * h)) & 15u) != 0u; }
 // max(v, 0) that keeps a NaN (fmaxf(NaN, 0) = 0 would turn a poisoned distance into a perfect match)
 __device__ __forceinline__ float clamp0(float v)
 {
@@ -99,25 +69,6 @@ __device__ __forceinline__ float clamp0(float v)
   asm("max.NaN.f32 %0, %1, 0f00000000;" : "=f"(r) : "f"(v));
   return r;
 }
-
-enum TcPost : int { POST_NONE = 0, POST_CLAMP = 1, POST_CLAMP_SQRT = 2,
-                    POST_JACCARD = 3,  // d = 1 - a / (s - a), a = <x,y>, s = |x|^2 + |y|^2 (0/0 -> 0)
-                    POST_DICE    = 4,  // d = 1 - 2 a / s
-                    // kernel Gram matrices (gram_post; TcParams::gamma / coef0 / degree):
-                    POST_RBF     = 5,  // exp(-gamma d), d the POST_CLAMP distance
-                    POST_POLY    = 6,  // (gamma <x,y> + coef0)^degree
-                    POST_TANH    = 7 };  // tanh(gamma <x,y> + coef0)
-
-// the ratio metrics: computed from the inner product and the squared norms at once (never K-chunked)
-__host__ __device__ constexpr bool tc_post_ratio(int post) { return post == POST_JACCARD || post == POST_DICE; }
-// the squared L2 distance, clamped at 0 (with d(i, i) = 0 when x and y alias) before anything else is done with it
-__host__ __device__ constexpr bool tc_post_clamps(int post)
-{
-  return post == POST_CLAMP || post == POST_CLAMP_SQRT || post == POST_RBF;
-}
-__host__ __device__ constexpr bool tc_post_gram(int post) { return post == POST_RBF || post == POST_POLY || post == POST_TANH; }
-// EPI_STORE from registers: dist [.][ldd] takes 8-byte vector accesses at every even column of every row
-__host__ __device__ __forceinline__ bool tc_dist_vec2(uintptr_t dist, int64_t ldd) { return ((dist | static_cast<uintptr_t>(ldd * 4)) & 7u) == 0; }
 
 // Gram-matrix transform of one finished value u (RBF: the clamped squared distance; POLY / TANH: the inner product), in
 // full-precision fp32: one rounding for gamma u (+ coef0), then expf / tanhf, or the power by binary exponentiation
@@ -143,189 +94,6 @@ __device__ __forceinline__ float post_ratio(float a, float s)
   const float den = kPost == POST_JACCARD ? s - a : s;
   const float num = kPost == POST_JACCARD ? a : 2.f * a;
   return !(den <= 0.f) ? clamp0(1.f - __fdividef(num, den)) : 0.f;   // (NaN inputs give NaN, 0/0 gives 0)
-}
-
-struct TcParams {
-  int64_t m, n;
-  int nkb;                // k-blocks of 32 source columns
-  int tiles_m, tiles_n;   // ceil(m/128), ceil(n/256)
-  int tiles_sel;          // y blocks this launch visits (all of them unless sel_s > 1)
-  int sel_s, sel_lo, sel_hi;  // sel_s > 1: only the y blocks with sel_lo <= index % sel_s < sel_hi
-  int chunk;              // m-tiles per work item
-  int chunks_m;           // ceil(tiles_m/chunk)
-  int64_t n_items;        // tiles_n * chunks_m
-  const float* xt;        // [m] row term t_x[i]
-  const float* yt;        // [n] column term t_y[j]
-  const float* coef;      // [1] scalar c: d = acc * c + (t_x[i] + t_y[j])  (prep.cuh)
-  const unsigned* has_lo; // [1] 0: every operand is exact in fp16 -> the cross-term MMAs are skipped
-  const float* xsc;       // [m] per-row scale of x: d = acc * c * xsc[i] * ysc[j] + ...  (1 unless the row took its own
-  const float* ysc;       // [n]   exponent in prep.cuh -- rows far below the matrix maximum)
-  const unsigned* nonuni; // [2] some row of x / of y has a scale != 1 (y: the per-column factor is applied)
-  // EPI_STORE
-  float* dist;
-  int64_t ldd;
-  int diag_zero;          // x and y alias: force d(i,i) = 0 (reference: CHANGELOG.md:1057,1213)
-  int tma_store;          // dist goes out through the staging boxes and the dist tensor map (api.cu: aligned, single pass)
-  int acc_mode;           // K-chunked accumulation: 0 single pass, 1 first chunk (raw store), 2 middle (+=), 3 last (+=, post)
-  // EPI_MINLOC
-  long long* keys;        // [m] packed (ordered bits of the distance << 32 | index)
-  int64_t idx_offset;
-  const int* col_map;     // non-null: column j of the packed y is source row col_map[j] (norm-sorted chunk, api.cu)
-  const unsigned* run_flag;  // non-null: the whole launch is a no-op unless *run_flag != 0
-  // EPI_TOPK (fused brute-force kNN): every pair at or below the row's current k-th best joins the row's list
-  const float* knn_thr;   // [m] current k-th best squared distance of the row (+inf until k are known)
-  unsigned* knn_cnt;      // [m] fill counter of the row's candidate list
-  long long* knn_cand;    // [m][knn_cap] packed (ordered bits of the distance << 32 | index)
-  unsigned knn_cap;
-  long long* knn_dropmin; // [m] smallest key that did not fit into the row's list this pass (knn_merge_kernel decides whether
-                          //     anything that matters was lost; rows where it was are redone by knn_fix_kernel)
-  // EPI_MINLOC_MASKED (masked_nn.cuh): only pairs whose row of x is adjacent to the group of the row of y are candidates
-  const uint8_t* mask_cls;    // [tiles_n][tiles_m] tile classes (MaskClass, see mask_class_of)
-  const int* mask_grp;        // [n] group of every row of y (-1: in no group)
-  const unsigned* mask_bits;  // [ceil(m/32)][mask_groups] bit i % 32 of word (i / 32, g): row i of x is adjacent to group g
-  int64_t mask_groups;
-  // EPI_EPS (epsilon neighbourhood): adj[i][j] = (d(i, j) <= eps) with d the EPI_STORE / POST_CLAMP distance; vd[j] += the
-  // number of adjacent rows of column j, vd[n] += the total.  tma_store: adj leaves through the staging boxes
-  uint8_t* adj;           // [m][ld_adj] 0 / 1 bytes (null: count only)
-  int64_t ld_adj;
-  void* vd;               // [n + 1] uint32 counts, or uint64 when vd64 (null: adjacency only)
-  int vd64;
-  float eps;              // the squared radius
-  int64_t diag_off;       // row j of y is row j + diag_off of x (same memory): d = 0 there; TC_NO_DIAG: no such rows
-  // EPI_STORE with POST_RBF / POST_POLY / POST_TANH (gram_post): the kernel parameters, applied to the final value only
-  float gamma;
-  float coef0;
-  int degree;
-};
-
-constexpr size_t TC_SMEM_OPERANDS = (size_t)TC_MAX_RES_KB * TC_B_BYTES + (size_t)TC_STAGES_RES * TC_A_BYTES;  // 208 KB
-static_assert((size_t)TC_STAGES_STR * (TC_A_BYTES + TC_BH_BYTES) <= TC_SMEM_OPERANDS, "streaming carve fits");
-
-// Shared-memory carve of one instantiation: [resident y block][x (+ y half) stages][output staging][t_y][barriers].
-// The arg-min / top-k epilogues store nothing and keep 208 KB of operands; EPI_STORE trades one x stage for 32 KB of
-// output staging (the streaming variant fits it beside all of its stages).
-// x rings: streaming, one ring of `stages` stages that both consumer warpgroups read.  Resident, one ring of `stages`
-// 64-row k-blocks (8 KB) per consumer warpgroup, laid out in the same bytes: slot s of ring w is the 8 KB at w * 8 KB of
-// the 16 KB stage s, and every ring has full / empty mbarriers of its own.
-// mbarriers (after t_y): afull[rings * TC_MAX_STAGES], aempty[rings * TC_MAX_STAGES] (slot s of ring w at rings * s + w),
-// bfull[TC_MAX_RES_KB], bempty[TC_MAX_RES_KB].
-// EPI_EPS has the carve of EPI_STORE (its adjacency boxes are the same 8 KB) plus the [256] column counts in the slot of the
-// masked kernel's groups.
-template <bool kResident, int kEpi>
-struct TcCarve {
-  static constexpr bool staged = kEpi == EPI_STORE || kEpi == EPI_EPS;
-  static constexpr int stages = staged ? (kResident ? TC_STAGES_RES_ST : TC_STAGES_STR_ST)
-                                       : (kResident ? TC_STAGES_RES : TC_STAGES_STR);
-  static constexpr int rings  = kResident ? 2 : 1;
-  static constexpr uint32_t stage_bytes = kResident ? TC_A_BYTES : TC_A_BYTES + TC_BH_BYTES;
-  static constexpr size_t a_off   = kResident ? (size_t)TC_MAX_RES_KB * TC_B_BYTES : 0;
-  static constexpr size_t stg_off = a_off + (size_t)stages * stage_bytes;
-  static constexpr size_t tb_off  = staged ? stg_off + 2 * (size_t)TC_STG_BOXES * TC_D_BOX_BYTES : TC_SMEM_OPERANDS;
-  static constexpr size_t grp_off = tb_off + TC_BN * 4 + 256;   // EPI_MINLOC_MASKED: [256] group, EPI_EPS: count of every column
-  static constexpr size_t bytes   = grp_off + (kEpi == EPI_MINLOC_MASKED || kEpi == EPI_EPS ? TC_BN * 4 : 0);
-  static_assert(stages <= TC_MAX_STAGES, "barrier arrays hold TC_MAX_STAGES stages");
-  static_assert((2 * rings * TC_MAX_STAGES + 2 * TC_MAX_RES_KB) * 8 <= grp_off - tb_off - TC_BN * 4,
-                "the mbarriers of every ring fit in the 256 bytes after t_y");
-  static_assert(!kResident || stages >= TC_MAX_RES_KB, "resident: the ring holds every x k-block of a tile (both halves read them)");
-  static_assert(stg_off % 1024 == 0, "SWIZZLE_128B staging boxes need 1024-byte alignment");
-  static_assert(staged || stg_off <= TC_SMEM_OPERANDS, "operands fit");
-  static_assert(bytes <= 232448, "exceeds the 227 KB per-CTA limit");
-};
-
-// index of the s-th selected y block (see TcParams::sel_s)
-__host__ __device__ __forceinline__ int sel_to_blk(int s, int S, int lo, int hi)
-{
-  if (S <= 1) return s;
-  const int w = hi - lo;
-  return (s / w) * S + lo + (s % w);
-}
-// how many of the blocks [0, tiles_n) are selected
-__host__ __device__ __forceinline__ int sel_count(int tiles_n, int S, int lo, int hi)
-{
-  if (S <= 1) return tiles_n;
-  const int rem = tiles_n % S;
-  return (tiles_n / S) * (hi - lo) + max(0, min(rem, hi) - lo);
-}
-
-// Work item `item` of a persistent tensor-core launch (TcParams or ScreenParams): y block n_blk, x tiles [mt0, mt1), and
-// the nh halves of the y block that lie inside the matrix.
-struct TcItem {
-  int n_blk, mt0, mt1, nh;
-};
-template <class P>
-__host__ __device__ __forceinline__ TcItem tc_item(const P& p, int64_t item)
-{
-  TcItem t;
-  t.n_blk = sel_to_blk(static_cast<int>(item % p.tiles_sel), p.sel_s, p.sel_lo, p.sel_hi);
-  t.mt0   = static_cast<int>(item / p.tiles_sel) * p.chunk;
-  t.mt1   = min(t.mt0 + p.chunk, p.tiles_m);
-  t.nh    = static_cast<int64_t>(t.n_blk) * TC_BN + TC_HN < p.n ? 2 : 1;
-  return t;
-}
-
-// EPI_MINLOC_MASKED skip decisions (DESIGN.md section 2 K3m), shared by the producer, the consumers and the host replay of
-// the schedule (tests/cpp/masked_schedule_test.cu).  Class bytes are read through mask_cls_at.
-__host__ __device__ __forceinline__ unsigned mask_cls_at(const uint8_t* cls, int mt)
-{
-#ifdef __CUDA_ARCH__
-  return __ldg(&cls[mt]);
-#else
-  return cls[mt];
-#endif
-}
-// the item's last loaded tile (its y block is handed back after it); -1: no tile is loaded, the item is skipped
-__host__ __device__ __forceinline__ int mask_mt_last(const uint8_t* cls, int mt0, int mt1)
-{
-  int mt_last = -1;
-  for (int mt = mt0; mt < mt1; ++mt)
-    if (mask_cls_at(cls, mt) != 0u) mt_last = mt;
-  return mt_last;
-}
-// half h of a tile with class byte tcls != 0 has stages in the ring: resident, the tile's stages serve both halves;
-// streaming, a half no slab needs is not loaded
-__host__ __device__ __forceinline__ bool mask_half_loaded(bool resident, unsigned tcls, int h)
-{
-  return resident || mask_half_live(tcls, h);
-}
-// half h of nh hands its stages back (resident: the tile's last half, after both have read them)
-__host__ __device__ __forceinline__ bool tc_half_releases(bool resident, int h, int nh) { return !resident || h == nh - 1; }
-
-// The producer's load order, one definition for every instantiation and for the host replay of the masked schedule:
-// load_b(kb, it_local, t) for each k-block of a resident y block, load_a(a_it, t, mt, h, kb) for each stage (t: the
-// work item, tc_item).
-// kMasked skips the loads of dead tiles: a tile whose class byte is 0 loads nothing; in the streaming variant a half no
-// slab needs loads nothing; an item without a live tile loads no y block and does not count in it_local (the bfull /
-// bempty parity).
-#pragma nv_exec_check_disable
-template <bool kResident, bool kMasked, class P, class LoadB, class LoadA>
-__host__ __device__ __forceinline__ void tc_producer_walk(const P& p, int nkb, int64_t first_item, int64_t stride,
-                                                          LoadB&& load_b, LoadA&& load_a)
-{
-  uint32_t a_it = 0, it_local = 0;
-  for (int64_t item = first_item; item < p.n_items; item += stride) {
-    const TcItem t     = tc_item(p, item);
-    const uint8_t* cls = kMasked ? p.mask_cls + static_cast<int64_t>(t.n_blk) * p.tiles_m : nullptr;
-    bool b_loaded      = false;
-    for (int mt = t.mt0; mt < t.mt1; ++mt) {
-      unsigned tcls = 0u;
-      if constexpr (kMasked) {
-        tcls = mask_cls_at(cls, mt);
-        if (tcls == 0u) continue;
-      }
-      // resident: one load of an x k-block serves both halves of the tile; streaming: every stage carries its y half
-      for (int h = 0; h < (kResident ? 1 : t.nh); ++h) {
-        if constexpr (kMasked)
-          if (!mask_half_loaded(kResident, tcls, h)) continue;
-        for (int kb = 0; kb < nkb; ++kb, ++a_it) {
-          // the item's first loaded tile brings its y block (unmasked, every tile is loaded)
-          if (kResident && (kMasked ? !b_loaded : mt == t.mt0)) load_b(kb, it_local, t);
-          load_a(a_it, t, mt, h, kb);
-        }
-        b_loaded = true;
-      }
-    }
-    if (!kMasked || b_loaded) ++it_local;
-  }
 }
 
 __device__ __forceinline__ float min3(float a, float b, float c) { return fminf(fminf(a, b), c); }
@@ -1006,377 +774,6 @@ expanded_tc_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_cons
       tc_eps_flush(p, col_cnt, tc_item(p, last_item).n_blk, ct);
     }
   }
-}
-
-// ---------------------------------------------------------------------------------------------
-// small helper kernels for the NN path
-
-__global__ void minloc_init_kernel(long long* keys, int64_t m)
-{
-  int64_t i = static_cast<int64_t>(blockIdx.x) * blockDim.x + threadIdx.x;
-  if (i < m) keys[i] = KEY_EMPTY;
-}
-
-struct KvpIF {
-  int key;
-  float value;
-};
-
-// packed key -> raft::KeyValuePair<int,float>{argmin, min distance}: clamp at 0, optional sqrt.
-__global__ void minloc_finalize_kernel(KvpIF* out, const long long* keys, int64_t m, int do_sqrt,
-                                       int merge_existing)
-{
-  int64_t i = static_cast<int64_t>(blockIdx.x) * blockDim.x + threadIdx.x;
-  if (i >= m) return;
-  const long long key = keys[i];
-  const float v       = key_dist(key);
-  float d             = v < 0.f ? 0.f : v;  // clamp at 0; NaN (zero-norm rows under cosine / NaN inputs) stays NaN
-  if (do_sqrt) d = sqrtf(d);
-  KvpIF o;
-  o.key   = static_cast<int>(key_index(key));
-  o.value = d;
-  if (key == KEY_EMPTY) {  // no candidate (n == 0)
-    o.key   = 0x7fffffff;
-    o.value = __int_as_float(0x7f7fffff);
-  }
-  if (merge_existing) {
-    // initOutBuffer == false: reduce into what the caller already has (argmin_op)
-    KvpIF e = out[i];
-    if ((e.value < o.value) || (e.value == o.value && e.key < o.key)) o = e;
-  }
-  out[i] = o;
-}
-
-// ---------------------------------------------------------------------------------------------
-// Screened fusedL2NN (64 < k <= 128, large n; orchestration: fused_nn_keys_chunk in api.cu).  The chunk of y is packed
-// in the order of its squared row norms; an exact pass over every 32nd block gives each row an upper bound of its
-// minimum; the coarse pass of screen_tc.cuh (1 tensor product instead of 3) over ALL blocks keeps only the columns
-// whose rigorous LOWER bound reaches that upper bound; those few are re-evaluated exactly, straight from the fp32
-// inputs (sum (x-y)^2), together with the incumbent, so every finalist is measured with the same arithmetic.
-
-// sort key of a database row: the bits of its squared norm (fp32, non-negative: the unsigned order is the float order)
-__global__ void __launch_bounds__(256) nn_sortkey_kernel(const float* y, int64_t ldy, int64_t n, int k, const float* yn,
-                                                         unsigned* key, int* val)
-{
-  const int lane  = threadIdx.x & 31;
-  const int64_t r = static_cast<int64_t>(blockIdx.x) * 8 + (threadIdx.x >> 5);
-  if (r >= n) return;
-  float ss = 0.f;
-  if (yn != nullptr) {
-    ss = __ldg(&yn[r]);
-  } else {
-    const float* row = y + r * ldy;
-    for (int t = lane; t < k; t += 32) { const float v = __ldg(row + t); ss = fmaf(v, v, ss); }
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) ss += __shfl_xor_sync(0xffffffffu, ss, o);
-  }
-  if (lane == 0) {
-    key[r] = (ss >= 0.f) ? __float_as_uint(ss) : 0xffffffffu;   // NaN / negative caller norms: last
-    val[r] = static_cast<int>(r);
-  }
-}
-
-// after the exact sub-sampled pass: thr = incumbent distance, incumbent -> candidate, keys reset
-__global__ void nn_seed_kernel(long long* keys, float4* aux, const float* xt, const float* xlo, int2* cand, unsigned* flags,
-                               int64_t m, int64_t n, int64_t idx_offset)
-{
-  int64_t i = static_cast<int64_t>(blockIdx.x) * blockDim.x + threadIdx.x;
-  if (i == 0) {  // [0] list slots in use [1] overflow [2] go_screen [3] go_exact [4] redo_trial [5] candidates after the trial
-    flags[0] = static_cast<unsigned>(m);   // [6] candidates found by the screen (slots are reserved in blocks)
-    flags[1] = flags[2] = flags[3] = flags[4] = flags[5] = flags[6] = 0u;
-  }
-  if (i >= m) return;
-  const long long key = keys[i];
-  float t             = __int_as_float(0x7f800000);   // no incumbent: no bound
-  int2 c              = make_int2(-1, -1);
-  if (key != KEY_EMPTY) {
-    t                 = key_dist(key);
-    const long long j = key_index(key) - idx_offset;
-    if (j >= 0 && j < n) {  // incumbent of THIS shard: re-measured with the exact arithmetic below
-      c       = make_int2(static_cast<int>(i), static_cast<int>(j));
-      keys[i] = KEY_EMPTY;
-    }                        // else: a key merged in from another shard stays as it is
-  }
-  // screening compares v = d - |x|^2 with (bound - |x|^2), rounded up so that it stays an upper bound
-  const float xn = xt[i];
-  aux[i]  = make_float4((t - xn) + (t + xn) * (1.f / 2097152.f), sqrtf(xn) * (1.f + 1.f / 4194304.f), xlo[i], 0.f);
-  cand[i] = c;
-}
-
-// device-side control of the screened search (fused_nn_keys in api.cu)
-//   stage 1, after the trial screen: candidates per row above tau (or a full list) -> exact for the rest
-//   stage 2, after the main screen : a full list -> exact for the blocks it covered
-__global__ void nn_decide_kernel(unsigned* flags, unsigned m, float tau, int stage, const unsigned* nonuni)
-{
-  if (stage == 1) {
-    flags[5]            = flags[6];
-    // per-column scales (rows of y with their own exponent): the screen's single coefficient does not hold ->
-    // everything it covered is redone by the exact kernel
-    const unsigned redo = (flags[1] != 0u || nonuni[1] != 0u) ? 1u : 0u;
-    const bool many     = static_cast<float>(flags[6]) > tau * static_cast<float>(m);
-    flags[4]            = redo;
-    flags[3]            = (redo || many) ? 1u : 0u;
-    flags[2]            = flags[3] ? 0u : 1u;
-  } else if (flags[2] != 0u && flags[1] != 0u) {
-    flags[3] = 1u;
-  }
-}
-
-// one warp per candidate, straight from the original fp32 inputs:
-//   family 0  d = sum (x_i - y_j)^2
-//   family 1  d = 1 - <x', y'> / (|x'| |y'|), x' = x - mean(x) when centred (correlation), else x (cosine)
-// (k <= 128 on this path: a lane holds at most 4 elements of each row in registers)
-__global__ void __launch_bounds__(256) nn_exact_kernel(long long* keys, const int2* cand, const unsigned* cnt,
-                                                       unsigned cap, const float* x, int64_t ldx, const float* y,
-                                                       int64_t ldy, int k, int64_t idx_offset, int family, int center,
-                                                       unsigned n_seed, const int* col_map)
-{
-  const int lane       = threadIdx.x & 31;
-  const unsigned total = min(*cnt, cap);
-  const unsigned nwarp = gridDim.x * (blockDim.x >> 5);
-  for (unsigned c = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5); c < total; c += nwarp) {
-    int2 ij = cand[c];
-    if (ij.x < 0) continue;
-    // the first n_seed entries (nn_seed_kernel: the incumbents) hold source rows of y, the screen's entries packed
-    // positions of the norm-sorted chunk
-    if (c >= n_seed && col_map != nullptr) ij.y = __ldg(&col_map[ij.y]);
-    const float* xr = x + static_cast<int64_t>(ij.x) * ldx;
-    const float* yr = y + static_cast<int64_t>(ij.y) * ldy;
-    float xv[4], yv[4];
-#pragma unroll
-    for (int u = 0; u < 4; ++u) {
-      const int t = lane + 32 * u;
-      xv[u]       = t < k ? __ldg(xr + t) : 0.f;
-      yv[u]       = t < k ? __ldg(yr + t) : 0.f;
-    }
-    float res;
-    if (family == 0) {
-      float acc = 0.f;
-#pragma unroll
-      for (int u = 0; u < 4; ++u) { const float d = xv[u] - yv[u]; acc = fmaf(d, d, acc); }
-#pragma unroll
-      for (int o = 16; o > 0; o >>= 1) acc += __shfl_xor_sync(0xffffffffu, acc, o);
-      res = acc;
-    } else {
-      float mx = 0.f, my = 0.f;
-      if (center) {
-        float sx = (xv[0] + xv[1]) + (xv[2] + xv[3]), sy = (yv[0] + yv[1]) + (yv[2] + yv[3]);
-#pragma unroll
-        for (int o = 16; o > 0; o >>= 1) { sx += __shfl_xor_sync(0xffffffffu, sx, o); sy += __shfl_xor_sync(0xffffffffu, sy, o); }
-        mx = sx / static_cast<float>(k);
-        my = sy / static_cast<float>(k);
-      }
-      float dot = 0.f, nx = 0.f, ny = 0.f;
-#pragma unroll
-      for (int u = 0; u < 4; ++u) {
-        const bool in = lane + 32 * u < k;
-        const float a = in ? xv[u] - mx : 0.f, b = in ? yv[u] - my : 0.f;
-        dot = fmaf(a, b, dot); nx = fmaf(a, a, nx); ny = fmaf(b, b, ny);
-      }
-#pragma unroll
-      for (int o = 16; o > 0; o >>= 1) {
-        dot += __shfl_xor_sync(0xffffffffu, dot, o);
-        nx += __shfl_xor_sync(0xffffffffu, nx, o);
-        ny += __shfl_xor_sync(0xffffffffu, ny, o);
-      }
-      res = 1.f - dot / sqrtf(nx * ny);
-    }
-    if (lane == 0) atomicMin(&keys[ij.x], key_pack(res, static_cast<long long>(ij.y) + idx_offset));
-  }
-}
-
-// ---------------------------------------------------------------------------------------------
-// Fused brute-force kNN (SURVEY.md 8(f2)): the distance tiles are never written.  The database is
-// swept in passes of doubling width; EPI_TOPK appends every pair at or below the row's current k-th
-// best to the row's list (~k per row and pass on unordered data), knn_merge_kernel folds the list
-// into the row's sorted top-k and publishes the new k-th best.
-
-constexpr int KNN_MAX_K = 64;
-constexpr int KNN_CAP   = 128;   // list entries per row and pass
-constexpr int KNN_SORT  = 256;   // KNN_MAX_K + KNN_CAP padded to a power of two
-
-__global__ void knn_init_kernel(long long* topk, float* thr, unsigned* cnt, long long* dropmin, unsigned* dirty_cnt,
-                                unsigned* repaired, int64_t m, int kk)
-{
-  const int64_t i = static_cast<int64_t>(blockIdx.x) * blockDim.x + threadIdx.x;
-  if (i < 65) dirty_cnt[i] = 0u;   // one counter per pass, then the counter of the repaired-row list
-  if (i < m) { thr[i] = __int_as_float(0x7f800000); cnt[i] = 0u; dropmin[i] = KEY_EMPTY; repaired[i] = 0u; }
-  if (i < m * kk) topk[i] = KEY_EMPTY;
-}
-
-// one warp per row: sort (top-k so far) + (this pass's list) by (distance, index), keep the first kk.  A row whose list
-// was full lost entries; that only matters if the best dropped key could still enter the new top-k -- such rows go
-// to the pass's dirty list and knn_fix_kernel redoes them over the pass's columns (no host round trip anywhere).  A row
-// dirty for the first time also goes to the repaired-row list (rep_list / rep_cnt, flag repaired[row]), which is measured
-// again over all columns after the last pass.
-__global__ void __launch_bounds__(256) knn_merge_kernel(long long* topk, const long long* cand, unsigned* cnt, float* thr,
-                                                        long long* dropmin, int* dirty, unsigned* dirty_cnt, unsigned* repaired,
-                                                        int* rep_list, unsigned* rep_cnt, int64_t m, int kk)
-{
-  __shared__ long long buf[8][KNN_SORT];
-  const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
-  const int64_t row = static_cast<int64_t>(blockIdx.x) * 8 + wid;
-  if (row >= m) return;
-  const unsigned craw = cnt[row];
-  const unsigned nc   = min(craw, static_cast<unsigned>(KNN_CAP));
-  if (nc == 0u) return;  // nothing new for this row (the common case in the late passes)
-  long long* b = buf[wid];
-  // sort only as much as there is (warp-uniform): with k = 16 and ~16 new entries per pass that is 32 or 64 keys,
-  // not KNN_SORT = 256 -- the merge launches were a third of a 100000 x 100000 kNN
-  int ssz = 32;
-  while (ssz < kk + static_cast<int>(nc)) ssz <<= 1;
-  for (int t = lane; t < ssz; t += 32) {
-    long long key = KEY_EMPTY;
-    if (t < kk) key = topk[row * kk + t];
-    else if (t - kk < static_cast<int>(nc)) key = cand[row * KNN_CAP + (t - kk)];
-    b[t] = key;
-  }
-  __syncwarp();
-  for (int size = 2; size <= ssz; size <<= 1)
-    for (int stride = size >> 1; stride > 0; stride >>= 1) {
-      for (int t = lane; t < ssz / 2; t += 32) {
-        const int i = 2 * t - (t & (stride - 1)), j = i + stride;
-        const bool up = (i & size) == 0;
-        const long long a = b[i], c = b[j];
-        if ((a > c) == up) { b[i] = c; b[j] = a; }
-      }
-      __syncwarp();
-    }
-  for (int t = lane; t < kk; t += 32) topk[row * kk + t] = b[t];
-  if (lane == 0) {
-    cnt[row]            = 0u;
-    const long long kth = b[kk - 1];
-    if (kth != KEY_EMPTY) thr[row] = key_dist(kth);
-    if (craw > static_cast<unsigned>(KNN_CAP)) {
-      if (dropmin[row] <= kth) {
-        dirty[atomicAdd(dirty_cnt, 1u)] = static_cast<int>(row);
-        if (!repaired[row]) {   // (one warp owns the row, and the merges of the passes run one after another)
-          repaired[row]                    = 1u;
-          rep_list[atomicAdd(rep_cnt, 1u)] = static_cast<int>(row);
-        }
-      }
-      dropmin[row] = KEY_EMPTY;
-    }
-  }
-}
-
-// Rows whose candidate list overflowed in a way that matters (database ordered by decreasing distance, duplicates of one
-// near point, ...): one block per dirty row re-evaluates the pass's columns [off, off + width) straight from the fp32
-// inputs -- family 0: sum (x - y)^2, family 1: 1 - <x', y'> / (|x'||y'|) with x' centred for correlation -- one column per
-// thread, and folds them into the row's top-k (entries this pass had already contributed are taken out first, so no
-// column can appear twice).  Exact for any input order; costs O(width * k) per dirty row, nothing when the list is empty.
-// After the last pass the same kernel measures every repaired row again over all columns (off = 0, width = n): the
-// entries of a repaired row would otherwise come from two arithmetics (tensor and direct), and exact duplicates could
-// then be ranked out of index order.
-__global__ void __launch_bounds__(256) knn_fix_kernel(long long* topk, float* thr, const int* dirty, const unsigned* dirty_cnt,
-                                                      const float* x, int64_t ldx, const float* y, int64_t ldy, int k, int kk,
-                                                      int64_t off, int64_t width, int family, int center)
-{
-  __shared__ float xs[320];
-  __shared__ long long keys[512];
-  __shared__ unsigned ncand;
-  __shared__ float xstat[2];
-  const int tid = threadIdx.x;
-  const unsigned total = *dirty_cnt;
-  for (unsigned d = blockIdx.x; d < total; d += gridDim.x) {
-    const int64_t row = dirty[d];
-    __syncthreads();
-    if (tid == 0) {
-      float mean = 0.f;
-      if (family == 1 && center) {
-        for (int t = 0; t < k; ++t) mean += x[row * ldx + t];
-        mean /= static_cast<float>(k);
-      }
-      float nx = 0.f;
-      for (int t = 0; t < k; ++t) { const float v = x[row * ldx + t] - mean; nx = fmaf(v, v, nx); }
-      xstat[0] = mean; xstat[1] = nx;
-    }
-    __syncthreads();
-    for (int t = tid; t < k; t += 256) xs[t] = x[row * ldx + t] - xstat[0];
-    // the row's top-k without what this pass had put in
-    for (int t = tid; t < 512; t += 256) {
-      long long key = KEY_EMPTY;
-      if (t < kk) {
-        key = topk[row * kk + t];
-        const long long j = key_index(key);
-        if (key != KEY_EMPTY && j >= off && j < off + width) key = KEY_EMPTY;
-      }
-      keys[t] = key;
-    }
-    if (tid == 0) ncand = 0u;
-    __syncthreads();
-    for (int64_t j0 = 0; j0 < width; j0 += 256) {
-      // (the k-th best of what is in keys[0, kk) bounds what can still enter; unsorted holes are +max)
-      long long kth = 0;
-      for (int t = 0; t < kk; ++t) kth = max(kth, keys[t]);
-      const int64_t j = j0 + tid;
-      bool appended   = false;
-      if (j < width) {
-        const float* yr = y + (off + j) * ldy;
-        float val;
-        if (family == 0) {
-          float acc = 0.f;
-          for (int t = 0; t < k; ++t) { const float df = xs[t] - __ldg(yr + t); acc = fmaf(df, df, acc); }
-          val = acc;
-        } else {
-          float my = 0.f;
-          if (center) {
-            for (int t = 0; t < k; ++t) my += __ldg(yr + t);
-            my /= static_cast<float>(k);
-          }
-          float dot = 0.f, ny = 0.f;
-          for (int t = 0; t < k; ++t) { const float b = __ldg(yr + t) - my; dot = fmaf(xs[t], b, dot); ny = fmaf(b, b, ny); }
-          val = 1.f - dot / sqrtf(xstat[1] * ny);
-        }
-        const long long key = key_pack(val, off + j);
-        if (key < kth && val == val) {   // (kk + 256 <= 320 < 512)
-          keys[kk + atomicAdd(&ncand, 1u)] = key;
-          appended = true;
-        }
-      }
-      // the branch must be block-uniform: a thread that read ncand after a barrier could see the next iteration's
-      // atomicAdd of a faster warp, so the decision comes from the barrier itself
-      if (__syncthreads_or(appended)) {   // block-wide bitonic sort of the 512 slots, smallest first
-        for (int size = 2; size <= 512; size <<= 1)
-          for (int stride = size >> 1; stride > 0; stride >>= 1) {
-            const int t = tid;
-            const int i = 2 * t - (t & (stride - 1)), jj = i + stride;
-            const bool up = (i & size) == 0;
-            const long long a = keys[i], c = keys[jj];
-            if ((a > c) == up) { keys[i] = c; keys[jj] = a; }
-            __syncthreads();
-          }
-        for (int t = kk + tid; t < 512; t += 256) keys[t] = KEY_EMPTY;
-        if (tid == 0) ncand = 0u;
-        __syncthreads();
-      }
-    }
-    // final order (holes from the removed entries may have left the first kk slots unsorted)
-    for (int size = 2; size <= 512; size <<= 1)
-      for (int stride = size >> 1; stride > 0; stride >>= 1) {
-        const int t = tid;
-        const int i = 2 * t - (t & (stride - 1)), jj = i + stride;
-        const bool up = (i & size) == 0;
-        const long long a = keys[i], c = keys[jj];
-        if ((a > c) == up) { keys[i] = c; keys[jj] = a; }
-        __syncthreads();
-      }
-    for (int t = tid; t < kk; t += 256) topk[row * kk + t] = keys[t];
-    if (tid == 0) thr[row] = key_bound(keys[kk - 1]);
-  }
-}
-
-// sorted packed keys -> (index, distance) arrays: clamp at 0, optional sqrt
-__global__ void knn_finalize_kernel(int64_t* out_idx, float* out_dist, const long long* topk, int64_t total, int do_sqrt)
-{
-  const int64_t i = static_cast<int64_t>(blockIdx.x) * blockDim.x + threadIdx.x;
-  if (i >= total) return;
-  const long long key = topk[i];
-  float d             = key_dist(key);
-  d                   = d < 0.f ? 0.f : d;  // NaN propagates
-  if (do_sqrt) d = sqrtf(d);
-  out_idx[i]  = key == KEY_EMPTY ? -1 : static_cast<int64_t>(key_index(key));
-  out_dist[i] = key == KEY_EMPTY ? __int_as_float(0x7f800000) : d;
 }
 
 }  // namespace b2d

@@ -1,4 +1,4 @@
-// Masked fusedL2NN (b2d_masked_l2_nn in api.cu; raft::distance::masked_l2_nn, the 1-NN step of connect_components):
+// Masked fusedL2NN (b2d_masked_l2_nn in nearest.cu; raft::distance::masked_l2_nn, the 1-NN step of connect_components):
 // for every row i of x the nearest row j of y among the rows whose group g has adj[i, g] != 0.  Group g holds the rows
 // [group_idxs[g-1], group_idxs[g]) of y (group_idxs[-1] = 0); rows at or after group_idxs[G-1] are in no group.
 //
@@ -8,10 +8,11 @@
 //                            finalisation then writes NaN / 0x7fffffff to every row, masked_poison_kernel)
 //   masked_group_map_kernel  [n] group of every row of y (-1: none)
 //   masked_adj_bits_kernel   the caller's byte matrix adj [m][G] as bits [ceil(m/32)][G]
-//   masked_classify_kernel   per (x tile, y block) one byte of four tile classes (expanded_tc.cuh MaskClass)
+//   masked_classify_kernel   per (x tile, y block) one byte of four tile classes (tc_params.cuh MaskClass)
 #pragma once
 #include <cstdint>
-#include "expanded_tc.cuh"
+#include "nn_key.cuh"
+#include "tc_params.cuh"
 
 namespace b2d {
 

@@ -29,4 +29,10 @@ __device__ __forceinline__ float key_bound(long long key)
   return d;
 }
 
+// raft::KeyValuePair<int, float> as the 1-NN entry points write it
+struct KvpIF {
+  int key;
+  float value;
+};
+
 }  // namespace b2d

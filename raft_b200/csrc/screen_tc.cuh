@@ -1,6 +1,6 @@
 // K3b: coarse screening pass of the screened fusedL2NN (sm_90a, wgmma).
 //
-// fused_nn_keys (api.cu) first runs the exact arg-min kernel on every S-th 256-row block of y, which
+// fused_nn_keys (nearest.cu) first runs the exact arg-min kernel on every S-th 256-row block of y, which
 // leaves each x row with an upper bound U_i of its minimum.  This kernel visits the other blocks with
 // ONE tensor product per k-block (hi*hi only: a third of the exact kernel's MMA work, half of its
 // operand bytes) and computes, per pair, a rigorous LOWER bound of the fp32-grade distance
@@ -13,7 +13,7 @@
 // is a per-row constant inside a y block, so it moves into the row's threshold.  The element loop does not even form
 // L_ij: it bounds the thread's 8 values of a 32-column group G by  c max acc_ij + min_{j in G} |y_j|^2 (1 - 2^-21)
 // (c < 0), and only a group that reaches the threshold is looked at column by column.  The database chunk is packed
-// in the order of |y_j|^2 (api.cu), which makes the group bound as good as the per-column one and the per-block
+// in the order of |y_j|^2 (nearest.cu), which makes the group bound as good as the per-column one and the per-block
 // margin (max_j' |y_j'|) local; `col_map` translates a packed position back to the caller's row where an index
 // leaves the kernel.
 //

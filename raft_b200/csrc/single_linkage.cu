@@ -1,0 +1,388 @@
+// Minimum spanning forest and single-linkage clustering (single_linkage.cuh).
+#include <cuda_runtime.h>
+#include <algorithm>
+#include <string>
+#include <vector>
+#include <cub/device/device_radix_sort.cuh>
+
+#include "host.cuh"
+#include "single_linkage.cuh"
+
+using namespace b2d;
+
+// ------------------------------------------------------------------------------------------
+// Minimum spanning forest and single-linkage clustering (single_linkage.cuh): edge-list Borůvka under the key order
+// key_pack(w, e); single_linkage runs it on the kNN graph, connects the components the graph leaves apart with the
+// masked arg-min, and builds the dendrogram on the host.
+namespace {
+constexpr int64_t kSlMaxRows  = 1ll << 30;
+constexpr int64_t kSlMaxEdges = 0xFFFFFFFFll;   // positions are the low 32 bits of a key (2^32 - 1 only in KEY_EMPTY)
+
+struct MstLayout {
+  SlCtrl* ctrl;
+  int* colour;        // [n] component of every vertex (the id of a vertex of it)
+  int* parent;        // [n] hook forest of the components of a round; at the end the smallest vertex of each tree
+  long long* best;    // [n] minimum key of every component in a round
+  long long* keys;    // [n] keys of the forest edges in the order they were chosen (KEY_EMPTY behind them)
+  long long* alt;     // [n] the other buffer of the radix sort
+  void* sort_tmp;
+  size_t sort_bytes;
+  size_t bytes;
+};
+
+static MstLayout mst_regions(Carve& c, int64_t n)
+{
+  MstLayout L{};
+  L.ctrl       = c.take<SlCtrl>(1);
+  L.colour     = c.take<int>(n);
+  L.parent     = c.take<int>(n);
+  L.best       = c.take<long long>(n);
+  L.keys       = c.take<long long>(n);
+  L.alt        = c.take<long long>(n);
+  L.sort_bytes = kSortTmpBytes + static_cast<size_t>(n) * 4;   // (checked at run time)
+  L.sort_tmp   = c.take<char>(L.sort_bytes);
+  L.bytes      = c.bytes;
+  return L;
+}
+
+static MstLayout mst_layout(void* base, int64_t n)
+{
+  Carve c(base, 1024);
+  return mst_regions(c, n);
+}
+
+static int ceil_log2(int64_t n)
+{
+  int r = 0;
+  while ((1ll << r) < n) ++r;
+  return r;
+}
+
+// Borůvka rounds over the edges [e0, e1) of a graph on n vertices with at most `comps` components, every other edge
+// already inside a component.  Only enqueues: the non-isolated components at least halve in every round, so
+// ceil(log2 comps) rounds finish, and every kernel after a round that appended nothing returns at once.
+static int mst_rounds(cudaStream_t s, const MstLayout& L, const int* src, const int* dst, const float* w, int64_t n,
+                      int64_t e0, int64_t e1, int64_t comps)
+{
+  const int rounds = ceil_log2(comps) + 1;
+  const int jumps  = std::min(kSlMaxJumps, ceil_log2(comps) + 1);   // hook chains are shorter than comps
+  const unsigned ge = static_cast<unsigned>(std::max<int64_t>(1, std::min<int64_t>((e1 - e0 + 255) / 256, 1 << 16)));
+  for (int r = 0; r < rounds; ++r) {
+    sl_round_begin_kernel<<<sl_grid(std::max<int64_t>(n, kSlMaxJumps)), 256, 0, s>>>(L.ctrl, L.best, n);
+    sl_edge_kernel<<<ge, 256, 0, s>>>(L.ctrl, src, dst, w, e0, e1, n, L.colour, L.best);
+    sl_hook_kernel<<<sl_grid(n), 256, 0, s>>>(L.ctrl, src, dst, L.colour, L.best, L.parent, L.keys, n);
+    for (int j = 0; j < jumps; ++j) sl_jump_kernel<<<sl_grid(n), 256, 0, s>>>(L.ctrl, L.colour, L.parent, n, j);
+    sl_relabel_kernel<<<sl_grid(n), 256, 0, s>>>(L.ctrl, L.colour, L.parent, n);
+    sl_round_end_kernel<<<1, 1, 0, s>>>(L.ctrl);
+    B2D_CUDA(cudaGetLastError());
+  }
+  return B2D_OK;
+}
+
+// the forest edges in key order: endpoints, weights (their square roots with do_sqrt) and the count
+static int mst_emit(cudaStream_t s, const MstLayout& L, const int* src, const int* dst, const float* w, int64_t n,
+                    int do_sqrt, int* out_src, int* out_dst, float* out_w, int* out_count)
+{
+  cub::DoubleBuffer<long long> db(L.keys, L.alt);
+  size_t need = 0;
+  B2D_CUDA(cub::DeviceRadixSort::SortKeys(nullptr, need, db, static_cast<int>(n), 0, 64, s));
+  if (need > L.sort_bytes) return fail(B2D_ERR_WORKSPACE, "internal: radix sort scratch " + std::to_string(need) + " bytes");
+  B2D_CUDA(cub::DeviceRadixSort::SortKeys(L.sort_tmp, need, db, static_cast<int>(n), 0, 64, s));
+  sl_emit_kernel<<<sl_grid(n), 256, 0, s>>>(L.ctrl, db.Current(), src, dst, w, std::max<int64_t>(n - 1, 0), do_sqrt,
+                                            out_src, out_dst, out_w, out_count);
+  B2D_CUDA(cudaGetLastError());
+  return B2D_OK;
+}
+
+// kNN neighbours of single_linkage: min(m, max(2, floor(log2 m) + c))
+static int64_t sl_neighbors(int64_t m, int64_t c)
+{
+  if (m < 1) return 0;
+  const int64_t fl = 63 - __builtin_clzll(static_cast<unsigned long long>(m));
+  return std::min<int64_t>(m, std::max<int64_t>(2, fl + c));
+}
+
+// Rows of x per masked arg-min launch of connect_components: the m x c adjacency bytes (and its m c / 8 bytes of bits)
+// stay below 128 m, and the tile classes below 64 MiB; a multiple of TC_BM, at least TC_BM (c <= m).
+static int64_t sl_max_chunk(int64_t m)
+{
+  const int64_t mm = std::max<int64_t>(m, 1);
+  const int64_t cap = std::max<int64_t>(TC_BM, ((1ll << 40) / mm) / TC_BM * TC_BM);
+  return std::min<int64_t>((mm + TC_BM - 1) / TC_BM * TC_BM, cap);
+}
+
+static int64_t sl_chunk_rows(int64_t m, int64_t c)
+{
+  const int64_t r = std::max<int64_t>(TC_BM, (128 * m / std::max<int64_t>(c, 1)) / TC_BM * TC_BM);
+  return std::min(r, sl_max_chunk(m));
+}
+
+// Persistent regions first (the forest, the edge list, the host copies), then one scratch region used by the kNN phase
+// and, afterwards, by connect_components.  Sized for any number of components up to m, so the workspace depends on
+// (m, d, n_nb) only.
+struct SlLayout {
+  MstLayout mst;            // over the m rows
+  int *src, *dst;           // [m n_nb + m] edge list: the kNN graph (position i n_nb + s), then the connecting edges
+  float* w;                 //              squared L2 weights
+  int *hsrc, *hdst;         // [m] forest edges in key order, for the host
+  void* knn_ws;             // kNN phase: b2d_knn's workspace, then its outputs
+  size_t knn_bytes;
+  int64_t* idx;             // [m n_nb]
+  float* dist;              // [m n_nb]
+  TcWorkspace tc;           // connect phase: the colour-sorted rows as both operands
+  float* xs;                // [m, d] the colour-sorted rows
+  long long *keys, *cbest;  // [m] masked arg-min of every sorted row, [c] best row of every component
+  unsigned* bad;            // [8] masked_classify's flag: 0 (the component ends are valid by construction)
+  int *grp, *lab, *ends;    // [m]
+  unsigned* ids;            // [m] root flags, scanned into dense component ids
+  KmSort sort;              // the rows sorted by component, for up to m components
+  unsigned* bits;           // [5 m] adjacency bits of one chunk
+  uint8_t* cls;             // tile classes of one chunk
+  uint8_t* adj;             // [128 m] adjacency of one chunk
+  size_t bytes;
+};
+
+static SlLayout sl_layout(void* base, int64_t m, int64_t d, int64_t n_nb)
+{
+  Carve c(base, 1024);
+  SlLayout L{};
+  L.mst  = mst_regions(c, m);
+  const size_t ne = static_cast<size_t>(m) * n_nb + m;
+  L.src  = c.take<int>(ne);
+  L.dst  = c.take<int>(ne);
+  L.w    = c.take<float>(ne);
+  L.hsrc = c.take<int>(m);
+  L.hdst = c.take<int>(m);
+  char* scratch = base ? static_cast<char*>(base) + c.bytes : nullptr;
+  // kNN phase
+  const KnnLayout K = knn_layout(nullptr, m, m, d, n_nb);
+  Carve a(scratch, 1024);
+  L.knn_ws    = a.take<char>(K.bytes);
+  L.knn_bytes = K.bytes;
+  L.idx       = a.take<int64_t>(static_cast<size_t>(m) * n_nb);
+  L.dist      = a.take<float>(static_cast<size_t>(m) * n_nb);
+  // connect phase
+  Carve b(scratch, 1024);
+  L.tc    = tc_layout(b, m, m, d, false);
+  L.xs    = b.take<float>(static_cast<size_t>(m) * d);
+  L.keys  = b.take<long long>(m);
+  L.cbest = b.take<long long>(m);
+  L.bad   = b.take<unsigned>(8);
+  L.grp   = b.take<int>(m);
+  L.lab   = b.take<int>(m);
+  L.ends  = b.take<int>(m);
+  L.ids   = b.take<unsigned>(m);
+  L.sort  = km_sort_regions(b, m, m, true);
+  const int64_t mm = std::max<int64_t>(m, 1);
+  L.bits  = b.take<unsigned>(static_cast<size_t>(5) * mm);
+  L.cls   = b.take<uint8_t>(static_cast<size_t>(sl_max_chunk(m) / TC_BM) * ((mm + TC_BN - 1) / TC_BN));
+  L.adj   = b.take<uint8_t>(static_cast<size_t>(128) * mm);
+  L.bytes = c.bytes + std::max(a.bytes, b.bytes);
+  return L;
+}
+
+// One round of connect_components for c > 1 components: dense component ids, the rows sorted by component (stable),
+// the masked arg-min of every sorted row against the rows of other components in row chunks, and for every component
+// the edge from its row of smallest (distance, row) to that row's nearest row: edges [e0, e0 + c).
+static int sl_connect(cudaStream_t s, const SlLayout& L, const float* x, int64_t ldx, int64_t m, int64_t d, int64_t c,
+                      int64_t e0)
+{
+  const MstLayout& T = L.mst;
+  const KmSort& S = L.sort;
+  sl_root_flags_kernel<<<sl_grid(m), 256, 0, s>>>(T.colour, L.ids, m);
+  int rc = km_scan(s, nullptr, L.ids, m, S.tiles, S.ctrl);
+  if (rc) return rc;
+  sl_dense_label_kernel<<<sl_grid(m), 256, 0, s>>>(T.colour, L.ids, L.lab, m);
+  B2D_CUDA(cudaGetLastError());
+  const KmSortPlan P = km_sort_plan(m, c);
+  rc = km_sort_count(s, S, P, L.lab, m, c);
+  if (rc) return rc;
+  rc = km_sort_scatter(s, nullptr, S, P, L.lab, m, c);
+  if (rc) return rc;
+  sl_ends_kernel<<<sl_grid(c), 256, 0, s>>>(S.hist, P.nblk, c, L.ends);
+  km_gather_rows(s, static_cast<unsigned>(m), x, ldx, static_cast<int>(d), S.perm, static_cast<int>(m), L.xs);
+  B2D_CUDA(cudaGetLastError());
+  // y (and x) prepared once per round; every chunk takes a window of the x side
+  rc = launch_prep<float>(s, L.tc, L.xs, d, 1, m, L.xs, d, 1, m, d, nullptr, nullptr, PREP_L2, 0);
+  if (rc) return rc;
+  masked_group_map(s, sl_grid(m), L.grp, L.ends, c, m);
+  B2D_CUDA(cudaMemsetAsync(L.bad, 0, 32, s));
+  minloc_init(s, sl_grid(m), L.keys, m);
+  minloc_init(s, sl_grid(c), L.cbest, c);
+  B2D_CUDA(cudaGetLastError());
+  const int64_t mc = sl_chunk_rows(m, c);
+  for (int64_t r0 = 0; r0 < m; r0 += mc) {
+    const int64_t rows = std::min(mc, m - r0);
+    sl_adj_kernel<<<km_grid(rows * c), 256, 0, s>>>(S.slab, r0, rows, c, L.adj);
+    B2D_CUDA(cudaGetLastError());
+    rc = masked_keys(s, tc_rows(L.tc, 0, r0, d), L.keys + r0, L.grp, L.bits, L.cls, L.bad, L.adj, c, L.ends, c, rows, m, d);
+    if (rc) return rc;
+  }
+  sl_comp_best_kernel<<<sl_grid(m), 256, 0, s>>>(L.keys, S.slab, m, L.cbest);
+  sl_connect_kernel<<<sl_grid(c), 256, 0, s>>>(L.cbest, L.keys, S.perm, S.slab, c, e0, L.src, L.dst, L.w, T.ctrl);
+  B2D_CUDA(cudaGetLastError());
+  return B2D_OK;
+}
+
+static int sl_read_ctrl(cudaStream_t s, const SlCtrl* d, SlCtrl* h)
+{
+  B2D_CUDA(cudaMemcpyAsync(h, d, sizeof(SlCtrl), cudaMemcpyDeviceToHost, s));
+  B2D_CUDA(cudaStreamSynchronize(s));
+  return B2D_OK;
+}
+
+static int uf_find(std::vector<int>& p, int v)
+{
+  while (p[v] != v) v = p[v] = p[p[v]];
+  return v;
+}
+}  // namespace
+
+size_t b2d_mst_workspace_bytes(int64_t n_vertices, int64_t n_edges)
+{
+  if (n_vertices < 0 || n_edges < 0) return static_cast<size_t>(-1);
+  return mst_layout(nullptr, n_vertices).bytes;
+}
+
+int b2d_mst(void* stream, const int32_t* src, const int32_t* dst, const float* w, int64_t n_vertices, int64_t n_edges,
+            int32_t* out_src, int32_t* out_dst, float* out_w, int32_t* out_colour, int32_t* out_count, void* workspace,
+            size_t workspace_bytes)
+{
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  const int64_t n = n_vertices, E = n_edges;
+  if (n < 0 || E < 0) return fail(B2D_ERR_INVALID_ARG, "negative extent");
+  if (n >= kSlMaxRows) return fail(B2D_ERR_UNSUPPORTED, "mst: n_vertices must be below 2^30");
+  if (E >= kSlMaxEdges) return fail(B2D_ERR_UNSUPPORTED, "mst: n_edges must be below 2^32 - 1");
+  if (E > 0 && (!src || !dst || !w)) return fail(B2D_ERR_INVALID_ARG, "null src / dst / w");
+  if (!out_count || (n > 0 && !out_colour) || (n > 1 && (!out_src || !out_dst || !out_w)))
+    return fail(B2D_ERR_INVALID_ARG, "null out_src / out_dst / out_w / out_colour / out_count");
+  int rc = check_workspace(workspace, workspace_bytes, mst_layout(nullptr, n).bytes);
+  if (rc) return rc;
+  if (n == 0) {
+    B2D_CUDA(cudaMemsetAsync(out_count, 0, sizeof(int32_t), s));
+    return B2D_OK;
+  }
+  const MstLayout L = mst_layout(workspace, n);
+  sl_mst_init_kernel<<<sl_grid(n), 256, 0, s>>>(L.ctrl, L.colour, L.keys, n);
+  B2D_CUDA(cudaGetLastError());
+  rc = mst_rounds(s, L, src, dst, w, n, 0, E, n);
+  if (rc) return rc;
+  rc = mst_emit(s, L, src, dst, w, n, 0, out_src, out_dst, out_w, out_count);
+  if (rc) return rc;
+  sl_fill_kernel<<<sl_grid(n), 256, 0, s>>>(L.parent, 0x7fffffff, n);
+  sl_min_vertex_kernel<<<sl_grid(n), 256, 0, s>>>(L.colour, L.parent, n);
+  sl_colour_out_kernel<<<sl_grid(n), 256, 0, s>>>(L.colour, L.parent, out_colour, n);
+  B2D_CUDA(cudaGetLastError());
+  return B2D_OK;
+}
+
+size_t b2d_single_linkage_workspace_bytes(int64_t m, int64_t d, int c)
+{
+  if (m < 0 || d < 0) return static_cast<size_t>(-1);
+  const int64_t n_nb = sl_neighbors(m, c);
+  if (n_nb > KNN_MAX_K || m >= kSlMaxRows) return static_cast<size_t>(-1);
+  return sl_layout(nullptr, m, d, n_nb).bytes;
+}
+
+int b2d_single_linkage(void* stream, int metric, const float* x, int64_t ldx, int64_t m, int64_t d, int c, int n_clusters,
+                       int32_t* children, float* deltas, int32_t* sizes, int32_t* labels, int32_t* n_components_out,
+                       void* workspace, size_t workspace_bytes)
+{
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  if (metric != B2D_L2Expanded && metric != B2D_L2SqrtExpanded)
+    return fail(B2D_ERR_UNSUPPORTED, "single_linkage supports the L2Expanded and L2SqrtExpanded metrics");
+  if (m < 1 || d < 1) return fail(B2D_ERR_INVALID_ARG, "m and d must be positive");
+  if (d > 320) return fail(B2D_ERR_UNSUPPORTED, "single_linkage supports d <= 320 (the fused kNN's limit)");
+  if (m >= kSlMaxRows) return fail(B2D_ERR_UNSUPPORTED, "single_linkage: m must be below 2^30");
+  if (n_clusters < 1 || n_clusters > m) return fail(B2D_ERR_INVALID_ARG, "n_clusters must be in [1, m]");
+  const int64_t n_nb = sl_neighbors(m, c);
+  if (n_nb > KNN_MAX_K)
+    return fail(B2D_ERR_UNSUPPORTED, "single_linkage: min(m, max(2, floor(log2 m) + c)) = " + std::to_string(n_nb) +
+                                         " neighbours exceeds 64: lower c (" + std::to_string(c) + ")");
+  if (m * n_nb + m >= kSlMaxEdges)
+    return fail(B2D_ERR_UNSUPPORTED, "single_linkage: m * (n_nb + 1) edges must stay below 2^32 - 1");
+  if (!x || !labels || !n_components_out || (m > 1 && (!children || !deltas || !sizes)))
+    return fail(B2D_ERR_INVALID_ARG, "null x / children / deltas / sizes / labels / n_components_out");
+  if (ldx < d) return fail(B2D_ERR_INVALID_ARG, "leading dimension smaller than d");
+  int rc = check_workspace(workspace, workspace_bytes, sl_layout(nullptr, m, d, n_nb).bytes);
+  if (rc) return rc;
+  const SlLayout L = sl_layout(workspace, m, d, n_nb);
+  const MstLayout& T = L.mst;
+  SlCtrl h;
+  sl_mst_init_kernel<<<sl_grid(m), 256, 0, s>>>(T.ctrl, T.colour, T.keys, m);
+  sl_finite_kernel<<<km_grid(m * d), 256, 0, s>>>(x, ldx, m, static_cast<int>(d), T.ctrl);
+  B2D_CUDA(cudaGetLastError());
+  // 1. the kNN graph (squared distances, whatever the metric)
+  if (m > 1) {
+    rc = b2d_knn(s, L.idx, L.dist, B2D_L2Expanded, x, ldx, x, ldx, m, m, d, n_nb, L.knn_ws, L.knn_bytes);
+    if (rc) return rc;
+    sl_knn_edges_kernel<<<sl_grid(m * n_nb), 256, 0, s>>>(L.idx, L.dist, m, static_cast<int>(n_nb), L.src, L.dst, L.w);
+    B2D_CUDA(cudaGetLastError());
+    // 2.-3. its minimum spanning forest
+    rc = mst_rounds(s, T, L.src, L.dst, L.w, m, 0, m * n_nb, m);
+    if (rc) return rc;
+  }
+  rc = sl_read_ctrl(s, T.ctrl, &h);
+  if (rc) return rc;
+  if (h.bad & 1u) return fail(B2D_ERR_INVALID_ARG, "single_linkage: X holds a non-finite value");
+  int64_t comps = m - h.n_mst;
+  *n_components_out = static_cast<int32_t>(comps);
+  // 4. connect_components: each round at least halves the components
+  int64_t e = m * n_nb;
+  while (comps > 1) {
+    rc = sl_connect(s, L, x, ldx, m, d, comps, e);
+    if (rc) return rc;
+    sl_rearm_kernel<<<1, 1, 0, s>>>(T.ctrl);
+    B2D_CUDA(cudaGetLastError());
+    rc = mst_rounds(s, T, L.src, L.dst, L.w, m, e, e + comps, comps);
+    if (rc) return rc;
+    e += comps;
+    rc = sl_read_ctrl(s, T.ctrl, &h);
+    if (rc) return rc;
+    const int64_t next = m - h.n_mst;
+    if ((h.bad & 2u) || 2 * next > comps)
+      return fail(B2D_ERR_CUDA, "internal: connect_components left " + std::to_string(next) + " of " +
+                                    std::to_string(comps) + " components");
+    comps = next;
+  }
+  // 5. dendrogram: the m - 1 forest edges in key order, union-find on the host
+  std::vector<int> hs(m - 1), hd(m - 1);
+  if (m > 1) {
+    rc = mst_emit(s, T, L.src, L.dst, L.w, m, metric == B2D_L2SqrtExpanded ? 1 : 0, L.hsrc, L.hdst, deltas, nullptr);
+    if (rc) return rc;
+    B2D_CUDA(cudaMemcpyAsync(hs.data(), L.hsrc, (m - 1) * sizeof(int), cudaMemcpyDeviceToHost, s));
+    B2D_CUDA(cudaMemcpyAsync(hd.data(), L.hdst, (m - 1) * sizeof(int), cudaMemcpyDeviceToHost, s));
+    B2D_CUDA(cudaStreamSynchronize(s));
+  }
+  std::vector<int> uf(m), cid(m), sz(m, 1), hch(2 * (m - 1)), hsz(m - 1), hlab(m);
+  for (int64_t i = 0; i < m; ++i) uf[i] = cid[i] = static_cast<int>(i);
+  const int64_t cut = m - n_clusters;   // labels: the components after the first m - n_clusters merges
+  for (int64_t t = 0; t < m - 1; ++t) {
+    if (t == cut)
+      for (int64_t i = 0; i < m; ++i) hlab[i] = uf_find(uf, static_cast<int>(i));
+    const int a = uf_find(uf, hs[t]), b = uf_find(uf, hd[t]);
+    if (a == b) return fail(B2D_ERR_CUDA, "internal: the spanning tree has a cycle");
+    hch[2 * t]     = std::min(cid[a], cid[b]);
+    hch[2 * t + 1] = std::max(cid[a], cid[b]);
+    hsz[t]         = sz[a] + sz[b];
+    uf[b]          = a;
+    sz[a]          = hsz[t];
+    cid[a]         = static_cast<int>(m + t);
+  }
+  if (cut == m - 1)
+    for (int64_t i = 0; i < m; ++i) hlab[i] = uf_find(uf, static_cast<int>(i));
+  std::vector<int> num(m, -1);   // numbered in order of each cluster's smallest row
+  int next_label = 0;
+  for (int64_t i = 0; i < m; ++i) {
+    int& l = num[hlab[i]];
+    if (l < 0) l = next_label++;
+    hlab[i] = l;
+  }
+  if (m > 1) {
+    B2D_CUDA(cudaMemcpyAsync(children, hch.data(), hch.size() * sizeof(int), cudaMemcpyHostToDevice, s));
+    B2D_CUDA(cudaMemcpyAsync(sizes, hsz.data(), hsz.size() * sizeof(int), cudaMemcpyHostToDevice, s));
+  }
+  B2D_CUDA(cudaMemcpyAsync(labels, hlab.data(), m * sizeof(int), cudaMemcpyHostToDevice, s));
+  B2D_CUDA(cudaStreamSynchronize(s));
+  return B2D_OK;
+}

@@ -68,7 +68,7 @@ __device__ __forceinline__ void ux_acc(float& acc, float a, float b, float p)
     const float t = a * (__log2f(a) - __log2f(b));
     acc += (a == 0.f) ? 0.f : t;
   } else if (kMetric == UX_KL_REV) {
-    // the column-major entry point computes D^T with x and y exchanged (api.cu); KL is not symmetric,
+    // the column-major entry point computes D^T with x and y exchanged (pairwise.cu); KL is not symmetric,
     // so the kernel accumulates KL(b || a) there -- the reference's !is_row_major branch did the same swap
     const float t = b * (__log2f(b) - __log2f(a));
     acc += (b == 0.f) ? 0.f : t;

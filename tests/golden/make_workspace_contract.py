@@ -10,7 +10,12 @@ The fixtures:
   gram_workspace_contract.json            gram_matrix for every kernel id (and two invalid ones) and dtype;
   single_linkage_workspace_contract.json  single_linkage over row counts from 1 to 10^6 (around the 2048-row sort blocks
                                           and the 2^20-row tile-class cap) and c from -5 to 60 (n_nb from 2 to past 64),
-                                          and the edge-list MST.
+                                          and the edge-list MST;
+  dbscan_workspace_contract.json          dbscan over row counts around the 16-column adjacency pitch and the 256-column
+                                          batch step, every k, and batch sizes from the 2^30 default (0) through the
+                                          256-column floor (1) to one batch of every column; null, short or misaligned
+                                          workspaces for the euclidean, cosine (batched, optional outputs null) and
+                                          sqeuclidean (NaN eps) fits.
 Pointers are fake addresses: the calls must fail in validation, before anything reaches the device.  A case that
 returns B2D_OK or B2D_ERR_CUDA got past validation, so it is refused rather than recorded.  The library is the one
 raft_b200._lib loads (RAFT_B200_LIB selects another build of the same ABI).
@@ -186,11 +191,34 @@ def single_linkage_error_cases(L):
     ]
 
 
+DB_MS = [1, 15, 16, 256, 257, 32768, 100000, 1000000]
+DB_BATCH = [0, 1, 1 << 20, 1 << 26, (1 << 30) + 1, 1 << 40]
+
+
+def dbscan_byte_queries():
+    q = [(m, d, b) for m in DB_MS for d in KS for b in DB_BATCH] + \
+        [(0, 32, 0), (-1, 32, 0), (37, -1, 0), (37, 32, -1)]
+    return {"b2d_dbscan_workspace_bytes": q}
+
+
+def dbscan_error_cases(L):
+    m, d = 5000, 96
+    return [
+        ("dbscan euclidean", "b2d_dbscan_fit", [None, 1, D, d, m, d, 0.5, 5, 0, D, D, D],
+         L.b2d_dbscan_workspace_bytes(m, d, 0), True),
+        ("dbscan cosine batched", "b2d_dbscan_fit", [None, 2, D, d + 3, m, d, 0.1, 1, 1 << 20, D, None, None],
+         L.b2d_dbscan_workspace_bytes(m, d, 1 << 20), True),
+        ("dbscan sqeuclidean NaN eps", "b2d_dbscan_fit", [None, 0, D, d, m, d, float("nan"), 50, 12345, D, D, None],
+         L.b2d_dbscan_workspace_bytes(m, d, 12345), True),
+    ]
+
+
 FIXTURES = {   # file -> (size queries, error cases)
     "workspace_contract.json": (byte_queries, error_cases),
     "kmeans_workspace_contract.json": (kmeans_byte_queries, kmeans_error_cases),
     "gram_workspace_contract.json": (gram_byte_queries, gram_error_cases),
     "single_linkage_workspace_contract.json": (single_linkage_byte_queries, single_linkage_error_cases),
+    "dbscan_workspace_contract.json": (dbscan_byte_queries, dbscan_error_cases),
 }
 
 

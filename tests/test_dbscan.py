@@ -1,6 +1,7 @@
 """DBSCAN without a GPU: the reference (tests/dbscan_ref.py) against sklearn.cluster.DBSCAN on symmetric adjacency and
-against scipy's connected components on asymmetric adjacency, the ABI declarations, the workspace contract
-(tests/golden/dbscan_workspace_contract.json) and the argument checks of the C ABI."""
+against scipy's connected components on asymmetric adjacency, the ABI declarations, the workspace queries and the
+argument checks of the C ABI.  The workspace contract (tests/golden/dbscan_workspace_contract.json) is replayed by
+tests/test_workspace_contract.py."""
 import os
 import re
 
@@ -9,7 +10,7 @@ import pytest
 
 from dbscan_ref import dbscan_ref
 from raft_b200 import _lib
-from test_workspace_contract import SIZE_MAX, load, replay_bytes, replay_errors
+from test_workspace_contract import SIZE_MAX
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 P = 1 << 12   # a non-null pointer that is never dereferenced (every call below fails before any work)
@@ -118,15 +119,6 @@ def test_workspace_queries():
     small, big = L.b2d_dbscan_workspace_bytes(10 ** 5, 32, 1 << 26), L.b2d_dbscan_workspace_bytes(10 ** 5, 32, 1 << 30)
     assert big - small >= (1 << 30) - (1 << 26) - 10 ** 5 * 256
     assert L.b2d_dbscan_workspace_bytes(1000, 32, 0) >= 1000 * 1008   # one batch, pitch rounded up to 16
-
-
-def test_workspace_contract():
-    contract = load("dbscan_workspace_contract.json")
-    rows = replay_bytes(contract, "b2d_dbscan_workspace_bytes")
-    for *args, want in rows:
-        if min(args) < 0:
-            assert want == SIZE_MAX, args
-    assert replay_errors(contract) == 9
 
 
 def fit(metric=L2SQRT, x=P, ldx=8, m=100, d=8, eps=0.5, ms=5, mb=0, lab=P, csi=P, ncl=P, ws=P * 256, wsb=1 << 40):

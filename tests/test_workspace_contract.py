@@ -1,8 +1,8 @@
 """CPU tier: the workspace contract of the C ABI against the fixtures under tests/golden (all recorded by
 tests/golden/make_workspace_contract.py): the byte count of every *_workspace_bytes query over a grid that reaches every
 branch of the layouts, and the status and message of every entry point given a null, short or misaligned workspace.
-workspace_contract.json covers distances, nearest neighbours, select_k and the stats; the k-means, gram_matrix and
-single-linkage entry points have a fixture each."""
+workspace_contract.json covers distances, nearest neighbours, select_k and the stats; the k-means, gram_matrix,
+single-linkage and DBSCAN entry points have a fixture each."""
 import json
 import os
 
@@ -94,3 +94,14 @@ def test_mst_workspace_bytes():
 
 def test_single_linkage_workspace_errors():
     assert replay_errors(load("single_linkage_workspace_contract.json")) == 9
+
+
+def test_dbscan_workspace_bytes():
+    rows = replay_bytes(load("dbscan_workspace_contract.json"), "b2d_dbscan_workspace_bytes")
+    for *args, want in rows:
+        if min(args) < 0:
+            assert want == SIZE_MAX, args
+
+
+def test_dbscan_workspace_errors():
+    assert replay_errors(load("dbscan_workspace_contract.json")) == 9
