@@ -153,20 +153,24 @@ __global__ void __launch_bounds__(256) nn_exact_kernel(long long* keys, const in
       for (int o = 16; o > 0; o >>= 1) acc += __shfl_xor_sync(0xffffffffu, acc, o);
       res = acc;
     } else {
-      float mx = 0.f, my = 0.f;
+      // fp64 throughout, rounded once: like prep (which normalises in fp64), the result does not depend on the scale
+      // of the rows.  In fp32, nx * ny overflows for rows of norm ~2^32 and underflows for ~2^-32 (a distance of 1, or
+      // below 0, for every candidate of such a row); in fp64 every power-of-two scale of an fp32 row stays in range.
+      double mx = 0.0, my = 0.0;
       if (center) {
-        float sx = (xv[0] + xv[1]) + (xv[2] + xv[3]), sy = (yv[0] + yv[1]) + (yv[2] + yv[3]);
+        double sx = (static_cast<double>(xv[0]) + xv[1]) + (static_cast<double>(xv[2]) + xv[3]);
+        double sy = (static_cast<double>(yv[0]) + yv[1]) + (static_cast<double>(yv[2]) + yv[3]);
 #pragma unroll
         for (int o = 16; o > 0; o >>= 1) { sx += __shfl_xor_sync(0xffffffffu, sx, o); sy += __shfl_xor_sync(0xffffffffu, sy, o); }
-        mx = sx / static_cast<float>(k);
-        my = sy / static_cast<float>(k);
+        mx = sx / k;
+        my = sy / k;
       }
-      float dot = 0.f, nx = 0.f, ny = 0.f;
+      double dot = 0.0, nx = 0.0, ny = 0.0;
 #pragma unroll
       for (int u = 0; u < 4; ++u) {
-        const bool in = lane + 32 * u < k;
-        const float a = in ? xv[u] - mx : 0.f, b = in ? yv[u] - my : 0.f;
-        dot = fmaf(a, b, dot); nx = fmaf(a, a, nx); ny = fmaf(b, b, ny);
+        const bool in  = lane + 32 * u < k;
+        const double a = in ? xv[u] - mx : 0.0, b = in ? yv[u] - my : 0.0;
+        dot = fma(a, b, dot); nx = fma(a, a, nx); ny = fma(b, b, ny);
       }
 #pragma unroll
       for (int o = 16; o > 0; o >>= 1) {
@@ -174,7 +178,7 @@ __global__ void __launch_bounds__(256) nn_exact_kernel(long long* keys, const in
         nx += __shfl_xor_sync(0xffffffffu, nx, o);
         ny += __shfl_xor_sync(0xffffffffu, ny, o);
       }
-      res = 1.f - dot / sqrtf(nx * ny);
+      res = static_cast<float>(1.0 - dot / sqrt(nx * ny));
     }
     if (lane == 0) atomicMin(&keys[ij.x], key_pack(res, static_cast<long long>(ij.y) + idx_offset));
   }

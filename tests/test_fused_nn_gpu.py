@@ -294,7 +294,7 @@ def test_screened_nn_ragged_last_run_of_tiles():
 @pytest.mark.parametrize("kind", ["blobs", "gauss"])
 def test_screened_cosine_family_nn(metric, shape, kind):
     """The screened search also serves the cosine family: rows are unit vectors after prep, the screen's
-    margin is 1.05 * 2^-10 and the candidates are re-measured as 1 - <x', y'> / (|x'||y'|) in fp32."""
+    margin is 1.05 * 2^-10 and the candidates are re-measured as 1 - <x', y'> / (|x'||y'|) in fp64."""
     m, n, k = shape
     if kind == "blobs":
         x, y = blobs(m, n, k, seed=21)
