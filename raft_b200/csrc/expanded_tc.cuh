@@ -52,10 +52,15 @@
 //   EPI_EPS           epsilon neighbourhood: the EPI_STORE / POST_CLAMP distance, compared with eps; the 0/1 bytes go to
 //                     the EPI_STORE staging ring (one 64 x 128-byte box per tile), leave from there by TMA or a copy, and
 //                     are counted per column into shared memory (tc_eps_tile).
+//
+// Diagnostic builds (DESIGN.md section 5, scripts/tc_breakdown.py; never the library's own build): B2D_TC_DIAG = 1 keeps
+// the MMAs only (no epilogue, no staging; one sum of the accumulators keeps them live), 2 computes and stages every value
+// but issues no TMA store, 3 skips the MMAs (stages zeros, TMA stores on).  The results are wrong by design.
 #pragma once
 #include <cuda.h>
 #include <cuda_runtime.h>
 #include <cstdint>
+#include <type_traits>
 #include "nn_key.cuh"
 #include "ptx.cuh"
 #include "tc_params.cuh"
@@ -320,43 +325,80 @@ __device__ __forceinline__ void tc_epilogue(float (&v)[64], const TcParams& p, c
   }
 }
 
+// EPI_STORE through TMA, the common case (one warp-uniform test in the kernel: p.tma_store, p.acc_mode == 0, no diag_zero,
+// no per-column scales): tc_epilogue's arithmetic for it, without the branches of the other cases.  Ragged tiles take it
+// too: TMA clips what lies outside the matrix.  The kernel keeps the Gram matrices off it (kFastPost): a second inlined
+// copy of their expf / tanhf made the tanh instantiation spill.
+template <int kPost>
+__device__ __forceinline__ void tc_epilogue_store_fast(float (&v)[64], const TcParams& p, const float* col_tb, int cl0,
+                                                       const float (&ta)[2], const float (&cfr)[2])
+{
+#pragma unroll
+  for (int i = 0; i < 16; ++i) {
+    const float2 tb = *reinterpret_cast<const float2*>(&col_tb[cl0 + 8 * i]);
+#pragma unroll
+    for (int j = 0; j < 2; ++j)
+#pragma unroll
+      for (int e = 0; e < 2; ++e) {
+        float& d      = v[4 * i + 2 * j + e];
+        const float s = ta[j] + (e ? tb.y : tb.x);
+        if constexpr (tc_post_ratio(kPost)) d = post_ratio<kPost>(d * cfr[j], s);
+        else d = fmaf(d, cfr[j], s);
+        if constexpr (tc_post_clamps(kPost)) d = clamp0(d);
+        if constexpr (kPost == POST_CLAMP_SQRT) asm("sqrt.approx.f32 %0, %1;" : "=f"(d) : "f"(d));
+        if constexpr (tc_post_gram(kPost)) d = gram_post<kPost>(d, p.gamma, p.coef0, p.degree);
+      }
+  }
+}
+
 // EPI_STORE through TMA: the warpgroup's finished 64 x 128 tile v (fragment layout as in tc_epilogue) is written into
-// its ring of staging boxes and stored with one cp.async.bulk.tensor per 64 x 32 box (L2 evict-first: the result is not
-// read again here).  Only this warpgroup writes its boxes and only its lead thread (`issuer`) issues and waits for their
-// stores, so a box is rewritten only after that thread has seen the box's previous store finish reading it and the
-// warpgroup has passed its named barrier.  Boxes outside the matrix are skipped; TMA clips the ragged ones.  After the
-// CTA's last tile (`last`) the issuer waits for all its stores, so the CTA's shared memory outlives them.
+// its ring of two staging boxes and stored with one cp.async.bulk.tensor per 64 x 32 box (L2 evict-first: the result is
+// not read again here).  The tile's 4 boxes go out as two pairs, one box per slot: the lead thread (`issuer`) waits until
+// the previous pair's stores have finished reading both slots, the warpgroup meets at its named barrier, writes the pair,
+// fences it for the TMA unit once and meets again, and the lead issues both stores as one bulk group.  One fence (MEMBAR +
+// FENCE.VIEW.ASYNC in the SASS) and two barriers per pair measured faster than a fence per box or a per-slot mbarrier
+// hand-off (DESIGN.md section 5).  Only this warpgroup writes its boxes and only its lead issues and waits for their
+// stores.  Boxes outside the matrix are skipped; TMA clips the ragged ones.  After the CTA's last tile (`last`) the
+// issuer waits for all its stores, so the CTA's shared memory outlives them.
 //   box element (r, c) sits at byte r * 128 + ((c / 4) ^ (r % 8)) * 16 + (c % 4) * 4 (SWIZZLE_128B): the warp's 8-byte
 //   writes (8 rows x 2 adjacent 16-byte chunks) cover every bank exactly twice -- no conflicts.
 __device__ __forceinline__ void tc_stage_store(const float (&v)[64], const CUtensorMap* tmap_d, uint32_t stg, bool issuer,
                                                bool last, int wg, int64_t row_w, int64_t col_w, const TcParams& p)
 {
-  static_assert(TC_STG_BOXES == 2, "one box per barrier pair, slot = box parity, wait_group.read 1");
+  static_assert(TC_STG_BOXES == 2, "a pair of boxes fills the ring: wait_group.read 0 frees it");
   const int lane       = threadIdx.x & 31;
   const int quad = lane >> 2, tq = lane & 3;
   // this thread's rows 16 w + quad (+8) of the box and the swizzled 16-byte chunk of its column pair
   const uint32_t t_off = (16 * ((threadIdx.x >> 5) & 3) + quad) * 128 + 8 * (tq & 1);
   const uint32_t t_xor = static_cast<uint32_t>((tq >> 1) ^ quad) * 16;
 #pragma unroll
-  for (int b = 0; b < 4; ++b) {   // the tile's 4 boxes of 32 columns; a tile is 4 boxes, so box b uses slot b % 2
-    const uint32_t box = stg + (b & 1) * TC_D_BOX_BYTES;
-    // the store issued two boxes ago read this slot: it must be done (the latest store may still be reading)
-    if (issuer) ptx::tma_store_wait_read<1>();
+  for (int q = 0; q < 2; ++q) {   // the tile's 4 boxes of 32 columns as two pairs: box 2 q + s in slot s
+    // the previous pair's stores have read both slots
+    if (issuer) ptx::tma_store_wait_read<0>();
     ptx::bar_sync(2 + wg, 128);
 #pragma unroll
-    for (int ii = 0; ii < 4; ++ii) {
-      const int i = 4 * b + ii;   // 8-column group of the tile
+    for (int s = 0; s < 2; ++s)
 #pragma unroll
-      for (int j = 0; j < 2; ++j)
-        ptx::st_shared_v2(box + t_off + 8 * j * 128 + ((32 * ii) ^ t_xor), v[4 * i + 2 * j], v[4 * i + 2 * j + 1]);
-    }
+      for (int ii = 0; ii < 4; ++ii) {
+        const int i = 8 * q + 4 * s + ii;   // 8-column group of the tile
+#pragma unroll
+        for (int j = 0; j < 2; ++j)
+          ptx::st_shared_v2(stg + s * TC_D_BOX_BYTES + t_off + 8 * j * 128 + ((32 * ii) ^ t_xor), v[4 * i + 2 * j],
+                            v[4 * i + 2 * j + 1]);
+      }
     ptx::fence_proxy_async_smem();   // the generic-proxy writes become visible to the TMA unit
     ptx::bar_sync(2 + wg, 128);
     if (issuer) {
-      const int64_t gc = col_w + TC_D_BOX_COLS * b;
-      if (gc < p.n && row_w < p.m)
-        ptx::tma_store_2d(tmap_d, box, static_cast<int32_t>(gc), static_cast<int32_t>(row_w), ptx::policy_evict_first());
-      ptx::tma_store_commit();   // one group per box (possibly empty): the wait above counts boxes
+#pragma unroll
+      for (int s = 0; s < 2; ++s) {
+        const int64_t gc = col_w + TC_D_BOX_COLS * (2 * q + s);
+#if !defined(B2D_TC_DIAG) || B2D_TC_DIAG != 2
+        if (gc < p.n && row_w < p.m)
+          ptx::tma_store_2d(tmap_d, stg + s * TC_D_BOX_BYTES, static_cast<int32_t>(gc), static_cast<int32_t>(row_w),
+                            ptx::policy_evict_first());
+#endif
+      }
+      ptx::tma_store_commit();   // one group per pair (possibly empty): the wait above counts pairs
     }
   }
   if (issuer && last) ptx::tma_store_wait_all();   // the CTA's last tile: its shared memory outlives every store
@@ -567,6 +609,9 @@ expanded_tc_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_cons
   // rows with their own exponent (prep.cuh): per-row factor on x (one multiply per row and tile), per-column factor on y
   // only when some row of y has one (rare; read straight from global memory then)
   const bool xnu = __ldg(&p.nonuni[0]) != 0u, ynu = __ldg(&p.nonuni[1]) != 0u;
+  // EPI_STORE through TMA in one pass, without the diagonal or per-column scales: tc_epilogue_store_fast
+  constexpr bool kFastPost = !tc_post_gram(kPost);
+  const bool fast_store    = kEpi == EPI_STORE && kFastPost && p.tma_store && p.acc_mode == 0 && !p.diag_zero && !ynu;
   // the x ring this warpgroup reads: resident, its own (its rows of every stage); streaming, the one both read
   const int ring = kResident ? wg : 0;
   // Resident: ordered MMA turns.  Both warpgroups walk the same (item, tile, half) units; warpgroup w takes its turn at
@@ -683,6 +728,10 @@ expanded_tc_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_cons
 #pragma unroll
           for (int c = 0; c < 64; ++c) crs[c] = 0.f;
         }
+#if defined(B2D_TC_DIAG) && B2D_TC_DIAG == 3
+#pragma unroll
+        for (int c = 0; c < 64; ++c) acc[c] = crs[c] = 0.f;
+#endif
         // Resident: both halves read the tile's nkb x stages (a_it counts (tile, kb)), and only the last half hands
         // them back.  In an earlier half the stage's phase cannot advance, so waiting on it again returns at once.
         // (the rule of tc_half_releases, written out: through the call the resident instantiations schedule differently)
@@ -691,36 +740,45 @@ expanded_tc_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_cons
         if (kResident) take_turn();   // this unit's MMA turn
         // descriptor start-address units are 16 B; inside the 128-B swizzled row of a k-block:
         //   hi k[0,16) +0, hi k[16,32) +2, lo k[0,16) +4, lo k[16,32) +6
-        for (int kb = 0; kb < nkb; ++kb) {
-          const uint32_t it = it0 + kb;
-          const uint32_t s = it % kStages, ph = (it / kStages) & 1;
-          // (the first MMAs of the item on the resident y block wait for it; the other warpgroup has passed the turn,
-          // so its hand-back of the previous y block does not wait on this one)
-          if (kResident && (kMasked ? b_first : (mt == mt0 && h == 0))) ptx::mbar_wait(&bfull[kb], it_local & 1);
-          ptx::mbar_wait(&afull[kRings * s + ring], ph);
-          const uint64_t da = ptx::gmma_desc_sw128(ptx::smem_u32(a_base + s * kStageBytes) + wg * 64 * 128);
-          const uint64_t db = ptx::gmma_desc_sw128(kResident ? ptx::smem_u32(b_base + kb * TC_B_BYTES) + h * TC_BH_BYTES
-                                                             : ptx::smem_u32(a_base + s * kStageBytes + TC_A_BYTES));
-          const uint32_t accum = kb > 0 ? 1u : 0u;
-          ptx::fence_regs(acc);
-          ptx::fence_regs(crs);
-          ptx::wgmma_fence();
-          if (has_lo) {
-            ptx::wgmma_m64n128k16_f16(crs, da + 4, db + 0, accum);  // lo0 * hi0
-            ptx::wgmma_m64n128k16_f16(crs, da + 6, db + 2, 1u);     // lo1 * hi1
-            ptx::wgmma_m64n128k16_f16(crs, da + 0, db + 4, 1u);     // hi0 * lo0
-            ptx::wgmma_m64n128k16_f16(crs, da + 2, db + 6, 1u);     // hi1 * lo1
+        // One copy of the k-block loop with the cross terms and one without: a k-block's MMAs are one straight batch
+        // (one wgmma group, as the release waits below count them), with no branch for the compiler to split it at.
+        auto mma_unit = [&](auto with_lo) {
+          constexpr bool kLo = decltype(with_lo)::value;
+          for (int kb = 0; kb < nkb; ++kb) {
+            const uint32_t it = it0 + kb;
+            const uint32_t s = it % kStages, ph = (it / kStages) & 1;
+            // (the first MMAs of the item on the resident y block wait for it; the other warpgroup has passed the turn,
+            // so its hand-back of the previous y block does not wait on this one)
+            if (kResident && (kMasked ? b_first : (mt == mt0 && h == 0))) ptx::mbar_wait(&bfull[kb], it_local & 1);
+            ptx::mbar_wait(&afull[kRings * s + ring], ph);
+            const uint64_t da = ptx::gmma_desc_sw128(ptx::smem_u32(a_base + s * kStageBytes) + wg * 64 * 128);
+            const uint64_t db = ptx::gmma_desc_sw128(kResident ? ptx::smem_u32(b_base + kb * TC_B_BYTES) + h * TC_BH_BYTES
+                                                               : ptx::smem_u32(a_base + s * kStageBytes + TC_A_BYTES));
+            const uint32_t accum = kb > 0 ? 1u : 0u;
+            ptx::fence_regs(acc);
+            if (kLo) ptx::fence_regs(crs);
+            ptx::wgmma_fence();
+#if !defined(B2D_TC_DIAG) || B2D_TC_DIAG != 3
+            if constexpr (kLo) {
+              ptx::wgmma_m64n128k16_f16(crs, da + 4, db + 0, accum);  // lo0 * hi0
+              ptx::wgmma_m64n128k16_f16(crs, da + 6, db + 2, 1u);     // lo1 * hi1
+              ptx::wgmma_m64n128k16_f16(crs, da + 0, db + 4, 1u);     // hi0 * lo0
+              ptx::wgmma_m64n128k16_f16(crs, da + 2, db + 6, 1u);     // hi1 * lo1
+            }
+            ptx::wgmma_m64n128k16_f16(acc, da + 0, db + 0, accum);    // hi0 * hi0
+            ptx::wgmma_m64n128k16_f16(acc, da + 2, db + 2, 1u);       // hi1 * hi1
+#endif
+            ptx::wgmma_commit();
+            ptx::fence_regs(acc);
+            if (kLo) ptx::fence_regs(crs);
+            if (!kResident && release && kb > 0) {  // the previous k-block's MMAs have finished reading their stage: hand it back
+              ptx::wgmma_wait<1>();
+              if (lead) ptx::mbar_arrive(&aempty[kRings * ((it - 1) % kStages) + ring]);
+            }
           }
-          ptx::wgmma_m64n128k16_f16(acc, da + 0, db + 0, accum);    // hi0 * hi0
-          ptx::wgmma_m64n128k16_f16(acc, da + 2, db + 2, 1u);       // hi1 * hi1
-          ptx::wgmma_commit();
-          ptx::fence_regs(acc);
-          ptx::fence_regs(crs);
-          if (!kResident && release && kb > 0) {  // the previous k-block's MMAs have finished reading their stage: hand it back
-            ptx::wgmma_wait<1>();
-            if (lead) ptx::mbar_arrive(&aempty[kRings * ((it - 1) % kStages) + ring]);
-          }
-        }
+        };
+        if (has_lo) mma_unit(std::true_type{});
+        else mma_unit(std::false_type{});
         if (kResident) {
           // Every MMA of the unit is issued without waiting on any of them: the other warpgroup's turn.  Then the
           // stages go back as the MMAs that read them finish (k-block kb's group is done once at most nkb - 1 - kb
@@ -747,13 +805,26 @@ expanded_tc_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_cons
               for (int kb = 0; kb < nkb; ++kb) ptx::mbar_arrive(&bempty[kb]);
           }
         }
+#if defined(B2D_TC_DIAG) && B2D_TC_DIAG == 1
+        {   // the accumulators must have a use, or ptxas drops the MMAs that write them: a sum stored under a condition
+            // that never holds at run time (empty asm fences are not a use)
+          float sum = 0.f;
+#pragma unroll
+          for (int c = 0; c < 64; ++c) sum += acc[c] + crs[c];
+          if (p.m < 0) p.dist[threadIdx.x] = sum;
+          continue;
+        }
+#endif
 #pragma unroll
         for (int c = 0; c < 64; ++c) acc[c] += crs[c];
         const int cl0 = h * TC_HN + 2 * tq;  // this thread's first column inside the tile
         unsigned long long keep = ~0ull;
         if (kMasked && hcls == MASK_PARTIAL) keep = masked_keep64(col_grp, cl0, p.mask_bits, p.mask_groups, row0, p.m);
-        tc_epilogue<kEpi, kPost>(acc, p, col_tb, cl0, static_cast<int64_t>(n_blk) * TC_BN + cl0, row0, ta, cfr, thr, xnr,
-                                 ynu, keep);
+        if (kEpi == EPI_STORE && fast_store)
+          tc_epilogue_store_fast<kPost>(acc, p, col_tb, cl0, ta, cfr);
+        else
+          tc_epilogue<kEpi, kPost>(acc, p, col_tb, cl0, static_cast<int64_t>(n_blk) * TC_BN + cl0, row0, ta, cfr, thr, xnr,
+                                   ynu, keep);
         if (kEpi == EPI_STORE && p.tma_store)   // (this warpgroup's staging boxes: computed here, not kept live)
           tc_stage_store(acc, &tmap_d, ptx::smem_u32(smem + Carve::stg_off) + wg * TC_STG_BOXES * TC_D_BOX_BYTES, lead,
                          item + gridDim.x >= p.n_items && mt == mt1 - 1 && h == nh - 1, wg,
