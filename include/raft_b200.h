@@ -289,6 +289,32 @@ int b2d_eps_neighbors_l2sq(void* stream, uint8_t* adj, int64_t ld_adj, void* vd,
                            const float* x, int64_t ldx, const float* y, int64_t ldy, int64_t m, int64_t n, int64_t k,
                            float eps, void* workspace, size_t workspace_bytes);
 
+/* Radius neighbours (sklearn.neighbors.NearestNeighbors.radius_neighbors(sort_results=True); a project API, no upstream
+ * signature): for every row i of x:[m,k] the rows j of y:[n,k] with d(i, j) <= radius, as CSR, without the m x n matrix.
+ * fp32, row-major, pitches ldx / ldy >= k.
+ *   d(i, j) is exactly the fp32 value b2d_pairwise_distance(metric) returns for the pair, metric one of L2Expanded (radius
+ *     is then a squared distance), L2SqrtExpanded, CosineExpanded and CorrelationExpanded (else B2D_ERR_UNSUPPORTED),
+ *     including its self-pair rule: under an L2 metric with x == y, m == n and ldx == ldy, d(i, i) = 0.  A NaN distance
+ *     (NaN element, zero-norm row under cosine, constant row under correlation) is never in the result; a NaN or negative
+ *     radius gives no pairs; radius = +inf gives every non-NaN pair.
+ *   Output: indptr int64 [m + 1] (indptr[m] = nnz), indices int64 [nnz] (rows of y) and distances float [nnz].  Each row is
+ *     sorted by the packed (distance, index) key of the 1-NN and kNN entry points: ascending distance, equal distances by
+ *     ascending index, -0.0 before +0.0.  The result is reproducible byte for byte.
+ * Two calls: b2d_radius_neighbors_count writes indptr (the row degrees, scanned); the caller reads nnz = indptr[m],
+ * allocates and calls b2d_radius_neighbors_fill with the same inputs and that nnz (<= 2^31 - 1, else
+ * B2D_ERR_UNSUPPORTED: split the queries).  fill never writes past nnz entries: called with other inputs or a smaller nnz,
+ * its result is unspecified but stays inside the caller's buffers.  k <= 320 (else B2D_ERR_UNSUPPORTED); k == 0, ld < k,
+ * m or n >= 2^31, a negative extent or nnz and null pointers are B2D_ERR_INVALID_ARG; m == 0 or n == 0 give nnz = 0.  Both
+ * calls only enqueue work (no synchronisation, no allocation) and can be captured in a CUDA graph.  Workspace: the query
+ * with nnz = 0 for the count call and with the call's nnz for fill; SIZE_MAX for negative arguments. */
+size_t b2d_radius_neighbors_workspace_bytes(int64_t m, int64_t n, int64_t k, int64_t nnz);
+int b2d_radius_neighbors_count(void* stream, int64_t* indptr, int metric, const float* x, int64_t ldx, const float* y,
+                               int64_t ldy, int64_t m, int64_t n, int64_t k, float radius, void* workspace,
+                               size_t workspace_bytes);
+int b2d_radius_neighbors_fill(void* stream, const int64_t* indptr, int64_t nnz, int64_t* indices, float* distances,
+                              int metric, const float* x, int64_t ldx, const float* y, int64_t ldy, int64_t m, int64_t n,
+                              int64_t k, float radius, void* workspace, size_t workspace_bytes);
+
 /* raft::distance::kernels::KernelType ([RECALLED] raft/distance/distance_types.hpp, <= 25.12) */
 enum { B2D_KERNEL_LINEAR = 0, B2D_KERNEL_POLYNOMIAL = 1, B2D_KERNEL_RBF = 2, B2D_KERNEL_TANH = 3 };
 

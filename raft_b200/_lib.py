@@ -20,7 +20,8 @@ SYMBOLS = [
     "b2d_gram_matrix_workspace_bytes", "b2d_gram_matrix", "b2d_kmeans_workspace_bytes", "b2d_kmeans_fit",
     "b2d_kmeans_predict", "b2d_kmeans_update_centroids", "b2d_kmeans_init_plus_plus", "b2d_mst_workspace_bytes", "b2d_mst",
     "b2d_single_linkage_workspace_bytes", "b2d_single_linkage", "b2d_dbscan_workspace_bytes", "b2d_dbscan_fit",
-    "b2d_debug_pairwise_plan",
+    "b2d_debug_pairwise_plan", "b2d_radius_neighbors_workspace_bytes", "b2d_radius_neighbors_count",
+    "b2d_radius_neighbors_fill",
 ]
 
 B2D_OK, B2D_ERR_INVALID_ARG, B2D_ERR_CUDA, B2D_ERR_UNSUPPORTED, B2D_ERR_WORKSPACE = range(5)
@@ -134,6 +135,12 @@ def lib() -> ctypes.CDLL:
     L.b2d_dbscan_workspace_bytes.argtypes = [i64, i64, i64]
     L.b2d_dbscan_fit.restype = ci
     L.b2d_dbscan_fit.argtypes = [vp, ci, vp, i64, i64, i64, cd, i64, i64, vp, vp, vp, vp, sz]
+    L.b2d_radius_neighbors_workspace_bytes.restype = sz
+    L.b2d_radius_neighbors_workspace_bytes.argtypes = [i64, i64, i64, i64]
+    L.b2d_radius_neighbors_count.restype = ci
+    L.b2d_radius_neighbors_count.argtypes = [vp, vp, ci, vp, i64, vp, i64, i64, i64, i64, cf, vp, sz]
+    L.b2d_radius_neighbors_fill.restype = ci
+    L.b2d_radius_neighbors_fill.argtypes = [vp, vp, i64, vp, vp, ci, vp, i64, vp, i64, i64, i64, i64, cf, vp, sz]
     L.b2d_row_norm.restype = ci
     L.b2d_row_norm.argtypes = [vp, vp, vp, i64, i64, i64, ci, ci]
     _lib = L

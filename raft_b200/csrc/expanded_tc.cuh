@@ -52,6 +52,9 @@
 //   EPI_EPS           epsilon neighbourhood: the EPI_STORE / POST_CLAMP distance, compared with eps; the 0/1 bytes go to
 //                     the EPI_STORE staging ring (one 64 x 128-byte box per tile), leave from there by TMA or a copy, and
 //                     are counted per column into shared memory (tc_eps_tile).
+//   EPI_RADIUS        radius neighbours: the EPI_STORE distance of kPost, compared with eps as a 32-bit hit mask per
+//                     row and half tile in registers; count mode adds the row's hits to its degree, fill mode appends
+//                     them as packed keys to the row's CSR segment (radius_row32).
 //
 // Diagnostic builds (DESIGN.md section 5, scripts/tc_breakdown.py; never the library's own build): B2D_TC_DIAG = 1 keeps
 // the MMAs only (no epilogue, no staging; one sum of the accumulators keeps them live), 2 computes and stages every value
@@ -151,6 +154,53 @@ __device__ __noinline__ unsigned long long masked_keep64(const int* col_grp, int
   return keep;
 }
 
+// EPI_RADIUS, one row of a 64 x 128 warpgroup tile: a0..a31 are the thread's distances of the row (a[2 i + e] at column
+// col0 + 8 i + e) and bit t of `hits` is set when a[t] is within the radius.  The 4 lanes of a quad hold the row's 128
+// columns; the whole warp calls (the quad shuffles), a lane of a row outside the matrix with hits == 0.
+//   count: the quad's hits are added to cnt[row] (one atomic when there are any).
+//   fill:  one atomic on the row's fill counter cnt[row] reserves the quad's slots; each lane writes its hits, in column
+//          order after those of the lanes below it, as key_pack(d, j) to out[indptr[row] + slot].  A slot at or past
+//          min(indptr[row + 1], nnz) is dropped (the degrees no longer match the data): nothing is written outside out.
+// Not inlined, for the reason given at knn_append16.
+__device__ __noinline__ void radius_row32(unsigned* cnt, long long* out, const long long* indptr, long long nnz, int64_t row,
+                                          long long col0, unsigned hits, int fill, float a0, float a1, float a2, float a3,
+                                          float a4, float a5, float a6, float a7, float a8, float a9, float a10, float a11,
+                                          float a12, float a13, float a14, float a15, float a16, float a17, float a18,
+                                          float a19, float a20, float a21, float a22, float a23, float a24, float a25,
+                                          float a26, float a27, float a28, float a29, float a30, float a31)
+{
+  const unsigned tq = threadIdx.x & 3u;
+  const unsigned c  = __popc(hits);
+  if (!fill) {
+    unsigned t = c + __shfl_xor_sync(0xffffffffu, c, 1);
+    t += __shfl_xor_sync(0xffffffffu, t, 2);
+    if (tq == 0u && t != 0u) atomicAdd(&cnt[row], t);
+    return;
+  }
+  // exclusive prefix of the quad's counts, the quad's total from its last lane
+  unsigned incl = c, u = __shfl_up_sync(0xffffffffu, incl, 1, 4);
+  if (tq >= 1u) incl += u;
+  u = __shfl_up_sync(0xffffffffu, incl, 2, 4);
+  if (tq >= 2u) incl += u;
+  const unsigned total = __shfl_sync(0xffffffffu, incl, 3, 4);
+  unsigned base = 0u;
+  if (tq == 0u && total != 0u) base = atomicAdd(&cnt[row], total);
+  base = __shfl_sync(0xffffffffu, base, 0, 4);
+  if (c == 0u) return;
+  const long long start = indptr[row];
+  const long long lim   = min(indptr[row + 1], nnz);
+  long long pos         = start + base + (incl - c);
+  const float a[32] = {a0,  a1,  a2,  a3,  a4,  a5,  a6,  a7,  a8,  a9,  a10, a11, a12, a13, a14, a15,
+                       a16, a17, a18, a19, a20, a21, a22, a23, a24, a25, a26, a27, a28, a29, a30, a31};
+#pragma unroll
+  for (int t = 0; t < 32; ++t) {
+    if ((hits >> t) & 1u) {
+      if (pos < lim) out[pos] = key_pack(a[t], col0 + 8 * (t >> 1) + (t & 1));
+      ++pos;
+    }
+  }
+}
+
 // Epilogue of one 64 x 128 warpgroup tile.  v[4i + 2j + e] holds row row0 + 8j, column gc0 + 8i + e of the accumulator
 // (main + cross already summed); on return (EPI_STORE) v holds the finished distances, and they have been written
 // unless p.tma_store (then tc_stage_store writes them).  EPI_MINLOC_MASKED: the values whose bit in `keep` is clear
@@ -178,7 +228,7 @@ __device__ __forceinline__ void tc_epilogue(float (&v)[64], const TcParams& p, c
       if (kEpi == EPI_STORE && tc_post_ratio(kPost)) {
         v[4 * i + 2 * j]     = post_ratio<kPost>(a0 * cfr[j], ta[j] + tb.x);
         v[4 * i + 2 * j + 1] = post_ratio<kPost>(a1 * cfr[j], ta[j] + tb.y);
-      } else if (kEpi == EPI_STORE || kEpi == EPI_EPS) {
+      } else if (kEpi == EPI_STORE || kEpi == EPI_EPS || kEpi == EPI_RADIUS) {
         v[4 * i + 2 * j]     = fmaf(a0, cfr[j], ta[j] + tb.x);
         v[4 * i + 2 * j + 1] = fmaf(a1, cfr[j], ta[j] + tb.y);
       } else {
@@ -201,6 +251,43 @@ __device__ __forceinline__ void tc_epilogue(float (&v)[64], const TcParams& p, c
 #pragma unroll
           for (int e = 0; e < 2; ++e)
             if (dd == 8 * (i - j) + e && gc0 + 8 * i + e < p.n) v[4 * i + 2 * j + e] = 0.f;
+    }
+    return;
+  }
+  if constexpr (kEpi == EPI_RADIUS) {
+    // the EPI_STORE values of acc_mode 0 (clamp, diagonal, sqrt), then one hit mask per row instead of the stores.  Columns
+    // beyond n hold NaN (from t_y), rows beyond m are left out here.
+    if (tc_post_clamps(kPost)) {
+#pragma unroll
+      for (int c = 0; c < 64; ++c) v[c] = clamp0(v[c]);
+      if (p.diag_zero) {
+#pragma unroll
+        for (int i = 0; i < 16; ++i)
+#pragma unroll
+          for (int j = 0; j < 2; ++j) {
+            if (row0 + 8 * j == gc0 + 8 * i) v[4 * i + 2 * j] = 0.f;
+            if (row0 + 8 * j == gc0 + 8 * i + 1) v[4 * i + 2 * j + 1] = 0.f;
+          }
+      }
+      if (kPost == POST_CLAMP_SQRT) {
+#pragma unroll
+        for (int c = 0; c < 64; ++c) asm("sqrt.approx.f32 %0, %1;" : "=f"(v[c]) : "f"(v[c]));
+      }
+    }
+#pragma unroll
+    for (int j = 0; j < 2; ++j) {
+      unsigned hits = 0u;
+#pragma unroll
+      for (int t = 0; t < 32; ++t)
+        if (v[4 * (t >> 1) + 2 * j + (t & 1)] <= p.eps) hits |= 1u << t;
+      if (row0 + 8 * j >= p.m) hits = 0u;
+      if (__any_sync(0xffffffffu, hits != 0u))
+        radius_row32(p.knn_cnt, p.knn_cand, p.rad_indptr, p.rad_nnz, row0 + 8 * j, gc0, hits, p.rad_fill, v[2 * j],
+                     v[2 * j + 1], v[4 + 2 * j], v[5 + 2 * j], v[8 + 2 * j], v[9 + 2 * j], v[12 + 2 * j], v[13 + 2 * j],
+                     v[16 + 2 * j], v[17 + 2 * j], v[20 + 2 * j], v[21 + 2 * j], v[24 + 2 * j], v[25 + 2 * j],
+                     v[28 + 2 * j], v[29 + 2 * j], v[32 + 2 * j], v[33 + 2 * j], v[36 + 2 * j], v[37 + 2 * j],
+                     v[40 + 2 * j], v[41 + 2 * j], v[44 + 2 * j], v[45 + 2 * j], v[48 + 2 * j], v[49 + 2 * j],
+                     v[52 + 2 * j], v[53 + 2 * j], v[56 + 2 * j], v[57 + 2 * j], v[60 + 2 * j], v[61 + 2 * j]);
     }
     return;
   }
@@ -657,7 +744,8 @@ expanded_tc_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_cons
     {
       const int64_t gj = static_cast<int64_t>(n_blk) * TC_BN + ct;
       // +inf: never the arg-min; NaN: never within eps
-      float tv = kEpi == EPI_EPS ? __int_as_float(0x7fffffff) : kEpi != EPI_STORE ? __int_as_float(0x7f800000) : 0.f;
+      float tv = (kEpi == EPI_EPS || kEpi == EPI_RADIUS) ? __int_as_float(0x7fffffff)
+               : kEpi != EPI_STORE                     ? __int_as_float(0x7f800000) : 0.f;
       if (gj < p.n) tv = __ldg(&p.yt[gj]);
       if (kEpi == EPI_STORE && p.acc_mode >= 2) tv = 0.f;  // the t terms entered with the first K chunk
       col_tb[ct] = tv;

@@ -27,7 +27,7 @@ constexpr int TC_D_BOX_ROWS  = 64;
 constexpr int TC_D_BOX_BYTES = TC_D_BOX_COLS * TC_D_BOX_ROWS * 4;
 constexpr int TC_STG_BOXES   = 2;
 
-enum TcEpilogue : int { EPI_STORE = 0, EPI_MINLOC = 1, EPI_TOPK = 2, EPI_MINLOC_MASKED = 3, EPI_EPS = 4 };
+enum TcEpilogue : int { EPI_STORE = 0, EPI_MINLOC = 1, EPI_TOPK = 2, EPI_MINLOC_MASKED = 3, EPI_EPS = 4, EPI_RADIUS = 5 };
 constexpr int64_t TC_NO_DIAG = INT64_MIN;   // TcParams::diag_off: y is not a row window of x
 
 // EPI_MINLOC_MASKED (masked_nn.cuh): class of one (64-row slab of x, 128-column half of a y block) tile.  Byte
@@ -108,6 +108,12 @@ struct TcParams {
   float gamma;
   float coef0;
   int degree;
+  // EPI_RADIUS (radius_neighbors, radius.cu): the pairs with d(i, j) <= eps, d the EPI_STORE distance of post kPost (diag_zero
+  // as there).  Count mode: knn_cnt[i] += the row's pairs.  Fill mode: knn_cnt[i] is the row's fill counter and every pair
+  // is written as key_pack(d, j) to knn_cand[rad_indptr[i] + slot], a slot at or past min(rad_indptr[i + 1], rad_nnz) dropped
+  const long long* rad_indptr;   // [m + 1] (fill mode)
+  long long rad_nnz;
+  int rad_fill;                  // 0: count, 1: fill
 };
 
 constexpr size_t TC_SMEM_OPERANDS = (size_t)TC_MAX_RES_KB * TC_B_BYTES + (size_t)TC_STAGES_RES * TC_A_BYTES;  // 208 KB
@@ -122,7 +128,7 @@ static_assert((size_t)TC_STAGES_STR * (TC_A_BYTES + TC_BH_BYTES) <= TC_SMEM_OPER
 // mbarriers (after t_y): afull[rings * TC_MAX_STAGES], aempty[rings * TC_MAX_STAGES] (slot s of ring w at rings * s + w),
 // bfull[TC_MAX_RES_KB], bempty[TC_MAX_RES_KB].
 // EPI_EPS has the carve of EPI_STORE (its adjacency boxes are the same 8 KB) plus the [256] column counts in the slot of the
-// masked kernel's groups.
+// masked kernel's groups.  EPI_RADIUS stores nothing through shared memory: the carve of the arg-min epilogues.
 template <bool kResident, int kEpi>
 struct TcCarve {
   static constexpr bool staged = kEpi == EPI_STORE || kEpi == EPI_EPS;

@@ -130,6 +130,11 @@ static int launch_tc_epi(cudaStream_t s, const CUtensorMap& ma, const CUtensorMa
   if (epi == EPI_MINLOC_MASKED) return launch_tc_inst<kRes, EPI_MINLOC_MASKED, POST_NONE>(s, ma, mb, md, p, grid);
   if (epi == EPI_TOPK) return launch_tc_inst<kRes, EPI_TOPK, POST_NONE>(s, ma, mb, md, p, grid);
   if (epi == EPI_EPS) return launch_tc_inst<kRes, EPI_EPS, POST_CLAMP>(s, ma, mb, md, p, grid);
+  if (epi == EPI_RADIUS) {
+    if (post == POST_CLAMP) return launch_tc_inst<kRes, EPI_RADIUS, POST_CLAMP>(s, ma, mb, md, p, grid);
+    if (post == POST_CLAMP_SQRT) return launch_tc_inst<kRes, EPI_RADIUS, POST_CLAMP_SQRT>(s, ma, mb, md, p, grid);
+    return launch_tc_inst<kRes, EPI_RADIUS, POST_NONE>(s, ma, mb, md, p, grid);
+  }
   if (post == POST_NONE) return launch_tc_inst<kRes, EPI_STORE, POST_NONE>(s, ma, mb, md, p, grid);
   if (post == POST_CLAMP) return launch_tc_inst<kRes, EPI_STORE, POST_CLAMP>(s, ma, mb, md, p, grid);
   if (post == POST_JACCARD) return launch_tc_inst<kRes, EPI_STORE, POST_JACCARD>(s, ma, mb, md, p, grid);
