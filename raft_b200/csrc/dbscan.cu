@@ -2,7 +2,6 @@
 #include <cuda_runtime.h>
 #include <algorithm>
 #include <cmath>
-#include <cstring>
 
 #include "host.cuh"
 #include "dbscan.cuh"
@@ -63,8 +62,7 @@ static DbLayout db_layout(void* base, int64_t m, int64_t d, int64_t max_bytes)
 static int db_eps(cudaStream_t s, const DbLayout& L, int64_t m, int64_t d, float e, int64_t t, bool adj, bool deg)
 {
   const int64_t c0 = t * L.b, w = std::min(L.b, m - c0);
-  TcParams p;
-  memset(&p, 0, sizeof(p));
+  TcParams p{};
   p.m = m; p.n = w;
   p.adj = adj ? L.adj : nullptr; p.ld_adj = L.ld;
   p.vd = deg ? L.deg + c0 + t : nullptr; p.vd64 = 0; p.eps = e;
@@ -87,7 +85,8 @@ int b2d_dbscan_fit(void* stream, int metric, const float* x, int64_t ldx, int64_
                    int32_t* n_clusters, void* workspace, size_t workspace_bytes)
 {
   cudaStream_t s = static_cast<cudaStream_t>(stream);
-  if (metric != B2D_L2SqrtExpanded && metric != B2D_L2Expanded && metric != B2D_CosineExpanded)
+  TcMetric tm;
+  if ((metric != B2D_L2SqrtExpanded && metric != B2D_L2Expanded && metric != B2D_CosineExpanded) || !tc_metric(metric, d, &tm))
     return fail(B2D_ERR_UNSUPPORTED, "dbscan supports the L2SqrtExpanded, L2Expanded and CosineExpanded metrics");
   if (m < 0 || d < 0 || max_bytes_per_batch < 0) return fail(B2D_ERR_INVALID_ARG, "negative extent or batch size");
   if (m == 0) return B2D_OK;
@@ -105,8 +104,7 @@ int b2d_dbscan_fit(void* stream, int metric, const float* x, int64_t ldx, int64_
   const float e = !(eps >= 0.0) ? -INFINITY : static_cast<float>(metric == B2D_L2SqrtExpanded ? eps * eps : eps);
   const unsigned ms = static_cast<unsigned>(std::min<int64_t>(min_samples, m + 1));
   // 0. x prepared once, as both operands; every batch takes a window of the y side
-  rc = launch_prep<float>(s, L.tc, x, ldx, 1, m, x, ldx, 1, m, d, nullptr, nullptr,
-                          metric == B2D_CosineExpanded ? PREP_COSINE : PREP_L2, 0);
+  rc = launch_prep<float>(s, L.tc, x, ldx, 1, m, x, ldx, 1, m, d, nullptr, nullptr, tm);
   if (rc) return rc;
   // 1. degrees, then the core flags (one batch: the adjacency in the same launch)
   B2D_CUDA(cudaMemsetAsync(L.deg, 0, static_cast<size_t>(m + L.nb) * sizeof(unsigned), s));

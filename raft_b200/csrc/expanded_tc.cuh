@@ -201,6 +201,35 @@ __device__ __noinline__ void radius_row32(unsigned* cnt, long long* out, const l
   }
 }
 
+// The finished distance of a clamping post (tc_post_clamps) in the fragment layout of tc_epilogue: clamped at 0, 0 where
+// row i of x is row i - diag_off of y, then the sqrt of POST_CLAMP_SQRT.  kGuardN: only columns below n are zeroed.  EPI_EPS
+// needs that, since it counts every column of a row window; EPI_STORE and EPI_RADIUS set diag_off = 0 only with m == n, so
+// a column at or past n pairs with a row at or past m, which they never store or count.
+template <int kPost, bool kGuardN>
+__device__ __forceinline__ void tc_finish(float (&v)[64], const TcParams& p, int64_t row0, int64_t gc0)
+{
+#pragma unroll
+  for (int c = 0; c < 64; ++c) v[c] = clamp0(v[c]);
+  if (p.diag_off != TC_NO_DIAG) {
+    // row0 + 8 j - diag_off == gc0 + 8 i + e  <=>  dd == 8 (i - j) + e, which lies in [-8, 121]
+    const int64_t dd = row0 - p.diag_off - gc0;
+    if (dd >= -8 && dd < 128) {
+      const int d = static_cast<int>(dd);
+#pragma unroll
+      for (int i = 0; i < 16; ++i)
+#pragma unroll
+        for (int j = 0; j < 2; ++j)
+#pragma unroll
+          for (int e = 0; e < 2; ++e)
+            if (d == 8 * (i - j) + e && (!kGuardN || gc0 + 8 * i + e < p.n)) v[4 * i + 2 * j + e] = 0.f;
+    }
+  }
+  if (kPost == POST_CLAMP_SQRT) {
+#pragma unroll
+    for (int c = 0; c < 64; ++c) asm("sqrt.approx.f32 %0, %1;" : "=f"(v[c]) : "f"(v[c]));
+  }
+}
+
 // Epilogue of one 64 x 128 warpgroup tile.  v[4i + 2j + e] holds row row0 + 8j, column gc0 + 8i + e of the accumulator
 // (main + cross already summed); on return (EPI_STORE) v holds the finished distances, and they have been written
 // unless p.tma_store (then tc_stage_store writes them).  EPI_MINLOC_MASKED: the values whose bit in `keep` is clear
@@ -238,42 +267,15 @@ __device__ __forceinline__ void tc_epilogue(float (&v)[64], const TcParams& p, c
     }
   }
   if constexpr (kEpi == EPI_EPS) {
-    // the POST_CLAMP distance of EPI_STORE; where row i of x is row j of y (i == j + diag_off) it is 0, as pairwise_distance
-    // makes it when x is y.  (Columns beyond n hold NaN from t_y and stay unmatched; the row window check keeps them out.)
-#pragma unroll
-    for (int c = 0; c < 64; ++c) v[c] = clamp0(v[c]);
-    if (p.diag_off != TC_NO_DIAG) {
-      const int64_t dd = row0 - p.diag_off - gc0;   // row0 + 8 j == gc0 + 8 i + e + diag_off  <=>  dd == 8 (i - j) + e
-#pragma unroll
-      for (int i = 0; i < 16; ++i)
-#pragma unroll
-        for (int j = 0; j < 2; ++j)
-#pragma unroll
-          for (int e = 0; e < 2; ++e)
-            if (dd == 8 * (i - j) + e && gc0 + 8 * i + e < p.n) v[4 * i + 2 * j + e] = 0.f;
-    }
+    // the POST_CLAMP distance of EPI_STORE.  (Columns beyond n hold NaN from t_y and stay unmatched; the row window check
+    // keeps them out.)
+    tc_finish<POST_CLAMP, true>(v, p, row0, gc0);
     return;
   }
   if constexpr (kEpi == EPI_RADIUS) {
-    // the EPI_STORE values of acc_mode 0 (clamp, diagonal, sqrt), then one hit mask per row instead of the stores.  Columns
-    // beyond n hold NaN (from t_y), rows beyond m are left out here.
-    if (tc_post_clamps(kPost)) {
-#pragma unroll
-      for (int c = 0; c < 64; ++c) v[c] = clamp0(v[c]);
-      if (p.diag_zero) {
-#pragma unroll
-        for (int i = 0; i < 16; ++i)
-#pragma unroll
-          for (int j = 0; j < 2; ++j) {
-            if (row0 + 8 * j == gc0 + 8 * i) v[4 * i + 2 * j] = 0.f;
-            if (row0 + 8 * j == gc0 + 8 * i + 1) v[4 * i + 2 * j + 1] = 0.f;
-          }
-      }
-      if (kPost == POST_CLAMP_SQRT) {
-#pragma unroll
-        for (int c = 0; c < 64; ++c) asm("sqrt.approx.f32 %0, %1;" : "=f"(v[c]) : "f"(v[c]));
-      }
-    }
+    // the EPI_STORE values of acc_mode 0, then one hit mask per row instead of the stores.  Columns beyond n hold NaN (from
+    // t_y), rows beyond m are left out here.
+    if (tc_post_clamps(kPost)) tc_finish<kPost, false>(v, p, row0, gc0);
 #pragma unroll
     for (int j = 0; j < 2; ++j) {
       unsigned hits = 0u;
@@ -314,23 +316,7 @@ __device__ __forceinline__ void tc_epilogue(float (&v)[64], const TcParams& p, c
         }
       }
     }
-    if (tc_post_clamps(kPost) && (p.acc_mode == 0 || p.acc_mode == 3)) {
-#pragma unroll
-      for (int c = 0; c < 64; ++c) v[c] = clamp0(v[c]);
-      if (p.diag_zero) {
-#pragma unroll
-        for (int i = 0; i < 16; ++i)
-#pragma unroll
-          for (int j = 0; j < 2; ++j) {
-            if (row0 + 8 * j == gc0 + 8 * i) v[4 * i + 2 * j] = 0.f;
-            if (row0 + 8 * j == gc0 + 8 * i + 1) v[4 * i + 2 * j + 1] = 0.f;
-          }
-      }
-      if (kPost == POST_CLAMP_SQRT) {
-#pragma unroll
-        for (int c = 0; c < 64; ++c) asm("sqrt.approx.f32 %0, %1;" : "=f"(v[c]) : "f"(v[c]));
-      }
-    }
+    if (tc_post_clamps(kPost) && (p.acc_mode == 0 || p.acc_mode == 3)) tc_finish<kPost, false>(v, p, row0, gc0);
     if constexpr (tc_post_gram(kPost)) {
       if (p.acc_mode == 0 || p.acc_mode == 3) {   // (K-chunked: the earlier chunks store the partial sum untransformed)
 #pragma unroll
@@ -412,7 +398,7 @@ __device__ __forceinline__ void tc_epilogue(float (&v)[64], const TcParams& p, c
   }
 }
 
-// EPI_STORE through TMA, the common case (one warp-uniform test in the kernel: p.tma_store, p.acc_mode == 0, no diag_zero,
+// EPI_STORE through TMA, the common case (one warp-uniform test in the kernel: p.tma_store, p.acc_mode == 0, no self pairs,
 // no per-column scales): tc_epilogue's arithmetic for it, without the branches of the other cases.  Ragged tiles take it
 // too: TMA clips what lies outside the matrix.  The kernel keeps the Gram matrices off it (kFastPost): a second inlined
 // copy of their expf / tanhf made the tanh instantiation spill.
@@ -698,7 +684,7 @@ expanded_tc_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_cons
   const bool xnu = __ldg(&p.nonuni[0]) != 0u, ynu = __ldg(&p.nonuni[1]) != 0u;
   // EPI_STORE through TMA in one pass, without the diagonal or per-column scales: tc_epilogue_store_fast
   constexpr bool kFastPost = !tc_post_gram(kPost);
-  const bool fast_store    = kEpi == EPI_STORE && kFastPost && p.tma_store && p.acc_mode == 0 && !p.diag_zero && !ynu;
+  const bool fast_store    = kEpi == EPI_STORE && kFastPost && p.tma_store && p.acc_mode == 0 && p.diag_off == TC_NO_DIAG && !ynu;
   // the x ring this warpgroup reads: resident, its own (its rows of every stage); streaming, the one both read
   const int ring = kResident ? wg : 0;
   // Resident: ordered MMA turns.  Both warpgroups walk the same (item, tile, half) units; warpgroup w takes its turn at

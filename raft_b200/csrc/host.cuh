@@ -104,12 +104,25 @@ TcWorkspace tc_layout(void* base, int64_t m, int64_t n, int64_t k, bool with_key
 // w with side 0 (x) or side 1 (y) starting at prepared row r0: the operand, t and scale rows the tensor kernels read
 TcWorkspace tc_rows(TcWorkspace w, int side, int64_t r0, int64_t k);
 
+// How the tensor path computes an expanded metric: the operand preparation (PrepParams: mode, center, xform, coef_mul,
+// tx_const) and the epilogue's post-processing (TcPost)
+struct TcMetric {
+  int mode, center, post, xform;
+  float coef_mul, tx_const;
+};
+constexpr TcMetric TC_L2{PREP_L2, 0, POST_CLAMP, 0, 1.f, 0.f};   // L2Expanded
+// *out for `metric` with k columns; false: the metric is not on the tensor path
+bool tc_metric(int metric, int64_t k, TcMetric* out);
+// TcParams::diag_off of the operands x [m] and y [n] (element strides as launch_prep takes them): 0 when they are the same
+// matrix and the metric's distance is the clamped L2 one (d(i, i) = 0 exactly), TC_NO_DIAG otherwise
+int64_t tc_self_diag(const TcMetric& tm, const void* x, int64_t xrs, int64_t xcs, int64_t m, const void* y, int64_t yrs,
+                     int64_t ycs, int64_t n);
+
 // operand preparation (prep.cuh) of x [m, k] and y [n, k] into w; T is float or __half
 template <typename T>
 int launch_prep(cudaStream_t s, const TcWorkspace& w, const void* x, int64_t xrs, int64_t xcs, int64_t m,
                 const void* y, int64_t yrs, int64_t ycs, int64_t n, int64_t k, const float* xn, const float* yn,
-                int mode, int center, int xform = 0, float coef_mul = 1.f, float tx_const = 0.f,
-                const int* y_gather = nullptr, bool y_only = false, const unsigned* run_flag = nullptr);
+                const TcMetric& tm, const int* y_gather = nullptr, bool y_only = false, const unsigned* run_flag = nullptr);
 
 // one expanded_tc_kernel launch (K chunk [kb0, kb0 + nkb_chunk) when nkb_chunk > 0)
 int launch_tc(cudaStream_t s, const TcWorkspace& w, TcParams p, int64_t k, int epi, int post, int kb0 = 0,

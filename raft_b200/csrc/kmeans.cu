@@ -2,7 +2,6 @@
 #include <cuda_runtime.h>
 #include <algorithm>
 #include <cmath>
-#include <cstring>
 #include <string>
 
 #include "host.cuh"
@@ -152,12 +151,10 @@ static int km_assign(cudaStream_t s, const KmLayout& L, int64_t m, int64_t k, in
                                                            hist ? L.sort.hist : nullptr, nh);
   B2D_CUDA(cudaGetLastError());
   if (prep_y) {
-    int rc = launch_prep<float>(s, L.tc, nullptr, 0, 1, m, c, k, 1, nc, k, nullptr, nullptr, PREP_L2, 0, 0, 1.f, 0.f,
-                                nullptr, true, run);
+    int rc = launch_prep<float>(s, L.tc, nullptr, 0, 1, m, c, k, 1, nc, k, nullptr, nullptr, TC_L2, nullptr, true, run);
     if (rc) return rc;
   }
-  TcParams p;
-  memset(&p, 0, sizeof(p));
+  TcParams p{};
   p.m = m; p.n = nc; p.keys = L.tc.keys; p.run_flag = run;
   int rc = launch_tc(s, L.tc, p, k, EPI_MINLOC, POST_NONE);
   if (rc) return rc;
@@ -266,7 +263,7 @@ int b2d_kmeans_fit(void* stream, int n_clusters, int max_iter, double tol, int i
     km_fit_begin_kernel<<<1, 1, 0, s>>>(L.ctrl);
     B2D_CUDA(cudaGetLastError());
     if (r == 0) {   // x is prepared once per fit; every iteration prepares the centroids alone
-      rc = launch_prep<float>(s, L.tc, x, ldx, 1, m, centroids, k, 1, nc, k, nullptr, nullptr, PREP_L2, 0);
+      rc = launch_prep<float>(s, L.tc, x, ldx, 1, m, centroids, k, 1, nc, k, nullptr, nullptr, TC_L2);
       if (rc) return rc;
     }
     for (int it = 0; it < max_iter; ++it) {
@@ -316,7 +313,7 @@ int b2d_kmeans_predict(void* stream, const float* x, int64_t ldx, const float* s
   B2D_CUDA(cudaGetLastError());
   const float* w = km_weights(s, L, sample_weight, m, normalize_weight != 0);
   B2D_CUDA(cudaGetLastError());
-  rc = launch_prep<float>(s, L.tc, x, ldx, 1, m, centroids, k, 1, nc, k, nullptr, nullptr, PREP_L2, 0);
+  rc = launch_prep<float>(s, L.tc, x, ldx, 1, m, centroids, k, 1, nc, k, nullptr, nullptr, TC_L2);
   if (rc) return rc;
   int* lab = labels ? labels : L.labels;
   rc = km_assign(s, L, m, k, nc, centroids, w, lab, nullptr, false, false);

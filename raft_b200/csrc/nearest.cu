@@ -4,7 +4,6 @@
 #include <dlfcn.h>
 #include <algorithm>
 #include <atomic>
-#include <cstring>
 #include <mutex>
 #include <string>
 #include <vector>
@@ -69,13 +68,14 @@ size_t b2d_fused_l2_nn_workspace_bytes(int64_t m, int64_t n, int64_t k)
 // one chunk of y (prep + search); keys carry the result so far (and act as the rows' bounds)
 static int fused_nn_keys_chunk(cudaStream_t s, int64_t* keys, const float* x, int64_t ldx, const float* y, int64_t ldy,
                                const float* xn, const float* yn, int64_t m, int64_t n, int64_t k, int64_t idx_offset,
-                               void* workspace, int mode, int center, bool allow_screen, bool have_bounds)
+                               void* workspace, const TcMetric& tm, bool allow_screen, bool have_bounds)
 {
   TcWorkspace w = tc_layout(workspace, m, n, k, true);
   const int nkb = static_cast<int>((k + 31) / 32);
   // (k <= 64: the exact kernel is already epilogue-bound, screening would not pay)
-  const bool screen = (mode == PREP_L2 || mode == PREP_COSINE) && nkb >= 3 && nkb <= TC_MAX_RES_KB && n >= 16384 && allow_screen;
-  const int unit_norm = mode == PREP_COSINE ? 1 : 0;
+  const bool screen = (tm.mode == PREP_L2 || tm.mode == PREP_COSINE) && nkb >= 3 && nkb <= TC_MAX_RES_KB && n >= 16384 &&
+                      allow_screen;
+  const int unit_norm = tm.mode == PREP_COSINE ? 1 : 0;
   // The coarse pass bounds a whole 32-column group at once: c * max_j(acc_ij) + min_j |y_j|^2 (screen_tc.cuh).  That is
   // only tight when the rows of a group have nearly equal norms, so the L2 search packs the chunk in the order of
   // its squared row norms (stable radix sort on the top 24 bits of the fp32 norm: deterministic); the kernels
@@ -94,11 +94,10 @@ static int fused_nn_keys_chunk(cudaStream_t s, int64_t* keys, const float* x, in
     B2D_CUDA(cub::DeviceRadixSort::SortPairs(w.sort_tmp, tmp_need, dk, dv, static_cast<int>(n), 8, 32, s));
     col_map = dv.Current();
   }
-  int rc = launch_prep<float>(s, w, x, ldx, 1, m, y, ldy, 1, n, k, xn, yn, mode, center, 0, 1.f, 0.f, col_map);
+  int rc = launch_prep<float>(s, w, x, ldx, 1, m, y, ldy, 1, n, k, xn, yn, tm, col_map);
   if (rc) return rc;
   if (n == 0) return B2D_OK;
-  TcParams p;
-  memset(&p, 0, sizeof(p));
+  TcParams p{};
   p.m = m; p.n = n; p.keys = reinterpret_cast<long long*>(keys); p.idx_offset = idx_offset;
   p.col_map = col_map;
   if (!screen) return launch_tc(s, w, p, k, EPI_MINLOC, POST_NONE);
@@ -144,7 +143,7 @@ static int fused_nn_keys_chunk(cudaStream_t s, int64_t* keys, const float* x, in
   rc = device_sms(&sms);
   if (rc) return rc;
   nn_exact_kernel<<<sms * 8, 256, 0, s>>>(reinterpret_cast<long long*>(keys), w.cand, w.cand_cnt, w.cand_cap, x, ldx, y,
-                                          ldy, static_cast<int>(k), idx_offset, unit_norm, center, static_cast<unsigned>(m), col_map);
+                                          ldy, static_cast<int>(k), idx_offset, unit_norm, tm.center, static_cast<unsigned>(m), col_map);
   B2D_CUDA(cudaGetLastError());
   p.sel_lo = have_bounds ? 0 : 1; p.sel_hi = kSel; p.run_flag = flags + 3;
   rc = launch_tc(s, w, p, k, EPI_MINLOC, POST_NONE);
@@ -154,7 +153,7 @@ static int fused_nn_keys_chunk(cudaStream_t s, int64_t* keys, const float* x, in
 
 static int fused_nn_keys(void* stream, int64_t* keys, const float* x, int64_t ldx, const float* y, int64_t ldy,
                          const float* xn, const float* yn, int64_t m, int64_t n, int64_t k, int64_t idx_offset,
-                         int init_keys, void* workspace, size_t workspace_bytes, int mode, int center)
+                         int init_keys, void* workspace, size_t workspace_bytes, const TcMetric& tm)
 {
   cudaStream_t s = static_cast<cudaStream_t>(stream);
   if (m < 0 || n < 0 || k < 0) return fail(B2D_ERR_INVALID_ARG, "negative extent");
@@ -173,15 +172,15 @@ static int fused_nn_keys(void* stream, int64_t* keys, const float* x, int64_t ld
   // The screened search (below) works through y in chunks of 2^20 rows: the candidate list is sized per
   // chunk, and every chunk starts from the bounds the earlier ones left in the keys.
   const int nkb_all    = static_cast<int>((k + 31) / 32);
-  const bool screen_ok = (mode == PREP_L2 || mode == PREP_COSINE) && nkb_all >= 3 && nkb_all <= TC_MAX_RES_KB && !screen_off;
+  const bool screen_ok = (tm.mode == PREP_L2 || tm.mode == PREP_COSINE) && nkb_all >= 3 && nkb_all <= TC_MAX_RES_KB && !screen_off;
   constexpr int64_t kChunkRows = kNnChunkRows;
   if (!screen_ok || n <= kChunkRows)
-    return fused_nn_keys_chunk(s, keys, x, ldx, y, ldy, xn, yn, m, n, k, idx_offset, workspace, mode, center, screen_ok,
+    return fused_nn_keys_chunk(s, keys, x, ldx, y, ldy, xn, yn, m, n, k, idx_offset, workspace, tm, screen_ok,
                                init_keys == 0);
   for (int64_t off = 0; off < n; off += kChunkRows) {
     const int64_t nc = std::min<int64_t>(kChunkRows, n - off);
     int rc = fused_nn_keys_chunk(s, keys, x, ldx, y + off * ldy, ldy, xn, yn ? yn + off : nullptr, m, nc, k,
-                                 idx_offset + off, workspace, mode, center, true, init_keys == 0 || off > 0);
+                                 idx_offset + off, workspace, tm, true, init_keys == 0 || off > 0);
     if (rc) return rc;
   }
   return B2D_OK;
@@ -192,7 +191,7 @@ int b2d_fused_l2_nn_keys(void* stream, int64_t* keys, const float* x, int64_t ld
                          int init_keys, void* workspace, size_t workspace_bytes)
 {
   return fused_nn_keys(stream, keys, x, ldx, y, ldy, xn, yn, m, n, k, idx_offset, init_keys, workspace,
-                       workspace_bytes, PREP_L2, 0);
+                       workspace_bytes, TC_L2);
 }
 
 int b2d_fused_l2_nn_finalize(void* stream, b2d_kvp_if* out, const int64_t* keys, int64_t m, int do_sqrt,
@@ -211,11 +210,12 @@ int b2d_fused_l2_nn_finalize(void* stream, b2d_kvp_if* out, const int64_t* keys,
   return B2D_OK;
 }
 
-// fusedL2NN and fusedDistanceNN: the keys of every row in the workspace, then unpacked into out.  (The cosine family,
-// mode PREP_COSINE: rows are normalised in prep, keys hold -cos, the row term t_x = 1 turns it into 1 - cos.)
+// fusedL2NN and fusedDistanceNN: the keys of every row in the workspace, then unpacked into out (the square root taken
+// for POST_CLAMP_SQRT).  (The cosine family, mode PREP_COSINE: rows are normalised in prep, keys hold -cos, the row term
+// t_x = 1 turns it into 1 - cos.)
 static int fused_nn(void* stream, b2d_kvp_if* out, const float* x, int64_t ldx, const float* y, int64_t ldy,
-                    const float* xn, const float* yn, int64_t m, int64_t n, int64_t k, int mode, int center, int do_sqrt,
-                    int init_out, void* workspace, size_t workspace_bytes)
+                    const float* xn, const float* yn, int64_t m, int64_t n, int64_t k, const TcMetric& tm, int init_out,
+                    void* workspace, size_t workspace_bytes)
 {
   cudaStream_t s = static_cast<cudaStream_t>(stream);
   if (m < 0 || n < 0 || k < 0) return fail(B2D_ERR_INVALID_ARG, "negative extent");
@@ -226,10 +226,10 @@ static int fused_nn(void* stream, b2d_kvp_if* out, const float* x, int64_t ldx, 
   if (rc) return rc;
   TcWorkspace w = tc_layout(workspace, m, n, k, true);
   rc = fused_nn_keys(stream, reinterpret_cast<int64_t*>(w.keys), x, ldx, y, ldy, xn, yn, m, n, k, 0, 1, workspace,
-                     workspace_bytes, mode, center);
+                     workspace_bytes, tm);
   if (rc) return rc;
   minloc_finalize_kernel<<<static_cast<unsigned>((m + 255) / 256), 256, 0, s>>>(
-    reinterpret_cast<KvpIF*>(out), w.keys, m, do_sqrt, init_out ? 0 : 1);
+    reinterpret_cast<KvpIF*>(out), w.keys, m, tm.post == POST_CLAMP_SQRT ? 1 : 0, init_out ? 0 : 1);
   B2D_CUDA(cudaGetLastError());
   return B2D_OK;
 }
@@ -238,7 +238,9 @@ int b2d_fused_l2_nn(void* stream, b2d_kvp_if* out, const float* x, int64_t ldx, 
                     const float* xn, const float* yn, int64_t m, int64_t n, int64_t k, int do_sqrt, int init_out,
                     void* workspace, size_t workspace_bytes)
 {
-  return fused_nn(stream, out, x, ldx, y, ldy, xn, yn, m, n, k, PREP_L2, 0, do_sqrt, init_out, workspace, workspace_bytes);
+  TcMetric tm;
+  tc_metric(do_sqrt ? B2D_L2SqrtExpanded : B2D_L2Expanded, k, &tm);
+  return fused_nn(stream, out, x, ldx, y, ldy, xn, yn, m, n, k, tm, init_out, workspace, workspace_bytes);
 }
 
 // ------------------------------------------------------------------------------------------
@@ -332,13 +334,14 @@ int b2d_fused_distance_nn(void* stream, b2d_kvp_if* out, int metric, const float
                           int64_t ldy, const float* xn, const float* yn, int64_t m, int64_t n, int64_t k, int init_out,
                           void* workspace, size_t workspace_bytes)
 {
-  if (metric == B2D_L2Expanded || metric == B2D_L2SqrtExpanded)
-    return b2d_fused_l2_nn(stream, out, x, ldx, y, ldy, xn, yn, m, n, k, metric == B2D_L2SqrtExpanded ? 1 : 0, init_out,
-                           workspace, workspace_bytes);
-  if (metric != B2D_CosineExpanded && metric != B2D_CorrelationExpanded)
+  TcMetric tm;
+  if ((metric != B2D_L2Expanded && metric != B2D_L2SqrtExpanded && metric != B2D_CosineExpanded &&
+       metric != B2D_CorrelationExpanded) || !tc_metric(metric, k, &tm))
     return fail(B2D_ERR_UNSUPPORTED, "fusedDistanceNN supports L2Expanded, L2SqrtExpanded, CosineExpanded, CorrelationExpanded");
-  return fused_nn(stream, out, x, ldx, y, ldy, nullptr, nullptr, m, n, k, PREP_COSINE,
-                  metric == B2D_CorrelationExpanded ? 1 : 0, 0, init_out, workspace, workspace_bytes);
+  // (xn / yn are the squared norms of the L2 metrics; the cosine family computes its own)
+  const bool l2 = tm.mode == PREP_L2;
+  return fused_nn(stream, out, x, ldx, y, ldy, l2 ? xn : nullptr, l2 ? yn : nullptr, m, n, k, tm, init_out, workspace,
+                  workspace_bytes);
 }
 
 // ------------------------------------------------------------------------------------------
@@ -381,8 +384,7 @@ int masked_keys(cudaStream_t s, const TcWorkspace& w, long long* keys, const int
   masked_classify_kernel<<<static_cast<unsigned>((ntiles + 255) / 256), 256, 0, s>>>(cls, bits, group_idxs, G, m, n,
                                                                                      tiles_m, tiles_n, bad);
   B2D_CUDA(cudaGetLastError());
-  TcParams p;
-  memset(&p, 0, sizeof(p));
+  TcParams p{};
   p.m = m; p.n = n; p.keys = keys;
   p.mask_cls = cls; p.mask_grp = grp; p.mask_bits = bits; p.mask_groups = G;
   ProfileScope prof(s);
@@ -420,7 +422,7 @@ int b2d_masked_l2_nn(void* stream, b2d_kvp_if* out, const float* x, int64_t ldx,
   masked_validate_kernel<<<1, 1024, 0, s>>>(L.bad, group_idxs, G, n);
   B2D_CUDA(cudaGetLastError());
   if (n > 0 && G > 0) {
-    rc = launch_prep<float>(s, L.w, x, ldx, 1, m, y, ldy, 1, n, k, xn, yn, PREP_L2, 0);
+    rc = launch_prep<float>(s, L.w, x, ldx, 1, m, y, ldy, 1, n, k, xn, yn, TC_L2);
     if (rc) return rc;
     masked_group_map_kernel<<<static_cast<unsigned>((n + 255) / 256), 256, 0, s>>>(L.grp, group_idxs, G, n);
     B2D_CUDA(cudaGetLastError());

@@ -1,7 +1,6 @@
 // Fused brute-force kNN (knn.cuh) and the epsilon neighbourhood, both on the tensor path without the m x n matrix.
 #include <cuda_runtime.h>
 #include <algorithm>
-#include <cstring>
 
 #include "host.cuh"
 #include "knn.cuh"
@@ -93,12 +92,12 @@ int b2d_knn(void* stream, int64_t* out_idx, float* out_dist, int metric, const f
             int64_t ldy, int64_t m, int64_t n, int64_t k, int64_t n_neighbors, void* workspace, size_t workspace_bytes)
 {
   cudaStream_t s = static_cast<cudaStream_t>(stream);
-  int mode = PREP_L2, center = 0, do_sqrt = 0;
-  if (metric == B2D_L2Expanded || metric == B2D_L2Unexpanded) {}
-  else if (metric == B2D_L2SqrtExpanded || metric == B2D_L2SqrtUnexpanded) do_sqrt = 1;
-  else if (metric == B2D_CosineExpanded) mode = PREP_COSINE;
-  else if (metric == B2D_CorrelationExpanded) { mode = PREP_COSINE; center = 1; }
-  else return fail(B2D_ERR_UNSUPPORTED, "kNN supports the L2 metrics, CosineExpanded and CorrelationExpanded");
+  if (metric == B2D_L2Unexpanded) metric = B2D_L2Expanded;   // (the same distance)
+  if (metric == B2D_L2SqrtUnexpanded) metric = B2D_L2SqrtExpanded;
+  TcMetric tm;
+  if ((metric != B2D_L2Expanded && metric != B2D_L2SqrtExpanded && metric != B2D_CosineExpanded &&
+       metric != B2D_CorrelationExpanded) || !tc_metric(metric, k, &tm))
+    return fail(B2D_ERR_UNSUPPORTED, "kNN supports the L2 metrics, CosineExpanded and CorrelationExpanded");
   if (m < 0 || n < 0 || k < 0) return fail(B2D_ERR_INVALID_ARG, "negative extent");
   if (n_neighbors < 1 || n_neighbors > n) return fail(B2D_ERR_INVALID_ARG, "n_neighbors must be in [1, n]");
   if (n_neighbors > KNN_MAX_K) return fail(B2D_ERR_UNSUPPORTED, "n_neighbors > 64 is not supported");
@@ -119,14 +118,14 @@ int b2d_knn(void* stream, int64_t* out_idx, float* out_dist, int metric, const f
   c.k   = k;
   c.kk  = static_cast<int>(n_neighbors);
   c.pass = 0; c.any_fix = false; c.x = x; c.ldx = ldx; c.y = y; c.ldy = ldy;
-  c.family = mode == PREP_COSINE ? 1 : 0; c.center = center;
+  c.family = tm.mode == PREP_COSINE ? 1 : 0; c.center = tm.center;
   const KnnLayout& L = c.L;
-  rc = launch_prep<float>(s, L.w, x, ldx, 1, m, y, ldy, 1, n, k, nullptr, nullptr, mode, center);
+  rc = launch_prep<float>(s, L.w, x, ldx, 1, m, y, ldy, 1, n, k, nullptr, nullptr, tm);
   if (rc) return rc;
   const int64_t total = m * n_neighbors;
   knn_init_kernel<<<static_cast<unsigned>((std::max<int64_t>(std::max<int64_t>(total, m), 65) + 255) / 256), 256, 0, s>>>(L.topk, L.thr, L.cnt, L.dropmin, L.dirty_cnt, L.repaired, m, c.kk);
   B2D_CUDA(cudaGetLastError());
-  memset(&c.p, 0, sizeof(c.p));
+  c.p   = TcParams{};
   c.p.m = m;
   c.p.knn_thr = L.thr; c.p.knn_cnt = L.cnt; c.p.knn_cand = reinterpret_cast<long long*>(L.w.cand);
   c.p.knn_cap = KNN_CAP; c.p.knn_dropmin = L.dropmin;
@@ -147,7 +146,8 @@ int b2d_knn(void* stream, int64_t* out_idx, float* out_dist, int metric, const f
                                            c.family, c.center);
     B2D_CUDA(cudaGetLastError());
   }
-  knn_finalize_kernel<<<static_cast<unsigned>((total + 255) / 256), 256, 0, s>>>(out_idx, out_dist, L.topk, total, do_sqrt);
+  knn_finalize_kernel<<<static_cast<unsigned>((total + 255) / 256), 256, 0, s>>>(out_idx, out_dist, L.topk, total,
+                                                                                 tm.post == POST_CLAMP_SQRT ? 1 : 0);
   B2D_CUDA(cudaGetLastError());
   return B2D_OK;
 }
@@ -183,14 +183,12 @@ int b2d_eps_neighbors_l2sq(void* stream, uint8_t* adj, int64_t ld_adj, void* vd,
   if (vd && init_vd) B2D_CUDA(cudaMemsetAsync(vd, 0, static_cast<size_t>(n + 1) * (vd_int64 ? 8 : 4), s));
   if (!work) return B2D_OK;
   TcWorkspace w = tc_layout(workspace, m, n, k, false);
-  int rc = launch_prep<float>(s, w, x, ldx, 1, m, y, ldy, 1, n, k, nullptr, nullptr, PREP_L2, 0);
+  int rc = launch_prep<float>(s, w, x, ldx, 1, m, y, ldy, 1, n, k, nullptr, nullptr, TC_L2);
   if (rc) return rc;
-  TcParams p;
-  memset(&p, 0, sizeof(p));
+  TcParams p{};
   p.m = m; p.n = n;
   p.adj = adj; p.ld_adj = ld_adj; p.vd = vd; p.vd64 = vd_int64 ? 1 : 0; p.eps = eps;
   // y is a window of x's rows (same memory, same pitch): row j of y is row j + off of x
-  p.diag_off = TC_NO_DIAG;
   const intptr_t dy = reinterpret_cast<intptr_t>(y) - reinterpret_cast<intptr_t>(x);
   if (ldx == ldy && dy % (ldx * static_cast<intptr_t>(sizeof(float))) == 0)
     p.diag_off = dy / (ldx * static_cast<intptr_t>(sizeof(float)));

@@ -13,12 +13,6 @@
 
 namespace b2d {
 
-static bool is_expanded(int metric)
-{
-  return metric == B2D_L2Expanded || metric == B2D_L2SqrtExpanded || metric == B2D_CosineExpanded ||
-         metric == B2D_CorrelationExpanded || metric == B2D_InnerProduct || metric == B2D_HellingerExpanded ||
-         metric == B2D_RusselRaoExpanded || metric == B2D_JaccardExpanded || metric == B2D_DiceExpanded;
-}
 static bool is_unexpanded(int metric)
 {
   return metric == B2D_L1 || metric == B2D_L2Unexpanded || metric == B2D_L2SqrtUnexpanded ||
@@ -97,44 +91,31 @@ static int pairwise_f64(cudaStream_t s, int metric, const double* x, int64_t xrs
   }
 }
 
-// What one dense m x n result on the tensor path (EPI_STORE) is made of: the operand preparation (prep.cuh) and the
-// epilogue's post-processing, with the kernel parameters of the Gram matrices (gram_post).
-struct TcStore {
-  int mode = PREP_L2, center = 0, post = POST_NONE, xform = 0;
-  float coef_mul = 1.f, tx_const = 0.f;
-  float gamma = 0.f, coef0 = 0.f;
-  int degree = 0;
-};
-
 // The tensor path of b2d_pairwise_distance and b2d_gram_matrix: x [ma, k] and y [na, k] with element strides (xrs, xcs) and
-// (yrs, ycs) (a column-major call arrives with the operands exchanged), dist [ma][ldd].  alias: x and y are the same matrix
-// (then the L2 family has d(i, i) = 0 exactly).
-static int tc_store(cudaStream_t s, const TcStore& c, int dtype, const void* xa, int64_t xrs, int64_t xcs, int64_t ma,
-                    const void* ya, int64_t yrs, int64_t ycs, int64_t na, int64_t k, float* dist, int64_t ldd, bool alias,
-                    void* workspace, size_t workspace_bytes)
+// (yrs, ycs) (a column-major call arrives with the operands exchanged), dist [ma][ldd]; gamma, coef0 and degree are the
+// kernel parameters of the Gram matrices (gram_post).
+static int tc_store(cudaStream_t s, const TcMetric& tm, float gamma, float coef0, int degree, int dtype, const void* xa,
+                    int64_t xrs, int64_t xcs, int64_t ma, const void* ya, int64_t yrs, int64_t ycs, int64_t na, int64_t k,
+                    float* dist, int64_t ldd, void* workspace, size_t workspace_bytes)
 {
   int rc = check_workspace(workspace, workspace_bytes, tc_layout(nullptr, ma, na, k, false).bytes);
   if (rc) return rc;
   TcWorkspace w = tc_layout(workspace, ma, na, k, false);
-  rc = dtype == B2D_F32
-         ? launch_prep<float>(s, w, xa, xrs, xcs, ma, ya, yrs, ycs, na, k, nullptr, nullptr, c.mode, c.center, c.xform,
-                              c.coef_mul, c.tx_const)
-         : launch_prep<__half>(s, w, xa, xrs, xcs, ma, ya, yrs, ycs, na, k, nullptr, nullptr, c.mode, c.center, c.xform,
-                               c.coef_mul, c.tx_const);
+  rc = dtype == B2D_F32 ? launch_prep<float>(s, w, xa, xrs, xcs, ma, ya, yrs, ycs, na, k, nullptr, nullptr, tm)
+                        : launch_prep<__half>(s, w, xa, xrs, xcs, ma, ya, yrs, ycs, na, k, nullptr, nullptr, tm);
   if (rc) return rc;
-  TcParams p;
-  memset(&p, 0, sizeof(p));
+  TcParams p{};
   p.m = ma; p.n = na; p.dist = dist; p.ldd = ldd;
-  p.diag_zero = (c.post != POST_NONE && alias && c.mode == PREP_L2) ? 1 : 0;
-  p.gamma = c.gamma; p.coef0 = c.coef0; p.degree = c.degree;
+  p.diag_off = tc_self_diag(tm, xa, xrs, xcs, ma, ya, yrs, ycs, na);
+  p.gamma = gamma; p.coef0 = coef0; p.degree = degree;
   // (dispatch_plan.cuh: TMA or register stores; k > 320: K chunks accumulated in dist, post-processed on the last)
-  const TcStorePlan pl = tc_store_plan(c.post, ma, na, k, reinterpret_cast<uintptr_t>(dist), ldd);
+  const TcStorePlan pl = tc_store_plan(tm.post, ma, na, k, reinterpret_cast<uintptr_t>(dist), ldd);
   p.tma_store = pl.tma_store;
   ProfileScope prof(s);  // the main kernel(s) only: the operand preparation above is outside
   for (int i = 0; i < pl.launches; ++i) {
     const TcStoreLaunch l = tc_store_launch(pl, i);
     p.acc_mode = l.acc_mode;
-    rc = launch_tc(s, w, p, k, EPI_STORE, c.post, l.kb0, l.nkb);
+    rc = launch_tc(s, w, p, k, EPI_STORE, tm.post, l.kb0, l.nkb);
     if (rc) return rc;
   }
   return B2D_OK;
@@ -144,10 +125,12 @@ size_t b2d_pairwise_workspace_bytes(int metric, int dtype, int64_t m, int64_t n,
 {
   if (dtype != B2D_F32 && dtype != B2D_F16 && dtype != B2D_F64) return static_cast<size_t>(-1);
   if (m < 0 || n < 0 || k < 0) return static_cast<size_t>(-1);
+  TcMetric tm;
+  const bool expanded = tc_metric(metric, k, &tm);
   if (dtype == B2D_F64)   // per-row (sum, sum of squares) of x and y
-    return (is_expanded(metric) || is_unexpanded(metric)) ? align_up(static_cast<size_t>(m + n) * 16, 1024) : static_cast<size_t>(-1);
+    return (expanded || is_unexpanded(metric)) ? align_up(static_cast<size_t>(m + n) * 16, 1024) : static_cast<size_t>(-1);
   if (is_unexpanded(metric)) return dtype == B2D_F32 ? 0 : static_cast<size_t>(-1);
-  if (!is_expanded(metric)) return static_cast<size_t>(-1);
+  if (!expanded) return static_cast<size_t>(-1);
   return tc_layout(nullptr, m, n, k, false).bytes;
 }
 
@@ -166,11 +149,13 @@ static int pairwise_check(int metric, int dtype, const void* x, int64_t ldx, con
   } else {
     if (ldx < m || ldy < n || ldd < m) return fail(B2D_ERR_INVALID_ARG, "leading dimension smaller than the column length");
   }
-  if (!is_expanded(metric) && !is_unexpanded(metric))
+  TcMetric tm;
+  const bool expanded = tc_metric(metric, k, &tm);
+  if (!expanded && !is_unexpanded(metric))
     return fail(B2D_ERR_UNSUPPORTED, "metric " + std::to_string(metric) + " is not on the tensor-core / SIMT distance path");
   if (dtype != B2D_F32 && dtype != B2D_F16 && dtype != B2D_F64) return fail(B2D_ERR_UNSUPPORTED, "dtype");
   if (metric == B2D_LpUnexpanded && !(metric_arg > 0.f)) return fail(B2D_ERR_INVALID_ARG, "LpUnexpanded needs p > 0");
-  if (dtype == B2D_F16 && !is_expanded(metric)) return fail(B2D_ERR_UNSUPPORTED, "unexpanded metrics take fp32 inputs");
+  if (dtype == B2D_F16 && !expanded) return fail(B2D_ERR_UNSUPPORTED, "unexpanded metrics take fp32 inputs");
   return B2D_OK;
 }
 
@@ -188,22 +173,6 @@ static PairwiseOperands pairwise_operands(const void* x, int64_t ldx, const void
   return PairwiseOperands{y, x, n, m, 1, ldy, 1, ldx};
 }
 
-// preparation and epilogue of the expanded metrics on the tensor path
-static TcStore pairwise_tc_store(int metric, int64_t k)
-{
-  TcStore c;
-  if (metric == B2D_L2Expanded) { c.post = POST_CLAMP; }
-  else if (metric == B2D_L2SqrtExpanded) { c.post = POST_CLAMP_SQRT; }
-  else if (metric == B2D_CosineExpanded) { c.mode = PREP_COSINE; }
-  else if (metric == B2D_CorrelationExpanded) { c.mode = PREP_COSINE; c.center = 1; }
-  else if (metric == B2D_HellingerExpanded) { c.mode = PREP_INNER; c.post = POST_CLAMP_SQRT; c.xform = 1; c.coef_mul = -1.f; c.tx_const = 1.f; }
-  else if (metric == B2D_RusselRaoExpanded) { c.mode = PREP_INNER; c.coef_mul = -1.f / static_cast<float>(k); c.tx_const = 1.f; }
-  else if (metric == B2D_JaccardExpanded) { c.mode = PREP_INNER_NORM; c.post = POST_JACCARD; }
-  else if (metric == B2D_DiceExpanded) { c.mode = PREP_INNER_NORM; c.post = POST_DICE; }
-  else { c.mode = PREP_INNER; }
-  return c;
-}
-
 int b2d_debug_pairwise_plan(int metric, int dtype, const void* x, int64_t ldx, const void* y, int64_t ldy, const void* dist,
                             int64_t ldd, int64_t m, int64_t n, int64_t k, int row_major, int* out, int out_len)
 {
@@ -215,8 +184,9 @@ int b2d_debug_pairwise_plan(int metric, int dtype, const void* x, int64_t ldx, c
   if (empty) { out[0] = B2D_PLAN_NONE; return B2D_OK; }
   if (dtype == B2D_F64) { out[0] = B2D_PLAN_F64_SIMT; return B2D_OK; }
   const PairwiseOperands o = pairwise_operands(x, ldx, y, ldy, m, n, row_major);
-  if (is_expanded(metric)) {
-    const TcStorePlan pl = tc_store_plan(pairwise_tc_store(metric, k).post, o.ma, o.na, k, reinterpret_cast<uintptr_t>(dist), ldd);
+  TcMetric tm;
+  if (tc_metric(metric, k, &tm)) {
+    const TcStorePlan pl = tc_store_plan(tm.post, o.ma, o.na, k, reinterpret_cast<uintptr_t>(dist), ldd);
     out[0] = B2D_PLAN_TENSOR; out[1] = pl.tma_store; out[2] = pl.vec2; out[5] = pl.launches;
     for (int i = 0; i < pl.launches && 6 + 4 * i + 3 < out_len; ++i) {
       const TcStoreLaunch l = tc_store_launch(pl, i);
@@ -247,9 +217,10 @@ int b2d_pairwise_distance(void* stream, int metric, int dtype, const void* x, in
                         static_cast<double*>(dist_v), ldd, n, m, k, 1, metric_arg, workspace, workspace_bytes);
   }
   const PairwiseOperands o = pairwise_operands(x, ldx, y, ldy, m, n, row_major);
-  if (is_expanded(metric))
-    return tc_store(s, pairwise_tc_store(metric, k), dtype, o.xa, o.xrs, o.xcs, o.ma, o.ya, o.yrs, o.ycs, o.na, k, dist, ldd,
-                    x == y && m == n && ldx == ldy, workspace, workspace_bytes);
+  TcMetric tm;
+  if (tc_metric(metric, k, &tm))
+    return tc_store(s, tm, 0.f, 0.f, 0, dtype, o.xa, o.xrs, o.xcs, o.ma, o.ya, o.yrs, o.ycs, o.na, k, dist, ldd, workspace,
+                    workspace_bytes);
 
   UxParams p;
   memset(&p, 0, sizeof(p));
@@ -325,16 +296,17 @@ int b2d_gram_matrix(void* stream, int kernel, int degree, double gamma, double c
     return pairwise_f64(s, metric, static_cast<const double*>(y), 1, ldy, static_cast<const double*>(x), 1, ldx,
                         static_cast<double*>(out), ldo, n, m, k, 1, 2.0, workspace, workspace_bytes, gamma, coef0, degree);
   }
-  // Fortran order: the row-major [n, m] matrix of K(y_j, x_i), the same values (every kernel is symmetric)
-  TcStore c;
-  c.mode   = kernel == B2D_KERNEL_RBF ? PREP_L2 : PREP_INNER;
-  c.post   = kernel == B2D_KERNEL_LINEAR ? POST_NONE
-           : kernel == B2D_KERNEL_POLYNOMIAL ? POST_POLY
-           : kernel == B2D_KERNEL_RBF ? POST_RBF : POST_TANH;
-  c.gamma  = static_cast<float>(gamma);
-  c.coef0  = static_cast<float>(coef0);
-  c.degree = degree;
-  const bool alias = x == y && m == n && ldx == ldy;
-  if (row_major) return tc_store(s, c, dtype, x, ldx, 1, m, y, ldy, 1, n, k, static_cast<float*>(out), ldo, alias, workspace, workspace_bytes);
-  return tc_store(s, c, dtype, y, 1, ldy, n, x, 1, ldx, m, k, static_cast<float*>(out), ldo, alias, workspace, workspace_bytes);
+  // the base metric's preparation, its value transformed by the kernel's post.  Fortran order: the row-major [n, m] matrix
+  // of K(y_j, x_i), the same values (every kernel is symmetric)
+  TcMetric tm;
+  tc_metric(gram_base_metric(kernel), k, &tm);
+  tm.post = kernel == B2D_KERNEL_LINEAR ? POST_NONE
+          : kernel == B2D_KERNEL_POLYNOMIAL ? POST_POLY
+          : kernel == B2D_KERNEL_RBF ? POST_RBF : POST_TANH;
+  const float g = static_cast<float>(gamma), c0 = static_cast<float>(coef0);
+  if (row_major)
+    return tc_store(s, tm, g, c0, degree, dtype, x, ldx, 1, m, y, ldy, 1, n, k, static_cast<float*>(out), ldo, workspace,
+                    workspace_bytes);
+  return tc_store(s, tm, g, c0, degree, dtype, y, 1, ldy, n, x, 1, ldx, m, k, static_cast<float*>(out), ldo, workspace,
+                  workspace_bytes);
 }

@@ -9,7 +9,6 @@
 #include <thrust/iterator/counting_iterator.h>
 #include <thrust/iterator/transform_iterator.h>
 #include <algorithm>
-#include <cstring>
 #include <string>
 
 #include "host.cuh"
@@ -52,20 +51,13 @@ RadiusLayout radius_layout(void* base, int64_t m, int64_t n, int64_t k, int64_t 
   return L;
 }
 
-// operand preparation and epilogue post of a metric: those of b2d_pairwise_distance
-struct RadiusMetric {
-  int mode, center, post;
-};
-
 // The argument checks both calls share.  *work: there are pairs to look at (m > 0 and n > 0).
 int radius_check(int metric, const int64_t* indptr, const float* x, int64_t ldx, const float* y, int64_t ldy, int64_t m,
-                 int64_t n, int64_t k, RadiusMetric* rm, bool* work)
+                 int64_t n, int64_t k, TcMetric* tm, bool* work)
 {
-  if (metric == B2D_L2Expanded) *rm = RadiusMetric{PREP_L2, 0, POST_CLAMP};
-  else if (metric == B2D_L2SqrtExpanded) *rm = RadiusMetric{PREP_L2, 0, POST_CLAMP_SQRT};
-  else if (metric == B2D_CosineExpanded) *rm = RadiusMetric{PREP_COSINE, 0, POST_NONE};
-  else if (metric == B2D_CorrelationExpanded) *rm = RadiusMetric{PREP_COSINE, 1, POST_NONE};
-  else
+  // (the distance of b2d_pairwise_distance)
+  if ((metric != B2D_L2Expanded && metric != B2D_L2SqrtExpanded && metric != B2D_CosineExpanded &&
+       metric != B2D_CorrelationExpanded) || !tc_metric(metric, k, tm))
     return fail(B2D_ERR_UNSUPPORTED, "radius_neighbors supports L2Expanded, L2SqrtExpanded, CosineExpanded and "
                                      "CorrelationExpanded, got metric " + std::to_string(metric));
   if (m < 0 || n < 0 || k < 0) return fail(B2D_ERR_INVALID_ARG, "negative extent");
@@ -80,16 +72,15 @@ int radius_check(int metric, const int64_t* indptr, const float* x, int64_t ldx,
   return B2D_OK;
 }
 
-// prep and the parameters of an EPI_RADIUS launch; x and y the same matrix under an L2 metric: d(i, i) = 0, as
-// b2d_pairwise_distance makes it
-int radius_prep(cudaStream_t s, const RadiusLayout& L, const RadiusMetric& rm, const float* x, int64_t ldx, const float* y,
+// prep and the parameters of an EPI_RADIUS launch, with the self pairs of b2d_pairwise_distance
+int radius_prep(cudaStream_t s, const RadiusLayout& L, const TcMetric& tm, const float* x, int64_t ldx, const float* y,
                 int64_t ldy, int64_t m, int64_t n, int64_t k, float radius, TcParams* p)
 {
-  const int rc = launch_prep<float>(s, L.w, x, ldx, 1, m, y, ldy, 1, n, k, nullptr, nullptr, rm.mode, rm.center);
+  const int rc = launch_prep<float>(s, L.w, x, ldx, 1, m, y, ldy, 1, n, k, nullptr, nullptr, tm);
   if (rc) return rc;
-  memset(p, 0, sizeof(*p));
+  *p = TcParams{};
   p->m = m; p->n = n; p->eps = radius;
-  p->diag_zero = (rm.post != POST_NONE && x == y && m == n && ldx == ldy) ? 1 : 0;
+  p->diag_off = tc_self_diag(tm, x, ldx, 1, m, y, ldy, 1, n);
   return B2D_OK;
 }
 
@@ -106,9 +97,9 @@ int b2d_radius_neighbors_count(void* stream, int64_t* indptr, int metric, const 
                                size_t workspace_bytes)
 {
   cudaStream_t s = static_cast<cudaStream_t>(stream);
-  RadiusMetric rm;
+  TcMetric tm;
   bool work = false;
-  int rc = radius_check(metric, indptr, x, ldx, y, ldy, m, n, k, &rm, &work);
+  int rc = radius_check(metric, indptr, x, ldx, y, ldy, m, n, k, &tm, &work);
   if (rc) return rc;
   if (work) {
     rc = check_workspace(workspace, workspace_bytes, radius_layout(nullptr, m, n, k, 0).bytes);
@@ -120,14 +111,14 @@ int b2d_radius_neighbors_count(void* stream, int64_t* indptr, int metric, const 
   }
   const RadiusLayout L = radius_layout(workspace, m, n, k, 0);
   TcParams p;
-  rc = radius_prep(s, L, rm, x, ldx, y, ldy, m, n, k, radius, &p);
+  rc = radius_prep(s, L, tm, x, ldx, y, ldy, m, n, k, radius, &p);
   if (rc) return rc;
   B2D_CUDA(cudaMemsetAsync(L.deg, 0, static_cast<size_t>(m + 1) * sizeof(unsigned), s));
   p.knn_cnt  = L.deg;
   p.rad_fill = 0;
   {
     ProfileScope prof(s);
-    rc = launch_tc(s, L.w, p, k, EPI_RADIUS, rm.post);
+    rc = launch_tc(s, L.w, p, k, EPI_RADIUS, tm.post);
     if (rc) return rc;
   }
   const thrust::transform_iterator<RadiusDeg64, const unsigned*, long long> deg(L.deg, RadiusDeg64{});
@@ -143,9 +134,9 @@ int b2d_radius_neighbors_fill(void* stream, const int64_t* indptr, int64_t nnz, 
                               int64_t k, float radius, void* workspace, size_t workspace_bytes)
 {
   cudaStream_t s = static_cast<cudaStream_t>(stream);
-  RadiusMetric rm;
+  TcMetric tm;
   bool work = false;
-  int rc = radius_check(metric, indptr, x, ldx, y, ldy, m, n, k, &rm, &work);
+  int rc = radius_check(metric, indptr, x, ldx, y, ldy, m, n, k, &tm, &work);
   if (rc) return rc;
   if (nnz < 0) return fail(B2D_ERR_INVALID_ARG, "negative nnz");
   if (nnz > 0x7fffffffll)
@@ -159,7 +150,7 @@ int b2d_radius_neighbors_fill(void* stream, const int64_t* indptr, int64_t nnz, 
   if (!work || nnz == 0 || !(radius >= 0.f)) return B2D_OK;
   const RadiusLayout L = radius_layout(workspace, m, n, k, nnz);
   TcParams p;
-  rc = radius_prep(s, L, rm, x, ldx, y, ldy, m, n, k, radius, &p);
+  rc = radius_prep(s, L, tm, x, ldx, y, ldy, m, n, k, radius, &p);
   if (rc) return rc;
   B2D_CUDA(cudaMemsetAsync(L.fill, 0, static_cast<size_t>(m) * sizeof(unsigned), s));
   p.knn_cnt    = L.fill;
@@ -169,7 +160,7 @@ int b2d_radius_neighbors_fill(void* stream, const int64_t* indptr, int64_t nnz, 
   p.rad_fill   = 1;
   {
     ProfileScope prof(s);
-    rc = launch_tc(s, L.w, p, k, EPI_RADIUS, rm.post);
+    rc = launch_tc(s, L.w, p, k, EPI_RADIUS, tm.post);
     if (rc) return rc;
   }
   // every row's keys in ascending order (they are distinct: one per column), segments clipped to the nnz slots

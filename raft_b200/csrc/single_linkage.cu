@@ -203,7 +203,7 @@ static int sl_connect(cudaStream_t s, const SlLayout& L, const float* x, int64_t
   km_gather_rows(s, static_cast<unsigned>(m), x, ldx, static_cast<int>(d), S.perm, static_cast<int>(m), L.xs);
   B2D_CUDA(cudaGetLastError());
   // y (and x) prepared once per round; every chunk takes a window of the x side
-  rc = launch_prep<float>(s, L.tc, L.xs, d, 1, m, L.xs, d, 1, m, d, nullptr, nullptr, PREP_L2, 0);
+  rc = launch_prep<float>(s, L.tc, L.xs, d, 1, m, L.xs, d, 1, m, d, nullptr, nullptr, TC_L2);
   if (rc) return rc;
   masked_group_map(s, sl_grid(m), L.grp, L.ends, c, m);
   B2D_CUDA(cudaMemsetAsync(L.bad, 0, 32, s));

@@ -57,6 +57,7 @@ __host__ __device__ constexpr bool tc_post_gram(int post) { return post == POST_
 // EPI_STORE from registers: dist [.][ldd] takes 8-byte vector accesses at every even column of every row
 __host__ __device__ __forceinline__ bool tc_dist_vec2(uintptr_t dist, int64_t ldd) { return ((dist | static_cast<uintptr_t>(ldd * 4)) & 7u) == 0; }
 
+// Construct as TcParams p{}: every member 0 / null except diag_off, so a launch has no self pairs unless it asks for them.
 struct TcParams {
   int64_t m, n;
   int nkb;                // k-blocks of 32 source columns
@@ -76,8 +77,7 @@ struct TcParams {
   // EPI_STORE
   float* dist;
   int64_t ldd;
-  int diag_zero;          // x and y alias: force d(i,i) = 0 (reference: CHANGELOG.md:1057,1213)
-  int tma_store;          // dist goes out through the staging boxes and the dist tensor map (tc_store_plan: aligned, single pass)
+  int tma_store;         // dist goes out through the staging boxes and the dist tensor map (tc_store_plan: aligned, single pass)
   int acc_mode;           // K-chunked accumulation: 0 single pass, 1 first chunk (raw store), 2 middle (+=), 3 last (+=, post)
   // EPI_MINLOC
   long long* keys;        // [m] packed (ordered bits of the distance << 32 | index)
@@ -103,12 +103,14 @@ struct TcParams {
   void* vd;               // [n + 1] uint32 counts, or uint64 when vd64 (null: adjacency only)
   int vd64;
   float eps;              // the squared radius
-  int64_t diag_off;       // row j of y is row j + diag_off of x (same memory): d = 0 there; TC_NO_DIAG: no such rows
+  // EPI_STORE, EPI_EPS, EPI_RADIUS with a clamping post (tc_finish): row j of y is row j + diag_off of x (the same memory),
+  // and d = 0 there exactly, which the expanded form alone does not give (reference: CHANGELOG.md:1057,1213).  0: x is y
+  int64_t diag_off = TC_NO_DIAG;
   // EPI_STORE with POST_RBF / POST_POLY / POST_TANH (gram_post): the kernel parameters, applied to the final value only
   float gamma;
   float coef0;
   int degree;
-  // EPI_RADIUS (radius_neighbors, radius.cu): the pairs with d(i, j) <= eps, d the EPI_STORE distance of post kPost (diag_zero
+  // EPI_RADIUS (radius_neighbors, radius.cu): the pairs with d(i, j) <= eps, d the EPI_STORE distance of post kPost (diag_off
   // as there).  Count mode: knn_cnt[i] += the row's pairs.  Fill mode: knn_cnt[i] is the row's fill counter and every pair
   // is written as key_pack(d, j) to knn_cand[rad_indptr[i] + slot], a slot at or past min(rad_indptr[i + 1], rad_nnz) dropped
   const long long* rad_indptr;   // [m + 1] (fill mode)

@@ -80,18 +80,40 @@ TcWorkspace tc_rows(TcWorkspace w, int side, int64_t r0, int64_t k)
   return w;
 }
 
+bool tc_metric(int metric, int64_t k, TcMetric* out)
+{
+  switch (metric) {  // {mode, center, post, xform, coef_mul, tx_const}
+    case B2D_L2Expanded:         *out = TC_L2; return true;
+    case B2D_L2SqrtExpanded:      *out = TcMetric{PREP_L2,         0, POST_CLAMP_SQRT, 0,  1.f, 0.f}; return true;
+    case B2D_CosineExpanded:      *out = TcMetric{PREP_COSINE,     0, POST_NONE,       0,  1.f, 0.f}; return true;
+    case B2D_CorrelationExpanded: *out = TcMetric{PREP_COSINE,     1, POST_NONE,       0,  1.f, 0.f}; return true;
+    case B2D_InnerProduct:        *out = TcMetric{PREP_INNER,      0, POST_NONE,       0,  1.f, 0.f}; return true;
+    case B2D_HellingerExpanded:   *out = TcMetric{PREP_INNER,      0, POST_CLAMP_SQRT, 1, -1.f, 1.f}; return true;
+    case B2D_RusselRaoExpanded:   *out = TcMetric{PREP_INNER,      0, POST_NONE,       0, -1.f / static_cast<float>(k), 1.f}; return true;
+    case B2D_JaccardExpanded:     *out = TcMetric{PREP_INNER_NORM, 0, POST_JACCARD,    0,  1.f, 0.f}; return true;
+    case B2D_DiceExpanded:        *out = TcMetric{PREP_INNER_NORM, 0, POST_DICE,       0,  1.f, 0.f}; return true;
+    default: return false;
+  }
+}
+
+int64_t tc_self_diag(const TcMetric& tm, const void* x, int64_t xrs, int64_t xcs, int64_t m, const void* y, int64_t yrs,
+                     int64_t ycs, int64_t n)
+{
+  const bool same = x == y && m == n && xrs == yrs && xcs == ycs;
+  return same && tm.mode == PREP_L2 && tc_post_clamps(tm.post) ? 0 : TC_NO_DIAG;
+}
+
 template <typename T>
 int launch_prep(cudaStream_t s, const TcWorkspace& w, const void* x, int64_t xrs, int64_t xcs, int64_t m,
                 const void* y, int64_t yrs, int64_t ycs, int64_t n, int64_t k, const float* xn, const float* yn,
-                int mode, int center, int xform, float coef_mul, float tx_const, const int* y_gather, bool y_only,
-                const unsigned* run_flag)
+                const TcMetric& tm, const int* y_gather, bool y_only, const unsigned* run_flag)
 {
   PrepParams p;
   p.side[0] = PrepSide{x, xrs, xcs, m, w.xop, w.xt, w.xsc, xn, w.xlo, nullptr};
   p.side[1] = PrepSide{y, yrs, ycs, n, w.yop, w.yt, w.ysc, yn, w.ylo, y_gather};
-  p.k = static_cast<int>(k); p.nkb = static_cast<int>((k + 31) / 32); p.mode = mode; p.center = center;
+  p.k = static_cast<int>(k); p.nkb = static_cast<int>((k + 31) / 32); p.mode = tm.mode; p.center = tm.center;
   p.gmax = w.gmax; p.coef = w.coef; p.has_lo = w.has_lo; p.nonuni = w.nonuni;
-  p.xform = xform; p.coef_mul = coef_mul; p.tx_const = tx_const;
+  p.xform = tm.xform; p.coef_mul = tm.coef_mul; p.tx_const = tm.tx_const;
   p.first_side = y_only ? 1 : 0; p.run_flag = run_flag;
   // (y_only: the caller has zeroed gmax[1] and nonuni[1] on the stream -- km_begin_kernel)
   if (!y_only) B2D_CUDA(cudaMemsetAsync(w.gmax, 0, 32, s));
@@ -103,11 +125,11 @@ int launch_prep(cudaStream_t s, const TcWorkspace& w, const void* x, int64_t xrs
   return B2D_OK;
 }
 template int launch_prep<float>(cudaStream_t, const TcWorkspace&, const void*, int64_t, int64_t, int64_t, const void*,
-                                int64_t, int64_t, int64_t, int64_t, const float*, const float*, int, int, int, float,
-                                float, const int*, bool, const unsigned*);
+                                int64_t, int64_t, int64_t, int64_t, const float*, const float*, const TcMetric&,
+                                const int*, bool, const unsigned*);
 template int launch_prep<__half>(cudaStream_t, const TcWorkspace&, const void*, int64_t, int64_t, int64_t, const void*,
-                                 int64_t, int64_t, int64_t, int64_t, const float*, const float*, int, int, int, float,
-                                 float, const int*, bool, const unsigned*);
+                                 int64_t, int64_t, int64_t, int64_t, const float*, const float*, const TcMetric&,
+                                 const int*, bool, const unsigned*);
 
 template <bool kRes, int kEpi, int kPost>
 static int launch_tc_inst(cudaStream_t s, const CUtensorMap& ma, const CUtensorMap& mb, const CUtensorMap& md,
