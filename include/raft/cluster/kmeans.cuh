@@ -3,6 +3,9 @@
 //   fit            centroids [n_clusters, k] in/out (read for InitMethod::Array), inertia and n_iter to the host
 //   predict        labels [m] on the device, inertia to the host
 //   cluster_cost   sum_i min_j ||x_i - c_j||^2 to the host
+// InitMethod::KMeansPlusPlus with oversampling_factor > 0 seeds with k-means|| (b2d_kmeans_fit_scalable).  Departure:
+// the reference's default oversampling_factor is 2.0, which selects k-means||; here the default is 0.0 (greedy
+// k-means++), so k-means|| must be asked for explicitly.
 // Temporaries come from the handle's workspace (raft/core/b200_workspace.hpp).  The host outputs are read after a sync of
 // the handle's stream, as the reference's host_scalar_view outputs were.  Departures from the recalled signatures: the
 // optional sample weights are a nullable device pointer and the host scalars are plain pointers (the 1-d and scalar
@@ -30,7 +33,7 @@ struct KMeansParams {
   struct { uint64_t seed = 0; } rng_state;
   raft::distance::DistanceType metric = raft::distance::DistanceType::L2Expanded;
   int n_init = 1;
-  double oversampling_factor = 2.0;                    // k-means|| is not provided: accepted, no effect
+  double oversampling_factor = 0.0;                    // > 0 with KMeansPlusPlus: k-means|| seeding (reference: 2.0)
   int batch_samples = 1 << 15;                         // accepted, no effect (the assignment is never batched)
   int batch_centroids = 0;                             // accepted, no effect
   bool inertia_check = false;
@@ -75,14 +78,22 @@ void fit(raft::resources const& handle, const KMeansParams& params, raft::device
   RAFT_EXPECTS(centroids.extent(0) == params.n_clusters && centroids.extent(1) == k,
                "kmeans: centroids must be [n_clusters, n_features]");
   const int64_t ldx = detail::row_pitch(X);
-  const size_t need = b2d_kmeans_workspace_bytes(m, k, params.n_clusters);
-  RAFT_EXPECTS(need != SIZE_MAX, "kmeans: invalid extents");
+  const bool scalable = params.init == InitMethod::KMeansPlusPlus && params.oversampling_factor > 0;
+  const size_t need = scalable ? b2d_kmeans_scalable_workspace_bytes(m, k, params.n_clusters, params.oversampling_factor)
+                               : b2d_kmeans_workspace_bytes(m, k, params.n_clusters);
+  RAFT_EXPECTS(need != SIZE_MAX, "kmeans: invalid extents or oversampling_factor");
   detail::km_scratch s(handle, need);
   cudaStream_t st = raft::resource::get_cuda_stream(handle);
-  raft::distance::detail::b2d_check(b2d_kmeans_fit(
-    st, params.n_clusters, params.max_iter, params.tol, static_cast<int>(params.init), params.n_init, params.rng_state.seed,
-    params.inertia_check ? 1 : 0, X.data_handle(), ldx, sample_weight, m, k, centroids.data_handle(), s.d(), s.i(),
-    s.base(), need));
+  if (scalable)
+    raft::distance::detail::b2d_check(b2d_kmeans_fit_scalable(
+      st, params.n_clusters, params.max_iter, params.tol, params.oversampling_factor, params.n_init, params.rng_state.seed,
+      params.inertia_check ? 1 : 0, X.data_handle(), ldx, sample_weight, m, k, centroids.data_handle(), s.d(), s.i(),
+      s.base(), need));
+  else
+    raft::distance::detail::b2d_check(b2d_kmeans_fit(
+      st, params.n_clusters, params.max_iter, params.tol, static_cast<int>(params.init), params.n_init, params.rng_state.seed,
+      params.inertia_check ? 1 : 0, X.data_handle(), ldx, sample_weight, m, k, centroids.data_handle(), s.d(), s.i(),
+      s.base(), need));
   double hi = 0.0;
   int32_t hn = 0;
   if (m > 0) {

@@ -376,6 +376,42 @@ int b2d_kmeans_update_centroids(void* stream, const float* x, int64_t ldx, const
 int b2d_kmeans_init_plus_plus(void* stream, const float* x, int64_t ldx, const float* sample_weight, int64_t m, int64_t k,
                               int n_clusters, uint64_t seed, float* centroids, void* workspace, size_t workspace_bytes);
 
+/* k-means|| seeding (scalable k-means++, Bahmani et al. 2012; [RECALLED] RAFT InitMethod::KMeansPlusPlus with
+ * oversampling_factor > 0) for the k-means above.  f = oversampling_factor must be finite and > 0.
+ *   Sizes: L = min(m, max(ceil(f n_clusters), ceil((n_clusters - 1) / 8))) rows per round over R = 8 rounds, so the
+ *     candidate set has exactly C = 1 + 8L >= n_clusters rows and no call synchronises.  C > 2^31 - 1 is
+ *     B2D_ERR_UNSUPPORTED.  Departure: the reference runs min(8, ceil(ln psi)) rounds (psi: the initial cost) of
+ *     independent Bernoulli draws and tops a short candidate set up with random rows; here R and C are fixed.
+ *   Draws: fixed-size weighted sampling without replacement (Efraimidis-Spirakis).  Round r gives row i the key
+ *     ln(E_ir) - ln(p_i), E_ir = -ln(u_ir), u_ir uniform in (0, 1) from Philox4x32-10 keyed by (seed, r, i), computed in
+ *     fp64 logs and rounded to fp32.  Round 0 has p_i = w_i and takes the smallest key; rounds 1..8 have
+ *     p_i = w_i D2_i and take the L smallest (b2d_select_k: ties to the smaller row).  Mass 0 (w_i <= 0, D2_i = 0, a row
+ *     already taken) gives +inf; a row with NaN distances a NaN key, ranked after +inf.  So a row without mass is taken
+ *     only once every row with mass has been.
+ *   D2: after each round D2_i = min(D2_i, squared distance of x_i to the nearest candidate of the round), by the exact
+ *     arg-min of b2d_fused_l2_nn; the rows taken get D2 = 0.
+ *   Candidate weights: W_c = sum of w_i over the rows whose arg-min among all C candidates is c, in fp64 in a fixed
+ *     order, rounded once to fp32: weight_per_cluster of b2d_kmeans_update_centroids.  A duplicate candidate loses its
+ *     ties to the earlier copy and gets weight 0.
+ *   Recluster: greedy k-means++ (as PLUS_PLUS) on the C candidate rows with weights W, then b2d_kmeans_fit's loop on them
+ *     with max_iter 300, tol 1e-4 and no inertia check.  The centroids are weighted means of candidates, not
+ *     necessarily rows of x.  Results are bit-identical from run to run; no floating-point atomics.
+ * init_scalable: the seeding alone, weights as given; optional device outputs candidates [C] (row ids) and
+ *   candidate_weights [C] (W): a weighted coreset of x.  fit_scalable: b2d_kmeans_fit with init = PLUS_PLUS and this
+ *   seeding in place of greedy k-means++ (run r seeded with seed + r; weights scaled to sum to m, also for the seeding).
+ * Argument checks are those of b2d_kmeans_fit, plus B2D_ERR_INVALID_ARG for an oversampling_factor that is not finite or
+ * not > 0; m == 0 does nothing.  The workspace query covers both calls and returns SIZE_MAX for negative extents, an
+ * invalid oversampling_factor or C > 2^31 - 1; it is at least b2d_kmeans_workspace_bytes(m, k, n_clusters). */
+size_t b2d_kmeans_scalable_workspace_bytes(int64_t m, int64_t k, int64_t n_clusters, double oversampling_factor);
+int b2d_kmeans_init_scalable(void* stream, const float* x, int64_t ldx, const float* sample_weight, int64_t m, int64_t k,
+                             int n_clusters, double oversampling_factor, uint64_t seed, float* centroids,
+                             int32_t* candidates /* optional [C] row ids */, float* candidate_weights /* optional [C] */,
+                             void* workspace, size_t workspace_bytes);
+int b2d_kmeans_fit_scalable(void* stream, int n_clusters, int max_iter, double tol, double oversampling_factor, int n_init,
+                            uint64_t seed, int inertia_check, const float* x, int64_t ldx, const float* sample_weight,
+                            int64_t m, int64_t k, float* centroids, double* inertia, int32_t* n_iter,
+                            void* workspace, size_t workspace_bytes);
+
 /* Minimum spanning forest of an edge list (the MST step of raft::cluster::single_linkage, [RECALLED]
  * raft::sparse::solver::mst): Borůvka on the device.  Edge e = (src[e], dst[e], w[e]) (int32 vertices, fp32 weights) is
  * ordered by (w[e], e): this order is strict, so the forest is unique.  Self-loops, duplicate and reversed edges are

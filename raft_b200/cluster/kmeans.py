@@ -4,6 +4,7 @@
 run."""
 from __future__ import annotations
 
+import math
 from collections import namedtuple
 
 import numpy as np
@@ -23,9 +24,10 @@ INIT_METHODS = {
 
 class KMeansParams:
     """Parameters of a fit ([RECALLED] pylibraft.cluster.kmeans.KMeansParams).  Only ``metric="sqeuclidean"`` is
-    supported (anything else raises LogicError).  ``oversampling_factor`` (k-means||), ``batch_samples``,
-    ``batch_centroids`` and ``verbosity`` are accepted for signature compatibility and have no effect: the
-    initialisation is greedy k-means++ and the assignment is never batched."""
+    supported (anything else raises LogicError).  ``oversampling_factor``: None or 0 keeps greedy k-means++; a positive
+    value with ``init_method="KMeansPlusPlus"`` seeds with k-means|| (see ``init_scalable``) instead; a negative or
+    non-finite value raises ValueError.  ``batch_samples``, ``batch_centroids`` and ``verbosity`` are accepted for
+    signature compatibility and have no effect: the assignment is never batched."""
 
     def __init__(self, n_clusters=None, max_iter=300, tol=1e-4, verbosity=None, seed=0, metric="sqeuclidean",
                  init_method="KMeansPlusPlus", n_init=1, oversampling_factor=None, batch_samples=None,
@@ -42,6 +44,10 @@ class KMeansParams:
         self.metric = metric
         self.init_method = init_method
         self.n_init = int(n_init)
+        if oversampling_factor is not None:
+            oversampling_factor = float(oversampling_factor)
+            if not math.isfinite(oversampling_factor) or oversampling_factor < 0:
+                raise ValueError("oversampling_factor must be None or finite and >= 0, got %r" % (oversampling_factor,))
         self.oversampling_factor = oversampling_factor
         self.batch_samples = batch_samples
         self.batch_centroids = batch_centroids
@@ -82,6 +88,13 @@ def _ws(m, k, nc, handle):
     return handle.workspace(_lib.lib().b2d_kmeans_workspace_bytes(m, k, nc))
 
 
+def _ws_scalable(m, k, nc, f, handle):
+    need = _lib.lib().b2d_kmeans_scalable_workspace_bytes(m, k, nc, f)
+    if need == 2 ** 64 - 1:
+        raise _lib.LogicError("k-means|| needs a finite oversampling_factor > 0 and fewer than 2^31 candidates")
+    return handle.workspace(need)
+
+
 @auto_sync_handle
 def fit(params, X, centroids=None, sample_weights=None, handle=None):
     """Returns ``FitOutput(centroids, inertia, n_iter)``.  ``centroids``: [n_clusters, k] float32, the initial
@@ -106,11 +119,20 @@ def fit(params, X, centroids=None, sample_weights=None, handle=None):
     w = _vector(sample_weights, m, np.float32, "sample_weights")
     inertia = _new((1,), torch.float64, handle)
     n_iter = _new((1,), torch.int32, handle)
-    ws = _ws(m, k, nc, handle)
-    _lib.check(_lib.lib().b2d_kmeans_fit(handle.stream_ptr, nc, params.max_iter, params.tol,
-                                         INIT_METHODS[params.init_method], params.n_init, params.seed & (2 ** 64 - 1),
-                                         1 if params.inertia_check else 0, x.data, k, w.data if w else None, m, k,
-                                         c.data, inertia.data_ptr(), n_iter.data_ptr(), ws.data_ptr(), ws.numel()))
+    seed = params.seed & (2 ** 64 - 1)
+    f = params.oversampling_factor
+    if params.init_method == "KMeansPlusPlus" and f:   # k-means|| seeding
+        ws = _ws_scalable(m, k, nc, f, handle)
+        _lib.check(_lib.lib().b2d_kmeans_fit_scalable(handle.stream_ptr, nc, params.max_iter, params.tol, f, params.n_init,
+                                                      seed, 1 if params.inertia_check else 0, x.data, k,
+                                                      w.data if w else None, m, k, c.data, inertia.data_ptr(),
+                                                      n_iter.data_ptr(), ws.data_ptr(), ws.numel()))
+    else:
+        ws = _ws(m, k, nc, handle)
+        _lib.check(_lib.lib().b2d_kmeans_fit(handle.stream_ptr, nc, params.max_iter, params.tol,
+                                             INIT_METHODS[params.init_method], params.n_init, seed,
+                                             1 if params.inertia_check else 0, x.data, k, w.data if w else None, m, k,
+                                             c.data, inertia.data_ptr(), n_iter.data_ptr(), ws.data_ptr(), ws.numel()))
     handle.sync()
     return FitOutput(out, float(inertia.item()), int(n_iter.item()))
 
@@ -189,4 +211,44 @@ def init_plus_plus(X, n_clusters=None, seed=None, handle=None, centroids=None):
     _lib.check(_lib.lib().b2d_kmeans_init_plus_plus(handle.stream_ptr, x.data, k, None, m, k, nc,
                                                     (0 if seed is None else int(seed)) & (2 ** 64 - 1), c.data,
                                                     ws.data_ptr(), ws.numel()))
+    return out
+
+
+@auto_sync_handle
+@auto_convert_output
+def init_scalable(X, n_clusters=None, oversampling_factor=2.0, seed=None, sample_weights=None, centroids=None,
+                  return_candidates=False, handle=None):
+    """k-means|| seeding (include/raft_b200.h: b2d_kmeans_init_scalable): 1 + 8L candidate rows drawn in 9 rounds
+    (L = min(m, max(ceil(oversampling_factor * n_clusters), ceil((n_clusters - 1) / 8)))), weighted by the weights of
+    the rows nearest to them, reclustered into [n_clusters, k] float32 centroids (written into ``centroids`` when
+    given).  ``sample_weights``: optional float32 [m], used as given.  With ``return_candidates`` returns
+    ``(centroids, candidate_rows int32 [C], candidate_weights float32 [C])``."""
+    x = _matrix(X, "X")
+    m, k = x.shape
+    if n_clusters is None:
+        if centroids is None:
+            raise ValueError("n_clusters or centroids must be given")
+        n_clusters = cai_wrapper(centroids).shape[0]
+    nc = int(n_clusters)
+    f = float(oversampling_factor)
+    if not math.isfinite(f) or f <= 0:
+        raise ValueError("oversampling_factor must be finite and > 0, got %r" % (oversampling_factor,))
+    if centroids is None:
+        out = device_ndarray(_new((nc, k), torch.float32, handle))
+        c = cai_wrapper(out)
+    else:
+        out = centroids
+        c = _centroids_out(centroids, nc, k, handle)
+    w = _vector(sample_weights, m, np.float32, "sample_weights")
+    ws = _ws_scalable(m, k, nc, f, handle)
+    n_cand = 1 + 8 * min(m, max(math.ceil(f * nc), math.ceil((nc - 1) / 8)))
+    rows = _new((n_cand,), torch.int32, handle) if return_candidates else None
+    wts = _new((n_cand,), torch.float32, handle) if return_candidates else None
+    _lib.check(_lib.lib().b2d_kmeans_init_scalable(handle.stream_ptr, x.data, k, w.data if w else None, m, k, nc, f,
+                                                   (0 if seed is None else int(seed)) & (2 ** 64 - 1), c.data,
+                                                   rows.data_ptr() if rows is not None else None,
+                                                   wts.data_ptr() if wts is not None else None, ws.data_ptr(),
+                                                   ws.numel()))
+    if return_candidates:
+        return out, device_ndarray(rows), device_ndarray(wts)
     return out

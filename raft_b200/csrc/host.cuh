@@ -7,6 +7,7 @@
 #include <algorithm>
 #include <cstddef>
 #include <cstdint>
+#include <functional>
 #include <string>
 
 #include "../../include/raft_b200.h"
@@ -205,6 +206,56 @@ int km_sort_scatter(cudaStream_t s, const unsigned* run, const KmSort& S, const 
                     int64_t m, int64_t nc);
 // launch of km_gather_rows_kernel<int>: rows idx[0, nc) of x into out [nc, k], one 128-thread block per row
 void km_gather_rows(cudaStream_t s, unsigned grid, const float* x, int64_t ldx, int k, const int* idx, int nc, float* out);
+
+// The workspace of one k-means call on m rows, k columns and nc clusters (b2d_kmeans_workspace_bytes)
+struct KmLayout {
+  TcWorkspace tc;   // x (side 0) and the centroids (side 1) of the arg-min, keys[m]
+  KmSortPlan P;
+  KmSort sort;
+  KmCtrl* ctrl;     // the fit's control words: sort.ctrl
+  int* labels;      // [m]
+  float* w;         // [m] the normalised weights
+  float* rowf;      // [m] k-means++ D^2 / Random: the uniforms
+  double *sums, *wsums, *part, *wpart, *shift, *ipart, *bs;
+  float* best;      // [nc * k] n_init: the best centroids so far
+  float* sk_val;    // Random: select_k outputs and workspace
+  int64_t* sk_idx;
+  void* sk_ws;
+  size_t sk_bytes;
+  int64_t nchunks, nb;
+  size_t bytes;
+};
+
+KmLayout km_layout(void* base, int64_t m, int64_t k, int64_t nc);
+// the argument checks every k-means entry shares (c: the centroids)
+int km_args(const float* x, int64_t ldx, int64_t m, int64_t k, int64_t nc, const void* c);
+// the arguments of a fit besides km_args
+int km_fit_args(const double* inertia, const int32_t* n_iter, int max_iter, double tol, int init, int n_init);
+// arg-min of every row against the centroids c [nc, k] (prepared first when prep_y): labels, inertia partials, label
+// histogram (when hist)
+int km_assign(cudaStream_t s, const KmLayout& L, int64_t m, int64_t k, int64_t nc, const float* c, const float* w,
+              int* labels, const unsigned* run, bool prep_y, bool hist);
+// new centroids (and, when wpc, the fp32 weight per cluster) from the histogram km_assign left
+int km_update(cudaStream_t s, const KmLayout& L, const float* x, int64_t ldx, int64_t m, int64_t k, int64_t nc,
+              const float* w, const int* labels, const float* old_c, float* out_c, float* wpc, const unsigned* run);
+// the weights of a fit (normalize: scaled to sum to m) or null; marks L.ctrl bad for negative / NaN weights or a zero sum
+const float* km_weights(cudaStream_t s, const KmLayout& L, const float* w, int64_t m, bool normalize);
+// greedy k-means++ seeding of c [nc, k] from the rows of x
+int km_plus_plus(cudaStream_t s, const KmLayout& L, const float* x, int64_t ldx, const float* w, int64_t m, int64_t k,
+                 int64_t nc, uint64_t seed, float* c);
+// A fit after its checks, its km_ctrl_init_kernel and its weights: `runs` times seed_run(r) (which writes the initial
+// centroids) then Lloyd's loop; with runs > 1 the first run of strictly lowest inertia is kept.  inertia / n_iter may be
+// null.
+int km_fit_runs(cudaStream_t s, const KmLayout& L, const float* x, int64_t ldx, const float* w, int64_t m, int64_t k,
+                int64_t nc, int max_iter, double tol, int inertia_check, int runs, float* centroids, double* inertia,
+                int32_t* n_iter, const std::function<int(int)>& seed_run);
+// launch of km_ctrl_init_kernel: the control words at the start of a fit
+void km_ctrl_init(cudaStream_t s, KmCtrl* ctrl);
+// k-means|| launches (kmeans.cuh): km_par_keys_kernel over m rows and km_par_take_kernel for n candidates
+void km_par_keys(cudaStream_t s, const long long* fold_keys, float* d2, const float* w, int64_t m, uint64_t seed, int round,
+                 float* key);
+void km_par_take(cudaStream_t s, const float* x, int64_t ldx, int k, const int64_t* idx, int n, float* cand, int* ids,
+                 float* d2);
 
 // ------------------------------------------------------------------------------------------
 // single_linkage.cu

@@ -80,26 +80,8 @@ void km_gather_rows(cudaStream_t s, unsigned grid, const float* x, int64_t ldx, 
 }
 }  // namespace b2d
 
-namespace {
-struct KmLayout {
-  TcWorkspace tc;   // x (side 0) and the centroids (side 1) of the arg-min, keys[m]
-  KmSortPlan P;
-  KmSort sort;
-  KmCtrl* ctrl;     // the fit's control words: sort.ctrl
-  int* labels;      // [m]
-  float* w;         // [m] the normalised weights
-  float* rowf;      // [m] k-means++ D^2 / Random: the uniforms
-  double *sums, *wsums, *part, *wpart, *shift, *ipart, *bs;
-  float* best;      // [nc * k] n_init: the best centroids so far
-  float* sk_val;    // Random: select_k outputs and workspace
-  int64_t* sk_idx;
-  void* sk_ws;
-  size_t sk_bytes;
-  int64_t nchunks, nb;
-  size_t bytes;
-};
-
-static KmLayout km_layout(void* base, int64_t m, int64_t k, int64_t nc)
+namespace b2d {
+KmLayout km_layout(void* base, int64_t m, int64_t k, int64_t nc)
 {
   Carve c(base, 1024);
   KmLayout L{};
@@ -130,7 +112,7 @@ static KmLayout km_layout(void* base, int64_t m, int64_t k, int64_t nc)
   return L;
 }
 
-static int km_args(const float* x, int64_t ldx, int64_t m, int64_t k, int64_t nc, const void* c)
+int km_args(const float* x, int64_t ldx, int64_t m, int64_t k, int64_t nc, const void* c)
 {
   if (m < 0 || k < 0) return fail(B2D_ERR_INVALID_ARG, "negative extent");
   if (k < 1 || k > (1 << 24)) return fail(B2D_ERR_INVALID_ARG, "k must be in [1, 2^24]");
@@ -142,8 +124,8 @@ static int km_args(const float* x, int64_t ldx, int64_t m, int64_t k, int64_t nc
 }
 
 // arg-min of every row against the prepared centroids: labels, inertia partials, label histogram (when hist)
-static int km_assign(cudaStream_t s, const KmLayout& L, int64_t m, int64_t k, int64_t nc, const float* c, const float* w,
-                     int* labels, const unsigned* run, bool prep_y, bool hist)
+int km_assign(cudaStream_t s, const KmLayout& L, int64_t m, int64_t k, int64_t nc, const float* c, const float* w,
+              int* labels, const unsigned* run, bool prep_y, bool hist)
 {
   const int64_t nh = hist ? L.P.nhist : 0;
   // (the centroid side's exponent and scale flag are zeroed only where it is prepared again below)
@@ -166,8 +148,8 @@ static int km_assign(cudaStream_t s, const KmLayout& L, int64_t m, int64_t k, in
 }
 
 // new centroids from the histogram km_assign (or km_sort_count) left: scan, stable scatter, fp64 sums
-static int km_update(cudaStream_t s, const KmLayout& L, const float* x, int64_t ldx, int64_t m, int64_t k, int64_t nc,
-                     const float* w, const int* labels, const float* old_c, float* out_c, float* wpc, const unsigned* run)
+int km_update(cudaStream_t s, const KmLayout& L, const float* x, int64_t ldx, int64_t m, int64_t k, int64_t nc,
+              const float* w, const int* labels, const float* old_c, float* out_c, float* wpc, const unsigned* run)
 {
   int rc = km_sort_scatter(s, run, L.sort, L.P, labels, m, nc);
   if (rc) return rc;
@@ -182,7 +164,7 @@ static int km_update(cudaStream_t s, const KmLayout& L, const float* x, int64_t 
 }
 
 // fit / predict weights: scaled to sum to m; a negative or NaN weight, or a zero sum, marks the inertia NaN
-static const float* km_weights(cudaStream_t s, const KmLayout& L, const float* w, int64_t m, bool normalize)
+const float* km_weights(cudaStream_t s, const KmLayout& L, const float* w, int64_t m, bool normalize)
 {
   if (!w) return nullptr;
   km_wsum_kernel<<<static_cast<unsigned>(L.nb), kKmThreads, 0, s>>>(w, m, L.bs, L.ctrl);
@@ -192,8 +174,8 @@ static const float* km_weights(cudaStream_t s, const KmLayout& L, const float* w
   return L.w;
 }
 
-static int km_plus_plus(cudaStream_t s, const KmLayout& L, const float* x, int64_t ldx, const float* w, int64_t m, int64_t k,
-                        int64_t nc, uint64_t seed, float* c)
+int km_plus_plus(cudaStream_t s, const KmLayout& L, const float* x, int64_t ldx, const float* w, int64_t m, int64_t k,
+                 int64_t nc, uint64_t seed, float* c)
 {
   const int trials = std::min(kKmPpMaxTrials, 2 + static_cast<int>(std::floor(std::log(static_cast<double>(nc)))));
   km_pp_init_kernel<<<static_cast<unsigned>(L.nb), kKmThreads, 0, s>>>(w, m, L.rowf, L.bs, L.ctrl);
@@ -211,54 +193,24 @@ static int km_plus_plus(cudaStream_t s, const KmLayout& L, const float* x, int64
   return B2D_OK;
 }
 
-// n_clusters distinct rows: the positions of the n_clusters smallest of m seeded uniforms (select_k)
-static int km_random(cudaStream_t s, const KmLayout& L, const float* x, int64_t ldx, int64_t m, int64_t k, int64_t nc,
-                     uint64_t seed, float* c)
+int km_fit_args(const double* inertia, const int32_t* n_iter, int max_iter, double tol, int init, int n_init)
 {
-  km_uniforms_kernel<<<km_grid(m), 256, 0, s>>>(L.rowf, m, seed);
-  B2D_CUDA(cudaGetLastError());
-  int rc = b2d_select_k(s, L.rowf, m, nullptr, 1, m, nc, 1, L.sk_val, L.sk_idx, L.sk_ws, L.sk_bytes);
-  if (rc) return rc;
-  km_gather_rows_kernel<int64_t><<<static_cast<unsigned>(nc), 128, 0, s>>>(x, ldx, static_cast<int>(k), L.sk_idx,
-                                                                           static_cast<int>(nc), c);
-  B2D_CUDA(cudaGetLastError());
-  return B2D_OK;
-}
-}  // namespace
-
-size_t b2d_kmeans_workspace_bytes(int64_t m, int64_t k, int64_t n_clusters)
-{
-  if (m < 0 || k < 0 || n_clusters < 0) return static_cast<size_t>(-1);
-  return km_layout(nullptr, m, k, n_clusters).bytes;
-}
-
-int b2d_kmeans_fit(void* stream, int n_clusters, int max_iter, double tol, int init, int n_init, uint64_t seed,
-                   int inertia_check, const float* x, int64_t ldx, const float* sample_weight, int64_t m, int64_t k,
-                   float* centroids, double* inertia, int32_t* n_iter, void* workspace, size_t workspace_bytes)
-{
-  cudaStream_t s = static_cast<cudaStream_t>(stream);
-  if (m == 0) return B2D_OK;
-  int rc = km_args(x, ldx, m, k, n_clusters, centroids);
-  if (rc) return rc;
   if (!inertia || !n_iter) return fail(B2D_ERR_INVALID_ARG, "null inertia / n_iter");
   if (max_iter < 0) return fail(B2D_ERR_INVALID_ARG, "max_iter must be >= 0");
   if (!(tol >= 0.0)) return fail(B2D_ERR_INVALID_ARG, "tol must be >= 0");
   if (init != B2D_KMEANS_INIT_PLUS_PLUS && init != B2D_KMEANS_INIT_RANDOM && init != B2D_KMEANS_INIT_ARRAY)
     return fail(B2D_ERR_INVALID_ARG, "unknown init method " + std::to_string(init));
   if (n_init < 1) return fail(B2D_ERR_INVALID_ARG, "n_init must be >= 1");
-  const int64_t nc = n_clusters;
-  rc = check_workspace(workspace, workspace_bytes, km_layout(nullptr, m, k, nc).bytes);
-  if (rc) return rc;
-  const KmLayout L = km_layout(workspace, m, k, nc);
-  km_ctrl_init_kernel<<<1, 1, 0, s>>>(L.ctrl);
-  B2D_CUDA(cudaGetLastError());
-  const float* w = km_weights(s, L, sample_weight, m, true);
-  B2D_CUDA(cudaGetLastError());
-  const int runs = init == B2D_KMEANS_INIT_ARRAY ? 1 : n_init;
-  unsigned* run  = &L.ctrl->run;
+  return B2D_OK;
+}
+
+int km_fit_runs(cudaStream_t s, const KmLayout& L, const float* x, int64_t ldx, const float* w, int64_t m, int64_t k,
+                int64_t nc, int max_iter, double tol, int inertia_check, int runs, float* centroids, double* inertia,
+                int32_t* n_iter, const std::function<int(int)>& seed_run)
+{
+  unsigned* run = &L.ctrl->run;
   for (int r = 0; r < runs; ++r) {
-    if (init == B2D_KMEANS_INIT_RANDOM) rc = km_random(s, L, x, ldx, m, k, nc, seed + r, centroids);
-    if (init == B2D_KMEANS_INIT_PLUS_PLUS) rc = km_plus_plus(s, L, x, ldx, w, m, k, nc, seed + r, centroids);
+    int rc = seed_run(r);
     if (rc) return rc;
     km_fit_begin_kernel<<<1, 1, 0, s>>>(L.ctrl);
     B2D_CUDA(cudaGetLastError());
@@ -295,6 +247,70 @@ int b2d_kmeans_fit(void* stream, int n_clusters, int max_iter, double tol, int i
     B2D_CUDA(cudaGetLastError());
   }
   return B2D_OK;
+}
+
+void km_ctrl_init(cudaStream_t s, KmCtrl* ctrl) { km_ctrl_init_kernel<<<1, 1, 0, s>>>(ctrl); }
+
+void km_par_keys(cudaStream_t s, const long long* fold_keys, float* d2, const float* w, int64_t m, uint64_t seed, int round,
+                 float* key)
+{
+  km_par_keys_kernel<<<static_cast<unsigned>((m + 255) / 256), 256, 0, s>>>(fold_keys, d2, w, m, seed, round, key);
+}
+
+void km_par_take(cudaStream_t s, const float* x, int64_t ldx, int k, const int64_t* idx, int n, float* cand, int* ids,
+                 float* d2)
+{
+  km_par_take_kernel<<<static_cast<unsigned>(n), 128, 0, s>>>(x, ldx, k, idx, n, cand, ids, d2);
+}
+}  // namespace b2d
+
+namespace {
+// n_clusters distinct rows: the positions of the n_clusters smallest of m seeded uniforms (select_k)
+static int km_random(cudaStream_t s, const KmLayout& L, const float* x, int64_t ldx, int64_t m, int64_t k, int64_t nc,
+                     uint64_t seed, float* c)
+{
+  km_uniforms_kernel<<<km_grid(m), 256, 0, s>>>(L.rowf, m, seed);
+  B2D_CUDA(cudaGetLastError());
+  int rc = b2d_select_k(s, L.rowf, m, nullptr, 1, m, nc, 1, L.sk_val, L.sk_idx, L.sk_ws, L.sk_bytes);
+  if (rc) return rc;
+  km_gather_rows_kernel<int64_t><<<static_cast<unsigned>(nc), 128, 0, s>>>(x, ldx, static_cast<int>(k), L.sk_idx,
+                                                                           static_cast<int>(nc), c);
+  B2D_CUDA(cudaGetLastError());
+  return B2D_OK;
+}
+}  // namespace
+
+size_t b2d_kmeans_workspace_bytes(int64_t m, int64_t k, int64_t n_clusters)
+{
+  if (m < 0 || k < 0 || n_clusters < 0) return static_cast<size_t>(-1);
+  return km_layout(nullptr, m, k, n_clusters).bytes;
+}
+
+int b2d_kmeans_fit(void* stream, int n_clusters, int max_iter, double tol, int init, int n_init, uint64_t seed,
+                   int inertia_check, const float* x, int64_t ldx, const float* sample_weight, int64_t m, int64_t k,
+                   float* centroids, double* inertia, int32_t* n_iter, void* workspace, size_t workspace_bytes)
+{
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  if (m == 0) return B2D_OK;
+  int rc = km_args(x, ldx, m, k, n_clusters, centroids);
+  if (rc) return rc;
+  rc = km_fit_args(inertia, n_iter, max_iter, tol, init, n_init);
+  if (rc) return rc;
+  const int64_t nc = n_clusters;
+  rc = check_workspace(workspace, workspace_bytes, km_layout(nullptr, m, k, nc).bytes);
+  if (rc) return rc;
+  const KmLayout L = km_layout(workspace, m, k, nc);
+  km_ctrl_init_kernel<<<1, 1, 0, s>>>(L.ctrl);
+  B2D_CUDA(cudaGetLastError());
+  const float* w = km_weights(s, L, sample_weight, m, true);
+  B2D_CUDA(cudaGetLastError());
+  const int runs = init == B2D_KMEANS_INIT_ARRAY ? 1 : n_init;
+  return km_fit_runs(s, L, x, ldx, w, m, k, nc, max_iter, tol, inertia_check, runs, centroids, inertia, n_iter,
+                     [&](int r) {
+                       if (init == B2D_KMEANS_INIT_RANDOM) return km_random(s, L, x, ldx, m, k, nc, seed + r, centroids);
+                       if (init == B2D_KMEANS_INIT_PLUS_PLUS) return km_plus_plus(s, L, x, ldx, w, m, k, nc, seed + r, centroids);
+                       return static_cast<int>(B2D_OK);
+                     });
 }
 
 int b2d_kmeans_predict(void* stream, const float* x, int64_t ldx, const float* sample_weight, int64_t m, int64_t k,

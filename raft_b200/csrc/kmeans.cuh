@@ -672,4 +672,60 @@ __global__ void __launch_bounds__(kKmThreads) km_pp_choose_kernel(const float* x
   }
 }
 
+// ---- k-means|| (kmeans_scalable.cu): Efraimidis-Spirakis keys, so each round's draw is one select_k of the smallest keys
+// uniform in the open interval (0, 1): 53 bits of Philox4x32-10 keyed by (seed, stream), plus one half
+__device__ __forceinline__ double km_open_uniform(unsigned long long seed, unsigned long long stream_id)
+{
+  curandStatePhilox4_32_10_t st;
+  curand_init(seed, stream_id, 0, &st);
+  const unsigned a = curand(&st), b = curand(&st);
+  const unsigned long long u53 = (static_cast<unsigned long long>(a) << 21) | (b >> 11);
+  return (static_cast<double>(u53) + 0.5) * 0x1p-53;
+}
+
+// One pass over the rows before the draw of round `round`.  fold_keys != null: D2_i <- min(D2_i, distance to the nearest
+// candidate of the previous round) from the arg-min keys (NaN stays NaN); fold_keys == null (round 0): D2_i <- +inf.
+// Then key_i = ln(E_i) - ln(p_i), E_i = -ln(u_i), p_i = w_i (round 0) or w_i D2_i, in fp64 logs: the smallest keys are a
+// weighted sample without replacement.  Mass 0 (w_i <= 0, or D2_i = 0: a row already taken) gives +inf, a NaN D2 NaN.
+__global__ void km_par_keys_kernel(const long long* fold_keys, float* d2, const float* w, int64_t m,
+                                   unsigned long long seed, int round, float* key)
+{
+  const int64_t i = static_cast<int64_t>(blockIdx.x) * blockDim.x + threadIdx.x;
+  if (i >= m) return;
+  float D = __int_as_float(0x7f800000);
+  if (fold_keys) {
+    const long long kk = fold_keys[i];
+    const float d      = kk == KEY_EMPTY ? __int_as_float(0x7fffffff) : fmaxf(key_dist(kk), 0.f);
+    D                  = d2[i];
+    D                  = (d != d || D != D) ? __int_as_float(0x7fffffff) : fminf(D, d);
+  }
+  d2[i] = D;
+  const float wi = w ? w[i] : 1.f;
+  float out;
+  if (!(wi > 0.f) || D == 0.f) {
+    out = __int_as_float(0x7f800000);
+  } else if (D != D) {
+    out = __int_as_float(0x7fffffff);
+  } else {
+    const double u  = km_open_uniform(seed, (static_cast<unsigned long long>(round) << 32) | static_cast<unsigned long long>(i));
+    const double lp = log(static_cast<double>(wi)) + (fold_keys ? log(static_cast<double>(D)) : 0.0);
+    out = static_cast<float>(log(-log(u)) - lp);
+  }
+  key[i] = out;
+}
+
+// Candidate c of a round = row idx[c] of x: its copy into cand [n, k], its id into ids, and D2 of the row <- 0
+__global__ void km_par_take_kernel(const float* x, int64_t ldx, int k, const int64_t* idx, int n, float* cand, int* ids,
+                                   float* d2)
+{
+  const int c = blockIdx.x;
+  if (c >= n) return;
+  const int64_t r = idx[c];
+  for (int col = threadIdx.x; col < k; col += blockDim.x) cand[static_cast<int64_t>(c) * k + col] = x[r * ldx + col];
+  if (threadIdx.x == 0) {
+    ids[c] = static_cast<int>(r);
+    d2[r]  = 0.f;
+  }
+}
+
 }  // namespace b2d
