@@ -412,6 +412,49 @@ int b2d_kmeans_fit_scalable(void* stream, int n_clusters, int max_iter, double t
                             int64_t m, int64_t k, float* centroids, double* inertia, int32_t* n_iter,
                             void* workspace, size_t workspace_bytes);
 
+/* Hierarchical balanced k-means ([RECALLED] raft::cluster::kmeans_balanced::fit, L2Expanded, fp32): n_clusters
+ * centroids [n_clusters, k] of x [m, k] in three stages of balanced EM, with G = min(n_clusters,
+ * max(1, round(sqrt(n_clusters)))) mesoclusters.  Labels are predicted with b2d_kmeans_predict.
+ *   Balanced EM on a problem (a set of rows and a set of centroids): every iteration assigns each row to its nearest
+ *     centroid of the problem (ties to the smaller index), updates the centroids (b2d_kmeans_update_centroids: fp64 sums
+ *     in a fixed order; an empty cluster keeps its centroid), then adjusts them: with a = rows / centroids of the
+ *     problem, a centroid j of size s_j < a / 4 draws a donor row d uniformly from the problem's rows (Philox4x32-10,
+ *     counter (j, iteration, stage, 0), key seed; position floor(((w0 << 32) | w1) * rows / 2^64)); when the donor's
+ *     cluster has size >= a, c_j <- (w c_j + x_d) / (w + 1) with w = min(s_j, 7), in fp64 rounded once.  The last
+ *     iteration of a problem has no adjust.  Initial centroid t of a problem with R rows and C centroids is its row
+ *     floor(t R / C) in the problem's row order.
+ *   Stage 0: the G mesoclusters, one problem on all finite rows in row order, n_iters iterations.
+ *   Allocation: mesocluster g of S_g rows (R in all) gets floor(n_clusters S_g / R) fine clusters, plus one for the
+ *     largest remainders n_clusters S_g mod R (ties to the lower g) until they sum to n_clusters; a non-empty
+ *     mesocluster left with none takes one from the mesocluster of the largest count / S_g holding at least two (ties to
+ *     the lower g).  Mesocluster g owns the fine centroids [F_{g-1}, F_g).  With R >= n_clusters no mesocluster gets
+ *     more fine clusters than rows.
+ *   Stage 1: every mesocluster is a problem of its rows and its fine centroids, n_iters iterations, all at once on the
+ *     rows sorted stably by mesocluster with the masked fused arg-min (b2d_masked_l2_nn's kernel).
+ *   Stage 2: one problem on all finite rows and all n_clusters centroids in the caller's row order,
+ *     max(n_iters / 10, 2) iterations.  So the centroids returned are b2d_kmeans_update_centroids(x, labels) bit for
+ *     bit, with labels [m] (optional output) the assignment that update used and sizes [n_clusters] (optional output)
+ *     its cluster sizes.
+ * A row with a non-finite element gets label -1, belongs to no problem and is never a donor; every centroid is finite.
+ * Results are bit-identical from run to run and independent of the device's SM count; nothing synchronises, so a fit
+ * can be captured in a CUDA graph.  Argument checks are those of b2d_kmeans_fit (n_clusters in [1, m], ...) plus
+ * n_iters >= 1; m == 0 does nothing.  The workspace query returns SIZE_MAX for negative extents. */
+size_t b2d_kmeans_balanced_workspace_bytes(int64_t m, int64_t k, int64_t n_clusters);
+int b2d_kmeans_balanced_fit(void* stream, int n_clusters, int n_iters, uint64_t seed, const float* x, int64_t ldx,
+                            int64_t m, int64_t k, float* centroids, int32_t* labels /* optional [m] */,
+                            int32_t* sizes /* optional [n_clusters] */, void* workspace, size_t workspace_bytes);
+/* The assignment step of the fit's stage 1 on its own, for tests: x [m, k] holds G = num_groups groups of rows
+ * [row_ends[g-1], row_ends[g]) and centroids [n_clusters, k] the groups [centroid_ends[g-1], centroid_ends[g])
+ * (row_ends[-1] = centroid_ends[-1] = 0; device arrays, non-decreasing, row_ends[G-1] <= m and centroid_ends[G-1] <=
+ * n_clusters, not checked).  labels[i] = the nearest centroid of row i's group (ties to the smaller index), -1 for a row
+ * in no group or with NaN distances.  Same kernels and tables as the fit: adjacency bits from the row ranges, tile
+ * classes, one EPI_MINLOC_MASKED launch.  Argument checks of b2d_kmeans_balanced_fit, plus num_groups in
+ * [1, round(sqrt(n_clusters))]; the workspace is b2d_kmeans_balanced_workspace_bytes(m, k, n_clusters). */
+int b2d_debug_kmeans_balanced_fine_assign(void* stream, const float* x, int64_t ldx, int64_t m, int64_t k,
+                                          const int32_t* row_ends, const float* centroids, int n_clusters,
+                                          const int32_t* centroid_ends, int64_t num_groups, int32_t* labels,
+                                          void* workspace, size_t workspace_bytes);
+
 /* Minimum spanning forest of an edge list (the MST step of raft::cluster::single_linkage, [RECALLED]
  * raft::sparse::solver::mst): Borůvka on the device.  Edge e = (src[e], dst[e], w[e]) (int32 vertices, fp32 weights) is
  * ordered by (w[e], e): this order is strict, so the forest is unique.  Self-loops, duplicate and reversed edges are

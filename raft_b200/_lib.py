@@ -19,7 +19,9 @@ SYMBOLS = [
     "b2d_select_k_workspace_bytes", "b2d_select_k", "b2d_eps_neighbors_l2sq_workspace_bytes", "b2d_eps_neighbors_l2sq",
     "b2d_gram_matrix_workspace_bytes", "b2d_gram_matrix", "b2d_kmeans_workspace_bytes", "b2d_kmeans_fit",
     "b2d_kmeans_predict", "b2d_kmeans_update_centroids", "b2d_kmeans_init_plus_plus", "b2d_kmeans_scalable_workspace_bytes",
-    "b2d_kmeans_init_scalable", "b2d_kmeans_fit_scalable", "b2d_mst_workspace_bytes", "b2d_mst",
+    "b2d_kmeans_init_scalable", "b2d_kmeans_fit_scalable", "b2d_kmeans_balanced_workspace_bytes",
+    "b2d_kmeans_balanced_fit", "b2d_debug_kmeans_balanced_fine_assign",
+    "b2d_mst_workspace_bytes", "b2d_mst",
     "b2d_single_linkage_workspace_bytes", "b2d_single_linkage", "b2d_dbscan_workspace_bytes", "b2d_dbscan_fit",
     "b2d_debug_pairwise_plan", "b2d_radius_neighbors_workspace_bytes", "b2d_radius_neighbors_count",
     "b2d_radius_neighbors_fill",
@@ -130,6 +132,12 @@ def lib() -> ctypes.CDLL:
     L.b2d_kmeans_init_scalable.argtypes = [vp, vp, i64, vp, i64, i64, ci, cd, u64, vp, vp, vp, vp, sz]
     L.b2d_kmeans_fit_scalable.restype = ci
     L.b2d_kmeans_fit_scalable.argtypes = [vp, ci, ci, cd, cd, ci, u64, ci, vp, i64, vp, i64, i64, vp, vp, vp, vp, sz]
+    L.b2d_kmeans_balanced_workspace_bytes.restype = sz
+    L.b2d_kmeans_balanced_workspace_bytes.argtypes = [i64, i64, i64]
+    L.b2d_kmeans_balanced_fit.restype = ci
+    L.b2d_kmeans_balanced_fit.argtypes = [vp, ci, ci, u64, vp, i64, i64, i64, vp, vp, vp, vp, sz]
+    L.b2d_debug_kmeans_balanced_fine_assign.restype = ci
+    L.b2d_debug_kmeans_balanced_fine_assign.argtypes = [vp, vp, i64, i64, i64, vp, vp, ci, vp, i64, vp, vp, sz]
     L.b2d_mst_workspace_bytes.restype = sz
     L.b2d_mst_workspace_bytes.argtypes = [i64, i64]
     L.b2d_mst.restype = ci

@@ -143,6 +143,12 @@ int launch_screen(cudaStream_t s, const TcWorkspace& w, int64_t m, int64_t n, in
 int masked_keys(cudaStream_t s, const TcWorkspace& w, long long* keys, const int* grp, unsigned* bits, uint8_t* cls,
                 const unsigned* bad, const uint8_t* adj, int64_t ld_adj, const int32_t* group_idxs, int64_t G,
                 int64_t m, int64_t n, int64_t k);
+// masked_keys in two steps, for callers that build the adjacency bits themselves and reuse the tile classes: the tile
+// classes cls of (x, y) from the bits (all MASK_NONE when *bad), then the EPI_MINLOC_MASKED launch
+int masked_classify(cudaStream_t s, uint8_t* cls, const unsigned* bits, const int32_t* group_idxs, int64_t G, int64_t m,
+                    int64_t n, const unsigned* bad);
+int masked_launch(cudaStream_t s, const TcWorkspace& w, long long* keys, const int* grp, const unsigned* bits,
+                  const uint8_t* cls, int64_t G, int64_t m, int64_t n, int64_t k);
 // launches of minloc_init_kernel / masked_group_map_kernel, 256 threads per block
 void minloc_init(cudaStream_t s, unsigned grid, long long* keys, int64_t m);
 void masked_group_map(cudaStream_t s, unsigned grid, int* grp, const int* group_idxs, int64_t G, int64_t n);
@@ -235,6 +241,12 @@ int km_fit_args(const double* inertia, const int32_t* n_iter, int max_iter, doub
 // histogram (when hist)
 int km_assign(cudaStream_t s, const KmLayout& L, int64_t m, int64_t k, int64_t nc, const float* c, const float* w,
               int* labels, const unsigned* run, bool prep_y, bool hist);
+// km_assign in two halves around the arg-min launch, for a caller with its own (masked) launch: keys <- KEY_EMPTY and
+// the histogram zeroed, the centroids prepared when prep_y; then the labels, inertia partials and histogram from the keys
+int km_assign_prep(cudaStream_t s, const KmLayout& L, int64_t m, int64_t k, int64_t nc, const float* c, const unsigned* run,
+                   bool prep_y, bool hist);
+int km_assign_labels(cudaStream_t s, const KmLayout& L, int64_t m, int64_t nc, const float* w, int* labels,
+                     const unsigned* run, bool hist);
 // new centroids (and, when wpc, the fp32 weight per cluster) from the histogram km_assign left
 int km_update(cudaStream_t s, const KmLayout& L, const float* x, int64_t ldx, int64_t m, int64_t k, int64_t nc,
               const float* w, const int* labels, const float* old_c, float* out_c, float* wpc, const unsigned* run);

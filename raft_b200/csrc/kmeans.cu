@@ -123,9 +123,9 @@ int km_args(const float* x, int64_t ldx, int64_t m, int64_t k, int64_t nc, const
   return B2D_OK;
 }
 
-// arg-min of every row against the prepared centroids: labels, inertia partials, label histogram (when hist)
-int km_assign(cudaStream_t s, const KmLayout& L, int64_t m, int64_t k, int64_t nc, const float* c, const float* w,
-              int* labels, const unsigned* run, bool prep_y, bool hist)
+// the start of an assignment: keys <- KEY_EMPTY, histogram <- 0, and the centroids prepared again when prep_y
+int km_assign_prep(cudaStream_t s, const KmLayout& L, int64_t m, int64_t k, int64_t nc, const float* c, const unsigned* run,
+                   bool prep_y, bool hist)
 {
   const int64_t nh = hist ? L.P.nhist : 0;
   // (the centroid side's exponent and scale flag are zeroed only where it is prepared again below)
@@ -136,15 +136,31 @@ int km_assign(cudaStream_t s, const KmLayout& L, int64_t m, int64_t k, int64_t n
     int rc = launch_prep<float>(s, L.tc, nullptr, 0, 1, m, c, k, 1, nc, k, nullptr, nullptr, TC_L2, nullptr, true, run);
     if (rc) return rc;
   }
-  TcParams p{};
-  p.m = m; p.n = nc; p.keys = L.tc.keys; p.run_flag = run;
-  int rc = launch_tc(s, L.tc, p, k, EPI_MINLOC, POST_NONE);
-  if (rc) return rc;
+  return B2D_OK;
+}
+
+// the end of an assignment: labels from the keys, inertia partials, label histogram (when hist)
+int km_assign_labels(cudaStream_t s, const KmLayout& L, int64_t m, int64_t nc, const float* w, int* labels,
+                     const unsigned* run, bool hist)
+{
   km_assign_kernel<<<static_cast<unsigned>(L.P.nblk), kKmThreads, 0, s>>>(run, L.tc.keys, labels, w, m, static_cast<int>(nc),
                                                                           L.P.rb, L.P.nblk, hist ? L.sort.hist : nullptr,
                                                                           L.ipart);
   B2D_CUDA(cudaGetLastError());
   return B2D_OK;
+}
+
+// arg-min of every row against the prepared centroids: labels, inertia partials, label histogram (when hist)
+int km_assign(cudaStream_t s, const KmLayout& L, int64_t m, int64_t k, int64_t nc, const float* c, const float* w,
+              int* labels, const unsigned* run, bool prep_y, bool hist)
+{
+  int rc = km_assign_prep(s, L, m, k, nc, c, run, prep_y, hist);
+  if (rc) return rc;
+  TcParams p{};
+  p.m = m; p.n = nc; p.keys = L.tc.keys; p.run_flag = run;
+  rc = launch_tc(s, L.tc, p, k, EPI_MINLOC, POST_NONE);
+  if (rc) return rc;
+  return km_assign_labels(s, L, m, nc, w, labels, run, hist);
 }
 
 // new centroids from the histogram km_assign (or km_sort_count) left: scan, stable scatter, fp64 sums

@@ -231,12 +231,6 @@ __global__ void __launch_bounds__(kKmThreads) km_scatter_kernel(const unsigned* 
   }
 }
 
-__device__ __forceinline__ void km_cluster_range(const unsigned* cur, int64_t nblk, int c, int64_t& cs, int64_t& ce)
-{
-  cs = c > 0 ? cur[static_cast<int64_t>(c) * nblk - 1] : 0;
-  ce = cur[static_cast<int64_t>(c) * nblk + nblk - 1];
-}
-
 // Chunk q = sorted positions [q * kKmChunk, (q + 1) * kKmChunk), columns [kKmCols * blockIdx.y, ...).  Each run of one
 // label is summed in fp64 in row order.  A run that is a whole cluster goes to sums / wsums; a run cut by the chunk
 // boundary goes to part / wpart slot 2q (it starts the chunk) or 2q + 1 (it ends the chunk).

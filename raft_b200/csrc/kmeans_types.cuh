@@ -1,4 +1,4 @@
-// Constants and control words of k-means (kmeans.cuh), without kernels: the label sort and scan of the host code
+// Constants, control words and the sorted cluster ranges of k-means (kmeans.cuh), without kernels: the label sort and scan of the host code
 // serve single linkage and DBSCAN too.
 #pragma once
 #include <cstdint>
@@ -30,5 +30,14 @@ struct KmCtrl {
   int pp_trials;        // k-means++: trials of the current round
   int pp_cand[kKmPpMaxTrials];
 };
+
+#ifdef __CUDACC__
+// rows [cs, ce) of cluster c in the sorted order, from the cursors the stable counting sort leaves (km_scatter_kernel)
+__device__ __forceinline__ void km_cluster_range(const unsigned* cur, int64_t nblk, int c, int64_t& cs, int64_t& ce)
+{
+  cs = c > 0 ? cur[static_cast<int64_t>(c) * nblk - 1] : 0;
+  ce = cur[static_cast<int64_t>(c) * nblk + nblk - 1];
+}
+#endif
 
 }  // namespace b2d

@@ -19,18 +19,6 @@ namespace b2d {
 constexpr int MASK_SLAB_ROWS = 64;    // rows of x one consumer warpgroup owns in a tile
 constexpr int MASK_HALF_COLS = TC_HN; // columns of y one wgmma covers
 
-// group of row c of y: the first g with group_idxs[g] > c, -1 if there is none (for a valid group_idxs)
-__host__ __device__ inline int masked_group_of(const int* group_idxs, int64_t G, int64_t c)
-{
-  int64_t lo = 0, hi = G;
-  while (lo < hi) {
-    const int64_t mid = (lo + hi) / 2;
-    if (group_idxs[mid] > c) hi = mid;
-    else lo = mid + 1;
-  }
-  return lo < G ? static_cast<int>(lo) : -1;
-}
-
 // Class of the tile (64-row slab `slab` of x, 128-column half `half` of y), from the adjacency bits
 // ([ceil(m/32)][G], masked_adj_bits_kernel) and a valid group_idxs:
 //   MASK_NONE     no (row, column) pair of the tile is adjacent (also: a tile outside the matrices)

@@ -373,22 +373,36 @@ static MaskedLayout masked_layout(void* base, int64_t m, int64_t n, int64_t k, i
 }
 
 namespace b2d {
+int masked_classify(cudaStream_t s, uint8_t* cls, const unsigned* bits, const int32_t* group_idxs, int64_t G, int64_t m,
+                    int64_t n, const unsigned* bad)
+{
+  const int tiles_m = static_cast<int>((m + TC_BM - 1) / TC_BM), tiles_n = static_cast<int>((n + TC_BN - 1) / TC_BN);
+  const int64_t ntiles = static_cast<int64_t>(tiles_m) * tiles_n;
+  masked_classify_kernel<<<static_cast<unsigned>((ntiles + 255) / 256), 256, 0, s>>>(cls, bits, group_idxs, G, m, n,
+                                                                                     tiles_m, tiles_n, bad);
+  B2D_CUDA(cudaGetLastError());
+  return B2D_OK;
+}
+
+int masked_launch(cudaStream_t s, const TcWorkspace& w, long long* keys, const int* grp, const unsigned* bits,
+                  const uint8_t* cls, int64_t G, int64_t m, int64_t n, int64_t k)
+{
+  TcParams p{};
+  p.m = m; p.n = n; p.keys = keys;
+  p.mask_cls = cls; p.mask_grp = grp; p.mask_bits = bits; p.mask_groups = G;
+  ProfileScope prof(s);
+  return launch_tc(s, w, p, k, EPI_MINLOC_MASKED, POST_NONE);
+}
+
 int masked_keys(cudaStream_t s, const TcWorkspace& w, long long* keys, const int* grp, unsigned* bits, uint8_t* cls,
                 const unsigned* bad, const uint8_t* adj, int64_t ld_adj, const int32_t* group_idxs, int64_t G,
                 int64_t m, int64_t n, int64_t k)
 {
   masked_adj_bits_kernel<<<static_cast<unsigned>((m + 31) / 32), 256, 0, s>>>(bits, adj, ld_adj, m, G);
   B2D_CUDA(cudaGetLastError());
-  const int tiles_m = static_cast<int>((m + TC_BM - 1) / TC_BM), tiles_n = static_cast<int>((n + TC_BN - 1) / TC_BN);
-  const int64_t ntiles = static_cast<int64_t>(tiles_m) * tiles_n;
-  masked_classify_kernel<<<static_cast<unsigned>((ntiles + 255) / 256), 256, 0, s>>>(cls, bits, group_idxs, G, m, n,
-                                                                                     tiles_m, tiles_n, bad);
-  B2D_CUDA(cudaGetLastError());
-  TcParams p{};
-  p.m = m; p.n = n; p.keys = keys;
-  p.mask_cls = cls; p.mask_grp = grp; p.mask_bits = bits; p.mask_groups = G;
-  ProfileScope prof(s);
-  return launch_tc(s, w, p, k, EPI_MINLOC_MASKED, POST_NONE);
+  int rc = masked_classify(s, cls, bits, group_idxs, G, m, n, bad);
+  if (rc) return rc;
+  return masked_launch(s, w, keys, grp, bits, cls, G, m, n, k);
 }
 }  // namespace b2d
 

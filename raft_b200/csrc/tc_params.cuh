@@ -38,6 +38,18 @@ __host__ __device__ __forceinline__ int mask_class_of(unsigned cls_byte, int h, 
 // some slab of half h is live: the streaming variant loads the half's stages
 __host__ __device__ __forceinline__ bool mask_half_live(unsigned cls_byte, int h) { return ((cls_byte >> (4 * h)) & 15u) != 0u; }
 
+// group of row c of y: the first g with group_idxs[g] > c, -1 if there is none (for a valid group_idxs)
+__host__ __device__ inline int masked_group_of(const int* group_idxs, int64_t G, int64_t c)
+{
+  int64_t lo = 0, hi = G;
+  while (lo < hi) {
+    const int64_t mid = (lo + hi) / 2;
+    if (group_idxs[mid] > c) hi = mid;
+    else lo = mid + 1;
+  }
+  return lo < G ? static_cast<int>(lo) : -1;
+}
+
 enum TcPost : int { POST_NONE = 0, POST_CLAMP = 1, POST_CLAMP_SQRT = 2,
                     POST_JACCARD = 3,  // d = 1 - a / (s - a), a = <x,y>, s = |x|^2 + |y|^2 (0/0 -> 0)
                     POST_DICE    = 4,  // d = 1 - 2 a / s
