@@ -1,6 +1,7 @@
 """fp64 reference of masked_l2_nn (raft::distance::masked_l2_nn), shared by the CPU and GPU tests: the distances in
 blocks of rows of y like oracle.fused_l2_nn, non-adjacent pairs excluded, ties to the smaller index, and the value of a
-row without any candidate that the library writes ({0x7fffffff, FLT_MAX})."""
+row without any candidate that the library writes ({0x7fffffff, FLT_MAX}).  NaN distances (NaN rows, inf - inf) are no
+candidates, as in the library's arg-min: a row whose every adjacent distance is NaN keeps that value."""
 import numpy as np
 
 NO_CANDIDATE = 0x7FFFFFFF
@@ -33,7 +34,7 @@ def masked_l2_nn(x, y, adj, group_idxs, sqrt=False, block=4096):
         gb = grp[j0:j0 + block]
         d = np.maximum(xx[:, None] + (yb * yb).sum(1)[None, :] - 2.0 * (x64 @ yb.T), 0.0)
         ok = (gb >= 0)[None, :] & adj[:, np.maximum(gb, 0)] if adj.shape[1] else np.zeros(d.shape, bool)
-        d = np.where(ok, d, np.inf)
+        d = np.where(ok & ~np.isnan(d), d, np.inf)     # a NaN distance never wins (np.argmin would pick it)
         loc = np.argmin(d, axis=1)
         v = d[np.arange(m), loc]
         upd = v < best_v                     # strict: the earlier (smaller) index wins ties

@@ -51,6 +51,23 @@ def test_reference_against_brute_force():
     assert (ri3 == ri).all() and np.allclose(rv3[rv < FLT_MAX], np.sqrt(rv[rv < FLT_MAX]))
 
 
+def test_reference_nan_distances_never_win():
+    """A NaN distance is no candidate (the library's NaN rule): a NaN row of y in an adjacent group must not hide the
+    finite minimum of its block, and a row whose only adjacent row of y is NaN has no candidate."""
+    x = np.array([[0, 0]], dtype=np.float32)
+    y = np.array([[np.nan, 0], [1, 0], [3, 0]], dtype=np.float32)
+    ri, rv = ref_masked_l2_nn(x, y, np.ones((1, 1), bool), np.array([3], np.int32))
+    assert ri.tolist() == [1] and rv.tolist() == [1.0]
+    ri, rv = ref_masked_l2_nn(x, y, np.ones((1, 1), bool), np.array([3], np.int32), sqrt=True)
+    assert ri.tolist() == [1] and rv.tolist() == [1.0]
+    # groups {0} (the NaN row) and {1, 2}: adjacent to the NaN row alone -> the sentinel; to both -> index 1
+    gidx = np.array([1, 3], np.int32)
+    x2 = np.array([[0, 0], [0, 0], [np.nan, 0]], dtype=np.float32)
+    adj = np.array([[1, 0], [1, 1], [1, 1]], bool)
+    ri, rv = ref_masked_l2_nn(x2, y, adj, gidx, block=2)
+    assert ri.tolist() == [NO_CANDIDATE, 1, NO_CANDIDATE] and rv.tolist() == [FLT_MAX, 1.0, FLT_MAX]
+
+
 def test_workspace_query():
     L = _lib.lib()
     base = L.b2d_masked_l2_nn_workspace_bytes(1000, 2000, 64, 10)
