@@ -33,7 +33,7 @@
 //
 // Epilogues (straight from the registers; d = acc * c + (t_x[i] + t_y[j]), c one scalar):
 //   EPI_STORE         the finished 64 x 128 fragment goes to the warpgroup's own staging boxes in shared
-//                     memory (SWIZZLE_128B, a ring of 64-row x 32-column boxes) and leaves by TMA stores that
+//                     memory (SWIZZLE_128B, a ring of 32-row x 64-column boxes) and leaves by TMA stores that
 //                     drain while the warpgroup runs the next half's MMAs (tc_stage_store).  Where TMA cannot
 //                     address dist (unaligned base or pitch) and in the read-modify-write path of K-chunked
 //                     accumulation (k > 320), each thread stores its 2 adjacent columns of 2 rows per
@@ -425,50 +425,67 @@ __device__ __forceinline__ void tc_epilogue_store_fast(float (&v)[64], const TcP
 }
 
 // EPI_STORE through TMA: the warpgroup's finished 64 x 128 tile v (fragment layout as in tc_epilogue) is written into
-// its ring of two staging boxes and stored with one cp.async.bulk.tensor per 64 x 32 box (L2 evict-first: the result is
-// not read again here).  The tile's 4 boxes go out as two pairs, one box per slot: the lead thread (`issuer`) waits until
-// the previous pair's stores have finished reading both slots, the warpgroup meets at its named barrier, writes the pair,
-// fences it for the TMA unit once and meets again, and the lead issues both stores as one bulk group.  One fence (MEMBAR +
-// FENCE.VIEW.ASYNC in the SASS) and two barriers per pair measured faster than a fence per box or a per-slot mbarrier
-// hand-off (DESIGN.md section 5).  Only this warpgroup writes its boxes and only its lead issues and waits for their
-// stores.  Boxes outside the matrix are skipped; TMA clips the ragged ones.  After the CTA's last tile (`last`) the
-// issuer waits for all its stores, so the CTA's shared memory outlives them.
-//   box element (r, c) sits at byte r * 128 + ((c / 4) ^ (r % 8)) * 16 + (c % 4) * 4 (SWIZZLE_128B): the warp's 8-byte
-//   writes (8 rows x 2 adjacent 16-byte chunks) cover every bank exactly twice -- no conflicts.
-__device__ __forceinline__ void tc_stage_store(const float (&v)[64], const CUtensorMap* tmap_d, uint32_t stg, bool issuer,
-                                               bool last, int wg, int64_t row_w, int64_t col_w, const TcParams& p)
+// its ring of two staging boxes and stored with one cp.async.bulk.tensor per 32-row x 64-column box (L2 evict-first: the
+// result is not read again here).  The box goes through a 3-D view of dist, {32 columns, column group, row} with box
+// {32, 2, 32}, so each store writes 256 contiguous bytes of each of its 32 rows; 64 x 32 boxes of 128-byte row pieces
+// made the kernel measurably slower (DESIGN.md section 5).  The tile's 4 boxes go out as two pairs: pair q holds columns
+// [64 q, 64 q + 64), rows [32 s, 32 s + 32) in slot s, written by warps 2 s and 2 s + 1.  The lead thread (`issuer`)
+// waits until the previous pair's stores have finished reading both slots, the warpgroup meets at its named barrier,
+// writes the pair, fences it for the TMA unit once and meets again, and the lead issues both stores as one bulk group.
+// One fence (MEMBAR + FENCE.VIEW.ASYNC in the SASS) and two barriers per pair measured faster than a fence per box or a
+// per-slot mbarrier hand-off (DESIGN.md section 5).  Only this warpgroup writes its boxes and only its lead issues and
+// waits for their stores.  Boxes outside the matrix are skipped; TMA clips the ragged ones at row m and at the last whole
+// column group of tmap_d ({32, n / 32, m}).  When n % 32 != 0, the box holding the last, partial group ng = n / 32 also
+// goes out through tmap_dt, a view of the groups from the box's first one, gb = ng rounded down to even (boxes start at
+// even groups), to ng: {n % 32, ng - gb + 1, m}, same box, at coordinates (0, 0, row).  TMA clips every column at or past
+// n there, so nothing lands in the caller's padding; when ng is odd it also writes the first n % 32 columns of group
+// ng - 1 again, with the values tmap_d wrote there.  (The view starts at the box, not at the partial group, so that no
+// coordinate is negative: a store at group coordinate -1 ended in a device fault on an H100.)  After the CTA's last
+// tile (`last`) the issuer waits for all its stores, so the CTA's shared memory outlives them.
+//   box element (r, g, c) (row, column group, column of the group) sits in 128-byte line L = 2 r + g, at byte
+//   L * 128 + ((c / 4) ^ (L % 8)) * 16 + (c % 4) * 4 (SWIZZLE_128B).  L % 8 = (2 quad + g) % 8 for the warp's rows, so
+//   rows quad and quad + 4 share a phase, but the warp's 8-byte writes (8 rows x 2 adjacent 16-byte chunks) still cover
+//   every bank exactly twice -- no conflicts.
+__device__ __forceinline__ void tc_stage_store(const float (&v)[64], const CUtensorMap* tmap_d, const CUtensorMap* tmap_dt,
+                                               uint32_t stg, bool issuer, bool last, int wg, int64_t row_w, int64_t col_w,
+                                               const TcParams& p)
 {
   static_assert(TC_STG_BOXES == 2, "a pair of boxes fills the ring: wait_group.read 0 frees it");
-  const int lane       = threadIdx.x & 31;
+  static_assert(TC_D_BOX_GROUPS == 2 && TC_D_BOX_ROWS == 32, "the addressing below is written for 32 x 64 boxes");
+  const int lane = threadIdx.x & 31, w = (threadIdx.x >> 5) & 3;
   const int quad = lane >> 2, tq = lane & 3;
-  // this thread's rows 16 w + quad (+8) of the box and the swizzled 16-byte chunk of its column pair
-  const uint32_t t_off = (16 * ((threadIdx.x >> 5) & 3) + quad) * 128 + 8 * (tq & 1);
-  const uint32_t t_xor = static_cast<uint32_t>((tq >> 1) ^ quad) * 16;
+  // this thread's rows 16 (w % 2) + quad (+8) of the box in slot w / 2 and the swizzled 16-byte chunk of its column pair
+  const uint32_t t_off = stg + (w >> 1) * TC_D_BOX_BYTES + (16 * (w & 1) + quad) * 256 + 8 * (tq & 1);
+  const uint32_t t_xor = static_cast<uint32_t>((tq >> 1) ^ (2 * (quad & 3))) * 16;
 #pragma unroll
-  for (int q = 0; q < 2; ++q) {   // the tile's 4 boxes of 32 columns as two pairs: box 2 q + s in slot s
+  for (int q = 0; q < 2; ++q) {
     // the previous pair's stores have read both slots
     if (issuer) ptx::tma_store_wait_read<0>();
     ptx::bar_sync(2 + wg, 128);
 #pragma unroll
-    for (int s = 0; s < 2; ++s)
+    for (int ii = 0; ii < 8; ++ii) {
+      const int i = 8 * q + ii, g = ii >> 2;   // 8-column group of the tile, column group of the box
 #pragma unroll
-      for (int ii = 0; ii < 4; ++ii) {
-        const int i = 8 * q + 4 * s + ii;   // 8-column group of the tile
-#pragma unroll
-        for (int j = 0; j < 2; ++j)
-          ptx::st_shared_v2(stg + s * TC_D_BOX_BYTES + t_off + 8 * j * 128 + ((32 * ii) ^ t_xor), v[4 * i + 2 * j],
-                            v[4 * i + 2 * j + 1]);
-      }
+      for (int j = 0; j < 2; ++j)
+        ptx::st_shared_v2(t_off + j * 8 * 256 + g * 128 + ((32 * (ii & 3) + 16 * g) ^ t_xor), v[4 * i + 2 * j],
+                          v[4 * i + 2 * j + 1]);
+    }
     ptx::fence_proxy_async_smem();   // the generic-proxy writes become visible to the TMA unit
     ptx::bar_sync(2 + wg, 128);
     if (issuer) {
+      // (32-bit coordinates: the TMA path is only taken with m and n below 2^31, tc_store_plan)
+      const int n = static_cast<int>(p.n), ng = n >> 5;                          // whole column groups of dist
+      const int gc = static_cast<int>(col_w) + TC_D_BOX_COLS * q, gg = gc >> 5;   // the pair's first column and group
 #pragma unroll
       for (int s = 0; s < 2; ++s) {
-        const int64_t gc = col_w + TC_D_BOX_COLS * (2 * q + s);
+        const int gr = static_cast<int>(row_w) + TC_D_BOX_ROWS * s;
 #if !defined(B2D_TC_DIAG) || B2D_TC_DIAG != 2
-        if (gc < p.n && row_w < p.m)
-          ptx::tma_store_2d(tmap_d, stg + s * TC_D_BOX_BYTES, static_cast<int32_t>(gc), static_cast<int32_t>(row_w),
-                            ptx::policy_evict_first());
+        if (gc < n && gr < static_cast<int>(p.m)) {
+          const uint32_t box = stg + s * TC_D_BOX_BYTES;
+          if (gg < ng) ptx::tma_store_3d(tmap_d, box, 0, gg, gr, ptx::policy_evict_first());
+          if ((n & 31) != 0 && gg == (ng & ~1))   // the box holds the partial group ng
+            ptx::tma_store_3d(tmap_dt, box, 0, 0, gr, ptx::policy_evict_first());
+        }
 #endif
       }
       ptx::tma_store_commit();   // one group per pair (possibly empty): the wait above counts pairs
@@ -594,7 +611,7 @@ __device__ __forceinline__ void tc_eps_flush(const TcParams& p, const uint32_t* 
 template <bool kResident, int kEpi, int kPost>
 __global__ void __launch_bounds__(TC_THREADS, 1)
 expanded_tc_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b,
-                   const __grid_constant__ CUtensorMap tmap_d, const TcParams p)
+                   const __grid_constant__ CUtensorMap tmap_d, const __grid_constant__ CUtensorMap tmap_dt, const TcParams p)
 {
   using Carve                    = TcCarve<kResident, kEpi>;
   constexpr int kStages          = Carve::stages;
@@ -628,6 +645,7 @@ expanded_tc_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_cons
     ptx::prefetch_tmap(&tmap_a);
     ptx::prefetch_tmap(&tmap_b);
     if ((kEpi == EPI_STORE || kEpi == EPI_EPS) && p.tma_store) ptx::prefetch_tmap(&tmap_d);
+    if (kEpi == EPI_STORE && p.tma_store && p.n % 32 != 0) ptx::prefetch_tmap(&tmap_dt);
   }
   __syncthreads();
 
@@ -900,7 +918,8 @@ expanded_tc_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_cons
           tc_epilogue<kEpi, kPost>(acc, p, col_tb, cl0, static_cast<int64_t>(n_blk) * TC_BN + cl0, row0, ta, cfr, thr, xnr,
                                    ynu, keep);
         if (kEpi == EPI_STORE && p.tma_store)   // (this warpgroup's staging boxes: computed here, not kept live)
-          tc_stage_store(acc, &tmap_d, ptx::smem_u32(smem + Carve::stg_off) + wg * TC_STG_BOXES * TC_D_BOX_BYTES, lead,
+          tc_stage_store(acc, &tmap_d, &tmap_dt,
+                         ptx::smem_u32(smem + Carve::stg_off) + wg * TC_STG_BOXES * TC_D_BOX_BYTES, lead,
                          item + gridDim.x >= p.n_items && mt == mt1 - 1 && h == nh - 1, wg,
                          static_cast<int64_t>(mt) * TC_BM + 64 * wg, static_cast<int64_t>(n_blk) * TC_BN + h * TC_HN, p);
         if constexpr (kEpi == EPI_EPS)

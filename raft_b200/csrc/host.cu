@@ -50,21 +50,38 @@ static EncodeTiledFn get_encode()
   return fn;
 }
 
+static int encode_tiled(CUtensorMap* map, CUtensorMapDataType dtype, int rank, const void* base, const cuuint64_t* dims,
+                        const cuuint64_t* strides, const cuuint32_t* box, CUtensorMapSwizzle swizzle,
+                        CUtensorMapL2promotion promotion, const char* tag)
+{
+  EncodeTiledFn enc = get_encode();
+  if (!enc) return fail(B2D_ERR_CUDA, "cuTensorMapEncodeTiled entry point unavailable (no CUDA driver?)");
+  const cuuint32_t estr[3] = {1, 1, 1};
+  CUresult r = enc(map, dtype, static_cast<cuuint32_t>(rank), const_cast<void*>(base), dims, strides, box, estr,
+                   CU_TENSOR_MAP_INTERLEAVE_NONE, swizzle, promotion, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  if (r != CUDA_SUCCESS)
+    return fail(B2D_ERR_CUDA, std::string("cuTensorMapEncodeTiled") + tag + " failed: " + std::to_string((int)r));
+  return B2D_OK;
+}
+
 int encode_2d(CUtensorMap* map, CUtensorMapDataType dtype, const void* base, int64_t cols, int64_t rows,
               int64_t pitch_bytes, unsigned box_cols, unsigned box_rows, CUtensorMapSwizzle swizzle,
               CUtensorMapL2promotion promotion, const char* tag)
 {
-  EncodeTiledFn enc = get_encode();
-  if (!enc) return fail(B2D_ERR_CUDA, "cuTensorMapEncodeTiled entry point unavailable (no CUDA driver?)");
-  cuuint64_t dims[2]    = {static_cast<cuuint64_t>(cols), static_cast<cuuint64_t>(rows)};
-  cuuint64_t strides[1] = {static_cast<cuuint64_t>(pitch_bytes)};
-  cuuint32_t box[2]     = {box_cols, box_rows};
-  cuuint32_t estr[2]    = {1, 1};
-  CUresult r = enc(map, dtype, 2, const_cast<void*>(base), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, swizzle,
-                   promotion, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  if (r != CUDA_SUCCESS)
-    return fail(B2D_ERR_CUDA, std::string("cuTensorMapEncodeTiled") + tag + " failed: " + std::to_string((int)r));
-  return B2D_OK;
+  const cuuint64_t dims[2]    = {static_cast<cuuint64_t>(cols), static_cast<cuuint64_t>(rows)};
+  const cuuint64_t strides[1] = {static_cast<cuuint64_t>(pitch_bytes)};
+  const cuuint32_t box[2]     = {box_cols, box_rows};
+  return encode_tiled(map, dtype, 2, base, dims, strides, box, swizzle, promotion, tag);
+}
+
+int encode_3d(CUtensorMap* map, CUtensorMapDataType dtype, const void* base, const int64_t (&dims)[3],
+              const int64_t (&pitch_bytes)[2], const unsigned (&box)[3], CUtensorMapSwizzle swizzle,
+              CUtensorMapL2promotion promotion, const char* tag)
+{
+  const cuuint64_t d[3] = {static_cast<cuuint64_t>(dims[0]), static_cast<cuuint64_t>(dims[1]), static_cast<cuuint64_t>(dims[2])};
+  const cuuint64_t s[2] = {static_cast<cuuint64_t>(pitch_bytes[0]), static_cast<cuuint64_t>(pitch_bytes[1])};
+  const cuuint32_t b[3] = {box[0], box[1], box[2]};
+  return encode_tiled(map, dtype, 3, base, d, s, b, swizzle, promotion, tag);
 }
 
 int device_sms(int* sms)

@@ -56,6 +56,10 @@ int check_workspace(const void* ws, size_t bytes, size_t need, size_t align = 25
 int encode_2d(CUtensorMap* map, CUtensorMapDataType dtype, const void* base, int64_t cols, int64_t rows,
               int64_t pitch_bytes, unsigned box_cols, unsigned box_rows, CUtensorMapSwizzle swizzle,
               CUtensorMapL2promotion promotion, const char* tag);
+// the same for a 3-D view: dims and box innermost first, pitch_bytes of dimensions 1 and 2
+int encode_3d(CUtensorMap* map, CUtensorMapDataType dtype, const void* base, const int64_t (&dims)[3],
+              const int64_t (&pitch_bytes)[2], const unsigned (&box)[3], CUtensorMapSwizzle swizzle,
+              CUtensorMapL2promotion promotion, const char* tag);
 
 // SM count of the current device; every kernel of the library is built for sm_90a only, so any other device is an error
 int device_sms(int* sms);

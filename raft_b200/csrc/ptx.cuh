@@ -108,6 +108,16 @@ __device__ __forceinline__ void tma_store_2d(const void* tmap, uint32_t smem_src
     : "l"(reinterpret_cast<uint64_t>(tmap)), "r"(smem_src), "r"(c0), "r"(c1), "l"(policy)
     : "memory");
 }
+// the same through a 3-D tensor map (coordinates innermost first)
+__device__ __forceinline__ void tma_store_3d(const void* tmap, uint32_t smem_src, int32_t c0, int32_t c1, int32_t c2,
+                                             uint64_t policy)
+{
+  asm volatile(
+    "cp.async.bulk.tensor.3d.global.shared::cta.bulk_group.L2::cache_hint [%0, {%2, %3, %4}], [%1], %5;"
+    :
+    : "l"(reinterpret_cast<uint64_t>(tmap)), "r"(smem_src), "r"(c0), "r"(c1), "r"(c2), "l"(policy)
+    : "memory");
+}
 __device__ __forceinline__ void tma_store_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
 // all but the N most recent committed bulk-store groups of this thread have finished READING shared memory
 template <int N>

@@ -19,13 +19,16 @@ constexpr int TC_STAGES_RES_ST = 4;          // the same with the output staging
 constexpr int TC_STAGES_STR_ST = 6;
 constexpr int TC_MAX_STAGES  = 6;
 constexpr int TC_THREADS     = 384;
-// EPI_STORE output staging: TMA boxes of 64 rows x 32 fp32 columns (128-byte rows, SWIZZLE_128B), a ring of
-// TC_STG_BOXES per consumer warpgroup (DESIGN.md section 2 K1: the carve against the x stages, measured).  The ring
-// logic of tc_stage_store is written for exactly two boxes.
-constexpr int TC_D_BOX_COLS  = 32;
-constexpr int TC_D_BOX_ROWS  = 64;
-constexpr int TC_D_BOX_BYTES = TC_D_BOX_COLS * TC_D_BOX_ROWS * 4;
-constexpr int TC_STG_BOXES   = 2;
+// EPI_STORE output staging: TMA boxes of 32 rows x 64 fp32 columns, stored through a 3-D view of dist (32 columns x
+// column group x row, box {32, TC_D_BOX_GROUPS, TC_D_BOX_ROWS}, SWIZZLE_128B over its 128-byte lines), so that each
+// store writes 256 contiguous bytes of every row it touches; a ring of TC_STG_BOXES per consumer warpgroup (DESIGN.md
+// section 2 K1: the box shape and the carve against the x stages, measured).  The ring logic of tc_stage_store is
+// written for exactly two boxes of this shape.  EPI_EPS stages its 64 x 128-byte adjacency tiles in the same 8 KB slots.
+constexpr int TC_D_BOX_GROUPS = 2;
+constexpr int TC_D_BOX_COLS   = 32 * TC_D_BOX_GROUPS;
+constexpr int TC_D_BOX_ROWS   = 32;
+constexpr int TC_D_BOX_BYTES  = TC_D_BOX_COLS * TC_D_BOX_ROWS * 4;
+constexpr int TC_STG_BOXES    = 2;
 
 enum TcEpilogue : int { EPI_STORE = 0, EPI_MINLOC = 1, EPI_TOPK = 2, EPI_MINLOC_MASKED = 3, EPI_EPS = 4, EPI_RADIUS = 5 };
 constexpr int64_t TC_NO_DIAG = INT64_MIN;   // TcParams::diag_off: y is not a row window of x

@@ -132,20 +132,20 @@ template int launch_prep<__half>(cudaStream_t, const TcWorkspace&, const void*, 
                                  const int*, bool, const unsigned*);
 
 template <bool kRes, int kEpi, int kPost>
-static int launch_tc_inst(cudaStream_t s, const CUtensorMap& ma, const CUtensorMap& mb, const CUtensorMap& md,
+static int launch_tc_inst(cudaStream_t s, const CUtensorMap& ma, const CUtensorMap& mb, const CUtensorMap (&md)[2],
                           const TcParams& p, int grid)
 {
   constexpr size_t smem = TcCarve<kRes, kEpi>::bytes;
   // the attribute is per device and per function: cheap, set on every launch
   B2D_CUDA(cudaFuncSetAttribute(expanded_tc_kernel<kRes, kEpi, kPost>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                 static_cast<int>(smem)));
-  expanded_tc_kernel<kRes, kEpi, kPost><<<grid, TC_THREADS, smem, s>>>(ma, mb, md, p);
+  expanded_tc_kernel<kRes, kEpi, kPost><<<grid, TC_THREADS, smem, s>>>(ma, mb, md[0], md[1], p);
   B2D_CUDA(cudaGetLastError());
   return B2D_OK;
 }
 
 template <bool kRes>
-static int launch_tc_epi(cudaStream_t s, const CUtensorMap& ma, const CUtensorMap& mb, const CUtensorMap& md,
+static int launch_tc_epi(cudaStream_t s, const CUtensorMap& ma, const CUtensorMap& mb, const CUtensorMap (&md)[2],
                          const TcParams& p, int grid, int epi, int post)
 {
   if (epi == EPI_MINLOC) return launch_tc_inst<kRes, EPI_MINLOC, POST_NONE>(s, ma, mb, md, p, grid);
@@ -214,17 +214,31 @@ int launch_tc(cudaStream_t s, const TcWorkspace& w, TcParams p, int64_t k, int e
   // resident: the whole 256-row y block in one box per k-block; streaming: one 128-row half per stage
   rc = make_operand_map(&mb, w.yop, p.n, p.nkb, resident ? TC_BN : TC_HN, kb0, nkb_total);
   if (rc) return rc;
-  CUtensorMap md;   // only read by the kernel when EPI_STORE or EPI_EPS goes through TMA
-  memset(&md, 0, sizeof(md));
-  // both need a 16-byte aligned base and pitch.  EPI_STORE: dist [m][n] fp32 in boxes of 32 columns x 64 rows
-  // (expanded_tc.cuh tc_stage_store); EPI_EPS: adj [m][n] bytes in boxes of 128 columns x 64 rows (tc_eps_tile)
+  CUtensorMap md[2];   // only read by the kernel when EPI_STORE or EPI_EPS goes through TMA
+  memset(md, 0, sizeof(md));
+  // both need a 16-byte aligned base and pitch.  EPI_STORE: dist [m][n] fp32 as {32 columns, column group, row} in boxes
+  // of 32 x 2 x 32 (expanded_tc.cuh tc_stage_store): md[0] holds the ng = n / 32 whole column groups; when n % 32 != 0,
+  // md[1] holds n % 32 columns of the groups from the box that contains the partial group ng (from group ng rounded down
+  // to even) to ng.  With no whole group md[0] is a copy of md[1]: the kernel then never stores through md[0].
+  // EPI_EPS: adj [m][n] bytes in boxes of 128 columns x 64 rows (tc_eps_tile)
   if (epi == EPI_STORE && p.tma_store) {
-    rc = encode_2d(&md, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, p.dist, p.n, p.m, p.ldd * 4, TC_D_BOX_COLS, TC_D_BOX_ROWS,
-                   CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_NONE, "(dist)");
-    if (rc) return rc;
+    const int64_t ng = p.n / 32, tail = p.n % 32, gb = ng & ~int64_t{1}, pitch[2] = {128, p.ldd * 4};
+    const unsigned box[3] = {32, TC_D_BOX_GROUPS, TC_D_BOX_ROWS};
+    if (tail != 0) {
+      rc = encode_3d(&md[1], CU_TENSOR_MAP_DATA_TYPE_FLOAT32, p.dist + gb * 32, {tail, ng - gb + 1, p.m}, pitch, box,
+                     CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_NONE, "(dist, last column group)");
+      if (rc) return rc;
+    }
+    if (ng != 0) {
+      rc = encode_3d(&md[0], CU_TENSOR_MAP_DATA_TYPE_FLOAT32, p.dist, {32, ng, p.m}, pitch, box,
+                     CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_NONE, "(dist)");
+      if (rc) return rc;
+    } else {
+      md[0] = md[1];
+    }
   }
   if (epi == EPI_EPS && p.tma_store) {
-    rc = encode_2d(&md, CU_TENSOR_MAP_DATA_TYPE_UINT8, p.adj, p.n, p.m, p.ld_adj, TC_HN, TC_D_BOX_ROWS,
+    rc = encode_2d(&md[0], CU_TENSOR_MAP_DATA_TYPE_UINT8, p.adj, p.n, p.m, p.ld_adj, TC_HN, TC_BM / 2,
                    CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_NONE, "(adj)");
     if (rc) return rc;
   }
