@@ -10,12 +10,12 @@ median of --reps.
 
 Inputs: Gaussian blobs of three spreads with 10 % uniform noise; eps is set from a row sample so that about --density of
 the pairs are adjacent, which leaves core, border and noise points.  Shapes: 100000 x 128 (one 2^30-byte batch plan of
-ten batches) and 1000000 x 32 (977 batches of 1024 columns).  Prints one JSON line per measurement (card, power limit
-and SM clock included) and writes them to --out."""
+ten batches) and 1000000 x 32 (977 batches of 1024 columns).  Prints one JSON line per measurement (the card, its power
+limit and max SM clock included) and writes them to --out."""
 import argparse
 import json
 import os
-import subprocess
+import statistics
 import sys
 import time
 
@@ -23,14 +23,9 @@ import numpy as np
 import torch
 
 sys.path.insert(0, os.path.join(os.path.dirname(os.path.abspath(__file__)), ".."))
+from measure import card, time_ms  # noqa: E402
 from raft_b200.cluster import dbscan  # noqa: E402
 from raft_b200.neighbors.epsilon_neighborhood import eps_neighbors_l2sq  # noqa: E402
-
-
-def card():
-    q = "name,power.limit,clocks.sm,clocks.max.sm"
-    return subprocess.run(["nvidia-smi", "--query-gpu=" + q, "--format=csv,noheader"], capture_output=True,
-                          text=True).stdout.strip()
 
 
 def blobs(m, d, n_blobs, seed):
@@ -48,20 +43,6 @@ def pick_eps(x, density):
     s = x[torch.randperm(x.shape[0], device="cuda")[:4000]].double()
     d2 = torch.cdist(s, s).pow(2)
     return float(torch.quantile(d2[~torch.eye(len(s), dtype=torch.bool, device="cuda")][:10 ** 7], density).sqrt())
-
-
-def total_ms(x, eps, ms, reps):
-    dbscan(x, eps, min_samples=ms)
-    ts = []
-    for _ in range(reps):
-        a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-        torch.cuda.synchronize()
-        a.record()
-        dbscan(x, eps, min_samples=ms)
-        b.record()
-        torch.cuda.synchronize()
-        ts.append(a.elapsed_time(b))
-    return float(np.median(ts))
 
 
 def passes(x, eps, ms):
@@ -142,11 +123,11 @@ def main():
     ap.add_argument("--no-baseline", action="store_true")
     ap.add_argument("--out", default=None)
     a = ap.parse_args()
-    assert torch.cuda.is_available(), "needs a GPU"
+    gpu = card()
     rows = []
 
     def emit(r):
-        r["card"] = card()
+        r["card"] = gpu
         rows.append(r)
         print(json.dumps(r), flush=True)
 
@@ -155,7 +136,7 @@ def main():
         x = blobs(m, d, max(10, m // 1000), seed=m + d)
         eps = pick_eps(x, dens)
         r = {"shape": shape, "eps": eps, "min_samples": a.min_samples, "what": "dbscan",
-             "total_ms": total_ms(x, eps, a.min_samples, a.reps)}
+             "total_ms": statistics.median(time_ms(lambda: dbscan(x, eps, min_samples=a.min_samples), a.reps))}
         p, out = passes(x, eps, a.min_samples)
         r.update(p)
         emit(r)
@@ -173,7 +154,9 @@ def main():
             t_sk = (time.perf_counter() - t) * 1e3
             o = dbscan(xs, eps, min_samples=a.min_samples)
             emit({"shape": "%dx%d" % (a.sk_rows, d), "what": "sklearn.cluster.DBSCAN n_jobs=-1 (host)",
-                  "cpus": os.cpu_count(), "total_ms": t_sk, "gpu_total_ms": total_ms(xs, eps, a.min_samples, a.reps),
+                  "cpus": os.cpu_count(), "total_ms": t_sk,
+                  "gpu_total_ms": statistics.median(time_ms(lambda: dbscan(xs, eps, min_samples=a.min_samples),
+                                                            a.reps)),
                   "labels_equal": bool((o.labels.cpu().numpy() == sk.labels_).all())})
         del x
         torch.cuda.empty_cache()

@@ -15,13 +15,13 @@ import argparse
 import json
 import os
 import statistics
-import subprocess
 import sys
 
 import torch
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import oracle  # noqa: E402
+from measure import card, time_ms  # noqa: E402
 from raft_b200.common import DeviceResources  # noqa: E402
 from raft_b200.distance import pairwise_distance  # noqa: E402
 from raft_b200.neighbors import eps_neighbors_l2sq  # noqa: E402
@@ -29,35 +29,14 @@ from raft_b200.neighbors import eps_neighbors_l2sq  # noqa: E402
 WORKLOADS = [(100000, 100000, 128), (1000000, 8192, 32), (1000000, 8190, 32)]
 
 
-def card():
-    name = torch.cuda.get_device_name(0)
-    q = subprocess.run(["nvidia-smi", "--id=0", "--query-gpu=power.limit,clocks.max.sm", "--format=csv,noheader"],
-                       capture_output=True, text=True, timeout=30).stdout.strip()
-    return name, q
-
-
-def timed(fn, runs):
-    fn()
-    torch.cuda.synchronize()
-    ts = []
-    for _ in range(runs):
-        a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-        a.record()
-        fn()
-        b.record()
-        b.synchronize()
-        ts.append(a.elapsed_time(b))
-    return statistics.median(ts), ts
-
-
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--runs", type=int, default=5)
     ap.add_argument("--only", default="")
     a = ap.parse_args()
-    assert torch.cuda.is_available(), "needs a GPU"
-    name, pl = card()
-    print("card: %s, power limit, max SM clock: %s" % (name, pl), flush=True)
+    gpu = card()
+    pl = "%s W, %s MHz" % (gpu["power_limit"], gpu["clocks_max_sm"])
+    print("card: %s, power limit, max SM clock: %s" % (gpu["name"], pl), flush=True)
     h = DeviceResources()
     sel = [int(s) for s in a.only.split(",") if s] or range(len(WORKLOADS))
     for wi in sel:
@@ -103,9 +82,9 @@ def main():
         del ra, cnt
         res = {}
         for arm, fn in (("fused_adj", fused), ("fused_count", count_only), ("composition", composition)):
-            med, ts = timed(lambda: (fn(), h.sync()), a.runs)
-            res[arm] = {"median_ms": round(med, 3), "ms": [round(t, 3) for t in ts]}
-        print(json.dumps({"m": m, "n": n, "k": k, "eps": eps, "adjacent_fraction": round(frac, 5), "card": name,
+            ts = time_ms(lambda: (fn(), h.sync()), a.runs)
+            res[arm] = {"median_ms": round(statistics.median(ts), 3), "ms": [round(t, 3) for t in ts]}
+        print(json.dumps({"m": m, "n": n, "k": k, "eps": eps, "adjacent_fraction": round(frac, 5), "card": gpu["name"],
                           "power_limit_max_sm_clock": pl, **res}), flush=True)
         del x, y, dist, adj, vd
         torch.cuda.empty_cache()

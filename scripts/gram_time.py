@@ -9,41 +9,16 @@ import argparse
 import json
 import os
 import statistics
-import subprocess
 import sys
 
 import torch
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
+from measure import card, time_ms  # noqa: E402
 from raft_b200.distance import gram_matrix, pairwise_distance  # noqa: E402
 from raft_b200.common import DeviceResources  # noqa: E402
 
 PARAMS = {"linear": (0, 1.0, 0.0), "polynomial": (3, 1.0 / 128, 1.0), "rbf": (0, 1.0 / 256, 0.0), "tanh": (0, 1.0 / 128, -0.5)}
-
-
-def card():
-    name = torch.cuda.get_device_name(0)
-    try:
-        q = subprocess.run(["nvidia-smi", "--query-gpu=power.limit,clocks.max.sm", "--format=csv,noheader"],
-                           capture_output=True, text=True, timeout=30).stdout.strip().splitlines()[0]
-    except (OSError, IndexError, subprocess.TimeoutExpired):
-        q = "power limit unknown"
-    return name, q
-
-
-def timed(fn, h, runs, warmup):
-    for _ in range(warmup):
-        fn()
-    h.sync()
-    ms = []
-    for _ in range(runs):
-        a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-        a.record(h.torch_stream)
-        fn()
-        b.record(h.torch_stream)
-        b.synchronize()
-        ms.append(a.elapsed_time(b))
-    return statistics.median(ms)
 
 
 def transform(out, kernel, degree, gamma, coef0):
@@ -68,21 +43,24 @@ def case(label, m, n, k, col_major, kernels, h, args, compose):
         out = torch.empty((m, n), device="cuda")
     rows = []
     base_ms = {}
-    with torch.cuda.stream(h.torch_stream):
+    st = h.torch_stream   # the events go on the handle's stream, where the calls run
+    with torch.cuda.stream(st):
         for kernel in kernels:
             degree, gamma, coef0 = PARAMS[kernel]
             metric = "sqeuclidean" if kernel == "rbf" else "inner_product"
             if metric not in base_ms:
-                base_ms[metric] = timed(lambda: pairwise_distance(x, y, out=out, metric=metric, handle=h), h, args.runs,
-                                        args.warmup)
-            fused = timed(lambda: gram_matrix(x, y, kernel, degree=degree, gamma=gamma, coef0=coef0, out=out, handle=h), h,
-                          args.runs, args.warmup)
+                base_ms[metric] = statistics.median(time_ms(
+                    lambda: pairwise_distance(x, y, out=out, metric=metric, handle=h), args.runs, args.warmup,
+                    stream=st))
+            fused = statistics.median(time_ms(
+                lambda: gram_matrix(x, y, kernel, degree=degree, gamma=gamma, coef0=coef0, out=out, handle=h), args.runs,
+                args.warmup, stream=st))
             comp = None
             if compose:
                 def composition():
                     pairwise_distance(x, y, out=out, metric=metric, handle=h)
                     transform(out, kernel, degree, gamma, coef0)
-                comp = timed(composition, h, args.runs, args.warmup)
+                comp = statistics.median(time_ms(composition, args.runs, args.warmup, stream=st))
             r = {"shape": label, "kernel": kernel, "fused_ms": round(fused, 3), "pairwise_ms": round(base_ms[metric], 3),
                  "ratio_to_pairwise": round(fused / base_ms[metric], 3),
                  "composition_ms": None if comp is None else round(comp, 3)}
@@ -102,10 +80,8 @@ def main():
     ap.add_argument("--warmup", type=int, default=2)
     ap.add_argument("--json", action="store_true")
     args = ap.parse_args()
-    if not torch.cuda.is_available():
-        raise SystemExit("gram_time.py needs a CUDA device")
-    name, q = card()
-    print("card: %s, power limit / max SM clock: %s" % (name, q))
+    c = card()
+    print("card: %s, power limit / max SM clock: %s W, %s MHz" % (c["name"], c["power_limit"], c["clocks_max_sm"]))
     print("| m x n x k | kernel | fused ms | pairwise ms | fused / pairwise | composition ms |")
     print("|---|---|---|---|---|---|")
     h = DeviceResources()

@@ -8,13 +8,13 @@ import argparse
 import ctypes
 import json
 import os
-import subprocess
+import statistics
 import sys
 
-import numpy as np
 import torch
 
 sys.path.insert(0, os.path.join(os.path.dirname(os.path.abspath(__file__)), ".."))
+from measure import card, time_ms  # noqa: E402
 from raft_b200.cluster import KMeansParams, fit as km_fit, predict as km_predict  # noqa: E402
 from raft_b200 import _lib  # noqa: E402
 from raft_b200.cluster import kmeans_balanced as kb  # noqa: E402
@@ -32,29 +32,6 @@ def stage_ms(fn, n_iters):
     ms = list(buf)[:cnt.value]
     assert cnt.value == 3 + n_iters, cnt.value
     return ms[0], ms[1], sum(ms[2:2 + n_iters]), ms[2 + n_iters]
-
-
-def card():
-    try:
-        out = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader", "-i", "0"],
-                             capture_output=True, text=True, timeout=30).stdout.strip()
-        name, power = [s.strip() for s in out.split(",")]
-        return name, power
-    except Exception:
-        return torch.cuda.get_device_name(0), "unknown"
-
-
-def timed(fn, reps):
-    ts = []
-    out = None
-    for _ in range(reps):
-        a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-        a.record()
-        out = fn()
-        b.record()
-        torch.cuda.synchronize()
-        ts.append(a.elapsed_time(b))
-    return float(np.median(ts)), out
 
 
 def blobs(m, k, centers, seed):
@@ -79,24 +56,26 @@ def main():
     ap.add_argument("--reps", type=int, default=3)
     ap.add_argument("--out")
     a = ap.parse_args()
-    name, power = card()
+    gpu = card()
     x = blobs(a.m, a.k, 2048, 0)
     lines = []
     for nc in a.clusters:
         p = kb.KMeansBalancedParams(n_iters=a.n_iters)
-        kb.fit_predict(p, x, nc)   # warm-up
-        ms, (c, lab, sizes) = timed(lambda: kb.fit_predict(p, x, nc), a.reps)
+        c, lab, sizes = kb.fit_predict(p, x, nc)   # the warm-up; every fit returns the same result
+        ms = statistics.median(time_ms(lambda: kb.fit_predict(p, x, nc), a.reps, warmup=0))
         c = torch.as_tensor(c, device="cuda")
         _, inertia = km_predict(KMeansParams(n_clusters=nc), x, c)
         lo, hi = spreads(torch.as_tensor(sizes, device="cuda"))
         s0, s1, s1_argmin, s2 = stage_ms(lambda: kb.fit_predict(p, x, nc), a.n_iters)
         rec = dict(what="kmeans_balanced.fit_predict", m=a.m, k=a.k, n_clusters=nc, n_iters=a.n_iters, ms=ms,
                    inertia=inertia, stage0_ms=s0, stage1_ms=s1,
-                   stage1_masked_argmin_ms=s1_argmin, stage2_ms=s2, min_over_avg=lo, max_over_avg=hi, gpu=name, power_limit=power)
+                   stage1_masked_argmin_ms=s1_argmin, stage2_ms=s2, min_over_avg=lo, max_over_avg=hi, gpu=gpu["name"],
+                   power_limit=gpu["power_limit"])
         if nc <= a.kmeans_max:
             iters = a.n_iters * 2 + max(a.n_iters // 10, 2)
             kp = KMeansParams(n_clusters=nc, max_iter=iters, tol=0.0, oversampling_factor=2.0)
-            kms, o = timed(lambda: km_fit(kp, x), 1)
+            o = km_fit(kp, x)   # the warm-up; seeded, so every fit returns the same result
+            kms = time_ms(lambda: km_fit(kp, x), 1, warmup=0)[0]
             klab, _ = km_predict(KMeansParams(n_clusters=nc), x, o.centroids)
             klo, khi = spreads(torch.bincount(torch.as_tensor(klab, device="cuda").long(), minlength=nc))
             rec.update(kmeans_ms=kms, kmeans_max_iter=iters, inertia_over_kmeans=inertia / o.inertia,

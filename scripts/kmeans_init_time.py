@@ -9,36 +9,21 @@ and, with --out, writes them to that file."""
 import argparse
 import json
 import os
-import subprocess
 import sys
+from statistics import median
 
-import numpy as np
 import torch
 
 sys.path.insert(0, os.path.join(os.path.dirname(os.path.abspath(__file__)), "..", "tests"))
 sys.path.insert(0, os.path.join(os.path.dirname(os.path.abspath(__file__)), ".."))
 import kmeans_ref  # noqa: E402
 import kmeans_scalable_ref  # noqa: E402
+from measure import card, time_ms  # noqa: E402
 from raft_b200 import _lib  # noqa: E402
 from raft_b200.cluster import (KMeansParams, cluster_cost, compute_new_centroids, fit, init_plus_plus,  # noqa: E402
                                init_scalable)
 from raft_b200.common import DeviceResources  # noqa: E402
 from raft_b200.distance import fused_l2_nn  # noqa: E402
-
-
-def timed(f, reps):
-    f()
-    torch.cuda.synchronize()
-    ts = []
-    r = None
-    for _ in range(reps):
-        a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-        a.record()
-        r = f()
-        b.record()
-        torch.cuda.synchronize()
-        ts.append(a.elapsed_time(b))
-    return float(np.median(ts)), r
 
 
 def select_k_1xm(keys, n, h):
@@ -62,9 +47,7 @@ def main():
     ap.add_argument("--reps", type=int, default=3)
     ap.add_argument("--out", default=None)
     a = ap.parse_args()
-    q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"],
-                       capture_output=True, text=True)
-    rows = [{"gpu": q.stdout.strip()}]
+    rows = [{"gpu": card()}]
     print(json.dumps(rows[0]), flush=True)
     x, _, _ = kmeans_ref.blobs(a.m, a.k, 64, seed=1, spread=0.3)
     xd = torch.from_numpy(x).cuda()
@@ -72,14 +55,16 @@ def main():
     for nc in [int(s) for s in a.ncs.split(",")]:
         L, C = kmeans_scalable_ref.sizes(a.m, nc, a.f)
         r = {"n_clusters": nc, "L": L, "C": C}
-        r["scalable_ms"], cs = timed(lambda: init_scalable(xd, n_clusters=nc, oversampling_factor=a.f, seed=0, handle=h),
-                                     a.reps)
+        # a call whose result is used is its own warm-up: the calls are seeded, so every call returns the same result
+        cs = init_scalable(xd, n_clusters=nc, oversampling_factor=a.f, seed=0, handle=h)
+        r["scalable_ms"] = median(time_ms(
+            lambda: init_scalable(xd, n_clusters=nc, oversampling_factor=a.f, seed=0, handle=h), a.reps, warmup=0))
         r["scalable_cost"] = cluster_cost(xd, cs, handle=h)
         # the split, through the public calls that run the same kernels
         keys = torch.rand(a.m, device="cuda")
         cand = xd[torch.randperm(a.m, device="cuda")[:C]].contiguous()
-        r["draw_ms"], _ = timed(lambda: select_k_1xm(keys, L, h), a.reps)
-        r["round_argmin_ms"], _ = timed(lambda: fused_l2_nn(xd, cand[:L], sqrt=False, handle=h), a.reps)
+        r["draw_ms"] = median(time_ms(lambda: select_k_1xm(keys, L, h), a.reps))
+        r["round_argmin_ms"] = median(time_ms(lambda: fused_l2_nn(xd, cand[:L], sqrt=False, handle=h), a.reps))
         r["rounds_ms_est"] = 9 * r["draw_ms"] + 8 * r["round_argmin_ms"]
 
         def weights_pass():
@@ -88,14 +73,18 @@ def main():
             wpc = torch.empty(C, dtype=torch.float32, device="cuda")
             compute_new_centroids(xd, cand, lab.to(torch.int32), new, weight_per_cluster=wpc, handle=h)
             return wpc
-        r["weights_pass_ms"], wpc = timed(weights_pass, a.reps)
+        wpc = weights_pass()
+        r["weights_pass_ms"] = median(time_ms(weights_pass, a.reps, warmup=0))
         rp = KMeansParams(n_clusters=nc, max_iter=300, tol=1e-4, seed=0)
-        r["recluster_ms"], _ = timed(lambda: fit(rp, cand, sample_weights=wpc, handle=h), a.reps)
-        r["recluster_greedy_ms"], _ = timed(lambda: init_plus_plus(cand, n_clusters=nc, seed=0, handle=h), a.reps)
+        r["recluster_ms"] = median(time_ms(lambda: fit(rp, cand, sample_weights=wpc, handle=h), a.reps))
+        r["recluster_greedy_ms"] = median(time_ms(lambda: init_plus_plus(cand, n_clusters=nc, seed=0, handle=h),
+                                                  a.reps))
         fs = fit(KMeansParams(n_clusters=nc, seed=0, oversampling_factor=a.f), xd, handle=h)
         r["scalable_fit_inertia"], r["scalable_fit_n_iter"] = fs.inertia, fs.n_iter
         if nc <= a.greedy_max:
-            r["greedy_ms"], cg = timed(lambda: init_plus_plus(xd, n_clusters=nc, seed=0, handle=h), a.reps)
+            cg = init_plus_plus(xd, n_clusters=nc, seed=0, handle=h)
+            r["greedy_ms"] = median(time_ms(lambda: init_plus_plus(xd, n_clusters=nc, seed=0, handle=h), a.reps,
+                                            warmup=0))
             r["greedy_cost"] = cluster_cost(xd, cg, handle=h)
             fg = fit(KMeansParams(n_clusters=nc, seed=0), xd, handle=h)
             r["greedy_fit_inertia"], r["greedy_fit_n_iter"] = fg.inertia, fg.n_iter

@@ -4,9 +4,8 @@ Array init, tol = 0, max_iter = 20.  Prints one JSON line per measurement, and w
 import argparse
 import json
 import os
-import subprocess
 import sys
-import time
+from statistics import median
 
 import numpy as np
 import torch
@@ -14,24 +13,11 @@ import torch
 sys.path.insert(0, os.path.join(os.path.dirname(os.path.abspath(__file__)), "..", "tests"))
 sys.path.insert(0, os.path.join(os.path.dirname(os.path.abspath(__file__)), ".."))
 import kmeans_ref  # noqa: E402
+from measure import card, time_ms  # noqa: E402
 from raft_b200 import _lib  # noqa: E402
 from raft_b200.cluster import KMeansParams, fit, init_plus_plus  # noqa: E402
 from raft_b200.common import DeviceResources  # noqa: E402
 from raft_b200.distance import fused_l2_nn  # noqa: E402
-
-
-def timed(f, reps):
-    f()
-    torch.cuda.synchronize()
-    ts = []
-    for _ in range(reps):
-        a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-        a.record()
-        r = f()
-        b.record()
-        torch.cuda.synchronize()
-        ts.append(a.elapsed_time(b))
-    return float(np.median(ts)), r
 
 
 def composition(x, x64, c0, iters, tol, h):
@@ -61,11 +47,7 @@ def main():
     ap.add_argument("--reps", type=int, default=3)
     ap.add_argument("--out", default=None)
     a = ap.parse_args()
-    if not torch.cuda.is_available():
-        raise SystemExit("kmeans_time.py needs a GPU")
-    q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"],
-                       capture_output=True, text=True).stdout.strip()
-    rows = [{"gpu": q}]
+    rows = [{"gpu": card()}]
     print(json.dumps(rows[0]), flush=True)
     h = DeviceResources()
     for nc in [int(v) for v in a.clusters.split(",")]:
@@ -78,11 +60,14 @@ def main():
             cf.copy_(c0)
             return fit(KMeansParams(n_clusters=nc, max_iter=max_iter, tol=tol, init_method="Array"), x, cf, handle=h)
 
-        t_fit, out = timed(run_fit, a.reps)
+        # a call whose result is used is its own warm-up
+        out = run_fit()
+        t_fit = median(time_ms(run_fit, a.reps, warmup=0))
         fused_c = cf.clone()
         _lib.check(_lib.lib().b2d_set_option(b"nn_screen", 0))
         x64 = x.double()
-        t_comp, comp_c = timed(lambda: composition(x, x64, c0, a.iters, 0.0, h), a.reps)
+        comp_c = composition(x, x64, c0, a.iters, 0.0, h)
+        t_comp = median(time_ms(lambda: composition(x, x64, c0, a.iters, 0.0, h), a.reps, warmup=0))
         del x64
         _lib.check(_lib.lib().b2d_set_option(b"nn_screen", 1))
         lab_f, _ = fused_l2_nn(x, fused_c, sqrt=False, handle=h)
@@ -90,9 +75,9 @@ def main():
         ia = fused_c.view(torch.int32).long()
         ib = comp_c.view(torch.int32).long()
         # default tol: the no-op iterations after convergence
-        _, conv = timed(lambda: run_fit(300, 1e-4), 1)
-        t300, _ = timed(lambda: run_fit(300, 1e-4), a.reps)
-        tn, _ = timed(lambda: run_fit(conv.n_iter, 1e-4), a.reps)
+        conv = run_fit(300, 1e-4)
+        t300 = median(time_ms(lambda: run_fit(300, 1e-4), a.reps, warmup=0))
+        tn = median(time_ms(lambda: run_fit(conv.n_iter, 1e-4), a.reps))
         byte_floor_ms = 8.0 * a.m * a.k / 3.35e12 * 1e3
         r = {"n_clusters": nc, "m": a.m, "k": a.k, "fit_ms_per_iter": t_fit / out.n_iter,
              "composition_ms_per_iter": t_comp / a.iters, "byte_floor_ms_per_iter": byte_floor_ms,
@@ -103,7 +88,7 @@ def main():
         print(json.dumps(r), flush=True)
     x_np, _, _ = kmeans_ref.blobs(a.m, a.k, 1024, seed=1, spread=0.3)
     x = torch.from_numpy(x_np).cuda()
-    t_pp, _ = timed(lambda: init_plus_plus(x, n_clusters=1024, seed=0, handle=h), 1)
+    t_pp = time_ms(lambda: init_plus_plus(x, n_clusters=1024, seed=0, handle=h), 1)[0]
     rows.append({"kmeans_plus_plus_ms": t_pp, "n_clusters": 1024, "m": a.m, "k": a.k})
     print(json.dumps(rows[-1]), flush=True)
     if a.out:

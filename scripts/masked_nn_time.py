@@ -4,9 +4,9 @@ Patterns (m = n = 262144, k = 64 by default; x sorted by group):
   cc      connect_components: 64 groups, adj[i, g] = colour(i) != g
   sparse  256 groups of 1024 rows; each 64-row slab of x is adjacent to 8 random groups
   worst   groups of 16 rows, adjacency random with p = 0.5: every tile is PARTIAL
-For each pattern: the share of live tiles (from the pattern), the median of --runs wall-clock times of each call (host
-clock around the call and a device synchronise, warm-up excluded), the card and its power limit.  Every run is checked
-against an fp64 re-evaluation of a sample of rows.  Prints one JSON line per pattern.
+For each pattern: the share of live tiles (from the pattern), the median of --runs times of each call (CUDA events
+around the call, after a warm-up call), the card and its power limit.  Every masked_l2_nn call, the warm-up included, is
+checked against an fp64 re-evaluation of a sample of rows.  Prints one JSON line per pattern.
 
   python scripts/masked_nn_time.py [--m 262144] [--n 262144] [--k 64] [--runs 5] [--patterns cc,sparse,worst]
 """
@@ -14,27 +14,15 @@ import argparse
 import json
 import os
 import statistics
-import subprocess
 import sys
-import time
 
-import numpy as np
 import torch
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
+from measure import card, time_ms  # noqa: E402
 from raft_b200 import _lib  # noqa: E402
 from raft_b200.common import DeviceResources  # noqa: E402
 from raft_b200.distance import fused_l2_nn, masked_l2_nn  # noqa: E402
-
-
-def card():
-    name = torch.cuda.get_device_name(0)
-    try:
-        q = subprocess.run(["nvidia-smi", "--id=0", "--query-gpu=power.limit", "--format=csv,noheader"],
-                           capture_output=True, text=True, timeout=30).stdout.strip()
-    except Exception:
-        q = "unknown"
-    return name, q
 
 
 def pattern(kind, m, n, dev, gen):
@@ -97,20 +85,6 @@ def check(xd, yd, adj, size, gi, gv, rows):
     return bad
 
 
-def timed(fn, runs):
-    fn()
-    torch.cuda.synchronize()
-    ts, outs = [], []
-    for _ in range(runs):
-        torch.cuda.synchronize()
-        t0 = time.perf_counter()
-        out = fn()
-        torch.cuda.synchronize()
-        ts.append((time.perf_counter() - t0) * 1e3)
-        outs.append(out)
-    return ts, outs
-
-
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--m", type=int, default=262144)
@@ -121,9 +95,8 @@ def main():
     a = ap.parse_args()
     if a.n % 1024 or a.m % 64:
         ap.error("--n must be a multiple of 1024 and --m of 64 (the patterns' group sizes and 64-row slabs)")
-    assert torch.cuda.is_available(), "needs a GPU"
     dev = torch.device("cuda:0")
-    name, plimit = card()
+    gpu = card(dev)
     gen = torch.Generator().manual_seed(7)
     torch.manual_seed(7)
     m, n, k = a.m, a.n, a.k
@@ -136,22 +109,23 @@ def main():
         adj, size = pattern(kind, m, n, dev, gen)
         gidx = torch.arange(size, n + 1, size, dtype=torch.int32, device=dev)
         share = live_share(adj, size, m, n)
-        t_mask, outs = timed(lambda: masked_l2_nn(xd, yd, adj, gidx, handle=h), a.runs)
-        torch.cuda.synchronize()
+        outs = []
+        t_mask = time_ms(lambda: outs.append(masked_l2_nn(xd, yd, adj, gidx, handle=h)), a.runs)
         bad = sum(check(xd, yd, adj, size, gi, gv, rows) for gi, gv in outs)
         _lib.check(L.b2d_set_option(b"nn_screen", 0.0))
         try:
-            t_exact, _ = timed(lambda: fused_l2_nn(xd, yd, sqrt=False, handle=h), a.runs)
+            t_exact = time_ms(lambda: fused_l2_nn(xd, yd, sqrt=False, handle=h), a.runs)
         finally:
             _lib.check(L.b2d_set_option(b"nn_screen", 1.0))
-        t_default, _ = timed(lambda: fused_l2_nn(xd, yd, sqrt=False, handle=h), a.runs)
+        t_default = time_ms(lambda: fused_l2_nn(xd, yd, sqrt=False, handle=h), a.runs)
         med = statistics.median
         print(json.dumps({"pattern": kind, "m": m, "n": n, "k": k, "groups": int(adj.shape[1]), "live_tile_share": round(share, 4),
                           "masked_ms": round(med(t_mask), 3), "exact_fused_ms": round(med(t_exact), 3),
                           "default_fused_ms": round(med(t_default), 3),
                           "masked_over_exact": round(med(t_mask) / med(t_exact), 3),
                           "runs": a.runs, "masked_ms_all": [round(t, 3) for t in t_mask],
-                          "sample_mismatches": bad, "card": name, "power_limit": plimit}), flush=True)
+                          "sample_mismatches": bad, "card": gpu["name"], "power_limit": gpu["power_limit"]}),
+              flush=True)
         del adj
         torch.cuda.empty_cache()
         if bad:

@@ -22,13 +22,13 @@ import argparse
 import json
 import os
 import statistics
-import subprocess
 import sys
 
 import torch
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import oracle  # noqa: E402
+from measure import card, time_ms  # noqa: E402
 from raft_b200 import _lib  # noqa: E402
 from raft_b200.common import DeviceResources  # noqa: E402
 from raft_b200.distance import pairwise_distance  # noqa: E402
@@ -37,27 +37,6 @@ from raft_b200.neighbors import eps_neighbors_l2sq, radius_neighbors  # noqa: E4
 WORKLOADS = [(100000, 100000, 128), (200000, 1000000, 32)]
 NEIGHBOURS = [100, 1000]
 SLAB_BYTES = 4 << 30   # dense slab of the compositions
-
-
-def card():
-    name = torch.cuda.get_device_name(0)
-    q = subprocess.run(["nvidia-smi", "--id=0", "--query-gpu=power.limit,clocks.max.sm", "--format=csv,noheader"],
-                       capture_output=True, text=True, timeout=30).stdout.strip()
-    return name, q
-
-
-def timed(fn, runs):
-    fn()
-    torch.cuda.synchronize()
-    ts = []
-    for _ in range(runs):
-        a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-        a.record()
-        fn()
-        b.record()
-        b.synchronize()
-        ts.append(a.elapsed_time(b))
-    return statistics.median(ts), ts
 
 
 def packed_key(d, j):
@@ -81,9 +60,9 @@ def main():
     ap.add_argument("--runs", type=int, default=3)
     ap.add_argument("--only", default="")
     a = ap.parse_args()
-    assert torch.cuda.is_available(), "needs a GPU"
-    name, pl = card()
-    print("card: %s, power limit, max SM clock: %s" % (name, pl), flush=True)
+    gpu = card()
+    pl = "%s W, %s MHz" % (gpu["power_limit"], gpu["clocks_max_sm"])
+    print("card: %s, power limit, max SM clock: %s" % (gpu["name"], pl), flush=True)
     h = DeviceResources()
     L = _lib.lib()
     sel = [int(s) for s in a.only.split(",") if s] or range(len(WORKLOADS))
@@ -162,8 +141,8 @@ def main():
             res = {}
             for arm, fn in (("fused_total", fused), ("count_call", count), ("fill_call", fill),
                             ("pairwise_composition", comp_pairwise), ("eps_composition", comp_eps)):
-                med, ts = timed(lambda: (fn(), h.sync()), a.runs)
-                res[arm] = {"median_ms": round(med, 3), "ms": [round(t, 3) for t in ts]}
+                ts = time_ms(lambda: (fn(), h.sync()), a.runs)
+                res[arm] = {"median_ms": round(statistics.median(ts), 3), "ms": [round(t, 3) for t in ts]}
             kern = {}
             for arm, fn in (("count_kernel", count), ("fill_kernel", fill)):
                 vals = []
@@ -178,7 +157,7 @@ def main():
             res.update(kern)
             res["fill_prep_sort_split_ms"] = round(res["fill_call"]["median_ms"] - kern["fill_kernel"], 3)
             print(json.dumps({"m": m, "n": n, "k": k, "radius": r, "neighbours_per_row": round(nnz / m, 1), "nnz": nnz,
-                              "card": name, "power_limit_max_sm_clock": pl, **res}), flush=True)
+                              "card": gpu["name"], "power_limit_max_sm_clock": pl, **res}), flush=True)
             del ws
         del q, x, dist, adj, vd
         torch.cuda.empty_cache()

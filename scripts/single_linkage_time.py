@@ -4,8 +4,8 @@ brute_force.knn, the graph copied to the host, scipy.sparse.csgraph.minimum_span
 Stages come from one torch.profiler run of the call, cut at marker kernels in stream order: kNN (up to
 sl_knn_edges_kernel), Borůvka (the rounds before the first connect), each connect round (sl_root_flags_kernel up to the
 round's last Borůvka kernel, including its host synchronisation), and the dendrogram (the radix sort to the end of the
-call: device sort and gather, copies, union-find on the host).  The total is a host clock around the call (which
-synchronises), without the profiler, median of --reps.
+call: device sort and gather, copies, union-find on the host).  The total is CUDA events around the call (which
+synchronises before it returns) after a warm-up, without the profiler, median of --reps.
 
 Inputs: blobs with overlapping centres (a connected kNN graph: the baseline's MST is then the same spanning tree) and
 blobs with separated centres (several kNN components: connect_components runs), at 100000 x 128 and 1000000 x 32, c = 15.
@@ -13,7 +13,7 @@ Prints one JSON line per measurement, and writes them to --out."""
 import argparse
 import json
 import os
-import subprocess
+import statistics
 import sys
 import time
 
@@ -21,6 +21,7 @@ import numpy as np
 import torch
 
 sys.path.insert(0, os.path.join(os.path.dirname(os.path.abspath(__file__)), ".."))
+from measure import card, time_ms  # noqa: E402
 from raft_b200.cluster import single_linkage  # noqa: E402
 from raft_b200.neighbors import brute_force  # noqa: E402
 
@@ -53,17 +54,6 @@ def stages(x, c):
     res["dendrogram_ms"] = (t_end - kern[i_sort].time_range.start) / 1e3
     res["n_connected_components"] = out.n_connected_components
     return res
-
-
-def total_ms(x, c, reps):
-    single_linkage(x, 10, c=c)
-    ts = []
-    for _ in range(reps):
-        torch.cuda.synchronize()
-        t = time.perf_counter()
-        single_linkage(x, 10, c=c)
-        ts.append((time.perf_counter() - t) * 1e3)
-    return float(np.median(ts))
 
 
 def baseline(x, c):
@@ -108,20 +98,19 @@ def main():
     ap.add_argument("--no-baseline", action="store_true")
     ap.add_argument("--out", default=None)
     a = ap.parse_args()
-    assert torch.cuda.is_available(), "needs a GPU"
-    card = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"], capture_output=True,
-                          text=True).stdout.strip()
+    gpu = card()
     rows = []
     for shape in a.shapes.split(","):
         m, d = map(int, shape.split("x"))
         for kind, sep in (("overlapping", 1.0), ("separated", 200.0)):
             x = blobs(m, d, 10, sep, seed=m + d)
-            r = {"shape": shape, "input": kind, "c": a.c, "card": card, "total_ms": total_ms(x, a.c, a.reps)}
+            r = {"shape": shape, "input": kind, "c": a.c, "card": gpu,
+                 "total_ms": statistics.median(time_ms(lambda: single_linkage(x, 10, c=a.c), a.reps))}
             r.update(stages(x, a.c))
             rows.append(r)
             print(json.dumps(r), flush=True)
             if kind == "overlapping" and not a.no_baseline:
-                b = {"shape": shape, "input": kind, "c": a.c, "card": card, "what": "baseline knn+scipy"}
+                b = {"shape": shape, "input": kind, "c": a.c, "card": gpu, "what": "baseline knn+scipy"}
                 b.update(baseline(x, a.c))
                 rows.append(b)
                 print(json.dumps(b), flush=True)

@@ -31,10 +31,9 @@ import sys
 import tempfile
 
 HERE = os.path.dirname(os.path.abspath(__file__))
-sys.path.insert(0, HERE)
 sys.path.insert(0, os.path.dirname(HERE))
 
-from tc_breakdown import SmClocks, smi  # noqa: E402
+from measure import SmClocks, card, summary, time_ms  # noqa: E402
 from raft_b200 import _build  # noqa: E402
 
 M, N = 100_000, 100_000
@@ -107,34 +106,22 @@ def main():
             raise RuntimeError(f"{v[0]}: {bad} sampled entries wrong")
     torch.cuda.synchronize()
 
-    names = [v[0] for v in vs] + ["fill_", "st.global.v4 sweep"]
-    times = {nm: [] for nm in names}
-    ev0, ev1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-
-    def timed(fn):
-        fn()   # one warm-up after the previous variant
-        ev0.record()
-        for _ in range(args.steps):
-            fn()
-        ev1.record()
-        ev1.synchronize()
-        return ev0.elapsed_time(ev1) / args.steps
-
-    card = smi("name,power.limit,clocks.max.sm")
-    with SmClocks() as clk:
+    arms = [(v[0], lambda v=v: launch(v)) for v in vs] + [
+        ("fill_", lambda: d.fill_(1.0)),
+        ("st.global.v4 sweep", lambda: L.probe_launch(d.data_ptr(), M, N, N, 0, 0, 0, 0, 0, stream))]
+    times = {nm: [] for nm, _ in arms}
+    gpu = card(dev)
+    with SmClocks(gpu["uuid"]) as clk:
         for _ in range(args.runs):
-            for v in vs:
-                times[v[0]].append(timed(lambda: launch(v)))
-            times["fill_"].append(timed(lambda: d.fill_(1.0)))
-            times["st.global.v4 sweep"].append(timed(lambda: L.probe_launch(d.data_ptr(), M, N, N, 0, 0, 0, 0, 0, stream)))
+            for nm, fn in arms:
+                fn()   # one warm-up launch after the previous arm: after a whole warm-up pass, the idle arms ran slower
+                times[nm].append(time_ms(lambda: [fn() for _ in range(args.steps)], 1, warmup=0)[0] / args.steps)
     gb = M * N * 4 / 1e9
     res = {"shape": f"{M}x{N} fp32 ({gb:.0f} GB)", "runs": args.runs, "steps_per_run": args.steps,
-           "card": card[0] if card else None, "power_limit_w": card[1] if card else None,
-           "clocks_max_sm_mhz": card[2] if card else None,
+           "card": gpu["name"], "power_limit_w": gpu["power_limit"], "clocks_max_sm_mhz": gpu["clocks_max_sm"],
            "clocks_sm_mhz": {"min": min(clk.samples), "median": statistics.median(clk.samples),
                              "max": max(clk.samples)} if clk.samples else None,
-           "ms": {nm: {"median": round(statistics.median(t), 3), "min": round(min(t), 3), "max": round(max(t), 3),
-                       "tb_s": round(gb / statistics.median(t), 3)} for nm, t in times.items()}}
+           "ms": {nm: {**summary(t), "tb_s": round(gb / statistics.median(t), 3)} for nm, t in times.items()}}
     line = json.dumps(res)
     print(line)
     if args.out:

@@ -28,11 +28,11 @@ import statistics
 import subprocess
 import sys
 import tempfile
-import threading
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 
+from measure import SmClocks, card, summary  # noqa: E402
 from raft_b200 import _build  # noqa: E402
 
 M, N, K = 100_000, 100_000, 128
@@ -84,33 +84,6 @@ def check(L, rc):
         raise RuntimeError(L.b2d_last_error().decode("utf-8", "replace"))
 
 
-def smi(query):
-    res = subprocess.run(["nvidia-smi", "-i", "0", f"--query-gpu={query}", "--format=csv,noheader,nounits"],
-                         capture_output=True, text=True)
-    return [v.strip() for v in res.stdout.strip().split(",")] if res.returncode == 0 else None
-
-
-class SmClocks:
-    """SM clock samples (MHz) while the timed rounds run (read-only nvidia-smi queries)."""
-
-    def __init__(self):
-        self.samples, self._stop = [], threading.Event()
-
-    def __enter__(self):
-        def loop():
-            while not self._stop.wait(0.2):
-                v = smi("clocks.sm")
-                if v and v[0].isdigit():
-                    self.samples.append(int(v[0]))
-        self._t = threading.Thread(target=loop, daemon=True)
-        self._t.start()
-        return self
-
-    def __exit__(self, *a):
-        self._stop.set()
-        self._t.join()
-
-
 def main():
     ap = argparse.ArgumentParser(description=__doc__, formatter_class=argparse.RawDescriptionHelpFormatter)
     ap.add_argument("--lib-dir", default=None)
@@ -149,9 +122,9 @@ def main():
         call(L)
         call(L)
     torch.cuda.synchronize()
-    card = smi("name,power.limit,clocks.max.sm")
+    gpu = card(dev)
     times = {name: [] for name, _ in libs}
-    with SmClocks() as clk:
+    with SmClocks(gpu["uuid"]) as clk:
         for _ in range(args.runs):
             for name, L in libs:
                 call(L)   # one warm-up call after the previous variant
@@ -164,12 +137,10 @@ def main():
                 times[name].append(sum(buf[i] for i in range(cnt.value)) / max(1, cnt.value))
     res = {"kernel": "expanded_tc_kernel<resident, EPI_STORE, POST_CLAMP>",
            "shape": f"L2Expanded {M}x{N}x{K} fp32", "runs": args.runs, "steps_per_run": args.steps,
-           "card": card[0] if card else None, "power_limit_w": card[1] if card else None,
-           "clocks_max_sm_mhz": card[2] if card else None,
+           "card": gpu["name"], "power_limit_w": gpu["power_limit"], "clocks_max_sm_mhz": gpu["clocks_max_sm"],
            "clocks_sm_mhz": {"min": min(clk.samples), "median": statistics.median(clk.samples),
                              "max": max(clk.samples)} if clk.samples else None,
-           "kernel_ms": {name: {"median": statistics.median(v), "min": min(v), "max": max(v), "runs": v}
-                         for name, v in times.items()}}
+           "kernel_ms": {name: summary(v) for name, v in times.items()}}
     line = json.dumps(res)
     print(line)
     if args.out:
