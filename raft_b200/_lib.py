@@ -24,13 +24,15 @@ SYMBOLS = [
     "b2d_mst_workspace_bytes", "b2d_mst",
     "b2d_single_linkage_workspace_bytes", "b2d_single_linkage", "b2d_dbscan_workspace_bytes", "b2d_dbscan_fit",
     "b2d_debug_pairwise_plan", "b2d_radius_neighbors_workspace_bytes", "b2d_radius_neighbors_count",
-    "b2d_radius_neighbors_fill",
+    "b2d_radius_neighbors_fill", "b2d_kde_workspace_bytes", "b2d_kde_score_samples",
 ]
 
 B2D_OK, B2D_ERR_INVALID_ARG, B2D_ERR_CUDA, B2D_ERR_UNSUPPORTED, B2D_ERR_WORKSPACE = range(5)
 B2D_F32, B2D_F16, B2D_F64 = 0, 1, 2
 B2D_KERNEL_LINEAR, B2D_KERNEL_POLYNOMIAL, B2D_KERNEL_RBF, B2D_KERNEL_TANH = range(4)
 B2D_KMEANS_INIT_PLUS_PLUS, B2D_KMEANS_INIT_RANDOM, B2D_KMEANS_INIT_ARRAY = range(3)
+(B2D_KDE_GAUSSIAN, B2D_KDE_TOPHAT, B2D_KDE_EPANECHNIKOV, B2D_KDE_EXPONENTIAL, B2D_KDE_LINEAR,
+ B2D_KDE_COSINE) = range(6)
 
 
 class RaftB200Error(RuntimeError):
@@ -156,6 +158,10 @@ def lib() -> ctypes.CDLL:
     L.b2d_radius_neighbors_count.argtypes = [vp, vp, ci, vp, i64, vp, i64, i64, i64, i64, cf, vp, sz]
     L.b2d_radius_neighbors_fill.restype = ci
     L.b2d_radius_neighbors_fill.argtypes = [vp, vp, i64, vp, vp, ci, vp, i64, vp, i64, i64, i64, i64, cf, vp, sz]
+    L.b2d_kde_workspace_bytes.restype = sz
+    L.b2d_kde_workspace_bytes.argtypes = [i64, i64, i64, i64]
+    L.b2d_kde_score_samples.restype = ci
+    L.b2d_kde_score_samples.argtypes = [vp, ci, cd, vp, i64, vp, vp, i64, i64, i64, i64, i64, vp, vp, sz]
     L.b2d_row_norm.restype = ci
     L.b2d_row_norm.argtypes = [vp, vp, vp, i64, i64, i64, ci, ci]
     _lib = L

@@ -55,6 +55,9 @@
 //   EPI_RADIUS        radius neighbours: the EPI_STORE distance of kPost, compared with eps as a 32-bit hit mask per
 //                     row and half tile in registers; count mode adds the row's hits to its degree, fill mode appends
 //                     them as packed keys to the row's CSR segment (radius_row32).
+//   EPI_KDE           kernel density: the EPI_STORE / POST_CLAMP distance, reduced per row and 128-column half to one
+//                     (max, sum) pair of a log-sum-exp or one plain sum of weighted kernel values (kde_row32), written to
+//                     the partials that kde.cuh folds.
 //
 // Diagnostic builds (DESIGN.md section 5, scripts/tc_breakdown.py; never the library's own build): B2D_TC_DIAG = 1 keeps
 // the MMAs only (no epilogue, no staging; one sum of the accumulators keeps them live), 2 computes and stages every value
@@ -201,6 +204,90 @@ __device__ __noinline__ void radius_row32(unsigned* cnt, long long* out, const l
   }
 }
 
+// EPI_KDE, one row of a 64 x 128 warpgroup tile: d0..d31 are the thread's squared distances of the row (d[2 i + e] at
+// column 8 i + e of cw, the row's column weights in shared memory from the thread's first column).  The thread reduces
+// its 32 columns (TcParams::kde_*: gaussian / exponential to a base-2 log-sum-exp (M, S), the compact kernels to M = 0 and
+// the sum of w K over d^2 < h2), the quad's 4 lanes combine theirs, and lane 0 of the quad writes the row's pair to *out
+// unless out is null (a row outside the matrix).  A NaN distance makes S NaN: fmaxf leaves it out of M, the exp2 or the
+// product takes it into S, and max.NaN keeps it through the clamp of K at 0.  The whole warp calls (the quad shuffles).
+// Kernel ids as B2D_KDE_* (include/raft_b200.h).  Not inlined, for the reason given at knn_append16.
+__device__ __noinline__ void kde_row32(float2* out, int kern, float s, float h2, const float* cw, float d0, float d1,
+                                       float d2, float d3, float d4, float d5, float d6, float d7, float d8, float d9,
+                                       float d10, float d11, float d12, float d13, float d14, float d15, float d16, float d17,
+                                       float d18, float d19, float d20, float d21, float d22, float d23, float d24, float d25,
+                                       float d26, float d27, float d28, float d29, float d30, float d31)
+{
+  float u[32] = {d0,  d1,  d2,  d3,  d4,  d5,  d6,  d7,  d8,  d9,  d10, d11, d12, d13, d14, d15,
+                 d16, d17, d18, d19, d20, d21, d22, d23, d24, d25, d26, d27, d28, d29, d30, d31};
+  float c[32];
+#pragma unroll
+  for (int i = 0; i < 16; ++i) {
+    const float2 w = *reinterpret_cast<const float2*>(&cw[8 * i]);
+    c[2 * i]     = w.x;
+    c[2 * i + 1] = w.y;
+  }
+  float mx = 0.f;
+  const bool lse = kern == 0 || kern == 3;   // B2D_KDE_GAUSSIAN, B2D_KDE_EXPONENTIAL
+  if (lse) {
+    if (kern == 0) {
+#pragma unroll
+      for (int t = 0; t < 32; ++t) u[t] = fmaf(-u[t], s, c[t]);
+    } else {
+#pragma unroll
+      for (int t = 0; t < 32; ++t) {
+        float r;
+        asm("sqrt.approx.f32 %0, %1;" : "=f"(r) : "f"(u[t]));
+        u[t] = fmaf(-r, s, c[t]);
+      }
+    }
+    mx = u[0];
+#pragma unroll
+    for (int t = 1; t < 32; ++t) mx = fmaxf(mx, u[t]);
+    const float ref = mx == __int_as_float(0xff800000) ? 0.f : mx;
+#pragma unroll
+    for (int t = 0; t < 32; ++t) u[t] = exp2f(u[t] - ref);
+  } else {
+#pragma unroll
+    for (int t = 0; t < 32; ++t) {
+      const float d = u[t];
+      float k;
+      if (kern == 1 || kern == 2) {   // tophat (s = 0), epanechnikov (s = -1 / h^2)
+        k = fmaf(d, s, 1.f);
+      } else {
+        float r;
+        asm("sqrt.approx.f32 %0, %1;" : "=f"(r) : "f"(d));
+        k = kern == 4 ? fmaf(r, s, 1.f) : __cosf(r * s);   // linear (s = -1 / h), cosine (s = pi / 2h)
+      }
+      u[t] = d >= h2 ? 0.f : clamp0(k) * c[t];
+    }
+  }
+  // the thread's sum as a balanced tree (5 roundings deep)
+#pragma unroll
+  for (int w = 16; w >= 1; w >>= 1)
+#pragma unroll
+    for (int t = 0; t < w; ++t) u[t] += u[t + w];
+  float sum = u[0];
+  if (lse) {
+#pragma unroll
+    for (int o = 1; o <= 2; o <<= 1) {
+      const float mo = __shfl_xor_sync(0xffffffffu, mx, o), so = __shfl_xor_sync(0xffffffffu, sum, o);
+      const float mn = fmaxf(mx, mo);
+      const float ref = mn == __int_as_float(0xff800000) ? 0.f : mn;
+      // (the lane order of the two terms is the same on both lanes, so they hold the same bits afterwards)
+      const bool lo = (threadIdx.x & o) == 0u;
+      sum = lo ? sum * exp2f(mx - ref) + so * exp2f(mo - ref) : so * exp2f(mo - ref) + sum * exp2f(mx - ref);
+      mx  = mn;
+    }
+  } else {
+    const bool lo1 = (threadIdx.x & 1u) == 0u, lo2 = (threadIdx.x & 2u) == 0u;
+    float so = __shfl_xor_sync(0xffffffffu, sum, 1);
+    sum      = lo1 ? sum + so : so + sum;
+    so       = __shfl_xor_sync(0xffffffffu, sum, 2);
+    sum      = lo2 ? sum + so : so + sum;
+  }
+  if ((threadIdx.x & 3u) == 0u && out != nullptr) *out = make_float2(mx, sum);
+}
+
 // The finished distance of a clamping post (tc_post_clamps) in the fragment layout of tc_epilogue: clamped at 0, 0 where
 // row i of x is row i - diag_off of y, then the sqrt of POST_CLAMP_SQRT.  kGuardN: only columns below n are zeroed.  EPI_EPS
 // needs that, since it counts every column of a row window; EPI_STORE and EPI_RADIUS set diag_off = 0 only with m == n, so
@@ -237,7 +324,8 @@ __device__ __forceinline__ void tc_finish(float (&v)[64], const TcParams& p, int
 template <int kEpi, int kPost>
 __device__ __forceinline__ void tc_epilogue(float (&v)[64], const TcParams& p, const float* col_tb, int cl0, int64_t gc0,
                                             int64_t row0, const float (&ta)[2], const float (&cfr)[2], float (&thr)[2],
-                                            const float (&xnr)[2], bool ynu, unsigned long long keep = ~0ull)
+                                            const float (&xnr)[2], bool ynu, unsigned long long keep = ~0ull,
+                                            const float* col_w = nullptr)
 {
   // d = acc * c_row (* column factor) + (t_x + t_y); the arg-min modes leave the row-constant t_x out (added on the
   // slow path only)
@@ -257,7 +345,7 @@ __device__ __forceinline__ void tc_epilogue(float (&v)[64], const TcParams& p, c
       if (kEpi == EPI_STORE && tc_post_ratio(kPost)) {
         v[4 * i + 2 * j]     = post_ratio<kPost>(a0 * cfr[j], ta[j] + tb.x);
         v[4 * i + 2 * j + 1] = post_ratio<kPost>(a1 * cfr[j], ta[j] + tb.y);
-      } else if (kEpi == EPI_STORE || kEpi == EPI_EPS || kEpi == EPI_RADIUS) {
+      } else if (kEpi == EPI_STORE || kEpi == EPI_EPS || kEpi == EPI_RADIUS || kEpi == EPI_KDE) {
         v[4 * i + 2 * j]     = fmaf(a0, cfr[j], ta[j] + tb.x);
         v[4 * i + 2 * j + 1] = fmaf(a1, cfr[j], ta[j] + tb.y);
       } else {
@@ -290,6 +378,23 @@ __device__ __forceinline__ void tc_epilogue(float (&v)[64], const TcParams& p, c
                      v[28 + 2 * j], v[29 + 2 * j], v[32 + 2 * j], v[33 + 2 * j], v[36 + 2 * j], v[37 + 2 * j],
                      v[40 + 2 * j], v[41 + 2 * j], v[44 + 2 * j], v[45 + 2 * j], v[48 + 2 * j], v[49 + 2 * j],
                      v[52 + 2 * j], v[53 + 2 * j], v[56 + 2 * j], v[57 + 2 * j], v[60 + 2 * j], v[61 + 2 * j]);
+    }
+    return;
+  }
+  if constexpr (kEpi == EPI_KDE) {
+    // the EPI_STORE / POST_CLAMP values of acc_mode 0, then one partial per row and half tile.  Columns beyond n have t_y = 0
+    // and weight kde_pad, so they add nothing; rows beyond m write nothing.
+    tc_finish<POST_CLAMP, false>(v, p, row0, gc0);
+    const int64_t g = gc0 / TC_HN;   // the launch's 128-column half
+#pragma unroll
+    for (int j = 0; j < 2; ++j) {
+      const int64_t r = row0 + 8 * j;
+      kde_row32(r < p.m ? p.kde_part + g * p.kde_ld + r : nullptr, p.kde_kernel, p.kde_s, p.kde_h2, col_w + cl0, v[2 * j],
+                v[2 * j + 1], v[4 + 2 * j], v[5 + 2 * j], v[8 + 2 * j], v[9 + 2 * j], v[12 + 2 * j], v[13 + 2 * j],
+                v[16 + 2 * j], v[17 + 2 * j], v[20 + 2 * j], v[21 + 2 * j], v[24 + 2 * j], v[25 + 2 * j], v[28 + 2 * j],
+                v[29 + 2 * j], v[32 + 2 * j], v[33 + 2 * j], v[36 + 2 * j], v[37 + 2 * j], v[40 + 2 * j], v[41 + 2 * j],
+                v[44 + 2 * j], v[45 + 2 * j], v[48 + 2 * j], v[49 + 2 * j], v[52 + 2 * j], v[53 + 2 * j], v[56 + 2 * j],
+                v[57 + 2 * j], v[60 + 2 * j], v[61 + 2 * j]);
     }
     return;
   }
@@ -748,12 +853,13 @@ expanded_tc_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_cons
     {
       const int64_t gj = static_cast<int64_t>(n_blk) * TC_BN + ct;
       // +inf: never the arg-min; NaN: never within eps
-      float tv = (kEpi == EPI_EPS || kEpi == EPI_RADIUS) ? __int_as_float(0x7fffffff)
-               : kEpi != EPI_STORE                     ? __int_as_float(0x7f800000) : 0.f;
+      float tv = (kEpi == EPI_EPS || kEpi == EPI_RADIUS)  ? __int_as_float(0x7fffffff)
+               : kEpi != EPI_STORE && kEpi != EPI_KDE     ? __int_as_float(0x7f800000) : 0.f;
       if (gj < p.n) tv = __ldg(&p.yt[gj]);
       if (kEpi == EPI_STORE && p.acc_mode >= 2) tv = 0.f;  // the t terms entered with the first K chunk
       col_tb[ct] = tv;
       if (kMasked) col_grp[ct] = gj < p.n ? __ldg(&p.mask_grp[gj]) : -1;
+      if (kEpi == EPI_KDE) reinterpret_cast<float*>(col_grp)[ct] = gj < p.n ? __ldg(&p.kde_colw[gj]) : p.kde_pad;
     }
     ptx::bar_sync(1, 256);
 
@@ -916,7 +1022,7 @@ expanded_tc_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_cons
           tc_epilogue_store_fast<kPost>(acc, p, col_tb, cl0, ta, cfr);
         else
           tc_epilogue<kEpi, kPost>(acc, p, col_tb, cl0, static_cast<int64_t>(n_blk) * TC_BN + cl0, row0, ta, cfr, thr, xnr,
-                                   ynu, keep);
+                                   ynu, keep, reinterpret_cast<const float*>(col_grp));
         if (kEpi == EPI_STORE && p.tma_store)   // (this warpgroup's staging boxes: computed here, not kept live)
           tc_stage_store(acc, &tmap_d, &tmap_dt,
                          ptx::smem_u32(smem + Carve::stg_off) + wg * TC_STG_BOXES * TC_D_BOX_BYTES, lead,

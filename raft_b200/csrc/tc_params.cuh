@@ -30,7 +30,8 @@ constexpr int TC_D_BOX_ROWS   = 32;
 constexpr int TC_D_BOX_BYTES  = TC_D_BOX_COLS * TC_D_BOX_ROWS * 4;
 constexpr int TC_STG_BOXES    = 2;
 
-enum TcEpilogue : int { EPI_STORE = 0, EPI_MINLOC = 1, EPI_TOPK = 2, EPI_MINLOC_MASKED = 3, EPI_EPS = 4, EPI_RADIUS = 5 };
+enum TcEpilogue : int { EPI_STORE = 0, EPI_MINLOC = 1, EPI_TOPK = 2, EPI_MINLOC_MASKED = 3, EPI_EPS = 4, EPI_RADIUS = 5,
+                         EPI_KDE = 6 };
 constexpr int64_t TC_NO_DIAG = INT64_MIN;   // TcParams::diag_off: y is not a row window of x
 
 // EPI_MINLOC_MASKED (masked_nn.cuh): class of one (64-row slab of x, 128-column half of a y block) tile.  Byte
@@ -131,6 +132,18 @@ struct TcParams {
   const long long* rad_indptr;   // [m + 1] (fill mode)
   long long rad_nnz;
   int rad_fill;                  // 0: count, 1: fill
+  // EPI_KDE (kernel_density, kde.cu): per row i and 128-column half g of the launch, kde_part[g * kde_ld + i] = (M, S)
+  // over the half's columns j < n, with d the EPI_STORE / POST_CLAMP distance (diag_off as there) and c_j = kde_colw[j]:
+  //   gaussian, exponential (log-sum-exp, base 2): u_j = c_j - s d^2 resp. c_j - s sqrt(d^2), c_j = log2 w_j; M = max u_j,
+  //     S = sum 2^(u_j - M) (M = -inf: S = sum 2^u_j)
+  //   tophat, epanechnikov, linear, cosine (the pairs with d^2 < kde_h2 only): M = 0, S = sum c_j K_j, c_j = w_j
+  int kde_kernel;                // B2D_KDE_*
+  float kde_s;                   // the kernel's fp32 scale factor (kde_row32)
+  float kde_h2;                  // fp32(h^2): the support d^2 < kde_h2 of the compact kernels
+  float kde_pad;                 // c_j of the columns at or past n: -inf (log-sum-exp) or 0
+  const float* kde_colw;         // [n]
+  float2* kde_part;              // [halves][kde_ld]
+  int64_t kde_ld;
 };
 
 constexpr size_t TC_SMEM_OPERANDS = (size_t)TC_MAX_RES_KB * TC_B_BYTES + (size_t)TC_STAGES_RES * TC_A_BYTES;  // 208 KB
@@ -145,7 +158,8 @@ static_assert((size_t)TC_STAGES_STR * (TC_A_BYTES + TC_BH_BYTES) <= TC_SMEM_OPER
 // mbarriers (after t_y): afull[rings * TC_MAX_STAGES], aempty[rings * TC_MAX_STAGES] (slot s of ring w at rings * s + w),
 // bfull[TC_MAX_RES_KB], bempty[TC_MAX_RES_KB].
 // EPI_EPS has the carve of EPI_STORE (its adjacency boxes are the same 8 KB) plus the [256] column counts in the slot of the
-// masked kernel's groups.  EPI_RADIUS stores nothing through shared memory: the carve of the arg-min epilogues.
+// masked kernel's groups.  EPI_RADIUS stores nothing through shared memory: the carve of the arg-min epilogues.  EPI_KDE:
+// the carve of the arg-min epilogues plus the [256] column weights of the y block in that slot.
 template <bool kResident, int kEpi>
 struct TcCarve {
   static constexpr bool staged = kEpi == EPI_STORE || kEpi == EPI_EPS;
@@ -156,8 +170,9 @@ struct TcCarve {
   static constexpr size_t a_off   = kResident ? (size_t)TC_MAX_RES_KB * TC_B_BYTES : 0;
   static constexpr size_t stg_off = a_off + (size_t)stages * stage_bytes;
   static constexpr size_t tb_off  = staged ? stg_off + 2 * (size_t)TC_STG_BOXES * TC_D_BOX_BYTES : TC_SMEM_OPERANDS;
-  static constexpr size_t grp_off = tb_off + TC_BN * 4 + 256;   // EPI_MINLOC_MASKED: [256] group, EPI_EPS: count of every column
-  static constexpr size_t bytes   = grp_off + (kEpi == EPI_MINLOC_MASKED || kEpi == EPI_EPS ? TC_BN * 4 : 0);
+  static constexpr size_t grp_off = tb_off + TC_BN * 4 + 256;   // EPI_MINLOC_MASKED: [256] group, EPI_EPS: count of every column,
+                                                                // EPI_KDE: weight of every column
+  static constexpr size_t bytes   = grp_off + (kEpi == EPI_MINLOC_MASKED || kEpi == EPI_EPS || kEpi == EPI_KDE ? TC_BN * 4 : 0);
   static_assert(stages <= TC_MAX_STAGES, "barrier arrays hold TC_MAX_STAGES stages");
   static_assert((2 * rings * TC_MAX_STAGES + 2 * TC_MAX_RES_KB) * 8 <= grp_off - tb_off - TC_BN * 4,
                 "the mbarriers of every ring fit in the 256 bytes after t_y");
