@@ -559,6 +559,47 @@ int b2d_dbscan_fit(void* stream, int metric, const float* x, int64_t ldx, int64_
                    int32_t* core_sample_indices /* [m] or NULL */, int32_t* n_clusters /* device, or NULL */,
                    void* workspace, size_t workspace_bytes);
 
+/* Mean shift (sklearn.cluster.MeanShift(bandwidth = h, seeds, bin_seeding, min_bin_freq, cluster_all, max_iter).fit(x)
+ * with sklearn's test dist <= h replaced by the engine's rule; a project API, no upstream signature) for fp32 x:[n,d]
+ * (row-major, pitch ldx >= d, d <= 320):
+ *   Neighbourhood: row j of x is within h of a point p when d^2(p, x_j) <= e = fp32(h^2), h^2 formed in fp64, d^2 the
+ *     value b2d_eps_neighbors_l2sq computes for the pair with the points as x and the data as y (DBSCAN's
+ *     L2SqrtExpanded rule).
+ *   Seeds: seeds:[n_seeds,d] (pitch lds >= d) when not NULL; else with bin_seeding sklearn's get_bin_seeds: the bin of a
+ *     row is rint(x / h) per coordinate (fp64 division, ties to even), the bins holding >= min_bin_freq rows are seeds
+ *     at fp32(bin) * fp32(h) (one fp32 product), and when that makes every row a seed the seeds are the rows of x;
+ *     else the seeds are the rows of x.  Bin seeding runs on the device.
+ *   Iteration (sklearn's _mean_shift_single_seed), per seed: N = the neighbourhood of the current mean; an empty N drops
+ *     the seed; else the new mean is the mean of x over N (fp64, rounded once to fp32); the seed stops when
+ *     ||new - old||_2 <= 1e-3 h (fp64) or after max_iter completed iterations, else its count goes up by one.  So
+ *     max_iter = 0 still moves every seed once.  A stopped seed is frozen with intensity |N| of its last step;
+ *     *n_iter = the largest completed count over all seeds, dropped ones included.
+ *   Centres: surviving seeds with bitwise-equal means merge (intensity: the largest); they are ordered by (intensity,
+ *     coordinates lexicographically by their fp32 order) descending and walked greedily: a centre no earlier kept centre
+ *     suppresses is kept and suppresses every later one within h of it, where i and j are within h when d^2(c_i, c_j)
+ *     <= e or d^2(c_j, c_i) <= e (the symmetric rule, from the candidates prepared once as both operands).
+ *   Labels: the nearest kept centre of every row by the fused L2 arg-min (b2d_fused_l2_nn's distance, ties to the
+ *     smaller centre index); with cluster_all == 0 a row whose squared distance to it is > e gets -1.
+ * Outputs (device): centers [n_seeds or n][d], kept centres first in walk order; *n_centers (int32; 0: no seed had a
+ * neighbour, labels all -1); labels [n] (int32); *n_iter (int32, may be NULL).  Results are bit-identical from run to run
+ * and independent of max_bytes_per_batch, the device's SM count and the seed order: every sum is fp64 over fp32 partials
+ * of fixed chunks of 2048 data rows, folded in ascending order; the only atomics are integer ones.
+ * The adjacency is formed for batches of b = min(S rounded up to 128, max(128, floor(max_bytes_per_batch / ld / 128) *
+ * 128)) seeds (S the seed capacity, ld = max(n, S) rounded up to 16; 0 means 2^30 bytes).  The iterations are enqueued
+ * without a host round trip (the ones after every seed has stopped return at once); the call synchronises its stream
+ * after bin seeding, after the iterations and after the walk, to size what follows.  d > 320 is B2D_ERR_UNSUPPORTED;
+ * n == 0, n or n_seeds >= 2^31, d < 1, a bandwidth that is not finite or > 0 or whose square is not finite in fp32,
+ * max_iter < 0, seeds without n_seeds or the reverse, lds < d, ldx < d, bin_seeding with min_bin_freq < 1, a negative
+ * max_bytes_per_batch and null x / centers / labels / n_centers are B2D_ERR_INVALID_ARG.  Precondition: x and seeds
+ * finite.  The workspace depends on (n, d, n_seeds, max_bytes_per_batch) only (n_seeds = 0: no caller seeds); the
+ * query returns SIZE_MAX for negative arguments. */
+size_t b2d_mean_shift_fit_workspace_bytes(int64_t n, int64_t d, int64_t n_seeds, int64_t max_bytes_per_batch);
+int b2d_mean_shift_fit(void* stream, const float* x, int64_t ldx, int64_t n, int64_t d, double bandwidth,
+                       const float* seeds /* [n_seeds][lds] or NULL */, int64_t lds, int64_t n_seeds, int bin_seeding,
+                       int64_t min_bin_freq, int cluster_all, int max_iter, int64_t max_bytes_per_batch,
+                       float* centers, int32_t* n_centers, int32_t* labels, int32_t* n_iter /* or NULL */,
+                       void* workspace, size_t workspace_bytes);
+
 #ifdef __cplusplus
 }
 #endif

@@ -25,6 +25,7 @@ SYMBOLS = [
     "b2d_single_linkage_workspace_bytes", "b2d_single_linkage", "b2d_dbscan_workspace_bytes", "b2d_dbscan_fit",
     "b2d_debug_pairwise_plan", "b2d_radius_neighbors_workspace_bytes", "b2d_radius_neighbors_count",
     "b2d_radius_neighbors_fill", "b2d_kde_workspace_bytes", "b2d_kde_score_samples",
+    "b2d_mean_shift_fit_workspace_bytes", "b2d_mean_shift_fit",
 ]
 
 B2D_OK, B2D_ERR_INVALID_ARG, B2D_ERR_CUDA, B2D_ERR_UNSUPPORTED, B2D_ERR_WORKSPACE = range(5)
@@ -162,6 +163,10 @@ def lib() -> ctypes.CDLL:
     L.b2d_kde_workspace_bytes.argtypes = [i64, i64, i64, i64]
     L.b2d_kde_score_samples.restype = ci
     L.b2d_kde_score_samples.argtypes = [vp, ci, cd, vp, i64, vp, vp, i64, i64, i64, i64, i64, vp, vp, sz]
+    L.b2d_mean_shift_fit_workspace_bytes.restype = sz
+    L.b2d_mean_shift_fit_workspace_bytes.argtypes = [i64, i64, i64, i64]
+    L.b2d_mean_shift_fit.restype = ci
+    L.b2d_mean_shift_fit.argtypes = [vp, vp, i64, i64, i64, cd, vp, i64, i64, ci, i64, ci, ci, i64, vp, vp, vp, vp, vp, sz]
     L.b2d_row_norm.restype = ci
     L.b2d_row_norm.argtypes = [vp, vp, vp, i64, i64, i64, ci, ci]
     _lib = L

@@ -3,4 +3,5 @@ from .kmeans import (  # noqa: F401
 )
 from . import kmeans_balanced  # noqa: F401  (a module: its fit / predict are not k-means')
 from .dbscan import DbscanOutput, dbscan  # noqa: F401
+from .mean_shift import MeanShiftOutput, estimate_bandwidth, mean_shift  # noqa: F401
 from .single_linkage import LinkageOutput, MstOutput, mst, single_linkage  # noqa: F401

@@ -123,11 +123,13 @@ bool tc_metric(int metric, int64_t k, TcMetric* out);
 int64_t tc_self_diag(const TcMetric& tm, const void* x, int64_t xrs, int64_t xcs, int64_t m, const void* y, int64_t yrs,
                      int64_t ycs, int64_t n);
 
-// operand preparation (prep.cuh) of x [m, k] and y [n, k] into w; T is float or __half
+// operand preparation (prep.cuh) of x [m, k] and y [n, k] into w; T is float or __half.  x_only (with n == 0): the rows
+// of x alone, against the y side an earlier launch prepared (the seeds of every mean-shift iteration)
 template <typename T>
 int launch_prep(cudaStream_t s, const TcWorkspace& w, const void* x, int64_t xrs, int64_t xcs, int64_t m,
                 const void* y, int64_t yrs, int64_t ycs, int64_t n, int64_t k, const float* xn, const float* yn,
-                const TcMetric& tm, const int* y_gather = nullptr, bool y_only = false, const unsigned* run_flag = nullptr);
+                const TcMetric& tm, const int* y_gather = nullptr, bool y_only = false, const unsigned* run_flag = nullptr,
+                bool x_only = false);
 
 // one expanded_tc_kernel launch (K chunk [kb0, kb0 + nkb_chunk) when nkb_chunk > 0)
 int launch_tc(cudaStream_t s, const TcWorkspace& w, TcParams p, int64_t k, int epi, int post, int kb0 = 0,

@@ -106,7 +106,7 @@ int64_t tc_self_diag(const TcMetric& tm, const void* x, int64_t xrs, int64_t xcs
 template <typename T>
 int launch_prep(cudaStream_t s, const TcWorkspace& w, const void* x, int64_t xrs, int64_t xcs, int64_t m,
                 const void* y, int64_t yrs, int64_t ycs, int64_t n, int64_t k, const float* xn, const float* yn,
-                const TcMetric& tm, const int* y_gather, bool y_only, const unsigned* run_flag)
+                const TcMetric& tm, const int* y_gather, bool y_only, const unsigned* run_flag, bool x_only)
 {
   PrepParams p;
   p.side[0] = PrepSide{x, xrs, xcs, m, w.xop, w.xt, w.xsc, xn, w.xlo, nullptr};
@@ -115,8 +115,14 @@ int launch_prep(cudaStream_t s, const TcWorkspace& w, const void* x, int64_t xrs
   p.gmax = w.gmax; p.coef = w.coef; p.has_lo = w.has_lo; p.nonuni = w.nonuni;
   p.xform = tm.xform; p.coef_mul = tm.coef_mul; p.tx_const = tm.tx_const;
   p.first_side = y_only ? 1 : 0; p.run_flag = run_flag;
-  // (y_only: the caller has zeroed gmax[1] and nonuni[1] on the stream -- km_begin_kernel)
-  if (!y_only) B2D_CUDA(cudaMemsetAsync(w.gmax, 0, 32, s));
+  // (y_only: the caller has zeroed gmax[1] and nonuni[1] on the stream -- km_begin_kernel.  x_only: n == 0, so only the
+  // rows of x are prepared, against the y exponent gmax[1] an earlier launch left)
+  if (x_only) {
+    B2D_CUDA(cudaMemsetAsync(w.gmax, 0, sizeof(unsigned), s));
+    B2D_CUDA(cudaMemsetAsync(w.nonuni, 0, sizeof(unsigned), s));
+  } else if (!y_only) {
+    B2D_CUDA(cudaMemsetAsync(w.gmax, 0, 32, s));
+  }
   const int64_t blocks = ((y_only ? 0 : m) + n + 7) / 8;
   prep_max_kernel<T><<<static_cast<unsigned>(blocks), 256, 0, s>>>(p);
   B2D_CUDA(cudaGetLastError());
@@ -126,10 +132,10 @@ int launch_prep(cudaStream_t s, const TcWorkspace& w, const void* x, int64_t xrs
 }
 template int launch_prep<float>(cudaStream_t, const TcWorkspace&, const void*, int64_t, int64_t, int64_t, const void*,
                                 int64_t, int64_t, int64_t, int64_t, const float*, const float*, const TcMetric&,
-                                const int*, bool, const unsigned*);
+                                const int*, bool, const unsigned*, bool);
 template int launch_prep<__half>(cudaStream_t, const TcWorkspace&, const void*, int64_t, int64_t, int64_t, const void*,
                                  int64_t, int64_t, int64_t, int64_t, const float*, const float*, const TcMetric&,
-                                 const int*, bool, const unsigned*);
+                                 const int*, bool, const unsigned*, bool);
 
 template <bool kRes, int kEpi, int kPost>
 static int launch_tc_inst(cudaStream_t s, const CUtensorMap& ma, const CUtensorMap& mb, const CUtensorMap (&md)[2],
