@@ -590,15 +590,31 @@ int b2d_dbscan_fit(void* stream, int metric, const float* x, int64_t ldx, int64_
  * after bin seeding, after the iterations and after the walk, to size what follows.  d > 320 is B2D_ERR_UNSUPPORTED;
  * n == 0, n or n_seeds >= 2^31, d < 1, a bandwidth that is not finite or > 0 or whose square is not finite in fp32,
  * max_iter < 0, seeds without n_seeds or the reverse, lds < d, ldx < d, bin_seeding with min_bin_freq < 1, a negative
- * max_bytes_per_batch and null x / centers / labels / n_centers are B2D_ERR_INVALID_ARG.  Precondition: x and seeds
- * finite.  The workspace depends on (n, d, n_seeds, max_bytes_per_batch) only (n_seeds = 0: no caller seeds); the
- * query returns SIZE_MAX for negative arguments. */
+ * max_bytes_per_batch and null x / centers / labels / n_centers are B2D_ERR_INVALID_ARG.  A row of x with a non-finite
+ * element is within h of no point: it adds to no mean, no intensity and no count, a seed it gives (the rows, or its bin)
+ * is dropped, and its label is -1; every other result is what the fit gives without that row's contributions.
+ * Precondition: seeds finite.  The workspace depends on (n, d, n_seeds, max_bytes_per_batch) only (n_seeds = 0: no
+ * caller seeds); the query returns SIZE_MAX for negative arguments. */
 size_t b2d_mean_shift_fit_workspace_bytes(int64_t n, int64_t d, int64_t n_seeds, int64_t max_bytes_per_batch);
 int b2d_mean_shift_fit(void* stream, const float* x, int64_t ldx, int64_t n, int64_t d, double bandwidth,
                        const float* seeds /* [n_seeds][lds] or NULL */, int64_t lds, int64_t n_seeds, int bin_seeding,
                        int64_t min_bin_freq, int cluster_all, int max_iter, int64_t max_bytes_per_batch,
                        float* centers, int32_t* n_centers, int32_t* labels, int32_t* n_iter /* or NULL */,
                        void* workspace, size_t workspace_bytes);
+/* The neighbour sums of one mean-shift step on their own, for tests.  adj [m][ld_adj] (device bytes, 0 or 1 in the
+ * columns [0, n); the rest of a row is never read) is the adjacency of m seeds against the data x [n][d] (pitch ldx >= d,
+ * d <= 320).  x is prepared as the fit prepares its data (a row with a non-finite element cleared) and summed by the fit's
+ * kernel.  Outputs: part [nchunks][m][d] (device, fp32) and counts [nchunks][m] (device, uint32) with nchunks = ceil(n /
+ * 2048): for chunk c (data rows [2048 c, 2048 c + 2048)), part[c][i][t] = 2^E times the sum of x[j][t] over the rows j of
+ * the chunk with adj[i][j] = 1, in the fit's fp32 arithmetic, and counts[c][i] the number of those rows, exactly;
+ * *exponent (device, int32) = E, the power of two the data was scaled by; info[6] (host, int64) = {k-blocks per group,
+ * groups, nchunks, work items, CTAs, 1 when some data row took its own exponent else 0}.  m, n in [1, 2^31), d >= 1,
+ * ldx >= d, ld_adj >= n a multiple of 16 with adj 16-byte aligned, non-null pointers and adjacency bytes 0 or 1 (checked
+ * on the device) else B2D_ERR_INVALID_ARG; d > 320 is B2D_ERR_UNSUPPORTED.  The workspace is
+ * b2d_mean_shift_fit_workspace_bytes(n, d, m, 0).  Synchronises its stream twice. */
+int b2d_debug_mean_shift_sums(void* stream, const uint8_t* adj, int64_t ld_adj, int64_t m, const float* x, int64_t ldx,
+                              int64_t n, int64_t d, float* part, uint32_t* counts, int32_t* exponent, int64_t* info,
+                              void* workspace, size_t workspace_bytes);
 
 #ifdef __cplusplus
 }

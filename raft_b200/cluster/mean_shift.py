@@ -69,13 +69,18 @@ def mean_shift(X, bandwidth=None, seeds=None, bin_seeding=False, min_bin_freq=1,
 
     Returns ``MeanShiftOutput(cluster_centers, labels, n_iter)``: float32 [n_centers, d] and int32 [n] torch tensors on
     the device (-1: a row farther than bandwidth from every centre, with cluster_all=False) and the largest iteration
-    count of any seed.  Raises ValueError when no seed has a neighbour, as sklearn does."""
+    count of any seed.  Raises ValueError when X holds a NaN or an infinity, and when no seed has a neighbour, as sklearn
+    does."""
     x = cai_wrapper(X)
     n, d, ldx = _rows(x, "X")
     if n == 0:
         raise ValueError("X has no rows")
     if d > MAX_D:
         raise _lib.LogicError("mean_shift supports d <= %d, got %d" % (MAX_D, d))
+    with torch.cuda.stream(handle.torch_stream):
+        finite = bool(torch.isfinite(torch.as_tensor(X, device=handle.device)).all().item())
+    if not finite:
+        raise ValueError("Input X contains NaN or infinity.")
     if bandwidth is None:
         bandwidth = estimate_bandwidth(X, handle=handle)
     bandwidth = float(bandwidth)

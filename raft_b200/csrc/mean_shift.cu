@@ -14,6 +14,9 @@ using namespace b2d;
 namespace {
 constexpr int64_t kMsDefaultBatchBytes = 1ll << 30;
 
+// fp32 partials per seed of the neighbour sums: one per chunk of kMsChunk data rows
+int64_t ms_nchunks(int64_t n) { return (n + kMsChunk - 1) / kMsChunk; }
+
 // The workspace of a fit with n data rows and a seed capacity S (the caller's seed count, or n): the tensor path's
 // operands for max(n, S) rows on both sides (seeds x data while iterating, candidates x candidates for the walk, data x
 // centres for the labels), the seed state, one batch of adjacency and partials, and the sort regions.
@@ -66,7 +69,7 @@ MsLayout ms_layout(void* base, int64_t n, int64_t d, int64_t n_seeds, int64_t ma
   L.tc      = tc_layout(c, R, R, d, false);
   L.ld      = (std::max<int64_t>(R, 1) + 15) / 16 * 16;
   L.b       = ms_batch(L.S, L.ld, max_bytes);
-  L.nchunks = (n + kMsChunk - 1) / kMsChunk;
+  L.nchunks = ms_nchunks(n);
   L.ctrl    = c.take<MsCtrl>(1);
   L.scan    = c.take<KmCtrl>(2);
   L.mean    = c.take<float>(static_cast<size_t>(L.S) * d);
@@ -114,19 +117,27 @@ int ms_eps(cudaStream_t s, const MsLayout& L, int64_t r0, int64_t w, int64_t n, 
 }
 
 template <int G>
-int ms_sum_launch(cudaStream_t s, const CUtensorMap& ma, const CUtensorMap& mb, MsSumParams p, int sms)
+int ms_sum_launch(cudaStream_t s, const CUtensorMap& ma, const CUtensorMap& mb, MsSumParams p, int grid)
 {
   constexpr size_t smem = MsCarve<G>::bytes;
   p.stages = MsCarve<G>::stages;
   B2D_CUDA(cudaFuncSetAttribute(ms_sum_kernel<G>, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem)));
-  const int grid = static_cast<int>(std::min<int64_t>(p.n_items, sms));
   ms_sum_kernel<G><<<grid, kMsThreads, smem, s>>>(ma, mb, p);
   B2D_CUDA(cudaGetLastError());
   return B2D_OK;
 }
 
-// The neighbour sums of the w seeds of the current adjacency batch against the n prepared data rows (y side)
-int ms_sums(cudaStream_t s, const MsLayout& L, int64_t w, int64_t n, int64_t d, const unsigned* run)
+// How ms_sums cut its work (b2d_debug_mean_shift_sums reports it)
+struct MsSumPlan {
+  int gsz, ngroups, nchunks;
+  int64_t n_items;
+  int grid;
+};
+
+// The neighbour sums of the w seeds of adj [w][ld] (bytes, columns [0, n) read; ld a multiple of 16) against the n data
+// rows prepared as the y side of tc: part [ms_nchunks(n)][w][d] and cnt [ms_nchunks(n)][w] (ms_sum_kernel)
+int ms_sums(cudaStream_t s, const TcWorkspace& tc, const uint8_t* adj, int64_t ld, int64_t w, int64_t n, int64_t d,
+            float* part, unsigned* cnt, const unsigned* run, MsSumPlan* plan = nullptr)
 {
   int sms = 0;
   int rc  = device_sms(&sms);
@@ -136,20 +147,30 @@ int ms_sums(cudaStream_t s, const MsLayout& L, int64_t w, int64_t n, int64_t d, 
   p.gsz     = p.nkb >= 3 ? 4 : p.nkb;
   p.ngroups = (p.nkb + p.gsz - 1) / p.gsz;
   p.tiles_m = static_cast<int>((w + kMsTileM - 1) / kMsTileM);
-  p.nchunks = static_cast<int>(L.nchunks);
+  p.nchunks = static_cast<int>(ms_nchunks(n));
   p.n_items = static_cast<int64_t>(p.tiles_m) * p.nchunks * p.ngroups;
-  p.ysc = L.tc.ysc; p.nonuni = L.tc.nonuni; p.part = L.part; p.cnt = L.part_cnt; p.run_flag = run;
+  p.ysc = tc.ysc; p.nonuni = tc.nonuni; p.part = part; p.cnt = cnt; p.run_flag = run;
+  const int grid = static_cast<int>(std::min<int64_t>(p.n_items, sms));
+  if (plan) *plan = MsSumPlan{p.gsz, p.ngroups, p.nchunks, p.n_items, grid};
   CUtensorMap ma, mb;
-  rc = encode_2d(&ma, CU_TENSOR_MAP_DATA_TYPE_UINT8, L.adj, n, w, L.ld, kMsKs, kMsTileM, CU_TENSOR_MAP_SWIZZLE_128B,
+  rc = encode_2d(&ma, CU_TENSOR_MAP_DATA_TYPE_UINT8, adj, n, w, ld, kMsKs, kMsTileM, CU_TENSOR_MAP_SWIZZLE_128B,
                  CU_TENSOR_MAP_L2_PROMOTION_L2_256B, "(mean_shift adj)");
   if (rc) return rc;
-  rc = encode_2d(&mb, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, L.tc.yop, static_cast<int64_t>(p.nkb) * 64, n,
+  rc = encode_2d(&mb, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, tc.yop, static_cast<int64_t>(p.nkb) * 64, n,
                  static_cast<int64_t>(p.nkb) * 128, 64, kMsKs, CU_TENSOR_MAP_SWIZZLE_128B,
                  CU_TENSOR_MAP_L2_PROMOTION_L2_256B, "(mean_shift data)");
   if (rc) return rc;
-  if (p.gsz == 1) return ms_sum_launch<1>(s, ma, mb, p, sms);
-  if (p.gsz == 2) return ms_sum_launch<2>(s, ma, mb, p, sms);
-  return ms_sum_launch<4>(s, ma, mb, p, sms);
+  if (p.gsz == 1) return ms_sum_launch<1>(s, ma, mb, p, grid);
+  if (p.gsz == 2) return ms_sum_launch<2>(s, ma, mb, p, grid);
+  return ms_sum_launch<4>(s, ma, mb, p, grid);
+}
+
+// the data rows of tc's y side with a non-finite element out of every sum (ms_clear_nonfinite_kernel)
+int ms_clear_nonfinite(cudaStream_t s, const TcWorkspace& tc, int64_t n, int64_t d)
+{
+  ms_clear_nonfinite_kernel<<<ms_grid(n, 256), 256, 0, s>>>(tc.yt, n, static_cast<int>((d + 31) / 32), tc.yop);
+  B2D_CUDA(cudaGetLastError());
+  return B2D_OK;
 }
 
 __global__ void ms_ctrl_init_kernel(MsCtrl* ctrl)
@@ -274,6 +295,8 @@ int b2d_mean_shift_fit(void* stream, const float* x, int64_t ldx, int64_t n, int
   //    device once no seed is active
   rc = launch_prep<float>(s, L.tc, L.mean, d, 1, ns, x, ldx, 1, n, d, nullptr, nullptr, TC_L2);
   if (rc) return rc;
+  rc = ms_clear_nonfinite(s, L.tc, n, d);
+  if (rc) return rc;
   for (int it = 0; it <= max_iter; ++it) {
     ProfileScope prof(s);
     if (it > 0) {
@@ -285,7 +308,7 @@ int b2d_mean_shift_fit(void* stream, const float* x, int64_t ldx, int64_t n, int
       const int64_t w = std::min(L.b, ns - r0);
       rc = ms_eps(s, L, r0, w, n, d, e, TC_NO_DIAG, run);
       if (rc) return rc;
-      rc = ms_sums(s, L, w, n, d, run);
+      rc = ms_sums(s, L.tc, L.adj, L.ld, w, n, d, L.part, L.part_cnt, run);
       if (rc) return rc;
       ms_update_kernel<<<ms_grid(w, 8), 256, 0, s>>>(run, L.part, L.part_cnt, static_cast<int>(L.nchunks), w, r0, dd,
                                                      L.tc.gmax, thr, max_iter, L.mean, L.state, L.iters, L.inten, L.ctrl);
@@ -354,5 +377,48 @@ int b2d_mean_shift_fit(void* stream, const float* x, int64_t ldx, int64_t n, int
   if (rc) return rc;
   ms_label_kernel<<<ms_grid(n, 256), 256, 0, s>>>(L.keys, n, cluster_all, e, labels);
   B2D_CUDA(cudaGetLastError());
+  return B2D_OK;
+}
+
+int b2d_debug_mean_shift_sums(void* stream, const uint8_t* adj, int64_t ld_adj, int64_t m, const float* x, int64_t ldx,
+                              int64_t n, int64_t d, float* part, uint32_t* counts, int32_t* exponent, int64_t* info,
+                              void* workspace, size_t workspace_bytes)
+{
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  if (m < 1 || n < 1) return fail(B2D_ERR_INVALID_ARG, "m and n must be positive");
+  if (m > 0x7fffffffll || n > 0x7fffffffll) return fail(B2D_ERR_INVALID_ARG, "mean_shift: m and n must be below 2^31");
+  if (d < 1) return fail(B2D_ERR_INVALID_ARG, "d must be positive");
+  if (d > 320) return fail(B2D_ERR_UNSUPPORTED, "mean_shift supports d <= 320 (the whole distance at once)");
+  if (!adj || !x || !part || !counts || !exponent || !info)
+    return fail(B2D_ERR_INVALID_ARG, "null adj / x / part / counts / exponent / info");
+  if (ldx < d) return fail(B2D_ERR_INVALID_ARG, "leading dimension smaller than d");
+  if (ld_adj < n || ld_adj % 16 != 0 || reinterpret_cast<uintptr_t>(adj) % 16 != 0)
+    return fail(B2D_ERR_INVALID_ARG, "adjacency pitch must be >= n and a multiple of 16, on a 16-byte boundary");
+  int rc = check_workspace(workspace, workspace_bytes, ms_layout(nullptr, n, d, m, 0).bytes);
+  if (rc) return rc;
+  const MsLayout L = ms_layout(workspace, n, d, m, 0);
+  unsigned bad = 0;
+  B2D_CUDA(cudaMemsetAsync(L.flag, 0, sizeof(unsigned), s));
+  ms_adj_check_kernel<<<static_cast<unsigned>(std::min<int64_t>(ms_grid(m * n, 256), 4096)), 256, 0, s>>>(adj, ld_adj, m,
+                                                                                                        n, L.flag);
+  B2D_CUDA(cudaGetLastError());
+  rc = ms_read(s, L.flag, &bad);
+  if (rc) return rc;
+  if (bad) return fail(B2D_ERR_INVALID_ARG, "adjacency bytes must be 0 or 1");
+  // the data side of a fit: prepared, non-finite rows cleared, then the fit's launcher
+  rc = launch_prep<float>(s, L.tc, nullptr, 0, 1, 0, x, ldx, 1, n, d, nullptr, nullptr, TC_L2);
+  if (rc) return rc;
+  rc = ms_clear_nonfinite(s, L.tc, n, d);
+  if (rc) return rc;
+  MsSumPlan plan{};
+  rc = ms_sums(s, L.tc, adj, ld_adj, m, n, d, part, counts, nullptr, &plan);
+  if (rc) return rc;
+  ms_exponent_kernel<<<1, 1, 0, s>>>(L.tc.gmax, exponent);
+  B2D_CUDA(cudaGetLastError());
+  unsigned scaled = 0;
+  rc = ms_read(s, L.tc.nonuni + 1, &scaled);
+  if (rc) return rc;
+  const int64_t out[6] = {plan.gsz, plan.ngroups, plan.nchunks, plan.n_items, plan.grid, scaled};
+  std::copy(out, out + 6, info);
   return B2D_OK;
 }

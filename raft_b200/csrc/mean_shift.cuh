@@ -257,6 +257,30 @@ __global__ void __launch_bounds__(kMsThreads, 1) ms_sum_kernel(const __grid_cons
   }
 }
 
+// After the data's preparation (y side): the packed row of every data row with a non-finite element (its squared norm t
+// is NaN or +inf) becomes 0.  EPI_EPS still rejects the row through its t, so it is adjacent to no seed, and the zero
+// operand keeps it out of the sums: A . X would otherwise take 0 * NaN = NaN into the column of every seed of its chunk.
+// (A finite row whose squared norm overflows fp32 is at distance +inf from every seed too, and is cleared with them.)
+__global__ void ms_clear_nonfinite_kernel(const float* t, int64_t n, int nkb, __half* op)
+{
+  const int64_t r = static_cast<int64_t>(blockIdx.x) * blockDim.x + threadIdx.x;
+  if (r >= n || isfinite(t[r])) return;
+  uint4* row = reinterpret_cast<uint4*>(op + r * static_cast<int64_t>(nkb) * 64);   // 128 bytes per k-block
+  for (int i = 0; i < nkb * 8; ++i) row[i] = make_uint4(0u, 0u, 0u, 0u);
+}
+
+// b2d_debug_mean_shift_sums: *bad = 1 when a byte of adj [m][ld] in the columns [0, n) is neither 0 nor 1
+__global__ void ms_adj_check_kernel(const uint8_t* adj, int64_t ld, int64_t m, int64_t n, unsigned* bad)
+{
+  const int64_t total = m * n;
+  for (int64_t q = static_cast<int64_t>(blockIdx.x) * blockDim.x + threadIdx.x; q < total;
+       q += static_cast<int64_t>(gridDim.x) * blockDim.x)
+    if (adj[(q / n) * ld + q % n] > 1u) *bad = 1u;
+}
+
+// b2d_debug_mean_shift_sums: the data exponent E of the prepared y side (the one ms_update_kernel undoes)
+__global__ void ms_exponent_kernel(const unsigned* gmax, int* e) { *e = scale_exponent(__uint_as_float(gmax[1])); }
+
 // One warp per seed of the batch [r0, r0 + m): the partials folded in fp64 in ascending chunk order (each lane its own
 // columns, the squared shift reduced in a fixed xor tree), the mean rounded once to fp32, and sklearn's stop rule:
 // no neighbour drops the seed; a shift <= thr or `max_iter` completed iterations stops it; else it goes on.

@@ -18,6 +18,30 @@ def exact_within(h):
     return lambda P, Q: np.sqrt(exact_d2(P, Q)) <= h
 
 
+def scale_exponent(a):
+    """prep.cuh scale_exponent: the e that puts a > 0 into [2^14, 2^15), clamped to [-100, 100]; 0 for 0 or >= 3e38"""
+    if not 0.0 < a < 3.0e38:
+        return 0
+    return int(np.clip(15 - np.frexp(a)[1], -100, 100))
+
+
+def prep_scales(X):
+    """The exponents the operand preparation (prep.cuh) gives the data rows of X [n, d] (fp32): (E, M, svec, own) with
+    M the largest |element| of the rows whose maximum is finite (a NaN element is skipped), E = scale_exponent(M),
+    own[j] when row j took its own exponent e_j and svec[j] = 2^(E - e_j) (1 for the other rows).  The neighbour sums
+    multiply row j by fp16(svec[j]): rows with svec[j] < 2^-24 (fp16 rounds it to 0) are left out of the sums."""
+    a = np.abs(np.asarray(X, np.float32).astype(np.float64))
+    amax = np.where(np.isnan(a), 0.0, a).max(1)
+    valid = (amax > 0) & (amax < 3.0e38)
+    M = float(amax[valid].max()) if valid.any() else 0.0
+    E = scale_exponent(M)
+    own = valid & (amax * 2.0 ** E < 8.0)
+    svec = np.ones(len(a))
+    for j in np.flatnonzero(own):
+        svec[j] = 2.0 ** (E - max(E, min(scale_exponent(amax[j]), E + 120)))
+    return E, M, svec, own
+
+
 def ordered_bits(v):
     """the fp32 order of v as int64, -0 before +0"""
     b = np.asarray(v, np.float32).view(np.int32).astype(np.int64)

@@ -7,7 +7,11 @@ Accuracy bound of one step.  The new mean of a seed is sum_{j in N} x_j / |N| wi
     (relative 2^-23 at most, truncation included), so a chunk partial is off by <= 128 * 2^-23 sum |x_j| = 2^-16 sum |x_j|;
     adding the hi and lo halves rounds once more (2^-23 of it); the fp64 fold of the chunks adds nothing that matters;
   * the mean is rounded once to fp32 (2^-24 relative).
-So per coordinate |got - ref| <= 2^-15 mean_{j in N} |x_j| + 2^-23 |ref| + 2^-37 M, with ref the fp64 mean over N.  When
+  * a row more than about 2^24 below M that took its own exponent (prep.cuh) enters the sums with the factor
+    2^(E - e_j) rounded to fp16; below 2^-24 that is 0, so the row is left out of the sums (but not of |N|): the
+    mean loses sum_{j in N, dropped} |x_j| / |N| at most (tests/mean_shift_ref.py prep_scales names those rows).
+So per coordinate |got - ref| <= 2^-15 mean_{j in N} |x_j| + 2^-23 |ref| + 2^-37 M + sum_{j in N, dropped} |x_j| / |N|,
+with ref the fp64 mean over N (tests/test_mean_shift_paths_gpu.py checks the sums per chunk).  When
 every step of a fit sees the same neighbourhoods as the exact model, the final centres are one such step from the model's,
 so the same bound holds for them; the fits below check that their data keep every decision (neighbourhood, stop rule,
 suppression, label radius) at least 2^-14 max |x| away from its threshold."""
@@ -23,8 +27,11 @@ torch = pytest.importorskip("torch")
 def step_bound(X, nb, ref):
     """the per-coordinate bound above for the means of the rows nb [s, n] of X"""
     ax = np.abs(X.astype(np.float64))
-    mean_abs = (nb.astype(np.float64) @ ax) / np.maximum(nb.sum(1, keepdims=True), 1)
-    return 2.0 ** -15 * mean_abs + 2.0 ** -23 * np.abs(ref) + 2.0 ** -37 * ax.max()
+    dropped = R.prep_scales(X)[2] < 2.0 ** -24
+    cnt = np.maximum(nb.sum(1, keepdims=True), 1)
+    mean_abs = (nb.astype(np.float64) @ ax) / cnt
+    lost = (nb.astype(np.float64) @ (ax * dropped[:, None])) / cnt
+    return 2.0 ** -15 * mean_abs + 2.0 ** -23 * np.abs(ref) + 2.0 ** -37 * ax.max() + lost
 
 
 def grid(k, d, step):
@@ -84,10 +91,10 @@ def exact_model(x, h, **kw):
     return out, min(gaps)
 
 
-def check_fit(x, h, x_gpu=None, **kw):
+def check_fit(x, h, x_gpu=None, max_mbytes_per_batch=None, **kw):
     (mc, ml, mi), gap = exact_model(x, h, **kw)
     assert gap > 2.0 ** -14 * np.abs(x).max(), "the data put a decision within %g of its threshold" % gap
-    gc, gl, gi = gpu(x if x_gpu is None else x_gpu, h, **kw)
+    gc, gl, gi = gpu(x if x_gpu is None else x_gpu, h, max_mbytes_per_batch=max_mbytes_per_batch, **kw)
     assert gi == mi
     assert gc.shape == mc.shape
     bound = 2.0 ** -15 * np.abs(x).max() + 2.0 ** -23 * np.abs(mc)
