@@ -616,6 +616,44 @@ int b2d_debug_mean_shift_sums(void* stream, const uint8_t* adj, int64_t ld_adj, 
                               int64_t n, int64_t d, float* part, uint32_t* counts, int32_t* exponent, int64_t* info,
                               void* workspace, size_t workspace_bytes);
 
+/* Random ball cover (raft::neighbors::ball_cover before the move to cuVS): exact kNN and epsilon-neighbourhood queries for
+ * 2-D and 3-D points without the m x n pairs of the tensor path.  x [n][d] fp32, row-major, pitch ldx >= d; d in {2, 3}
+ * and metric L2Unexpanded or L2SqrtUnexpanded (else B2D_ERR_UNSUPPORTED); 1 <= n < 2^31.
+ *   The value of a pair is fixed bit for bit: s = ((q0-p0)*(q0-p0) + (q1-p1)*(q1-p1)) + (q2-p2)*(q2-p2), every operation
+ *     rounded separately (no FMA contraction; no third term at d = 2); the distance is s (L2Unexpanded) or sqrt(s)
+ *     correctly rounded (L2SqrtUnexpanded).  Neighbours are ordered by the packed (distance, index) key of the other
+ *     neighbour entry points, index = the caller's row of x.  b2d_knn computes the expanded form: its distances can differ
+ *     in the last bits, and so can the order of near-ties.
+ *   A pair whose distance is NaN (a NaN coordinate on either side, inf - inf) is never a neighbour.
+ *   The answers are exact: they do not depend on seed, n_landmarks, the device or the order of the queries.
+ * The index is one caller-owned device buffer of b2d_ball_cover_index_bytes(n, d, n_landmarks) bytes (256-byte aligned),
+ * written by b2d_ball_cover_build; it holds its own copy of the points, so x need not outlive the build.  n_landmarks in
+ * [1, n], or 0 for ceil(sqrt(n)); landmarks are a seeded uniform sample without replacement of the rows without a
+ * non-finite coordinate.  Every query takes the n, d, metric and n_landmarks the index was built with.
+ * Every call only enqueues work (no synchronisation, no allocation) and checks its arguments before any device work; the
+ * size queries return SIZE_MAX for invalid extents. */
+size_t b2d_ball_cover_index_bytes(int64_t n, int64_t d, int64_t n_landmarks);
+size_t b2d_ball_cover_build_workspace_bytes(int64_t n, int64_t d, int64_t n_landmarks);
+int b2d_ball_cover_build(void* stream, void* index, const float* x, int64_t ldx, int64_t n, int64_t d, int metric,
+                         int64_t n_landmarks, uint64_t seed, void* workspace, size_t workspace_bytes);
+/* out_idx int64 [m][k], out_dist float [m][k]: the k nearest rows of each query row q [m][d] (pitch ldq >= d) in ascending
+ * key order.  1 <= k <= n (else B2D_ERR_INVALID_ARG) and k <= 64 (else B2D_ERR_UNSUPPORTED).  A slot without a comparable
+ * row (a NaN query, fewer than k rows at a non-NaN distance) holds index -1, distance +inf, as in b2d_knn.  No workspace. */
+int b2d_ball_cover_knn(void* stream, int64_t* out_idx, float* out_dist, const void* index, int64_t n, int64_t d,
+                       int metric, int64_t n_landmarks, const float* q, int64_t ldq, int64_t m, int64_t k);
+/* Every row at distance <= eps of each query row as CSR (indptr int64 [m + 1], indices int64 [nnz], distances float [nnz]),
+ * rows sorted by the key; under L2Unexpanded eps is a squared distance.  A NaN or negative eps gives no pairs, eps = +inf
+ * every non-NaN pair.  The two calls of b2d_radius_neighbors_count / _fill: count writes indptr, the caller reads
+ * nnz = indptr[m] and calls fill with the same inputs and that nnz (<= 2^31 - 1, else B2D_ERR_UNSUPPORTED); fill never
+ * writes past nnz entries.  Workspace: b2d_ball_cover_eps_workspace_bytes(m, 0) for count, (m, nnz) for fill. */
+size_t b2d_ball_cover_eps_workspace_bytes(int64_t m, int64_t nnz);
+int b2d_ball_cover_eps_count(void* stream, int64_t* indptr, const void* index, int64_t n, int64_t d, int metric,
+                             int64_t n_landmarks, const float* q, int64_t ldq, int64_t m, float eps, void* workspace,
+                             size_t workspace_bytes);
+int b2d_ball_cover_eps_fill(void* stream, const int64_t* indptr, int64_t nnz, int64_t* indices, float* distances,
+                            const void* index, int64_t n, int64_t d, int metric, int64_t n_landmarks, const float* q,
+                            int64_t ldq, int64_t m, float eps, void* workspace, size_t workspace_bytes);
+
 #ifdef __cplusplus
 }
 #endif

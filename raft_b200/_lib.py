@@ -26,6 +26,8 @@ SYMBOLS = [
     "b2d_debug_pairwise_plan", "b2d_radius_neighbors_workspace_bytes", "b2d_radius_neighbors_count",
     "b2d_radius_neighbors_fill", "b2d_kde_workspace_bytes", "b2d_kde_score_samples",
     "b2d_mean_shift_fit_workspace_bytes", "b2d_mean_shift_fit", "b2d_debug_mean_shift_sums",
+    "b2d_ball_cover_index_bytes", "b2d_ball_cover_build_workspace_bytes", "b2d_ball_cover_build", "b2d_ball_cover_knn",
+    "b2d_ball_cover_eps_workspace_bytes", "b2d_ball_cover_eps_count", "b2d_ball_cover_eps_fill",
 ]
 
 B2D_OK, B2D_ERR_INVALID_ARG, B2D_ERR_CUDA, B2D_ERR_UNSUPPORTED, B2D_ERR_WORKSPACE = range(5)
@@ -169,6 +171,20 @@ def lib() -> ctypes.CDLL:
     L.b2d_mean_shift_fit.argtypes = [vp, vp, i64, i64, i64, cd, vp, i64, i64, ci, i64, ci, ci, i64, vp, vp, vp, vp, vp, sz]
     L.b2d_debug_mean_shift_sums.restype = ci
     L.b2d_debug_mean_shift_sums.argtypes = [vp, vp, i64, i64, vp, i64, i64, i64, vp, vp, vp, vp, vp, sz]
+    L.b2d_ball_cover_index_bytes.restype = sz
+    L.b2d_ball_cover_index_bytes.argtypes = [i64, i64, i64]
+    L.b2d_ball_cover_build_workspace_bytes.restype = sz
+    L.b2d_ball_cover_build_workspace_bytes.argtypes = [i64, i64, i64]
+    L.b2d_ball_cover_build.restype = ci
+    L.b2d_ball_cover_build.argtypes = [vp, vp, vp, i64, i64, i64, ci, i64, u64, vp, sz]
+    L.b2d_ball_cover_knn.restype = ci
+    L.b2d_ball_cover_knn.argtypes = [vp, vp, vp, vp, i64, i64, ci, i64, vp, i64, i64, i64]
+    L.b2d_ball_cover_eps_workspace_bytes.restype = sz
+    L.b2d_ball_cover_eps_workspace_bytes.argtypes = [i64, i64]
+    L.b2d_ball_cover_eps_count.restype = ci
+    L.b2d_ball_cover_eps_count.argtypes = [vp, vp, vp, i64, i64, ci, i64, vp, i64, i64, cf, vp, sz]
+    L.b2d_ball_cover_eps_fill.restype = ci
+    L.b2d_ball_cover_eps_fill.argtypes = [vp, vp, i64, vp, vp, vp, i64, i64, ci, i64, vp, i64, i64, cf, vp, sz]
     L.b2d_row_norm.restype = ci
     L.b2d_row_norm.argtypes = [vp, vp, vp, i64, i64, i64, ci, ci]
     _lib = L

@@ -1,0 +1,395 @@
+// Kernels of the random ball cover (ball_cover.cu): exact kNN and epsilon queries for 2-D and 3-D points, SIMT.
+//
+// A pair's value is fixed bit for bit: s = ((q0-p0)^2 + (q1-p1)^2) + (q2-p2)^2, every operation rounded separately
+// (bc_s), and the distance f = s (L2Unexpanded) or sqrt(s) (L2SqrtUnexpanded).  The queries prune whole balls and ball
+// members by the triangle inequality on the TRUE distances of the fp32 points, bounded from the rounded s values with the
+// margin below (DESIGN.md K19 derives it); every bound is formed with directed rounding, so a pruned row provably has
+// f(q, p) above the current k-th value (or above eps) and can never order before it.
+//
+//   D^2 (1 - 6u) - A  <=  s  <=  D^2 (1 + 6u) + A,   u = 2^-24, A = 2^-148 >= 3 squares' underflow (3 * 2^-150),
+//   s = inf only if D^2 >= 2^127 (an overflowing difference, square or sum).
+#pragma once
+#include <cuda_runtime.h>
+#include <cstdint>
+
+#include "nn_key.cuh"
+
+namespace b2d {
+
+// The index, one caller-owned buffer (its regions: bc_index in ball_cover.cu).  Positions are the rows sorted by
+// (ball, s to the ball's landmark, row); rows with a non-finite coordinate follow the last ball.
+struct BcIndex {
+  float* lm;    // [nl][d] landmark coordinates
+  float* rhi;   // [nl] bc_dhi of the ball's largest member s: an upper bound of its true radius; -1: empty ball
+  int* off;     // [nl + 2] ball b holds positions [off[b], off[b + 1]); [off[nl], off[nl + 1] = n) the non-finite rows
+  float* pts;   // [n][d] coordinates by position
+  int* ids;     // [n] the caller's row at each position
+  float* rl;    // [n] s(landmark, row), ascending inside each ball (0 for the non-finite rows)
+};
+
+constexpr int kBcWarps = 8;   // queries per block of the query kernels (one warp each)
+
+constexpr float BC_INF = __builtin_huge_valf();
+constexpr float BC_A   = 0x1p-148f;         // absolute slack of s
+constexpr float BC_UP  = 1.f + 0x1p-21f;    // >= 1 + 6u, >= 1 / (1 - 6u) and >= 1 / (1 - u)^2
+constexpr float BC_DN  = 1.f - 0x1p-21f;    // <= 1 / (1 + 6u)
+constexpr float BC_CAP = 0x1p126f;          // a threshold above this cannot be compared with an s of inf
+
+template <int D>
+__device__ __forceinline__ float bc_s(const float* q, const float* p)
+{
+  const float t0 = __fsub_rn(q[0], p[0]), t1 = __fsub_rn(q[1], p[1]);
+  float s = __fadd_rn(__fmul_rn(t0, t0), __fmul_rn(t1, t1));
+  if (D == 3) {
+    const float t2 = __fsub_rn(q[2], p[2]);
+    s = __fadd_rn(s, __fmul_rn(t2, t2));
+  }
+  return s;
+}
+
+// lower / upper bound of the true distance of a pair whose s is s
+__device__ __forceinline__ float bc_dlo(float s)
+{
+  if (s == BC_INF) return 0x1p63f;
+  return __fsqrt_rd(__fmul_rd(fmaxf(__fsub_rd(s, BC_A), 0.f), BC_DN));
+}
+__device__ __forceinline__ float bc_dhi(float s) { return __fsqrt_ru(__fmul_ru(__fadd_ru(s, BC_A), BC_UP)); }
+// an s above bc_above(t) proves the true distance above t
+__device__ __forceinline__ float bc_above(float t)
+{
+  const float v = __fadd_ru(__fmul_ru(__fmul_ru(t, t), BC_UP), BC_A);
+  return v <= BC_CAP ? v : BC_INF;
+}
+// an s below bc_below(g) proves the true distance below g
+__device__ __forceinline__ float bc_below(float g) { return g > 0.f ? __fsub_rd(__fmul_rd(__fmul_rd(g, g), BC_DN), BC_A) : -1.f; }
+// the largest true distance of a pair whose distance f is at most v
+__device__ __forceinline__ float bc_dmax(float v, int root) { return bc_dhi(root ? __fmul_ru(__fmul_ru(v, v), BC_UP) : v); }
+
+// The member window of a ball for a query at s = sq from its landmark and a distance bound dmax: members with s outside
+// [*lo, *hi] are farther than dmax from the query (|D(q, L) - D(L, p)| > dmax).
+__device__ __forceinline__ void bc_window(float sq, float dmax, float* lo, float* hi)
+{
+  *lo = bc_below(__fsub_rd(bc_dlo(sq), dmax));
+  *hi = bc_above(__fadd_ru(bc_dhi(sq), dmax));
+}
+
+// the ball lies farther than dmax from a query at s = sq from its landmark
+__device__ __forceinline__ bool bc_ball_out(float sq, float rhi, float dmax) { return sq > bc_above(__fadd_ru(rhi, dmax)); }
+
+// first position in [lo, hi) whose rl is not below t (upper: above t)
+__device__ __forceinline__ int bc_search(const float* rl, int lo, int hi, float t, bool upper)
+{
+  while (lo < hi) {
+    const int mid = (lo + hi) >> 1;
+    const float r = rl[mid];
+    if (upper ? !(r > t) : r < t) lo = mid + 1;
+    else hi = mid;
+  }
+  return lo;
+}
+
+// ------------------------------------------------------------------------------------------
+// build
+
+// sampling keys: (31-bit hash of (seed, row)) << 32 | row, rows with a non-finite coordinate last
+template <int D>
+__global__ void bc_sample_kernel(const float* x, int64_t ldx, int n, unsigned long long seed, unsigned long long* keys)
+{
+  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
+    bool fin = true;
+    for (int c = 0; c < D; ++c) fin = fin && isfinite(x[i * ldx + c]);
+    unsigned long long z = seed + 0x9E3779B97F4A7C15ull * (static_cast<unsigned long long>(i) + 1);   // splitmix64
+    z = (z ^ (z >> 30)) * 0xBF58476D1CE4E5B9ull;
+    z = (z ^ (z >> 27)) * 0x94D049BB133111EBull;
+    z ^= z >> 31;
+    const unsigned long long h = fin ? (z >> 33) : 0xFFFFFFFFull;
+    keys[i] = (h << 32) | static_cast<unsigned>(i);
+  }
+}
+
+// landmark j = the row of sorted key j
+template <int D>
+__global__ void bc_landmark_kernel(const float* x, int64_t ldx, const unsigned long long* keys, int nl, float* lm)
+{
+  for (int j = blockIdx.x * blockDim.x + threadIdx.x; j < nl; j += gridDim.x * blockDim.x) {
+    const int64_t row = static_cast<unsigned>(keys[j]);
+    for (int c = 0; c < D; ++c) lm[j * D + c] = x[row * ldx + c];
+  }
+}
+
+// Every finite row to its nearest finite landmark by (s, landmark): key (landmark << 32) | bits of s, value the row.
+// Rows with a non-finite coordinate get landmark nl.  Landmarks are staged in shared memory, kBcTile at a time.
+constexpr int kBcTile = 1024;
+template <int D>
+__global__ void __launch_bounds__(256) bc_assign_kernel(const float* x, int64_t ldx, int n, const float* lm, int nl,
+                                                        unsigned long long* keys, int* vals)
+{
+  __shared__ float tile[kBcTile * D];
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  float p[D];
+  bool fin = i < n;
+  for (int c = 0; c < D; ++c) {
+    p[c] = i < n ? x[static_cast<int64_t>(i) * ldx + c] : 0.f;
+    fin  = fin && isfinite(p[c]);
+  }
+  long long best = KEY_EMPTY;
+  for (int t0 = 0; t0 < nl; t0 += kBcTile) {
+    const int cnt = min(kBcTile, nl - t0);
+    __syncthreads();
+    for (int e = threadIdx.x; e < cnt * D; e += blockDim.x) tile[e] = lm[t0 * D + e];
+    __syncthreads();
+    if (fin)
+      for (int j = 0; j < cnt; ++j) {
+        const float* L = tile + j * D;
+        bool lf = true;
+        for (int c = 0; c < D; ++c) lf = lf && isfinite(L[c]);
+        if (lf) best = min(best, key_pack(bc_s<D>(p, L), t0 + j));
+      }
+  }
+  if (i < n) {
+    const unsigned long long lab = fin ? static_cast<unsigned long long>(key_index(best)) : static_cast<unsigned long long>(nl);
+    const unsigned sb            = fin ? static_cast<unsigned>(best >> 32) : 0u;   // s >= 0: its ordered bits are its bits
+    keys[i] = (lab << 32) | sb;
+    vals[i] = i;
+  }
+}
+
+// ball offsets from the sorted keys: off[l] = first position whose landmark is >= l, l in [0, nl + 1]
+__global__ void bc_offsets_kernel(const unsigned long long* keys, int n, int nl, int* off)
+{
+  for (int t = blockIdx.x * blockDim.x + threadIdx.x; t <= n; t += gridDim.x * blockDim.x) {
+    const int prev = t > 0 ? static_cast<int>(keys[t - 1] >> 32) : -1;
+    const int cur  = t < n ? static_cast<int>(keys[t] >> 32) : nl + 1;
+    for (int l = prev + 1; l <= cur; ++l) off[l] = t;
+  }
+}
+
+// the rows in position order: coordinates, caller's row, s to the landmark
+template <int D>
+__global__ void bc_permute_kernel(const float* x, int64_t ldx, const unsigned long long* keys, const int* perm, int n,
+                                  float* pts, int* ids, float* rl)
+{
+  for (int t = blockIdx.x * blockDim.x + threadIdx.x; t < n; t += gridDim.x * blockDim.x) {
+    const int row = perm[t];
+    for (int c = 0; c < D; ++c) pts[static_cast<int64_t>(t) * D + c] = x[static_cast<int64_t>(row) * ldx + c];
+    ids[t] = row;
+    rl[t]  = __uint_as_float(static_cast<unsigned>(keys[t]));
+  }
+}
+
+__global__ void bc_radius_kernel(const int* off, const float* rl, int nl, float* rhi)
+{
+  for (int j = blockIdx.x * blockDim.x + threadIdx.x; j < nl; j += gridDim.x * blockDim.x)
+    rhi[j] = off[j + 1] > off[j] ? bc_dhi(rl[off[j + 1] - 1]) : -1.f;
+}
+
+// ------------------------------------------------------------------------------------------
+// queries
+
+// The landmarks and their rhi in shared memory when they fit (smem), else read where they are.
+template <int D>
+__device__ __forceinline__ void bc_stage(const BcIndex& ix, int nl, bool smem, const float** lm, const float** rhi)
+{
+  extern __shared__ float bc_sm[];
+  *lm  = ix.lm;
+  *rhi = ix.rhi;
+  if (!smem) return;
+  for (int e = threadIdx.x; e < nl * D; e += blockDim.x) bc_sm[e] = ix.lm[e];
+  for (int e = threadIdx.x; e < nl; e += blockDim.x) bc_sm[nl * D + e] = ix.rhi[e];
+  __syncthreads();
+  *lm  = bc_sm;
+  *rhi = bc_sm + nl * D;
+}
+
+// A warp's sorted list of the 64 best keys so far: lane l holds slots l (a0) and l + 32 (a1).
+struct BcTopK {
+  long long a0 = KEY_EMPTY, a1 = KEY_EMPTY;
+
+  __device__ __forceinline__ long long slot(int j) const
+  {
+    return j < 32 ? __shfl_sync(0xffffffffu, a0, j) : __shfl_sync(0xffffffffu, a1, j - 32);
+  }
+  // insert c (warp-uniform, not in the list): every slot at or after c's place takes its predecessor
+  __device__ __forceinline__ void insert(long long c, int lane)
+  {
+    long long u0       = __shfl_up_sync(0xffffffffu, a0, 1);
+    long long u1       = __shfl_up_sync(0xffffffffu, a1, 1);
+    const long long l0 = __shfl_sync(0xffffffffu, a0, 31);
+    if (lane == 0) { u0 = KEY_EMPTY; u1 = l0; }
+    const bool first0 = lane == 0 || u0 < c;
+    a0 = a0 < c ? a0 : (first0 ? c : u0);
+    a1 = a1 < c ? a1 : (u1 < c ? c : u1);
+  }
+};
+
+// The kNN state of one query: the list, its k-th key and the distance bound that k-th key gives.
+struct BcKnn {
+  BcTopK list;
+  long long kth = KEY_EMPTY;
+  float dmax    = BC_INF;
+};
+
+// Scans the members [lo, hi) of one ball (or the non-finite rows, sq = 0: nothing is pruned there) into the list.
+template <int D>
+__device__ __forceinline__ void bc_knn_ball(const BcIndex& ix, int lo, int hi, float sq, const float* q, int k, int root,
+                                            BcKnn& st, int lane)
+{
+  float wlo, whi;
+  bc_window(sq, st.dmax, &wlo, &whi);
+  for (int p = bc_search(ix.rl, lo, hi, wlo, false); p < hi; p += 32) {
+    const int i    = p + lane;
+    const float r  = i < hi ? ix.rl[i] : BC_INF;
+    const bool out = i < hi && r > whi;
+    long long key  = KEY_EMPTY;
+    if (i < hi && !out && r >= wlo) {
+      const float s = bc_s<D>(q, ix.pts + static_cast<int64_t>(i) * D);
+      const float f = root ? __fsqrt_rn(s) : s;
+      if (f == f) key = key_pack(f, ix.ids[i]);
+    }
+    unsigned mask = __ballot_sync(0xffffffffu, key < st.kth);
+    if (mask) {
+      do {
+        const int src     = __ffs(mask) - 1;
+        mask             &= mask - 1;
+        const long long c = __shfl_sync(0xffffffffu, key, src);
+        if (c < st.kth) {
+          st.list.insert(c, lane);
+          st.kth = st.list.slot(k - 1);
+        }
+      } while (mask);
+      if (st.kth != KEY_EMPTY) {
+        st.dmax = bc_dmax(key_dist(st.kth), root);
+        bc_window(sq, st.dmax, &wlo, &whi);
+      }
+    }
+    if (__any_sync(0xffffffffu, out)) break;
+  }
+}
+
+// One warp per query: the nearest ball first, then every ball the bound does not rule out, then the non-finite rows.
+template <int D>
+__global__ void __launch_bounds__(kBcWarps * 32) bc_knn_kernel(BcIndex ix, int n, int nl, int root, const float* qs,
+                                                               int64_t ldq, int m, int k, int64_t* out_idx,
+                                                               float* out_dist, int smem)
+{
+  const float *lm, *rhi;
+  bc_stage<D>(ix, nl, smem, &lm, &rhi);
+  const int lane = threadIdx.x & 31;
+  const int qi   = blockIdx.x * kBcWarps + (threadIdx.x >> 5);
+  if (qi >= m) return;
+  float q[D];
+  bool nan = false;
+  for (int c = 0; c < D; ++c) {
+    q[c] = qs[static_cast<int64_t>(qi) * ldq + c];
+    nan  = nan || isnan(q[c]);
+  }
+  BcKnn st;
+  if (!nan) {
+    long long best = KEY_EMPTY;
+    for (int j = lane; j < nl; j += 32)
+      if (rhi[j] >= 0.f) best = min(best, key_pack(bc_s<D>(q, lm + j * D), j));
+    for (int o = 16; o > 0; o >>= 1) best = min(best, __shfl_xor_sync(0xffffffffu, best, o));
+    const int b0 = best == KEY_EMPTY ? -1 : static_cast<int>(key_index(best));
+    if (b0 >= 0) bc_knn_ball<D>(ix, ix.off[b0], ix.off[b0 + 1], key_dist(best), q, k, root, st, lane);
+    for (int base = 0; base < nl; base += 32) {
+      const int j = base + lane;
+      float s     = 0.f;
+      bool want   = false;
+      if (j < nl && j != b0 && rhi[j] >= 0.f) {
+        s    = bc_s<D>(q, lm + j * D);
+        want = !bc_ball_out(s, rhi[j], st.dmax);
+      }
+      unsigned mask = __ballot_sync(0xffffffffu, want);
+      while (mask) {
+        const int src  = __ffs(mask) - 1;
+        mask          &= mask - 1;
+        const float sj = __shfl_sync(0xffffffffu, s, src);
+        const int b    = base + src;
+        if (!bc_ball_out(sj, rhi[b], st.dmax)) bc_knn_ball<D>(ix, ix.off[b], ix.off[b + 1], sj, q, k, root, st, lane);
+      }
+    }
+    bc_knn_ball<D>(ix, ix.off[nl], n, 0.f, q, k, root, st, lane);
+  }
+  for (int j = lane; j < k; j += 32) {
+    const long long key = j < 32 ? st.list.a0 : st.list.a1;
+    const int64_t o     = static_cast<int64_t>(qi) * k + j;
+    out_idx[o]          = key == KEY_EMPTY ? -1 : key_index(key);
+    out_dist[o]         = key == KEY_EMPTY ? BC_INF : key_dist(key);
+  }
+}
+
+// Epsilon queries, one warp per query: every ball the bound does not rule out, the member window by binary search, then
+// the non-finite rows.  Count (keys == nullptr): indptr[qi + 1] = the query's pairs (indptr[0] = 0).  Fill: the pairs as
+// packed keys into keys[indptr[qi], min(indptr[qi + 1], nnz)).
+template <int D>
+__global__ void __launch_bounds__(kBcWarps * 32) bc_eps_kernel(BcIndex ix, int n, int nl, int root, const float* qs,
+                                                               int64_t ldq, int m, float eps, int64_t* indptr,
+                                                               long long* keys, int64_t nnz, int smem)
+{
+  const float *lm, *rhi;
+  bc_stage<D>(ix, nl, smem, &lm, &rhi);
+  const int lane = threadIdx.x & 31;
+  const int qi   = blockIdx.x * kBcWarps + (threadIdx.x >> 5);
+  if (qi >= m) return;
+  float q[D];
+  bool nan = false;
+  for (int c = 0; c < D; ++c) {
+    q[c] = qs[static_cast<int64_t>(qi) * ldq + c];
+    nan  = nan || isnan(q[c]);
+  }
+  int64_t at = 0, end = 0;
+  if (keys) {
+    at  = indptr[qi];
+    end = min(indptr[qi + 1], nnz);
+  }
+  int64_t cnt      = 0;
+  const float dmax = bc_dmax(eps, root);
+  // the pairs among positions [lo, hi) of a ball at s = sq from the query
+  auto scan = [&](int lo, int hi, float sq) {
+    float wlo, whi;
+    bc_window(sq, dmax, &wlo, &whi);
+    lo = bc_search(ix.rl, lo, hi, wlo, false);
+    hi = bc_search(ix.rl, lo, hi, whi, true);
+    for (int p = lo; p < hi; p += 32) {
+      const int i = p + lane;
+      float f     = BC_INF;
+      bool hit    = false;
+      if (i < hi) {
+        const float s = bc_s<D>(q, ix.pts + static_cast<int64_t>(i) * D);
+        f             = root ? __fsqrt_rn(s) : s;
+        hit           = f <= eps;
+      }
+      const unsigned mask = __ballot_sync(0xffffffffu, hit);
+      if (keys) {
+        const int64_t e = at + cnt + __popc(mask & ((1u << lane) - 1u));
+        if (hit && e < end) keys[e] = key_pack(f, ix.ids[i]);
+      }
+      cnt += __popc(mask);
+    }
+  };
+  if (!nan) {
+    for (int base = 0; base < nl; base += 32) {
+      const int j = base + lane;
+      float s     = 0.f;
+      bool want   = false;
+      if (j < nl && rhi[j] >= 0.f) {
+        s    = bc_s<D>(q, lm + j * D);
+        want = !bc_ball_out(s, rhi[j], dmax);
+      }
+      unsigned mask = __ballot_sync(0xffffffffu, want);
+      while (mask) {
+        const int src  = __ffs(mask) - 1;
+        mask          &= mask - 1;
+        const int b    = base + src;
+        scan(ix.off[b], ix.off[b + 1], __shfl_sync(0xffffffffu, s, src));
+      }
+    }
+    scan(ix.off[nl], n, 0.f);
+  }
+  if (!keys && lane == 0) {
+    indptr[qi + 1] = cnt;
+    if (qi == 0) indptr[0] = 0;
+  }
+}
+
+}  // namespace b2d

@@ -276,6 +276,17 @@ void km_par_take(cudaStream_t s, const float* x, int64_t ldx, int k, const int64
                  float* d2);
 
 // ------------------------------------------------------------------------------------------
+// radius.cu: the CSR row sort, which the ball cover's epsilon query runs too
+
+// scratch of the segmented sort below: it is given both key buffers and needs next to nothing else
+constexpr size_t kRowSortBytes = static_cast<size_t>(1) << 20;
+// The packed (distance, index) keys of CSR rows at indices[0, nnz) sorted row by row (segments clipped to the nnz slots;
+// alt: a second key buffer of nnz entries, sort_tmp: sort_bytes >= kRowSortBytes of scratch), then split into the
+// indices and distances.
+int radius_sort_split(cudaStream_t s, const int64_t* indptr, int64_t m, int64_t nnz, int64_t* indices, float* distances,
+                      long long* alt, void* sort_tmp, size_t sort_bytes);
+
+// ------------------------------------------------------------------------------------------
 // single_linkage.cu
 
 inline unsigned sl_grid(int64_t n) { return static_cast<unsigned>(std::max<int64_t>(1, (n + 255) / 256)); }

@@ -21,8 +21,7 @@ namespace {
 // The workspace of both calls: the tensor path's operands, the row degrees [m + 1] (the last one stays 0, so the exclusive
 // scan of m + 1 words ends in nnz), the fill counters [m], the sort's second key buffer [nnz] and the CUB scratch.  CUB
 // reports its scratch only with a device present, so the workspace holds a bound that the calls check at run time: the
-// scan's look-back state of at most one 16-byte word per 64 rows, and 1 MiB for the segmented sort (fill only), which is
-// given both key buffers and needs next to nothing else.
+// scan's look-back state of at most one 16-byte word per 64 rows, and kRowSortBytes for the segmented sort (fill only).
 struct RadiusLayout {
   TcWorkspace w;
   unsigned* deg;
@@ -45,7 +44,7 @@ RadiusLayout radius_layout(void* base, int64_t m, int64_t n, int64_t k, int64_t 
   L.alt        = c.take<long long>(nnz);
   L.scan_bytes = 16 * static_cast<size_t>(m / 64 + 256);
   L.scan_tmp   = c.take<char>(L.scan_bytes);
-  L.sort_bytes = nnz > 0 ? static_cast<size_t>(1) << 20 : 0;
+  L.sort_bytes = nnz > 0 ? kRowSortBytes : 0;
   L.sort_tmp   = c.take<char>(L.sort_bytes);
   L.bytes      = c.bytes;
   return L;
@@ -85,6 +84,33 @@ int radius_prep(cudaStream_t s, const RadiusLayout& L, const TcMetric& tm, const
 }
 
 }  // namespace
+
+namespace b2d {
+
+int radius_sort_split(cudaStream_t s, const int64_t* indptr, int64_t m, int64_t nnz, int64_t* indices, float* distances,
+                      long long* alt, void* sort_tmp, size_t sort_bytes)
+{
+  // every row's keys in ascending order (they are distinct: one per column), segments clipped to the nnz slots
+  cub::DoubleBuffer<long long> keys(reinterpret_cast<long long*>(indices), alt);
+  using RowIt = thrust::counting_iterator<int64_t>;
+  const thrust::transform_iterator<RadiusRowStart, RowIt, long long> begin(RowIt(0), RadiusRowStart{indptr, nnz});
+  const thrust::transform_iterator<RadiusRowStart, RowIt, long long> end(RowIt(0), RadiusRowStart{indptr + 1, nnz});
+  size_t need = 0;
+  B2D_CUDA(cub::DeviceSegmentedRadixSort::SortKeys(nullptr, need, keys, static_cast<int>(nnz), static_cast<int>(m), begin, end,
+                                                   0, 64, s));
+  if (need > sort_bytes) return fail(B2D_ERR_WORKSPACE, "internal: segmented sort scratch " + std::to_string(need) + " bytes");
+  B2D_CUDA(cub::DeviceSegmentedRadixSort::SortKeys(sort_tmp, need, keys, static_cast<int>(nnz), static_cast<int>(m), begin,
+                                                   end, 0, 64, s));
+  int sms = 0;
+  const int rc = device_sms(&sms);
+  if (rc) return rc;
+  const int64_t blocks = std::min<int64_t>((nnz + 255) / 256, static_cast<int64_t>(sms) * 8);
+  radius_split_kernel<<<static_cast<unsigned>(blocks), 256, 0, s>>>(keys.Current(), indices, distances, nnz);
+  B2D_CUDA(cudaGetLastError());
+  return B2D_OK;
+}
+
+}  // namespace b2d
 
 size_t b2d_radius_neighbors_workspace_bytes(int64_t m, int64_t n, int64_t k, int64_t nnz)
 {
@@ -163,22 +189,5 @@ int b2d_radius_neighbors_fill(void* stream, const int64_t* indptr, int64_t nnz, 
     rc = launch_tc(s, L.w, p, k, EPI_RADIUS, tm.post);
     if (rc) return rc;
   }
-  // every row's keys in ascending order (they are distinct: one per column), segments clipped to the nnz slots
-  cub::DoubleBuffer<long long> keys(reinterpret_cast<long long*>(indices), L.alt);
-  using RowIt = thrust::counting_iterator<int64_t>;
-  const thrust::transform_iterator<RadiusRowStart, RowIt, long long> begin(RowIt(0), RadiusRowStart{indptr, nnz});
-  const thrust::transform_iterator<RadiusRowStart, RowIt, long long> end(RowIt(0), RadiusRowStart{indptr + 1, nnz});
-  size_t need = 0;
-  B2D_CUDA(cub::DeviceSegmentedRadixSort::SortKeys(nullptr, need, keys, static_cast<int>(nnz), static_cast<int>(m), begin, end,
-                                                   0, 64, s));
-  if (need > L.sort_bytes) return fail(B2D_ERR_WORKSPACE, "internal: segmented sort scratch " + std::to_string(need) + " bytes");
-  B2D_CUDA(cub::DeviceSegmentedRadixSort::SortKeys(L.sort_tmp, need, keys, static_cast<int>(nnz), static_cast<int>(m), begin,
-                                                   end, 0, 64, s));
-  int sms = 0;
-  rc = device_sms(&sms);
-  if (rc) return rc;
-  const int64_t blocks = std::min<int64_t>((nnz + 255) / 256, static_cast<int64_t>(sms) * 8);
-  radius_split_kernel<<<static_cast<unsigned>(blocks), 256, 0, s>>>(keys.Current(), indices, distances, nnz);
-  B2D_CUDA(cudaGetLastError());
-  return B2D_OK;
+  return radius_sort_split(s, indptr, m, nnz, indices, distances, L.alt, L.sort_tmp, L.sort_bytes);
 }

@@ -1,5 +1,7 @@
 """Mirror of the (removed) ``pylibraft.neighbors`` entry points that sit directly behind the distance path, and
-``radius_neighbors`` and ``kernel_density``, project APIs on the same path."""
+``radius_neighbors`` and ``kernel_density``, project APIs on the same path, and ``ball_cover``, exact low-dimensional
+search by the random ball cover."""
+from . import ball_cover  # noqa: F401
 from . import brute_force  # noqa: F401
 from . import epsilon_neighborhood  # noqa: F401
 from . import radius  # noqa: F401
