@@ -558,6 +558,32 @@ int b2d_dbscan_fit(void* stream, int metric, const float* x, int64_t ldx, int64_
                    int64_t min_samples, int64_t max_bytes_per_batch, int32_t* labels /* [m] */,
                    int32_t* core_sample_indices /* [m] or NULL */, int32_t* n_clusters /* device, or NULL */,
                    void* workspace, size_t workspace_bytes);
+/* DBSCAN on the random ball cover (cuML's DBSCAN(algorithm="rbc"), EpsNnMethod::RBC) for 2-D and 3-D points: the rules of
+ * b2d_dbscan_fit on another adjacency, formed without the m x m pairs.  x:[m,d] fp32, row-major, pitch ldx >= d.
+ *   A[i, j] holds when f(x_i, x_j) <= e = fp32(eps), where f is the ball cover's pair value: s = ((q0-p0)*(q0-p0) +
+ *     (q1-p1)*(q1-p1)) + (q2-p2)*(q2-p2), every operation rounded separately, for B2D_L2Unexpanded, and sqrt(s) correctly
+ *     rounded for B2D_L2SqrtUnexpanded: the comparison of b2d_ball_cover_eps_count.  A is exactly the CSR
+ *     b2d_ball_cover_eps_count / _fill give for x against an index of x.
+ *   A is symmetric bit for bit: fl(a - b) = -fl(b - a) under round-to-nearest and the two squares are equal, so
+ *     s(i, j) = s(j, i); with the diagonal 0 (every row is its own neighbour for eps >= 0) the rules of b2d_dbscan_fit
+ *     give exactly sklearn.cluster.DBSCAN(metric="precomputed") on A.  A NaN or negative eps makes every row noise;
+ *     eps = +inf links every pair.
+ *   b2d_dbscan_fit compares the expanded form |x|^2 + |y|^2 - 2 x.y: the two fits can disagree only on pairs whose
+ *     distance lies within rounding of eps.
+ * The result does not depend on seed, n_landmarks, the device or the scheduling: the ball cover's pruning is exact, and
+ * the only atomic is the union-find's integer CAS.  The index (landmarks: n_landmarks in [0, m], 0 meaning ceil(sqrt(m)), a
+ * seeded sample of the rows) is built in the workspace; three walks over it (degrees, stopping at min_samples; links
+ * between core rows; the border rule) replace the passes over A.  Outputs as b2d_dbscan_fit.  Precondition: x finite (a
+ * non-finite x is safe, its labels are unspecified).  metric outside the two above and d outside {2, 3} are
+ * B2D_ERR_UNSUPPORTED; m >= 2^31, a negative or too large n_landmarks, min_samples < 1, ldx < d and a null x / labels are
+ * B2D_ERR_INVALID_ARG; m == 0 does nothing.  Only enqueues work (no synchronisation, no allocation), so the call can be
+ * captured in a CUDA graph.  The workspace (256-byte aligned) depends on (m, d, n_landmarks) only; the query returns
+ * SIZE_MAX for arguments the fit rejects. */
+size_t b2d_dbscan_rbc_workspace_bytes(int64_t m, int64_t d, int64_t n_landmarks);
+int b2d_dbscan_rbc_fit(void* stream, int metric, const float* x, int64_t ldx, int64_t m, int64_t d, double eps,
+                       int64_t min_samples, int64_t n_landmarks, uint64_t seed, int32_t* labels /* [m] */,
+                       int32_t* core_sample_indices /* [m] or NULL */, int32_t* n_clusters /* device, or NULL */,
+                       void* workspace, size_t workspace_bytes);
 
 /* Mean shift (sklearn.cluster.MeanShift(bandwidth = h, seeds, bin_seeding, min_bin_freq, cluster_all, max_iter).fit(x)
  * with sklearn's test dist <= h replaced by the engine's rule; a project API, no upstream signature) for fp32 x:[n,d]

@@ -9,16 +9,14 @@
 #include <cmath>
 #include <string>
 
-#include "ball_cover.cuh"
+#include "ball_cover_build.cuh"
 #include "host.cuh"
 
 using namespace b2d;
 
-namespace {
-
 constexpr size_t kBcSmemMax = 64 << 10;   // landmarks staged in shared memory up to this many bytes per block
 
-int64_t bc_landmarks(int64_t n, int64_t nl)
+int64_t b2d::bc_landmarks(int64_t n, int64_t nl)
 {
   if (nl > 0) return nl;
   int64_t r = static_cast<int64_t>(std::sqrt(static_cast<double>(n)));
@@ -27,13 +25,7 @@ int64_t bc_landmarks(int64_t n, int64_t nl)
   return r;
 }
 
-// the index's regions (256-byte aligned)
-struct BcLayout {
-  BcIndex ix;
-  size_t bytes;
-};
-
-BcLayout bc_layout(void* base, int64_t n, int64_t d, int64_t nl)
+BcLayout b2d::bc_layout(void* base, int64_t n, int64_t d, int64_t nl)
 {
   Carve c(base, 256);
   BcLayout L;
@@ -47,18 +39,7 @@ BcLayout bc_layout(void* base, int64_t n, int64_t d, int64_t nl)
   return L;
 }
 
-// The build's workspace: two key and two value buffers of the radix sorts, and their scratch.  CUB reports its scratch
-// only with a device present; the onesweep sort needs its digit counters and one 1 KiB look-back row per tile of at
-// least 256 items of a 2^28-item portion, which the bound below covers (checked at run time).
-struct BcBuildLayout {
-  unsigned long long* keys[2];
-  int* vals[2];
-  void* tmp;
-  size_t tmp_bytes;
-  size_t bytes;
-};
-
-BcBuildLayout bc_build_layout(void* base, int64_t n)
+BcBuildLayout b2d::bc_build_layout(void* base, int64_t n)
 {
   Carve c(base, 256);
   BcBuildLayout L;
@@ -69,6 +50,8 @@ BcBuildLayout bc_build_layout(void* base, int64_t n)
   L.bytes     = c.bytes;
   return L;
 }
+
+namespace {
 
 // The epsilon queries' workspace: the scan's look-back state (at most one 16-byte word per 64 rows), then, for fill,
 // the sort's second key buffer [nnz] and its scratch.
@@ -121,9 +104,9 @@ int bc_check_queries(const float* q, int64_t ldq, int64_t m, int64_t d)
 
 unsigned bc_grid(int64_t items, int sms) { return static_cast<unsigned>(std::max<int64_t>(1, std::min<int64_t>((items + 255) / 256, int64_t(sms) * 16))); }
 
-// shared memory of a query launch: the landmarks and their rhi when they fit, else 0
-template <typename Kernel>
-int bc_query_smem(Kernel kernel, int64_t nl, int64_t d, size_t* bytes)
+}  // namespace
+
+int b2d::bc_query_smem(const void* kernel, int64_t nl, int64_t d, size_t* bytes)
 {
   const size_t b = static_cast<size_t>(nl) * (d + 1) * sizeof(float);
   *bytes         = b <= kBcSmemMax ? b : 0;
@@ -132,8 +115,8 @@ int bc_query_smem(Kernel kernel, int64_t nl, int64_t d, size_t* bytes)
 }
 
 template <int D>
-int bc_build(cudaStream_t s, const BcIndex& ix, const BcBuildLayout& W, const float* x, int64_t ldx, int n, int nl,
-             uint64_t seed)
+int b2d::bc_build(cudaStream_t s, const BcIndex& ix, const BcBuildLayout& W, const float* x, int64_t ldx, int n, int nl,
+                  uint64_t seed)
 {
   int sms = 0;
   int rc  = device_sms(&sms);
@@ -168,13 +151,17 @@ int bc_build(cudaStream_t s, const BcIndex& ix, const BcBuildLayout& W, const fl
   B2D_CUDA(cudaGetLastError());
   return B2D_OK;
 }
+template int b2d::bc_build<2>(cudaStream_t, const BcIndex&, const BcBuildLayout&, const float*, int64_t, int, int, uint64_t);
+template int b2d::bc_build<3>(cudaStream_t, const BcIndex&, const BcBuildLayout&, const float*, int64_t, int, int, uint64_t);
+
+namespace {
 
 template <int D>
 int bc_knn(cudaStream_t s, const BcIndex& ix, int n, int nl, int root, const float* q, int64_t ldq, int m, int k,
            int64_t* out_idx, float* out_dist)
 {
   size_t smem = 0;
-  const int rc = bc_query_smem(bc_knn_kernel<D>, nl, D, &smem);
+  const int rc = bc_query_smem(reinterpret_cast<const void*>(bc_knn_kernel<D>), nl, D, &smem);
   if (rc) return rc;
   bc_knn_kernel<D><<<static_cast<unsigned>((m + kBcWarps - 1) / kBcWarps), kBcWarps * 32, smem, s>>>(
       ix, n, nl, root, q, ldq, m, k, out_idx, out_dist, smem > 0);
@@ -187,7 +174,7 @@ int bc_eps(cudaStream_t s, const BcIndex& ix, int n, int nl, int root, const flo
            int64_t* indptr, long long* keys, int64_t nnz)
 {
   size_t smem = 0;
-  const int rc = bc_query_smem(bc_eps_kernel<D>, nl, D, &smem);
+  const int rc = bc_query_smem(reinterpret_cast<const void*>(bc_eps_kernel<D>), nl, D, &smem);
   if (rc) return rc;
   bc_eps_kernel<D><<<static_cast<unsigned>((m + kBcWarps - 1) / kBcWarps), kBcWarps * 32, smem, s>>>(
       ix, n, nl, root, q, ldq, m, eps, indptr, keys, nnz, smem > 0);

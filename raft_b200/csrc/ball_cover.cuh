@@ -1,4 +1,5 @@
-// Kernels of the random ball cover (ball_cover.cu): exact kNN and epsilon queries for 2-D and 3-D points, SIMT.
+// Kernels of the random ball cover (ball_cover.cu): exact kNN and epsilon queries for 2-D and 3-D points, SIMT, and the
+// epsilon walk DBSCAN's ball-cover fit shares (dbscan.cuh).  The build's kernels are in ball_cover_build.cuh.
 //
 // A pair's value is fixed bit for bit: s = ((q0-p0)^2 + (q1-p1)^2) + (q2-p2)^2, every operation rounded separately
 // (bc_s), and the distance f = s (L2Unexpanded) or sqrt(s) (L2SqrtUnexpanded).  The queries prune whole balls and ball
@@ -12,20 +13,10 @@
 #include <cuda_runtime.h>
 #include <cstdint>
 
+#include "ball_cover_types.cuh"
 #include "nn_key.cuh"
 
 namespace b2d {
-
-// The index, one caller-owned buffer (its regions: bc_index in ball_cover.cu).  Positions are the rows sorted by
-// (ball, s to the ball's landmark, row); rows with a non-finite coordinate follow the last ball.
-struct BcIndex {
-  float* lm;    // [nl][d] landmark coordinates
-  float* rhi;   // [nl] bc_dhi of the ball's largest member s: an upper bound of its true radius; -1: empty ball
-  int* off;     // [nl + 2] ball b holds positions [off[b], off[b + 1]); [off[nl], off[nl + 1] = n) the non-finite rows
-  float* pts;   // [n][d] coordinates by position
-  int* ids;     // [n] the caller's row at each position
-  float* rl;    // [n] s(landmark, row), ascending inside each ball (0 for the non-finite rows)
-};
 
 constexpr int kBcWarps = 8;   // queries per block of the query kernels (one warp each)
 
@@ -86,101 +77,6 @@ __device__ __forceinline__ int bc_search(const float* rl, int lo, int hi, float 
     else hi = mid;
   }
   return lo;
-}
-
-// ------------------------------------------------------------------------------------------
-// build
-
-// sampling keys: (31-bit hash of (seed, row)) << 32 | row, rows with a non-finite coordinate last
-template <int D>
-__global__ void bc_sample_kernel(const float* x, int64_t ldx, int n, unsigned long long seed, unsigned long long* keys)
-{
-  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
-    bool fin = true;
-    for (int c = 0; c < D; ++c) fin = fin && isfinite(x[i * ldx + c]);
-    unsigned long long z = seed + 0x9E3779B97F4A7C15ull * (static_cast<unsigned long long>(i) + 1);   // splitmix64
-    z = (z ^ (z >> 30)) * 0xBF58476D1CE4E5B9ull;
-    z = (z ^ (z >> 27)) * 0x94D049BB133111EBull;
-    z ^= z >> 31;
-    const unsigned long long h = fin ? (z >> 33) : 0xFFFFFFFFull;
-    keys[i] = (h << 32) | static_cast<unsigned>(i);
-  }
-}
-
-// landmark j = the row of sorted key j
-template <int D>
-__global__ void bc_landmark_kernel(const float* x, int64_t ldx, const unsigned long long* keys, int nl, float* lm)
-{
-  for (int j = blockIdx.x * blockDim.x + threadIdx.x; j < nl; j += gridDim.x * blockDim.x) {
-    const int64_t row = static_cast<unsigned>(keys[j]);
-    for (int c = 0; c < D; ++c) lm[j * D + c] = x[row * ldx + c];
-  }
-}
-
-// Every finite row to its nearest finite landmark by (s, landmark): key (landmark << 32) | bits of s, value the row.
-// Rows with a non-finite coordinate get landmark nl.  Landmarks are staged in shared memory, kBcTile at a time.
-constexpr int kBcTile = 1024;
-template <int D>
-__global__ void __launch_bounds__(256) bc_assign_kernel(const float* x, int64_t ldx, int n, const float* lm, int nl,
-                                                        unsigned long long* keys, int* vals)
-{
-  __shared__ float tile[kBcTile * D];
-  const int i = blockIdx.x * blockDim.x + threadIdx.x;
-  float p[D];
-  bool fin = i < n;
-  for (int c = 0; c < D; ++c) {
-    p[c] = i < n ? x[static_cast<int64_t>(i) * ldx + c] : 0.f;
-    fin  = fin && isfinite(p[c]);
-  }
-  long long best = KEY_EMPTY;
-  for (int t0 = 0; t0 < nl; t0 += kBcTile) {
-    const int cnt = min(kBcTile, nl - t0);
-    __syncthreads();
-    for (int e = threadIdx.x; e < cnt * D; e += blockDim.x) tile[e] = lm[t0 * D + e];
-    __syncthreads();
-    if (fin)
-      for (int j = 0; j < cnt; ++j) {
-        const float* L = tile + j * D;
-        bool lf = true;
-        for (int c = 0; c < D; ++c) lf = lf && isfinite(L[c]);
-        if (lf) best = min(best, key_pack(bc_s<D>(p, L), t0 + j));
-      }
-  }
-  if (i < n) {
-    const unsigned long long lab = fin ? static_cast<unsigned long long>(key_index(best)) : static_cast<unsigned long long>(nl);
-    const unsigned sb            = fin ? static_cast<unsigned>(best >> 32) : 0u;   // s >= 0: its ordered bits are its bits
-    keys[i] = (lab << 32) | sb;
-    vals[i] = i;
-  }
-}
-
-// ball offsets from the sorted keys: off[l] = first position whose landmark is >= l, l in [0, nl + 1]
-__global__ void bc_offsets_kernel(const unsigned long long* keys, int n, int nl, int* off)
-{
-  for (int t = blockIdx.x * blockDim.x + threadIdx.x; t <= n; t += gridDim.x * blockDim.x) {
-    const int prev = t > 0 ? static_cast<int>(keys[t - 1] >> 32) : -1;
-    const int cur  = t < n ? static_cast<int>(keys[t] >> 32) : nl + 1;
-    for (int l = prev + 1; l <= cur; ++l) off[l] = t;
-  }
-}
-
-// the rows in position order: coordinates, caller's row, s to the landmark
-template <int D>
-__global__ void bc_permute_kernel(const float* x, int64_t ldx, const unsigned long long* keys, const int* perm, int n,
-                                  float* pts, int* ids, float* rl)
-{
-  for (int t = blockIdx.x * blockDim.x + threadIdx.x; t < n; t += gridDim.x * blockDim.x) {
-    const int row = perm[t];
-    for (int c = 0; c < D; ++c) pts[static_cast<int64_t>(t) * D + c] = x[static_cast<int64_t>(row) * ldx + c];
-    ids[t] = row;
-    rl[t]  = __uint_as_float(static_cast<unsigned>(keys[t]));
-  }
-}
-
-__global__ void bc_radius_kernel(const int* off, const float* rl, int nl, float* rhi)
-{
-  for (int j = blockIdx.x * blockDim.x + threadIdx.x; j < nl; j += gridDim.x * blockDim.x)
-    rhi[j] = off[j + 1] > off[j] ? bc_dhi(rl[off[j + 1] - 1]) : -1.f;
 }
 
 // ------------------------------------------------------------------------------------------
@@ -318,9 +214,56 @@ __global__ void __launch_bounds__(kBcWarps * 32) bc_knn_kernel(BcIndex ix, int n
   }
 }
 
-// Epsilon queries, one warp per query: every ball the bound does not rule out, the member window by binary search, then
-// the non-finite rows.  Count (keys == nullptr): indptr[qi + 1] = the query's pairs (indptr[0] = 0).  Fill: the pairs as
-// packed keys into keys[indptr[qi], min(indptr[qi + 1], nnz)).
+// The epsilon walk of one query q (not NaN) of a warp: every ball the bound does not rule out, the member window by
+// binary search, then the non-finite rows.  Every step of 32 positions calls act(i, f, hit) on all lanes: i = the lane's
+// position, f = its distance and hit = (f <= eps) for a position inside the window, else hit = false.  act returns true
+// (the same on every lane) to end the walk there.  The epsilon queries and DBSCAN's walks (dbscan.cuh) share it, so the
+// pruning and its margin have one definition.
+template <int D, typename Act>
+__device__ __forceinline__ void bc_eps_walk(const BcIndex& ix, int n, int nl, const float* lm, const float* rhi,
+                                            const float* q, int root, float eps, int lane, Act&& act)
+{
+  const float dmax = bc_dmax(eps, root);
+  // the positions [lo, hi) of a ball at s = sq from the query; true: the walk ends
+  auto scan = [&](int lo, int hi, float sq) {
+    float wlo, whi;
+    bc_window(sq, dmax, &wlo, &whi);
+    lo = bc_search(ix.rl, lo, hi, wlo, false);
+    hi = bc_search(ix.rl, lo, hi, whi, true);
+    for (int p = lo; p < hi; p += 32) {
+      const int i = p + lane;
+      float f     = BC_INF;
+      bool hit    = false;
+      if (i < hi) {
+        const float s = bc_s<D>(q, ix.pts + static_cast<int64_t>(i) * D);
+        f             = root ? __fsqrt_rn(s) : s;
+        hit           = f <= eps;
+      }
+      if (act(i, f, hit)) return true;
+    }
+    return false;
+  };
+  for (int base = 0; base < nl; base += 32) {
+    const int j = base + lane;
+    float s     = 0.f;
+    bool want   = false;
+    if (j < nl && rhi[j] >= 0.f) {
+      s    = bc_s<D>(q, lm + j * D);
+      want = !bc_ball_out(s, rhi[j], dmax);
+    }
+    unsigned mask = __ballot_sync(0xffffffffu, want);
+    while (mask) {
+      const int src  = __ffs(mask) - 1;
+      mask          &= mask - 1;
+      const int b    = base + src;
+      if (scan(ix.off[b], ix.off[b + 1], __shfl_sync(0xffffffffu, s, src))) return;
+    }
+  }
+  scan(ix.off[nl], n, 0.f);
+}
+
+// Epsilon queries, one warp per query, by bc_eps_walk.  Count (keys == nullptr): indptr[qi + 1] = the query's pairs
+// (indptr[0] = 0).  Fill: the pairs as packed keys into keys[indptr[qi], min(indptr[qi + 1], nnz)).
 template <int D>
 __global__ void __launch_bounds__(kBcWarps * 32) bc_eps_kernel(BcIndex ix, int n, int nl, int root, const float* qs,
                                                                int64_t ldq, int m, float eps, int64_t* indptr,
@@ -342,50 +285,17 @@ __global__ void __launch_bounds__(kBcWarps * 32) bc_eps_kernel(BcIndex ix, int n
     at  = indptr[qi];
     end = min(indptr[qi + 1], nnz);
   }
-  int64_t cnt      = 0;
-  const float dmax = bc_dmax(eps, root);
-  // the pairs among positions [lo, hi) of a ball at s = sq from the query
-  auto scan = [&](int lo, int hi, float sq) {
-    float wlo, whi;
-    bc_window(sq, dmax, &wlo, &whi);
-    lo = bc_search(ix.rl, lo, hi, wlo, false);
-    hi = bc_search(ix.rl, lo, hi, whi, true);
-    for (int p = lo; p < hi; p += 32) {
-      const int i = p + lane;
-      float f     = BC_INF;
-      bool hit    = false;
-      if (i < hi) {
-        const float s = bc_s<D>(q, ix.pts + static_cast<int64_t>(i) * D);
-        f             = root ? __fsqrt_rn(s) : s;
-        hit           = f <= eps;
-      }
+  int64_t cnt = 0;
+  if (!nan)
+    bc_eps_walk<D>(ix, n, nl, lm, rhi, q, root, eps, lane, [&](int i, float f, bool hit) {
       const unsigned mask = __ballot_sync(0xffffffffu, hit);
       if (keys) {
         const int64_t e = at + cnt + __popc(mask & ((1u << lane) - 1u));
         if (hit && e < end) keys[e] = key_pack(f, ix.ids[i]);
       }
       cnt += __popc(mask);
-    }
-  };
-  if (!nan) {
-    for (int base = 0; base < nl; base += 32) {
-      const int j = base + lane;
-      float s     = 0.f;
-      bool want   = false;
-      if (j < nl && rhi[j] >= 0.f) {
-        s    = bc_s<D>(q, lm + j * D);
-        want = !bc_ball_out(s, rhi[j], dmax);
-      }
-      unsigned mask = __ballot_sync(0xffffffffu, want);
-      while (mask) {
-        const int src  = __ffs(mask) - 1;
-        mask          &= mask - 1;
-        const int b    = base + src;
-        scan(ix.off[b], ix.off[b + 1], __shfl_sync(0xffffffffu, s, src));
-      }
-    }
-    scan(ix.off[nl], n, 0.f);
-  }
+      return false;
+    });
   if (!keys && lane == 0) {
     indptr[qi + 1] = cnt;
     if (qi == 0) indptr[0] = 0;

@@ -1,7 +1,8 @@
-// DBSCAN (dbscan.cuh) on the epsilon neighbourhood of the tensor path.
+// DBSCAN (dbscan.cuh) on the epsilon neighbourhood of the tensor path, and on the random ball cover for 2-D and 3-D points.
 #include <cuda_runtime.h>
 #include <algorithm>
 #include <cmath>
+#include <string>
 
 #include "host.cuh"
 #include "dbscan.cuh"
@@ -137,6 +138,133 @@ int b2d_dbscan_fit(void* stream, int metric, const float* x, int64_t ldx, int64_
     db_border_kernel<<<db_warp_grid(m), kDbThreads, 0, s>>>(L.adj, L.ld, m, c0, w, L.parent, L.border);
     B2D_CUDA(cudaGetLastError());
   }
+  // 4. cluster numbers = ranks of the roots; core_sample_indices positions = ranks of the core rows
+  rc = km_scan(s, nullptr, L.root, m, L.tiles, L.ctrl);
+  if (rc) return rc;
+  rc = km_scan(s, nullptr, L.core, m, L.tiles, L.ctrl + 1);
+  if (rc) return rc;
+  db_label_kernel<<<sl_grid(m), 256, 0, s>>>(L.parent, L.border, L.root, L.core, m, &L.ctrl[0].total, &L.ctrl[1].total,
+                                             labels, core_sample_indices, n_clusters);
+  B2D_CUDA(cudaGetLastError());
+  return B2D_OK;
+}
+
+// ------------------------------------------------------------------------------------------
+// DBSCAN on the random ball cover (dbscan.cuh, db_rbc_*): the index of x, then the degree, link and border walks over it.
+// Only enqueues work.
+namespace {
+
+// The index, then the build's scratch, which is dead once the index is built: the fit's arrays overlap it.
+struct DbRbcLayout {
+  BcIndex ix;
+  BcBuildLayout build;
+  unsigned* deg;     // [m] hits per row, up to min_samples
+  int* parent;       // [m] union-find forest over the core rows (-1: not core)
+  int* border;       // [m] smallest root reaching a non-core row (INT_MAX: none)
+  unsigned* root;    // [m] root flags, scanned into cluster numbers
+  unsigned* core;    // [m] core flags, scanned into core_sample_indices positions
+  unsigned* tiles;   // scan tile sums
+  KmCtrl* ctrl;      // [2] scan totals: clusters, core rows
+  size_t bytes;
+};
+
+static DbRbcLayout db_rbc_layout(void* base, int64_t m, int64_t d, int64_t nl)
+{
+  DbRbcLayout L{};
+  const BcLayout I = bc_layout(base, m, d, nl);
+  L.ix             = I.ix;
+  char* rest       = base ? static_cast<char*>(base) + I.bytes : nullptr;   // I.bytes is a multiple of 256
+  L.build          = bc_build_layout(rest, m);
+  Carve c(rest, 256);
+  L.deg    = c.take<unsigned>(m);
+  L.parent = c.take<int>(m);
+  L.border = c.take<int>(m);
+  L.root   = c.take<unsigned>(m);
+  L.core   = c.take<unsigned>(m);
+  L.tiles  = c.take<unsigned>((m + kKmScanTile - 1) / kKmScanTile);
+  L.ctrl   = c.take<KmCtrl>(2);
+  L.bytes  = I.bytes + std::max(L.build.bytes, c.bytes);
+  return L;
+}
+
+// one warp-per-position walk over the index, with the landmarks staged when they fit
+template <typename Kernel, typename... Args>
+static int db_rbc_walk(cudaStream_t s, Kernel kernel, int64_t m, int64_t d, int64_t nl, Args... args)
+{
+  size_t smem = 0;
+  const int rc = bc_query_smem(reinterpret_cast<const void*>(kernel), nl, d, &smem);
+  if (rc) return rc;
+  kernel<<<static_cast<unsigned>((m + kBcWarps - 1) / kBcWarps), kBcWarps * 32, smem, s>>>(args..., smem > 0);
+  B2D_CUDA(cudaGetLastError());
+  return B2D_OK;
+}
+
+template <int D>
+static int db_rbc_fit(cudaStream_t s, const DbRbcLayout& L, int root, const float* x, int64_t ldx, int n, int nl, float e,
+                      unsigned ms, uint64_t seed)
+{
+  // 0. the index of x
+  int rc = bc_build<D>(s, L.ix, L.build, x, ldx, n, nl, seed);
+  if (rc) return rc;
+  // 1. degrees, then the core flags; a NaN or negative eps matches nothing
+  if (e >= 0.f) {
+    rc = db_rbc_walk(s, db_rbc_degree_kernel<D>, n, D, nl, L.ix, n, nl, root, e, ms, L.deg);
+    if (rc) return rc;
+  } else {
+    B2D_CUDA(cudaMemsetAsync(L.deg, 0, static_cast<size_t>(n) * sizeof(unsigned), s));
+  }
+  db_core_kernel<<<sl_grid(n), 256, 0, s>>>(L.deg, n, n, ms, L.parent, L.border, L.core);
+  B2D_CUDA(cudaGetLastError());
+  // 2. links between core points; 3. border points (no core point without a hit)
+  if (e >= 0.f) {
+    rc = db_rbc_walk(s, db_rbc_link_kernel<D>, n, D, nl, L.ix, n, nl, root, e, static_cast<const unsigned*>(L.core),
+                     L.parent);
+    if (rc) return rc;
+  }
+  db_rbc_compress_kernel<<<sl_grid(n), 256, 0, s>>>(L.parent, n, L.root);
+  B2D_CUDA(cudaGetLastError());
+  if (e >= 0.f) {
+    rc = db_rbc_walk(s, db_rbc_border_kernel<D>, n, D, nl, L.ix, n, nl, root, e, static_cast<const int*>(L.parent),
+                     L.border);
+    if (rc) return rc;
+  }
+  return B2D_OK;
+}
+}  // namespace
+
+size_t b2d_dbscan_rbc_workspace_bytes(int64_t m, int64_t d, int64_t n_landmarks)
+{
+  if (m < 0 || m > 0x7fffffffll || (d != 2 && d != 3) || n_landmarks < 0 || n_landmarks > m) return static_cast<size_t>(-1);
+  return db_rbc_layout(nullptr, m, d, bc_landmarks(m, n_landmarks)).bytes;
+}
+
+int b2d_dbscan_rbc_fit(void* stream, int metric, const float* x, int64_t ldx, int64_t m, int64_t d, double eps,
+                       int64_t min_samples, int64_t n_landmarks, uint64_t seed, int32_t* labels,
+                       int32_t* core_sample_indices, int32_t* n_clusters, void* workspace, size_t workspace_bytes)
+{
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  if (metric != B2D_L2Unexpanded && metric != B2D_L2SqrtUnexpanded)
+    return fail(B2D_ERR_UNSUPPORTED, "dbscan rbc supports the L2Unexpanded and L2SqrtUnexpanded metrics, got metric " +
+                                         std::to_string(metric));
+  if (m < 0 || n_landmarks < 0) return fail(B2D_ERR_INVALID_ARG, "negative extent or n_landmarks");
+  if (m == 0) return B2D_OK;
+  if (m > 0x7fffffffll) return fail(B2D_ERR_INVALID_ARG, "dbscan: m must be below 2^31");
+  if (d != 2 && d != 3) return fail(B2D_ERR_UNSUPPORTED, "dbscan rbc supports d = 2 and d = 3, got d = " + std::to_string(d));
+  if (n_landmarks > m) return fail(B2D_ERR_INVALID_ARG, "n_landmarks must be in [0, m] (0: ceil(sqrt(m)))");
+  if (min_samples < 1) return fail(B2D_ERR_INVALID_ARG, "min_samples must be >= 1");
+  if (!x || !labels) return fail(B2D_ERR_INVALID_ARG, "null x / labels");
+  if (ldx < d) return fail(B2D_ERR_INVALID_ARG, "leading dimension smaller than d");
+  const int64_t nl = bc_landmarks(m, n_landmarks);
+  int rc           = check_workspace(workspace, workspace_bytes, db_rbc_layout(nullptr, m, d, nl).bytes);
+  if (rc) return rc;
+  const DbRbcLayout L = db_rbc_layout(workspace, m, d, nl);
+  // the ball cover's comparison: f <= fp32(eps) with f = s or sqrt(s) (a NaN or negative eps matches nothing)
+  const float e     = static_cast<float>(eps);
+  const unsigned ms = static_cast<unsigned>(std::min<int64_t>(min_samples, m + 1));
+  const int root    = metric == B2D_L2SqrtUnexpanded;
+  rc = d == 2 ? db_rbc_fit<2>(s, L, root, x, ldx, static_cast<int>(m), static_cast<int>(nl), e, ms, seed)
+              : db_rbc_fit<3>(s, L, root, x, ldx, static_cast<int>(m), static_cast<int>(nl), e, ms, seed);
+  if (rc) return rc;
   // 4. cluster numbers = ranks of the roots; core_sample_indices positions = ranks of the core rows
   rc = km_scan(s, nullptr, L.root, m, L.tiles, L.ctrl);
   if (rc) return rc;

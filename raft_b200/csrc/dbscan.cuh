@@ -9,10 +9,13 @@
 //   db_label_kernel     labels, core_sample_indices and n_clusters from the two scanned flag arrays
 // The union hooks the larger root under the smaller (CAS on parent), so the root of a component is its smallest core
 // row whatever the interleaving; every atomic is an integer CAS or atomicMin, and the results do not depend on order.
+// The ball-cover fit's three walks (db_rbc_*) take the place of the EPI_EPS batches for 2-D and 3-D points.
 #pragma once
 #include <cuda_runtime.h>
 #include <climits>
 #include <cstdint>
+
+#include "ball_cover.cuh"
 
 namespace b2d {
 
@@ -138,6 +141,127 @@ __global__ void __launch_bounds__(kDbThreads) db_border_kernel(const uint8_t* ad
     if (lane == 0 && best != INT_MAX) atomicMin(&border[i], best);
   }
 }
+
+// ------------------------------------------------------------------------------------------
+// The ball-cover fit (b2d_dbscan_rbc_fit, DESIGN.md K20): A from the ball cover's epsilon walk (bc_eps_walk) over the
+// index of x itself.  One warp per position t of the index, whose point is ix.pts[t] and caller row ix.ids[t]: warps next
+// to each other walk the same balls, and x is not read again.  A is symmetric bit for bit, so a row's hits are its
+// column's too.
+//   db_rbc_degree_kernel    deg[i] = the hits of row i, the walk ending once min_samples is reached
+//   db_rbc_link_kernel      core rows: every core hit j < i unites the trees of i and j
+//   db_rbc_compress_kernel  parent[i] = root of i, root flags, with a find that only reads
+//   db_rbc_border_kernel    non-core rows: border[i] = the smallest root (parent, compressed) among the core hits
+// The core flags and the labels are db_core_kernel (b = m) and db_label_kernel.
+
+// the point and caller row of position t; false: a NaN coordinate (the point is nobody's neighbour)
+template <int D>
+__device__ __forceinline__ bool db_rbc_query(const BcIndex& ix, int t, float (&q)[D], int* row)
+{
+  bool nan = false;
+  for (int c = 0; c < D; ++c) {
+    q[c] = ix.pts[static_cast<int64_t>(t) * D + c];
+    nan  = nan || isnan(q[c]);
+  }
+  *row = ix.ids[t];
+  return !nan;
+}
+
+template <int D>
+__global__ void __launch_bounds__(kBcWarps * 32) db_rbc_degree_kernel(BcIndex ix, int n, int nl, int root, float eps,
+                                                                      unsigned min_samples, unsigned* deg, int smem)
+{
+  const float *lm, *rhi;
+  bc_stage<D>(ix, nl, smem, &lm, &rhi);
+  const int lane = threadIdx.x & 31;
+  const int t    = blockIdx.x * kBcWarps + (threadIdx.x >> 5);
+  if (t >= n) return;
+  float q[D];
+  int row;
+  unsigned cnt = 0;
+  if (db_rbc_query<D>(ix, t, q, &row))
+    bc_eps_walk<D>(ix, n, nl, lm, rhi, q, root, eps, lane, [&](int, float, bool hit) {
+      cnt += __popc(__ballot_sync(0xffffffffu, hit));
+      return cnt >= min_samples;   // only the core test reads the degree
+    });
+  if (lane == 0) deg[row] = cnt;
+}
+
+// One find per hit, and no atomic for a hit already in the row's tree; each lane keeps the row's root between its hits,
+// as db_link_kernel does.  Only hits below the row: A is symmetric, so the larger end of every core pair takes it.
+template <int D>
+__global__ void __launch_bounds__(kBcWarps * 32) db_rbc_link_kernel(BcIndex ix, int n, int nl, int root, float eps,
+                                                                    const unsigned* core, int* parent, int smem)
+{
+  const float *lm, *rhi;
+  bc_stage<D>(ix, nl, smem, &lm, &rhi);
+  const int lane = threadIdx.x & 31;
+  const int t    = blockIdx.x * kBcWarps + (threadIdx.x >> 5);
+  if (t >= n) return;
+  float q[D];
+  int row;
+  if (!db_rbc_query<D>(ix, t, q, &row) || __ldg(&core[row]) == 0u) return;
+  int ri = -1;
+  bc_eps_walk<D>(ix, n, nl, lm, rhi, q, root, eps, lane, [&](int i, float, bool hit) {
+    if (hit) {
+      const int j = __ldg(&ix.ids[i]);
+      if (j < row && __ldg(&core[j]) != 0u) {
+        if (ri < 0) ri = db_find(parent, row);
+        const int rj = db_find(parent, j);
+        if (rj != ri) {
+          ri = db_find(parent, ri);
+          db_union(parent, ri, rj);
+          ri = db_find(parent, ri);
+        }
+      }
+    }
+    return false;
+  });
+}
+
+// parent[i] <- root of i for core rows; root[i] = 1 for the roots, else 0.  db_compress_kernel's path-halving find writes
+// parent[v] = grandparent while walking, and can so overwrite the root another thread just stored at v with a non-root
+// ancestor, which the labels then read.  This find only reads: every value it can see at a node (the parent from the
+// link walk, or the root stored here) is an ancestor, so it ends at the root, and the only store is parent[i] = root.
+// The ball-cover fit's link order leaves deeper trees than the batched fit's, which makes that race likely there.
+__global__ void db_rbc_compress_kernel(int* parent, int64_t m, unsigned* root)
+{
+  const int64_t i = static_cast<int64_t>(blockIdx.x) * blockDim.x + threadIdx.x;
+  if (i >= m) return;
+  const volatile int* p = parent;
+  int r = p[i];
+  if (r >= 0) {
+    for (int v = p[r]; v != r; v = p[r]) r = v;
+    parent[i] = r;
+  }
+  root[i] = r == static_cast<int>(i) ? 1u : 0u;
+}
+
+// One warp owns each non-core row, so its smallest root is a plain store.
+template <int D>
+__global__ void __launch_bounds__(kBcWarps * 32) db_rbc_border_kernel(BcIndex ix, int n, int nl, int root, float eps,
+                                                                      const int* parent, int* border, int smem)
+{
+  const float *lm, *rhi;
+  bc_stage<D>(ix, nl, smem, &lm, &rhi);
+  const int lane = threadIdx.x & 31;
+  const int t    = blockIdx.x * kBcWarps + (threadIdx.x >> 5);
+  if (t >= n) return;
+  float q[D];
+  int row;
+  if (!db_rbc_query<D>(ix, t, q, &row) || __ldg(&parent[row]) >= 0) return;
+  int best = INT_MAX;
+  bc_eps_walk<D>(ix, n, nl, lm, rhi, q, root, eps, lane, [&](int i, float, bool hit) {
+    if (hit) {
+      const int r = __ldg(&parent[__ldg(&ix.ids[i])]);   // -1: not core
+      if (r >= 0) best = min(best, r);
+    }
+    return false;
+  });
+  best = __reduce_min_sync(0xffffffffu, best);
+  if (lane == 0) border[row] = best;
+}
+
+// ------------------------------------------------------------------------------------------
 
 // rank: the root flags scanned (cluster number of root r = rank[r]); crank: the core flags scanned, ctrl_c->total core rows
 __global__ void db_label_kernel(const int* parent, const int* border, const unsigned* rank, const unsigned* crank, int64_t m,

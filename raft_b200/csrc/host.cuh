@@ -11,6 +11,7 @@
 #include <string>
 
 #include "../../include/raft_b200.h"
+#include "ball_cover_types.cuh"
 #include "kmeans_types.cuh"
 #include "prep.cuh"   // PrepMode (its kernels are templates, instantiated by launch_prep alone)
 #include "tc_params.cuh"
@@ -285,6 +286,40 @@ constexpr size_t kRowSortBytes = static_cast<size_t>(1) << 20;
 // indices and distances.
 int radius_sort_split(cudaStream_t s, const int64_t* indptr, int64_t m, int64_t nnz, int64_t* indices, float* distances,
                       long long* alt, void* sort_tmp, size_t sort_bytes);
+
+// ------------------------------------------------------------------------------------------
+// ball_cover.cu: the index and its build, which DBSCAN's ball-cover fit runs too
+
+// n_landmarks, or ceil(sqrt(n)) for 0
+int64_t bc_landmarks(int64_t n, int64_t nl);
+
+// the index's regions (256-byte aligned)
+struct BcLayout {
+  BcIndex ix;
+  size_t bytes;
+};
+BcLayout bc_layout(void* base, int64_t n, int64_t d, int64_t nl);
+
+// The build's workspace: two key and two value buffers of the radix sorts, and their scratch.  CUB reports its scratch
+// only with a device present; the onesweep sort needs its digit counters and one 1 KiB look-back row per tile of at
+// least 256 items of a 2^28-item portion, which the bound below covers (checked at run time).
+struct BcBuildLayout {
+  unsigned long long* keys[2];
+  int* vals[2];
+  void* tmp;
+  size_t tmp_bytes;
+  size_t bytes;
+};
+BcBuildLayout bc_build_layout(void* base, int64_t n);
+
+// the index of x [n][D] (pitch ldx) with nl landmarks into ix, scratch W (D = 2 and 3 are instantiated)
+template <int D>
+int bc_build(cudaStream_t s, const BcIndex& ix, const BcBuildLayout& W, const float* x, int64_t ldx, int n, int nl,
+             uint64_t seed);
+
+// shared memory of a query launch of `kernel` (one of the ball_cover.cuh walks): the landmarks and their rhi when they
+// fit, else 0 (*bytes), set as the kernel's dynamic shared memory limit
+int bc_query_smem(const void* kernel, int64_t nl, int64_t d, size_t* bytes);
 
 // ------------------------------------------------------------------------------------------
 // single_linkage.cu
