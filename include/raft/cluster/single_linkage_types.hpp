@@ -4,7 +4,8 @@
 namespace raft {
 namespace cluster {
 
-// How the graph the MST is built on is formed.  Only KNN_GRAPH is provided (include/raft_b200.h, b2d_single_linkage).
+// How the graph the MST is built on is formed: KNN_GRAPH (include/raft_b200.h, b2d_single_linkage) or, for d = 2 and 3,
+// PAIRWISE, the complete graph (b2d_single_linkage_rbc).
 enum LinkageDistance { PAIRWISE = 0, KNN_GRAPH = 1 };
 
 // The dendrogram and flat labels of a linkage ([RECALLED] raft::cluster::linkage_output): device pointers owned by the

@@ -532,6 +532,36 @@ size_t b2d_single_linkage_workspace_bytes(int64_t m, int64_t d, int c);
 int b2d_single_linkage(void* stream, int metric, const float* x, int64_t ldx, int64_t m, int64_t d, int c, int n_clusters,
                        int32_t* children, float* deltas, int32_t* sizes, int32_t* labels, int32_t* n_components_out,
                        void* workspace, size_t workspace_bytes);
+/* The exact Euclidean minimum spanning tree of 2-D and 3-D points (raft::cluster::single_linkage's LinkageDistance::
+ * PAIRWISE for d <= 3), by Borůvka over the random ball cover.  x:[m,d] fp32, row-major, pitch ldx >= d.
+ *   The graph is complete; pair (i, j) weighs s(i, j) = ((q0-p0)*(q0-p0) + (q1-p1)*(q1-p1)) + (q2-p2)*(q2-p2), every
+ *     operation rounded separately: the ball cover's pair value (b2d_ball_cover_knn), with s(i, j) = s(j, i) bit for bit.
+ *   Edges are ordered by (s, min(i, j), max(i, j)), i and j the caller's rows: a strict order, so the tree is unique; it
+ *     is the tree Kruskal builds over all m (m - 1) / 2 pairs in that order.
+ *   Outputs (device, capacity m - 1): the m - 1 tree edges in that order, out_src[t] < out_dst[t] (int32 rows) and
+ *     out_w[t] = s (B2D_L2Unexpanded) or its correctly rounded square root (B2D_L2SqrtUnexpanded): the metric changes
+ *     the weights only, never the tree or the order.
+ * The bytes do not depend on seed, n_landmarks (in [0, m], 0 meaning ceil(sqrt(m))), the device or the scheduling.  The
+ * index is built in the workspace, then at most ceil(log2 m) + 1 rounds are enqueued, each a cross-component 1-NN walk
+ * over the index; rounds after the last merge return at once.  Only enqueues work (no synchronisation, no allocation), so
+ * the call can be captured in a CUDA graph.  Precondition: x finite (a non-finite x is safe, the output unspecified).
+ * metric outside the two above, d outside {2, 3} and m >= 2^30 are B2D_ERR_UNSUPPORTED; m < 1, a negative or too large
+ * n_landmarks, ldx < d and null pointers (the outputs may be null for m = 1) are B2D_ERR_INVALID_ARG.  The workspace
+ * (256-byte aligned) depends on (m, d, n_landmarks) only; the query returns SIZE_MAX for arguments the call rejects. */
+size_t b2d_emst_rbc_workspace_bytes(int64_t m, int64_t d, int64_t n_landmarks);
+int b2d_emst_rbc(void* stream, int metric, const float* x, int64_t ldx, int64_t m, int64_t d, int64_t n_landmarks,
+                 uint64_t seed, int32_t* out_src, int32_t* out_dst, float* out_w, void* workspace, size_t workspace_bytes);
+/* Exact single linkage of 2-D and 3-D points: the tree of b2d_emst_rbc, merged on the host into the outputs of
+ * b2d_single_linkage's step 5 (children [m-1][2], deltas [m-1] = out_w, sizes [m-1], labels [m]; device pointers).  This
+ * is scipy.cluster.hierarchy.linkage(method="single") on the matrix of s (of sqrt(s) for B2D_L2SqrtUnexpanded) up to
+ * the order scipy picks among equal heights; on data with distinct distances the tree is the same.  Arguments as
+ * b2d_emst_rbc, plus 1 <= n_clusters <= m (else B2D_ERR_INVALID_ARG); a non-finite x is B2D_ERR_INVALID_ARG, found on
+ * the device.  The call synchronises its stream twice (the edges to the host, the dendrogram back).  The workspace depends
+ * on (m, d, n_landmarks) only; the query returns SIZE_MAX for arguments the call rejects. */
+size_t b2d_single_linkage_rbc_workspace_bytes(int64_t m, int64_t d, int64_t n_landmarks);
+int b2d_single_linkage_rbc(void* stream, int metric, const float* x, int64_t ldx, int64_t m, int64_t d,
+                           int64_t n_landmarks, uint64_t seed, int n_clusters, int32_t* children, float* deltas,
+                           int32_t* sizes, int32_t* labels, void* workspace, size_t workspace_bytes);
 
 /* DBSCAN (cuML's DBSCAN(eps, min_samples, metric, max_mbytes_per_batch), sklearn.cluster.DBSCAN's labels_ and
  * core_sample_indices_) for fp32 x:[m,d] (row-major, pitch ldx), on the epsilon neighbourhood of b2d_eps_neighbors_l2sq.

@@ -29,6 +29,7 @@ SYMBOLS = [
     "b2d_ball_cover_index_bytes", "b2d_ball_cover_build_workspace_bytes", "b2d_ball_cover_build", "b2d_ball_cover_knn",
     "b2d_ball_cover_eps_workspace_bytes", "b2d_ball_cover_eps_count", "b2d_ball_cover_eps_fill",
     "b2d_dbscan_rbc_workspace_bytes", "b2d_dbscan_rbc_fit",
+    "b2d_emst_rbc_workspace_bytes", "b2d_emst_rbc", "b2d_single_linkage_rbc_workspace_bytes", "b2d_single_linkage_rbc",
 ]
 
 B2D_OK, B2D_ERR_INVALID_ARG, B2D_ERR_CUDA, B2D_ERR_UNSUPPORTED, B2D_ERR_WORKSPACE = range(5)
@@ -160,6 +161,14 @@ def lib() -> ctypes.CDLL:
     L.b2d_dbscan_rbc_workspace_bytes.argtypes = [i64, i64, i64]
     L.b2d_dbscan_rbc_fit.restype = ci
     L.b2d_dbscan_rbc_fit.argtypes = [vp, ci, vp, i64, i64, i64, cd, i64, i64, u64, vp, vp, vp, vp, sz]
+    L.b2d_emst_rbc_workspace_bytes.restype = sz
+    L.b2d_emst_rbc_workspace_bytes.argtypes = [i64, i64, i64]
+    L.b2d_emst_rbc.restype = ci
+    L.b2d_emst_rbc.argtypes = [vp, ci, vp, i64, i64, i64, i64, u64, vp, vp, vp, vp, sz]
+    L.b2d_single_linkage_rbc_workspace_bytes.restype = sz
+    L.b2d_single_linkage_rbc_workspace_bytes.argtypes = [i64, i64, i64]
+    L.b2d_single_linkage_rbc.restype = ci
+    L.b2d_single_linkage_rbc.argtypes = [vp, ci, vp, i64, i64, i64, i64, u64, ci, vp, vp, vp, vp, vp, sz]
     L.b2d_radius_neighbors_workspace_bytes.restype = sz
     L.b2d_radius_neighbors_workspace_bytes.argtypes = [i64, i64, i64, i64]
     L.b2d_radius_neighbors_count.restype = ci

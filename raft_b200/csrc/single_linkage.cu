@@ -7,6 +7,7 @@
 
 #include "host.cuh"
 #include "single_linkage.cuh"
+#include "single_linkage_rbc.cuh"
 
 using namespace b2d;
 
@@ -236,6 +237,174 @@ static int uf_find(std::vector<int>& p, int v)
   while (p[v] != v) v = p[v] = p[p[v]];
   return v;
 }
+
+// Step 5 of single_linkage: the m - 1 tree edges (hs[t], hd[t]) in key order merged on the host into children, sizes and
+// labels (device pointers; children and sizes unused for m = 1).  Synchronises the stream.
+static int sl_dendrogram(cudaStream_t s, int64_t m, int64_t n_clusters, const std::vector<int>& hs,
+                         const std::vector<int>& hd, int32_t* children, int32_t* sizes, int32_t* labels)
+{
+  std::vector<int> uf(m), cid(m), sz(m, 1), hch(2 * (m - 1)), hsz(m - 1), hlab(m);
+  for (int64_t i = 0; i < m; ++i) uf[i] = cid[i] = static_cast<int>(i);
+  const int64_t cut = m - n_clusters;   // labels: the components after the first m - n_clusters merges
+  for (int64_t t = 0; t < m - 1; ++t) {
+    if (t == cut)
+      for (int64_t i = 0; i < m; ++i) hlab[i] = uf_find(uf, static_cast<int>(i));
+    const int a = uf_find(uf, hs[t]), b = uf_find(uf, hd[t]);
+    if (a == b) return fail(B2D_ERR_CUDA, "internal: the spanning tree has a cycle");
+    hch[2 * t]     = std::min(cid[a], cid[b]);
+    hch[2 * t + 1] = std::max(cid[a], cid[b]);
+    hsz[t]         = sz[a] + sz[b];
+    uf[b]          = a;
+    sz[a]          = hsz[t];
+    cid[a]         = static_cast<int>(m + t);
+  }
+  if (cut == m - 1)
+    for (int64_t i = 0; i < m; ++i) hlab[i] = uf_find(uf, static_cast<int>(i));
+  std::vector<int> num(m, -1);   // numbered in order of each cluster's smallest row
+  int next_label = 0;
+  for (int64_t i = 0; i < m; ++i) {
+    int& l = num[hlab[i]];
+    if (l < 0) l = next_label++;
+    hlab[i] = l;
+  }
+  if (m > 1) {
+    B2D_CUDA(cudaMemcpyAsync(children, hch.data(), hch.size() * sizeof(int), cudaMemcpyHostToDevice, s));
+    B2D_CUDA(cudaMemcpyAsync(sizes, hsz.data(), hsz.size() * sizeof(int), cudaMemcpyHostToDevice, s));
+  }
+  B2D_CUDA(cudaMemcpyAsync(labels, hlab.data(), m * sizeof(int), cudaMemcpyHostToDevice, s));
+  B2D_CUDA(cudaStreamSynchronize(s));
+  return B2D_OK;
+}
+
+// ------------------------------------------------------------------------------------------
+// The exact EMST of 2-D and 3-D points (single_linkage_rbc.cuh): the ball-cover index of x, then Borůvka rounds whose
+// edges come from a cross-component 1-NN walk over it.  Only enqueues work.
+
+// The index, then the build's scratch, which is dead once the index is built: the rounds' arrays overlap it.
+struct EmstLayout {
+  BcIndex ix;
+  BcBuildLayout build;
+  SlCtrl* ctrl;
+  int* colour;        // [m] component of every position (the position of its root)
+  int* parent;        // [m] hook forest of a round
+  int* pos;           // [m] the position of every caller row
+  int* bcol;          // [nl] the single colour of every ball, or -1
+  long long* best1;   // [m] per component: min of (s, min row)
+  int* best2;         // [m] per component: min of the max row at best1
+  long long* cand1;   // [m] per position: its row's candidate (s, min row) ... (the sort's second key buffer after the rounds)
+  int* cand2;         // [m] ... and max row (the sort's second value buffer)
+  long long* mst1;    // [m] the tree edges as appended: (s, min row) ...
+  int* mst2;          // [m] ... and max row
+  int *hsrc, *hdst;   // [m] single_linkage_rbc: the edges in order, for the host
+  void* sort_tmp;
+  size_t sort_bytes;
+  size_t bytes;
+};
+
+static EmstLayout emst_layout(void* base, int64_t m, int64_t d, int64_t nl, bool host_edges)
+{
+  EmstLayout L{};
+  const BcLayout I = bc_layout(base, m, d, nl);
+  L.ix             = I.ix;
+  char* rest       = base ? static_cast<char*>(base) + I.bytes : nullptr;   // I.bytes is a multiple of 256
+  L.build          = bc_build_layout(rest, m);
+  Carve c(rest, 256);
+  L.ctrl   = c.take<SlCtrl>(1);
+  L.colour = c.take<int>(m);
+  L.parent = c.take<int>(m);
+  L.pos    = c.take<int>(m);
+  L.bcol   = c.take<int>(nl);
+  L.best1  = c.take<long long>(m);
+  L.best2  = c.take<int>(m);
+  L.cand1  = c.take<long long>(m);
+  L.cand2  = c.take<int>(m);
+  L.mst1   = c.take<long long>(m);
+  L.mst2   = c.take<int>(m);
+  if (host_edges) {
+    L.hsrc = c.take<int>(m);
+    L.hdst = c.take<int>(m);
+  }
+  // onesweep scratch: at most one 1 KiB look-back row per tile of >= 256 items, as the build's (checked at run time)
+  L.sort_bytes = 4 * static_cast<size_t>(std::min<int64_t>(m, int64_t(1) << 28)) + (static_cast<size_t>(1) << 20);
+  L.sort_tmp   = c.take<char>(L.sort_bytes);
+  L.bytes      = I.bytes + std::max(L.build.bytes, c.bytes);
+  return L;
+}
+
+// the checks b2d_emst_rbc and b2d_single_linkage_rbc share
+static int emst_args(const char* fn, int metric, const float* x, int64_t ldx, int64_t m, int64_t d, int64_t nl)
+{
+  if (metric != B2D_L2Unexpanded && metric != B2D_L2SqrtUnexpanded)
+    return fail(B2D_ERR_UNSUPPORTED, std::string(fn) + " supports the L2Unexpanded and L2SqrtUnexpanded metrics, got metric " +
+                                         std::to_string(metric));
+  if (m < 1 || nl < 0) return fail(B2D_ERR_INVALID_ARG, "m must be positive and n_landmarks non-negative");
+  if (d != 2 && d != 3) return fail(B2D_ERR_UNSUPPORTED, std::string(fn) + " supports d = 2 and d = 3, got d = " + std::to_string(d));
+  if (m >= kSlMaxRows) return fail(B2D_ERR_UNSUPPORTED, std::string(fn) + ": m must be below 2^30");
+  if (nl > m) return fail(B2D_ERR_INVALID_ARG, "n_landmarks must be in [0, m] (0: ceil(sqrt(m)))");
+  if (!x) return fail(B2D_ERR_INVALID_ARG, "null x");
+  if (ldx < d) return fail(B2D_ERR_INVALID_ARG, "leading dimension smaller than d");
+  return B2D_OK;
+}
+
+static bool emst_extents_ok(int64_t m, int64_t d, int64_t nl)
+{
+  return m >= 1 && m < kSlMaxRows && (d == 2 || d == 3) && nl >= 0 && nl <= m;
+}
+
+// the index, the rounds, and the m - 1 tree edges sorted into (s, min row, max row) order as (out_src, out_dst, out_w)
+template <int D>
+static int emst_run(cudaStream_t s, const EmstLayout& L, int root, const float* x, int64_t ldx, int n, int nl,
+                    uint64_t seed, int* out_src, int* out_dst, float* out_w)
+{
+  int rc = bc_build<D>(s, L.ix, L.build, x, ldx, n, nl, seed);
+  if (rc) return rc;
+  // (after the build: its scratch lies under these arrays)
+  sl_mst_init_kernel<<<sl_grid(n), 256, 0, s>>>(L.ctrl, L.colour, L.mst1, n);
+  slr_pos_kernel<<<sl_grid(n), 256, 0, s>>>(L.ix.ids, n, L.pos);
+  B2D_CUDA(cudaGetLastError());
+  if (n < 2) return B2D_OK;
+  size_t smem = 0;
+  rc = bc_query_smem(reinterpret_cast<const void*>(slr_walk_kernel<D>), nl, D, &smem);
+  if (rc) return rc;
+  const unsigned wg = static_cast<unsigned>((n + kBcWarps - 1) / kBcWarps);
+  const unsigned bg = static_cast<unsigned>((nl + kBcWarps - 1) / kBcWarps);
+  const int rounds  = ceil_log2(n) + 1;   // the components at least halve in every round
+  const int jumps   = std::min(kSlMaxJumps, ceil_log2(n) + 1);
+  for (int r = 0; r < rounds; ++r) {
+    sl_round_begin_kernel<<<sl_grid(std::max<int64_t>(n, kSlMaxJumps)), 256, 0, s>>>(L.ctrl, L.best1, n);
+    slr_ball_kernel<<<bg, kBcWarps * 32, 0, s>>>(L.ctrl, L.ix.off, L.colour, nl, L.bcol);
+    slr_walk_kernel<D><<<wg, kBcWarps * 32, smem, s>>>(L.ctrl, L.ix, n, nl, L.colour, L.bcol, L.best1, L.best2, L.cand1,
+                                                       L.cand2, smem > 0);
+    slr_tie_kernel<<<sl_grid(n), 256, 0, s>>>(L.ctrl, L.colour, L.cand1, L.cand2, L.best1, L.best2, n);
+    slr_hook_kernel<<<sl_grid(n), 256, 0, s>>>(L.ctrl, L.colour, L.pos, L.best1, L.best2, L.parent, L.mst1, L.mst2, n);
+    for (int j = 0; j < jumps; ++j) sl_jump_kernel<<<sl_grid(n), 256, 0, s>>>(L.ctrl, L.colour, L.parent, n, j);
+    sl_relabel_kernel<<<sl_grid(n), 256, 0, s>>>(L.ctrl, L.colour, L.parent, n);
+    sl_round_end_kernel<<<1, 1, 0, s>>>(L.ctrl);
+    B2D_CUDA(cudaGetLastError());
+  }
+  // the edges in (s, min row, max row) order: stable radix sorts by the max row, then by (s, min row)
+  const int ne = n - 1;
+  cub::DoubleBuffer<int> k2(L.mst2, L.cand2);
+  cub::DoubleBuffer<long long> k1(L.mst1, L.cand1);
+  size_t need = 0;
+  B2D_CUDA(cub::DeviceRadixSort::SortPairs(nullptr, need, k2, k1, ne, 0, 32, s));
+  if (need > L.sort_bytes) return fail(B2D_ERR_WORKSPACE, "internal: radix sort scratch " + std::to_string(need) + " bytes");
+  B2D_CUDA(cub::DeviceRadixSort::SortPairs(L.sort_tmp, need, k2, k1, ne, 0, 32, s));
+  B2D_CUDA(cub::DeviceRadixSort::SortPairs(nullptr, need, k1, k2, ne, 0, 64, s));
+  if (need > L.sort_bytes) return fail(B2D_ERR_WORKSPACE, "internal: radix sort scratch " + std::to_string(need) + " bytes");
+  B2D_CUDA(cub::DeviceRadixSort::SortPairs(L.sort_tmp, need, k1, k2, ne, 0, 64, s));
+  slr_emit_kernel<<<sl_grid(ne), 256, 0, s>>>(L.ctrl, k1.Current(), k2.Current(), ne, root, out_src, out_dst, out_w);
+  B2D_CUDA(cudaGetLastError());
+  return B2D_OK;
+}
+
+static int emst_dispatch(cudaStream_t s, const EmstLayout& L, int metric, const float* x, int64_t ldx, int64_t m,
+                         int64_t d, int64_t nl, uint64_t seed, int* out_src, int* out_dst, float* out_w)
+{
+  const int root = metric == B2D_L2SqrtUnexpanded;
+  return d == 2 ? emst_run<2>(s, L, root, x, ldx, static_cast<int>(m), static_cast<int>(nl), seed, out_src, out_dst, out_w)
+                : emst_run<3>(s, L, root, x, ldx, static_cast<int>(m), static_cast<int>(nl), seed, out_src, out_dst, out_w);
+}
 }  // namespace
 
 size_t b2d_mst_workspace_bytes(int64_t n_vertices, int64_t n_edges)
@@ -354,35 +523,66 @@ int b2d_single_linkage(void* stream, int metric, const float* x, int64_t ldx, in
     B2D_CUDA(cudaMemcpyAsync(hd.data(), L.hdst, (m - 1) * sizeof(int), cudaMemcpyDeviceToHost, s));
     B2D_CUDA(cudaStreamSynchronize(s));
   }
-  std::vector<int> uf(m), cid(m), sz(m, 1), hch(2 * (m - 1)), hsz(m - 1), hlab(m);
-  for (int64_t i = 0; i < m; ++i) uf[i] = cid[i] = static_cast<int>(i);
-  const int64_t cut = m - n_clusters;   // labels: the components after the first m - n_clusters merges
-  for (int64_t t = 0; t < m - 1; ++t) {
-    if (t == cut)
-      for (int64_t i = 0; i < m; ++i) hlab[i] = uf_find(uf, static_cast<int>(i));
-    const int a = uf_find(uf, hs[t]), b = uf_find(uf, hd[t]);
-    if (a == b) return fail(B2D_ERR_CUDA, "internal: the spanning tree has a cycle");
-    hch[2 * t]     = std::min(cid[a], cid[b]);
-    hch[2 * t + 1] = std::max(cid[a], cid[b]);
-    hsz[t]         = sz[a] + sz[b];
-    uf[b]          = a;
-    sz[a]          = hsz[t];
-    cid[a]         = static_cast<int>(m + t);
-  }
-  if (cut == m - 1)
-    for (int64_t i = 0; i < m; ++i) hlab[i] = uf_find(uf, static_cast<int>(i));
-  std::vector<int> num(m, -1);   // numbered in order of each cluster's smallest row
-  int next_label = 0;
-  for (int64_t i = 0; i < m; ++i) {
-    int& l = num[hlab[i]];
-    if (l < 0) l = next_label++;
-    hlab[i] = l;
-  }
+  return sl_dendrogram(s, m, n_clusters, hs, hd, children, sizes, labels);
+}
+
+size_t b2d_emst_rbc_workspace_bytes(int64_t m, int64_t d, int64_t n_landmarks)
+{
+  if (!emst_extents_ok(m, d, n_landmarks)) return static_cast<size_t>(-1);
+  return emst_layout(nullptr, m, d, bc_landmarks(m, n_landmarks), false).bytes;
+}
+
+int b2d_emst_rbc(void* stream, int metric, const float* x, int64_t ldx, int64_t m, int64_t d, int64_t n_landmarks,
+                 uint64_t seed, int32_t* out_src, int32_t* out_dst, float* out_w, void* workspace, size_t workspace_bytes)
+{
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  int rc         = emst_args("emst rbc", metric, x, ldx, m, d, n_landmarks);
+  if (rc) return rc;
+  if (m > 1 && (!out_src || !out_dst || !out_w)) return fail(B2D_ERR_INVALID_ARG, "null out_src / out_dst / out_w");
+  const int64_t nl = bc_landmarks(m, n_landmarks);
+  rc = check_workspace(workspace, workspace_bytes, emst_layout(nullptr, m, d, nl, false).bytes);
+  if (rc) return rc;
+  const EmstLayout L = emst_layout(workspace, m, d, nl, false);
+  return emst_dispatch(s, L, metric, x, ldx, m, d, nl, seed, out_src, out_dst, out_w);
+}
+
+size_t b2d_single_linkage_rbc_workspace_bytes(int64_t m, int64_t d, int64_t n_landmarks)
+{
+  if (!emst_extents_ok(m, d, n_landmarks)) return static_cast<size_t>(-1);
+  return emst_layout(nullptr, m, d, bc_landmarks(m, n_landmarks), true).bytes;
+}
+
+int b2d_single_linkage_rbc(void* stream, int metric, const float* x, int64_t ldx, int64_t m, int64_t d,
+                           int64_t n_landmarks, uint64_t seed, int n_clusters, int32_t* children, float* deltas,
+                           int32_t* sizes, int32_t* labels, void* workspace, size_t workspace_bytes)
+{
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  int rc         = emst_args("single_linkage rbc", metric, x, ldx, m, d, n_landmarks);
+  if (rc) return rc;
+  if (n_clusters < 1 || n_clusters > m) return fail(B2D_ERR_INVALID_ARG, "n_clusters must be in [1, m]");
+  if (!labels || (m > 1 && (!children || !deltas || !sizes)))
+    return fail(B2D_ERR_INVALID_ARG, "null children / deltas / sizes / labels");
+  const int64_t nl = bc_landmarks(m, n_landmarks);
+  rc = check_workspace(workspace, workspace_bytes, emst_layout(nullptr, m, d, nl, true).bytes);
+  if (rc) return rc;
+  const EmstLayout L = emst_layout(workspace, m, d, nl, true);
+  // 1.-3. the tree edges in order, their weights (the metric's distance) straight into deltas
+  rc = emst_dispatch(s, L, metric, x, ldx, m, d, nl, seed, L.hsrc, L.hdst, deltas);
+  if (rc) return rc;
+  sl_finite_kernel<<<km_grid(m * d), 256, 0, s>>>(x, ldx, m, static_cast<int>(d), L.ctrl);
+  B2D_CUDA(cudaGetLastError());
+  // 4. the dendrogram on the host (the one synchronisation before it reads the control words and the edges)
+  SlCtrl h;
+  std::vector<int> hs(m - 1), hd(m - 1);
+  B2D_CUDA(cudaMemcpyAsync(&h, L.ctrl, sizeof(SlCtrl), cudaMemcpyDeviceToHost, s));
   if (m > 1) {
-    B2D_CUDA(cudaMemcpyAsync(children, hch.data(), hch.size() * sizeof(int), cudaMemcpyHostToDevice, s));
-    B2D_CUDA(cudaMemcpyAsync(sizes, hsz.data(), hsz.size() * sizeof(int), cudaMemcpyHostToDevice, s));
+    B2D_CUDA(cudaMemcpyAsync(hs.data(), L.hsrc, (m - 1) * sizeof(int), cudaMemcpyDeviceToHost, s));
+    B2D_CUDA(cudaMemcpyAsync(hd.data(), L.hdst, (m - 1) * sizeof(int), cudaMemcpyDeviceToHost, s));
   }
-  B2D_CUDA(cudaMemcpyAsync(labels, hlab.data(), m * sizeof(int), cudaMemcpyHostToDevice, s));
   B2D_CUDA(cudaStreamSynchronize(s));
-  return B2D_OK;
+  if (h.bad & 1u) return fail(B2D_ERR_INVALID_ARG, "single_linkage rbc: X holds a non-finite value");
+  if (m > 1 && h.n_mst != static_cast<unsigned>(m - 1))
+    return fail(B2D_ERR_CUDA, "internal: the rounds chose " + std::to_string(h.n_mst) + " of " + std::to_string(m - 1) +
+                                  " tree edges");
+  return sl_dendrogram(s, m, n_clusters, hs, hd, children, sizes, labels);
 }
