@@ -14,8 +14,6 @@
 
 using namespace b2d;
 
-constexpr size_t kBcSmemMax = 64 << 10;   // landmarks staged in shared memory up to this many bytes per block
-
 int64_t b2d::bc_landmarks(int64_t n, int64_t nl)
 {
   if (nl > 0) return nl;
@@ -45,7 +43,7 @@ BcBuildLayout b2d::bc_build_layout(void* base, int64_t n)
   BcBuildLayout L;
   for (int b = 0; b < 2; ++b) L.keys[b] = c.take<unsigned long long>(n);
   for (int b = 0; b < 2; ++b) L.vals[b] = c.take<int>(n);
-  L.tmp_bytes = 4 * static_cast<size_t>(std::min<int64_t>(n, int64_t(1) << 28)) + (static_cast<size_t>(1) << 20);
+  L.tmp_bytes = bc_sort_bytes(n);
   L.tmp       = c.take<char>(L.tmp_bytes);
   L.bytes     = c.bytes;
   return L;
@@ -106,14 +104,6 @@ unsigned bc_grid(int64_t items, int sms) { return static_cast<unsigned>(std::max
 
 }  // namespace
 
-int b2d::bc_query_smem(const void* kernel, int64_t nl, int64_t d, size_t* bytes)
-{
-  const size_t b = static_cast<size_t>(nl) * (d + 1) * sizeof(float);
-  *bytes         = b <= kBcSmemMax ? b : 0;
-  B2D_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(*bytes)));
-  return B2D_OK;
-}
-
 template <int D>
 int b2d::bc_build(cudaStream_t s, const BcIndex& ix, const BcBuildLayout& W, const float* x, int64_t ldx, int n, int nl,
                   uint64_t seed)
@@ -153,36 +143,6 @@ int b2d::bc_build(cudaStream_t s, const BcIndex& ix, const BcBuildLayout& W, con
 }
 template int b2d::bc_build<2>(cudaStream_t, const BcIndex&, const BcBuildLayout&, const float*, int64_t, int, int, uint64_t);
 template int b2d::bc_build<3>(cudaStream_t, const BcIndex&, const BcBuildLayout&, const float*, int64_t, int, int, uint64_t);
-
-namespace {
-
-template <int D>
-int bc_knn(cudaStream_t s, const BcIndex& ix, int n, int nl, int root, const float* q, int64_t ldq, int m, int k,
-           int64_t* out_idx, float* out_dist)
-{
-  size_t smem = 0;
-  const int rc = bc_query_smem(reinterpret_cast<const void*>(bc_knn_kernel<D>), nl, D, &smem);
-  if (rc) return rc;
-  bc_knn_kernel<D><<<static_cast<unsigned>((m + kBcWarps - 1) / kBcWarps), kBcWarps * 32, smem, s>>>(
-      ix, n, nl, root, q, ldq, m, k, out_idx, out_dist, smem > 0);
-  B2D_CUDA(cudaGetLastError());
-  return B2D_OK;
-}
-
-template <int D>
-int bc_eps(cudaStream_t s, const BcIndex& ix, int n, int nl, int root, const float* q, int64_t ldq, int m, float eps,
-           int64_t* indptr, long long* keys, int64_t nnz)
-{
-  size_t smem = 0;
-  const int rc = bc_query_smem(reinterpret_cast<const void*>(bc_eps_kernel<D>), nl, D, &smem);
-  if (rc) return rc;
-  bc_eps_kernel<D><<<static_cast<unsigned>((m + kBcWarps - 1) / kBcWarps), kBcWarps * 32, smem, s>>>(
-      ix, n, nl, root, q, ldq, m, eps, indptr, keys, nnz, smem > 0);
-  B2D_CUDA(cudaGetLastError());
-  return B2D_OK;
-}
-
-}  // namespace
 
 size_t b2d_ball_cover_index_bytes(int64_t n, int64_t d, int64_t n_landmarks)
 {
@@ -228,10 +188,9 @@ int b2d_ball_cover_knn(void* stream, int64_t* out_idx, float* out_dist, const vo
   const int64_t nl = bc_landmarks(n, n_landmarks);
   const BcIndex ix = bc_layout(const_cast<void*>(index), n, d, nl).ix;
   const int root   = metric == B2D_L2SqrtUnexpanded;
-  return d == 2 ? bc_knn<2>(s, ix, static_cast<int>(n), static_cast<int>(nl), root, q, ldq, static_cast<int>(m),
-                            static_cast<int>(k), out_idx, out_dist)
-                : bc_knn<3>(s, ix, static_cast<int>(n), static_cast<int>(nl), root, q, ldq, static_cast<int>(m),
-                            static_cast<int>(k), out_idx, out_dist);
+  const int ni = static_cast<int>(n), nli = static_cast<int>(nl), mi = static_cast<int>(m), ki = static_cast<int>(k);
+  return d == 2 ? bc_walk_launch(s, bc_knn_kernel<2>, m, nl, d, ix, ni, nli, root, q, ldq, mi, ki, out_idx, out_dist)
+                : bc_walk_launch(s, bc_knn_kernel<3>, m, nl, d, ix, ni, nli, root, q, ldq, mi, ki, out_idx, out_dist);
 }
 
 size_t b2d_ball_cover_eps_workspace_bytes(int64_t m, int64_t nnz)
@@ -262,10 +221,9 @@ int b2d_ball_cover_eps_count(void* stream, int64_t* indptr, const void* index, i
   const BcIndex ix     = bc_layout(const_cast<void*>(index), n, d, nl).ix;
   const BcEpsLayout L  = bc_eps_layout(workspace, m, 0);
   const int root       = metric == B2D_L2SqrtUnexpanded;
-  rc = d == 2 ? bc_eps<2>(s, ix, static_cast<int>(n), static_cast<int>(nl), root, q, ldq, static_cast<int>(m), eps, indptr,
-                          nullptr, 0)
-              : bc_eps<3>(s, ix, static_cast<int>(n), static_cast<int>(nl), root, q, ldq, static_cast<int>(m), eps, indptr,
-                          nullptr, 0);
+  const int ni = static_cast<int>(n), nli = static_cast<int>(nl), mi = static_cast<int>(m);
+  rc = d == 2 ? bc_walk_launch(s, bc_eps_kernel<2>, m, nl, d, ix, ni, nli, root, q, ldq, mi, eps, indptr, nullptr, 0)
+              : bc_walk_launch(s, bc_eps_kernel<3>, m, nl, d, ix, ni, nli, root, q, ldq, mi, eps, indptr, nullptr, 0);
   if (rc) return rc;
   size_t need = 0;
   B2D_CUDA(cub::DeviceScan::InclusiveSum(nullptr, need, indptr + 1, indptr + 1, m, s));
@@ -299,10 +257,10 @@ int b2d_ball_cover_eps_fill(void* stream, const int64_t* indptr, int64_t nnz, in
   const BcEpsLayout L  = bc_eps_layout(workspace, m, nnz);
   const int root       = metric == B2D_L2SqrtUnexpanded;
   long long* keys      = reinterpret_cast<long long*>(indices);
-  rc = d == 2 ? bc_eps<2>(s, ix, static_cast<int>(n), static_cast<int>(nl), root, q, ldq, static_cast<int>(m), eps,
-                          const_cast<int64_t*>(indptr), keys, nnz)
-              : bc_eps<3>(s, ix, static_cast<int>(n), static_cast<int>(nl), root, q, ldq, static_cast<int>(m), eps,
-                          const_cast<int64_t*>(indptr), keys, nnz);
+  int64_t* ip          = const_cast<int64_t*>(indptr);
+  const int ni = static_cast<int>(n), nli = static_cast<int>(nl), mi = static_cast<int>(m);
+  rc = d == 2 ? bc_walk_launch(s, bc_eps_kernel<2>, m, nl, d, ix, ni, nli, root, q, ldq, mi, eps, ip, keys, nnz)
+              : bc_walk_launch(s, bc_eps_kernel<3>, m, nl, d, ix, ni, nli, root, q, ldq, mi, eps, ip, keys, nnz);
   if (rc) return rc;
   return radius_sort_split(s, indptr, m, nnz, indices, distances, L.alt, L.sort_tmp, L.sort_bytes);
 }

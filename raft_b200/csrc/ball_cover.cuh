@@ -1,5 +1,6 @@
 // Kernels of the random ball cover (ball_cover.cu): exact kNN and epsilon queries for 2-D and 3-D points, SIMT, and the
-// epsilon walk DBSCAN's ball-cover fit shares (dbscan.cuh).  The build's kernels are in ball_cover_build.cuh.
+// one ball walk (bc_walk) they, DBSCAN's ball-cover fit (dbscan.cuh) and the EMST (single_linkage_rbc.cuh) run on.  The
+// build's kernels are in ball_cover_build.cuh.
 //
 // A pair's value is fixed bit for bit: s = ((q0-p0)^2 + (q1-p1)^2) + (q2-p2)^2, every operation rounded separately
 // (bc_s), and the distance f = s (L2Unexpanded) or sqrt(s) (L2SqrtUnexpanded).  The queries prune whole balls and ball
@@ -17,8 +18,6 @@
 #include "nn_key.cuh"
 
 namespace b2d {
-
-constexpr int kBcWarps = 8;   // queries per block of the query kernels (one warp each)
 
 constexpr float BC_INF = __builtin_huge_valf();
 constexpr float BC_A   = 0x1p-148f;         // absolute slack of s
@@ -97,6 +96,59 @@ __device__ __forceinline__ void bc_stage(const BcIndex& ix, int nl, bool smem, c
   *rhi = bc_sm + nl * D;
 }
 
+// the query point at p; false: a NaN coordinate (the query has no neighbour)
+template <int D>
+__device__ __forceinline__ bool bc_query(const float* p, float (&q)[D])
+{
+  bool nan = false;
+  for (int c = 0; c < D; ++c) {
+    q[c] = p[c];
+    nan  = nan || isnan(q[c]);
+  }
+  return !nan;
+}
+
+// The ball loop of every walk, for one query q (not NaN) of a warp: the balls in index order, every admitted non-empty
+// ball that bc_ball_out does not rule out at the bound of the moment it is reached, then the non-finite rows [off[nl], n)
+// with sq = 0 (nothing is pruned there).  The walker v gives admit(j) (the ball filter), dmax (the distance bound) and
+// scan(lo, hi, sq), which visits the positions [lo, hi) of a ball at s = sq from the query and returns true (the same on
+// every lane) to end the walk.  Shrinking: v's bound decreases as it scans (kNN, EMST), so the nearest admitted ball goes
+// first to tighten it early, and each ball is tested again when it is reached; a fixed bound (epsilon) needs neither.
+// The kNN, epsilon, DBSCAN (dbscan.cuh) and EMST (single_linkage_rbc.cuh) walks all run on it, so the ball pruning has
+// one definition.
+template <int D, bool Shrinking, typename Walker>
+__device__ __forceinline__ void bc_walk(const BcIndex& ix, int n, int nl, const float* lm, const float* rhi, const float* q,
+                                        int lane, Walker& v)
+{
+  int b0 = -1;
+  if (Shrinking) {
+    long long near = KEY_EMPTY;
+    for (int j = lane; j < nl; j += 32)
+      if (rhi[j] >= 0.f && v.admit(j)) near = min(near, key_pack(bc_s<D>(q, lm + j * D), j));
+    for (int o = 16; o > 0; o >>= 1) near = min(near, __shfl_xor_sync(0xffffffffu, near, o));
+    b0 = near == KEY_EMPTY ? -1 : static_cast<int>(key_index(near));
+    if (b0 >= 0 && v.scan(ix.off[b0], ix.off[b0 + 1], key_dist(near))) return;
+  }
+  for (int base = 0; base < nl; base += 32) {
+    const int j = base + lane;
+    float s     = 0.f;
+    bool want   = false;
+    if (j < nl && j != b0 && rhi[j] >= 0.f && v.admit(j)) {
+      s    = bc_s<D>(q, lm + j * D);
+      want = !bc_ball_out(s, rhi[j], v.dmax);
+    }
+    unsigned mask = __ballot_sync(0xffffffffu, want);
+    while (mask) {
+      const int src  = __ffs(mask) - 1;
+      mask          &= mask - 1;
+      const float sj = __shfl_sync(0xffffffffu, s, src);
+      const int b    = base + src;
+      if ((!Shrinking || !bc_ball_out(sj, rhi[b], v.dmax)) && v.scan(ix.off[b], ix.off[b + 1], sj)) return;
+    }
+  }
+  v.scan(ix.off[nl], n, 0.f);
+}
+
 // A warp's sorted list of the 64 best keys so far: lane l holds slots l (a0) and l + 32 (a1).
 struct BcTopK {
   long long a0 = KEY_EMPTY, a1 = KEY_EMPTY;
@@ -118,51 +170,56 @@ struct BcTopK {
   }
 };
 
-// The kNN state of one query: the list, its k-th key and the distance bound that k-th key gives.
+// The kNN walker of one query of a warp: the list, its k-th key and the distance bound that k-th key gives.
+template <int D>
 struct BcKnn {
+  const BcIndex& ix;
+  const float* q;
+  int k, root, lane;
   BcTopK list;
   long long kth = KEY_EMPTY;
   float dmax    = BC_INF;
+
+  __device__ __forceinline__ bool admit(int) const { return true; }
+
+  // the members [lo, hi) of one ball at s = sq from the query into the list, in a window that shrinks with the k-th key
+  __device__ __forceinline__ bool scan(int lo, int hi, float sq)
+  {
+    float wlo, whi;
+    bc_window(sq, dmax, &wlo, &whi);
+    for (int p = bc_search(ix.rl, lo, hi, wlo, false); p < hi; p += 32) {
+      const int i    = p + lane;
+      const float r  = i < hi ? ix.rl[i] : BC_INF;
+      const bool out = i < hi && r > whi;
+      long long key  = KEY_EMPTY;
+      if (i < hi && !out && r >= wlo) {
+        const float s = bc_s<D>(q, ix.pts + static_cast<int64_t>(i) * D);
+        const float f = root ? __fsqrt_rn(s) : s;
+        if (f == f) key = key_pack(f, ix.ids[i]);
+      }
+      unsigned mask = __ballot_sync(0xffffffffu, key < kth);
+      if (mask) {
+        do {
+          const int src     = __ffs(mask) - 1;
+          mask             &= mask - 1;
+          const long long c = __shfl_sync(0xffffffffu, key, src);
+          if (c < kth) {
+            list.insert(c, lane);
+            kth = list.slot(k - 1);
+          }
+        } while (mask);
+        if (kth != KEY_EMPTY) {
+          dmax = bc_dmax(key_dist(kth), root);
+          bc_window(sq, dmax, &wlo, &whi);
+        }
+      }
+      if (__any_sync(0xffffffffu, out)) break;
+    }
+    return false;
+  }
 };
 
-// Scans the members [lo, hi) of one ball (or the non-finite rows, sq = 0: nothing is pruned there) into the list.
-template <int D>
-__device__ __forceinline__ void bc_knn_ball(const BcIndex& ix, int lo, int hi, float sq, const float* q, int k, int root,
-                                            BcKnn& st, int lane)
-{
-  float wlo, whi;
-  bc_window(sq, st.dmax, &wlo, &whi);
-  for (int p = bc_search(ix.rl, lo, hi, wlo, false); p < hi; p += 32) {
-    const int i    = p + lane;
-    const float r  = i < hi ? ix.rl[i] : BC_INF;
-    const bool out = i < hi && r > whi;
-    long long key  = KEY_EMPTY;
-    if (i < hi && !out && r >= wlo) {
-      const float s = bc_s<D>(q, ix.pts + static_cast<int64_t>(i) * D);
-      const float f = root ? __fsqrt_rn(s) : s;
-      if (f == f) key = key_pack(f, ix.ids[i]);
-    }
-    unsigned mask = __ballot_sync(0xffffffffu, key < st.kth);
-    if (mask) {
-      do {
-        const int src     = __ffs(mask) - 1;
-        mask             &= mask - 1;
-        const long long c = __shfl_sync(0xffffffffu, key, src);
-        if (c < st.kth) {
-          st.list.insert(c, lane);
-          st.kth = st.list.slot(k - 1);
-        }
-      } while (mask);
-      if (st.kth != KEY_EMPTY) {
-        st.dmax = bc_dmax(key_dist(st.kth), root);
-        bc_window(sq, st.dmax, &wlo, &whi);
-      }
-    }
-    if (__any_sync(0xffffffffu, out)) break;
-  }
-}
-
-// One warp per query: the nearest ball first, then every ball the bound does not rule out, then the non-finite rows.
+// One warp per query: bc_walk with the nearest ball first, which seeds the list.
 template <int D>
 __global__ void __launch_bounds__(kBcWarps * 32) bc_knn_kernel(BcIndex ix, int n, int nl, int root, const float* qs,
                                                                int64_t ldq, int m, int k, int64_t* out_idx,
@@ -174,38 +231,8 @@ __global__ void __launch_bounds__(kBcWarps * 32) bc_knn_kernel(BcIndex ix, int n
   const int qi   = blockIdx.x * kBcWarps + (threadIdx.x >> 5);
   if (qi >= m) return;
   float q[D];
-  bool nan = false;
-  for (int c = 0; c < D; ++c) {
-    q[c] = qs[static_cast<int64_t>(qi) * ldq + c];
-    nan  = nan || isnan(q[c]);
-  }
-  BcKnn st;
-  if (!nan) {
-    long long best = KEY_EMPTY;
-    for (int j = lane; j < nl; j += 32)
-      if (rhi[j] >= 0.f) best = min(best, key_pack(bc_s<D>(q, lm + j * D), j));
-    for (int o = 16; o > 0; o >>= 1) best = min(best, __shfl_xor_sync(0xffffffffu, best, o));
-    const int b0 = best == KEY_EMPTY ? -1 : static_cast<int>(key_index(best));
-    if (b0 >= 0) bc_knn_ball<D>(ix, ix.off[b0], ix.off[b0 + 1], key_dist(best), q, k, root, st, lane);
-    for (int base = 0; base < nl; base += 32) {
-      const int j = base + lane;
-      float s     = 0.f;
-      bool want   = false;
-      if (j < nl && j != b0 && rhi[j] >= 0.f) {
-        s    = bc_s<D>(q, lm + j * D);
-        want = !bc_ball_out(s, rhi[j], st.dmax);
-      }
-      unsigned mask = __ballot_sync(0xffffffffu, want);
-      while (mask) {
-        const int src  = __ffs(mask) - 1;
-        mask          &= mask - 1;
-        const float sj = __shfl_sync(0xffffffffu, s, src);
-        const int b    = base + src;
-        if (!bc_ball_out(sj, rhi[b], st.dmax)) bc_knn_ball<D>(ix, ix.off[b], ix.off[b + 1], sj, q, k, root, st, lane);
-      }
-    }
-    bc_knn_ball<D>(ix, ix.off[nl], n, 0.f, q, k, root, st, lane);
-  }
+  BcKnn<D> st{ix, q, k, root, lane};
+  if (bc_query<D>(qs + static_cast<int64_t>(qi) * ldq, q)) bc_walk<D, true>(ix, n, nl, lm, rhi, q, lane, st);
   for (int j = lane; j < k; j += 32) {
     const long long key = j < 32 ? st.list.a0 : st.list.a1;
     const int64_t o     = static_cast<int64_t>(qi) * k + j;
@@ -214,18 +241,22 @@ __global__ void __launch_bounds__(kBcWarps * 32) bc_knn_kernel(BcIndex ix, int n
   }
 }
 
-// The epsilon walk of one query q (not NaN) of a warp: every ball the bound does not rule out, the member window by
-// binary search, then the non-finite rows.  Every step of 32 positions calls act(i, f, hit) on all lanes: i = the lane's
-// position, f = its distance and hit = (f <= eps) for a position inside the window, else hit = false.  act returns true
-// (the same on every lane) to end the walk there.  The epsilon queries and DBSCAN's walks (dbscan.cuh) share it, so the
-// pruning and its margin have one definition.
+// The epsilon walker: the fixed bound of eps, and in each ball the member window by two binary searches, every position
+// of which is measured.
 template <int D, typename Act>
-__device__ __forceinline__ void bc_eps_walk(const BcIndex& ix, int n, int nl, const float* lm, const float* rhi,
-                                            const float* q, int root, float eps, int lane, Act&& act)
-{
-  const float dmax = bc_dmax(eps, root);
-  // the positions [lo, hi) of a ball at s = sq from the query; true: the walk ends
-  auto scan = [&](int lo, int hi, float sq) {
+struct BcEpsWalk {
+  const BcIndex& ix;
+  const float* q;
+  int root;
+  float eps;
+  int lane;
+  float dmax;
+  Act& act;
+
+  __device__ __forceinline__ bool admit(int) const { return true; }
+
+  __device__ __forceinline__ bool scan(int lo, int hi, float sq)
+  {
     float wlo, whi;
     bc_window(sq, dmax, &wlo, &whi);
     lo = bc_search(ix.rl, lo, hi, wlo, false);
@@ -242,24 +273,19 @@ __device__ __forceinline__ void bc_eps_walk(const BcIndex& ix, int n, int nl, co
       if (act(i, f, hit)) return true;
     }
     return false;
-  };
-  for (int base = 0; base < nl; base += 32) {
-    const int j = base + lane;
-    float s     = 0.f;
-    bool want   = false;
-    if (j < nl && rhi[j] >= 0.f) {
-      s    = bc_s<D>(q, lm + j * D);
-      want = !bc_ball_out(s, rhi[j], dmax);
-    }
-    unsigned mask = __ballot_sync(0xffffffffu, want);
-    while (mask) {
-      const int src  = __ffs(mask) - 1;
-      mask          &= mask - 1;
-      const int b    = base + src;
-      if (scan(ix.off[b], ix.off[b + 1], __shfl_sync(0xffffffffu, s, src))) return;
-    }
   }
-  scan(ix.off[nl], n, 0.f);
+};
+
+// The epsilon walk of one query q (not NaN) of a warp, bc_walk with the fixed bound of eps.  Every step of 32 positions calls
+// act(i, f, hit) on all lanes: i = the lane's position, f = its distance and hit = (f <= eps) for a position inside the
+// window, else hit = false.  act returns true (the same on every lane) to end the walk there.  The epsilon queries and
+// DBSCAN's walks (dbscan.cuh) share it.
+template <int D, typename Act>
+__device__ __forceinline__ void bc_eps_walk(const BcIndex& ix, int n, int nl, const float* lm, const float* rhi,
+                                            const float* q, int root, float eps, int lane, Act&& act)
+{
+  BcEpsWalk<D, Act> w{ix, q, root, eps, lane, bc_dmax(eps, root), act};
+  bc_walk<D, false>(ix, n, nl, lm, rhi, q, lane, w);
 }
 
 // Epsilon queries, one warp per query, by bc_eps_walk.  Count (keys == nullptr): indptr[qi + 1] = the query's pairs
@@ -275,18 +301,14 @@ __global__ void __launch_bounds__(kBcWarps * 32) bc_eps_kernel(BcIndex ix, int n
   const int qi   = blockIdx.x * kBcWarps + (threadIdx.x >> 5);
   if (qi >= m) return;
   float q[D];
-  bool nan = false;
-  for (int c = 0; c < D; ++c) {
-    q[c] = qs[static_cast<int64_t>(qi) * ldq + c];
-    nan  = nan || isnan(q[c]);
-  }
+  const bool ok = bc_query<D>(qs + static_cast<int64_t>(qi) * ldq, q);
   int64_t at = 0, end = 0;
   if (keys) {
     at  = indptr[qi];
     end = min(indptr[qi + 1], nnz);
   }
   int64_t cnt = 0;
-  if (!nan)
+  if (ok)
     bc_eps_walk<D>(ix, n, nl, lm, rhi, q, root, eps, lane, [&](int i, float f, bool hit) {
       const unsigned mask = __ballot_sync(0xffffffffu, hit);
       if (keys) {

@@ -1,8 +1,10 @@
-// The ball cover's index, the one type its kernels (ball_cover.cuh) and the host code of the files that build an index
-// (host.cuh) share.
+// The ball cover's index and the walks' block shape, which its kernels (ball_cover.cuh) and the host code of the files
+// that build an index (host.cuh) share.
 #pragma once
 
 namespace b2d {
+
+constexpr int kBcWarps = 8;   // items (queries or index positions) per block of the walks, one warp each
 
 // The index, one caller-owned buffer (its regions: bc_layout in ball_cover.cu).  Positions are the rows sorted by
 // (ball, s to the ball's landmark, row); rows with a non-finite coordinate follow the last ball.

@@ -15,6 +15,45 @@ using namespace b2d;
 namespace {
 constexpr int64_t kDbDefaultBatchBytes = 1ll << 30;
 
+// The degrees and the union-find forest of both fits, and the scans that number its roots and core rows.
+struct DbForest {
+  unsigned* deg;     // the degrees (db_core_kernel's layout)
+  int* parent;       // [m] union-find forest over the core rows (-1: not core)
+  int* border;       // [m] smallest root reaching a non-core row (INT_MAX: none)
+  unsigned* root;    // [m] root flags, scanned into cluster numbers
+  unsigned* core;    // [m] core flags, scanned into core_sample_indices positions
+  unsigned* tiles;   // scan tile sums
+  KmCtrl* ctrl;      // [2] scan totals: clusters, core rows
+};
+
+static DbForest db_forest(Carve& c, int64_t m, int64_t deg_rows)
+{
+  DbForest F;
+  F.deg    = c.take<unsigned>(deg_rows);
+  F.parent = c.take<int>(m);
+  F.border = c.take<int>(m);
+  F.root   = c.take<unsigned>(m);
+  F.core   = c.take<unsigned>(m);
+  F.tiles  = c.take<unsigned>((m + kKmScanTile - 1) / kKmScanTile);
+  F.ctrl   = c.take<KmCtrl>(2);
+  return F;
+}
+
+// the labels from the compressed forest and the border roots: cluster numbers = ranks of the roots, core_sample_indices
+// positions = ranks of the core rows
+static int db_label(cudaStream_t s, const DbForest& F, int64_t m, int32_t* labels, int32_t* core_sample_indices,
+                    int32_t* n_clusters)
+{
+  int rc = km_scan(s, nullptr, F.root, m, F.tiles, F.ctrl);
+  if (rc) return rc;
+  rc = km_scan(s, nullptr, F.core, m, F.tiles, F.ctrl + 1);
+  if (rc) return rc;
+  db_label_kernel<<<sl_grid(m), 256, 0, s>>>(F.parent, F.border, F.root, F.core, m, &F.ctrl[0].total, &F.ctrl[1].total,
+                                             labels, core_sample_indices, n_clusters);
+  B2D_CUDA(cudaGetLastError());
+  return B2D_OK;
+}
+
 // columns per batch: min(m, max(256, floor(max_bytes / m / 256) * 256)); max_bytes 0 means 2^30
 static int64_t db_batch(int64_t m, int64_t max_bytes)
 {
@@ -27,13 +66,7 @@ struct DbLayout {
   TcWorkspace tc;    // x prepared once, as both operands
   int64_t b, nb;     // columns per batch, batches
   int64_t ld;        // adjacency row pitch: b rounded up to 16
-  unsigned* deg;     // [m + nb] per-column degrees, each batch's total behind its columns
-  int* parent;       // [m] union-find forest over the core rows (-1: not core)
-  int* border;       // [m] smallest root reaching a non-core row (INT_MAX: none)
-  unsigned* root;    // [m] root flags, scanned into cluster numbers
-  unsigned* core;    // [m] core flags, scanned into core_sample_indices positions
-  unsigned* tiles;   // scan tile sums
-  KmCtrl* ctrl;      // [2] scan totals: clusters, core rows
+  DbForest f;        // deg [m + nb]: per-column degrees, each batch's total behind its columns
   uint8_t* adj;      // [m][ld] adjacency of one batch
   size_t bytes;
 };
@@ -46,13 +79,7 @@ static DbLayout db_layout(void* base, int64_t m, int64_t d, int64_t max_bytes)
   L.b      = db_batch(m, max_bytes);
   L.nb     = (m + L.b - 1) / L.b;
   L.ld     = (L.b + 15) / 16 * 16;
-  L.deg    = c.take<unsigned>(m + L.nb);
-  L.parent = c.take<int>(m);
-  L.border = c.take<int>(m);
-  L.root   = c.take<unsigned>(m);
-  L.core   = c.take<unsigned>(m);
-  L.tiles  = c.take<unsigned>((m + kKmScanTile - 1) / kKmScanTile);
-  L.ctrl   = c.take<KmCtrl>(2);
+  L.f      = db_forest(c, m, m + L.nb);
   L.adj    = c.take<uint8_t>(static_cast<size_t>(m) * L.ld);
   L.bytes  = c.bytes;
   return L;
@@ -66,7 +93,7 @@ static int db_eps(cudaStream_t s, const DbLayout& L, int64_t m, int64_t d, float
   TcParams p{};
   p.m = m; p.n = w;
   p.adj = adj ? L.adj : nullptr; p.ld_adj = L.ld;
-  p.vd = deg ? L.deg + c0 + t : nullptr; p.vd64 = 0; p.eps = e;
+  p.vd = deg ? L.f.deg + c0 + t : nullptr; p.vd64 = 0; p.eps = e;
   p.diag_off = c0;
   p.tma_store = (adj && w % 16 == 0) ? 1 : 0;   // (L.adj is 1024-byte aligned and L.ld a multiple of 16)
   return launch_tc(s, tc_rows(L.tc, 1, c0, d), p, d, EPI_EPS, POST_CLAMP);
@@ -99,7 +126,8 @@ int b2d_dbscan_fit(void* stream, int metric, const float* x, int64_t ldx, int64_
   if (ldx < d) return fail(B2D_ERR_INVALID_ARG, "leading dimension smaller than d");
   int rc = check_workspace(workspace, workspace_bytes, db_layout(nullptr, m, d, max_bytes_per_batch).bytes);
   if (rc) return rc;
-  const DbLayout L = db_layout(workspace, m, d, max_bytes_per_batch);
+  const DbLayout L  = db_layout(workspace, m, d, max_bytes_per_batch);
+  const DbForest& F = L.f;
   // the threshold on the distance the kernel compares: eps^2 (rounded once from fp64) for L2SqrtExpanded; a NaN or
   // negative eps matches nothing (every distance is >= 0 or NaN)
   const float e = !(eps >= 0.0) ? -INFINITY : static_cast<float>(metric == B2D_L2SqrtExpanded ? eps * eps : eps);
@@ -108,13 +136,13 @@ int b2d_dbscan_fit(void* stream, int metric, const float* x, int64_t ldx, int64_
   rc = launch_prep<float>(s, L.tc, x, ldx, 1, m, x, ldx, 1, m, d, nullptr, nullptr, tm);
   if (rc) return rc;
   // 1. degrees, then the core flags (one batch: the adjacency in the same launch)
-  B2D_CUDA(cudaMemsetAsync(L.deg, 0, static_cast<size_t>(m + L.nb) * sizeof(unsigned), s));
+  B2D_CUDA(cudaMemsetAsync(F.deg, 0, static_cast<size_t>(m + L.nb) * sizeof(unsigned), s));
   const bool one = L.nb == 1;
   for (int64_t t = 0; t < L.nb; ++t) {
     rc = db_eps(s, L, m, d, e, t, one, true);
     if (rc) return rc;
   }
-  db_core_kernel<<<sl_grid(m), 256, 0, s>>>(L.deg, m, L.b, ms, L.parent, L.border, L.core);
+  db_core_kernel<<<sl_grid(m), 256, 0, s>>>(F.deg, m, L.b, ms, F.parent, F.border, F.core);
   B2D_CUDA(cudaGetLastError());
   // 2. links between core points
   for (int64_t t = 0; t < L.nb; ++t) {
@@ -123,10 +151,10 @@ int b2d_dbscan_fit(void* stream, int metric, const float* x, int64_t ldx, int64_
       rc = db_eps(s, L, m, d, e, t, true, false);
       if (rc) return rc;
     }
-    db_link_kernel<<<db_warp_grid(m), kDbThreads, 0, s>>>(L.adj, L.ld, m, c0, w, L.core, L.parent);
+    db_link_kernel<<<db_warp_grid(m), kDbThreads, 0, s>>>(L.adj, L.ld, m, c0, w, F.core, F.parent);
     B2D_CUDA(cudaGetLastError());
   }
-  db_compress_kernel<<<sl_grid(m), 256, 0, s>>>(L.parent, m, L.root);
+  db_compress_kernel<<<sl_grid(m), 256, 0, s>>>(F.parent, m, F.root);
   B2D_CUDA(cudaGetLastError());
   // 3. border points
   for (int64_t t = 0; t < L.nb; ++t) {
@@ -135,18 +163,11 @@ int b2d_dbscan_fit(void* stream, int metric, const float* x, int64_t ldx, int64_
       rc = db_eps(s, L, m, d, e, t, true, false);
       if (rc) return rc;
     }
-    db_border_kernel<<<db_warp_grid(m), kDbThreads, 0, s>>>(L.adj, L.ld, m, c0, w, L.parent, L.border);
+    db_border_kernel<<<db_warp_grid(m), kDbThreads, 0, s>>>(L.adj, L.ld, m, c0, w, F.parent, F.border);
     B2D_CUDA(cudaGetLastError());
   }
-  // 4. cluster numbers = ranks of the roots; core_sample_indices positions = ranks of the core rows
-  rc = km_scan(s, nullptr, L.root, m, L.tiles, L.ctrl);
-  if (rc) return rc;
-  rc = km_scan(s, nullptr, L.core, m, L.tiles, L.ctrl + 1);
-  if (rc) return rc;
-  db_label_kernel<<<sl_grid(m), 256, 0, s>>>(L.parent, L.border, L.root, L.core, m, &L.ctrl[0].total, &L.ctrl[1].total,
-                                             labels, core_sample_indices, n_clusters);
-  B2D_CUDA(cudaGetLastError());
-  return B2D_OK;
+  // 4. the labels
+  return db_label(s, F, m, labels, core_sample_indices, n_clusters);
 }
 
 // ------------------------------------------------------------------------------------------
@@ -158,74 +179,49 @@ namespace {
 struct DbRbcLayout {
   BcIndex ix;
   BcBuildLayout build;
-  unsigned* deg;     // [m] hits per row, up to min_samples
-  int* parent;       // [m] union-find forest over the core rows (-1: not core)
-  int* border;       // [m] smallest root reaching a non-core row (INT_MAX: none)
-  unsigned* root;    // [m] root flags, scanned into cluster numbers
-  unsigned* core;    // [m] core flags, scanned into core_sample_indices positions
-  unsigned* tiles;   // scan tile sums
-  KmCtrl* ctrl;      // [2] scan totals: clusters, core rows
+  DbForest f;        // deg [m]: hits per row, up to min_samples
   size_t bytes;
 };
 
 static DbRbcLayout db_rbc_layout(void* base, int64_t m, int64_t d, int64_t nl)
 {
+  BcOverlay o(base, m, d, nl);
   DbRbcLayout L{};
-  const BcLayout I = bc_layout(base, m, d, nl);
-  L.ix             = I.ix;
-  char* rest       = base ? static_cast<char*>(base) + I.bytes : nullptr;   // I.bytes is a multiple of 256
-  L.build          = bc_build_layout(rest, m);
-  Carve c(rest, 256);
-  L.deg    = c.take<unsigned>(m);
-  L.parent = c.take<int>(m);
-  L.border = c.take<int>(m);
-  L.root   = c.take<unsigned>(m);
-  L.core   = c.take<unsigned>(m);
-  L.tiles  = c.take<unsigned>((m + kKmScanTile - 1) / kKmScanTile);
-  L.ctrl   = c.take<KmCtrl>(2);
-  L.bytes  = I.bytes + std::max(L.build.bytes, c.bytes);
+  L.ix    = o.ix;
+  L.build = o.build;
+  L.f     = db_forest(o.rest, m, m);
+  L.bytes = o.bytes();
   return L;
-}
-
-// one warp-per-position walk over the index, with the landmarks staged when they fit
-template <typename Kernel, typename... Args>
-static int db_rbc_walk(cudaStream_t s, Kernel kernel, int64_t m, int64_t d, int64_t nl, Args... args)
-{
-  size_t smem = 0;
-  const int rc = bc_query_smem(reinterpret_cast<const void*>(kernel), nl, d, &smem);
-  if (rc) return rc;
-  kernel<<<static_cast<unsigned>((m + kBcWarps - 1) / kBcWarps), kBcWarps * 32, smem, s>>>(args..., smem > 0);
-  B2D_CUDA(cudaGetLastError());
-  return B2D_OK;
 }
 
 template <int D>
 static int db_rbc_fit(cudaStream_t s, const DbRbcLayout& L, int root, const float* x, int64_t ldx, int n, int nl, float e,
                       unsigned ms, uint64_t seed)
 {
+  const DbForest& F = L.f;
   // 0. the index of x
   int rc = bc_build<D>(s, L.ix, L.build, x, ldx, n, nl, seed);
   if (rc) return rc;
   // 1. degrees, then the core flags; a NaN or negative eps matches nothing
   if (e >= 0.f) {
-    rc = db_rbc_walk(s, db_rbc_degree_kernel<D>, n, D, nl, L.ix, n, nl, root, e, ms, L.deg);
+    rc = bc_walk_launch(s, db_rbc_degree_kernel<D>, n, nl, D, L.ix, n, nl, root, e, ms, F.deg);
     if (rc) return rc;
   } else {
-    B2D_CUDA(cudaMemsetAsync(L.deg, 0, static_cast<size_t>(n) * sizeof(unsigned), s));
+    B2D_CUDA(cudaMemsetAsync(F.deg, 0, static_cast<size_t>(n) * sizeof(unsigned), s));
   }
-  db_core_kernel<<<sl_grid(n), 256, 0, s>>>(L.deg, n, n, ms, L.parent, L.border, L.core);
+  db_core_kernel<<<sl_grid(n), 256, 0, s>>>(F.deg, n, n, ms, F.parent, F.border, F.core);
   B2D_CUDA(cudaGetLastError());
   // 2. links between core points; 3. border points (no core point without a hit)
   if (e >= 0.f) {
-    rc = db_rbc_walk(s, db_rbc_link_kernel<D>, n, D, nl, L.ix, n, nl, root, e, static_cast<const unsigned*>(L.core),
-                     L.parent);
+    rc = bc_walk_launch(s, db_rbc_link_kernel<D>, n, nl, D, L.ix, n, nl, root, e, static_cast<const unsigned*>(F.core),
+                        F.parent);
     if (rc) return rc;
   }
-  db_rbc_compress_kernel<<<sl_grid(n), 256, 0, s>>>(L.parent, n, L.root);
+  db_compress_kernel<<<sl_grid(n), 256, 0, s>>>(F.parent, n, F.root);
   B2D_CUDA(cudaGetLastError());
   if (e >= 0.f) {
-    rc = db_rbc_walk(s, db_rbc_border_kernel<D>, n, D, nl, L.ix, n, nl, root, e, static_cast<const int*>(L.parent),
-                     L.border);
+    rc = bc_walk_launch(s, db_rbc_border_kernel<D>, n, nl, D, L.ix, n, nl, root, e, static_cast<const int*>(F.parent),
+                        F.border);
     if (rc) return rc;
   }
   return B2D_OK;
@@ -265,13 +261,6 @@ int b2d_dbscan_rbc_fit(void* stream, int metric, const float* x, int64_t ldx, in
   rc = d == 2 ? db_rbc_fit<2>(s, L, root, x, ldx, static_cast<int>(m), static_cast<int>(nl), e, ms, seed)
               : db_rbc_fit<3>(s, L, root, x, ldx, static_cast<int>(m), static_cast<int>(nl), e, ms, seed);
   if (rc) return rc;
-  // 4. cluster numbers = ranks of the roots; core_sample_indices positions = ranks of the core rows
-  rc = km_scan(s, nullptr, L.root, m, L.tiles, L.ctrl);
-  if (rc) return rc;
-  rc = km_scan(s, nullptr, L.core, m, L.tiles, L.ctrl + 1);
-  if (rc) return rc;
-  db_label_kernel<<<sl_grid(m), 256, 0, s>>>(L.parent, L.border, L.root, L.core, m, &L.ctrl[0].total, &L.ctrl[1].total,
-                                             labels, core_sample_indices, n_clusters);
-  B2D_CUDA(cudaGetLastError());
-  return B2D_OK;
+  // 4. the labels
+  return db_label(s, L.f, m, labels, core_sample_indices, n_clusters);
 }

@@ -4,7 +4,7 @@
 // points take the smallest root among the core columns of their row.
 //   db_core_kernel      degrees -> core flags, parent[i] = i (core) or -1, border[i] = INT_MAX
 //   db_link_kernel      per batch: every set byte (i, s + c) with both ends core unites their trees
-//   db_compress_kernel  parent[i] = root of i, root flags
+//   db_compress_kernel  parent[i] = root of i (a find that only reads), root flags
 //   db_border_kernel    per batch: every non-core row i, atomicMin of the smallest root among its core columns
 //   db_label_kernel     labels, core_sample_indices and n_clusters from the two scanned flag arrays
 // The union hooks the larger root under the smaller (CAS on parent), so the root of a component is its smallest core
@@ -97,14 +97,19 @@ __global__ void __launch_bounds__(kDbThreads) db_link_kernel(const uint8_t* adj,
   }
 }
 
-// parent[i] <- root of i for core rows; root[i] = 1 for the roots (i == its root), else 0
+// parent[i] <- root of i for core rows; root[i] = 1 for the roots (i == its root), else 0.  The find only reads: a
+// path-halving find (db_find) stores parent[v] = grandparent while walking, and can so overwrite the root another thread
+// just stored at v with a non-root ancestor, which the labels would then read.  Every value this find can see at a node
+// (the parent the links left, or the root stored here) is an ancestor, so it ends at the root, and its one store is
+// parent[i] = root.
 __global__ void db_compress_kernel(int* parent, int64_t m, unsigned* root)
 {
   const int64_t i = static_cast<int64_t>(blockIdx.x) * blockDim.x + threadIdx.x;
   if (i >= m) return;
-  int r = -1;
-  if (parent[i] >= 0) {
-    r         = db_find(parent, static_cast<int>(i));
+  const volatile int* p = parent;
+  int r = p[i];
+  if (r >= 0) {
+    for (int v = p[r]; v != r; v = p[r]) r = v;
     parent[i] = r;
   }
   root[i] = r == static_cast<int>(i) ? 1u : 0u;
@@ -149,22 +154,9 @@ __global__ void __launch_bounds__(kDbThreads) db_border_kernel(const uint8_t* ad
 // column's too.
 //   db_rbc_degree_kernel    deg[i] = the hits of row i, the walk ending once min_samples is reached
 //   db_rbc_link_kernel      core rows: every core hit j < i unites the trees of i and j
-//   db_rbc_compress_kernel  parent[i] = root of i, root flags, with a find that only reads
 //   db_rbc_border_kernel    non-core rows: border[i] = the smallest root (parent, compressed) among the core hits
-// The core flags and the labels are db_core_kernel (b = m) and db_label_kernel.
-
-// the point and caller row of position t; false: a NaN coordinate (the point is nobody's neighbour)
-template <int D>
-__device__ __forceinline__ bool db_rbc_query(const BcIndex& ix, int t, float (&q)[D], int* row)
-{
-  bool nan = false;
-  for (int c = 0; c < D; ++c) {
-    q[c] = ix.pts[static_cast<int64_t>(t) * D + c];
-    nan  = nan || isnan(q[c]);
-  }
-  *row = ix.ids[t];
-  return !nan;
-}
+// The core flags, the compression and the labels are db_core_kernel (b = m), db_compress_kernel and db_label_kernel.
+// A NaN query point (bc_query) is nobody's neighbour.
 
 template <int D>
 __global__ void __launch_bounds__(kBcWarps * 32) db_rbc_degree_kernel(BcIndex ix, int n, int nl, int root, float eps,
@@ -176,9 +168,10 @@ __global__ void __launch_bounds__(kBcWarps * 32) db_rbc_degree_kernel(BcIndex ix
   const int t    = blockIdx.x * kBcWarps + (threadIdx.x >> 5);
   if (t >= n) return;
   float q[D];
-  int row;
-  unsigned cnt = 0;
-  if (db_rbc_query<D>(ix, t, q, &row))
+  const bool ok = bc_query<D>(ix.pts + static_cast<int64_t>(t) * D, q);
+  const int row = ix.ids[t];
+  unsigned cnt  = 0;
+  if (ok)
     bc_eps_walk<D>(ix, n, nl, lm, rhi, q, root, eps, lane, [&](int, float, bool hit) {
       cnt += __popc(__ballot_sync(0xffffffffu, hit));
       return cnt >= min_samples;   // only the core test reads the degree
@@ -198,8 +191,9 @@ __global__ void __launch_bounds__(kBcWarps * 32) db_rbc_link_kernel(BcIndex ix, 
   const int t    = blockIdx.x * kBcWarps + (threadIdx.x >> 5);
   if (t >= n) return;
   float q[D];
-  int row;
-  if (!db_rbc_query<D>(ix, t, q, &row) || __ldg(&core[row]) == 0u) return;
+  const bool ok = bc_query<D>(ix.pts + static_cast<int64_t>(t) * D, q);
+  const int row = ix.ids[t];
+  if (!ok || __ldg(&core[row]) == 0u) return;
   int ri = -1;
   bc_eps_walk<D>(ix, n, nl, lm, rhi, q, root, eps, lane, [&](int i, float, bool hit) {
     if (hit) {
@@ -218,24 +212,6 @@ __global__ void __launch_bounds__(kBcWarps * 32) db_rbc_link_kernel(BcIndex ix, 
   });
 }
 
-// parent[i] <- root of i for core rows; root[i] = 1 for the roots, else 0.  db_compress_kernel's path-halving find writes
-// parent[v] = grandparent while walking, and can so overwrite the root another thread just stored at v with a non-root
-// ancestor, which the labels then read.  This find only reads: every value it can see at a node (the parent from the
-// link walk, or the root stored here) is an ancestor, so it ends at the root, and the only store is parent[i] = root.
-// The ball-cover fit's link order leaves deeper trees than the batched fit's, which makes that race likely there.
-__global__ void db_rbc_compress_kernel(int* parent, int64_t m, unsigned* root)
-{
-  const int64_t i = static_cast<int64_t>(blockIdx.x) * blockDim.x + threadIdx.x;
-  if (i >= m) return;
-  const volatile int* p = parent;
-  int r = p[i];
-  if (r >= 0) {
-    for (int v = p[r]; v != r; v = p[r]) r = v;
-    parent[i] = r;
-  }
-  root[i] = r == static_cast<int>(i) ? 1u : 0u;
-}
-
 // One warp owns each non-core row, so its smallest root is a plain store.
 template <int D>
 __global__ void __launch_bounds__(kBcWarps * 32) db_rbc_border_kernel(BcIndex ix, int n, int nl, int root, float eps,
@@ -247,8 +223,9 @@ __global__ void __launch_bounds__(kBcWarps * 32) db_rbc_border_kernel(BcIndex ix
   const int t    = blockIdx.x * kBcWarps + (threadIdx.x >> 5);
   if (t >= n) return;
   float q[D];
-  int row;
-  if (!db_rbc_query<D>(ix, t, q, &row) || __ldg(&parent[row]) >= 0) return;
+  const bool ok = bc_query<D>(ix.pts + static_cast<int64_t>(t) * D, q);
+  const int row = ix.ids[t];
+  if (!ok || __ldg(&parent[row]) >= 0) return;
   int best = INT_MAX;
   bc_eps_walk<D>(ix, n, nl, lm, rhi, q, root, eps, lane, [&](int i, float, bool hit) {
     if (hit) {

@@ -288,7 +288,7 @@ int radius_sort_split(cudaStream_t s, const int64_t* indptr, int64_t m, int64_t 
                       long long* alt, void* sort_tmp, size_t sort_bytes);
 
 // ------------------------------------------------------------------------------------------
-// ball_cover.cu: the index and its build, which DBSCAN's ball-cover fit runs too
+// ball_cover.cu: the index, its build and the walk launch, which DBSCAN's ball-cover fit and the EMST run too
 
 // n_landmarks, or ceil(sqrt(n)) for 0
 int64_t bc_landmarks(int64_t n, int64_t nl);
@@ -300,9 +300,14 @@ struct BcLayout {
 };
 BcLayout bc_layout(void* base, int64_t n, int64_t d, int64_t nl);
 
-// The build's workspace: two key and two value buffers of the radix sorts, and their scratch.  CUB reports its scratch
-// only with a device present; the onesweep sort needs its digit counters and one 1 KiB look-back row per tile of at
-// least 256 items of a 2^28-item portion, which the bound below covers (checked at run time).
+// Scratch bound of a onesweep radix sort of n items: its digit counters and one 1 KiB look-back row per tile of at least
+// 256 items of a 2^28-item portion.  CUB reports its scratch only with a device present, so the sorts check it at run time.
+inline size_t bc_sort_bytes(int64_t n)
+{
+  return 4 * static_cast<size_t>(std::min<int64_t>(n, int64_t(1) << 28)) + (static_cast<size_t>(1) << 20);
+}
+
+// The build's workspace: two key and two value buffers of the radix sorts, and their scratch (bc_sort_bytes).
 struct BcBuildLayout {
   unsigned long long* keys[2];
   int* vals[2];
@@ -312,14 +317,47 @@ struct BcBuildLayout {
 };
 BcBuildLayout bc_build_layout(void* base, int64_t n);
 
+// The workspace of a call that builds its own index: the index, then one region that holds first the build's scratch and,
+// once the index is built, the caller's arrays, carved from `rest` (256-byte aligned) over that scratch.
+struct BcOverlay {
+  BcIndex ix;
+  BcBuildLayout build;
+  size_t index_bytes;
+  Carve rest;
+
+  BcOverlay(void* base, int64_t n, int64_t d, int64_t nl)
+      : rest(nullptr, 256)
+  {
+    const BcLayout I = bc_layout(base, n, d, nl);
+    ix               = I.ix;
+    index_bytes      = I.bytes;   // a multiple of 256
+    rest.base        = base ? static_cast<char*>(base) + I.bytes : nullptr;
+    build            = bc_build_layout(rest.base, n);
+  }
+  size_t bytes() const { return index_bytes + std::max(build.bytes, rest.bytes); }
+};
+
 // the index of x [n][D] (pitch ldx) with nl landmarks into ix, scratch W (D = 2 and 3 are instantiated)
 template <int D>
 int bc_build(cudaStream_t s, const BcIndex& ix, const BcBuildLayout& W, const float* x, int64_t ldx, int n, int nl,
              uint64_t seed);
 
-// shared memory of a query launch of `kernel` (one of the ball_cover.cuh walks): the landmarks and their rhi when they
-// fit, else 0 (*bytes), set as the kernel's dynamic shared memory limit
-int bc_query_smem(const void* kernel, int64_t nl, int64_t d, size_t* bytes);
+constexpr size_t kBcSmemMax = 64 << 10;   // landmarks staged in shared memory up to this many bytes per block
+
+// One launch of a walk kernel of ball_cover.cuh (or of a walk built on it) over `items` queries or index positions:
+// one warp each, kBcWarps per block, with the nl landmarks of d coordinates and their rhi in dynamic shared memory when
+// they fit in kBcSmemMax.  The kernel takes args followed by the staging flag.
+template <typename Kernel, typename... Args>
+int bc_walk_launch(cudaStream_t s, Kernel kernel, int64_t items, int64_t nl, int64_t d, Args... args)
+{
+  size_t smem = static_cast<size_t>(nl) * (d + 1) * sizeof(float);
+  if (smem > kBcSmemMax) smem = 0;
+  B2D_CUDA(cudaFuncSetAttribute(reinterpret_cast<const void*>(kernel), cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                static_cast<int>(smem)));
+  kernel<<<static_cast<unsigned>((items + kBcWarps - 1) / kBcWarps), kBcWarps * 32, smem, s>>>(args..., smem > 0);
+  B2D_CUDA(cudaGetLastError());
+  return B2D_OK;
+}
 
 // ------------------------------------------------------------------------------------------
 // single_linkage.cu

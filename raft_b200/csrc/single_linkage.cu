@@ -303,12 +303,11 @@ struct EmstLayout {
 
 static EmstLayout emst_layout(void* base, int64_t m, int64_t d, int64_t nl, bool host_edges)
 {
+  BcOverlay o(base, m, d, nl);
+  Carve& c = o.rest;
   EmstLayout L{};
-  const BcLayout I = bc_layout(base, m, d, nl);
-  L.ix             = I.ix;
-  char* rest       = base ? static_cast<char*>(base) + I.bytes : nullptr;   // I.bytes is a multiple of 256
-  L.build          = bc_build_layout(rest, m);
-  Carve c(rest, 256);
+  L.ix     = o.ix;
+  L.build  = o.build;
   L.ctrl   = c.take<SlCtrl>(1);
   L.colour = c.take<int>(m);
   L.parent = c.take<int>(m);
@@ -324,10 +323,9 @@ static EmstLayout emst_layout(void* base, int64_t m, int64_t d, int64_t nl, bool
     L.hsrc = c.take<int>(m);
     L.hdst = c.take<int>(m);
   }
-  // onesweep scratch: at most one 1 KiB look-back row per tile of >= 256 items, as the build's (checked at run time)
-  L.sort_bytes = 4 * static_cast<size_t>(std::min<int64_t>(m, int64_t(1) << 28)) + (static_cast<size_t>(1) << 20);
+  L.sort_bytes = bc_sort_bytes(m);
   L.sort_tmp   = c.take<char>(L.sort_bytes);
-  L.bytes      = I.bytes + std::max(L.build.bytes, c.bytes);
+  L.bytes      = o.bytes();
   return L;
 }
 
@@ -363,18 +361,15 @@ static int emst_run(cudaStream_t s, const EmstLayout& L, int root, const float* 
   slr_pos_kernel<<<sl_grid(n), 256, 0, s>>>(L.ix.ids, n, L.pos);
   B2D_CUDA(cudaGetLastError());
   if (n < 2) return B2D_OK;
-  size_t smem = 0;
-  rc = bc_query_smem(reinterpret_cast<const void*>(slr_walk_kernel<D>), nl, D, &smem);
-  if (rc) return rc;
-  const unsigned wg = static_cast<unsigned>((n + kBcWarps - 1) / kBcWarps);
   const unsigned bg = static_cast<unsigned>((nl + kBcWarps - 1) / kBcWarps);
   const int rounds  = ceil_log2(n) + 1;   // the components at least halve in every round
   const int jumps   = std::min(kSlMaxJumps, ceil_log2(n) + 1);
   for (int r = 0; r < rounds; ++r) {
     sl_round_begin_kernel<<<sl_grid(std::max<int64_t>(n, kSlMaxJumps)), 256, 0, s>>>(L.ctrl, L.best1, n);
     slr_ball_kernel<<<bg, kBcWarps * 32, 0, s>>>(L.ctrl, L.ix.off, L.colour, nl, L.bcol);
-    slr_walk_kernel<D><<<wg, kBcWarps * 32, smem, s>>>(L.ctrl, L.ix, n, nl, L.colour, L.bcol, L.best1, L.best2, L.cand1,
-                                                       L.cand2, smem > 0);
+    rc = bc_walk_launch(s, slr_walk_kernel<D>, n, nl, D, L.ctrl, L.ix, n, nl, L.colour, L.bcol, L.best1, L.best2,
+                        L.cand1, L.cand2);
+    if (rc) return rc;
     slr_tie_kernel<<<sl_grid(n), 256, 0, s>>>(L.ctrl, L.colour, L.cand1, L.cand2, L.best1, L.best2, n);
     slr_hook_kernel<<<sl_grid(n), 256, 0, s>>>(L.ctrl, L.colour, L.pos, L.best1, L.best2, L.parent, L.mst1, L.mst2, n);
     for (int j = 0; j < jumps; ++j) sl_jump_kernel<<<sl_grid(n), 256, 0, s>>>(L.ctrl, L.colour, L.parent, n, j);

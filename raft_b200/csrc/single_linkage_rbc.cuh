@@ -53,12 +53,13 @@ __global__ void slr_ball_kernel(const SlCtrl* ctrl, const int* off, const int* c
 // (a1, a2) before (b1, b2) in the edge order
 __device__ __forceinline__ bool slr_before(long long a1, int a2, long long b1, int b2) { return a1 < b1 || (a1 == b1 && a2 < b2); }
 
-// The cross-component 1-NN state of one query row of a warp: its best edge (b1, b2) so far, the component slot's value
-// as last read (seen) and the distance bound dmax they give.
+// The cross-component 1-NN walker of one query row of a warp: its best edge (b1, b2) so far, the component slot's value
+// as last read (seen) and the distance bound dmax they give.  A ball of the query's colour is not admitted.
 template <int D>
 struct SlrWalk {
   const BcIndex& ix;
   const int* colour;
+  const int* bcol;
   long long* slot;   // best1 of the query's colour
   float q[D];
   int row, col, lane;
@@ -66,13 +67,16 @@ struct SlrWalk {
   int b2     = INT_MAX;
   float dmax = BC_INF;
 
-  __device__ __forceinline__ SlrWalk(const BcIndex& i, const int* c, long long* s) : ix(i), colour(c), slot(s) {}
+  __device__ __forceinline__ SlrWalk(const BcIndex& i, const int* c, const int* bc, long long* s)
+      : ix(i), colour(c), bcol(bc), slot(s) {}
+
+  __device__ __forceinline__ bool admit(int j) const { return bcol[j] != col; }
 
   // the bound is the smaller of the two s: a pair proven farther than bc_dhi(bound) has s > bound
   __device__ __forceinline__ void bound() { dmax = bc_dhi(fminf(key_bound(b1), key_bound(seen))); }
 
-  // the positions [lo, hi) of one ball at s = sq from the query (or the non-finite rows, sq = 0: nothing is pruned)
-  __device__ __forceinline__ void scan(int lo, int hi, float sq)
+  // the positions [lo, hi) of one ball at s = sq from the query, members of the query's colour skipped
+  __device__ __forceinline__ bool scan(int lo, int hi, float sq)
   {
     seen = min(seen, *reinterpret_cast<volatile long long*>(slot));
     bound();
@@ -108,14 +112,15 @@ struct SlrWalk {
     // an improvement is published at once, so that the component's other rows prune with it
     if (lane == 0 && b1 < seen) atomicMin(slot, b1);
     seen = min(seen, b1);
+    return false;
   }
 };
 
 // One warp per position t: the first edge in the order from t's row to a row of another colour, into cand1[t] /
-// cand2[t] and (atomicMin) best1[colour].  bc_knn_kernel's walk with k = 1 and a colour filter: a ball of the query's
-// colour and a member of it are skipped.  The bound also comes from the component's best1, read while the walk runs: it
-// only decreases, so every value read bounds the component's minimum.  Only the K19 margin helpers prune, and only what
-// is proven farther than bc_dhi(bound): such a pair has s > bound and orders strictly after it, so every pair at the
+// cand2[t] and (atomicMin) best1[colour].  bc_walk with the nearest ball first and SlrWalk: bc_knn_kernel's walk with
+// k = 1 and a colour filter.  The bound also comes from the component's best1, read while the walk runs: it only
+// decreases, so every value read bounds the component's minimum.  Only the K19 margin helpers prune, and only what is
+// proven farther than bc_dhi(bound): such a pair has s > bound and orders strictly after it, so every pair at the
 // bound's s (the ties the rows break) is still compared.
 template <int D>
 __global__ void __launch_bounds__(kBcWarps * 32) slr_walk_kernel(const SlCtrl* ctrl, BcIndex ix, int n, int nl,
@@ -128,42 +133,11 @@ __global__ void __launch_bounds__(kBcWarps * 32) slr_walk_kernel(const SlCtrl* c
   const int t = blockIdx.x * kBcWarps + (threadIdx.x >> 5);
   if (t >= n) return;
   const int col = colour[t];
-  SlrWalk<D> w(ix, colour, best1 + col);
-  w.lane   = threadIdx.x & 31;
-  w.row    = ix.ids[t];
-  w.col    = col;
-  bool nan = false;
-  for (int c = 0; c < D; ++c) {
-    w.q[c] = ix.pts[static_cast<int64_t>(t) * D + c];
-    nan    = nan || isnan(w.q[c]);
-  }
-  if (!nan) {
-    // the nearest ball of another colour first, then every other ball of another colour the bound does not rule out
-    long long near = KEY_EMPTY;
-    for (int j = w.lane; j < nl; j += 32)
-      if (rhi[j] >= 0.f && bcol[j] != col) near = min(near, key_pack(bc_s<D>(w.q, lm + j * D), j));
-    for (int o = 16; o > 0; o >>= 1) near = min(near, __shfl_xor_sync(0xffffffffu, near, o));
-    const int b0 = near == KEY_EMPTY ? -1 : static_cast<int>(key_index(near));
-    if (b0 >= 0) w.scan(ix.off[b0], ix.off[b0 + 1], key_dist(near));
-    for (int base = 0; base < nl; base += 32) {
-      const int j = base + w.lane;
-      float s     = 0.f;
-      bool want   = false;
-      if (j < nl && j != b0 && rhi[j] >= 0.f && bcol[j] != col) {
-        s    = bc_s<D>(w.q, lm + j * D);
-        want = !bc_ball_out(s, rhi[j], w.dmax);
-      }
-      unsigned mask = __ballot_sync(0xffffffffu, want);
-      while (mask) {
-        const int src  = __ffs(mask) - 1;
-        mask          &= mask - 1;
-        const float sj = __shfl_sync(0xffffffffu, s, src);
-        const int b    = base + src;
-        if (!bc_ball_out(sj, rhi[b], w.dmax)) w.scan(ix.off[b], ix.off[b + 1], sj);
-      }
-    }
-    w.scan(ix.off[nl], n, 0.f);
-  }
+  SlrWalk<D> w(ix, colour, bcol, best1 + col);
+  w.lane = threadIdx.x & 31;
+  w.row  = ix.ids[t];
+  w.col  = col;
+  if (bc_query<D>(ix.pts + static_cast<int64_t>(t) * D, w.q)) bc_walk<D, true>(ix, n, nl, lm, rhi, w.q, w.lane, w);
   if (w.lane == 0) {
     cand1[t] = w.b1;
     cand2[t] = w.b2;

@@ -19,8 +19,13 @@ METRIC_IDS = {"sqeuclidean": 0, "euclidean": 1, "cosine": 2}
 
 
 def make_data(kind, m, d, seed):
-    """blobs of several spreads with uniform noise around them, uniform points, or blobs of exact duplicates"""
+    """blobs of several spreads with uniform noise around them, uniform points, blobs of exact duplicates, or the integer
+    lattice 1 .. sqrt(m) in 2-D (every distance exact, massive ties: deep union-find trees; no zero row for cosine)"""
     rng = np.random.default_rng(seed)
+    if kind == "lattice":
+        side = int(round(m ** 0.5))
+        g = np.arange(1, side + 1)
+        return np.stack(np.meshgrid(g, g, indexing="ij"), -1).reshape(m, d).astype(np.float32)
     if kind == "uniform":
         return rng.uniform(-1, 1, (m, d)).astype(np.float32)
     centers = rng.uniform(-10, 10, (max(1, m // 150), d))
@@ -100,7 +105,8 @@ def raw_fit(xp, ldx, m, d, eps, min_samples, metric, max_bytes=0, stream=None):
 
 
 CASES = [("blobs", 1000, 32), ("blobs", 2049, 3), ("blobs", 1537, 128), ("blobs", 333, 320), ("uniform", 777, 2),
-         ("uniform", 1200, 33), ("uniform", 500, 1), ("dups", 900, 31), ("blobs", 1, 5), ("blobs", 2, 1), ("blobs", 17, 3)]
+         ("uniform", 1200, 33), ("uniform", 500, 1), ("dups", 900, 31), ("blobs", 1, 5), ("blobs", 2, 1), ("blobs", 17, 3),
+         ("lattice", 2500, 2)]
 
 
 @pytest.mark.parametrize("metric", ["euclidean", "sqeuclidean", "cosine"])
