@@ -562,6 +562,32 @@ size_t b2d_single_linkage_rbc_workspace_bytes(int64_t m, int64_t d, int64_t n_la
 int b2d_single_linkage_rbc(void* stream, int metric, const float* x, int64_t ldx, int64_t m, int64_t d,
                            int64_t n_landmarks, uint64_t seed, int n_clusters, int32_t* children, float* deltas,
                            int32_t* sizes, int32_t* labels, void* workspace, size_t workspace_bytes);
+/* HDBSCAN of 2-D and 3-D points (sklearn.cluster.HDBSCAN(metric="precomputed") on the matrix of b2d_emst_rbc's pair
+ * values; cuML's HDBSCAN without alpha and max_cluster_size), by the ball cover.  x:[m,d] fp32, row-major, pitch ldx >= d.
+ *   core_i = the min_samples-th smallest s(i, j) over every j, i included (s(i, i) = 0); pair (i, j) weighs
+ *     w = max(core_i, core_j, s(i, j)), and edges are ordered by (w, min(i, j), max(i, j)): the mutual-reachability tree
+ *     is unique.  mst_src / mst_dst / mst_w (device, capacity m - 1) receive its m - 1 edges in that order, src < dst,
+ *     w or its correctly rounded square root (B2D_L2SqrtUnexpanded), as b2d_emst_rbc writes its tree.
+ *   The tree stages run on the host on those edges, in that order, at the metric's distance: the single-linkage merges,
+ *     the condensed tree of min_cluster_size, the stabilities, the selection (method B2D_HDBSCAN_EOM or
+ *     B2D_HDBSCAN_LEAF, allow_single_cluster, cluster_selection_epsilon in the metric's units), labels [m] (int32,
+ *     device; -1 noise, clusters numbered in order of their smallest row) and probabilities [m] (fp32, device; fp64
+ *     arithmetic, lambda = 1 / distance and an infinite lambda as sklearn handles it).  *n_clusters (host) = the
+ *     cluster count.
+ * The results do not depend on seed, n_landmarks (in [0, m], 0 meaning ceil(sqrt(m))), the device or the scheduling.
+ * metric outside L2Unexpanded / L2SqrtUnexpanded, d outside {2, 3} and m >= 2^30 are B2D_ERR_UNSUPPORTED; m < 1, a
+ * negative or too large n_landmarks, ldx < d, min_samples outside [1, min(64, m)], min_cluster_size < 2, a negative or
+ * non-finite cluster_selection_epsilon, another method, allow_single_cluster outside {0, 1} and null pointers (the tree
+ * outputs may be null for m = 1) are B2D_ERR_INVALID_ARG; a non-finite x is B2D_ERR_INVALID_ARG, found on the device.
+ * The call synchronises its stream twice (the tree to the host, the labels back).  The workspace (256-byte aligned)
+ * depends on (m, d, n_landmarks) only; the query returns SIZE_MAX for arguments the call rejects. */
+#define B2D_HDBSCAN_EOM 0
+#define B2D_HDBSCAN_LEAF 1
+size_t b2d_hdbscan_rbc_workspace_bytes(int64_t m, int64_t d, int64_t n_landmarks);
+int b2d_hdbscan_rbc_fit(void* stream, int metric, const float* x, int64_t ldx, int64_t m, int64_t d, int min_samples,
+                        int min_cluster_size, double cluster_selection_epsilon, int method, int allow_single_cluster,
+                        int64_t n_landmarks, uint64_t seed, int32_t* labels, float* probabilities, int32_t* mst_src,
+                        int32_t* mst_dst, float* mst_w, int32_t* n_clusters, void* workspace, size_t workspace_bytes);
 
 /* DBSCAN (cuML's DBSCAN(eps, min_samples, metric, max_mbytes_per_batch), sklearn.cluster.DBSCAN's labels_ and
  * core_sample_indices_) for fp32 x:[m,d] (row-major, pitch ldx), on the epsilon neighbourhood of b2d_eps_neighbors_l2sq.

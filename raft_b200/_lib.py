@@ -30,10 +30,12 @@ SYMBOLS = [
     "b2d_ball_cover_eps_workspace_bytes", "b2d_ball_cover_eps_count", "b2d_ball_cover_eps_fill",
     "b2d_dbscan_rbc_workspace_bytes", "b2d_dbscan_rbc_fit",
     "b2d_emst_rbc_workspace_bytes", "b2d_emst_rbc", "b2d_single_linkage_rbc_workspace_bytes", "b2d_single_linkage_rbc",
+    "b2d_hdbscan_rbc_workspace_bytes", "b2d_hdbscan_rbc_fit",
 ]
 
 B2D_OK, B2D_ERR_INVALID_ARG, B2D_ERR_CUDA, B2D_ERR_UNSUPPORTED, B2D_ERR_WORKSPACE = range(5)
 B2D_F32, B2D_F16, B2D_F64 = 0, 1, 2
+B2D_HDBSCAN_EOM, B2D_HDBSCAN_LEAF = range(2)
 B2D_KERNEL_LINEAR, B2D_KERNEL_POLYNOMIAL, B2D_KERNEL_RBF, B2D_KERNEL_TANH = range(4)
 B2D_KMEANS_INIT_PLUS_PLUS, B2D_KMEANS_INIT_RANDOM, B2D_KMEANS_INIT_ARRAY = range(3)
 (B2D_KDE_GAUSSIAN, B2D_KDE_TOPHAT, B2D_KDE_EPANECHNIKOV, B2D_KDE_EXPONENTIAL, B2D_KDE_LINEAR,
@@ -169,6 +171,11 @@ def lib() -> ctypes.CDLL:
     L.b2d_single_linkage_rbc_workspace_bytes.argtypes = [i64, i64, i64]
     L.b2d_single_linkage_rbc.restype = ci
     L.b2d_single_linkage_rbc.argtypes = [vp, ci, vp, i64, i64, i64, i64, u64, ci, vp, vp, vp, vp, vp, sz]
+    L.b2d_hdbscan_rbc_workspace_bytes.restype = sz
+    L.b2d_hdbscan_rbc_workspace_bytes.argtypes = [i64, i64, i64]
+    L.b2d_hdbscan_rbc_fit.restype = ci
+    L.b2d_hdbscan_rbc_fit.argtypes = [vp, ci, vp, i64, i64, i64, ci, ci, cd, ci, ci, i64, u64, vp, vp, vp, vp, vp, vp,
+                                      vp, sz]
     L.b2d_radius_neighbors_workspace_bytes.restype = sz
     L.b2d_radius_neighbors_workspace_bytes.argtypes = [i64, i64, i64, i64]
     L.b2d_radius_neighbors_count.restype = ci

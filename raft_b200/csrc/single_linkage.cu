@@ -5,6 +5,8 @@
 #include <vector>
 #include <cub/device/device_radix_sort.cuh>
 
+#include "hdbscan_rbc.cuh"
+#include "hdbscan_tree.cuh"
 #include "host.cuh"
 #include "single_linkage.cuh"
 #include "single_linkage_rbc.cuh"
@@ -232,34 +234,15 @@ static int sl_read_ctrl(cudaStream_t s, const SlCtrl* d, SlCtrl* h)
   return B2D_OK;
 }
 
-static int uf_find(std::vector<int>& p, int v)
-{
-  while (p[v] != v) v = p[v] = p[p[v]];
-  return v;
-}
-
 // Step 5 of single_linkage: the m - 1 tree edges (hs[t], hd[t]) in key order merged on the host into children, sizes and
 // labels (device pointers; children and sizes unused for m = 1).  Synchronises the stream.
 static int sl_dendrogram(cudaStream_t s, int64_t m, int64_t n_clusters, const std::vector<int>& hs,
                          const std::vector<int>& hd, int32_t* children, int32_t* sizes, int32_t* labels)
 {
-  std::vector<int> uf(m), cid(m), sz(m, 1), hch(2 * (m - 1)), hsz(m - 1), hlab(m);
-  for (int64_t i = 0; i < m; ++i) uf[i] = cid[i] = static_cast<int>(i);
-  const int64_t cut = m - n_clusters;   // labels: the components after the first m - n_clusters merges
-  for (int64_t t = 0; t < m - 1; ++t) {
-    if (t == cut)
-      for (int64_t i = 0; i < m; ++i) hlab[i] = uf_find(uf, static_cast<int>(i));
-    const int a = uf_find(uf, hs[t]), b = uf_find(uf, hd[t]);
-    if (a == b) return fail(B2D_ERR_CUDA, "internal: the spanning tree has a cycle");
-    hch[2 * t]     = std::min(cid[a], cid[b]);
-    hch[2 * t + 1] = std::max(cid[a], cid[b]);
-    hsz[t]         = sz[a] + sz[b];
-    uf[b]          = a;
-    sz[a]          = hsz[t];
-    cid[a]         = static_cast<int>(m + t);
-  }
-  if (cut == m - 1)
-    for (int64_t i = 0; i < m; ++i) hlab[i] = uf_find(uf, static_cast<int>(i));
+  std::vector<int> hch(2 * (m - 1)), hsz(m - 1), hlab(m);
+  // labels: the components after the first m - n_clusters merges
+  if (!sl_merges(m, hs.data(), hd.data(), hch.data(), hsz.data(), m - n_clusters, hlab.data()))
+    return fail(B2D_ERR_CUDA, "internal: the spanning tree has a cycle");
   std::vector<int> num(m, -1);   // numbered in order of each cluster's smallest row
   int next_label = 0;
   for (int64_t i = 0; i < m; ++i) {
@@ -296,12 +279,14 @@ struct EmstLayout {
   long long* mst1;    // [m] the tree edges as appended: (s, min row) ...
   int* mst2;          // [m] ... and max row
   int *hsrc, *hdst;   // [m] single_linkage_rbc: the edges in order, for the host
+  float* core;        // [m] HDBSCAN: the core distance of every position ...
+  float* cmin;        // [nl] ... and the smallest of every ball
   void* sort_tmp;
   size_t sort_bytes;
   size_t bytes;
 };
 
-static EmstLayout emst_layout(void* base, int64_t m, int64_t d, int64_t nl, bool host_edges)
+static EmstLayout emst_layout(void* base, int64_t m, int64_t d, int64_t nl, bool host_edges, bool mr = false)
 {
   BcOverlay o(base, m, d, nl);
   Carve& c = o.rest;
@@ -322,6 +307,10 @@ static EmstLayout emst_layout(void* base, int64_t m, int64_t d, int64_t nl, bool
   if (host_edges) {
     L.hsrc = c.take<int>(m);
     L.hdst = c.take<int>(m);
+  }
+  if (mr) {
+    L.core = c.take<float>(m);
+    L.cmin = c.take<float>(nl);
   }
   L.sort_bytes = bc_sort_bytes(m);
   L.sort_tmp   = c.take<char>(L.sort_bytes);
@@ -349,10 +338,12 @@ static bool emst_extents_ok(int64_t m, int64_t d, int64_t nl)
   return m >= 1 && m < kSlMaxRows && (d == 2 || d == 3) && nl >= 0 && nl <= m;
 }
 
-// the index, the rounds, and the m - 1 tree edges sorted into (s, min row, max row) order as (out_src, out_dst, out_w)
+// The index, the rounds, and the m - 1 tree edges sorted into (s, min row, max row) order as (out_src, out_dst, out_w).
+// min_samples > 0 (HDBSCAN): the core distances first, and the rounds weigh pairs by mutual reachability, (s, ...)
+// reading (w, ...).
 template <int D>
 static int emst_run(cudaStream_t s, const EmstLayout& L, int root, const float* x, int64_t ldx, int n, int nl,
-                    uint64_t seed, int* out_src, int* out_dst, float* out_w)
+                    uint64_t seed, int* out_src, int* out_dst, float* out_w, int min_samples = 0)
 {
   int rc = bc_build<D>(s, L.ix, L.build, x, ldx, n, nl, seed);
   if (rc) return rc;
@@ -362,13 +353,23 @@ static int emst_run(cudaStream_t s, const EmstLayout& L, int root, const float* 
   B2D_CUDA(cudaGetLastError());
   if (n < 2) return B2D_OK;
   const unsigned bg = static_cast<unsigned>((nl + kBcWarps - 1) / kBcWarps);
+  if (min_samples > 0) {
+    rc = bc_walk_launch(s, hdb_core_kernel<D>, n, nl, D, L.ix, n, nl, min_samples, L.core);
+    if (rc) return rc;
+    hdb_cmin_kernel<<<bg, kBcWarps * 32, 0, s>>>(L.ix.off, L.core, nl, L.cmin);
+    B2D_CUDA(cudaGetLastError());
+  }
   const int rounds  = ceil_log2(n) + 1;   // the components at least halve in every round
   const int jumps   = std::min(kSlMaxJumps, ceil_log2(n) + 1);
   for (int r = 0; r < rounds; ++r) {
     sl_round_begin_kernel<<<sl_grid(std::max<int64_t>(n, kSlMaxJumps)), 256, 0, s>>>(L.ctrl, L.best1, n);
     slr_ball_kernel<<<bg, kBcWarps * 32, 0, s>>>(L.ctrl, L.ix.off, L.colour, nl, L.bcol);
-    rc = bc_walk_launch(s, slr_walk_kernel<D>, n, nl, D, L.ctrl, L.ix, n, nl, L.colour, L.bcol, L.best1, L.best2,
-                        L.cand1, L.cand2);
+    if (min_samples > 0)
+      rc = bc_walk_launch(s, hdb_walk_kernel<D>, n, nl, D, L.ctrl, L.ix, n, nl, L.colour, L.bcol, L.core, L.cmin,
+                          L.best1, L.best2, L.cand1, L.cand2);
+    else
+      rc = bc_walk_launch(s, slr_walk_kernel<D>, n, nl, D, L.ctrl, L.ix, n, nl, L.colour, L.bcol, L.best1, L.best2,
+                          L.cand1, L.cand2);
     if (rc) return rc;
     slr_tie_kernel<<<sl_grid(n), 256, 0, s>>>(L.ctrl, L.colour, L.cand1, L.cand2, L.best1, L.best2, n);
     slr_hook_kernel<<<sl_grid(n), 256, 0, s>>>(L.ctrl, L.colour, L.pos, L.best1, L.best2, L.parent, L.mst1, L.mst2, n);
@@ -394,11 +395,13 @@ static int emst_run(cudaStream_t s, const EmstLayout& L, int root, const float* 
 }
 
 static int emst_dispatch(cudaStream_t s, const EmstLayout& L, int metric, const float* x, int64_t ldx, int64_t m,
-                         int64_t d, int64_t nl, uint64_t seed, int* out_src, int* out_dst, float* out_w)
+                         int64_t d, int64_t nl, uint64_t seed, int* out_src, int* out_dst, float* out_w,
+                         int min_samples = 0)
 {
   const int root = metric == B2D_L2SqrtUnexpanded;
-  return d == 2 ? emst_run<2>(s, L, root, x, ldx, static_cast<int>(m), static_cast<int>(nl), seed, out_src, out_dst, out_w)
-                : emst_run<3>(s, L, root, x, ldx, static_cast<int>(m), static_cast<int>(nl), seed, out_src, out_dst, out_w);
+  const int n = static_cast<int>(m), l = static_cast<int>(nl);
+  return d == 2 ? emst_run<2>(s, L, root, x, ldx, n, l, seed, out_src, out_dst, out_w, min_samples)
+                : emst_run<3>(s, L, root, x, ldx, n, l, seed, out_src, out_dst, out_w, min_samples);
 }
 }  // namespace
 
@@ -580,4 +583,68 @@ int b2d_single_linkage_rbc(void* stream, int metric, const float* x, int64_t ldx
     return fail(B2D_ERR_CUDA, "internal: the rounds chose " + std::to_string(h.n_mst) + " of " + std::to_string(m - 1) +
                                   " tree edges");
   return sl_dendrogram(s, m, n_clusters, hs, hd, children, sizes, labels);
+}
+
+// ------------------------------------------------------------------------------------------
+// HDBSCAN of 2-D and 3-D points (hdbscan_rbc.cuh, hdbscan_tree.cuh): the core distances and the mutual-reachability tree
+// by the EMST's rounds, then the tree stages on the host.
+
+size_t b2d_hdbscan_rbc_workspace_bytes(int64_t m, int64_t d, int64_t n_landmarks)
+{
+  if (!emst_extents_ok(m, d, n_landmarks)) return static_cast<size_t>(-1);
+  return emst_layout(nullptr, m, d, bc_landmarks(m, n_landmarks), false, true).bytes;
+}
+
+int b2d_hdbscan_rbc_fit(void* stream, int metric, const float* x, int64_t ldx, int64_t m, int64_t d, int min_samples,
+                        int min_cluster_size, double cluster_selection_epsilon, int method, int allow_single_cluster,
+                        int64_t n_landmarks, uint64_t seed, int32_t* labels, float* probabilities, int32_t* mst_src,
+                        int32_t* mst_dst, float* mst_w, int32_t* n_clusters, void* workspace, size_t workspace_bytes)
+{
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  int rc         = emst_args("hdbscan rbc", metric, x, ldx, m, d, n_landmarks);
+  if (rc) return rc;
+  if (min_samples < 1 || min_samples > std::min<int64_t>(KNN_MAX_K, m))
+    return fail(B2D_ERR_INVALID_ARG, "min_samples must be in [1, min(64, m)], got " + std::to_string(min_samples));
+  if (min_cluster_size < 2)
+    return fail(B2D_ERR_INVALID_ARG, "min_cluster_size must be at least 2, got " + std::to_string(min_cluster_size));
+  if (!(cluster_selection_epsilon >= 0.0) || std::isinf(cluster_selection_epsilon))
+    return fail(B2D_ERR_INVALID_ARG, "cluster_selection_epsilon must be finite and non-negative");
+  if (method != B2D_HDBSCAN_EOM && method != B2D_HDBSCAN_LEAF)
+    return fail(B2D_ERR_INVALID_ARG, "method must be B2D_HDBSCAN_EOM or B2D_HDBSCAN_LEAF, got " + std::to_string(method));
+  if (allow_single_cluster != 0 && allow_single_cluster != 1)
+    return fail(B2D_ERR_INVALID_ARG, "allow_single_cluster must be 0 or 1");
+  if (!labels || !probabilities || !n_clusters || (m > 1 && (!mst_src || !mst_dst || !mst_w)))
+    return fail(B2D_ERR_INVALID_ARG, "null labels / probabilities / mst_src / mst_dst / mst_w / n_clusters");
+  const int64_t nl = bc_landmarks(m, n_landmarks);
+  rc = check_workspace(workspace, workspace_bytes, emst_layout(nullptr, m, d, nl, false, true).bytes);
+  if (rc) return rc;
+  const EmstLayout L = emst_layout(workspace, m, d, nl, false, true);
+  // 1.-2. the index, the core distances and the tree edges in (w, min row, max row) order
+  rc = emst_dispatch(s, L, metric, x, ldx, m, d, nl, seed, mst_src, mst_dst, mst_w, min_samples);
+  if (rc) return rc;
+  sl_finite_kernel<<<km_grid(m * d), 256, 0, s>>>(x, ldx, m, static_cast<int>(d), L.ctrl);
+  B2D_CUDA(cudaGetLastError());
+  // 3. the tree stages on the host (the one synchronisation before it reads the control words and the edges)
+  SlCtrl h;
+  std::vector<int> hs(m - 1), hd(m - 1), hl(m);
+  std::vector<float> hw(m - 1), hp(m);
+  B2D_CUDA(cudaMemcpyAsync(&h, L.ctrl, sizeof(SlCtrl), cudaMemcpyDeviceToHost, s));
+  if (m > 1) {
+    B2D_CUDA(cudaMemcpyAsync(hs.data(), mst_src, (m - 1) * sizeof(int), cudaMemcpyDeviceToHost, s));
+    B2D_CUDA(cudaMemcpyAsync(hd.data(), mst_dst, (m - 1) * sizeof(int), cudaMemcpyDeviceToHost, s));
+    B2D_CUDA(cudaMemcpyAsync(hw.data(), mst_w, (m - 1) * sizeof(float), cudaMemcpyDeviceToHost, s));
+  }
+  B2D_CUDA(cudaStreamSynchronize(s));
+  if (h.bad & 1u) return fail(B2D_ERR_INVALID_ARG, "hdbscan rbc: X holds a non-finite value");
+  if (m > 1 && h.n_mst != static_cast<unsigned>(m - 1))
+    return fail(B2D_ERR_CUDA, "internal: the rounds chose " + std::to_string(h.n_mst) + " of " + std::to_string(m - 1) +
+                                  " tree edges");
+  const HdbTreeParams P{min_cluster_size, cluster_selection_epsilon, method == B2D_HDBSCAN_LEAF, allow_single_cluster != 0};
+  const int nc = hdbscan_tree(m, hs.data(), hd.data(), hw.data(), P, hl.data(), hp.data());
+  if (nc < 0) return fail(B2D_ERR_CUDA, "internal: the spanning tree has a cycle");
+  B2D_CUDA(cudaMemcpyAsync(labels, hl.data(), m * sizeof(int), cudaMemcpyHostToDevice, s));
+  B2D_CUDA(cudaMemcpyAsync(probabilities, hp.data(), m * sizeof(float), cudaMemcpyHostToDevice, s));
+  B2D_CUDA(cudaStreamSynchronize(s));
+  *n_clusters = nc;
+  return B2D_OK;
 }

@@ -55,7 +55,11 @@ __device__ __forceinline__ bool slr_before(long long a1, int a2, long long b1, i
 
 // The cross-component 1-NN walker of one query row of a warp: its best edge (b1, b2) so far, the component slot's value
 // as last read (seen) and the distance bound dmax they give.  A ball of the query's colour is not admitted.
-template <int D>
+// Mr (HDBSCAN, hdbscan_rbc.cuh): pair (i, j) weighs w = max(core_i, core_j, s) instead of s, and the walk prunes by the
+// core distances too (core: by position, cmin: the smallest core of every ball, cq: the query's).  Each prune is strict
+// against the bound wb, so a pair at the bound's weight is still compared.  Since w >= s, the window and ball tests on s
+// stay valid at bc_dhi(wb).
+template <int D, bool Mr = false>
 struct SlrWalk {
   const BcIndex& ix;
   const int* colour;
@@ -66,20 +70,38 @@ struct SlrWalk {
   long long b1 = KEY_EMPTY, seen = KEY_EMPTY;
   int b2     = INT_MAX;
   float dmax = BC_INF;
+  const float* core = nullptr;
+  const float* cmin = nullptr;
+  float cq = 0.f;
+  float wb = BC_INF;   // Mr: the bound itself
 
   __device__ __forceinline__ SlrWalk(const BcIndex& i, const int* c, const int* bc, long long* s)
       : ix(i), colour(c), bcol(bc), slot(s) {}
 
-  __device__ __forceinline__ bool admit(int j) const { return bcol[j] != col; }
+  // Mr: a ball whose every pair weighs more than the bound (max(cq, cmin) > wb) is not admitted either
+  __device__ __forceinline__ bool admit(int j) const
+  {
+    if constexpr (Mr) return bcol[j] != col && !(fmaxf(cq, cmin[j]) > wb);
+    return bcol[j] != col;
+  }
 
-  // the bound is the smaller of the two s: a pair proven farther than bc_dhi(bound) has s > bound
-  __device__ __forceinline__ void bound() { dmax = bc_dhi(fminf(key_bound(b1), key_bound(seen))); }
+  // the bound is the smaller of the two weights: a pair proven farther than bc_dhi(bound) has s > bound, so w > bound
+  __device__ __forceinline__ void bound()
+  {
+    const float b = fminf(key_bound(b1), key_bound(seen));
+    if constexpr (Mr) wb = b;
+    dmax = bc_dhi(b);
+  }
 
-  // the positions [lo, hi) of one ball at s = sq from the query, members of the query's colour skipped
+  // the positions [lo, hi) of one ball at s = sq from the query, members of the query's colour skipped.  Mr: true (the
+  // walk ends) once the query's own core distance exceeds the bound on some lane, whose read of the slot bounds the
+  // component's minimum: every pair of the row then orders after it
   __device__ __forceinline__ bool scan(int lo, int hi, float sq)
   {
     seen = min(seen, *reinterpret_cast<volatile long long*>(slot));
     bound();
+    if constexpr (Mr)
+      if (__any_sync(0xffffffffu, cq > wb)) return true;
     float wlo, whi;
     bc_window(sq, dmax, &wlo, &whi);
     for (int p = bc_search(ix.rl, lo, hi, wlo, false); p < hi; p += 32) {
@@ -89,11 +111,23 @@ struct SlrWalk {
       long long k1   = KEY_EMPTY;
       int k2         = INT_MAX;
       if (i < hi && !out && r >= wlo && colour[i] != col) {
-        const float s = bc_s<D>(q, ix.pts + static_cast<int64_t>(i) * D);
-        if (s == s) {
-          const int j = ix.ids[i];
-          k1          = key_pack(s, min(row, j));
-          k2          = max(row, j);
+        if constexpr (Mr) {
+          const float cp = core[i];   // a member above the bound is not measured
+          if (!(cp > wb)) {
+            const float s = bc_s<D>(q, ix.pts + static_cast<int64_t>(i) * D);
+            if (s == s) {
+              const int j = ix.ids[i];
+              k1          = key_pack(fmaxf(fmaxf(cq, cp), s), min(row, j));
+              k2          = max(row, j);
+            }
+          }
+        } else {
+          const float s = bc_s<D>(q, ix.pts + static_cast<int64_t>(i) * D);
+          if (s == s) {
+            const int j = ix.ids[i];
+            k1          = key_pack(s, min(row, j));
+            k2          = max(row, j);
+          }
         }
       }
       if (__any_sync(0xffffffffu, slr_before(k1, k2, b1, b2))) {
