@@ -588,6 +588,48 @@ int b2d_hdbscan_rbc_fit(void* stream, int metric, const float* x, int64_t ldx, i
                         int min_cluster_size, double cluster_selection_epsilon, int method, int allow_single_cluster,
                         int64_t n_landmarks, uint64_t seed, int32_t* labels, float* probabilities, int32_t* mst_src,
                         int32_t* mst_dst, float* mst_w, int32_t* n_clusters, void* workspace, size_t workspace_bytes);
+/* HDBSCAN with a persisted model, for approximate_predict (the hdbscan package's and cuML's, exact here; DESIGN.md K23).
+ * b2d_hdbscan_rbc_fit_model is b2d_hdbscan_rbc_fit (same arguments, checks, errors, workspace and outputs, bit for bit)
+ * that also fills model (device, 256-byte aligned, b2d_hdbscan_rbc_model_bytes(m, d, n_landmarks) bytes; null or
+ * misaligned is B2D_ERR_INVALID_ARG, checked after the fit's arguments): its own copy of the fit's ball-cover index, the
+ * core distances and the condensed tree.  The model size depends on (m, d, n_landmarks) only; the query returns SIZE_MAX
+ * for the extents the fit rejects.
+ *
+ * b2d_hdbscan_rbc_approximate_predict places mq new points q:[mq,d] (fp32, device, pitch ldq >= d) in the fitted
+ * clustering.  m, d, metric, n_landmarks and min_samples are the fit's (the model records none of them).  X is the m
+ * fitted rows, s(q, j) the pair value of b2d_emst_rbc (unexpanded, every operation rounded), core_j the fit's core
+ * distance of row j; the "metric value" of an s-domain weight is the weight (B2D_L2Unexpanded) or its correctly rounded
+ * fp32 root (B2D_L2SqrtUnexpanded), as the fit writes mst_w.  For each query:
+ *   1. core_q = the min_samples-th smallest s(q, j) over the m fitted rows (a fitted row bit-equal to q counts, at 0).
+ *   2. Every fitted row weighs w_j = max(core_q, core_j, s(q, j)); the neighbour j* is the first row in the strict
+ *      order (w, s, row): ties on w go to the smaller s, as an arg-min over distance-sorted neighbours does.  The search
+ *      is exact over all m rows, not over the 2 min_samples nearest as in the hdbscan package's approximate_predict.
+ *   3. W = the metric value of w_{j*}; lambda_q = min(1 / W, lambda_{j*}) in fp64 (1 / 0 = +inf), lambda_{j*} = the
+ *      lambda at which j* leaves its parent cluster in the fit's condensed tree.
+ *   4. p = the condensed parent of j*; while p is not the root and birth(p) > lambda_q, p = parent(p) (a query exactly at
+ *      a cluster's birth stays inside it).
+ *   5. The fit's label rule on (p, lambda_q): the owner is the nearest selected ancestor of p, p included.  Not the
+ *      root: the fit's label of that cluster (-1 if no fitted row took it).  The root: the root's label when it is the
+ *      one selected cluster (allow_single_cluster) and lambda_q >= the fit's threshold, else -1.  probabilities[q] =
+ *      md == 0 || lambda_q == inf ? 1 : min(lambda_q, md) / md with md the owner's death (fp64, rounded to fp32), 0 for
+ *      noise.
+ *   6. nn_rows[q] = j* (int32) and nn_w[q] = W (fp32); either may be null.
+ *   7. A query with a non-finite coordinate gets label -1, probability 0, neighbour -1 and W = +inf.
+ * On data without duplicate rows, a query bit-equal to fitted row i gets the fit's labels[i] and probabilities[i].  The
+ * results do not depend on n_landmarks, seed, the device, the order of the queries or the batching.  The call only
+ * enqueues work (no synchronisation, no allocation, CUDA-graph capturable) and needs no workspace.  metric outside
+ * L2Unexpanded / L2SqrtUnexpanded and d outside {2, 3} are B2D_ERR_UNSUPPORTED; m outside [1, 2^30), n_landmarks
+ * outside [0, m], min_samples outside [1, min(64, m)], a null or misaligned model, mq outside [0, 2^31), ldq < d and
+ * null q / labels / probabilities (mq > 0) are B2D_ERR_INVALID_ARG.  mq = 0 does nothing. */
+size_t b2d_hdbscan_rbc_model_bytes(int64_t m, int64_t d, int64_t n_landmarks);
+int b2d_hdbscan_rbc_fit_model(void* stream, int metric, const float* x, int64_t ldx, int64_t m, int64_t d,
+                              int min_samples, int min_cluster_size, double cluster_selection_epsilon, int method,
+                              int allow_single_cluster, int64_t n_landmarks, uint64_t seed, int32_t* labels,
+                              float* probabilities, int32_t* mst_src, int32_t* mst_dst, float* mst_w, int32_t* n_clusters,
+                              void* workspace, size_t workspace_bytes, void* model);
+int b2d_hdbscan_rbc_approximate_predict(void* stream, const void* model, int64_t m, int64_t d, int metric,
+                                        int64_t n_landmarks, int min_samples, const float* q, int64_t ldq, int64_t mq,
+                                        int32_t* labels, float* probabilities, int32_t* nn_rows, float* nn_w);
 
 /* DBSCAN (cuML's DBSCAN(eps, min_samples, metric, max_mbytes_per_batch), sklearn.cluster.DBSCAN's labels_ and
  * core_sample_indices_) for fp32 x:[m,d] (row-major, pitch ldx), on the epsilon neighbourhood of b2d_eps_neighbors_l2sq.

@@ -30,7 +30,8 @@ SYMBOLS = [
     "b2d_ball_cover_eps_workspace_bytes", "b2d_ball_cover_eps_count", "b2d_ball_cover_eps_fill",
     "b2d_dbscan_rbc_workspace_bytes", "b2d_dbscan_rbc_fit",
     "b2d_emst_rbc_workspace_bytes", "b2d_emst_rbc", "b2d_single_linkage_rbc_workspace_bytes", "b2d_single_linkage_rbc",
-    "b2d_hdbscan_rbc_workspace_bytes", "b2d_hdbscan_rbc_fit",
+    "b2d_hdbscan_rbc_workspace_bytes", "b2d_hdbscan_rbc_fit", "b2d_hdbscan_rbc_model_bytes", "b2d_hdbscan_rbc_fit_model",
+    "b2d_hdbscan_rbc_approximate_predict",
 ]
 
 B2D_OK, B2D_ERR_INVALID_ARG, B2D_ERR_CUDA, B2D_ERR_UNSUPPORTED, B2D_ERR_WORKSPACE = range(5)
@@ -176,6 +177,13 @@ def lib() -> ctypes.CDLL:
     L.b2d_hdbscan_rbc_fit.restype = ci
     L.b2d_hdbscan_rbc_fit.argtypes = [vp, ci, vp, i64, i64, i64, ci, ci, cd, ci, ci, i64, u64, vp, vp, vp, vp, vp, vp,
                                       vp, sz]
+    L.b2d_hdbscan_rbc_model_bytes.restype = sz
+    L.b2d_hdbscan_rbc_model_bytes.argtypes = [i64, i64, i64]
+    L.b2d_hdbscan_rbc_fit_model.restype = ci
+    L.b2d_hdbscan_rbc_fit_model.argtypes = [vp, ci, vp, i64, i64, i64, ci, ci, cd, ci, ci, i64, u64, vp, vp, vp, vp, vp,
+                                            vp, vp, sz, vp]
+    L.b2d_hdbscan_rbc_approximate_predict.restype = ci
+    L.b2d_hdbscan_rbc_approximate_predict.argtypes = [vp, vp, i64, i64, ci, i64, ci, vp, i64, i64, vp, vp, vp, vp]
     L.b2d_radius_neighbors_workspace_bytes.restype = sz
     L.b2d_radius_neighbors_workspace_bytes.argtypes = [i64, i64, i64, i64]
     L.b2d_radius_neighbors_count.restype = ci

@@ -2,7 +2,8 @@
 // ball cover's kNN walk, then the mutual-reachability minimum spanning tree by the EMST's Borůvka rounds
 // (single_linkage_rbc.cuh) with the walker's Mr weight (DESIGN.md K22).  Everything is in the s domain: core[p] is the
 // min_samples-th smallest s of the row at position p (the row itself included), and pair (i, j) weighs
-// w = max(core_i, core_j, s(i, j)).  The tree stages run on the host (hdbscan_tree.cuh).
+// w = max(core_i, core_j, s(i, j)).  The tree stages run on the host (hdbscan_tree.cuh).  approximate_predict places new
+// points in a fitted model (hdb_predict_kernel, DESIGN.md K23).
 #pragma once
 #include "single_linkage_rbc.cuh"
 
@@ -65,6 +66,98 @@ __global__ void __launch_bounds__(kBcWarps * 32) hdb_walk_kernel(const SlCtrl* c
     cand2[t] = w.b2;
     best2[t] = INT_MAX;
   }
+}
+
+// A fitted model as the predict kernel reads it (its regions: hdb_model_layout in single_linkage.cu): the fit's index,
+// core by position, cmin by ball, pos by row, and the condensed tree of HdbTreeExport (rows by caller row, clusters by
+// id).
+struct HdbModelHead {
+  double thr;
+  int single_root;
+  int n_clusters;
+};
+struct HdbModel {
+  BcIndex ix;
+  float* core;          // [m] by position
+  float* cmin;          // [nl]
+  int* pos;             // [m] the position of every caller row
+  int* row_parent;      // [m]
+  double* row_lambda;   // [m]
+  int *parent, *owner, *label;   // [m] (clusters: at most m)
+  double *birth, *death;         // [m]
+  HdbModelHead* head;
+};
+
+// One warp per query qi: approximate_predict's contract (include/raft_b200.h).  The core walk is hdb_core_kernel's (the
+// list kept); the MR walk is SlrWalk's Pred mode, its bound seeded by the best (w, s, row) of that list, so it starts at
+// a real candidate.  Lane 0 then walks the condensed tree up from the neighbour's parent cluster and applies the fit's
+// label rule.  A query with a non-finite coordinate is noise with no neighbour.
+template <int D>
+__global__ void __launch_bounds__(kBcWarps * 32) hdb_predict_kernel(HdbModel M, int n, int nl, int k, int root,
+                                                                    const float* qs, int64_t ldq, int mq, int* labels,
+                                                                    float* prob, int* nn_rows, float* nn_w, int smem)
+{
+  const float *lm, *rhi;
+  bc_stage<D>(M.ix, nl, smem, &lm, &rhi);
+  const int lane = threadIdx.x & 31;
+  const int qi   = blockIdx.x * kBcWarps + (threadIdx.x >> 5);
+  if (qi >= mq) return;
+  SlrWalk<D, true, true> w(M.ix, nullptr, nullptr, nullptr);
+  bool ok = bc_query<D>(qs + static_cast<int64_t>(qi) * ldq, w.q);
+  for (int c = 0; c < D; ++c) ok = ok && isfinite(w.q[c]);
+  if (!ok) {
+    if (lane == 0) {
+      labels[qi] = -1;
+      prob[qi]   = 0.f;
+      if (nn_rows) nn_rows[qi] = -1;
+      if (nn_w) nn_w[qi] = BC_INF;
+    }
+    return;
+  }
+  BcKnn<D> kn{M.ix, w.q, k, 0, lane};
+  bc_walk<D, true>(M.ix, n, nl, lm, rhi, w.q, lane, kn);
+  w.lane = lane;
+  w.core = M.core;
+  w.cmin = M.cmin;
+  w.cq   = key_bound(kn.kth);
+  // the seed: the best of the list's k rows, lane l holding slots l and l + 32
+  for (int h = 0; h < 2; ++h) {
+    const long long e = h ? kn.list.a1 : kn.list.a0;
+    if (lane + 32 * h < k && e != KEY_EMPTY) {
+      const int j    = static_cast<int>(key_index(e));
+      const float s  = key_dist(e);
+      const long long k1 = key_pack(fmaxf(fmaxf(w.cq, M.core[M.pos[j]]), s), __float_as_int(s));
+      if (slr_before(k1, j, w.b1, w.b2)) { w.b1 = k1; w.b2 = j; }
+    }
+  }
+  for (int o = 16; o > 0; o >>= 1) {
+    const long long o1 = __shfl_xor_sync(0xffffffffu, w.b1, o);
+    const int o2       = __shfl_xor_sync(0xffffffffu, w.b2, o);
+    if (slr_before(o1, o2, w.b1, w.b2)) { w.b1 = o1; w.b2 = o2; }
+  }
+  w.bound();
+  bc_walk<D, true>(M.ix, n, nl, lm, rhi, w.q, lane, w);
+  if (lane != 0) return;
+  const int j   = w.b2;
+  const float ws = key_dist(w.b1);
+  const float W  = root ? __fsqrt_rn(ws) : ws;
+  const double wd = W;
+  double lam      = wd > 0.0 ? 1.0 / wd : static_cast<double>(BC_INF);
+  lam             = fmin(lam, M.row_lambda[j]);
+  int p = M.row_parent[j];
+  while (p != 0 && M.birth[p] > lam) p = M.parent[p];
+  const int o = M.owner[p];
+  int lab     = M.label[o];
+  if (o == 0 && !(M.head->single_root && lam >= M.head->thr)) lab = -1;
+  float pr = 0.f;
+  if (lab >= 0) {
+    const double md = M.death[o];
+    pr = static_cast<float>(md == 0.0 || isinf(lam) ? 1.0 : fmin(lam, md) / md);
+  }
+  labels[qi] = lab;
+  prob[qi]   = pr;
+  if (nn_rows) nn_rows[qi] = j;
+  if (nn_w) nn_w[qi] = W;
 }
 
 }  // namespace b2d

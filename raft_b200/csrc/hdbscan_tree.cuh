@@ -40,6 +40,20 @@ inline bool sl_merges(int64_t m, const int* src, const int* dst, int* children, 
   return true;
 }
 
+// What approximate_predict looks up, besides the ball cover: where every row left the condensed tree, and the clusters
+// (ids 0 = the root, 1, 2, ... as the condensing pass numbers them, so a parent's id is below its child's).
+struct HdbTreeExport {
+  std::vector<int> row_parent;      // [m] the cluster a row leaves
+  std::vector<double> row_lambda;   // [m] the lambda at which it leaves it
+  std::vector<int> parent;          // [nc] the parent cluster (-1: the root)
+  std::vector<int> owner;           // [nc] the nearest selected ancestor, the cluster itself included (0: the root)
+  std::vector<int> label;           // [nc] a selected cluster's label, or -1 (not selected, or no row took it)
+  std::vector<double> birth;        // [nc] the lambda of the cluster's birth (0 for the root)
+  std::vector<double> death;        // [nc] sklearn's max_lambdas of the cluster
+  bool single_root = false;         // the root is the one selected cluster ...
+  double thr       = 0.0;           // ... and a row that leaves it at a lambda >= thr takes its label
+};
+
 struct HdbTreeParams {
   int min_cluster_size;   // >= 2
   double epsilon;         // cluster_selection_epsilon >= 0
@@ -54,14 +68,16 @@ struct HdbTreeParams {
 // Clusters are numbered as the condensing pass meets them (breadth first from the root, smaller child first), so that
 // the row order of the condensed tree, which sums the stabilities and bounds the probabilities, is sklearn's.  A
 // cluster's "death" is the largest lambda of the last run of consecutive condensed rows it parents, as sklearn's
-// max_lambdas computes it.  The epsilon search visits the selected leaves in ascending cluster id.
+// max_lambdas computes it.  The epsilon search visits the selected leaves in ascending cluster id.  With ex, the tree
+// as HdbTreeExport describes it (one row: the root alone, which labels nothing).
 inline int hdbscan_tree(int64_t m64, const int* src, const int* dst, const float* w, const HdbTreeParams& p, int* labels,
-                        float* prob)
+                        float* prob, HdbTreeExport* ex = nullptr)
 {
   const int m = static_cast<int>(m64);
   if (m == 1) {
     labels[0] = -1;
     prob[0]   = 0.f;
+    if (ex) *ex = HdbTreeExport{{0}, {0.0}, {-1}, {0}, {-1}, {0.0}, {0.0}};
     return 0;
   }
   std::vector<int> ch(2 * static_cast<size_t>(m - 1)), sz(m - 1);
@@ -249,6 +265,19 @@ inline int hdbscan_tree(int64_t m64, const int* src, const int* dst, const float
     labels[i]       = canon[c];
     const double md = death[c];
     prob[i] = static_cast<float>(md == 0.0 || std::isinf(lam[i]) ? 1.0 : std::min(lam[i], md) / md);
+  }
+  if (ex) {
+    ex->row_parent.assign(m, 0);
+    for (size_t r = 0; r < nr; ++r)
+      if (cchild[r] < m) ex->row_parent[cchild[r]] = cpar[r] - m;
+    ex->row_lambda = lam;
+    ex->parent     = parent;
+    ex->owner      = owner;
+    ex->label      = canon;
+    ex->birth      = birth;
+    ex->death      = death;
+    ex->single_root = single_root;
+    ex->thr         = thr;
   }
   return next_label;
 }

@@ -394,6 +394,36 @@ static int emst_run(cudaStream_t s, const EmstLayout& L, int root, const float* 
   return B2D_OK;
 }
 
+// The model of b2d_hdbscan_rbc_fit_model (256-byte aligned regions): the fit's index (bc_layout, so one copy moves it),
+// then HdbModel's arrays, the clusters bounded by m.
+struct HdbModelLayout {
+  HdbModel M;
+  size_t index_bytes;
+  size_t bytes;
+};
+
+static HdbModelLayout hdb_model_layout(void* base, int64_t m, int64_t d, int64_t nl)
+{
+  const BcLayout I = bc_layout(base, m, d, nl);
+  Carve c(base ? static_cast<char*>(base) + I.bytes : nullptr, 256);
+  HdbModelLayout L{};
+  L.M.ix         = I.ix;
+  L.index_bytes  = I.bytes;
+  L.M.core       = c.take<float>(m);
+  L.M.cmin       = c.take<float>(nl);
+  L.M.pos        = c.take<int>(m);
+  L.M.row_parent = c.take<int>(m);
+  L.M.row_lambda = c.take<double>(m);
+  L.M.parent     = c.take<int>(m);
+  L.M.owner      = c.take<int>(m);
+  L.M.label      = c.take<int>(m);
+  L.M.birth      = c.take<double>(m);
+  L.M.death      = c.take<double>(m);
+  L.M.head       = c.take<HdbModelHead>(1);
+  L.bytes        = I.bytes + c.bytes;
+  return L;
+}
+
 static int emst_dispatch(cudaStream_t s, const EmstLayout& L, int metric, const float* x, int64_t ldx, int64_t m,
                          int64_t d, int64_t nl, uint64_t seed, int* out_src, int* out_dst, float* out_w,
                          int min_samples = 0)
@@ -595,10 +625,19 @@ size_t b2d_hdbscan_rbc_workspace_bytes(int64_t m, int64_t d, int64_t n_landmarks
   return emst_layout(nullptr, m, d, bc_landmarks(m, n_landmarks), false, true).bytes;
 }
 
-int b2d_hdbscan_rbc_fit(void* stream, int metric, const float* x, int64_t ldx, int64_t m, int64_t d, int min_samples,
-                        int min_cluster_size, double cluster_selection_epsilon, int method, int allow_single_cluster,
-                        int64_t n_landmarks, uint64_t seed, int32_t* labels, float* probabilities, int32_t* mst_src,
-                        int32_t* mst_dst, float* mst_w, int32_t* n_clusters, void* workspace, size_t workspace_bytes)
+size_t b2d_hdbscan_rbc_model_bytes(int64_t m, int64_t d, int64_t n_landmarks)
+{
+  if (!emst_extents_ok(m, d, n_landmarks)) return static_cast<size_t>(-1);
+  return hdb_model_layout(nullptr, m, d, bc_landmarks(m, n_landmarks)).bytes;
+}
+
+namespace {
+// b2d_hdbscan_rbc_fit, and with with_model b2d_hdbscan_rbc_fit_model, whose model is checked after the fit's arguments
+int hdbscan_fit(void* stream, int metric, const float* x, int64_t ldx, int64_t m, int64_t d, int min_samples,
+                int min_cluster_size, double cluster_selection_epsilon, int method, int allow_single_cluster,
+                int64_t n_landmarks, uint64_t seed, int32_t* labels, float* probabilities, int32_t* mst_src,
+                int32_t* mst_dst, float* mst_w, int32_t* n_clusters, void* workspace, size_t workspace_bytes, void* model,
+                bool with_model)
 {
   cudaStream_t s = static_cast<cudaStream_t>(stream);
   int rc         = emst_args("hdbscan rbc", metric, x, ldx, m, d, n_landmarks);
@@ -618,10 +657,25 @@ int b2d_hdbscan_rbc_fit(void* stream, int metric, const float* x, int64_t ldx, i
   const int64_t nl = bc_landmarks(m, n_landmarks);
   rc = check_workspace(workspace, workspace_bytes, emst_layout(nullptr, m, d, nl, false, true).bytes);
   if (rc) return rc;
+  if (with_model && !model) return fail(B2D_ERR_INVALID_ARG, "null model");
+  if (with_model && reinterpret_cast<uintptr_t>(model) % 256)
+    return fail(B2D_ERR_INVALID_ARG, "model must be 256-byte aligned");
   const EmstLayout L = emst_layout(workspace, m, d, nl, false, true);
   // 1.-2. the index, the core distances and the tree edges in (w, min row, max row) order
   rc = emst_dispatch(s, L, metric, x, ldx, m, d, nl, seed, mst_src, mst_dst, mst_w, min_samples);
   if (rc) return rc;
+  const HdbModelLayout ML = hdb_model_layout(model, m, d, nl);
+  if (model) {   // the index lies at the workspace's start in the model's own layout
+    B2D_CUDA(cudaMemcpyAsync(model, workspace, ML.index_bytes, cudaMemcpyDeviceToDevice, s));
+    B2D_CUDA(cudaMemcpyAsync(ML.M.pos, L.pos, m * sizeof(int), cudaMemcpyDeviceToDevice, s));
+    if (m > 1) {
+      B2D_CUDA(cudaMemcpyAsync(ML.M.core, L.core, m * sizeof(float), cudaMemcpyDeviceToDevice, s));
+      B2D_CUDA(cudaMemcpyAsync(ML.M.cmin, L.cmin, nl * sizeof(float), cudaMemcpyDeviceToDevice, s));
+    } else {   // one row: its core distance is s(0, 0) = 0 (the rounds computed none)
+      B2D_CUDA(cudaMemsetAsync(ML.M.core, 0, sizeof(float), s));
+      B2D_CUDA(cudaMemsetAsync(ML.M.cmin, 0, nl * sizeof(float), s));
+    }
+  }
   sl_finite_kernel<<<km_grid(m * d), 256, 0, s>>>(x, ldx, m, static_cast<int>(d), L.ctrl);
   B2D_CUDA(cudaGetLastError());
   // 3. the tree stages on the host (the one synchronisation before it reads the control words and the edges)
@@ -640,11 +694,79 @@ int b2d_hdbscan_rbc_fit(void* stream, int metric, const float* x, int64_t ldx, i
     return fail(B2D_ERR_CUDA, "internal: the rounds chose " + std::to_string(h.n_mst) + " of " + std::to_string(m - 1) +
                                   " tree edges");
   const HdbTreeParams P{min_cluster_size, cluster_selection_epsilon, method == B2D_HDBSCAN_LEAF, allow_single_cluster != 0};
-  const int nc = hdbscan_tree(m, hs.data(), hd.data(), hw.data(), P, hl.data(), hp.data());
+  HdbTreeExport ex;
+  const int nc = hdbscan_tree(m, hs.data(), hd.data(), hw.data(), P, hl.data(), hp.data(), model ? &ex : nullptr);
   if (nc < 0) return fail(B2D_ERR_CUDA, "internal: the spanning tree has a cycle");
   B2D_CUDA(cudaMemcpyAsync(labels, hl.data(), m * sizeof(int), cudaMemcpyHostToDevice, s));
   B2D_CUDA(cudaMemcpyAsync(probabilities, hp.data(), m * sizeof(float), cudaMemcpyHostToDevice, s));
+  const size_t nci = ex.parent.size();
+  const HdbModelHead head{ex.thr, ex.single_root ? 1 : 0, static_cast<int>(nci)};
+  if (model) {
+    const HdbModel& M = ML.M;
+    B2D_CUDA(cudaMemcpyAsync(M.row_parent, ex.row_parent.data(), m * sizeof(int), cudaMemcpyHostToDevice, s));
+    B2D_CUDA(cudaMemcpyAsync(M.row_lambda, ex.row_lambda.data(), m * sizeof(double), cudaMemcpyHostToDevice, s));
+    B2D_CUDA(cudaMemcpyAsync(M.parent, ex.parent.data(), nci * sizeof(int), cudaMemcpyHostToDevice, s));
+    B2D_CUDA(cudaMemcpyAsync(M.owner, ex.owner.data(), nci * sizeof(int), cudaMemcpyHostToDevice, s));
+    B2D_CUDA(cudaMemcpyAsync(M.label, ex.label.data(), nci * sizeof(int), cudaMemcpyHostToDevice, s));
+    B2D_CUDA(cudaMemcpyAsync(M.birth, ex.birth.data(), nci * sizeof(double), cudaMemcpyHostToDevice, s));
+    B2D_CUDA(cudaMemcpyAsync(M.death, ex.death.data(), nci * sizeof(double), cudaMemcpyHostToDevice, s));
+    B2D_CUDA(cudaMemcpyAsync(M.head, &head, sizeof(head), cudaMemcpyHostToDevice, s));
+  }
   B2D_CUDA(cudaStreamSynchronize(s));
   *n_clusters = nc;
   return B2D_OK;
+}
+}  // namespace
+
+int b2d_hdbscan_rbc_fit(void* stream, int metric, const float* x, int64_t ldx, int64_t m, int64_t d, int min_samples,
+                        int min_cluster_size, double cluster_selection_epsilon, int method, int allow_single_cluster,
+                        int64_t n_landmarks, uint64_t seed, int32_t* labels, float* probabilities, int32_t* mst_src,
+                        int32_t* mst_dst, float* mst_w, int32_t* n_clusters, void* workspace, size_t workspace_bytes)
+{
+  return hdbscan_fit(stream, metric, x, ldx, m, d, min_samples, min_cluster_size, cluster_selection_epsilon, method,
+                     allow_single_cluster, n_landmarks, seed, labels, probabilities, mst_src, mst_dst, mst_w, n_clusters,
+                     workspace, workspace_bytes, nullptr, false);
+}
+
+int b2d_hdbscan_rbc_fit_model(void* stream, int metric, const float* x, int64_t ldx, int64_t m, int64_t d,
+                              int min_samples, int min_cluster_size, double cluster_selection_epsilon, int method,
+                              int allow_single_cluster, int64_t n_landmarks, uint64_t seed, int32_t* labels,
+                              float* probabilities, int32_t* mst_src, int32_t* mst_dst, float* mst_w, int32_t* n_clusters,
+                              void* workspace, size_t workspace_bytes, void* model)
+{
+  return hdbscan_fit(stream, metric, x, ldx, m, d, min_samples, min_cluster_size, cluster_selection_epsilon, method,
+                     allow_single_cluster, n_landmarks, seed, labels, probabilities, mst_src, mst_dst, mst_w, n_clusters,
+                     workspace, workspace_bytes, model, true);
+}
+
+int b2d_hdbscan_rbc_approximate_predict(void* stream, const void* model, int64_t m, int64_t d, int metric,
+                                        int64_t n_landmarks, int min_samples, const float* q, int64_t ldq, int64_t mq,
+                                        int32_t* labels, float* probabilities, int32_t* nn_rows, float* nn_w)
+{
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  if (metric != B2D_L2Unexpanded && metric != B2D_L2SqrtUnexpanded)
+    return fail(B2D_ERR_UNSUPPORTED, "hdbscan approximate_predict supports the L2Unexpanded and L2SqrtUnexpanded metrics, "
+                                     "got metric " + std::to_string(metric));
+  if (d != 2 && d != 3)
+    return fail(B2D_ERR_UNSUPPORTED, "hdbscan approximate_predict supports d = 2 and d = 3, got d = " + std::to_string(d));
+  if (m < 1 || m >= kSlMaxRows) return fail(B2D_ERR_INVALID_ARG, "m must be in [1, 2^30)");
+  if (n_landmarks < 0 || n_landmarks > m)
+    return fail(B2D_ERR_INVALID_ARG, "n_landmarks must be in [0, m] (0: ceil(sqrt(m)))");
+  if (min_samples < 1 || min_samples > std::min<int64_t>(KNN_MAX_K, m))
+    return fail(B2D_ERR_INVALID_ARG, "min_samples must be in [1, min(64, m)], got " + std::to_string(min_samples));
+  if (!model) return fail(B2D_ERR_INVALID_ARG, "null model");
+  if (reinterpret_cast<uintptr_t>(model) % 256) return fail(B2D_ERR_INVALID_ARG, "model must be 256-byte aligned");
+  if (mq < 0 || mq > 0x7fffffffll) return fail(B2D_ERR_INVALID_ARG, "mq must be in [0, 2^31)");
+  if (mq > 0 && !q) return fail(B2D_ERR_INVALID_ARG, "null queries");
+  if (ldq < d) return fail(B2D_ERR_INVALID_ARG, "ldq smaller than d");
+  if (mq > 0 && (!labels || !probabilities)) return fail(B2D_ERR_INVALID_ARG, "null labels / probabilities");
+  if (mq == 0) return B2D_OK;
+  const int64_t nl = bc_landmarks(m, n_landmarks);
+  const HdbModel M = hdb_model_layout(const_cast<void*>(model), m, d, nl).M;
+  const int root   = metric == B2D_L2SqrtUnexpanded;
+  const int n = static_cast<int>(m), nli = static_cast<int>(nl), mqi = static_cast<int>(mq);
+  return d == 2 ? bc_walk_launch(s, hdb_predict_kernel<2>, mq, nl, d, M, n, nli, min_samples, root, q, ldq, mqi, labels,
+                                 probabilities, nn_rows, nn_w)
+                : bc_walk_launch(s, hdb_predict_kernel<3>, mq, nl, d, M, n, nli, min_samples, root, q, ldq, mqi, labels,
+                                 probabilities, nn_rows, nn_w);
 }

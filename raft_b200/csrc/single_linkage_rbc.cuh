@@ -59,7 +59,9 @@ __device__ __forceinline__ bool slr_before(long long a1, int a2, long long b1, i
 // core distances too (core: by position, cmin: the smallest core of every ball, cq: the query's).  Each prune is strict
 // against the bound wb, so a pair at the bound's weight is still compared.  Since w >= s, the window and ball tests on s
 // stay valid at bc_dhi(wb).
-template <int D, bool Mr = false>
+// Pred (HDBSCAN's approximate_predict, hdbscan_rbc.cuh; with Mr): the query is not a row of the index, so there is no
+// colour and no component slot; row j is keyed (w, s, j), b1 = key_pack(w, bits of s) and b2 = j.
+template <int D, bool Mr = false, bool Pred = false>
 struct SlrWalk {
   const BcIndex& ix;
   const int* colour;
@@ -81,6 +83,7 @@ struct SlrWalk {
   // Mr: a ball whose every pair weighs more than the bound (max(cq, cmin) > wb) is not admitted either
   __device__ __forceinline__ bool admit(int j) const
   {
+    if constexpr (Pred) return !(fmaxf(cq, cmin[j]) > wb);
     if constexpr (Mr) return bcol[j] != col && !(fmaxf(cq, cmin[j]) > wb);
     return bcol[j] != col;
   }
@@ -98,7 +101,7 @@ struct SlrWalk {
   // component's minimum: every pair of the row then orders after it
   __device__ __forceinline__ bool scan(int lo, int hi, float sq)
   {
-    seen = min(seen, *reinterpret_cast<volatile long long*>(slot));
+    if constexpr (!Pred) seen = min(seen, *reinterpret_cast<volatile long long*>(slot));
     bound();
     if constexpr (Mr)
       if (__any_sync(0xffffffffu, cq > wb)) return true;
@@ -110,8 +113,15 @@ struct SlrWalk {
       const bool out = i < hi && r > whi;
       long long k1   = KEY_EMPTY;
       int k2         = INT_MAX;
-      if (i < hi && !out && r >= wlo && colour[i] != col) {
-        if constexpr (Mr) {
+      if (i < hi && !out && r >= wlo && (Pred || colour[i] != col)) {
+        if constexpr (Pred) {
+          const float cp = core[i];
+          if (!(cp > wb)) {
+            const float s = bc_s<D>(q, ix.pts + static_cast<int64_t>(i) * D);
+            k1            = key_pack(fmaxf(fmaxf(cq, cp), s), __float_as_int(s));
+            k2            = ix.ids[i];
+          }
+        } else if constexpr (Mr) {
           const float cp = core[i];   // a member above the bound is not measured
           if (!(cp > wb)) {
             const float s = bc_s<D>(q, ix.pts + static_cast<int64_t>(i) * D);
@@ -144,8 +154,10 @@ struct SlrWalk {
       if (__any_sync(0xffffffffu, out)) break;
     }
     // an improvement is published at once, so that the component's other rows prune with it
-    if (lane == 0 && b1 < seen) atomicMin(slot, b1);
-    seen = min(seen, b1);
+    if constexpr (!Pred) {
+      if (lane == 0 && b1 < seen) atomicMin(slot, b1);
+      seen = min(seen, b1);
+    }
     return false;
   }
 };
