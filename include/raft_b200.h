@@ -516,8 +516,9 @@ int b2d_mst(void* stream, const int32_t* src, const int32_t* dst, const float* w
  *   2. edges ordered by (squared weight, position): the tree and the merge order do not depend on the metric;
  *   3. its minimum spanning forest by Borůvka (b2d_mst);
  *   4. connect_components while the forest has more than one tree: every tree's row i of smallest (d_i, i), d_i the
- *      squared distance to i's nearest row of another tree (the masked 1-NN), gives the edge (i, that row), appended
- *      after the edges so far; Borůvka again;
+ *      squared distance to i's nearest row of another tree (the masked 1-NN; among equidistant rows the first in
+ *      (smallest row of its tree, row) order), gives the edge (i, that row), appended after the edges so far with the
+ *      trees in order of their smallest row; Borůvka again;
  *   5. the m - 1 edges in key order, merged on the host: merge t creates cluster m + t; children[t] = the two merged ids,
  *      smaller first; deltas[t] = its weight (its square root for L2SqrtExpanded); sizes[t] = the new cluster's size
  *      (scipy.cluster.hierarchy.linkage's conventions).  labels[i] = the cluster of row i after the first
@@ -532,6 +533,11 @@ size_t b2d_single_linkage_workspace_bytes(int64_t m, int64_t d, int c);
 int b2d_single_linkage(void* stream, int metric, const float* x, int64_t ldx, int64_t m, int64_t d, int c, int n_clusters,
                        int32_t* children, float* deltas, int32_t* sizes, int32_t* labels, int32_t* n_components_out,
                        void* workspace, size_t workspace_bytes);
+/* How one connect_components round of b2d_single_linkage on m rows and `comps` trees (2 <= comps <= m) cuts its work,
+ * host arithmetic only: out[0] = rows per masked arg-min chunk, out[1] = chunks, out[2] = rows per block of the sort by
+ * tree (2048, or more when comps x blocks would pass 2^24 histogram words), out[3] = sort blocks.  B2D_ERR_INVALID_ARG
+ * for a null out, m outside [2, 2^30) or comps outside [2, m]. */
+int b2d_debug_single_linkage_plan(int64_t m, int64_t comps, int64_t* out);
 /* The exact Euclidean minimum spanning tree of 2-D and 3-D points (raft::cluster::single_linkage's LinkageDistance::
  * PAIRWISE for d <= 3), by Borůvka over the random ball cover.  x:[m,d] fp32, row-major, pitch ldx >= d.
  *   The graph is complete; pair (i, j) weighs s(i, j) = ((q0-p0)*(q0-p0) + (q1-p1)*(q1-p1)) + (q2-p2)*(q2-p2), every

@@ -22,7 +22,8 @@ SYMBOLS = [
     "b2d_kmeans_init_scalable", "b2d_kmeans_fit_scalable", "b2d_kmeans_balanced_workspace_bytes",
     "b2d_kmeans_balanced_fit", "b2d_debug_kmeans_balanced_fine_assign",
     "b2d_mst_workspace_bytes", "b2d_mst",
-    "b2d_single_linkage_workspace_bytes", "b2d_single_linkage", "b2d_dbscan_workspace_bytes", "b2d_dbscan_fit",
+    "b2d_single_linkage_workspace_bytes", "b2d_single_linkage", "b2d_debug_single_linkage_plan",
+    "b2d_dbscan_workspace_bytes", "b2d_dbscan_fit",
     "b2d_debug_pairwise_plan", "b2d_radius_neighbors_workspace_bytes", "b2d_radius_neighbors_count",
     "b2d_radius_neighbors_fill", "b2d_kde_workspace_bytes", "b2d_kde_score_samples",
     "b2d_mean_shift_fit_workspace_bytes", "b2d_mean_shift_fit", "b2d_debug_mean_shift_sums",
@@ -156,6 +157,8 @@ def lib() -> ctypes.CDLL:
     L.b2d_single_linkage_workspace_bytes.argtypes = [i64, i64, ci]
     L.b2d_single_linkage.restype = ci
     L.b2d_single_linkage.argtypes = [vp, ci, vp, i64, i64, i64, ci, ci, vp, vp, vp, vp, vp, vp, sz]
+    L.b2d_debug_single_linkage_plan.restype = ci
+    L.b2d_debug_single_linkage_plan.argtypes = [i64, i64, vp]
     L.b2d_dbscan_workspace_bytes.restype = sz
     L.b2d_dbscan_workspace_bytes.argtypes = [i64, i64, i64]
     L.b2d_dbscan_fit.restype = ci

@@ -184,18 +184,23 @@ static SlLayout sl_layout(void* base, int64_t m, int64_t d, int64_t n_nb)
   return L;
 }
 
-// One round of connect_components for c > 1 components: dense component ids, the rows sorted by component (stable),
-// the masked arg-min of every sorted row against the rows of other components in row chunks, and for every component
-// the edge from its row of smallest (distance, row) to that row's nearest row: edges [e0, e0 + c).
+// One round of connect_components for c > 1 components: dense component ids in order of each component's smallest row,
+// the rows sorted by component (stable), the masked arg-min of every sorted row against the rows of other components in
+// row chunks, and for every component the edge from its row of smallest (distance, row) to that row's nearest row:
+// edges [e0, e0 + c).  The arg-min takes the smallest sorted position among equidistant rows, so the nearest row's
+// ties go to the first in (smallest row of its component, row) order.
 static int sl_connect(cudaStream_t s, const SlLayout& L, const float* x, int64_t ldx, int64_t m, int64_t d, int64_t c,
                       int64_t e0)
 {
   const MstLayout& T = L.mst;
   const KmSort& S = L.sort;
-  sl_root_flags_kernel<<<sl_grid(m), 256, 0, s>>>(T.colour, L.ids, m);
+  int* minv = L.ends;   // [m] the smallest row of every component, by root (ends is written after the sort)
+  sl_tree_min_init_kernel<<<sl_grid(m), 256, 0, s>>>(T.colour, minv, m);
+  sl_min_vertex_kernel<<<sl_grid(m), 256, 0, s>>>(T.colour, minv, m);
+  sl_root_flags_kernel<<<sl_grid(m), 256, 0, s>>>(T.colour, minv, L.ids, m);
   int rc = km_scan(s, nullptr, L.ids, m, S.tiles, S.ctrl);
   if (rc) return rc;
-  sl_dense_label_kernel<<<sl_grid(m), 256, 0, s>>>(T.colour, L.ids, L.lab, m);
+  sl_dense_label_kernel<<<sl_grid(m), 256, 0, s>>>(T.colour, minv, L.ids, L.lab, m);
   B2D_CUDA(cudaGetLastError());
   const KmSortPlan P = km_sort_plan(m, c);
   rc = km_sort_count(s, S, P, L.lab, m, c);
@@ -552,6 +557,20 @@ int b2d_single_linkage(void* stream, int metric, const float* x, int64_t ldx, in
     B2D_CUDA(cudaStreamSynchronize(s));
   }
   return sl_dendrogram(s, m, n_clusters, hs, hd, children, sizes, labels);
+}
+
+int b2d_debug_single_linkage_plan(int64_t m, int64_t comps, int64_t* out)
+{
+  if (!out) return fail(B2D_ERR_INVALID_ARG, "null out");
+  if (m < 2 || m >= kSlMaxRows) return fail(B2D_ERR_INVALID_ARG, "m must be in [2, 2^30)");
+  if (comps < 2 || comps > m) return fail(B2D_ERR_INVALID_ARG, "comps must be in [2, m]");
+  const int64_t mc = sl_chunk_rows(m, comps);
+  const KmSortPlan P = km_sort_plan(m, comps);
+  out[0] = mc;
+  out[1] = (m + mc - 1) / mc;
+  out[2] = P.rb;
+  out[3] = P.nblk;
+  return B2D_OK;
 }
 
 size_t b2d_emst_rbc_workspace_bytes(int64_t m, int64_t d, int64_t n_landmarks)

@@ -179,17 +179,27 @@ __global__ void sl_knn_edges_kernel(const int64_t* idx, const float* dist, int64
   w[e]   = dist[e];
 }
 
-// flags[v] = 1 for a component root (scanned in place into the dense component ids), then lab[v] = id of v's root
-__global__ void sl_root_flags_kernel(const int* colour, unsigned* flags, int64_t n)
+// The dense component ids of a connect round, numbered in order of each component's smallest row (the root of a
+// component is not always its smallest row): minv[r] <- r for every root r, then sl_min_vertex_kernel lowers it to the
+// component's smallest row (only the roots' entries are written or read).
+__global__ void sl_tree_min_init_kernel(const int* colour, int* minv, int64_t n)
 {
   const int64_t v = static_cast<int64_t>(blockIdx.x) * blockDim.x + threadIdx.x;
-  if (v < n) flags[v] = colour[v] == v ? 1u : 0u;
+  if (v < n && colour[v] == v) minv[v] = static_cast<int>(v);
 }
 
-__global__ void sl_dense_label_kernel(const int* colour, const unsigned* ids, int* lab, int64_t n)
+// flags[v] = 1 for the smallest row of a component (scanned in place into the dense component ids), then lab[v] = the
+// id of v's component
+__global__ void sl_root_flags_kernel(const int* colour, const int* minv, unsigned* flags, int64_t n)
 {
   const int64_t v = static_cast<int64_t>(blockIdx.x) * blockDim.x + threadIdx.x;
-  if (v < n) lab[v] = static_cast<int>(ids[colour[v]]);
+  if (v < n) flags[v] = minv[colour[v]] == v ? 1u : 0u;
+}
+
+__global__ void sl_dense_label_kernel(const int* colour, const int* minv, const unsigned* ids, int* lab, int64_t n)
+{
+  const int64_t v = static_cast<int64_t>(blockIdx.x) * blockDim.x + threadIdx.x;
+  if (v < n) lab[v] = static_cast<int>(ids[minv[colour[v]]]);
 }
 
 // the end of every component in the sorted rows (km_scatter_kernel's cursors): the group_idxs of the masked arg-min

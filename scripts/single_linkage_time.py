@@ -2,7 +2,7 @@
 brute_force.knn, the graph copied to the host, scipy.sparse.csgraph.minimum_spanning_tree and a union-find dendrogram.
 
 Stages come from one torch.profiler run of the call, cut at marker kernels in stream order: kNN (up to
-sl_knn_edges_kernel), Borůvka (the rounds before the first connect), each connect round (sl_root_flags_kernel up to the
+sl_knn_edges_kernel), Borůvka (the rounds before the first connect), each connect round (sl_tree_min_init_kernel up to the
 round's last Borůvka kernel, including its host synchronisation), and the dendrogram (the radix sort to the end of the
 call: device sort and gather, copies, union-find on the host).  The total is CUDA events around the call (which
 synchronises before it returns) after a warm-up, without the profiler, median of --reps.
@@ -45,7 +45,7 @@ def stages(x, c):
     t0, t_end = call.time_range.start, call.time_range.end
     names = [k.name for k in kern]
     i_edges = max(i for i, n in enumerate(names) if "sl_knn_edges_kernel" in n)
-    i_rounds = [i for i, n in enumerate(names) if "sl_root_flags_kernel" in n]
+    i_rounds = [i for i, n in enumerate(names) if "sl_tree_min_init_kernel" in n]
     i_sort = min(i for i, n in enumerate(names) if "DeviceRadixSort" in n)
     res = {"knn_ms": (kern[i_edges].time_range.end - t0) / 1e3}
     cuts = i_rounds + [i_sort]

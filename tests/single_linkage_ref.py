@@ -64,16 +64,21 @@ def knn_edges(idx, dist):
 
 def connect_edges(x, colour):
     """Step 4 in fp64: for every tree, the edge from its row i of smallest (d_i, i) to that row's nearest row of another
-    tree (ties to the smaller row), d_i the squared distance; trees in order of their smallest row."""
+    tree, d_i the squared distance; trees in order of their smallest row.  colour[v] is the smallest row of v's tree.
+    Among equidistant nearest rows the first in (smallest row of its tree, row) order wins, not the smallest row: the
+    device's arg-min runs over the rows sorted by tree and takes the smallest sorted position."""
     x = np.asarray(x, np.float64)
+    colour = np.asarray(colour)
+    order = np.lexsort((np.arange(len(x)), colour))   # the candidates in (smallest row of their tree, row) order
+    xo, co = x[order], colour[order]
     nx = (x * x).sum(1)
     j = np.zeros(len(x), np.int64)
     di = np.zeros(len(x))
     for r0 in range(0, len(x), 1024):   # row blocks: m x m distances are never held at once
-        d2 = np.maximum(nx[r0:r0 + 1024, None] + nx[None, :] - 2 * x[r0:r0 + 1024] @ x.T, 0)
-        d2[colour[r0:r0 + 1024, None] == colour[None, :]] = np.inf
-        j[r0:r0 + 1024] = d2.argmin(1)
-        di[r0:r0 + 1024] = d2[np.arange(len(d2)), j[r0:r0 + 1024]]
+        d2 = np.maximum(nx[r0:r0 + 1024, None] + nx[order][None, :] - 2 * x[r0:r0 + 1024] @ xo.T, 0)
+        d2[colour[r0:r0 + 1024, None] == co[None, :]] = np.inf
+        j[r0:r0 + 1024] = order[d2.argmin(1)]
+        di[r0:r0 + 1024] = d2.min(1)
     out = []
     for g in np.unique(colour):
         rows = np.flatnonzero(colour == g)

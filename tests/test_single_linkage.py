@@ -1,5 +1,6 @@
 """single_linkage without a GPU: the fp64 reference (tests/single_linkage_ref.py) against scipy's single linkage and
 minimum spanning tree, the ABI declarations, the workspace queries and the argument checks of the C ABI."""
+import ctypes
 import os
 import re
 
@@ -12,7 +13,8 @@ from raft_b200 import _lib
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 SIZE_MAX = 2 ** 64 - 1
 P = 1 << 12   # a non-null pointer that is never dereferenced (every call below fails before any work)
-NEW = ["b2d_mst_workspace_bytes", "b2d_mst", "b2d_single_linkage_workspace_bytes", "b2d_single_linkage"]
+NEW = ["b2d_mst_workspace_bytes", "b2d_mst", "b2d_single_linkage_workspace_bytes", "b2d_single_linkage",
+       "b2d_debug_single_linkage_plan"]
 L2, L2SQRT, COSINE = 0, 1, 2
 
 
@@ -71,6 +73,66 @@ def test_reference_tie_order():
     chosen, _ = ref.kruskal(np.array([0, 0]), np.array([1, 1]), np.float32([0.0, -0.0]), 2)
     assert chosen.tolist() == [1]
     assert ref.n_neighbors(1) == 1 and ref.n_neighbors(2) == 2 and ref.n_neighbors(10 ** 6) == 34
+
+
+def test_connect_tie_goes_to_the_first_tree_by_smallest_row():
+    """Tree {2} (x = 0) has two nearest rows at squared distance 25: row 1 (tree {1}) and row 3 (tree {0, 3}).  The
+    smaller row is 1; the first in (smallest row of its tree, row) order is 3, and that one wins."""
+    x = np.array([[100.0], [5.0], [0.0], [-5.0]])
+    colour = np.array([0, 1, 2, 0])
+    src, dst, w = ref.connect_edges(x, colour)
+    assert src.tolist() == [3, 1, 2] and dst.tolist() == [2, 2, 3] and w.tolist() == [25, 25, 25]
+
+
+def sl_plan(m, comps):
+    """b2d_debug_single_linkage_plan: (chunk rows, chunks, sort block rows, sort blocks)."""
+    out = (ctypes.c_int64 * 4)()
+    _lib.check(_lib.lib().b2d_debug_single_linkage_plan(m, comps, ctypes.addressof(out)))
+    return tuple(out)
+
+
+def plan_model(m, c):
+    """The plan restated: chunk rows max(128, floor(128 m / c) rounded down to 128), capped at m rounded up to 128 and
+    at 2^40 / m rounded down to 128 (never below 128); sort blocks of 2048 rows, widened in steps of 2048 when
+    c x blocks would pass 2^24 histogram words."""
+    cap = max(128, (2 ** 40 // m) // 128 * 128)
+    rows = min(max(128, (128 * m // c) // 128 * 128), -(-m // 128) * 128, cap)
+    rb = 2048
+    if c * -(-m // 2048) > 2 ** 24:
+        nblk = max(1, 2 ** 24 // c)
+        rb = -(-(-(-m // nblk)) // 2048) * 2048
+    return rows, -(-m // rows), rb, -(-m // rb)
+
+
+@pytest.mark.parametrize("m,comps,want", [
+    (5000, 2, (5120, 1, 2048, 3)),            # one chunk: 128 m / c is past m rounded up to 128
+    (5000, 125, (5120, 1, 2048, 3)),          # the last single chunk (m = 39 x 128 + 8) ...
+    (5000, 126, (4992, 2, 2048, 3)),          # ... and the first split into two
+    (5000, 128, (4992, 2, 2048, 3)),
+    (5000, 257, (2432, 3, 2048, 3)),
+    (5000, 1000, (640, 8, 2048, 3)),
+    (5000, 2500, (256, 20, 2048, 3)),         # two-row trees: 256-row chunks
+    (5000, 5000, (128, 40, 2048, 3)),
+    (2047, 2, (2048, 1, 2048, 1)), (2048, 2, (2048, 1, 2048, 1)), (2049, 2, (2176, 1, 2048, 2)),
+    (6145, 3, (6272, 1, 2048, 4)),
+    (270000, 135000, (256, 1055, 4096, 66)),  # past the histogram cap: 135000 x 132 blocks > 2^24 words
+    (2 ** 29, 2, (2048, 2 ** 18, 2048, 2 ** 18)),   # chunks capped at 2^40 / m rows
+])
+def test_single_linkage_plan(m, comps, want):
+    assert sl_plan(m, comps) == want == plan_model(m, comps)
+
+
+def test_single_linkage_plan_model_and_arguments():
+    rng = np.random.default_rng(7)
+    for m in list(rng.integers(2, 10 ** 6, 40)) + [2, 3, 127, 128, 129, 2 ** 30 - 1]:
+        m = int(m)
+        for c in {2, m, int(rng.integers(2, m + 1)), max(2, m // 2), max(2, m // 128)}:
+            assert sl_plan(m, c) == plan_model(m, c), (m, c)
+    L = _lib.lib()
+    out = (ctypes.c_int64 * 4)()
+    for m, c in ((1, 1), (100, 1), (100, 101), (2 ** 30, 2)):
+        assert L.b2d_debug_single_linkage_plan(m, c, ctypes.addressof(out)) == _lib.B2D_ERR_INVALID_ARG, (m, c)
+    assert L.b2d_debug_single_linkage_plan(100, 2, None) == _lib.B2D_ERR_INVALID_ARG
 
 
 def test_abi_declarations():
